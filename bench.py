@@ -18,6 +18,10 @@ blocks (`config_c2`, `config_c3`).
 N>1: one Solve is a sequential first-fit chain and does not shard (DESIGN.md section 8: "replicas only"): every rank
 runs its own independent Solve of the same shape (seed 42 + rank), no collective on the data path; value = pods all ranks
 scheduled / slowest rank's time, scaling "weak".
+--steps K sets every timed loop (resident, e2e, feasibility kernel, secondary configurations, C5 passes).
+--dump-outputs DIR writes the result of the last timed step (rank 0's resident Solve; in the reference arm the oracle's
+Solve of its sample, min(--pods, CPU_SAMPLE) pods, which is then never shrunk to fit the time budget) as .npy files
+(dump_outputs), so that two builds can be compared output for output on identical seeded inputs.
 """
 import argparse
 import json
@@ -48,17 +52,36 @@ def measured_peak():
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
-def ncu_traffic(kernel):
-    p = ROOT / "profiles" / "traffic.json"
-    if p.exists():
-        try:
-            return json.loads(p.read_text()).get(kernel)
-        except Exception:
-            return None
-    return None
+DUMP_BYTES = 64 << 20  # --dump-outputs writes at most this much in all
+
+
+def dump_outputs(out_dir, res, n_types):
+    """What the timed path computed in its last step, as a caller of Scheduler.solve receives it, as float64 .npy files:
+    assign / relax_level per pod, new_node_info [n_new, 3] (provisioner, pods, options), new_node_options [n_new, ceil(T/32)]
+    (each node's surviving instance types as 32-bit words) and summary (scheduled pods, new nodes, the two 32-bit halves
+    of the whole-result digest). An array over its share of DUMP_BYTES keeps a fixed, seeded sample of its rows."""
+    import numpy as np
+    n_new = int(res.num_new_nodes)
+    words = np.zeros((n_new, (n_types + 31) // 32), dtype=np.uint32)
+    for i in range(n_new):
+        opts = res.new_node_options(i)
+        np.bitwise_or.at(words[i], opts >> 5, np.left_shift(np.uint32(1), (opts & 31).astype(np.uint32)))
+    assign = res.assign
+    digest = int(res.digest())
+    arrays = {"assign": assign, "relax_level": res.relax_level, "new_node_info": res.new_node_info(), "new_node_options": words,
+              "summary": np.array([(assign >= 0).sum(), n_new, digest >> 32, digest & 0xFFFFFFFF])}
+    out_dir = Path(out_dir)
+    out_dir.mkdir(parents=True, exist_ok=True)
+    share = DUMP_BYTES // len(arrays)
+    for name, a in arrays.items():
+        a = np.asarray(a, dtype=np.float64)
+        if a.nbytes > share:
+            keep = max(1, share // (a.nbytes // len(a)))
+            a = a[np.sort(np.random.default_rng(0).choice(len(a), keep, replace=False))]
+        np.save(out_dir / f"{name}.npy", a)
 
 
 def golden(config, pods, types, seed):
@@ -151,7 +174,8 @@ def run_reference(args, rank, world):
         t0 = time.perf_counter()
         oracle.solve(problem, res)
         first = time.perf_counter() - t0
-        if first * (args.steps + args.warmup) <= budget_s or sample <= 250:
+        # a dump must not depend on the host's speed: its sample is fixed by --config / --pods
+        if args.dump_outputs or first * (args.steps + args.warmup) <= budget_s or sample <= 250:
             break
         sample = max(250, sample // 2)
     for _ in range(max(0, args.warmup - 1)):
@@ -162,6 +186,8 @@ def run_reference(args, rank, world):
         oracle.solve(problem, res)
         total += time.perf_counter() - t0
         scheduled = int((res.assign >= 0).sum())
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, res, types)
     value = scheduled * args.steps / total
     sample_desc = f"first-fit Solve of a {sample}-pod batch of the same generator ({types} instance types), {args.steps} runs of {total / args.steps:.2f} s; " \
                   f"literal port, 1 thread of {os.cpu_count()}; the per-pod cost grows with the batch, so this over-states the reference at {pods} pods"
@@ -328,6 +354,7 @@ def main():
     ap.add_argument("--types", type=int, default=0)
     ap.add_argument("--no-cpu-baseline", action="store_true", help="skip the CPU legs and the secondary configurations (profiling runs)")
     ap.add_argument("--no-c5", action="store_true", help="skip the consolidation block (config_c5)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's result arrays to DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
 
@@ -405,6 +432,8 @@ def main():
     clocks = sampler.stop()
     dev_s = max_over_ranks(phase["total_us"] * 1e-6)
     res = rs.download()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, res, types)
     scheduled = int((res.assign >= 0).sum())
     tm = rs.timings()
     all_scheduled = sum_over_ranks(float(scheduled))
@@ -436,7 +465,7 @@ def main():
     # ---- feasibility kernel alone, cold L2, CUDA events on the launching stream
     rs.load()
     rs.run(flush_l2=False)
-    k1_us = sorted(rs.run_feasibility(flush_l2=True) for _ in range(max(8, args.steps)))
+    k1_us = sorted(rs.run_feasibility(flush_l2=True) for _ in range(args.steps))
     k1_avg = sum(k1_us) / len(k1_us)
     peak, peak_src = measured_peak()
     k1_bytes = tm["feasibility_bytes"]
@@ -479,15 +508,14 @@ def main():
                 "solve_only": {"value": all_scheduled * args.steps / so_s, "unit": "pods/s", "ms_per_step": 1000 * so_s / args.steps,
                                "path": "ksched_solve(handle, problem*, result*) with host buffers (flat structs in and out)"}},
         # own kernels per resident Solve: reset_kernel, sort_key1, gather_rows, class_feasibility, feasibility, pack, finalize_options
-        # (profiles/r02b_launch_shares.txt)
         "gpu_launches": 7 * args.steps,
         "roofline": {"kernel": "pack_kernel", "bound": "hbm", "achieved": pack_gbs, "peak": peak, "unit": "GB/s", "frac": pack_gbs / peak,
-                     "traffic": ncu_traffic(f"pack_kernel_c{args.config}"), "peak_source": peak_src, "algorithmic_bytes": int(pack_bytes),
+                     "peak_source": peak_src, "algorithmic_bytes": int(pack_bytes),
                      "us_per_launch": pack_avg_us,
                      "note": "latency-bound sequential first-fit chain; bytes = nodes_visited*128 + P*256 (SURVEY 8d K2) with the reference's "
                              "nodes_visited (it also walks full nodes; the kernel keeps them out of its active set)"},
         "roofline_feasibility": {"kernel": "feasibility_kernel", "bound": "hbm", "achieved": k1_gbs, "peak": peak, "unit": "GB/s", "frac": k1_gbs / peak,
-                                 "traffic": ncu_traffic(f"feasibility_kernel_c{args.config}"), "peak_source": peak_src, "algorithmic_bytes": int(k1_bytes),
+                                 "peak_source": peak_src, "algorithmic_bytes": int(k1_bytes),
                                  "us_per_launch": k1_avg, "us_min": k1_us[0],
                                  "physical_bytes": int(d["pods"] * 32 + d["pods"] * d["templates"] * d["type_words"] * 8 + d["pods"] * 8),
                                  "class_pass_us": rs.timings()["class_feasibility_us"],
@@ -498,7 +526,7 @@ def main():
     }
     if not args.no_c5:
         rs = None  # the handle now serves the consolidation pass
-        line["config_c5"] = c5_block(pkg, torch, dist, rank, world, 2)
+        line["config_c5"] = c5_block(pkg, torch, dist, rank, world, args.steps)
     if rank == 0:
         if gold:
             details["parity_vs_oracle"] = bool(int(res.digest()) == gold["digest"])
@@ -521,7 +549,7 @@ def main():
                 details["parity_vs_oracle"] = bool((want.assign == res.assign).all() and want.num_new_nodes == res.num_new_nodes)
             for c in (2, 3):
                 if c != args.config:
-                    line[f"config_c{c}"] = secondary(pkg, c)
+                    line[f"config_c{c}"] = secondary(pkg, c, args.steps)
         print(json.dumps(line), flush=True)
     if dist is not None:
         dist.destroy_process_group()

@@ -1,5 +1,5 @@
 /*
- * ksched — B200-native drop-in for Karpenter's provisioning scheduler hot path.
+ * ksched — H100-native (sm_90a) drop-in for Karpenter's provisioning scheduler hot path.
  *
  * C-ABI boundary: plain pointers and sizes only. A cgo shim in the reference would marshal the
  * arguments of scheduling.NewScheduler (pkg/controllers/provisioning/scheduling/scheduler.go:42-45)

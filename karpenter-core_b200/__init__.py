@@ -1,4 +1,4 @@
-"""karpenter-core_b200 — B200-native drop-in for Karpenter's provisioning scheduler hot path.
+"""karpenter-core_b200 — H100-native (sm_90a) drop-in for Karpenter's provisioning scheduler hot path.
 
 Python is only the test / bench harness here: every call goes through the C-ABI library
 `libksched.so` (include/ksched.h + the C++ host layer in host/). There is no Python or CPU

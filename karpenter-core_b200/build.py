@@ -13,7 +13,7 @@ from pathlib import Path
 PKG = Path(__file__).resolve().parent
 ROOT = PKG.parent
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 MODEL_SRCS = ["loader.cc", "synth.cc", "result_io.cc"]
 HOST_SRCS = ["encoder.cc", "scheduler.cc"]
@@ -36,6 +36,7 @@ def build_product(force=False, verbose_ptxas=False):
     out = PKG / "libksched.so"
     srcs = [PKG / "host" / s for s in HOST_SRCS] + [PKG / "csrc" / s for s in CUDA_SRCS]
     deps = srcs + list((PKG / "host").glob("*.h")) + list((PKG / "csrc").glob("*.cuh")) + list((ROOT / "include").glob("*.h"))
+    deps.append(Path(__file__))  # the flags (ARCH) live in this file
     if not force and not _newer(out, deps):
         return out
     cmd = [NVCC, *ARCH, "-O3", "-std=c++17", "-lineinfo", "-shared", "-Xcompiler", "-fPIC,-Wall",
@@ -53,7 +54,7 @@ def build_product(force=False, verbose_ptxas=False):
 def build_model(force=False):
     out = PKG / "libkmodel.so"
     srcs = [PKG / "host" / s for s in MODEL_SRCS]
-    deps = srcs + list((PKG / "host").glob("*.h"))
+    deps = srcs + list((PKG / "host").glob("*.h")) + [Path(__file__)]  # the flags (ARCH) live in this file
     if not force and not _newer(out, deps):
         return out
     # linked by nvcc's host toolchain like libksched.so (shared libstdc++): objects of one library are read by the other

@@ -1,4 +1,4 @@
-// ksched.cu — sm_100a kernels and the C-ABI of include/ksched.h.
+// ksched.cu — sm_90a kernels and the C-ABI of include/ksched.h.
 //
 //  K0  sort_keys / gather_rows   FFD order of the queue (queue.go:35-110) and the dense, FFD-ordered
 //                                P x 256 B pod-row matrix the feasibility kernel streams.
@@ -147,6 +147,7 @@ struct ksched_handle {
   K1Params k1_host;  // staging copies of the kernels' constant-memory parameters (must outlive the async copies)
   K2Params k2_host;  // staging copy of the pack kernel's constant-memory parameters (must outlive the async copy)
   int device = 0;
+  int n_sm = 132;  // streaming multiprocessors of `device` (grid sizes of the grid-stride kernels)
   cudaStream_t stream = nullptr;
   std::string err;
   // catalog
@@ -274,7 +275,9 @@ int ksched_create(int device_ordinal, ksched_handle** out) {
   if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0 || device_ordinal >= n) return KSCHED_ERR_NO_DEVICE;
   ksched_handle* h = new ksched_handle();
   h->device = device_ordinal;
-  if (cudaSetDevice(device_ordinal) != cudaSuccess || cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) {
+  if (cudaSetDevice(device_ordinal) != cudaSuccess || cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess ||
+      cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, device_ordinal) != cudaSuccess) {
+    if (h->stream) cudaStreamDestroy(h->stream);
     delete h;
     return KSCHED_ERR_CUDA;
   }
@@ -846,7 +849,7 @@ static int run_sort(ksched_handle* h) {
     size_t tmp1 = h->cub_tmp_bytes;
     CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(h->d_cub_tmp.ptr, tmp1, h->d_k_tie.ptr, h->d_k_tmp.ptr, h->d_idx_tmp.ptr, h->d_order.ptr, P, 0, h->sort1_bits,
                                                 h->stream));
-    const int gblocks1 = std::min((P + 7) / 8, 148 * 8);
+    const int gblocks1 = std::min((P + 7) / 8, h->n_sm * 8);
     gather_rows_kernel<<<gblocks1, 256, 0, h->stream>>>(P, h->d_classes.ptr, h->d_pod_class.ptr, h->d_order.ptr, h->d_rows.ptr);
     h->tm.sort_launches = 3;
     h->sorted = true;
@@ -865,7 +868,7 @@ static int run_sort(ksched_handle* h) {
   tmp = h->cub_tmp_bytes;
   CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(h->d_cub_tmp.ptr, tmp, h->d_k_tie.ptr, h->d_k_tmp.ptr, ia, ib, P, 0, 64, h->stream));
   CUDA_TRY(h, cudaMemcpyAsync(h->d_order.ptr, ib, (size_t)P * sizeof(uint32_t), cudaMemcpyDeviceToDevice, h->stream));
-  const int gblocks = std::min((P + 7) / 8, 148 * 8);
+  const int gblocks = std::min((P + 7) / 8, h->n_sm * 8);
   gather_rows_kernel<<<gblocks, 256, 0, h->stream>>>(P, h->d_classes.ptr, h->d_pod_class.ptr, h->d_order.ptr, h->d_rows.ptr);
   h->tm.sort_launches = 7;
   h->sorted = true;
@@ -907,9 +910,9 @@ static int run_class_feasibility(ksched_handle* h) {
   const size_t table_bytes = (size_t)(h->n_valrows + 2 * c.n_keys + h->n_offrows + 1 + c.n_templates) * c.W32 * sizeof(uint32_t);
   k1.tables_in_smem = smem + table_bytes <= (size_t)(160 << 10) ? 1 : 0;
   if (k1.tables_in_smem) smem += table_bytes;
-  // one warp per class row (a row evaluation is ~10k cycles of dependent work: no chunking)
+  // one warp per class row (a row evaluation is thousands of cycles of dependent work: no chunking)
   const int warps_per_block = kK1Threads / 32;
-  const int blocks = std::max(1, std::min(148 * 2, (h->n_classes + warps_per_block - 1) / warps_per_block));
+  const int blocks = std::max(1, std::min(h->n_sm * 2, (h->n_classes + warps_per_block - 1) / warps_per_block));
   k1.dbg = nullptr;
 #ifdef KSCHED_PROFILE_K1
   CUDA_TRY(h, h->d_k1dbg.ensure(8));
@@ -948,7 +951,7 @@ static int run_feasibility(ksched_handle* h) {
   if (h->n_pods == 0) return KSCHED_OK;
   const int RW = h->cat.n_templates * h->cat.W32;
   const int nblk = (h->n_pods + 31) / 32;
-  const int blocks = std::max(1, std::min(148 * 8, (nblk + 7) / 8));  // 8 warps per CTA, one 32-row block per warp and iteration
+  const int blocks = std::max(1, std::min(h->n_sm * 8, (nblk + 7) / 8));  // 8 warps per CTA, one 32-row block per warp and iteration
   feasibility_kernel<<<blocks, 256, 0, h->stream>>>(h->d_rows.ptr, h->n_pods, h->n_classes, RW, h->d_Fclass.ptr, h->d_best_class.ptr, h->d_F.ptr,
                                                     h->d_best.ptr);
   CUDA_TRY(h, cudaGetLastError());
@@ -1013,7 +1016,7 @@ static int reset_state(ksched_handle* h, const int64_t* d_remaining_src = nullpt
     CUDA_TRY(h, cudaMemcpyAsync(h->d_remaining.ptr, rem.data(), rem.size() * 8, cudaMemcpyHostToDevice, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // rem is a stack vector
   }
-  reset_kernel<<<148 * 2, 256, 0, h->stream>>>(t);
+  reset_kernel<<<h->n_sm * 2, 256, 0, h->stream>>>(t);
   CUDA_TRY(h, cudaGetLastError());
   return KSCHED_OK;
 }
@@ -1058,7 +1061,7 @@ static int run_pack(ksched_handle* h) {
   s.grp_active = h->d_grp_active.ptr; s.grp_min_slot = h->d_grp_min_slot.ptr;
   s.counters = h->d_counters.ptr;
   const size_t alloc_bytes = (size_t)h->cat.n_res * h->cat.n_types * sizeof(int64_t);
-  // 227 KB per CTA on sm_100a: the hot node window + ~4 KB of static shared memory come first
+  // 227 KB per CTA on sm_90a: the hot node window + ~4 KB of static shared memory come first
   const size_t static_smem = (size_t)(14 << 10);  // file-scope __shared__ objects (pod row, PodTopo, RunCtx with its variants, scratch)
   const size_t smem_left = (size_t)(227 << 10) - sizeof(HotSmem) - kRunArrayBytes - static_smem;
   s.alloc_in_smem = alloc_bytes <= smem_left ? 1 : 0;
@@ -1066,7 +1069,7 @@ static int run_pack(ksched_handle* h) {
   const size_t smem = sizeof(HotSmem) + (size_t)s.run_off + kRunArrayBytes;
   s.any_limits = 0;
   for (const ksched_template& tm : h->h_templates) if (tm.has_limits && tm.limit_present) s.any_limits = 1;
-  s.use_warp_loop = getenv("KSCHED_WARPLOOP") ? 1 : 0;  // superseded by the class-run loop (kept for A/B timing: 18 ms vs 8 ms on C2 when both are on)
+  s.use_warp_loop = getenv("KSCHED_WARPLOOP") ? 1 : 0;  // superseded by the class-run loop (kept for A/B timing)
   s.use_class_run = getenv("KSCHED_NO_CLASSRUN") ? 0 : 1;
   s.use_level_step = std::getenv("KSCHED_NO_LEVELSTEP") ? 0 : 1;
   s.use_level_run = std::getenv("KSCHED_NO_LEVELRUN") ? 0 : 1;
@@ -1089,15 +1092,15 @@ static int run_pack(ksched_handle* h) {
     CUDA_TRY(h, cudaGetLastError());
     CUDA_TRY(h, cudaEventRecord(done, h->stream));
   }
-  finalize_options_kernel<<<148, 256, 0, h->stream>>>(h->cat, h->d_counters.ptr, h->d_nn_req.ptr, h->d_nn_req_present.ptr, h->d_nn_opts.ptr, h->max_new);
+  finalize_options_kernel<<<h->n_sm, 256, 0, h->stream>>>(h->cat, h->d_counters.ptr, h->d_nn_req.ptr, h->d_nn_req_present.ptr, h->d_nn_opts.ptr, h->max_new);
   h->tm.pack_launches = 2;
   return KSCHED_OK;
 }
 
 static int flush_l2(ksched_handle* h) {
-  const size_t n = (size_t)64 << 20;  // 256 MiB of u32 > 126 MB L2
+  const size_t n = (size_t)64 << 20;  // 256 MiB of u32, five times the 50 MB L2 of an H100
   CUDA_TRY(h, h->d_flush.ensure(n));
-  flush_kernel<<<148 * 4, 512, 0, h->stream>>>(h->d_flush.ptr, n);
+  flush_kernel<<<h->n_sm * 4, 512, 0, h->stream>>>(h->d_flush.ptr, n);
   return KSCHED_OK;
 }
 
@@ -1235,7 +1238,7 @@ int ksched_download(ksched_handle* h, const ksched_problem* pb, ksched_result* r
   if (res->launch && n_new > 0) {
     if (!h->cat.offer_keys) { h->err = "ksched_result.launch needs ksched_catalog.offering_keys"; return KSCHED_ERR_INVALID; }
     CUDA_TRY(h, h->d_launch.ensure((size_t)n_new));
-    launch_choice_kernel<<<148, 256, 0, h->stream>>>(h->cat, h->d_counters.ptr, h->d_nn_vals.ptr, h->d_nn_meta.ptr, h->d_nn_opts.ptr, MAXN,
+    launch_choice_kernel<<<h->n_sm, 256, 0, h->stream>>>(h->cat, h->d_counters.ptr, h->d_nn_vals.ptr, h->d_nn_meta.ptr, h->d_nn_opts.ptr, MAXN,
                                                      h->d_launch.ptr);
     CUDA_TRY(h, cudaMemcpyAsync(res->launch, h->d_launch.ptr, (size_t)n_new * sizeof(ksched_launch_choice), cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));

@@ -1,6 +1,6 @@
 // K2 — pack_kernel: Scheduler.add's sequential first-fit (scheduler.go:174-219) in one persistent CTA.
 //
-// Design (B200-first, latency-bound integer work; DESIGN.md section 4 has the long form):
+// Design (latency-bound integer work; DESIGN.md section 4 has the long form):
 //  * one CTA (128..512 threads), one pod per iteration, three speeds: a register-resident warp loop when at most 32
 //    nodes are open and the pod cannot change any requirement (warp_resident_loop), a block-wide fast path over the
 //    shared-memory window of open nodes, and the out-of-line generic step (existing nodes, requirement / topology
@@ -181,8 +181,8 @@ __device__ __forceinline__ void block_min2_u32_db(unsigned a, unsigned b, unsign
 
 // compute_front with the whole CTA (same result, every thread calls it): the per-resource arg-max types are found by
 // probing each resource's descending order T positions at a time (block minimum of the first hit), the pair coverage test
-// runs one option word per thread. The serial version walks the orders and the words through dependent L2 loads - 30 000
-// cycles per fresh node of a new shape on the 1 000-type catalog (profiles/README.md, round 2).
+// runs one option word per thread. The serial version walks the orders and the words through dependent L2 loads, tens of
+// thousands of cycles per fresh node of a new shape on the 1 000-type catalog.
 __shared__ unsigned g_front_pairs;
 __device__ __noinline__ void compute_front_block(const uint32_t* opts, int stride, int n, long long* b1, long long* b2, unsigned short* bits,
                                                  unsigned long long (*red)[32], int& parity) {

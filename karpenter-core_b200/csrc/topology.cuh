@@ -130,7 +130,7 @@ struct K2Params {
 };
 // The pack kernel and every out-of-line device function it calls read their parameters from constant memory with
 // immediate offsets (a reference to a __grid_constant__ kernel parameter handed to a __noinline__ function degrades every
-// field access to a generic load with ~100 cycles of latency, on a code path that is one dependent chain).
+// field access to a generic load from the parameter window, on a code path that is one dependent chain).
 // One copy per device: run_pack() orders launches of different handles on the same device behind each other.
 __constant__ K2Params g_k2;
 #define KS_K2 const DevCatalog& c = g_k2.cat; const PackState& s = g_k2.st; (void)c; (void)s;

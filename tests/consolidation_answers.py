@@ -156,7 +156,7 @@ def will_not_merge_two_nodes_into_one_of_the_same_type():
 
 
 # ---- cases added after the round's GPU budget was spent: pinned on the oracle (CPU); the GPU parametrisation of
-# tests/test_gpu_parity.py takes CASES only, these join it once they have been run on a B200.
+# tests/test_gpu_parity.py takes CASES only, these join it once they have been run on the GPU.
 CPU_ONLY_CASES = []
 
 

@@ -1,5 +1,7 @@
-import sys, os
-sys.path.insert(0,'/root/repo'); sys.path.insert(0,'tests')
+import sys
+from pathlib import Path
+ROOT = Path(__file__).resolve().parent.parent
+sys.path.insert(0, str(ROOT / "tests")); sys.path.insert(0, str(ROOT))
 from __graft_entry__ import load_pkg
 k=load_pkg()
 p=k.Problem.synth(2,10000,500,42,0)

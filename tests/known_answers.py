@@ -760,7 +760,7 @@ def _eq(a, b):
 
 # ================================================================== cases added after the round's GPU budget was spent
 # Pinned on the oracle (tests/test_oracle_known_answers.py runs CASES + CPU_ONLY_CASES); tests/test_gpu_known_answers.py takes
-# CASES only - these move up once they have been run on a B200.
+# CASES only - these move up once they have been run on the GPU.
 CPU_ONLY_CASES = []
 
 

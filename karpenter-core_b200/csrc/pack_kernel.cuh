@@ -416,7 +416,10 @@ __device__ __forceinline__ bool class_has_volumes(const PackState& s, unsigned c
 }
 struct ExRunIO { int qi, head, qlen, seq, parity, placed; long long add_calls; };
 __shared__ ExRunIO g_xio;
-__shared__ int g_xscan[2][8];
+// one partial sum per warp, double-buffered: every warp of the largest block the kernel is launched with needs a slot
+constexpr int kScanWarps = kPackThreads / 32;
+static_assert(kScanWarps * 32 == kPackThreads, "block_scan_incl: kPackThreads is a whole number of warps");
+__shared__ int g_xscan[2][kScanWarps];
 __device__ __forceinline__ int block_scan_incl(int v, int* total, int& xpar) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
   int x = v;

@@ -6,6 +6,7 @@ import pytest
 
 import consolidation_answers as ca
 import fixtures as fx
+import run_problems
 from ranking_answers import CASES as RANK_CASES, SINGLE
 
 pytestmark = pytest.mark.gpu
@@ -140,6 +141,23 @@ def _candidate_cluster(seed):
             node["disruptionCost"] = float(rng.choice([0, 1, 1, 2, 3]))
             n += 1
     return prob, n
+
+
+@pytest.mark.parametrize("seed,zones,ct_spread", [(1, 9, False), (2, 16, False), (3, 9, True)])
+def test_snapshot_equals_oracle_on_wide_zone_clusters(pkg, oracle, seed, zones, ct_spread):
+    """run-shaped clusters: zone spread over 9 or 16 zones, and zone plus capacity-type spread (two mask relations)"""
+    problem = pkg.Problem.from_dict(run_problems.cluster(seed, zones, ct_spread))
+    cs = pkg.ClusterSession(problem)
+    assert cs.resident
+    n = cs.n_candidates
+    assert n == 3 * zones
+    prefixes = [list(range(c)) for c in range(1, n + 1)]
+    for s_, g in zip(prefixes, cs.probe_sets(prefixes, True)):
+        assert g == oracle.consolidate_probe(problem, len(s_)), ("prefix", len(s_))
+    singles = [[i] for i in range(n)]
+    for s_, g in zip(singles, cs.probe_sets(singles, False)):
+        w = oracle.consolidate_single(problem, s_[0])
+        assert g == (w["action"], w["options"]), ("single", s_)
 
 
 @pytest.mark.parametrize("seed", [s for s in range(400) if _candidate_cluster(s)[1] >= 2][:60])

@@ -3,6 +3,7 @@ loudly with KSCHED_ERR_UNSUPPORTED (never a silently different answer)."""
 import pytest
 
 from fuzz_problems import random_problem, random_problem_with_bounds
+from oracle_compare import compare
 
 pytestmark = pytest.mark.gpu
 
@@ -19,27 +20,4 @@ def test_gpu_equals_oracle_on_random_problem(pkg, oracle, seed):
 
 
 def _compare(pkg, oracle, prob):
-    problem = pkg.Problem.from_dict(prob)
-    want = pkg.Result()
-    assert oracle.solve(problem, want) == 0, want.error
-    try:
-        got = pkg.Scheduler(problem).solve()
-    except pkg.KschedError as e:
-        if e.code == pkg.KSCHED_ERR_UNSUPPORTED:
-            pytest.skip(f"refused loudly: {e}")
-        raise
-    g, w = got.to_dict(), want.to_dict()
-    assert g["assign"] == w["assign"]
-    assert g["relax"] == w["relax"]
-    assert g["existing"] == w["existing"]
-    assert len(g["newNodes"]) == len(w["newNodes"])
-    for a, b in zip(g["newNodes"], w["newNodes"]):
-        assert a["provisioner"] == b["provisioner"] and a["pods"] == b["pods"]
-        assert a["options"] == b["options"]
-        assert a["requests"] == b["requests"]
-        assert a["requirements"] == {k: v for k, v in b["requirements"].items() if k != "node.kubernetes.io/instance-type"}
-        assert a.get("launch") == b.get("launch") and a.get("launch") is not None  # launch choice (device kernel vs oracle)
-    assert got.nodes_visited == want.nodes_visited
-    fast = pkg.Scheduler(problem).solve(count_visited=False).to_dict()  # production setting: steady-state kernel paths
-    assert fast["assign"] == w["assign"] and fast["relax"] == w["relax"] and fast["existing"] == w["existing"]
-    assert fast["newNodes"] == g["newNodes"]
+    compare(pkg, oracle, pkg.Problem.from_dict(prob), add_calls=False, refusal_skips=True)

@@ -2,8 +2,9 @@
 
 Compared per problem: the pod->node assignment vector, relaxation levels, and for every new node its
 provisioner, pods in Add order, surviving instance-type options, requests and final requirements."""
-import numpy as np
 import pytest
+
+from oracle_compare import compare
 
 pytestmark = pytest.mark.gpu
 
@@ -21,44 +22,16 @@ SMALL = [
 ]
 
 
-def _compare(pkg, oracle, problem, candidates=()):
-    want = pkg.Result()
-    assert oracle.solve(problem, want, candidates) == 0, want.error
-    got = pkg.Scheduler(problem).solve(candidates)
-    w, g = want.to_dict(), got.to_dict()
-    assert g["assign"] == w["assign"]
-    assert g["relax"] == w["relax"]
-    assert len(g["newNodes"]) == len(w["newNodes"])
-    for i, (a, b) in enumerate(zip(g["newNodes"], w["newNodes"])):
-        assert a["provisioner"] == b["provisioner"], i
-        assert a["pods"] == b["pods"], i
-        assert a["options"] == b["options"], i
-        assert a["requests"] == b["requests"], i
-        breq = {k: v for k, v in b["requirements"].items() if k != "node.kubernetes.io/instance-type"}
-        assert a["requirements"] == breq, i
-        assert a.get("launch") == b.get("launch") and a.get("launch") is not None, i
-    assert g["existing"] == w["existing"]
-    assert got.nodes_visited == want.nodes_visited
-    assert got.add_calls == want.add_calls
-    # production setting (no nodes_visited statistic): the steady-state kernel paths must give the identical result
-    fast = pkg.Scheduler(problem).solve(candidates, count_visited=False)
-    f = fast.to_dict()
-    assert f["assign"] == w["assign"] and f["relax"] == w["relax"] and f["existing"] == w["existing"]
-    for a, b in zip(f["newNodes"], g["newNodes"]):
-        assert a == b
-    return got, want
-
-
 @pytest.mark.parametrize("config,pods,types,nodes,seed", SMALL)
 def test_synthetic_configs_match_oracle(pkg, oracle, config, pods, types, nodes, seed):
     problem = pkg.Problem.synth(config, pods, types, seed, nodes)
-    _compare(pkg, oracle, problem)
+    compare(pkg, oracle, problem)
 
 
 def test_simulation_with_candidates_matches_oracle(pkg, oracle):
     problem = pkg.Problem.synth(5, 600, 1000, 42, 60)
     for cands in ([0], [3, 4, 5], list(range(10))):
-        _compare(pkg, oracle, problem, cands)
+        compare(pkg, oracle, problem, cands)
 
 
 def test_multi_node_consolidation_matches_oracle(pkg, oracle):
@@ -141,7 +114,7 @@ def test_two_handles_on_one_device_solve_concurrently(pkg, oracle):
     b = pkg.Problem.synth(3, 2000, 1000, 6, 0)
     assert pkg.lib().kh_selftest_two_handles(a.ptr, b.ptr, 6) == 0
     # and the singleton handle still agrees with the oracle afterwards
-    _compare(pkg, oracle, a, [])
+    compare(pkg, oracle, a, [])
 
 
 from consolidation_answers import CASES as _CONS, CPU_ONLY_CASES as _CONS_LATE
@@ -170,7 +143,7 @@ def test_consolidation_known_answers_match_oracle(pkg, oracle, name, ref, build)
     check(probe, search)
 
 
-CLASS_RUN_SWITCHES = ("KSCHED_NO_LEVELWARP", "KSCHED_NO_MASKRUN", "KSCHED_NO_LEVELRUN", "KSCHED_NO_CLASSRUN")
+CLASS_RUN_SWITCHES = ("KSCHED_NO_LEVELWARP", "KSCHED_NO_MASKRUN", "KSCHED_NO_LEVELRUN", "KSCHED_NO_CLASSRUN", "KSCHED_NO_LEVELSTEP", "KSCHED_WARPLOOP")
 
 
 @pytest.mark.parametrize("config,pods,types,seed", [(4, 6000, 1000, 7), (4, 2500, 1000, 3), (3, 5000, 1000, 7), (2, 3000, 500, 7), (2, 4000, 40, 9)])
@@ -184,7 +157,8 @@ def test_class_run_modes_agree(pkg, monkeypatch, config, pods, types, seed):
     rs.set_count_visited(False)
     rs.load()
     digests = {}
-    for off in ("", "KSCHED_NO_LEVELWARP", "KSCHED_NO_MASKRUN", "KSCHED_NO_LEVELRUN,KSCHED_NO_MASKRUN", "KSCHED_NO_CLASSRUN"):
+    for off in ("", "KSCHED_NO_LEVELWARP", "KSCHED_NO_MASKRUN", "KSCHED_NO_LEVELRUN,KSCHED_NO_MASKRUN", "KSCHED_NO_CLASSRUN", "KSCHED_NO_LEVELSTEP",
+                "KSCHED_WARPLOOP"):
         for v in CLASS_RUN_SWITCHES:
             monkeypatch.delenv(v, raising=False)
         for v in off.split(","):

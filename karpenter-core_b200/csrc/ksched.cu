@@ -49,6 +49,7 @@ constexpr int kMaxCG = 8;        // topology groups that may constrain one pod c
 constexpr int kMaxTouched = 8;   // requirement keys one Add may touch (pod keys + topology keys)
 constexpr int kPackThreads = 512;
 constexpr int kFreshMemoSlots = 8192;  // PackState::fd_*
+constexpr int kNumCounters = 64;       // PackState::counters
 constexpr uint64_t kNoBest = ~0ull;
 
 #include "catalog.cuh"
@@ -228,7 +229,7 @@ struct ksched_handle {
   DevBuf<uint64_t> d_ex_vals, d_ex_vals0, d_ex_meta, d_ex_meta0, d_ex_hp, d_ex_hp0, d_nn_vals, d_nn_meta, d_nn_hp, d_grp_registered,
       d_grp_registered0;
   DevBuf<uint16_t> d_grp_host, d_grp_host0;
-  DevBuf<long long> d_counters, d_k1dbg;
+  DevBuf<long long> d_counters, d_k1dbg;  // d_counters: kNumCounters entries (0..5 results, the rest KSCHED_PROFILE_PACK)
   DevBuf<uint32_t> d_flush;
   size_t cub_tmp_bytes = 0;
   // one-pass queue order (feasibility_kernel.cuh: sort_key1_kernel): total key bits, 0 = the three-key path
@@ -825,7 +826,7 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
     CUDA_TRY(h, h->d_fd_bound.ensure(nfd * 4)); CUDA_TRY(h, h->d_fd_bound2.ensure(nfd * 4));
   }
   CUDA_TRY(h, h->d_remaining.ensure((size_t)V * KSCHED_MAX_RES));
-  CUDA_TRY(h, h->d_counters.ensure(48));
+  CUDA_TRY(h, h->d_counters.ensure(kNumCounters));
   {
     size_t need = 0, n2 = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, need, (uint64_t*)nullptr, (uint64_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)p1, 0, 64, h->stream);
@@ -1004,7 +1005,7 @@ static int reset_state(ksched_handle* h, const int64_t* d_remaining_src = nullpt
   add(h->d_grp_host.ptr, h->d_grp_host0.ptr, hs * 2);
   if (d_remaining_src)  // simulation on the cluster snapshot: limits with the removed nodes' capacity given back, already on the device
     add(h->d_remaining.ptr, d_remaining_src, (size_t)h->cat.n_templates * KSCHED_MAX_RES * 8);
-  add(h->d_counters.ptr, nullptr, 48 * sizeof(long long));
+  add(h->d_counters.ptr, nullptr, kNumCounters * sizeof(long long));
   add(h->d_fc_state.ptr, nullptr, (size_t)std::max(h->n_classes, 1) * h->cat.n_templates);
   add(h->d_fc_front_state.ptr, nullptr, (size_t)std::max(h->n_classes, 1) * h->cat.n_templates);
   add(h->d_fd_state.ptr, nullptr, (size_t)kFreshMemoSlots);
@@ -1175,6 +1176,9 @@ static void print_pack_profile(const long long* counters) {
           counters[14]);
   fprintf(stderr, "[pack profile] mask run steps=%lld with >1 admissible domain=%lld round-able=%lld (counters shared with generic n/fresh: ignore there)\n", counters[18], counters[19], counters[17]);
   fprintf(stderr, "[pack profile] mask run: build cycles=%lld (refused %lld) loop cycles=%lld pods=%lld entries=%lld\n", counters[38], counters[47], counters[6], counters[7], counters[16]);
+  fprintf(stderr, "[pack profile] mask run: single steps on the unpinned head=%lld | pin steps=%lld pods=%lld ended by "
+                  "[staged entries,count,key,refused,end of list or 32 pods]=%lld,%lld,%lld,%lld,%lld\n",
+          counters[48], counters[49], counters[50], counters[51], counters[52], counters[53], counters[54], counters[55]);
   fprintf(stderr, "[pack profile] class_run without mask-key spread: cycles=%lld pods=%lld level+fill iterations=%lld (fill %lld) fresh=%lld per-pod=%lld | with: cycles=%lld pods=%lld fresh=%lld per-pod=%lld\n",
           counters[32], counters[33], counters[34], counters[46], counters[35], counters[44], counters[36], counters[37], counters[39], counters[45]);
 }
@@ -1184,7 +1188,7 @@ int ksched_download(ksched_handle* h, const ksched_problem* pb, ksched_result* r
   if (!h || !pb || !res || !h->uploaded) return KSCHED_ERR_INVALID;
   CUDA_TRY(h, cudaSetDevice(h->device));
   const int P = h->n_pods, NE = h->n_existing, MAXN = h->max_new, W32 = h->cat.W32, W64 = h->W64, V = h->cat.n_templates;
-  long long counters[48];
+  long long counters[kNumCounters];
   CUDA_TRY(h, cudaMemcpyAsync(counters, h->d_counters.ptr, sizeof counters, cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
 #ifdef KSCHED_PROFILE_PACK
@@ -1418,7 +1422,7 @@ int ksched_simulate_batch(ksched_handle* h, const ksched_candidate_set* sets, in
   CUDA_TRY(h, cudaEventRecord(h->ev[4], h->stream));
 #ifdef KSCHED_PROFILE_PACK
   {
-    long long counters[48];
+    long long counters[kNumCounters];
     CUDA_TRY(h, cudaMemcpyAsync(counters, h->d_counters.ptr, sizeof counters, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     print_pack_profile(counters);  // the last simulation of the batch

@@ -1393,6 +1393,10 @@ struct M1Ctx {
   uint16_t ae[kM1Lv][kM1Lists];
   int bcnt[kM1Lv * kM1Lists];         // build: members per bucket (bucket = list * kM1Lv + count)
   int bad;                            // build: a node the lists cannot represent
+  int upos;                           // position of the unpinned list's head in arr: that list never gains a member (a node
+                                      // leaves it when a pod pins it, fresh nodes are pinned), so it is the rest of the
+                                      // segment the build sorted, and the pin step reads its next members without the links
+  uint16_t ps[32];                    // pin step: the node of each pod
   int out_adv, out_reason, out_tick, out_n_new, out_n_active;
   int n_fresh;                        // nodes created by this entry of the warp loop: slot | variant << 16; their global
   uint32_t fr[kRunChunk];             // state (option words, requirement values, requests, ...) is stored by the CTA afterwards
@@ -1755,6 +1759,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
             m1.tl[lv][list] = m1.ae[lv][list] > m1.ap[lv][list] ? m1_arr[m1.ae[lv][list] - 1] : kM1None;
           }
           if (tid < kM1Lists) m1.head[tid] = m1.ae[kM1Lv - 1][tid] > m1.ap[0][tid] ? m1_arr[m1.ap[0][tid]] : kM1None;
+          if (tid == 0) m1.upos = m1.ap[0][kM1Dom];
         }
         __syncthreads();
         if (bad) m1_ok = false;
@@ -1989,6 +1994,124 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
           }
           if (wkey != ~0ull) {
             const int wl = __ffs(__ballot_sync(FULL, key == wkey)) - 1;
+            if (wl == kM1Dom) {
+              // ---- pin step: the unpinned head wins, so the next pods take the next unpinned nodes one each, in list order
+              // (lane t: pod t), as long as no node of a domain list can come first: every member of the stretch has the
+              // first one's pod count c and a key below every pinned head (a node pinned by the stretch re-enters at c + 1).
+              // Pod t's domain is the t-th pick of run_pick's (count, id) order while the counts advance.
+              const int c = (int)(wkey >> 32);
+              const int upos = m1.upos;
+              int lim = i_end - li < 32 ? i_end - li : 32;
+              if (m1.ae[kM1Lv - 1][kM1Dom] - upos < lim) lim = m1.ae[kM1Lv - 1][kM1Dom] - upos;
+              const unsigned long long pmin = warp_min_u64(L < kM1Dom ? hk : ~0ull);
+              const bool in = L < lim;
+              const int a_t = in ? (int)m1_arr[upos + L] : 0;
+              const unsigned long long k_t = in ? hs->key[a_t] : ~0ull;
+              const uint32_t rp_t = in ? rpv[a_t] : 0u;
+              const uint32_t z_t = in ? zv[a_t] : 0u;
+              int d_t;
+              {
+                // domain e has a slot on every level >= its count; pod t takes the t-th slot in (level, id) order (without
+                // Record the counts stay, and every pod takes the first pick). Levels are counted from mn: pod t's level is
+                // at most t, so a domain more than 31 pods above mn never gets one. Byte e of dw: domain e's level.
+                const unsigned dl = !valid ? 0xFFu : (unsigned)(cnt_d - mn < 32 ? cnt_d - mn : 32);
+                const unsigned dw0 = __reduce_or_sync(FULL, L < 4 ? dl << (8 * L) : 0u);
+                const unsigned dw1 = __reduce_or_sync(FULL, L >= 4 && L < kM1Dom ? dl << (8 * (L - 4)) : 0u);
+                unsigned y = 0, r = m_rec0 ? L : 0, am;
+                while (true) {
+                  const unsigned yy = y * 0x01010101u;  // bit 0 of every byte of the compares -> bits 24..27 (no carries)
+                  am = (((__vcmpleu4(dw0, yy) & 0x01010101u) * 0x01020408u) >> 24) & 0xFu;
+                  am |= (((__vcmpleu4(dw1, yy) & 0x01010101u) * 0x01020408u) >> 20) & 0xF0u;
+                  const unsigned k = __popc(am);
+                  if (am == m_reg0) { r %= k; break; }  // every domain has a slot on every level from here on
+                  if (r < k) break;
+                  r -= k;
+                  ++y;
+                }
+                for (; r > 0; --r) am &= am - 1;
+                d_t = __ffs(am) - 1;
+              }
+              const bool same_c = (int)(k_t >> 32) == c, below = k_t < pmin;
+              const bool ok_t = in && same_c && below && (rp_t & 0xFFFF) != kRoomSlow && c + 1 < kM1Lv &&
+                                ((rc.m_neutral[0] >> d_t) & 1) && ((z_t & (1u << 17)) || rc.m_wk[0]);
+              const unsigned okb = __ballot_sync(FULL, ok_t);
+              const int J = okb == FULL ? 32 : __ffs(~okb) - 1;
+#ifdef KSCHED_PROFILE_PACK
+              if (J > 0 && L == J) s.counters[!in ? (lim == i_end - li ? 51 : 55) : !same_c ? 52 : !below ? 53 : 54] += 1;
+              if (J == 32 && L == 0) s.counters[55] += 1;
+              if (J > 0 && L == 0) { s.counters[49] += 1; s.counters[50] += J; }
+#endif
+              if (J > 0) {
+                bool closed_l = false;
+                if (L < J) {  // the single step's commit for pod L on node a_t, pinned to d_t
+                  const int a = a_t, mytick = ltick + L;
+                  uint32_t rp2 = rp_t - 1 + (1u << 16);
+                  for (int j = 0; j < n_host; ++j) {  // Topology.Record, hostname groups
+                    const int times = rc.h_times[j];
+                    const int old = hc[j * kTopoCap + a];
+                    const int now = old + times > 0xFFFF ? 0xFFFF : old + times;
+                    if (times) hc[j * kTopoCap + a] = (uint16_t)now;
+                    if (now > rc.h_lim[j]) rp2 |= kRpDead;
+                  }
+                  const int n = hs->node[a], k = rc.m_key[0];
+                  zv[a] = (1u << d_t) | (3u << 16);
+                  s.nn_vals[(size_t)k * MAXN + n] = 1ull << d_t;
+                  atomicOr(reinterpret_cast<unsigned long long*>(&s.nn_meta[n]), 1ull << (KSCHED_META_PRESENT_SHIFT + k));
+                  atomicAnd(reinterpret_cast<unsigned long long*>(&s.nn_meta[n]), ~(1ull << (KSCHED_META_COMPLEMENT_SHIFT + k)));
+                  rc.q_node[buf][li + L] = -(a + 2);
+                  unsigned long long skey = order_key(c + 1, -(mytick + 1));
+                  if ((rp2 & 0xFFFF) == 0) {  // the class no longer fits by resources: does anything? (node_closed)
+                    const int placed = (rp2 >> 16) & 0x7FFF;
+                    long long nq[kHotRes], cb1[kHotRes], cb2[kHotRes];
+#pragma unroll
+                    for (int r = 0; r < kHotRes; ++r) { nq[r] = hs->q[r][a] + placed * p_req[r]; cb1[r] = hs->bound[r][a]; cb2[r] = hs->bound2[r][a]; }
+                    const unsigned short fl = (unsigned short)(hs->flags[a] | ((p_res & 0xF) << 1));
+                    if (node_closed(nq, min_req, RH, cb1, cb2, fl)) {
+                      skey = ~0ull;
+                      hs->nn_last[a] = ((unsigned long long)(unsigned)(c + 1) << 32) | (unsigned)(-(mytick + 1));
+                      closed_l = true;
+                    }
+                  }
+                  hs->key[a] = skey;
+                  rpv[a] = rp2;
+                  m1.ps[L] = (uint16_t)a;
+                }
+                const unsigned tb = __ballot_sync(FULL, closed_l);
+                if (L == 0 && tb) rc.tomb = rc.tomb + __popc(tb);
+                unsigned mine = 0;  // the pods of this lane's domain
+#pragma unroll
+                for (int e = 0; e < kM1Dom; ++e) {
+                  const unsigned b = __ballot_sync(FULL, L < J && d_t == e);
+                  if (L == e) mine = b;
+                }
+                __syncwarp();  // ps, key and room words
+                // the nodes that still accept enter their domain's list at the front of block c + 1, in pod order: the
+                // last one ends up first (the smallest tie-break)
+                for (unsigned m = mine; m; m &= m - 1) {
+                  const int t = __ffs(m) - 1, a = m1.ps[t];
+                  const uint32_t rp2 = rpv[a];
+                  if ((rp2 & 0xFFFF) != 0 && !(rp2 & kRpDead)) insert_front(a, c + 1, order_key(c + 1, -(ltick + t + 1)), rp2);
+                }
+                if (m_rec0) cnt_d += __popc(mine);
+                if (L == 0) m1.upos = upos + J;
+                if (L == kM1Dom) {  // the unpinned list's new head and the node behind it
+                  h = upos + J < (int)m1.ae[kM1Lv - 1][kM1Dom] ? (int)m1_arr[upos + J] : -1;
+                  hk = ~0ull; hr = 0; n1 = -1; nk = ~0ull; nr = 0;
+                  if (h >= 0) {
+                    hk = hs->key[h]; hr = rpv[h]; n1 = nxt_of(h);
+                    if (n1 >= 0) { nk = hs->key[n1]; nr = rpv[n1]; }
+                  }
+                  if (h < 0 || (int)(hk >> 32) != c) {  // the bucket of count c is exhausted
+                    m1.tl[c][L] = kM1None;
+                    level_state();
+                  }
+                }
+                ltick += J;
+                li += J;
+                __syncwarp();
+                continue;
+              }
+            }
             const int a = __shfl_sync(FULL, h, wl);
             const uint32_t rp = __shfl_sync(FULL, hr, wl);
             if ((rp & 0xFFFF) == kRoomSlow) { reason = 1; break; }  // the winner needs the full evaluation
@@ -1998,9 +2121,13 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
               const int mc = __reduce_min_sync(FULL, allowed ? cnt_d : INT32_MAX);
               d = __ffs(__ballot_sync(FULL, allowed && cnt_d == mc)) - 1;
               if (!((rc.m_neutral[0] >> d) & 1) || !((zv[a] & (1u << 17)) || rc.m_wk[0])) { reason = 1; break; }
+#ifdef KSCHED_PROFILE_PACK
+              if (L == 0) s.counters[48] += 1;
+#endif
             }
             const int c = (int)(wkey >> 32);
             if (L == wl) pop_head(c);
+            if (pin && L == 0) m1.upos = m1.upos + 1;  // (read by the next pin step after the __syncwarp below)
             // ---- commit (the per-pod loop's commit, relation by relation on the first lanes)
             uint32_t rp2 = rp - 1 + (1u << 16);
             bool dead_l = false;

@@ -224,6 +224,7 @@ struct ksched_handle {
   DevBuf<uint32_t> d_fd_fc, d_fd_opts;
   DevBuf<uint64_t> d_fd_meta, d_fd_vals;
   DevBuf<long long> d_fd_bound, d_fd_bound2;
+  DevBuf<VarStoreEntry> d_vstore;
   int count_visited = 1;
   DevBuf<uint32_t> d_ex_req_present, d_ex_req_present0, d_ex_avail_present, d_ex_taintset, d_ex_itype, d_nn_req_present, d_nn_opts;
   DevBuf<uint64_t> d_ex_vals, d_ex_vals0, d_ex_meta, d_ex_meta0, d_ex_hp, d_ex_hp0, d_nn_vals, d_nn_meta, d_nn_hp, d_grp_registered,
@@ -827,6 +828,7 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
   }
   CUDA_TRY(h, h->d_remaining.ensure((size_t)V * KSCHED_MAX_RES));
   CUDA_TRY(h, h->d_counters.ensure(kNumCounters));
+  CUDA_TRY(h, h->d_vstore.ensure(kVarStore));
   {
     size_t need = 0, n2 = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, need, (uint64_t*)nullptr, (uint64_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)p1, 0, 64, h->stream);
@@ -1076,6 +1078,8 @@ static int run_pack(ksched_handle* h) {
   s.use_level_run = std::getenv("KSCHED_NO_LEVELRUN") ? 0 : 1;
   s.use_mask_run = std::getenv("KSCHED_NO_MASKRUN") ? 0 : 1;
   s.use_level_warp = std::getenv("KSCHED_NO_LEVELWARP") ? 0 : 1;
+  s.use_varstore = std::getenv("KSCHED_NO_VARSTORE") ? 0 : 1;
+  s.vstore = h->d_vstore.ptr;
   // block size: the chain is latency-bound on ONE thread's commit; more warps only help when there are many candidate
   // nodes to examine per pod (existing nodes, large in-flight sets)
   int threads = h->n_existing >= 2048 ? kPackThreads : (h->n_existing >= 256 ? 256 : 128);
@@ -1174,6 +1178,9 @@ static void print_pack_profile(const long long* counters) {
   fprintf(stderr, "[pack profile] in-flight commit: winner+barrier=%lld record=%lld rest=%lld\n", counters[30], counters[31], counters[11]);
   fprintf(stderr, "[pack profile] class_run: calls=%lld pods=%lld bails=%lld ineligible=%lld cycles=%lld\n", counters[40], counters[41], counters[42], counters[43],
           counters[14]);
+  fprintf(stderr, "[pack profile] class_run round trips (status-1 stop -> entry of the next call that places pods): cycles=%lld | "
+                  "stops for want of a variant=%lld, their round trips' cycles=%lld | variant store: hits=%lld entries=%lld\n",
+          counters[56], counters[57], counters[58], counters[59], counters[60]);
   fprintf(stderr, "[pack profile] mask run steps=%lld with >1 admissible domain=%lld round-able=%lld (counters shared with generic n/fresh: ignore there)\n", counters[18], counters[19], counters[17]);
   fprintf(stderr, "[pack profile] mask run: build cycles=%lld (refused %lld) loop cycles=%lld pods=%lld entries=%lld\n", counters[38], counters[47], counters[6], counters[7], counters[16]);
   fprintf(stderr, "[pack profile] mask run: single steps on the unpinned head=%lld | pin steps=%lld pods=%lld ended by "

@@ -1333,6 +1333,7 @@ constexpr int kRunMask = 2;      // spread relations over a mask key
 constexpr int kRunDom = 16;      // domains of such a key
 constexpr int kTopoCap = 768;    // open nodes whose per-class topology inputs fit in shared memory
 constexpr int kRunVariants = 4;
+constexpr int kVarStore = 256;   // fresh-node variants one Solve shares between classes (VarStoreEntry)
 constexpr int kRunW32 = 64;      // option words a variant holds (T <= 2048)
 constexpr int kRunWarps = kPackThreads / 32;
 constexpr int kRunChunk = 128;   // queue entries staged in shared memory at a time
@@ -1370,8 +1371,100 @@ struct RunCtx {
   int lv_cnt[2];          // level step: members appended to the tie list (double-buffered)
   int lv_fill[2];         // fill step: pods the only eligible node takes
   RunVariant var[kRunVariants];
+  unsigned long long sig; // vs_signature of the class
+  int vs_ok;              // the class may share variants through the store
+  int vs_n;               // entries of PackState::vstore filled in this Solve
+  int vs_got;             // block-wide fetch: ring slot the store filled, or -1
+  uint32_t vs_tag[kVarStore];  // vs_tag of every store entry: a miss is found without a global load
 };
 __shared__ RunCtx g_rc;
+
+// ---- variant store: fresh-node variants shared by the classes of one shape across the Solve ------------------------------
+// NewNode + Add on a fresh node reads nothing of the pod but the class row's requests, requirements, tolerations, host
+// ports and instance-type / hostname requirements, plus the domain every spread relation pins; with no provisioner limit
+// the outcome is a pure function of those (same argument as PackState::fd_*). FFD order puts many deployments of one
+// shape next to each other, so a variant captured for one class is replayed for the next classes of the same signature
+// instead of handing each one's first fresh node per domain back to generic_step. Entries are appended, never evicted;
+// a hit needs the signature hash, the relation pattern and a word-by-word compare of the two class rows to agree.
+struct VarStoreEntry {
+  unsigned long long sig;
+  uint32_t pat;           // vs_pattern
+  uint32_t cls;           // class the variant was captured for (its row is compared on a hit)
+  RunVariant v;           // v.rp: the room only (kRpDead depends on the class's hostname relations)
+};
+// words of ksched_pod_row NewNode + Add read: requests .. res_present (low half of word 28), itype_req, hostname_req
+__device__ __forceinline__ uint64_t vs_word(const ksched_pod_row* row, int w) {
+  const uint64_t x = w < 30 ? reinterpret_cast<const uint64_t*>(row)[w] : 0;
+  return w == 28 ? (x & 0xFFFFFFFFull) : x;
+}
+// hash of the signature fields the pod's registers hold (the requirement words are left to the full compare of a hit)
+__device__ __forceinline__ unsigned long long vs_signature(const PodRegs& p) {
+  unsigned long long x = 0;
+  auto mix = [&](uint64_t v) { x = (x ^ v) * 0x9E3779B97F4A7C15ull; x ^= x >> 29; };
+#pragma unroll
+  for (int r = 0; r < kHotRes; ++r) mix((uint64_t)p.req[r]);
+  mix(p.res); mix(p.tol); mix(p.meta); mix(p.hpc); mix(p.hpe); mix(p.itype | (uint64_t)p.hostname << 32);
+  return x;
+}
+__device__ __forceinline__ uint32_t vs_tag(unsigned long long sig, uint32_t pat) {
+  const unsigned long long x = (sig ^ pat) * 0x9E3779B97F4A7C15ull;
+  return (uint32_t)(x >> 32);
+}
+// warp-wide: some store entry carries the tag of (sig, pat)
+__device__ __forceinline__ bool vs_maybe(const RunCtx& rc, uint32_t tag, int lane) {
+  bool any = false;
+  for (int b = 0; b < rc.vs_n && !any; b += 32) any = __any_sync(0xffffffffu, b + lane < rc.vs_n && rc.vs_tag[b + lane] == tag);
+  return any;
+}
+// relation pattern of a variant: the mask keys of the spread relations and the domain each pinned
+__device__ __forceinline__ uint32_t vs_pattern(int n_mask, const uint8_t* keys, int d0, int d1) {
+  uint32_t p = (uint32_t)n_mask;
+  if (n_mask > 0) p |= (uint32_t)keys[0] << 2 | (uint32_t)d0 << 10;
+  if (n_mask > 1) p |= (uint32_t)keys[1] << 6 | (uint32_t)d1 << 14;
+  return p;
+}
+// warp-wide: the store entry of (class cls, pattern), or -1
+__device__ int vs_find(const RunCtx& rc, unsigned cls, uint32_t pat, int lane) {
+  KS_K2
+  const int n = rc.vs_n;
+  const unsigned long long sig = rc.sig;
+  const uint32_t tag = vs_tag(sig, pat);
+  for (int b = 0; b < n; b += 32) {
+    unsigned m = __ballot_sync(0xffffffffu, b + lane < n && rc.vs_tag[b + lane] == tag);
+    while (m) {
+      const int f = b + __ffs(m) - 1;
+      m &= m - 1;
+      if (s.vstore[f].sig != sig || s.vstore[f].pat != pat) continue;
+      const unsigned other = s.vstore[f].cls;
+      if (__all_sync(0xffffffffu, vs_word(s.classes + cls, lane) == vs_word(s.classes + other, lane))) return f;
+    }
+  }
+  return -1;
+}
+// warp-wide: replays the store's variant for (cls, pat) into ring slot rc.var_next, with the class's own kRpDead (a
+// fresh node holds one pod: its hostname counts are h_times); returns the slot, or -1 on a miss
+__device__ int vs_fetch(RunCtx& rc, unsigned cls, uint32_t pat, int lane) {
+  KS_K2
+  const int e = vs_find(rc, cls, pat, lane);
+  if (e < 0) return -1;
+  const int slot = rc.var_next;
+  const uint32_t* src = reinterpret_cast<const uint32_t*>(&s.vstore[e].v);
+  uint32_t* dst = reinterpret_cast<uint32_t*>(&rc.var[slot]);
+  for (int w = lane; w < (int)(sizeof(RunVariant) / 4); w += 32) dst[w] = src[w];
+  __syncwarp();
+  if (lane == 0) {
+    bool dead = false;
+    for (int j = 0; j < rc.n_host; ++j) dead = dead || rc.h_times[j] > rc.h_lim[j];
+    rc.var[slot].rp = s.vstore[e].v.rp | (dead ? kRpDead : 0u);
+    rc.var_next = (slot + 1) % kRunVariants;
+    if (rc.n_var < kRunVariants) rc.n_var++;
+#ifdef KSCHED_PROFILE_PACK
+    s.counters[59] += 1;
+#endif
+  }
+  __syncwarp();
+  return slot;
+}
 
 // ---- mask run: the class-run loop for ONE spread relation over a mask key (zone spread), driven by warp 0 alone ----------
 // The accepting nodes are kept in singly linked lists in the reference's order (pod count, then tie-break), one per
@@ -1521,6 +1614,12 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
       }
       rc.eligible = ok;
     }
+    if (tid == 0) {
+      // instance-type / hostname requirements and volumes: not shared (a volume limit reads more than the row)
+      rc.vs_ok = s.use_varstore && !s.any_limits && W32 <= kRunW32 && first_in.itype == KSCHED_NONE &&
+                 first_in.hostname == KSCHED_NONE && !class_has_volumes(s, cls);
+      rc.sig = vs_signature(first_in);
+    }
     __syncthreads();
   }
   if (!rc.eligible || (topo && n_active > kTopoCap)) {
@@ -1614,6 +1713,27 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
         if (rc.n_var < kRunVariants) rc.n_var++;
       }
       __syncthreads();
+      // into the store (not looked up first: a class captures a variant only after a miss, so duplicates are rare and
+      // harmless, and the capture stays free of dependent loads)
+      if (warp == 0 && rc.vs_ok && rc.vs_n < kVarStore) {
+        const uint32_t pat = vs_pattern(n_mask, rc.m_key, dom[0], dom[1]);
+        const int e = rc.vs_n;
+        VarStoreEntry& d = s.vstore[e];
+        const uint32_t* src = reinterpret_cast<const uint32_t*>(&rc.var[slot]);
+        uint32_t* dst = reinterpret_cast<uint32_t*>(&d.v);
+        for (int w = lane; w < (int)(sizeof(RunVariant) / 4); w += 32) dst[w] = src[w];
+        __syncwarp();
+        if (lane == 0) {
+          d.sig = rc.sig; d.pat = pat; d.cls = cls;
+          d.v.rp = rc.var[slot].rp & 0xFFFF;
+          rc.vs_tag[e] = vs_tag(rc.sig, pat);
+          rc.vs_n = e + 1;
+#ifdef KSCHED_PROFILE_PACK
+          s.counters[60] += 1;
+#endif
+        }
+        __syncwarp();
+      }
     }
   }
 
@@ -1640,6 +1760,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
 #ifdef KSCHED_PROFILE_PACK
   const long long cr_t0 = clock64();
   int cr_it[4] = {0, 0, 0, 0};  // iterations: level, fill, fresh, per-pod argmin
+  int cr_novar = 0;             // the run stopped because no variant was known for the fresh node's domain
 #define CR_IT(k) { ++cr_it[k]; }
 #else
 #define CR_IT(k)
@@ -1865,6 +1986,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
         // smallest head key first - a whole round is committed at once, every lane its own domain
         const bool rounds = m_rec0 && m_bias0 == 0;
         int li = i, ltick = tick, lnew = n_new, lact = n_active, nfr = 0;
+        unsigned fr_used = 0;  // ring slots the nodes created in this entry replay: a store fetch must not overwrite them
         int i_end = rc.q_end[buf];
         if (i + qlen < i_end) i_end = i + qlen;
         int reason = 0;  // 0: the staged entries of the class are consumed; 1: the pod at li needs generic_step; 2: per-pod loop from li on
@@ -1915,6 +2037,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
                 for (int j = 0; j < n_host; ++j) fresh_ok = fresh_ok && rc.h_lim[j] >= 0;
               }
               if (fresh_ok && !__any_sync(FULL, bad_l) && (hv == 0 || ukey > mx)) {
+                fr_used |= __reduce_or_sync(FULL, (act && !hd) ? 1u << vi_l : 0u);
                 int rank = 0;  // position of this lane's node in the round
                 for (unsigned m = hv; m; m &= m - 1) {
                   const unsigned long long k2 = __shfl_sync(FULL, hk, __ffs(m) - 1);
@@ -2177,7 +2300,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
             if (reason == 2) break;
           } else {
             // ---- nobody accepts: NewNode + Add replayed from the variant of the domain a fresh node gets
-            if (lnew >= MAXN || lact >= kActCap || lact >= kTopoCap || rc.n_var == 0) { reason = 1; break; }
+            if (lnew >= MAXN || lact >= kActCap || lact >= kTopoCap) { reason = 1; break; }
             bool ok = true;
             for (int j = 0; j < n_host; ++j) ok = ok && rc.h_lim[j] >= 0;
             const unsigned cand = rc.m_tallow[0] & okm;
@@ -2187,8 +2310,17 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
             const int fd = __ffs(__ballot_sync(FULL, in_c && cnt_d == mc)) - 1;
             int vi = -1;
             for (int v2 = 0; v2 < rc.n_var && vi < 0; ++v2) if (rc.var[v2].dom[0] == fd) vi = v2;
-            if (vi < 0) { reason = 1; break; }
+            if (vi < 0 && rc.vs_ok && !((fr_used >> rc.var_next) & 1))
+              vi = vs_fetch(rc, cls, vs_pattern(1, rc.m_key, fd, 0), L);
+            if (vi < 0) {
+              reason = 1;
+#ifdef KSCHED_PROFILE_PACK
+              cr_novar = 1;
+#endif
+              break;
+            }
             const RunVariant& v = rc.var[vi];
+            fr_used |= 1u << vi;
             const int n = lnew, a = lact;
             if (L < n_host) {
               const int times = rc.h_times[L];
@@ -2607,7 +2739,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
     }
     if (mode == 2) {
       // ---- nobody accepts: NewNode + Add replayed from a variant (templates: the one the variant was created from)
-      if (n_new >= MAXN || n_active >= kActCap || (topo && n_active >= kTopoCap) || rc.n_var == 0) { status = 1; break; }
+      if (n_new >= MAXN || n_active >= kActCap || (topo && n_active >= kTopoCap)) { status = 1; break; }
       bool ok = true;
 #pragma unroll
       for (int j = 0; j < kRunHost; ++j) ok = ok && (j >= n_host || rc.h_lim[j] >= 0);  // a fresh hostname has count 0
@@ -2622,7 +2754,23 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
       int vi = -1;
       for (int v2 = 0; v2 < rc.n_var && ok && vi < 0; ++v2)
         if ((n_mask < 1 || rc.var[v2].dom[0] == fd0) && (n_mask < 2 || rc.var[v2].dom[1] == fd1)) vi = v2;
-      if (vi < 0) { status = 1; break; }
+      const uint32_t pat = vs_pattern(n_mask, rc.m_key, fd0, fd1);
+      if (vi < 0 && ok && rc.vs_ok && vs_maybe(rc, vs_tag(rc.sig, pat), lane)) {  // (every warp finds the same answer)
+        __syncthreads();  // every warp has scanned the ring
+        if (warp == 0) {
+          const int got = vs_fetch(rc, cls, pat, lane);
+          if (lane == 0) rc.vs_got = got;
+        }
+        __syncthreads();
+        vi = rc.vs_got;
+      }
+      if (vi < 0) {
+        status = 1;
+#ifdef KSCHED_PROFILE_PACK
+        cr_novar = ok;
+#endif
+        break;
+      }
       const RunVariant& v = rc.var[vi];
       CR_IT(2)
       // Fill step on the fresh node: it takes `cap` further pods of the class while it is the only accepting node and then
@@ -2781,6 +2929,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
     s.counters[b] += clock64() - cr_t0; s.counters[b + 1] += placed_total; s.counters[b + 2] += cr_it[0] + cr_it[1]; s.counters[b + 3] += cr_it[2];
     s.counters[lvl ? 44 : 45] += cr_it[3];
     s.counters[46] += cr_it[1];
+    if (status == 1 && cr_novar) s.counters[57] += 1;
   }
 #endif
   if (tid == 0) {
@@ -2802,6 +2951,8 @@ __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
 #ifdef KSCHED_PROFILE_PACK
   long long pk_acc[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
   long long pk_last = clock64();
+  long long pk_bail = -1;  // when the last class_run call stopped with status 1 (-1: none since the last one that placed pods)
+  bool pk_bail_novar = false;
 #endif
   KS_K2
   const int tid = threadIdx.x;
@@ -2817,7 +2968,7 @@ __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
   uint32_t* tmpl_taintset = g_tmpl_taintset;
   __shared__ WarpIO wio;
   if (tid < c.n_templates) tmpl_taintset[tid] = c.templates[tid].taintset;
-  if (tid == 0) { pt.n = 0; g_rc.cls = KSCHED_NONE; g_rc.eligible = 0; }
+  if (tid == 0) { pt.n = 0; g_rc.cls = KSCHED_NONE; g_rc.eligible = 0; g_rc.vs_n = 0; }
 
   int head = 0, qlen = s.n_pods;
   const int qcap = s.n_pods + 1;
@@ -2920,6 +3071,10 @@ __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
         io.fresh_valid = fresh_valid; io.fresh_a = fresh_a; io.fresh_cls = fresh_cls;
       }
       __syncthreads();
+#ifdef KSCHED_PROFILE_PACK
+      const long long pk_entry = clock64();
+      const long long pk_novar0 = tid == 0 ? s.counters[57] : 0;
+#endif
       class_run(nxt);
       const RunIO& io = g_rio;
       const int placed = io.placed, status = io.status;
@@ -2927,7 +3082,16 @@ __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
       add_calls = io.add_calls;
       fresh_valid = 0;
 #ifdef KSCHED_PROFILE_PACK
-      if (tid == 0) { s.counters[40] += 1; s.counters[41] += placed; s.counters[42] += status == 1; s.counters[43] += status == 2; }
+      if (tid == 0) {
+        s.counters[40] += 1; s.counters[41] += placed; s.counters[42] += status == 1; s.counters[43] += status == 2;
+        // round trips: from a call that stopped with status 1 to the entry of the next call that places pods
+        if (placed > 0 && pk_bail >= 0) {
+          s.counters[56] += pk_entry - pk_bail;
+          if (pk_bail_novar) s.counters[58] += pk_entry - pk_bail;
+          pk_bail = -1;
+        }
+        if (status == 1 && pk_bail < 0) { pk_bail = clock64(); pk_bail_novar = s.counters[57] != pk_novar0; }
+      }
 #endif
       if (status == 2) run_block_cls = (unsigned)nxt.cls64;
       if (placed == 0 && status == 1) { run_fail = run_fail < 6 ? run_fail + 1 : 6; run_skip = (1 << run_fail) - 1; }

@@ -111,6 +111,8 @@ struct PackState {
   int use_level_run;                 // class_run: level / fill steps for classes without mask-key spread (KSCHED_NO_LEVELRUN=1: off)
   int use_level_warp;                // class_run: the level / fill steps on one warp while at most 32 nodes are open (KSCHED_NO_LEVELWARP=1: off)
   int use_mask_run;                  // class_run: list-driven warp loop for one mask-key spread relation (KSCHED_NO_MASKRUN=1: off)
+  int use_varstore;                  // class_run: fresh-node variants shared by classes of one shape (KSCHED_NO_VARSTORE=1: off)
+  struct VarStoreEntry* vstore;      // [kVarStore] (pack_kernel.cuh); valid entries: RunCtx::vs_n, reset per Solve
   // topology counters
   int32_t* grp_cnt;                  // [n_groups][64]
   uint64_t* grp_registered;          // [n_groups]

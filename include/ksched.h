@@ -81,6 +81,10 @@ typedef struct ksched_bounds {
  * A key also gets region bits (m = 0: one region) when some instance type carries a complement requirement on it
  * (NotIn / Exists / Gt / Lt): the region bits are what a complement node requirement and a complement type have in common.
  * Keys with neither have region_mask 0 and nothing changes for them.
+ * A caller that builds its own dictionary may collapse a wide key the same way the host encoder does (DESIGN.md §3, value
+ * classes): values that no requirement, label, threshold or topology domain of the problem names, and that appear only in
+ * instance types' In requirements or existing nodes' labels, can be replaced by one representative per class (unnamed
+ * integers of one region Ri, unnamed non-integers), kept as an ordinary dictionary value. The answers do not change.
  */
 #define KSCHED_MAX_THRESHOLDS 7
 typedef struct ksched_key_regions {

@@ -86,6 +86,10 @@ int kh_consolidate(const kh_problem* p, int* out4, int* options, int options_cap
  * node the command removes. */
 int kh_consolidate_single(const kh_problem* p, int first, int last, int batch, int* out4, int* node, int* options, int options_cap);
 
+/* ---- self-test of the encoder's value classes (CPU, no device): random wide keys and requirement pairs, the exact string
+ * algebra against the collapsed masks (host form and region form). Returns the number of mismatches. */
+int kh_value_class_selftest(unsigned seed, int iters);
+
 #ifdef __cplusplus
 }
 #endif

@@ -122,6 +122,8 @@ def lib():
     L.kh_encode.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.c_int]
     L.kh_encoded_free.argtypes = [C.c_void_p]
     L.kh_encoded_dims.argtypes = [C.c_void_p, C.POINTER(C.c_longlong)]
+    L.kh_encoded_key_info.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(C.c_longlong)]
+    L.kh_value_class_selftest.argtypes = [C.c_uint, C.c_int]
     L.kh_gpu_load.argtypes = [C.c_void_p]
     L.kh_encoded_set_count_visited.argtypes = [C.c_void_p, C.c_int]
     L.kh_gpu_run.argtypes = [C.c_int]
@@ -505,6 +507,14 @@ class ResidentSolve:
         d = (C.c_longlong * 10)()
         lib().kh_encoded_dims(self.enc, d)
         self.dims = dict(zip(["pods", "classes", "existing", "groups", "types", "templates", "keys", "resources", "type_words", "class_topo"], list(d)))
+
+    def key_info(self, key):
+        """dictionary of one mask key: {values, representatives (of unnamed value classes, 0 = none), thresholds}, or None
+        when the key is not a mask key of this encoding"""
+        out = (C.c_longlong * 3)()
+        if lib().kh_encoded_key_info(self.enc, key.encode(), out) != 0:
+            return None
+        return dict(zip(["values", "representatives", "thresholds"], list(out)))
 
     def set_count_visited(self, on):
         """exact nodes_visited statistic on/off (off for timed runs: it costs a pass over all in-flight nodes per pod)"""

@@ -350,8 +350,10 @@ struct NodeFacts {
 struct ClusterFacts : kmodel::ProblemDerived {
   std::vector<NodeFacts> node;           // parallel to Problem.nodes
   std::set<std::string> res_names;       // resource names mentioned by node allocatable / capacity / bound pods
+  std::set<std::string> req_names;       // resource names some bound pod requests
   std::set<std::string> anti_keys;       // topology keys of the bound pods' required anti-affinity terms
   std::set<std::pair<std::string, std::string>> label_pairs;  // every (key, value) some node carries as a label
+  std::set<std::pair<std::string, std::string>> named_pairs;  // (normalized key, value) a bound pod's node selector / affinity names
 };
 const ClusterFacts& cluster_facts(const Problem& P) {
   std::lock_guard<std::mutex> lock(P.derived_mu);
@@ -365,7 +367,15 @@ const ClusterFacts& cluster_facts(const Problem& P) {
       for (auto& kv : n.capacity) f->res_names.insert(kv.first);
       for (auto& p : n.pods) {
         const ResourceList r = pod_requests(p);
-        for (auto& kv : r) f->res_names.insert(kv.first);
+        for (auto& kv : r) { f->res_names.insert(kv.first); f->req_names.insert(kv.first); }
+        auto name = [&](const std::vector<NodeSelectorRequirement>& rs) {
+          for (auto& q : rs)
+            if (q.op == Op::In || q.op == Op::NotIn)
+              for (auto& v : q.values) f->named_pairs.insert({normalize_key(q.key), v});
+        };
+        for (auto& kv : p.node_selector) f->named_pairs.insert({normalize_key(kv.first), kv.second});
+        for (auto& t : p.required_node_terms) name(t);
+        for (auto& t : p.preferred_node_terms) name(t.preference);
         nf.pod_req = merge(nf.pod_req, r);
         if (p.is_daemonset) nf.ds_req = merge(nf.ds_req, r);
         for (auto& hp : host_ports(p)) nf.hostports.push_back(hp);
@@ -393,6 +403,7 @@ struct Builder {
   std::vector<std::vector<Taint>> taintsets;
   std::vector<HostPortEntry> hp_entries;
   std::map<std::string, int> type_col;                     // instance type name -> column
+  bool res_pruned = false;                                 // resource names no request reads were left out of res_id
 
   Builder(const Problem& p, Encoded& e) : P(p), E(e) {}
 
@@ -493,6 +504,7 @@ struct Builder {
     uint32_t present = 0;
     for (int i = 0; i < KSCHED_MAX_RES; ++i) out[i] = 0;
     for (auto& kv : r) {
+      if (res_pruned && !res_id.count(kv.first)) continue;  // no request or limit reads it: it cannot change an answer
       int id = resource(kv.first);
       out[id] = kv.second;
       present |= 1u << id;
@@ -541,6 +553,20 @@ struct Group {
 };
 
 }  // namespace
+
+std::map<std::string, std::string> value_classes(const std::set<std::string>& values, const std::set<std::string>& named,
+                                                 const std::set<int64_t>& thresholds) {
+  std::map<std::string, std::string> rep_of;
+  std::map<int, std::string> rep;  // class -> representative; class = region index of an integer (ksched.h), -1 non-integers
+  for (auto& v : values) {         // ascending string order: a class's first member is its smallest
+    int64_t iv;
+    const bool is_int = parse_int(v, &iv);
+    if (named.count(v) || (is_int && thresholds.count(iv))) continue;
+    const int cls = is_int ? (int)std::distance(thresholds.begin(), thresholds.lower_bound(iv)) : -1;
+    rep_of[v] = rep.emplace(cls, v).first->second;
+  }
+  return rep_of;
+}
 
 std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candidates, bool cluster_superset) {
   static const bool prof = std::getenv("KSCHED_ENCODE_PROFILE") != nullptr;
@@ -798,6 +824,87 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
     note_label_vals(l);
   }
   for (auto& kv : facts.label_pairs) { int k = B.key_of(kv.first); if (k >= 0) vals[k].insert(kv.second); }  // every node's labels (ClusterFacts)
+  const int zone_key = B.key_of(kZone), ct_key = B.key_of(kCapacityType);
+  // Every threshold any requirement of this problem names, per key; a key also gets one region when an instance type has a
+  // complement requirement on it (region form below).
+  std::vector<std::set<int64_t>> thr(NK);
+  std::vector<bool> type_complement(NK, false);
+  {
+    auto note_thr = [&](const std::vector<NodeSelectorRequirement>& rs, bool is_type) {
+      for (auto& r : rs) {
+        int k = B.key_of(r.key);
+        if (k < 0) continue;
+        if (r.op == Op::Gt || r.op == Op::Lt) { int64_t v = 0; if (!r.values.empty()) parse_int(r.values[0], &v); thr[k].insert(v); }
+        if (is_type && r.op != Op::In && r.op != Op::DoesNotExist) type_complement[k] = true;
+      }
+    };
+    auto note_pod_thr = [&](const Pod& p) {
+      for (auto& t : p.required_node_terms) note_thr(t, false);
+      for (auto& t : p.preferred_node_terms) note_thr(t.preference, false);
+    };
+    for (auto& sp : specs) note_pod_thr(sp.pod);
+    for (auto& d : daemons) note_pod_thr(d);
+    for (auto& it : P.instance_types) note_thr(it.requirements, true);
+    for (auto& pr : P.provisioners) note_thr(pr.requirements, false);
+  }
+  // Value classes (DESIGN.md §3). A key whose values do not fit the word keeps the values some requirement of the problem
+  // names, and one representative per class of the others: instance types' In values and node labels that no requirement
+  // tells apart. Keys that fit are encoded as they always were.
+  phase("  keys + thresholds");
+  E.key_representatives.assign(NK, 0);
+  std::vector<std::map<std::string, std::string>> rep_of(NK);  // unnamed value -> its class's representative
+  {
+    std::vector<int> wide;
+    for (int k = 0; k < NK; ++k) {
+      const size_t nd = vals[k].size(), m = thr[k].size();
+      if (nd > 63 || ((m > 0 || type_complement[k]) && nd + m + 1 > 63)) wide.push_back(k);
+    }
+    if (!wide.empty()) {
+      std::vector<std::set<std::string>> named(NK);
+      std::vector<bool> all_named(NK, false);
+      auto name_vals = [&](const std::vector<NodeSelectorRequirement>& rs, bool complement_only) {
+        for (auto& r : rs) {
+          int k = B.key_of(r.key);
+          if (k < 0 || (complement_only && r.op == Op::In)) continue;
+          if (r.op == Op::In || r.op == Op::NotIn) named[k].insert(r.values.begin(), r.values.end());
+        }
+      };
+      auto name_labels = [&](const Labels& l) { for (auto& kv : l) { int k = B.key_of(kv.first); if (k >= 0) named[k].insert(kv.second); } };
+      auto name_pod = [&](const Pod& p) {  // topology node filters are built from the same node selector and required terms
+        name_labels(p.node_selector);
+        for (auto& t : p.required_node_terms) name_vals(t, false);
+        for (auto& t : p.preferred_node_terms) name_vals(t.preference, false);
+        auto topo = [&](const std::string& key) { int k = B.key_of(key); if (k >= 0) all_named[k] = true; };
+        for (auto& t : p.topology_spread) topo(t.topology_key);
+        for (auto& t : p.pod_affinity_required) topo(t.topology_key);
+        for (auto& t : p.pod_affinity_preferred) topo(t.term.topology_key);
+        for (auto& t : p.pod_anti_affinity_required) topo(t.topology_key);
+        for (auto& t : p.pod_anti_affinity_preferred) topo(t.term.topology_key);
+      };
+      for (auto& s : specs) name_pod(s.pod);
+      for (auto& d : daemons) name_pod(d);
+      for (auto& kv : facts.named_pairs) { int k = B.key_of(kv.first); if (k >= 0) named[k].insert(kv.second); }  // bound pods
+      for (auto& key : facts.anti_keys) { int k = B.key_of(key); if (k >= 0) all_named[k] = true; }  // inverse anti-affinity groups
+      for (auto& pr : P.provisioners) {
+        name_vals(pr.requirements, false);
+        Labels l = pr.labels;
+        l[kProvisionerName] = pr.name;
+        name_labels(l);
+      }
+      for (auto& it : P.instance_types) name_vals(it.requirements, true);
+      if (zone_key >= 0) all_named[zone_key] = true;  // offering slots: they feed the launch choice
+      if (ct_key >= 0) all_named[ct_key] = true;
+      for (int k : wide) {
+        if (all_named[k]) continue;  // refused below when it does not fit
+        rep_of[k] = value_classes(vals[k], named[k], thr[k]);
+        for (auto& kv : rep_of[k]) {
+          if (kv.first != kv.second) vals[k].erase(kv.first);
+          else E.key_representatives[k]++;
+        }
+      }
+    }
+  }
+  phase("  value classes");
   B.value_id.resize(NK);
   E.key_values.resize(NK);
   E.keys.resize(NK);
@@ -816,33 +923,15 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
       if (parse_int(v, &iv)) { ki.int_mask |= 1ull << b; E.key_int_values[(size_t)k * 64 + b] = iv; }
       ++b;
     }
+    // every requirement, label and domain table looks an unnamed value up under its representative's id
+    for (auto& kv : rep_of[k]) B.value_id[k][kv.first] = B.value_id[k].at(kv.second);
     ki.well_known = B.well_known.count(E.key_names[k]) ? 1 : 0;
     ki.is_zone = E.key_names[k] == kZone;
     ki.is_capacity_type = E.key_names[k] == kCapacityType;
   }
   for (int k = 0; k < NK; ++k) B.key_meta[k] = KeyMeta{E.keys[k].int_mask, &E.key_int_values[(size_t)k * 64], nullptr};
-  const int zone_key = B.key_of(kZone), ct_key = B.key_of(kCapacityType);
-  // Region form of Gt/Lt (ksched.h: ksched_key_regions). Every threshold any requirement of this problem names, per key; a
-  // key also gets one region when an instance type has a complement requirement on it.
+  // Region form of Gt/Lt (ksched.h: ksched_key_regions).
   {
-    std::vector<std::set<int64_t>> thr(NK);
-    std::vector<bool> type_complement(NK, false);
-    auto note_thr = [&](const std::vector<NodeSelectorRequirement>& rs, bool is_type) {
-      for (auto& r : rs) {
-        int k = B.key_of(r.key);
-        if (k < 0) continue;
-        if (r.op == Op::Gt || r.op == Op::Lt) { int64_t v = 0; if (!r.values.empty()) parse_int(r.values[0], &v); thr[k].insert(v); }
-        if (is_type && r.op != Op::In && r.op != Op::DoesNotExist) type_complement[k] = true;
-      }
-    };
-    auto note_pod_thr = [&](const Pod& p) {
-      for (auto& t : p.required_node_terms) note_thr(t, false);
-      for (auto& t : p.preferred_node_terms) note_thr(t.preference, false);
-    };
-    for (auto& sp : specs) note_pod_thr(sp.pod);
-    for (auto& d : daemons) note_pod_thr(d);
-    for (auto& it : P.instance_types) note_thr(it.requirements, true);
-    for (auto& pr : P.provisioners) note_thr(pr.requirements, false);
     bool any = false;
     for (int k = 0; k < NK; ++k) any = any || !thr[k].empty() || type_complement[k];
     if (any) {
@@ -870,6 +959,18 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
     for (auto& n : facts.res_names) names.insert(n);  // node allocatable / capacity / bound pods (ClusterFacts)
     E.res_names = {"cpu", "memory", "pods"};
     for (auto& n : names) if (n != "cpu" && n != "memory" && n != "pods") E.res_names.push_back(n);
+    if (E.res_names.size() > KSCHED_MAX_RES) {
+      // Fits reads the request's keys only (resources.go:138-145), the limits bookkeeping the limit's keys only
+      // (scheduler.go:284-303): a name that no pod requests and no limit names cannot change an answer. Left out.
+      std::set<std::string> read = facts.req_names;
+      auto note_read = [&](const ResourceList& r) { for (auto& kv : r) read.insert(kv.first); };
+      for (auto& s : specs) note_read(s.req);
+      for (auto& d : daemons) note_read(pod_requests(d));
+      for (auto& pr : P.provisioners) note_read(pr.limits);
+      E.res_names = {"cpu", "memory", "pods"};
+      for (auto& n : read) if (n != "cpu" && n != "memory" && n != "pods") E.res_names.push_back(n);
+      B.res_pruned = true;
+    }
     if (E.res_names.size() > KSCHED_MAX_RES) unsupported("more than 8 distinct resources");
     for (size_t i = 0; i < E.res_names.size(); ++i) B.res_id[E.res_names[i]] = (int)i;
   }
@@ -1113,7 +1214,8 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
   std::vector<Group> groups;
   std::map<std::string, size_t> group_of;          // hash -> index, non-inverse
   std::map<std::string, size_t> inverse_group_of;  // hash -> index, inverse
-  // domain universe: provisioner.go:266-276 (requirement.Values() of every type + provisioner In requirements)
+  // domain universe: provisioner.go:266-276 (requirement.Values() of every type + provisioner In requirements). Only topology
+  // keys read it, and their values are never collapsed into classes, so the strings here are the dictionary's own.
   std::map<std::string, std::set<std::string>> universe;
   for (int v = 0; v < NV; ++v) {
     const Provisioner& pr = P.provisioners[E.template_provisioner[v]];

@@ -6,6 +6,7 @@
 #include <cstdlib>
 #include <map>
 #include <memory>
+#include <set>
 #include <string>
 #include <thread>
 #include <vector>
@@ -36,6 +37,8 @@ struct Encoded {
   // ---- dictionary
   std::vector<std::string> key_names;                 // mask keys
   std::vector<std::vector<std::string>> key_values;   // per key, ascending string order (canonical domain order)
+  std::vector<int32_t> key_representatives;           // per key: dictionary values that stand for a class of unnamed values
+                                                      // (value_classes below), 0 = every value of the key is its own
   std::vector<std::string> res_names;                 // resource ids: cpu, memory, pods, then ascending
   // ---- which objects take part (provisioner.go:119-144 / deprovisioning/helpers.go:42-93)
   std::vector<const kmodel::Pod*> pods;               // Solve's pod list
@@ -92,6 +95,13 @@ struct Encoded {
 // cluster_superset: the encoding ksched_load_cluster wants (ksched.h: ksched_cluster) - the candidates' pods form the batch as
 // usual but the candidate nodes STAY existing nodes, with all their pods bound; Encoded::pod_node says where each pod lives.
 std::unique_ptr<Encoded> encode(const kmodel::Problem& P, const std::vector<int>& candidates, bool cluster_superset = false);
+
+// Value classes of one label key (DESIGN.md §3). A value is named when some requirement, label or threshold of the problem
+// names it (`named`, plus every value equal to one of `thresholds`); no requirement tells apart two unnamed integers of the
+// same region between consecutive thresholds (ksched.h: ksched_key_regions), nor two unnamed non-integers. Returns, for every
+// unnamed value, its class's representative: the smallest member in string order (which maps to itself).
+std::map<std::string, std::string> value_classes(const std::set<std::string>& values, const std::set<std::string>& named,
+                                                 const std::set<int64_t>& thresholds);
 
 // metav1.LabelSelectorAsSelector(sel).Matches(labels); a nil selector matches nothing
 bool label_selector_matches(const kmodel::LabelSelector& sel, const kmodel::Labels& labels);

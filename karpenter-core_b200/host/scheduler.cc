@@ -1078,4 +1078,201 @@ int kh_region_selftest(unsigned seed, int iters) {
   }
   return bad;
 }
+
+// Value classes (khost::value_classes, DESIGN.md §3) against the exact string algebra (requirement.go:117-204). Each
+// iteration draws a wide key: 64-143 integer and non-integer values, some of them named, 0-7 thresholds. Over it, requirements
+// of the two kinds a problem carries: the named side (In / NotIn over named values, Exists, DoesNotExist, Gt / Lt: pods,
+// provisioners, complement instance types) and the type / node side (In over any values: instance types' In requirements,
+// node labels). Every pair is evaluated on the strings and on the collapsed masks, in the host algebra and in region form:
+// Len() == 0 of the intersection, Operator(), the excluded set, Intersects and Compatible must agree; Has must agree on every
+// named value, and on every value when both requirements are from the named side (no requirement tells a class's members
+// apart, which is the point). Also: at most m + 2 representatives. Returns the number of mismatches.
+int kh_value_class_selftest(unsigned seed, int iters) {
+  uint64_t st = seed * 0x9E3779B97F4A7C15ull + 777;
+  auto rnd = [&](int n) { st = st * 6364136223846793005ull + 1442695040888963407ull; return (int)((st >> 33) % (uint64_t)n); };
+  struct SReq {
+    bool present = true, complement = true, has_gt = false, has_lt = false;
+    int64_t gt = 0, lt = 0;
+    std::set<std::string> values;
+  };
+  int bad = 0;
+  for (int it = 0; it < iters; ++it) {
+    std::set<std::string> all;
+    std::map<std::string, int64_t> ival;  // strconv.Atoi of the integer values
+    const int n_values = 64 + rnd(80);
+    while ((int)all.size() < n_values) {
+      if (rnd(10) < 6) {
+        const int64_t x = rnd(120) - 10;
+        const std::string s = (rnd(8) == 0 && x >= 0 ? "0" : "") + std::to_string(x);
+        all.insert(s);
+        ival[s] = x;
+      } else {
+        all.insert(std::string(rnd(2) ? "fam-" : "g") + std::to_string(rnd(1000)));
+      }
+    }
+    const std::vector<std::string> pool(all.begin(), all.end());
+    std::set<int64_t> tset;
+    const int m = rnd(8);
+    while ((int)tset.size() < m) tset.insert(rnd(120) - 10);
+    const std::vector<int64_t> ts(tset.begin(), tset.end());
+    std::set<std::string> named;
+    for (int i = rnd(24); i > 0; --i) named.insert(pool[(size_t)rnd((int)pool.size())]);
+    const std::map<std::string, std::string> rep_of = khost::value_classes(all, named, tset);
+    // the collapsed dictionary, as the encoder builds it
+    std::map<std::string, int> id;
+    std::vector<std::string> dict_values;
+    int64_t ints[64] = {};
+    uint64_t int_mask = 0;
+    int n_reps = 0;
+    for (auto& v : all) {
+      auto r = rep_of.find(v);
+      if (r != rep_of.end() && r->second != v) continue;
+      n_reps += r != rep_of.end();
+      const int b = (int)dict_values.size();
+      id[v] = b;
+      dict_values.push_back(v);
+      auto iv = ival.find(v);
+      if (iv != ival.end()) { int_mask |= 1ull << b; ints[b] = iv->second; }
+    }
+    for (auto& kv : rep_of) id[kv.first] = id.at(kv.second);
+    const int nd = (int)dict_values.size();
+    if (n_reps > m + 2 || nd + m + 1 > 63) { ++bad; continue; }
+    const uint64_t dict = (1ull << nd) - 1;
+    const ksched::KeyMeta hk{int_mask, ints, nullptr};
+    ksched_key_regions g{};
+    const bool regions = m > 0 || rnd(2);
+    if (regions) ksched::regions_build(&g, ts.data(), m, nd, dict, hk);
+    const ksched::KeyMeta rk{int_mask, ints, regions ? &g : nullptr};
+
+    // ---- the string algebra
+    auto s_within = [&](const SReq& r, const std::string& v) {
+      if (!r.has_gt && !r.has_lt) return true;
+      auto iv = ival.find(v);
+      return iv != ival.end() && (!r.has_gt || iv->second > r.gt) && (!r.has_lt || iv->second < r.lt);
+    };
+    auto s_intersect = [&](const SReq& a, const SReq& b) {
+      SReq r;
+      r.complement = a.complement && b.complement;
+      r.has_gt = a.has_gt || b.has_gt;
+      r.has_lt = a.has_lt || b.has_lt;
+      r.gt = a.has_gt ? (b.has_gt ? std::max(a.gt, b.gt) : a.gt) : b.gt;
+      r.lt = a.has_lt ? (b.has_lt ? std::min(a.lt, b.lt) : a.lt) : b.lt;
+      if (r.has_gt && r.has_lt && r.gt >= r.lt) { SReq dne; dne.complement = false; return dne; }
+      std::set<std::string> v;
+      if (a.complement && b.complement) { v = a.values; v.insert(b.values.begin(), b.values.end()); }
+      else if (a.complement) { for (auto& x : b.values) if (!a.values.count(x)) v.insert(x); }
+      else if (b.complement) { for (auto& x : a.values) if (!b.values.count(x)) v.insert(x); }
+      else { for (auto& x : a.values) if (b.values.count(x)) v.insert(x); }
+      for (auto& x : v) if (s_within(r, x)) r.values.insert(x);
+      if (!r.complement) { r.has_gt = r.has_lt = false; r.gt = r.lt = 0; }
+      return r;
+    };
+    auto s_has = [&](const SReq& r, const std::string& v) { return s_within(r, v) && (r.complement ? !r.values.count(v) : r.values.count(v) > 0); };
+    auto s_len_zero = [](const SReq& r) { return !r.complement && r.values.empty(); };
+    auto s_negative = [](const SReq& r) { return r.complement ? !r.values.empty() : r.values.empty(); };
+    auto s_intersects = [&](const SReq& e, const SReq& i) {
+      if (!e.present || !i.present) return true;
+      if (!s_len_zero(s_intersect(e, i))) return true;
+      return s_negative(i) && s_negative(e);
+    };
+    auto s_compatible = [&](const SReq& n, const SReq& i, bool wk) {
+      if (!i.present) return true;
+      if (!wk && !n.present && !s_negative(i)) return false;
+      return s_intersects(n, i);
+    };
+    auto bits = [&](const std::set<std::string>& vs) { uint64_t b = 0; for (auto& v : vs) b |= 1ull << id.at(v); return b; };
+    auto to_mask = [&](const SReq& r) { return ksched::Req{bits(r.values), r.gt, r.lt, r.present, r.complement, r.has_gt, r.has_lt}; };
+
+    // ---- random requirements
+    const std::vector<std::string> named_list(named.begin(), named.end());
+    auto named_atom = [&]() {
+      SReq r;
+      const int op = rnd(m > 0 ? 6 : 4);
+      if ((op == 0 || op == 1) && !named_list.empty()) {
+        r.complement = op == 1;
+        for (int i = 1 + rnd(3); i > 0; --i) r.values.insert(named_list[(size_t)rnd((int)named_list.size())]);
+      }
+      else if (op == 3) r.complement = false;
+      else if (op == 4) { r.has_gt = true; r.gt = ts[(size_t)rnd(m)]; }
+      else if (op == 5) { r.has_lt = true; r.lt = ts[(size_t)rnd(m)]; }
+      return r;
+    };
+    auto named_compound = [&]() { SReq r = named_atom(); for (int i = rnd(3); i > 0; --i) r = s_intersect(named_atom(), r); return r; };
+    auto side_atom = [&]() {  // an instance type's In requirement or a node's label
+      SReq r;
+      r.complement = false;
+      for (int i = 1 + rnd(4); i > 0; --i) r.values.insert(pool[(size_t)rnd((int)pool.size())]);
+      return r;
+    };
+    const SReq a = named_compound();
+    const bool b_named = rnd(2) != 0;
+    const SReq b = b_named ? named_compound() : side_atom();
+    const ksched::Req ha = to_mask(a), hb = to_mask(b);
+    const SReq si = s_intersect(a, b);
+    bool ok = true;
+    // host algebra
+    const ksched::Req hi = ksched::req_intersect(ha, hb, hk);
+    ok = ok && s_len_zero(si) == ksched::req_len_zero(hi);
+    ok = ok && s_negative(si) == ksched::req_op_negative(hi, hk) && s_negative(a) == ksched::req_op_negative(ha, hk) &&
+         s_negative(b) == ksched::req_op_negative(hb, hk);
+    if (si.complement) ok = ok && bits(si.values) == hi.values;
+    const uint64_t allowed_a = ksched::req_allowed(ha, dict, hk), allowed_i = ksched::req_allowed(hi, dict, hk);
+    for (auto& v : all) {
+      ok = ok && s_has(a, v) == (((allowed_a >> id.at(v)) & 1) != 0);
+      if (b_named || !rep_of.count(v)) ok = ok && s_has(si, v) == (((allowed_i >> id.at(v)) & 1) != 0);
+    }
+    for (int wk = 0; wk < 2; ++wk)
+      for (int pa = 0; pa < 2; ++pa)
+        for (int pb = 0; pb < 2; ++pb) {
+          SReq na = a, nb = b;
+          na.present = pa != 0;
+          nb.present = pb != 0;
+          ok = ok && s_compatible(na, nb, wk != 0) == ksched::key_compatible(to_mask(na), to_mask(nb), wk != 0, hk) &&
+               s_compatible(nb, na, wk != 0) == ksched::key_compatible(to_mask(nb), to_mask(na), wk != 0, hk);
+        }
+    // region form (what crosses the C-ABI and what the device computes)
+    if (regions) {
+      ksched::Req ra, rb;
+      if (!ksched::req_to_region_form(ha, g, dict, &ra) || !ksched::req_to_region_form(hb, g, dict, &rb)) { ++bad; continue; }
+      const ksched::Req ri = ksched::req_intersect_regions(ra, rb, rk);
+      ok = ok && s_len_zero(si) == ksched::req_len_zero(ri) && s_negative(si) == ksched::req_op_negative(ri, rk) &&
+           s_negative(a) == ksched::req_op_negative(ra, rk);
+      if (si.complement) ok = ok && bits(si.values) == ksched::req_excluded(ri, rk);
+      const uint64_t allowed_r = ksched::req_allowed(ri, dict | g.region_mask, rk) & dict;
+      for (auto& v : all)
+        if (b_named || !rep_of.count(v)) ok = ok && s_has(si, v) == (((allowed_r >> id.at(v)) & 1) != 0);
+      for (int wk = 0; wk < 2; ++wk)
+        for (int pa = 0; pa < 2; ++pa) {
+          SReq na = a;
+          na.present = pa != 0;
+          ksched::Req nra = ra;
+          nra.present = na.present;
+          const bool device = [&] {  // key_compatible with the region-form intersection (what the device compiles)
+            if (!rb.present) return true;
+            if (!wk && !nra.present && !ksched::req_op_negative(rb, rk)) return false;
+            if (!nra.present) return true;
+            ksched::Req i = ksched::req_intersect_regions(nra, rb, rk);
+            if (!ksched::req_len_zero(i)) return true;
+            return ksched::req_op_negative(rb, rk) && ksched::req_op_negative(nra, rk);
+          }();
+          ok = ok && s_compatible(na, b, wk != 0) == device;
+        }
+    }
+    if (!ok) ++bad;
+  }
+  return bad;
+}
+
+// Dictionary facts of one mask key of an encoding (tests): out = [values, representatives of unnamed value classes,
+// Gt/Lt thresholds]. Returns -1 when `key` is not a mask key of the encoding.
+int kh_encoded_key_info(const Encoded* E, const char* key, long long* out) {
+  for (size_t k = 0; k < E->key_names.size(); ++k) {
+    if (E->key_names[k] != key) continue;
+    out[0] = (long long)E->key_values[k].size();
+    out[1] = E->key_representatives[k];
+    out[2] = E->key_regions.empty() ? 0 : E->key_regions[k].n_thresholds;
+    return 0;
+  }
+  return -1;
+}
 }

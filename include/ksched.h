@@ -409,7 +409,10 @@ int ksched_run_resident(ksched_handle* h, int flush_l2);
 int ksched_download(ksched_handle* h, const ksched_problem* problem, ksched_result* result);
 int ksched_run_feasibility_only(ksched_handle* h, int flush_l2, float* elapsed_us);
 
-/* Consolidation simulator on a device-resident cluster snapshot: upload once, then any number of simulations. */
+/* Consolidation simulator on a device-resident cluster snapshot: upload once, then any number of simulations. A handle holds
+   one snapshot: ksched_upload (and ksched_solve through it) reuses the snapshot's buffers and drops it, after which
+   ksched_simulate_batch fails with KSCHED_ERR_INVALID until the next ksched_load_cluster. Keep a snapshot that must survive
+   other work on a handle of its own. */
 int ksched_load_cluster(ksched_handle* h, const ksched_cluster* cluster);
 /* results[n_sets]; node0_types[n_sets][type_words] = surviving InstanceTypeOptions of each simulation's first new node.
    The simulations run back to back on the handle's stream with one synchronisation at the end. */

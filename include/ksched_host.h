@@ -14,12 +14,15 @@
  *   kh_rank_candidates        candidateNodes + sortAndFilterCandidates deprovisioning/helpers.go:171-249, consolidation.go:85-118
  *   kh_cluster_* / kh_consolidate          computeConsolidation + firstNNodeConsolidationOption
  *                                                                       consolidation.go:190-274, multinodeconsolidation.go:74-114
- *   kh_consolidate_single     SingleNodeConsolidation.ComputeCommand   singlenodeconsolidation.go:43-84
+ *   kh_consolidate_single     SingleNodeConsolidation.ComputeCommand   singlenodeconsolidation.go:43-84 (every command taken as valid)
+ *   kh_cluster_validate       Validation.IsValid + ValidateCommand     validation.go:63-172
+ *   kh_consolidate_validated  MultiNodeConsolidation.ComputeCommand    multinodeconsolidation.go:41-70
+ *   kh_consolidate_single_validated  SingleNodeConsolidation.ComputeCommand with validation  singlenodeconsolidation.go:43-84
  *
  * Conventions: opaque pointers are owned by the caller and freed with the matching *_free / *_close; int returns are
  * KSCHED_OK (0) or a negative KSCHED_ERR_* (ksched.h) unless stated; the message of the last failure on the calling thread
- * is kh_scheduler_error() (kh_last_error() for the loader). Actions: 0 do nothing, 1 delete, 2 replace
- * (deprovisioning/types.go). Instance types are named by their index in the problem's instanceTypes list, nodes by their
+ * is kh_scheduler_error() (kh_last_error() for the loader). Actions: 0 do nothing, 1 delete, 2 replace, 3 retry (a command
+ * failed validation, deprovisioning/types.go). Instance types are named by their index in the problem's instanceTypes list, nodes by their
  * index in its nodes list.
  */
 #ifndef KSCHED_HOST_H
@@ -85,6 +88,27 @@ int kh_consolidate(const kh_problem* p, int* out4, int* options, int options_cap
  * independent simulations per device call. out4 = [action, winning position or -1, simulations, n_options]; *node = the
  * node the command removes. */
 int kh_consolidate_single(const kh_problem* p, int first, int last, int batch, int* out4, int* node, int* options, int options_cap);
+
+/* ---- deprovisioning: validation against the cluster as it stands when the consolidation TTL ends (`after`; the wait itself
+ * is the caller's). Every validation of one ComputeCommand reads one snapshot of `after` (DESIGN.md section 6, R7), resident
+ * on a device handle of its own and opened at the first command that needs validation. Validation candidates:
+ * candidateNodes(after, Validation.ShouldDeprovision) in node-list order, matched to the command's nodes by name. */
+/* Validation.IsValid of n_sets commands of an open session, in one ksched_simulate_batch call. Command q = the candidates
+ * at positions sets[set_off[q] .. set_off[q+1]), actions[q] (1 or 2) and options[q * options_stride ...] (n_options[q]) -
+ * what kh_cluster_probe_sets returns. valid[q] = 1 / 0. The session keeps the snapshot of `after` until it closes or is
+ * handed a different problem (told apart by a process-unique problem id, not by address). */
+int kh_cluster_validate(kh_cluster* c, const kh_problem* after, const int* sets, const int* set_off, int n_sets, const int* actions, const int* options,
+                        int options_stride, const int* n_options, int* valid);
+/* MultiNodeConsolidation.ComputeCommand: the search of kh_consolidate on `before`, then one validation against `after`; a
+ * command that fails it becomes retry, out4 = [3, 0, simulations, 0]. *verdict = 1 valid, 0 invalid, -1 none run. */
+int kh_consolidate_validated(const kh_problem* before, const kh_problem* after, int* out4, int* options, int options_cap, int* probes,
+                             int* probe_actions, int probes_cap, int* n_probes, int* verdict);
+/* SingleNodeConsolidation.ComputeCommand: as kh_consolidate_single, but each batch's actionable commands are validated
+ * together against `after` and the first valid one wins; none, after a failed validation, is retry (3). trace / trace_valid =
+ * positions validated and verdicts up to and including the winner, *n_trace of them; *failed_validation = a validation failed.
+ * Shares [first, last) merge as: the first share with a winner wins; with none, retry when any share failed a validation. */
+int kh_consolidate_single_validated(const kh_problem* before, const kh_problem* after, int first, int last, int batch, int* out4, int* node,
+                                    int* options, int options_cap, int* trace, int* trace_valid, int trace_cap, int* n_trace, int* failed_validation);
 
 /* ---- self-test of the encoder's value classes (CPU, no device): random wide keys and requirement pairs, the exact string
  * algebra against the collapsed masks (host form and region form). Returns the number of mismatches. */

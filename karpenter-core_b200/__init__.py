@@ -142,6 +142,13 @@ def lib():
                                         C.POINTER(C.c_int)]
     L.kh_cluster_candidates.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.c_int]
     L.kh_consolidate_single.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int]
+    L.kh_consolidate_validated.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                           C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    L.kh_consolidate_single_validated.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                                  C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int),
+                                                  C.POINTER(C.c_int)]
+    L.kh_cluster_validate.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                      C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     L.kh_allgather_i32.argtypes = [C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int)]
     L.kh_nccl_init.argtypes = [C.c_void_p, C.c_int, C.c_int]
     L.kh_rank_candidates.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_double), C.c_int]
@@ -358,6 +365,27 @@ class ClusterSession:
                                            nopt))
         return [(int(actions[q]), list(opts[q * stride:q * stride + min(nopt[q], stride)])) for q in range(len(sets))]
 
+    def validate(self, after: Problem, commands):
+        """Validation.IsValid (validation.go:63-172) of commands against `after`, the cluster when the TTL ends, in one device
+        batch. commands = [(positions in the disruption order, action 1 or 2, options)], as probe_sets returns them -> [bool].
+        The session keeps the snapshot of `after` until it closes or is handed a different problem."""
+        if not commands:
+            return []
+        flat = [i for s_, _, _ in commands for i in s_]
+        off = [0]
+        for s_, _, _ in commands:
+            off.append(off[-1] + len(s_))
+        stride = max(1, max(len(o) for _, _, o in commands))
+        opts = (C.c_int * (stride * len(commands)))()
+        for q, (_, _, o) in enumerate(commands):
+            opts[q * stride:q * stride + len(o)] = list(o)
+        n = len(commands)
+        valid = (C.c_int * n)()
+        self._after = after   # the session's snapshot of `after` lives as long as the session or the next validate
+        _check(lib().kh_cluster_validate(self.ptr, after.ptr, (C.c_int * max(1, len(flat)))(*flat), (C.c_int * len(off))(*off), n,
+                                         (C.c_int * n)(*[a for _, a, _ in commands]), opts, stride, (C.c_int * n)(*[len(o) for _, _, o in commands]), valid))
+        return [bool(v) for v in valid]
+
     def close(self):
         if getattr(self, "ptr", None) and _lib is not None:
             _lib.kh_cluster_close(self.ptr)
@@ -406,6 +434,20 @@ class MultiNodeConsolidation:
         return {"action": out4[0], "nodes_removed": out4[1], "simulations": out4[2], "options": list(opts[:out4[3]]),
                 "probes": list(probes[:npr.value]), "probe_actions": list(acts[:npr.value])}
 
+    def compute_command(self, after: Problem):
+        """MultiNodeConsolidation.ComputeCommand (multinodeconsolidation.go:41-70): the search, then Validation.IsValid of its
+        command against `after`, the cluster when the TTL ends. A command that fails validation is retry (action 3).
+        validations = the verdicts of the validations run (none when the search finds nothing)."""
+        out4 = (C.c_int * 4)()
+        opts = (C.c_int * 8192)()
+        probes = (C.c_int * 256)()
+        acts = (C.c_int * 256)()
+        npr, verdict = C.c_int(), C.c_int()
+        _check(lib().kh_consolidate_validated(self.problem.ptr, after.ptr, out4, opts, 8192, probes, acts, 256, C.byref(npr), C.byref(verdict)))
+        return {"action": out4[0], "nodes_removed": out4[1], "simulations": out4[2], "options": list(opts[:out4[3]]),
+                "probes": list(probes[:npr.value]), "probe_actions": list(acts[:npr.value]),
+                "validations": [] if verdict.value < 0 else [bool(verdict.value)]}
+
     def candidates(self):
         return int(lib().kh_consolidate_candidates(self.problem.ptr))
 
@@ -442,12 +484,36 @@ class SingleNodeConsolidation:
     def __init__(self, problem: Problem):
         self.problem = problem
 
-    def compute_command(self, first=0, last=-1, batch=64):
+    def compute_command(self, first=0, last=-1, batch=64, after=None):
+        """after = the cluster when the TTL ends: each batch's actionable commands are validated against it in one more device
+        call, the first valid one wins, and none after a failed validation is retry (action 3). The result then also carries
+        "validations" = [(position, valid)] of what the sequential loop validates and "failed_validation"."""
         out4 = (C.c_int * 4)()
         node = C.c_int()
         opts = (C.c_int * 8192)()
-        _check(lib().kh_consolidate_single(self.problem.ptr, int(first), int(last), int(batch), out4, C.byref(node), opts, 8192))
-        return {"action": out4[0], "position": out4[1], "simulations": out4[2], "node": node.value, "options": list(opts[:out4[3]])}
+        if after is None:
+            _check(lib().kh_consolidate_single(self.problem.ptr, int(first), int(last), int(batch), out4, C.byref(node), opts, 8192))
+            return {"action": out4[0], "position": out4[1], "simulations": out4[2], "node": node.value, "options": list(opts[:out4[3]])}
+        cap = 1 << 16
+        trace, valid = (C.c_int * cap)(), (C.c_int * cap)()
+        ntr, failed = C.c_int(), C.c_int()
+        _check(lib().kh_consolidate_single_validated(self.problem.ptr, after.ptr, int(first), int(last), int(batch), out4, C.byref(node), opts, 8192,
+                                                     trace, valid, cap, C.byref(ntr), C.byref(failed)))
+        return {"action": out4[0], "position": out4[1], "simulations": out4[2], "node": node.value, "options": list(opts[:out4[3]]),
+                "validations": [(trace[i], bool(valid[i])) for i in range(min(ntr.value, cap))], "failed_validation": bool(failed.value)}
+
+
+def merge_single_node_shares(shares):
+    """SingleNodeConsolidation.ComputeCommand of a sweep split into shares [first, last) in order: the first share with a
+    winner gives the command; the trace is every earlier share's trace and the winner's; with no winner the result is retry
+    when any share failed a validation, else nothing."""
+    trace = []
+    for r in shares:
+        trace += r["validations"]
+        if r["action"] in (1, 2):
+            return dict(r, validations=trace, failed_validation=any(not v for _, v in trace))
+    failed = any(r["failed_validation"] for r in shares)
+    return {"action": 3 if failed else 0, "position": -1, "node": -1, "options": [], "validations": trace, "failed_validation": failed}
 
 
 def speculation_frontier(lo, hi, width):

@@ -626,6 +626,8 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
   for (int i = 0; i < pb->n_filter_terms; ++i)
     if (pb->filter_terms[i].meta >> KSCHED_META_HASGT_SHIFT) { h->err = "requirement with HASGT/HASLT set: pass Gt/Lt in region form"; return KSCHED_ERR_INVALID; }
   CUDA_TRY(h, cudaSetDevice(h->device));
+  // the superset buffers ksched_load_cluster filled are about to be overwritten: simulations need a new ksched_load_cluster
+  h->have_cluster = false;
   h->tm.h2d_bytes = 0;
   const DevCatalog& c = h->cat;
   const int P = pb->n_pods, NC = pb->n_classes, NE = pb->n_existing, NG = pb->n_groups, W32 = c.W32, V = c.n_templates;

@@ -12,6 +12,7 @@
 // Resource quantities are int64 MILLI-units (k8s resource.Quantity is exact
 // decimal; every quantity the reference tests use is a whole number of milli).
 #pragma once
+#include <atomic>
 #include <cstdint>
 #include <map>
 #include <memory>
@@ -182,7 +183,14 @@ struct ProblemDerived {
   virtual ~ProblemDerived() = default;
 };
 
+// A process-unique id per Problem: a cache keyed on a Problem must not take a new Problem at a freed one's address for it.
+inline uint64_t next_problem_id() {
+  static std::atomic<uint64_t> last{0};
+  return ++last;
+}
+
 struct Problem {
+  const uint64_t id = next_problem_id();
   mutable std::shared_ptr<ProblemDerived> derived;   // see khost::encode; a Problem is immutable once built
   mutable std::mutex derived_mu;
   std::vector<std::string> extra_well_known_labels;  // v1alpha5.WellKnownLabels additions

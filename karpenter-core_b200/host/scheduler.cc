@@ -31,6 +31,20 @@ namespace {
 thread_local std::string g_err;
 ksched_handle* g_handle = nullptr;
 int g_device = 0;
+// g_handle holds one cluster snapshot at a time: the id of the ClusterSession whose snapshot it holds, 0 when anything else
+// (a Solve, a fresh-encode simulation, ResidentSolve, another session) has been loaded onto it since
+uint64_t g_resident_session = 0;
+uint64_t g_last_session = 0;
+// The same for ResidentSolve (kh_gpu_*): the encoding kh_gpu_load / kh_gpu_solve_e2e last put on g_handle, and whether
+// g_handle still holds it. kh_gpu_run loads it again when something else took the handle since.
+const Encoded* g_gpu_encoded = nullptr;
+bool g_gpu_current = false;
+
+// something other than the recorded session / ResidentSolve encoding is about to be loaded onto g_handle
+void handle_taken() {
+  g_resident_session = 0;
+  g_gpu_current = false;
+}
 int g_count_visited = 0;  // exact nodes_visited statistic (opt-in: tests); switches the pack kernel's steady-state paths off
 
 int fail(int code, const std::string& msg) {
@@ -190,14 +204,19 @@ int error_code(const std::exception& e) {
   return m.rfind("unsupported:", 0) == 0 ? KSCHED_ERR_UNSUPPORTED : KSCHED_ERR_INVALID;
 }
 
-int solve_encoded(Encoded& E, ResultBuffers& B, bool want_feasibility) {
-  int rc = ensure_handle();
-  if (rc != KSCHED_OK) return rc;
-  rc = ksched_load_catalog(g_handle, &E.catalog);
-  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
+// One ksched_solve of E on h (default: the scheduler handle, whose cluster snapshot this displaces).
+int solve_encoded(Encoded& E, ResultBuffers& B, bool want_feasibility, ksched_handle* h = nullptr) {
+  if (!h) {
+    int rc = ensure_handle();
+    if (rc != KSCHED_OK) return rc;
+    h = g_handle;
+  }
+  if (h == g_handle) handle_taken();
+  int rc = ksched_load_catalog(h, &E.catalog);
+  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(h));
   B.prepare(E, want_feasibility);
-  rc = ksched_solve(g_handle, &E.problem, &B.r);
-  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
+  rc = ksched_solve(h, &E.problem, &B.r);
+  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(h));
   return KSCHED_OK;
 }
 
@@ -243,6 +262,8 @@ extern "C" {
 const char* kh_scheduler_error() { return g_err.c_str(); }
 int kh_set_device(int ordinal) {
   if (g_handle) { ksched_destroy(g_handle); g_handle = nullptr; }
+  handle_taken();
+  g_gpu_encoded = nullptr;
   g_device = ordinal;
   return KSCHED_OK;
 }
@@ -283,6 +304,7 @@ int kh_scheduler_solve_timed(const Problem* P, const int* candidates, int ncand,
     const auto t1 = clk::now();
     int rc = ensure_handle();
     if (rc != KSCHED_OK) return rc;
+    handle_taken();
     rc = ksched_load_catalog(g_handle, &E->catalog);
     if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
     const auto t2 = clk::now();
@@ -311,7 +333,10 @@ Encoded* kh_encode(const Problem* P, const int* candidates, int ncand) {
     return nullptr;
   }
 }
-void kh_encoded_free(Encoded* E) { delete E; }
+void kh_encoded_free(Encoded* E) {
+  if (E == g_gpu_encoded) { g_gpu_encoded = nullptr; g_gpu_current = false; }
+  delete E;
+}
 // dims: [pods, classes, existing, groups, types, templates, keys, resources, type_words, class_topo]
 void kh_encoded_dims(const Encoded* E, long long* out) {
   out[0] = (long long)E->pods.size(); out[1] = (long long)E->classes.size(); out[2] = (long long)E->existing.size();
@@ -325,21 +350,36 @@ const ksched_problem* kh_encoded_problem(const Encoded* E) { return &E->problem;
 int kh_gpu_load(Encoded* E) {
   int rc = ensure_handle();
   if (rc != KSCHED_OK) return rc;
+  handle_taken();
+  g_gpu_encoded = nullptr;
   rc = ksched_load_catalog(g_handle, &E->catalog);
   if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
   rc = ksched_upload(g_handle, &E->problem);
   if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
+  g_gpu_encoded = E;
+  g_gpu_current = true;
   return KSCHED_OK;
+}
+// the ResidentSolve encoding back on g_handle when a session, a Solve or a fresh-encode simulation took it since its load
+int gpu_make_current() {
+  if (!g_gpu_encoded || g_gpu_current) return KSCHED_OK;
+  return kh_gpu_load(const_cast<Encoded*>(g_gpu_encoded));
 }
 int kh_gpu_run(int flush_l2) {
   if (!g_handle) return fail(KSCHED_ERR_INVALID, "no handle");
-  int rc = ksched_run_resident(g_handle, flush_l2);
+  int rc = gpu_make_current();
+  if (rc != KSCHED_OK) return rc;
+  g_resident_session = 0;
+  rc = ksched_run_resident(g_handle, flush_l2);
   if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
   return rc;
 }
 int kh_gpu_run_feasibility(int flush_l2, float* us) {
   if (!g_handle) return fail(KSCHED_ERR_INVALID, "no handle");
-  int rc = ksched_run_feasibility_only(g_handle, flush_l2, us);
+  int rc = gpu_make_current();
+  if (rc != KSCHED_OK) return rc;
+  g_resident_session = 0;
+  rc = ksched_run_feasibility_only(g_handle, flush_l2, us);
   if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
   return rc;
 }
@@ -348,6 +388,7 @@ int kh_gpu_run_feasibility(int flush_l2, float* us) {
 int kh_gpu_download(Encoded* E, Result* out, unsigned long long* feasibility_out, unsigned long long* best_out) {
   if (!g_handle) return fail(KSCHED_ERR_INVALID, "no handle");
   *out = Result();
+  if (g_gpu_encoded && !g_gpu_current) return fail(KSCHED_ERR_INVALID, "the handle was used for other work since this problem's run: run it again");
   ResultBuffers B;
   B.prepare(*E, feasibility_out != nullptr || best_out != nullptr);
   int rc = ksched_download(g_handle, &E->problem, &B.r);
@@ -371,6 +412,8 @@ int kh_gpu_download(Encoded* E, Result* out, unsigned long long* feasibility_out
 // all inside the call (the catalog stays resident, as it would across reconciles). Returns wall-clock microseconds.
 int kh_gpu_solve_e2e(Encoded* E, Result* out, double* wall_us) {
   if (!g_handle) return fail(KSCHED_ERR_INVALID, "no handle");
+  handle_taken();
+  g_gpu_encoded = nullptr;
   ResultBuffers B;
   B.prepare(*E, false);
   auto t0 = std::chrono::steady_clock::now();
@@ -378,12 +421,15 @@ int kh_gpu_solve_e2e(Encoded* E, Result* out, double* wall_us) {
   auto t1 = std::chrono::steady_clock::now();
   if (wall_us) *wall_us = std::chrono::duration<double, std::micro>(t1 - t0).count();
   if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
+  g_gpu_encoded = E;
+  g_gpu_current = true;
   if (out) { *out = Result(); decode(*E, B, *out); }
   return KSCHED_OK;
 }
 int kh_gpu_load_catalog(Encoded* E) {
   int rc = ensure_handle();
   if (rc != KSCHED_OK) return rc;
+  g_resident_session = 0;
   rc = ksched_load_catalog(g_handle, &E->catalog);
   if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
   return KSCHED_OK;
@@ -396,6 +442,29 @@ int kh_gpu_timings(ksched_timings* t) { return g_handle ? ksched_get_timings(g_h
 namespace {
 struct Cand { int node; const InstanceType* it; std::string ct, zone; double cost; };
 struct Cmd { int action = 0; std::vector<int> options; };
+
+// candidateNodes (deprovisioning/helpers.go:171-249) with the ShouldDeprovision predicate consolidation and Validation share
+// (consolidation.go:104-118, validation.go:101-107); *prov = the node's provisioner or nullptr
+bool candidate_node(const Problem* P, const StateNode& n, const Provisioner** prov_out) {
+  const Provisioner* prov = nullptr;
+  auto pl = n.labels.find("karpenter.sh/provisioner-name");
+  if (pl != n.labels.end())
+    for (auto& pr : P->provisioners) if (pr.name == pl->second) prov = &pr;
+  *prov_out = prov;
+  bool ok = !n.marked_for_deletion && prov != nullptr;                                  // helpers.go:186-192
+  if (ok) {
+    auto itn = n.labels.find("node.kubernetes.io/instance-type");                       // :194-198
+    bool it_ok = false;
+    if (itn != n.labels.end())
+      for (int idx : prov->instance_types) if (P->instance_types[(size_t)idx].name == itn->second) it_ok = true;
+    ok = it_ok;
+  }
+  ok = ok && n.labels.count("karpenter.sh/capacity-type") && n.labels.count("topology.kubernetes.io/zone");  // :201-208
+  if (ok) { auto ini = n.labels.find("karpenter.sh/initialized"); ok = ini != n.labels.end() && ini->second == "true"; }  // :211-213
+  ok = ok && !n.nominated;                                                              // :215-217
+  if (ok) ok = n.do_not_consolidate != 0 ? n.do_not_consolidate != 1 : prov->consolidation_enabled;  // ShouldDeprovision
+  return ok;
+}
 
 // candidateNodes + sortAndFilterCandidates (deprovisioning/helpers.go:171-249,339-366, consolidation.go:85-118). The string /
 // API-object side (labels, annotations, PDB selectors) is decided here; the disruption costs, their lifetime scaling and the
@@ -418,21 +487,7 @@ void rank_on_device(const Problem* P, std::vector<int>* order, std::vector<doubl
       continue;
     }
     const Provisioner* prov = nullptr;
-    auto pl = n.labels.find("karpenter.sh/provisioner-name");
-    if (pl != n.labels.end())
-      for (auto& pr : P->provisioners) if (pr.name == pl->second) prov = &pr;
-    bool ok = !n.marked_for_deletion && prov != nullptr;                                  // helpers.go:186-192
-    if (ok) {
-      auto itn = n.labels.find("node.kubernetes.io/instance-type");                       // :194-198
-      bool it_ok = false;
-      if (itn != n.labels.end())
-        for (int idx : prov->instance_types) if (P->instance_types[(size_t)idx].name == itn->second) it_ok = true;
-      ok = it_ok;
-    }
-    ok = ok && n.labels.count("karpenter.sh/capacity-type") && n.labels.count("topology.kubernetes.io/zone");  // :201-208
-    if (ok) { auto ini = n.labels.find("karpenter.sh/initialized"); ok = ini != n.labels.end() && ini->second == "true"; }  // :211-213
-    ok = ok && !n.nominated;                                                              // :215-217
-    if (ok) ok = n.do_not_consolidate != 0 ? n.do_not_consolidate != 1 : prov->consolidation_enabled;  // consolidation.go:104-118
+    bool ok = candidate_node(P, n, &prov);
     ok = ok && !n.deleting;                                                               // canBeTerminated helpers.go:340
     eligible[i] = ok ? 1 : 0;
     if (prov && prov->has_ttl_until_expired) { ttl[i] = (double)prov->ttl_seconds_until_expired; age[i] = P->now_ts - n.creation_ts; }
@@ -577,16 +632,173 @@ Cmd compute_consolidation_encoded(const Problem* P, const std::vector<Cand>& sel
   return finish_command(P, *E, sel, scheduled == E->pods.size(), B.r.n_new_nodes, B.nodes[0].reqs, &B.types[0], multi);
 }
 
+// ksched_load_catalog + ksched_load_cluster of a superset encoding (khost::encode(..., true)) on h
+int load_snapshot(ksched_handle* h, Encoded& E) {
+  int rc = ksched_load_catalog(h, &E.catalog);
+  if (rc != KSCHED_OK) return rc;
+  ksched_cluster cl{};
+  cl.problem = &E.problem;
+  cl.pod_node = E.pod_node.data();
+  if (E.problem.n_groups > 0) {
+    cl.class_count_begin = E.class_count_begin.data();
+    cl.class_count = E.class_count.data();
+    cl.node_domain = E.node_domain.data();
+    cl.node_has_hostname_label = E.node_has_hostname_label.data();
+    cl.group_filter_match = E.group_filter_match.data();
+  }
+  return ksched_load_cluster(h, &cl);
+}
+
+// One ksched_simulate_batch on the snapshot of E that h holds: simulation q removes the existing slots slot_sets[q].
+// skip[q]: an uninitialised node stays, and simulateScheduling gives up on it (helpers.go:109-113).
+struct SimBatch {
+  std::vector<ksched_sim_result> res;
+  std::vector<uint64_t> types;  // [simulation][type_words]: the first new node's InstanceTypeOptions
+  std::vector<char> skip;
+};
+SimBatch simulate_on(ksched_handle* h, const Encoded& E, const std::vector<std::vector<int32_t>>& slot_sets) {
+  const size_t n = slot_sets.size(), NE = E.existing.size(), V = E.templates.size();
+  SimBatch out;
+  out.skip.assign(n, 0);
+  std::vector<std::vector<int64_t>> rem(n);
+  std::vector<ksched_candidate_set> cs(n);
+  std::vector<char> removed(NE);
+  for (size_t q = 0; q < n; ++q) {
+    std::fill(removed.begin(), removed.end(), 0);
+    rem[q].resize(V * KSCHED_MAX_RES);
+    for (size_t v = 0; v < V; ++v) for (int r = 0; r < KSCHED_MAX_RES; ++r) rem[q][v * KSCHED_MAX_RES + r] = E.templates[v].remaining[r];
+    for (int32_t e : slot_sets[q]) {
+      removed[(size_t)e] = 1;
+      const int v = E.existing_template[(size_t)e];  // scheduler.go:221-248 only charges the nodes that stay
+      if (v >= 0) for (int r = 0; r < KSCHED_MAX_RES; ++r) rem[q][(size_t)v * KSCHED_MAX_RES + r] += E.existing_capacity[(size_t)e * KSCHED_MAX_RES + r];
+    }
+    for (size_t e = 0; e < NE; ++e) if (!removed[e] && !E.existing_initialized[e]) out.skip[q] = 1;
+    cs[q] = ksched_candidate_set{slot_sets[q].data(), (int32_t)slot_sets[q].size(), 0, rem[q].data()};
+  }
+  out.res.resize(n);
+  out.types.resize(n * (size_t)E.type_words);
+  int rc = ksched_simulate_batch(h, cs.data(), (int)cs.size(), out.res.data(), out.types.data());
+  if (rc != KSCHED_OK) throw std::runtime_error(ksched_last_error(h));
+  for (size_t q = 0; q < n; ++q)
+    if (!out.skip[q] && out.res[q].error) throw std::runtime_error("simulation failed on the device");
+  return out;
+}
+
+// A consolidation command as Validation reads it: the names of the nodes it removes, delete (1) or replace (2), and the
+// names of the replacement's instance-type options (commands and the cluster after the TTL meet by name).
+struct VCmd {
+  std::vector<std::string> nodes;
+  int action = 0;
+  std::vector<std::string> options;
+};
+
+// ValidateCommand after its simulateScheduling (validation.go:122-171); bits = the first new node's options (unfiltered)
+bool command_valid(const Problem* A, const Encoded& E, const VCmd& c, bool all_scheduled, int n_new, const uint64_t* bits) {
+  if (!all_scheduled) return false;
+  if (n_new == 0) return c.action == 1;          // :132-140 valid only when no replacement was expected
+  if (n_new > 1 || c.action != 2) return false;  // :142-151
+  std::set<std::string> rhs;                     // instanceTypesAreSubset (helpers.go:118-122), by name
+  for (size_t col = 0; col < E.type_input_index.size(); ++col)
+    if ((bits[col / 64] >> (col % 64)) & 1) rhs.insert(A->instance_types[(size_t)E.type_input_index[col]].name);
+  for (auto& o : c.options) if (!rhs.count(o)) return false;
+  return true;
+}
+
+struct HandleDeleter { void operator()(ksched_handle* h) const { ksched_destroy(h); } };
+
+// The cluster after the TTL, resident on a handle of its own (the pass's session keeps the scheduler handle). Every
+// validation of one ComputeCommand reads this one snapshot (DESIGN.md §6 R7). The validation candidates are
+// candidateNodes(after, Validation.ShouldDeprovision) in node-list order (validation.go:78-83): they do not go through
+// sortAndFilterCandidates, so a node that a PDB or a DeletionTimestamp keeps out of the pass is still validated. With
+// "deriveCandidates": false they are the nodes marked "candidate" that are not marked for deletion. Clusters the snapshot refuses are validated one freshly
+// encoded ksched_solve at a time on the same handle.
+struct ValidationSnapshot {
+  const Problem* A = nullptr;
+  uint64_t problem_id = 0;          // Problem::id of A: never shared with a problem allocated later at the same address
+  std::vector<int> cands;           // Problem.nodes indices
+  std::set<std::string> nominated;  // Cluster.IsNodeNominated
+  std::unique_ptr<ksched_handle, HandleDeleter> h;
+  std::unique_ptr<Encoded> E;       // superset encoding (resident == true)
+  std::vector<int> slot_of_node;
+  bool resident = false;
+
+  explicit ValidationSnapshot(const Problem* a) : A(a), problem_id(a->id) {
+    for (size_t i = 0; i < A->nodes.size(); ++i) {
+      const StateNode& n = A->nodes[i];
+      if (n.nominated) nominated.insert(n.name);
+      const Provisioner* prov = nullptr;
+      // candidateNodes skips nodes marked for deletion in either mode (helpers.go:185-188)
+      if (A->derive_candidates ? candidate_node(A, n, &prov) : n.candidate && !n.marked_for_deletion) cands.push_back((int)i);
+    }
+    ksched_handle* raw = nullptr;
+    if (ksched_create(g_device, &raw) != KSCHED_OK) throw std::runtime_error("ksched_create failed: no usable CUDA device (the product has no CPU path)");
+    h.reset(raw);
+    auto sup = khost::encode(*A, cands, true);
+    sup->problem.count_nodes_visited = 0;
+    int rc = load_snapshot(h.get(), *sup);
+    if (rc == KSCHED_ERR_UNSUPPORTED) return;  // resident stays false
+    if (rc != KSCHED_OK) throw std::runtime_error(ksched_last_error(h.get()));
+    E = std::move(sup);
+    slot_of_node.assign(A->nodes.size(), -1);
+    for (size_t e = 0; e < E->existing_state_index.size(); ++e) slot_of_node[(size_t)E->existing_state_index[e]] = (int)e;
+    resident = true;
+  }
+
+  // Validation.IsValid for every command: the simulations of all of them in one ksched_simulate_batch call
+  std::vector<char> validate(const std::vector<VCmd>& cmds) {
+    std::vector<char> ok(cmds.size(), 0);
+    std::vector<size_t> run;               // commands that reach simulateScheduling
+    std::vector<std::vector<int>> mapped;  // their mapped nodes (Problem.nodes indices)
+    for (size_t q = 0; q < cmds.size(); ++q) {
+      bool nom = false;
+      for (auto& name : cmds[q].nodes) nom = nom || nominated.count(name) > 0;  // validation.go:85-91
+      if (nom) continue;
+      std::set<std::string> names(cmds[q].nodes.begin(), cmds[q].nodes.end());
+      std::vector<int> m;
+      for (int i : cands) if (names.count(A->nodes[(size_t)i].name)) m.push_back(i);  // mapNodes helpers.go:328-337
+      if (m.empty()) continue;                                                         // validation.go:113-116
+      run.push_back(q);
+      mapped.push_back(std::move(m));
+    }
+    if (run.empty()) return ok;
+    if (resident) {
+      std::vector<std::vector<int32_t>> slots(run.size());
+      for (size_t j = 0; j < run.size(); ++j) for (int i : mapped[j]) slots[j].push_back(slot_of_node[(size_t)i]);
+      SimBatch sb = simulate_on(h.get(), *E, slots);
+      for (size_t j = 0; j < run.size(); ++j)
+        if (!sb.skip[j])
+          ok[run[j]] = command_valid(A, *E, cmds[run[j]], sb.res[j].n_unscheduled == 0, sb.res[j].n_new_nodes, &sb.types[j * (size_t)E->type_words]);
+      return ok;
+    }
+    for (size_t j = 0; j < run.size(); ++j) {
+      auto F = khost::encode(*A, mapped[j]);
+      F->problem.count_nodes_visited = 0;
+      ResultBuffers B;
+      if (solve_encoded(*F, B, false, h.get()) != KSCHED_OK) throw std::runtime_error(g_err);
+      bool init = true;
+      for (size_t e = 0; e < F->existing.size(); ++e) init = init && F->existing_initialized[e];
+      size_t scheduled = 0;
+      for (auto a : B.assign) if (a >= 0) ++scheduled;
+      ok[run[j]] = init && command_valid(A, *F, cmds[run[j]], scheduled == F->pods.size(), B.r.n_new_nodes, &B.types[0]);
+    }
+    return ok;
+  }
+};
+
 // The consolidation pass over one cluster: candidates ranked once, the cluster resident on the device once
 // (ksched_load_cluster), every computeConsolidation a ksched_simulate_batch entry. Clusters the snapshot cannot hold
 // (topology groups) are simulated one freshly encoded ksched_solve at a time - still on the GPU, never on the CPU.
+// Sessions share the scheduler handle: a session whose snapshot something else displaced loads it again before its next
+// batch (g_resident_session).
 struct ClusterSession {
   const Problem* P = nullptr;
   std::vector<Cand> cands;            // disruption order
   std::unique_ptr<Encoded> E;         // superset encoding (resident == true)
   std::vector<int> slot_of_node;      // Problem.nodes index -> existing slot
   bool resident = false;
+  uint64_t id = 0;
   int simulations = 0;
+  std::unique_ptr<ValidationSnapshot> validation_snapshot;  // opened at the first command that needs validation
 
   explicit ClusterSession(const Problem* p) : P(p), cands(sorted_candidates(p)) {
     if (ensure_handle() != KSCHED_OK) throw std::runtime_error(g_err);
@@ -594,25 +806,16 @@ struct ClusterSession {
     for (auto& c : cands) nodes.push_back(c.node);
     auto sup = khost::encode(*P, nodes, true);
     sup->problem.count_nodes_visited = 0;
-    int rc = ksched_load_catalog(g_handle, &sup->catalog);
-    if (rc != KSCHED_OK) throw std::runtime_error(ksched_last_error(g_handle));
-    ksched_cluster cl{};
-    cl.problem = &sup->problem;
-    cl.pod_node = sup->pod_node.data();
-    if (sup->problem.n_groups > 0) {
-      cl.class_count_begin = sup->class_count_begin.data();
-      cl.class_count = sup->class_count.data();
-      cl.node_domain = sup->node_domain.data();
-      cl.node_has_hostname_label = sup->node_has_hostname_label.data();
-      cl.group_filter_match = sup->group_filter_match.data();
-    }
-    rc = ksched_load_cluster(g_handle, &cl);
+    handle_taken();
+    int rc = load_snapshot(g_handle, *sup);
     if (rc == KSCHED_ERR_UNSUPPORTED) return;  // resident stays false
     if (rc != KSCHED_OK) throw std::runtime_error(ksched_last_error(g_handle));
     E = std::move(sup);
     slot_of_node.assign(P->nodes.size(), -1);
     for (size_t e = 0; e < E->existing_state_index.size(); ++e) slot_of_node[(size_t)E->existing_state_index[e]] = (int)e;
     resident = true;
+    id = ++g_last_session;
+    g_resident_session = id;
   }
 
   // computeConsolidation for every set (positions in the disruption order), one ksched_simulate_batch call
@@ -627,38 +830,25 @@ struct ClusterSession {
       }
       return out;
     }
-    const size_t NE = E->existing.size(), V = E->templates.size();
     std::vector<std::vector<int32_t>> slots(sets.size());
-    std::vector<std::vector<int64_t>> rem(sets.size());
-    std::vector<ksched_candidate_set> cs(sets.size());
-    std::vector<char> skip(sets.size(), 0);
-    std::vector<char> removed(NE);
-    for (size_t q = 0; q < sets.size(); ++q) {
-      std::fill(removed.begin(), removed.end(), 0);
-      rem[q].resize(V * KSCHED_MAX_RES);
-      for (size_t v = 0; v < V; ++v) for (int r = 0; r < KSCHED_MAX_RES; ++r) rem[q][v * KSCHED_MAX_RES + r] = E->templates[v].remaining[r];
+    for (size_t q = 0; q < sets.size(); ++q)
       for (int i : sets[q]) {
         const int e = slot_of_node.at((size_t)cands.at((size_t)i).node);
         if (e < 0) throw std::runtime_error("candidate is not an existing node of the snapshot");
         slots[q].push_back(e);
-        removed[(size_t)e] = 1;
-        const int v = E->existing_template[(size_t)e];  // scheduler.go:221-248 only charges the nodes that stay
-        if (v >= 0) for (int r = 0; r < KSCHED_MAX_RES; ++r) rem[q][(size_t)v * KSCHED_MAX_RES + r] += E->existing_capacity[(size_t)e * KSCHED_MAX_RES + r];
       }
-      // helpers.go:109-113: an uninitialised node among those that stay ends the simulation with "do nothing"
-      for (size_t e = 0; e < NE; ++e) if (!removed[e] && !E->existing_initialized[e]) skip[q] = 1;
-      cs[q] = ksched_candidate_set{slots[q].data(), (int32_t)slots[q].size(), 0, rem[q].data()};
+    if (g_resident_session != id) {  // displaced: the time of one reload, the same answers
+      if (ensure_handle() != KSCHED_OK) throw std::runtime_error(g_err);
+      handle_taken();
+      if (load_snapshot(g_handle, *E) != KSCHED_OK) throw std::runtime_error(ksched_last_error(g_handle));
+      g_resident_session = id;
     }
-    std::vector<ksched_sim_result> res(sets.size());
-    std::vector<uint64_t> types(sets.size() * (size_t)E->type_words);
-    int rc = ksched_simulate_batch(g_handle, cs.data(), (int)cs.size(), res.data(), types.data());
-    if (rc != KSCHED_OK) throw std::runtime_error(ksched_last_error(g_handle));
+    SimBatch sb = simulate_on(g_handle, *E, slots);
     for (size_t q = 0; q < sets.size(); ++q) {
-      if (skip[q]) continue;
-      if (res[q].error) throw std::runtime_error("simulation failed on the device");
+      if (sb.skip[q]) continue;
       std::vector<Cand> sel;
       for (int i : sets[q]) sel.push_back(cands[(size_t)i]);
-      out[q] = finish_command(P, *E, sel, res[q].n_unscheduled == 0, res[q].n_new_nodes, res[q].node0.reqs, &types[q * (size_t)E->type_words], multi);
+      out[q] = finish_command(P, *E, sel, sb.res[q].n_unscheduled == 0, sb.res[q].n_new_nodes, sb.res[q].node0.reqs, &sb.types[q * (size_t)E->type_words], multi);
     }
     return out;
   }
@@ -667,7 +857,85 @@ struct ClusterSession {
     for (int i = 0; i < count; ++i) set.push_back(i);
     return compute_many({set}, true)[0];
   }
+
+  // the command that removes the candidates at `positions`, in the terms Validation compares (names)
+  VCmd command(const std::vector<int>& positions, int action, const std::vector<int>& options) const {
+    VCmd c;
+    c.action = action;
+    for (int i : positions) c.nodes.push_back(P->nodes[(size_t)cands.at((size_t)i).node].name);
+    for (int t : options) c.options.push_back(P->instance_types.at((size_t)t).name);
+    return c;
+  }
+  std::vector<char> validate(const Problem* after, const std::vector<VCmd>& cmds) {
+    if (!validation_snapshot || validation_snapshot->problem_id != after->id) {
+      validation_snapshot.reset();  // one extra device handle at a time
+      validation_snapshot = std::make_unique<ValidationSnapshot>(after);
+    }
+    return validation_snapshot->validate(cmds);
+  }
 };
+
+// MultiNodeConsolidation.firstNNodeConsolidationOption (multinodeconsolidation.go:74-114): binary search, one probe per step
+struct Search {
+  Cmd cmd;
+  int count = 0, sims = 0;
+  std::vector<int> probes, actions;
+};
+Search first_n_search(ClusterSession& cs) {
+  Search s;
+  if (cs.cands.size() < 2) return s;
+  int mn = 1, mx = (int)cs.cands.size() - 1;
+  while (mn <= mx) {
+    int mid = (mn + mx) / 2;
+    Cmd c = cs.compute_prefix(mid + 1);
+    ++s.sims;
+    s.probes.push_back(mid + 1);
+    s.actions.push_back(c.action);
+    if (c.action == 1 || c.action == 2) { s.cmd = c; s.count = mid + 1; mn = mid + 1; }
+    else mx = mid - 1;
+  }
+  return s;
+}
+
+// SingleNodeConsolidation.ComputeCommand's loop (singlenodeconsolidation.go:54-84) over positions [first, last), `batch`
+// independent simulations per device call. With `after`, the actionable commands of each batch are validated together in
+// one more device call and the first valid one wins; the trace holds (position, verdict) of what the sequential loop
+// validates - the positions up to and including the winner. Without `after` every command is taken as valid.
+struct Sweep {
+  Cmd cmd;
+  int position = -1, sims = 0;
+  bool failed_validation = false;
+  std::vector<std::pair<int, int>> trace;
+};
+Sweep single_sweep(ClusterSession& cs, const Problem* after, int first, int last, int batch) {
+  Sweep s;
+  const int n = (int)cs.cands.size();
+  if (last < 0 || last > n) last = n;
+  if (batch < 1) batch = 1;
+  for (int b = std::max(first, 0); b < last; b += batch) {
+    std::vector<std::vector<int>> sets;
+    for (int i = b; i < std::min(last, b + batch); ++i) sets.push_back({i});
+    auto cmds = cs.compute_many(sets, false);
+    s.sims += (int)sets.size();
+    std::vector<int> hits;
+    for (size_t q = 0; q < cmds.size(); ++q) if (cmds[q].action == 1 || cmds[q].action == 2) hits.push_back((int)q);
+    if (hits.empty()) continue;
+    std::vector<char> ok(hits.size(), 1);
+    if (after) {
+      std::vector<VCmd> vc;
+      for (int q : hits) vc.push_back(cs.command({b + q}, cmds[(size_t)q].action, cmds[(size_t)q].options));
+      ok = cs.validate(after, vc);
+    }
+    for (size_t j = 0; j < hits.size(); ++j) {
+      if (after) s.trace.push_back({b + hits[j], ok[j] ? 1 : 0});
+      if (!ok[j]) { s.failed_validation = true; continue; }
+      s.cmd = cmds[(size_t)hits[j]];
+      s.position = b + hits[j];
+      return s;
+    }
+  }
+  return s;
+}
 }  // namespace
 
 extern "C" {
@@ -747,26 +1015,72 @@ int kh_consolidate_probe(const Problem* P, int count, int* options, int options_
 int kh_consolidate(const Problem* P, int* out4, int* options, int options_cap, int* probes, int* probe_actions, int probes_cap, int* n_probes) {
   try {
     ClusterSession cs(P);
-    int sims = 0;
-    out4[0] = out4[1] = out4[2] = out4[3] = 0;
-    *n_probes = 0;
-    if (cs.cands.size() < 2) return KSCHED_OK;
-    int mn = 1, mx = (int)cs.cands.size() - 1, last_count = 0;
-    Cmd last;
-    while (mn <= mx) {
-      int mid = (mn + mx) / 2;
-      Cmd c = cs.compute_prefix(mid + 1);
-      ++sims;
-      if (*n_probes < probes_cap) { probes[*n_probes] = mid + 1; probe_actions[*n_probes] = c.action; }
-      ++*n_probes;
-      if (c.action == 1 || c.action == 2) { last = c; last_count = mid + 1; mn = mid + 1; }
-      else mx = mid - 1;
+    const Search s = first_n_search(cs);
+    *n_probes = (int)s.probes.size();
+    for (int i = 0; i < *n_probes && i < probes_cap; ++i) { probes[i] = s.probes[(size_t)i]; probe_actions[i] = s.actions[(size_t)i]; }
+    out4[0] = s.cmd.action;
+    out4[1] = s.count;
+    out4[2] = s.sims;
+    out4[3] = (int)s.cmd.options.size();
+    for (size_t i = 0; i < s.cmd.options.size() && (int)i < options_cap; ++i) options[i] = s.cmd.options[i];
+    return KSCHED_OK;
+  } catch (const std::exception& e) {
+    return fail(error_code(e), e.what());
+  }
+}
+
+// MultiNodeConsolidation.ComputeCommand (multinodeconsolidation.go:41-70): the search on `before`, then Validation.IsValid of
+// its command against `after`, the cluster when the TTL ends. out4 and the probes as kh_consolidate; a command that fails
+// validation becomes retry (out4 = [3, 0, simulations, 0]). *verdict = 1 valid, 0 invalid, -1 nothing to validate.
+int kh_consolidate_validated(const Problem* before, const Problem* after, int* out4, int* options, int options_cap, int* probes, int* probe_actions,
+                             int probes_cap, int* n_probes, int* verdict) {
+  try {
+    ClusterSession cs(before);
+    const Search s = first_n_search(cs);
+    *n_probes = (int)s.probes.size();
+    for (int i = 0; i < *n_probes && i < probes_cap; ++i) { probes[i] = s.probes[(size_t)i]; probe_actions[i] = s.actions[(size_t)i]; }
+    Cmd cmd = s.cmd;
+    int removed = s.count;
+    *verdict = -1;
+    if (cmd.action == 1 || cmd.action == 2) {
+      std::vector<int> positions;
+      for (int i = 0; i < s.count; ++i) positions.push_back(i);
+      *verdict = cs.validate(after, {cs.command(positions, cmd.action, cmd.options)})[0] ? 1 : 0;
+      if (!*verdict) { cmd = Cmd(); cmd.action = 3; removed = 0; }
     }
-    out4[0] = last.action;
-    out4[1] = last_count;
-    out4[2] = sims;
-    out4[3] = (int)last.options.size();
-    for (size_t i = 0; i < last.options.size() && (int)i < options_cap; ++i) options[i] = last.options[i];
+    out4[0] = cmd.action;
+    out4[1] = removed;
+    out4[2] = s.sims;
+    out4[3] = (int)cmd.options.size();
+    for (size_t i = 0; i < cmd.options.size() && (int)i < options_cap; ++i) options[i] = cmd.options[i];
+    return KSCHED_OK;
+  } catch (const std::exception& e) {
+    return fail(error_code(e), e.what());
+  }
+}
+
+// Validation.IsValid (validation.go:63-172) of n_sets commands of an open session against `after`, the cluster when the TTL
+// ends: command q removes the candidates at positions sets[set_off[q] .. set_off[q+1]) of the session's disruption order,
+// actions[q] is 1 (delete) or 2 (replace) and its options are options[q * options_stride ...], n_options[q] of them - what
+// kh_cluster_probe_sets returns. valid[q] = 1 / 0. The session keeps the snapshot of `after` until it closes or is handed a
+// different problem (Problem::id): every validation of one ComputeCommand passes the same one (DESIGN.md §6 R7).
+int kh_cluster_validate(ClusterSession* cs, const Problem* after, const int* sets, const int* set_off, int n_sets, const int* actions, const int* options,
+                        int options_stride, const int* n_options, int* valid) {
+  try {
+    std::vector<VCmd> cmds;
+    if (n_sets < 0 || (n_sets > 0 && set_off[0] < 0)) return fail(KSCHED_ERR_INVALID, "n_sets / set_off out of range");
+    for (int q = 0; q < n_sets; ++q) {
+      if (set_off[q + 1] < set_off[q]) return fail(KSCHED_ERR_INVALID, "set_off must be non-decreasing");
+      if (actions[q] != 1 && actions[q] != 2) return fail(KSCHED_ERR_INVALID, "only delete (1) and replace (2) commands are validated");
+      if (n_options[q] < 0 || n_options[q] > options_stride) return fail(KSCHED_ERR_INVALID, "n_options out of range");
+      std::vector<int> positions(sets + set_off[q], sets + set_off[q + 1]);
+      for (int i : positions) if (i < 0 || i >= (int)cs->cands.size()) return fail(KSCHED_ERR_INVALID, "position out of range");
+      std::vector<int> opts(options + (size_t)q * options_stride, options + (size_t)q * options_stride + n_options[q]);
+      for (int t : opts) if (t < 0 || t >= (int)cs->P->instance_types.size()) return fail(KSCHED_ERR_INVALID, "instance type out of range");
+      cmds.push_back(cs->command(positions, actions[q], opts));
+    }
+    auto ok = cs->validate(after, cmds);
+    for (int q = 0; q < n_sets; ++q) valid[q] = ok[(size_t)q] ? 1 : 0;
     return KSCHED_OK;
   } catch (const std::exception& e) {
     return fail(error_code(e), e.what());
@@ -791,34 +1105,46 @@ int kh_nccl_init(const void* id128, int rank, int world) {
   return KSCHED_OK;
 }
 
-// SingleNodeConsolidation.ComputeCommand (singlenodeconsolidation.go:43-84): the candidates in disruption order, the first
-// whose computeConsolidation yields delete / replace wins (Validation is taken as valid: it re-runs the same simulation
-// after a TTL). The independent simulations go to the device `batch` at a time (ksched_simulate_batch).
-// out4: [action, position of the winning candidate in the disruption order or -1, simulations, n_options]; *node = its
-// Problem.nodes index. first / last bound the positions tried (a rank's share of the sweep); last < 0 = all.
+// SingleNodeConsolidation.ComputeCommand (singlenodeconsolidation.go:43-84) without validation: the candidates in disruption
+// order, the first whose computeConsolidation yields delete / replace wins. The independent simulations go to the device
+// `batch` at a time (ksched_simulate_batch). out4: [action, position of the winning candidate in the disruption order or -1,
+// simulations, n_options]; *node = its Problem.nodes index. first / last bound the positions tried (a rank's share of the
+// sweep); last < 0 = all.
 int kh_consolidate_single(const Problem* P, int first, int last, int batch, int* out4, int* node, int* options, int options_cap) {
   try {
     ClusterSession cs(P);
-    out4[0] = 0; out4[1] = -1; out4[2] = 0; out4[3] = 0;
-    *node = -1;
-    const int n = (int)cs.cands.size();
-    if (last < 0 || last > n) last = n;
-    if (batch < 1) batch = 1;
-    for (int b = std::max(first, 0); b < last; b += batch) {
-      std::vector<std::vector<int>> sets;
-      for (int i = b; i < std::min(last, b + batch); ++i) sets.push_back({i});
-      auto cmds = cs.compute_many(sets, false);
-      out4[2] += (int)sets.size();
-      for (size_t q = 0; q < cmds.size(); ++q)
-        if (cmds[q].action == 1 || cmds[q].action == 2) {
-          out4[0] = cmds[q].action;
-          out4[1] = b + (int)q;
-          out4[3] = (int)cmds[q].options.size();
-          *node = cs.cands[(size_t)(b + (int)q)].node;
-          for (size_t i = 0; i < cmds[q].options.size() && (int)i < options_cap; ++i) options[i] = cmds[q].options[i];
-          return KSCHED_OK;
-        }
-    }
+    const Sweep s = single_sweep(cs, nullptr, first, last, batch);
+    out4[0] = s.cmd.action;
+    out4[1] = s.position;
+    out4[2] = s.sims;
+    out4[3] = (int)s.cmd.options.size();
+    *node = s.position >= 0 ? cs.cands[(size_t)s.position].node : -1;
+    for (size_t i = 0; i < s.cmd.options.size() && (int)i < options_cap; ++i) options[i] = s.cmd.options[i];
+    return KSCHED_OK;
+  } catch (const std::exception& e) {
+    return fail(error_code(e), e.what());
+  }
+}
+
+// SingleNodeConsolidation.ComputeCommand with Validation against `after` (singlenodeconsolidation.go:52-84): the first
+// actionable command that validates wins; none, after a failed validation, is retry (action 3). out4, *node and options as
+// kh_consolidate_single. trace[i] / trace_valid[i] = the positions validated and their verdicts, in order, *n_trace of them;
+// *failed_validation = a validation failed before the winner (or anywhere, without one). Shares [first, last) of one sweep
+// merge as: the first share with a winner gives the command; with none, retry when any share failed a validation.
+int kh_consolidate_single_validated(const Problem* before, const Problem* after, int first, int last, int batch, int* out4, int* node, int* options,
+                                    int options_cap, int* trace, int* trace_valid, int trace_cap, int* n_trace, int* failed_validation) {
+  try {
+    ClusterSession cs(before);
+    const Sweep s = single_sweep(cs, after, first, last, batch);
+    out4[0] = s.position >= 0 ? s.cmd.action : s.failed_validation ? 3 : 0;
+    out4[1] = s.position;
+    out4[2] = s.sims;
+    out4[3] = (int)s.cmd.options.size();
+    *node = s.position >= 0 ? cs.cands[(size_t)s.position].node : -1;
+    for (size_t i = 0; i < s.cmd.options.size() && (int)i < options_cap; ++i) options[i] = s.cmd.options[i];
+    *n_trace = (int)s.trace.size();
+    for (int i = 0; i < *n_trace && i < trace_cap; ++i) { trace[i] = s.trace[(size_t)i].first; trace_valid[i] = s.trace[(size_t)i].second; }
+    *failed_validation = s.failed_validation ? 1 : 0;
     return KSCHED_OK;
   } catch (const std::exception& e) {
     return fail(error_code(e), e.what());

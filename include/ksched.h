@@ -34,7 +34,7 @@ extern "C" {
 #define KSCHED_ABI_VERSION 4
 #define KSCHED_MAX_KEYS 16
 #define KSCHED_MAX_RES 8
-#define KSCHED_MAX_TEMPLATES 16
+#define KSCHED_MAX_TEMPLATES 64 /* ksched_type_row.template_members is one bit per template */
 #define KSCHED_ROW_WORDS 32 /* canonical 256-byte rows (SURVEY.md 8d: B_pod = B_col = 256 B) */
 #define KSCHED_KEY_HOSTNAME 255
 #define KSCHED_NONE 0xFFFFFFFFu
@@ -85,6 +85,11 @@ typedef struct ksched_bounds {
  * classes): values that no requirement, label, threshold or topology domain of the problem names, and that appear only in
  * instance types' In requirements or existing nodes' labels, can be replaced by one representative per class (unnamed
  * integers of one region Ri, unnamed non-integers), kept as an ordinary dictionary value. The answers do not change.
+ * Likewise a key that only templates name (no pod, daemonset, topology term, node filter or bound pod's anti-affinity term
+ * names it; neither zone nor capacity-type) needs no mask key at all: its node requirement is always the template's own, so
+ * it only decides which instance types a template admits, and can be folded into ksched_type_row.template_members. The
+ * caller then renders the template's requirement on that key into each new node's requirements itself (DESIGN.md §3,
+ * template-only keys).
  */
 #define KSCHED_MAX_THRESHOLDS 7
 typedef struct ksched_key_regions {
@@ -124,7 +129,7 @@ typedef struct ksched_type_row {
   uint64_t values[KSCHED_MAX_KEYS];
   uint64_t meta;
   uint64_t offerings;        /* bit (ct*16 + zone): an AVAILABLE offering exists (node.go:151-159) */
-  uint64_t template_members; /* bit v: type is in template v's GetInstanceTypes list */
+  uint64_t template_members; /* bit v: type is in template v's GetInstanceTypes list (and meets its template-only keys) */
   double min_price;          /* cheapest available offering */
   uint32_t res_present;      /* resources present in Capacity */
   uint32_t input_index;      /* position in the caller's instance-type slice */

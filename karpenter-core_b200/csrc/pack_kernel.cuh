@@ -2967,7 +2967,7 @@ __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
   PodTopo& pt = g_pt;
   uint32_t* tmpl_taintset = g_tmpl_taintset;
   __shared__ WarpIO wio;
-  if (tid < c.n_templates) tmpl_taintset[tid] = c.templates[tid].taintset;
+  for (int v = tid; v < c.n_templates; v += blockDim.x) tmpl_taintset[v] = c.templates[v].taintset;
   if (tid == 0) { pt.n = 0; g_rc.cls = KSCHED_NONE; g_rc.eligible = 0; g_rc.vs_n = 0; }
 
   int head = 0, qlen = s.n_pods;

@@ -552,6 +552,60 @@ struct Group {
   }
 };
 
+// Requirement::Canonical() of the oracle: "<Operator()> [values in string order]", then the bounds (" >gt", " <lt")
+std::string render_canonical(bool complement, uint64_t values, const std::vector<std::string>& dict, const std::string& bounds) {
+  const char* op;
+  if (complement) op = values ? "NotIn" : "Exists";
+  else op = values ? "In" : "DoesNotExist";
+  std::string s = std::string(op) + " [";
+  bool first = true;
+  for (size_t b = 0; b < dict.size(); ++b)
+    if ((values >> b) & 1) { if (!first) s += " "; s += dict[b]; first = false; }
+  return s + "]" + bounds;
+}
+
+// One template-only key (DESIGN.md §3) in the host algebra of reqmask.cuh, on a dictionary of its own: the values that the
+// given requirement lists name, in string order. Intersects only ever meets values both sides name, so this is exact.
+struct FoldedKey {
+  std::map<std::string, int> id;
+  std::vector<std::string> values;
+  uint64_t int_mask = 0;
+  int64_t ints[64] = {};
+  explicit FoldedKey(std::initializer_list<const std::vector<NodeSelectorRequirement>*> lists) {
+    std::set<std::string> named;
+    for (auto* l : lists)
+      for (auto& r : *l)
+        if (r.op == Op::In || r.op == Op::NotIn) named.insert(r.values.begin(), r.values.end());
+    if (named.size() > 64) unsupported("a template-only label key whose requirements name more than 64 values");
+    for (auto& v : named) {
+      const int b = (int)values.size();
+      id[v] = b;
+      values.push_back(v);
+      if (parse_int(v, &ints[b])) int_mask |= 1ull << b;
+    }
+  }
+  KeyMeta meta() const { return KeyMeta{int_mask, ints, nullptr}; }
+  // NewRequirement (requirement.go:44-68) of every requirement, combined by Requirements.Add (requirements.go:87-94)
+  Req req(const std::vector<NodeSelectorRequirement>& rs) const {
+    Req cur = ksched::req_absent();
+    for (auto& r : rs) {
+      Req x{0, 0, 0, true, !(r.op == Op::In || r.op == Op::DoesNotExist), false, false};
+      if (r.op == Op::In || r.op == Op::NotIn)
+        for (auto& v : r.values) x.values |= 1ull << id.at(v);
+      if (r.op == Op::Gt) { x.has_gt = true; parse_int(r.values.at(0), &x.gt); }
+      if (r.op == Op::Lt) { x.has_lt = true; parse_int(r.values.at(0), &x.lt); }
+      cur = ksched::key_add(cur, x, meta());
+    }
+    return cur;
+  }
+  std::string render(const Req& r) const {
+    std::string bounds;
+    if (r.has_gt) bounds += " >" + std::to_string(r.gt);
+    if (r.has_lt) bounds += " <" + std::to_string(r.lt);
+    return render_canonical(r.complement, r.values, values, bounds);
+  }
+};
+
 }  // namespace
 
 std::map<std::string, std::string> value_classes(const std::set<std::string>& values, const std::set<std::string>& named,
@@ -614,7 +668,7 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
   // that visits every pod anyway
   bool uids_ascending = true;
   if (P.provisioners.empty()) throw std::runtime_error("no provisioners found");
-  if (P.provisioners.size() > KSCHED_MAX_TEMPLATES) unsupported("more than 16 provisioners");
+  if (P.provisioners.size() > KSCHED_MAX_TEMPLATES) unsupported("more than 64 provisioners");
 
   B.well_known = {kProvisionerName, kZone, "topology.kubernetes.io/region", kInstanceType, "kubernetes.io/arch", "kubernetes.io/os", kCapacityType};
   B.well_known.insert(P.extra_well_known_labels.begin(), P.extra_well_known_labels.end());
@@ -785,125 +839,160 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
   (void)type_keys;
   active.erase(kHostname);
   active.erase(kInstanceType);
-  if (active.size() > KSCHED_MAX_KEYS) unsupported("more than 16 active label keys");
-  for (auto& k : active) {
-    B.key_id[k] = (int)E.key_names.size();
-    E.key_names.push_back(k);
-  }
-  const int NK = (int)E.key_names.size();
-  std::vector<std::set<std::string>> vals(NK);
-  auto note_vals = [&](const std::vector<NodeSelectorRequirement>& rs) {
-    for (auto& r : rs) {
-      int k = B.key_of(r.key);
-      if (k < 0) continue;
-      if (r.op == Op::In || r.op == Op::NotIn) vals[k].insert(r.values.begin(), r.values.end());
+  // Template-only keys (DESIGN.md §3): no pod-side source names them, so a node's requirement on one is always its template's
+  // own and the key only decides which instance types the template admits. Zone and capacity-type stay mask keys: offerings,
+  // the launch choice and the price helpers read them.
+  std::set<std::string> foldable;
+  for (auto& k : active)
+    if (!pod_side.count(k) && k != kZone && k != kCapacityType) foldable.insert(k);
+  // The dictionary of a set of mask keys: key ids, values, thresholds and value classes.
+  std::vector<std::set<std::string>> vals;
+  std::vector<std::set<int64_t>> thr;
+  std::vector<bool> type_complement;
+  std::vector<std::map<std::string, std::string>> rep_of;  // unnamed value -> its class's representative
+  auto dictionary = [&](const std::set<std::string>& keys) {
+    B.key_id.clear();
+    E.key_names.clear();
+    for (auto& k : keys) {
+      B.key_id[k] = (int)E.key_names.size();
+      E.key_names.push_back(k);
     }
-  };
-  auto note_label_vals = [&](const Labels& l) {
-    for (auto& kv : l) { int k = B.key_of(kv.first); if (k >= 0) vals[k].insert(kv.second); }
-  };
-  auto note_pod_vals = [&](const Pod& p) {
-    note_label_vals(p.node_selector);
-    for (auto& t : p.required_node_terms) note_vals(t);
-    for (auto& t : p.preferred_node_terms) note_vals(t.preference);
-  };
-  for (auto& s : specs) note_pod_vals(s.pod);
-  for (auto& d : daemons) note_pod_vals(d);
-  for (auto& it : P.instance_types) note_vals(it.requirements);
-  // offerings name zones / capacity types too (a node without a requirement on the key admits all of them)
-  for (auto& it : P.instance_types)
-    for (auto& o : it.offerings) {
-      int kz = B.key_of(kZone), kc = B.key_of(kCapacityType);
-      if (kz >= 0) vals[kz].insert(o.zone);
-      if (kc >= 0) vals[kc].insert(o.capacity_type);
-    }
-  for (auto& pr : P.provisioners) {
-    note_vals(pr.requirements);
-    Labels l = pr.labels;
-    l[kProvisionerName] = pr.name;
-    note_label_vals(l);
-  }
-  for (auto& kv : facts.label_pairs) { int k = B.key_of(kv.first); if (k >= 0) vals[k].insert(kv.second); }  // every node's labels (ClusterFacts)
-  const int zone_key = B.key_of(kZone), ct_key = B.key_of(kCapacityType);
-  // Every threshold any requirement of this problem names, per key; a key also gets one region when an instance type has a
-  // complement requirement on it (region form below).
-  std::vector<std::set<int64_t>> thr(NK);
-  std::vector<bool> type_complement(NK, false);
-  {
-    auto note_thr = [&](const std::vector<NodeSelectorRequirement>& rs, bool is_type) {
+    const int NK = (int)E.key_names.size();
+    vals.assign(NK, {});
+    auto note_vals = [&](const std::vector<NodeSelectorRequirement>& rs) {
       for (auto& r : rs) {
         int k = B.key_of(r.key);
         if (k < 0) continue;
-        if (r.op == Op::Gt || r.op == Op::Lt) { int64_t v = 0; if (!r.values.empty()) parse_int(r.values[0], &v); thr[k].insert(v); }
-        if (is_type && r.op != Op::In && r.op != Op::DoesNotExist) type_complement[k] = true;
+        if (r.op == Op::In || r.op == Op::NotIn) vals[k].insert(r.values.begin(), r.values.end());
       }
     };
-    auto note_pod_thr = [&](const Pod& p) {
-      for (auto& t : p.required_node_terms) note_thr(t, false);
-      for (auto& t : p.preferred_node_terms) note_thr(t.preference, false);
+    auto note_label_vals = [&](const Labels& l) {
+      for (auto& kv : l) { int k = B.key_of(kv.first); if (k >= 0) vals[k].insert(kv.second); }
     };
-    for (auto& sp : specs) note_pod_thr(sp.pod);
-    for (auto& d : daemons) note_pod_thr(d);
-    for (auto& it : P.instance_types) note_thr(it.requirements, true);
-    for (auto& pr : P.provisioners) note_thr(pr.requirements, false);
-  }
-  // Value classes (DESIGN.md §3). A key whose values do not fit the word keeps the values some requirement of the problem
-  // names, and one representative per class of the others: instance types' In values and node labels that no requirement
-  // tells apart. Keys that fit are encoded as they always were.
-  phase("  keys + thresholds");
-  E.key_representatives.assign(NK, 0);
-  std::vector<std::map<std::string, std::string>> rep_of(NK);  // unnamed value -> its class's representative
-  {
-    std::vector<int> wide;
-    for (int k = 0; k < NK; ++k) {
-      const size_t nd = vals[k].size(), m = thr[k].size();
-      if (nd > 63 || ((m > 0 || type_complement[k]) && nd + m + 1 > 63)) wide.push_back(k);
+    auto note_pod_vals = [&](const Pod& p) {
+      note_label_vals(p.node_selector);
+      for (auto& t : p.required_node_terms) note_vals(t);
+      for (auto& t : p.preferred_node_terms) note_vals(t.preference);
+    };
+    for (auto& s : specs) note_pod_vals(s.pod);
+    for (auto& d : daemons) note_pod_vals(d);
+    for (auto& it : P.instance_types) note_vals(it.requirements);
+    // offerings name zones / capacity types too (a node without a requirement on the key admits all of them)
+    for (auto& it : P.instance_types)
+      for (auto& o : it.offerings) {
+        int kz = B.key_of(kZone), kc = B.key_of(kCapacityType);
+        if (kz >= 0) vals[kz].insert(o.zone);
+        if (kc >= 0) vals[kc].insert(o.capacity_type);
+      }
+    for (auto& pr : P.provisioners) {
+      note_vals(pr.requirements);
+      Labels l = pr.labels;
+      l[kProvisionerName] = pr.name;
+      note_label_vals(l);
     }
-    if (!wide.empty()) {
-      std::vector<std::set<std::string>> named(NK);
-      std::vector<bool> all_named(NK, false);
-      auto name_vals = [&](const std::vector<NodeSelectorRequirement>& rs, bool complement_only) {
+    for (auto& kv : facts.label_pairs) { int k = B.key_of(kv.first); if (k >= 0) vals[k].insert(kv.second); }  // every node's labels (ClusterFacts)
+    const int zone_key = B.key_of(kZone), ct_key = B.key_of(kCapacityType);
+    // Every threshold any requirement of this problem names, per key; a key also gets one region when an instance type has a
+    // complement requirement on it (region form below).
+    thr.assign(NK, {});
+    type_complement.assign(NK, false);
+    {
+      auto note_thr = [&](const std::vector<NodeSelectorRequirement>& rs, bool is_type) {
         for (auto& r : rs) {
           int k = B.key_of(r.key);
-          if (k < 0 || (complement_only && r.op == Op::In)) continue;
-          if (r.op == Op::In || r.op == Op::NotIn) named[k].insert(r.values.begin(), r.values.end());
+          if (k < 0) continue;
+          if (r.op == Op::Gt || r.op == Op::Lt) { int64_t v = 0; if (!r.values.empty()) parse_int(r.values[0], &v); thr[k].insert(v); }
+          if (is_type && r.op != Op::In && r.op != Op::DoesNotExist) type_complement[k] = true;
         }
       };
-      auto name_labels = [&](const Labels& l) { for (auto& kv : l) { int k = B.key_of(kv.first); if (k >= 0) named[k].insert(kv.second); } };
-      auto name_pod = [&](const Pod& p) {  // topology node filters are built from the same node selector and required terms
-        name_labels(p.node_selector);
-        for (auto& t : p.required_node_terms) name_vals(t, false);
-        for (auto& t : p.preferred_node_terms) name_vals(t.preference, false);
-        auto topo = [&](const std::string& key) { int k = B.key_of(key); if (k >= 0) all_named[k] = true; };
-        for (auto& t : p.topology_spread) topo(t.topology_key);
-        for (auto& t : p.pod_affinity_required) topo(t.topology_key);
-        for (auto& t : p.pod_affinity_preferred) topo(t.term.topology_key);
-        for (auto& t : p.pod_anti_affinity_required) topo(t.topology_key);
-        for (auto& t : p.pod_anti_affinity_preferred) topo(t.term.topology_key);
+      auto note_pod_thr = [&](const Pod& p) {
+        for (auto& t : p.required_node_terms) note_thr(t, false);
+        for (auto& t : p.preferred_node_terms) note_thr(t.preference, false);
       };
-      for (auto& s : specs) name_pod(s.pod);
-      for (auto& d : daemons) name_pod(d);
-      for (auto& kv : facts.named_pairs) { int k = B.key_of(kv.first); if (k >= 0) named[k].insert(kv.second); }  // bound pods
-      for (auto& key : facts.anti_keys) { int k = B.key_of(key); if (k >= 0) all_named[k] = true; }  // inverse anti-affinity groups
-      for (auto& pr : P.provisioners) {
-        name_vals(pr.requirements, false);
-        Labels l = pr.labels;
-        l[kProvisionerName] = pr.name;
-        name_labels(l);
+      for (auto& sp : specs) note_pod_thr(sp.pod);
+      for (auto& d : daemons) note_pod_thr(d);
+      for (auto& it : P.instance_types) note_thr(it.requirements, true);
+      for (auto& pr : P.provisioners) note_thr(pr.requirements, false);
+    }
+    // Value classes (DESIGN.md §3). A key whose values do not fit the word keeps the values some requirement of the problem
+    // names, and one representative per class of the others: instance types' In values and node labels that no requirement
+    // tells apart. Keys that fit are encoded as they always were.
+    phase("  keys + thresholds");
+    E.key_representatives.assign(NK, 0);
+    rep_of.assign(NK, {});
+    {
+      std::vector<int> wide;
+      for (int k = 0; k < NK; ++k) {
+        const size_t nd = vals[k].size(), m = thr[k].size();
+        if (nd > 63 || ((m > 0 || type_complement[k]) && nd + m + 1 > 63)) wide.push_back(k);
       }
-      for (auto& it : P.instance_types) name_vals(it.requirements, true);
-      if (zone_key >= 0) all_named[zone_key] = true;  // offering slots: they feed the launch choice
-      if (ct_key >= 0) all_named[ct_key] = true;
-      for (int k : wide) {
-        if (all_named[k]) continue;  // refused below when it does not fit
-        rep_of[k] = value_classes(vals[k], named[k], thr[k]);
-        for (auto& kv : rep_of[k]) {
-          if (kv.first != kv.second) vals[k].erase(kv.first);
-          else E.key_representatives[k]++;
+      if (!wide.empty()) {
+        std::vector<std::set<std::string>> named(NK);
+        std::vector<bool> all_named(NK, false);
+        auto name_vals = [&](const std::vector<NodeSelectorRequirement>& rs, bool complement_only) {
+          for (auto& r : rs) {
+            int k = B.key_of(r.key);
+            if (k < 0 || (complement_only && r.op == Op::In)) continue;
+            if (r.op == Op::In || r.op == Op::NotIn) named[k].insert(r.values.begin(), r.values.end());
+          }
+        };
+        auto name_labels = [&](const Labels& l) { for (auto& kv : l) { int k = B.key_of(kv.first); if (k >= 0) named[k].insert(kv.second); } };
+        auto name_pod = [&](const Pod& p) {  // topology node filters are built from the same node selector and required terms
+          name_labels(p.node_selector);
+          for (auto& t : p.required_node_terms) name_vals(t, false);
+          for (auto& t : p.preferred_node_terms) name_vals(t.preference, false);
+          auto topo = [&](const std::string& key) { int k = B.key_of(key); if (k >= 0) all_named[k] = true; };
+          for (auto& t : p.topology_spread) topo(t.topology_key);
+          for (auto& t : p.pod_affinity_required) topo(t.topology_key);
+          for (auto& t : p.pod_affinity_preferred) topo(t.term.topology_key);
+          for (auto& t : p.pod_anti_affinity_required) topo(t.topology_key);
+          for (auto& t : p.pod_anti_affinity_preferred) topo(t.term.topology_key);
+        };
+        for (auto& s : specs) name_pod(s.pod);
+        for (auto& d : daemons) name_pod(d);
+        for (auto& kv : facts.named_pairs) { int k = B.key_of(kv.first); if (k >= 0) named[k].insert(kv.second); }  // bound pods
+        for (auto& key : facts.anti_keys) { int k = B.key_of(key); if (k >= 0) all_named[k] = true; }  // inverse anti-affinity groups
+        for (auto& pr : P.provisioners) {
+          name_vals(pr.requirements, false);
+          Labels l = pr.labels;
+          l[kProvisionerName] = pr.name;
+          name_labels(l);
+        }
+        for (auto& it : P.instance_types) name_vals(it.requirements, true);
+        if (zone_key >= 0) all_named[zone_key] = true;  // offering slots: they feed the launch choice
+        if (ct_key >= 0) all_named[ct_key] = true;
+        for (int k : wide) {
+          if (all_named[k]) continue;  // refused below when it does not fit
+          rep_of[k] = value_classes(vals[k], named[k], thr[k]);
+          for (auto& kv : rep_of[k]) {
+            if (kv.first != kv.second) vals[k].erase(kv.first);
+            else E.key_representatives[k]++;
+          }
         }
       }
     }
+  };
+  // What the checks of the dictionary below accept: a key that fails them is refused.
+  auto fits = [&](int k) {
+    const size_t nd = vals[k].size(), m = thr[k].size();
+    return nd <= 63 && m <= KSCHED_MAX_THRESHOLDS && !((m > 0 || type_complement[k]) && nd + m + 1 > 63);
+  };
+  // Folding is conditional, so that every problem that fits the word keeps its encoding byte for byte: the template-only keys
+  // are folded only when the problem would be refused otherwise, for more than 16 keys or for a template-only key whose values
+  // do not fit (karpenter.sh/provisioner-name with 64 provisioners).
+  bool fold = active.size() > KSCHED_MAX_KEYS;
+  if (!fold) {
+    dictionary(active);
+    for (auto& k : foldable) fold = fold || !fits(B.key_id.at(k));
   }
+  if (fold) {
+    for (auto& k : foldable) active.erase(k);
+    if (active.size() > KSCHED_MAX_KEYS) unsupported("more than 16 active label keys");
+    E.folded_keys.assign(foldable.begin(), foldable.end());
+    dictionary(active);
+  }
+  const int NK = (int)E.key_names.size();
+  const int zone_key = B.key_of(kZone), ct_key = B.key_of(kCapacityType);
   phase("  value classes");
   B.value_id.resize(NK);
   E.key_values.resize(NK);
@@ -1089,6 +1178,41 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
     if (t.reqs.meta >> KSCHED_META_HASGT_SHIFT) E.any_template_bounds = true;
   }
   E.template_bounds = tb;
+  // Template-only keys (DESIGN.md §3): filterInstanceTypesByRequirements (node.go:137-145) keeps a type only when its
+  // requirements intersect the node's, and on such a key the node's requirement is always its template's
+  // (NewMachineTemplate: provisioner requirements, then labels, machinetemplate.go:46-62). Types that fail it on some folded
+  // key leave the template's list; the requirement itself is kept, rendered, for the new nodes' requirements.
+  if (!E.folded_keys.empty()) E.template_folded.assign(NV, {});
+  for (auto& key : E.folded_keys) {
+    auto on_key = [&](const std::vector<NodeSelectorRequirement>& rs) {
+      std::vector<NodeSelectorRequirement> out;
+      for (auto& r : rs) if (normalize_key(r.key) == key) out.push_back(r);
+      return out;
+    };
+    std::map<std::string, std::pair<std::vector<NodeSelectorRequirement>, std::vector<int>>> type_groups;  // by requirements on the key
+    for (int c = 0; c < NT; ++c) {
+      auto rs = on_key(P.instance_types[E.type_input_index[c]].requirements);
+      if (rs.empty()) continue;  // Intersects skips a key the type does not define
+      auto& g = type_groups[reqs_key(rs)];
+      g.first = std::move(rs);
+      g.second.push_back(c);
+    }
+    for (int v = 0; v < NV; ++v) {
+      const Provisioner& pr = P.provisioners[E.template_provisioner[v]];
+      Labels l = pr.labels;
+      l[kProvisionerName] = pr.name;
+      std::vector<NodeSelectorRequirement> tmpl = on_key(pr.requirements);
+      for (auto& r : on_key(Builder::label_reqs(l))) tmpl.push_back(r);
+      if (tmpl.empty()) continue;
+      const FoldedKey own({&tmpl});
+      E.template_folded[v][key] = own.render(own.req(tmpl));
+      for (auto& g : type_groups) {
+        const FoldedKey d({&tmpl, &g.second.first});
+        if (ksched::key_intersects(d.req(g.second.first), d.req(tmpl), d.meta())) continue;
+        for (int c : g.second.second) E.types[c].template_members &= ~(1ull << v);
+      }
+    }
+  }
 
   phase("templates");
   // ------------------------------------------------------------------ daemonset overhead (scheduler.go:250-267)
@@ -1697,14 +1821,7 @@ std::string render_requirement(const Encoded& E, const ksched_reqset& rs, int k)
     if (low > 0) bounds += " >" + std::to_string(g.thresholds[low - 1]);
     if (high > 0) bounds += " <" + std::to_string(g.thresholds[g.n_thresholds - high]);
   }
-  const char* op;
-  if (r.complement) op = r.values ? "NotIn" : "Exists";
-  else op = r.values ? "In" : "DoesNotExist";
-  std::string s = std::string(op) + " [";
-  bool first = true;
-  for (size_t b = 0; b < E.key_values[k].size(); ++b)
-    if ((r.values >> b) & 1) { if (!first) s += " "; s += E.key_values[k][b]; first = false; }
-  return s + "]" + bounds;
+  return render_canonical(r.complement, r.values, E.key_values[k], bounds);
 }
 
 }  // namespace khost

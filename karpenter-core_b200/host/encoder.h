@@ -39,6 +39,9 @@ struct Encoded {
   std::vector<std::vector<std::string>> key_values;   // per key, ascending string order (canonical domain order)
   std::vector<int32_t> key_representatives;           // per key: dictionary values that stand for a class of unnamed values
                                                       // (value_classes below), 0 = every value of the key is its own
+  std::vector<std::string> folded_keys;               // template-only keys folded into template_members (DESIGN.md §3), ascending
+  std::vector<std::map<std::string, std::string>> template_folded;  // per template (empty when nothing is folded): folded key ->
+                                                      // the template's requirement on it, rendered as render_requirement does
   std::vector<std::string> res_names;                 // resource ids: cpu, memory, pods, then ascending
   // ---- which objects take part (provisioner.go:119-144 / deprovisioning/helpers.go:42-93)
   std::vector<const kmodel::Pod*> pods;               // Solve's pod list

@@ -183,6 +183,8 @@ void decode(const Encoded& E, const ResultBuffers& B, Result& out) {
           if (it == rendered[k].end()) it = rendered[k].emplace(memo_key, khost::render_requirement(E, src.reqs, (int)k)).first;
           dst.requirements[E.key_names[k]] = it->second;
         }
+      if ((size_t)src.template_index < E.template_folded.size())  // template-only keys: the template's own requirement
+        for (auto& kv : E.template_folded[(size_t)src.template_index]) dst.requirements[kv.first] = kv.second;
       // launch choice: column -> the provider's instance type, offering by its position in that type's Offerings list
       if (n < B.launch.size() && B.launch[n].type_column >= 0 && E.problem_ref) {
         const ksched_launch_choice& lc = B.launch[n];
@@ -1285,6 +1287,10 @@ extern "C" unsigned long long kh_encoded_digest(const Encoded* E) {
   vec(E->pod_class); vec(E->pod_timestamp); vec(E->pod_uid_rank); vec(E->existing); vec(E->groups); vec(E->group_domain_counts);
   vec(E->group_existing_counts); vec(E->class_topo); vec(E->filter_terms); vec(E->itype_req_sets); vec(E->itype_req_complement); vec(E->hostname_reqs);
   if (!E->class_volumes.empty()) { vec(E->class_volumes); vec(E->existing_volumes); bytes(E->volume_driver_mask, sizeof E->volume_driver_mask); }
+  if (!E->folded_keys.empty()) {  // absent when nothing is folded: those digests predate template-only keys
+    for (auto& k : E->folded_keys) str(k);
+    for (auto& m : E->template_folded) { size_t n = m.size(); bytes(&n, sizeof n); for (auto& kv : m) { str(kv.first); str(kv.second); } }
+  }
   const ksched_catalog& c = E->catalog;
   int cat[4] = {c.n_keys, c.n_res, c.n_types, c.n_templates};
   bytes(cat, sizeof cat);

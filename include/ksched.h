@@ -112,7 +112,7 @@ typedef struct ksched_pod_row {
   int64_t requests[KSCHED_MAX_RES]; /* includes pods: 1000 */
   uint64_t values[KSCHED_MAX_KEYS]; /* NewPodRequirements on the mask keys */
   uint64_t meta;
-  uint64_t tolerated_taintsets; /* bit s: pod tolerates every taint of taint set s */
+  uint64_t tolerated_taintsets; /* bit s: pod tolerates every taint of taint set s (s < 64; see problem.class_tolerated_ext) */
   uint64_t hostport_conflicts;  /* host-port entries this pod's ports clash with (hostportusage.go:45-57) */
   uint64_t hostport_entries;    /* host-port entries this pod reserves */
   uint32_t res_present;         /* bit r: resource r is a key of the pod's request map */
@@ -140,7 +140,7 @@ typedef struct ksched_template {
   ksched_reqset reqs;               /* NewMachineTemplate requirements (machinetemplate.go:46-62) */
   int64_t daemon_requests[KSCHED_MAX_RES]; /* getDaemonOverhead (scheduler.go:250-267); includes pods */
   uint32_t daemon_res_present;
-  uint32_t taintset;                /* index of this template's taint set */
+  uint32_t taintset;                /* index of this template's taint set, < 64 */
   int32_t has_limits;               /* provisioner.Spec.Limits != nil */
   uint32_t limit_present;           /* resources that are keys of the limits map */
   int64_t remaining[KSCHED_MAX_RES]; /* remainingResources after calculateExistingMachines */
@@ -258,6 +258,13 @@ typedef struct ksched_problem {
   const ksched_class_volumes* class_volumes;   /* [n_classes] */
   const ksched_node_volumes* existing_volumes; /* [n_existing] */
   uint64_t volume_driver_mask[KSCHED_MAX_VOLUME_DRIVERS]; /* tracked claim ids by driver */
+  /* Taint sets beyond the 64 of ksched_pod_row.tolerated_taintsets. Templates and existing nodes share one id space of taint
+     sets; template sets must have ids below 64 (ksched_load_catalog refuses others), so only existing nodes may carry an id
+     s >= 64. Bit (s - 64) % 64 of word [class][(s - 64) / 64] says that the class tolerates every taint of set s.
+     NULL (0 words) when every set id is below 64; ksched_upload refuses an existing node whose id the table does not cover. */
+  const uint64_t* class_tolerated_ext; /* [n_classes][n_tolerated_ext_words] */
+  int32_t n_tolerated_ext_words;
+  int32_t pad_ext;
 } ksched_problem;
 
 typedef struct ksched_new_node {

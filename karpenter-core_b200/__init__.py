@@ -570,9 +570,10 @@ class ResidentSolve:
         if not self.enc:
             msg = lib().kh_scheduler_error().decode()
             raise KschedError(KSCHED_ERR_UNSUPPORTED if msg.startswith("unsupported:") else KSCHED_ERR_INVALID, msg)
-        d = (C.c_longlong * 10)()
+        d = (C.c_longlong * 11)()
         lib().kh_encoded_dims(self.enc, d)
-        self.dims = dict(zip(["pods", "classes", "existing", "groups", "types", "templates", "keys", "resources", "type_words", "class_topo"], list(d)))
+        self.dims = dict(zip(["pods", "classes", "existing", "groups", "types", "templates", "keys", "resources", "type_words", "class_topo",
+                              "taintsets"], list(d)))
 
     def key_info(self, key):
         """dictionary of one mask key: {values, representatives (of unnamed value classes, 0 = none), thresholds}, or None

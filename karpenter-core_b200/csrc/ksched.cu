@@ -160,6 +160,8 @@ struct ksched_handle {
   DevBuf<ksched_key_regions> d_key_regions;
   DevBuf<ksched_class_volumes> d_cls_vol;
   DevBuf<int32_t> d_cls_cursor;
+  DevBuf<uint64_t> d_cls_tol_ext;  // [n_classes][tol_ext_words] taint sets from id 64 on (ksched_problem.class_tolerated_ext)
+  int tol_ext_words = 0;
   // device-resident cluster snapshot (ksched_load_cluster)
   bool have_cluster = false;
   int stop_new_nodes = 0;
@@ -317,8 +319,10 @@ int ksched_load_catalog(ksched_handle* h, const ksched_catalog* cat) {
       cat->n_types < 0) { h->err = "catalog dimensions out of range"; return KSCHED_ERR_INVALID; }
   // Gt/Lt cross the ABI in region form (ksched_key_regions): a requirement set that still carries gt / lt is a caller bug
   if (cat->type_bounds || cat->template_bounds) { h->err = "bounds arrays must be NULL: Gt/Lt requirements are passed in region form (ksched_key_regions)"; return KSCHED_ERR_INVALID; }
-  for (int v = 0; v < cat->n_templates; ++v)
+  for (int v = 0; v < cat->n_templates; ++v) {
     if (cat->templates[v].reqs.meta >> KSCHED_META_HASGT_SHIFT) { h->err = "template requirement with HASGT/HASLT set: pass Gt/Lt in region form"; return KSCHED_ERR_INVALID; }
+    if (cat->templates[v].taintset >= 64) { h->err = "template taint set id beyond 63: ids from 64 on belong to existing nodes only"; return KSCHED_ERR_INVALID; }
+  }
   for (int t = 0; t < cat->n_types; ++t)
     if (cat->types[t].meta >> KSCHED_META_HASGT_SHIFT) { h->err = "instance-type requirement with HASGT/HASLT set: pass Gt/Lt in region form"; return KSCHED_ERR_INVALID; }
   if (cat->key_regions)
@@ -625,6 +629,16 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
     if (pb->existing[i].reqs.meta >> KSCHED_META_HASGT_SHIFT) { h->err = "requirement with HASGT/HASLT set: pass Gt/Lt in region form"; return KSCHED_ERR_INVALID; }
   for (int i = 0; i < pb->n_filter_terms; ++i)
     if (pb->filter_terms[i].meta >> KSCHED_META_HASGT_SHIFT) { h->err = "requirement with HASGT/HASLT set: pass Gt/Lt in region form"; return KSCHED_ERR_INVALID; }
+  {
+    // taint sets from id 64 on: existing nodes only, each covered by the per-class table
+    const int tol_words = pb->class_tolerated_ext ? pb->n_tolerated_ext_words : 0;
+    if (tol_words < 0) { h->err = "n_tolerated_ext_words out of range"; return KSCHED_ERR_INVALID; }
+    for (int i = 0; i < pb->n_existing; ++i)
+      if (pb->existing[i].taintset >= 64 && (pb->existing[i].taintset - 64) / 64 >= (uint32_t)tol_words) {
+        h->err = "existing node with a taint set id from 64 on that class_tolerated_ext does not cover";
+        return KSCHED_ERR_INVALID;
+      }
+  }
   CUDA_TRY(h, cudaSetDevice(h->device));
   // the superset buffers ksched_load_cluster filled are about to be overwritten: simulations need a new ksched_load_cluster
   h->have_cluster = false;
@@ -656,6 +670,8 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
     h->min_req[r] = (NC == 0 || mn == INT64_MAX || mn < 0) ? 0 : mn;
   }
   CUDA_TRY(h, upload(h, h->d_classes, pb->classes, (size_t)NC));
+  h->tol_ext_words = pb->class_tolerated_ext ? pb->n_tolerated_ext_words : 0;
+  if (h->tol_ext_words > 0) CUDA_TRY(h, upload(h, h->d_cls_tol_ext, pb->class_tolerated_ext, (size_t)NC * h->tol_ext_words));
   {
     // queue.go:82-108 orders by cpu desc, memory desc, timestamp asc, UID asc. (cpu, memory) is a property of the class: rank
     // the classes once here, and the whole order is one packed key when rank, timestamp span and UID rank fit 64 bits.
@@ -1048,6 +1064,7 @@ static int run_pack(ksched_handle* h) {
   s.ex_vals = h->d_ex_vals.ptr; s.ex_meta = h->d_ex_meta.ptr; s.ex_taintset = h->d_ex_taintset.ptr; s.ex_itype = h->d_ex_itype.ptr;
   s.ex_hp = h->d_ex_hp.ptr; s.ex_closed = h->d_ex_closed.ptr;
   s.cls_cursor = h->d_cls_cursor.ptr;
+  s.cls_tol_ext = h->tol_ext_words > 0 ? h->d_cls_tol_ext.ptr : nullptr; s.tol_ext_words = h->tol_ext_words;
   s.cls_vol = h->have_volumes ? h->d_cls_vol.ptr : nullptr; s.ex_vol = h->have_volumes ? h->d_ex_vol.ptr : nullptr;
   for (int d = 0; d < KSCHED_MAX_VOLUME_DRIVERS; ++d) s.vol_mask[d] = h->vol_mask[d];
   s.nn_tmpl = h->d_nn_tmpl.ptr; s.nn_count = h->d_nn_count.ptr; s.nn_tb = h->d_nn_tb.ptr; s.nn_req = h->d_nn_req.ptr;

@@ -414,6 +414,12 @@ __device__ __forceinline__ bool class_has_volumes(const PackState& s, unsigned c
   const ksched_class_volumes v = s.cls_vol[cls];
   return (v.shared | v.priv[0] | v.priv[1] | v.priv[2] | v.priv[3]) != 0;
 }
+// Taints.Tolerates (taints.go:28-40) of an existing node's taint set. Ids below 64 are bits of the row's word; ids from 64 on
+// only existing nodes carry (ksched.h: class_tolerated_ext), and they live in the per-class table.
+__device__ __forceinline__ bool tolerates_node_set(const PackState& s, uint64_t tol, unsigned cls, uint32_t ts) {
+  const uint64_t w = ts < 64 ? tol : s.cls_tol_ext[(size_t)cls * s.tol_ext_words + ((ts - 64) >> 6)];
+  return (w >> (ts & 63)) & 1;
+}
 struct ExRunIO { int qi, head, qlen, seq, parity, placed; long long add_calls; };
 __shared__ ExRunIO g_xio;
 // one partial sum per warp, double-buffered: every warp of the largest block the kernel is launched with needs a slot
@@ -454,7 +460,7 @@ __device__ __noinline__ void existing_run(const PodRegs& first) {
   while (placed < m && e0 < NE) {
     const int e = e0 + tid;
     int k = 0;
-    if (e < NE && !s.ex_closed[e] && ((first.tol >> s.ex_taintset[e]) & 1)) {
+    if (e < NE && !s.ex_closed[e] && tolerates_node_set(s, first.tol, cls, s.ex_taintset[e])) {
       long long K = m - placed;
       const uint32_t qp = s.ex_req_present[e] | first.res, ap = s.ex_avail_present[e];
       for (int r = 0; r < R && K > 0; ++r) {
@@ -593,7 +599,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
       t.n = 0;
       for (int e = start + tid; e < NE; e += blockDim.x) {
         if (s.ex_closed[e]) continue;
-        if (!((p_tol >> s.ex_taintset[e]) & 1)) continue;
+        if (!tolerates_node_set(s, p_tol, cls, s.ex_taintset[e])) continue;
         if (p_hpc && (s.ex_hp[e] & p_hpc)) continue;
         if (has_vol) {  // volumeUsage.Validate(pod).Exceeds(volumeLimits) existingnode.go:88-96
           const ksched_node_volumes nv = s.ex_vol[e];

@@ -124,6 +124,9 @@ struct PackState {
   int64_t* remaining;                // [V][8] provisioner limits
   // outputs / counters: [0]=n_new [1]=n_unscheduled [2]=nodes_visited [3]=add_calls [4]=error [5]=steps
   long long* counters;
+  // taint sets from id 64 on, existing nodes only (ksched.h: class_tolerated_ext)
+  const uint64_t* cls_tol_ext;       // [n_classes][tol_ext_words], or nullptr
+  int tol_ext_words;
 };
 
 struct K2Params {

@@ -482,8 +482,7 @@ struct Builder {
     std::string k = taints_key(ts);
     auto it = taintset_id.find(k);
     if (it != taintset_id.end()) return it->second;
-    int id = (int)taintsets.size();
-    if (id >= 64) unsupported("more than 64 distinct taint sets");
+    int id = (int)taintsets.size();  // ids from 64 on only ever go to existing nodes' sets (class_tolerated_ext, ksched.h)
     taintset_id[k] = id;
     taintsets.push_back(ts);
     return id;
@@ -1173,6 +1172,8 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
       if (allowed[c]) E.types[c].template_members |= 1ull << v;
     }
     t.taintset = (uint32_t)B.taintset(pr.taints);
+    // at most KSCHED_MAX_TEMPLATES templates, encoded before any existing node: the template side reads only the 64-bit word
+    if (t.taintset >= 64) throw std::runtime_error("internal: template taint set id beyond 63");
     t.has_limits = pr.has_limits ? 1 : 0;
     t.limit_present = B.fill_resources(pr.limits, t.remaining);
     if (t.reqs.meta >> KSCHED_META_HASGT_SHIFT) E.any_template_bounds = true;
@@ -1728,14 +1729,22 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
       E.volume_driver_mask[d] |= 1ull << kv.second;
     }
   }
-  // host-port conflict masks and tolerated taint sets need the complete entry / taint-set tables
+  // host-port conflict masks and tolerated taint sets need the complete entry / taint-set tables. Sets from id 64 on are
+  // existing nodes' only; their bits go to a table of their own, so problems with at most 64 sets encode as before.
+  const size_t NS = B.taintsets.size();
+  E.n_taintsets = (int)NS;
+  E.tolerated_ext_words = NS > 64 ? (int)((NS - 64 + 63) / 64) : 0;
+  E.class_tolerated_ext.assign((size_t)NC * E.tolerated_ext_words, 0);
   for (int c = 0; c < NC; ++c) {
     const Pod& p = specs[c].pod;
     for (auto& hp : host_ports(p))
       for (size_t e = 0; e < B.hp_entries.size(); ++e)
         if (hp_matches(hp, B.hp_entries[e])) E.classes[c].hostport_conflicts |= 1ull << e;
-    for (size_t s = 0; s < B.taintsets.size(); ++s)
-      if (tolerates_all(B.taintsets[s], p.tolerations)) E.classes[c].tolerated_taintsets |= 1ull << s;
+    for (size_t s = 0; s < NS; ++s) {
+      if (!tolerates_all(B.taintsets[s], p.tolerations)) continue;
+      if (s < 64) E.classes[c].tolerated_taintsets |= 1ull << s;
+      else E.class_tolerated_ext[(size_t)c * E.tolerated_ext_words + (s - 64) / 64] |= 1ull << ((s - 64) % 64);
+    }
   }
 
   phase("class rows");
@@ -1792,6 +1801,8 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
     pr.existing_volumes = E.existing_volumes.data();
     for (int d = 0; d < KSCHED_MAX_VOLUME_DRIVERS; ++d) pr.volume_driver_mask[d] = E.volume_driver_mask[d];
   }
+  pr.class_tolerated_ext = E.class_tolerated_ext.empty() ? nullptr : E.class_tolerated_ext.data();
+  pr.n_tolerated_ext_words = E.tolerated_ext_words;
   pr.count_nodes_visited = 0;  // the exact nodes_visited statistic is opt-in (kh_set_count_visited / tests): it turns the pack kernel's steady-state paths off
   // Gt/Lt leave the host algebra here: templates and pod classes in region form (types and filter terms already are)
   for (int v = 0; v < NV; ++v) B.to_region_form(E.templates[v].reqs, tb[v]);

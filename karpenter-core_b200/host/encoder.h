@@ -89,6 +89,9 @@ struct Encoded {
   std::vector<ksched_class_volumes> class_volumes;    // CSI volume limits (ksched.h); empty when no pod mounts a limited claim
   std::vector<ksched_node_volumes> existing_volumes;
   uint64_t volume_driver_mask[KSCHED_MAX_VOLUME_DRIVERS] = {};
+  int n_taintsets = 0;                                // distinct taint sets of templates and existing nodes
+  std::vector<uint64_t> class_tolerated_ext;          // [n_classes][tolerated_ext_words] sets from id 64 on (ksched.h); empty with <= 64 sets
+  int tolerated_ext_words = 0;
 
   ksched_catalog catalog{};
   ksched_problem problem{};

@@ -339,12 +339,12 @@ void kh_encoded_free(Encoded* E) {
   if (E == g_gpu_encoded) { g_gpu_encoded = nullptr; g_gpu_current = false; }
   delete E;
 }
-// dims: [pods, classes, existing, groups, types, templates, keys, resources, type_words, class_topo]
+// dims: [pods, classes, existing, groups, types, templates, keys, resources, type_words, class_topo, taintsets]
 void kh_encoded_dims(const Encoded* E, long long* out) {
   out[0] = (long long)E->pods.size(); out[1] = (long long)E->classes.size(); out[2] = (long long)E->existing.size();
   out[3] = (long long)E->groups.size(); out[4] = (long long)E->types.size(); out[5] = (long long)E->templates.size();
   out[6] = (long long)E->key_names.size(); out[7] = (long long)E->res_names.size(); out[8] = E->type_words;
-  out[9] = (long long)E->class_topo.size();
+  out[9] = (long long)E->class_topo.size(); out[10] = E->n_taintsets;
 }
 void kh_encoded_set_count_visited(Encoded* E, int on) { E->problem.count_nodes_visited = on; }
 const ksched_catalog* kh_encoded_catalog(const Encoded* E) { return &E->catalog; }
@@ -1287,6 +1287,7 @@ extern "C" unsigned long long kh_encoded_digest(const Encoded* E) {
   vec(E->pod_class); vec(E->pod_timestamp); vec(E->pod_uid_rank); vec(E->existing); vec(E->groups); vec(E->group_domain_counts);
   vec(E->group_existing_counts); vec(E->class_topo); vec(E->filter_terms); vec(E->itype_req_sets); vec(E->itype_req_complement); vec(E->hostname_reqs);
   if (!E->class_volumes.empty()) { vec(E->class_volumes); vec(E->existing_volumes); bytes(E->volume_driver_mask, sizeof E->volume_driver_mask); }
+  if (!E->class_tolerated_ext.empty()) vec(E->class_tolerated_ext);  // absent with at most 64 taint sets: those digests predate it
   if (!E->folded_keys.empty()) {  // absent when nothing is folded: those digests predate template-only keys
     for (auto& k : E->folded_keys) str(k);
     for (auto& m : E->template_folded) { size_t n = m.size(); bytes(&n, sizeof n); for (auto& kv : m) { str(kv.first); str(kv.second); } }

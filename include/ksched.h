@@ -32,6 +32,7 @@ extern "C" {
 #endif
 
 #define KSCHED_ABI_VERSION 4
+#define KSCHED_MAX_RES_EXT 24 /* resources beyond the KSCHED_MAX_RES row slots (ksched_catalog.n_res_ext) */
 #define KSCHED_MAX_KEYS 16
 #define KSCHED_MAX_RES 8
 #define KSCHED_MAX_TEMPLATES 64 /* ksched_type_row.template_members is one bit per template */
@@ -171,6 +172,12 @@ typedef struct ksched_catalog {
      (rank of the offering's price among all distinct prices of the catalog) << 16 | position in the type's Offerings
      list << 8 | slot, for AVAILABLE offerings; ~0 elsewhere. NULL: ksched_result.launch is not filled. */
   const uint64_t* offering_keys;
+  /* Ext resources: resources from the 9th on (at most KSCHED_MAX_RES_EXT). n_res keeps its meaning (the <= 8 row slots), so
+     no reader of the rows indexes past them. Only pod classes request ext resources: no daemonset, provisioner limit or
+     existing node's remaining daemon overhead names one (the caller assigns the slots so). 0 / NULL: none. */
+  int32_t n_res_ext;
+  int32_t pad_ext;
+  const int64_t* type_alloc_ext;   /* [n_types][n_res_ext] allocatable of ext resource x (0 where the type lacks it) */
 } ksched_catalog;
 
 /* Existing (real / in-flight) node: NewExistingNode, existingnode.go:41-75. */
@@ -265,6 +272,11 @@ typedef struct ksched_problem {
   const uint64_t* class_tolerated_ext; /* [n_classes][n_tolerated_ext_words] */
   int32_t n_tolerated_ext_words;
   int32_t pad_ext;
+  /* Ext resources (ksched_catalog.n_res_ext). They are not bits of ksched_pod_row.res_present: code that walks that mask
+     indexes the 8 row slots. All three NULL when n_res_ext is 0. */
+  const int64_t* class_requests_ext;      /* [n_classes][n_res_ext] request (ceiling over init containers) */
+  const uint32_t* class_res_ext_present;  /* [n_classes] bit x: ext resource x is a key of the class's request map */
+  const int64_t* existing_available_ext;  /* [n_existing][n_res_ext] state.Node.Available() (0 where the node lacks it) */
 } ksched_problem;
 
 typedef struct ksched_new_node {
@@ -299,6 +311,10 @@ typedef struct ksched_result {
   int64_t nodes_visited; /* candidate nodes examined, reference scan order (SURVEY.md 8d K2 bytes) */
   int64_t add_calls;     /* queue pops = Scheduler.add calls */
   ksched_launch_choice* launch; /* [max_new_nodes] or NULL (needs ksched_catalog.offering_keys) */
+  /* Ext resources of the new nodes (ksched_catalog.n_res_ext), or NULL: [max_new_nodes][n_res_ext] requests and
+     [max_new_nodes] presence masks (bit x: ext resource x is a key of the node's request map). */
+  int64_t* new_node_requests_ext;
+  uint32_t* new_node_requests_ext_present;
 } ksched_result;
 
 /*

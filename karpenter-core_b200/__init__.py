@@ -123,6 +123,7 @@ def lib():
     L.kh_encoded_free.argtypes = [C.c_void_p]
     L.kh_encoded_dims.argtypes = [C.c_void_p, C.POINTER(C.c_longlong)]
     L.kh_encoded_key_info.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(C.c_longlong)]
+    L.kh_encoded_resource_id.argtypes = [C.c_void_p, C.c_char_p]
     L.kh_value_class_selftest.argtypes = [C.c_uint, C.c_int]
     L.kh_gpu_load.argtypes = [C.c_void_p]
     L.kh_encoded_set_count_visited.argtypes = [C.c_void_p, C.c_int]
@@ -570,10 +571,10 @@ class ResidentSolve:
         if not self.enc:
             msg = lib().kh_scheduler_error().decode()
             raise KschedError(KSCHED_ERR_UNSUPPORTED if msg.startswith("unsupported:") else KSCHED_ERR_INVALID, msg)
-        d = (C.c_longlong * 11)()
+        d = (C.c_longlong * 12)()
         lib().kh_encoded_dims(self.enc, d)
         self.dims = dict(zip(["pods", "classes", "existing", "groups", "types", "templates", "keys", "resources", "type_words", "class_topo",
-                              "taintsets"], list(d)))
+                              "taintsets", "resources_ext"], list(d)))
 
     def key_info(self, key):
         """dictionary of one mask key: {values, representatives (of unnamed value classes, 0 = none), thresholds}, or None
@@ -582,6 +583,10 @@ class ResidentSolve:
         if lib().kh_encoded_key_info(self.enc, key.encode(), out) != 0:
             return None
         return dict(zip(["values", "representatives", "thresholds"], list(out)))
+
+    def resource_id(self, name):
+        """id of a resource in this encoding: a row slot below 8, an ext resource from 8 on; -1 when it is not carried"""
+        return lib().kh_encoded_resource_id(self.enc, name.encode())
 
     def set_count_visited(self, on):
         """exact nodes_visited statistic on/off (off for timed runs: it costs a pass over all in-flight nodes per pod)"""

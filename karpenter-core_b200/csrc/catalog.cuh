@@ -37,7 +37,26 @@ struct DevCatalog {
   uint64_t pin_neutral[KSCHED_MAX_KEYS];
   const uint64_t* offer_keys;        // [n_types][64] launch-choice keys (ksched_catalog.offering_keys) or nullptr
   const uint32_t* input_index;       // [n_types] provider input order of the column
+  int n_res_ext;                     // ext resources (ksched.h: ksched_catalog.n_res_ext), 0 = none
+  const int64_t* alloc_ext;          // [n_types][n_res_ext] or nullptr
 };
+
+// Fits (resources.go:138-145) on the ext resources: the types of column word w of `word` whose allocatable holds
+// node[x] + pod[x] for every ext resource x of `present` (node: the node's ext sums, nullptr for a fresh node; an allocatable
+// the type lacks counts as 0). Only classes that request an ext resource call it, so a per-type loop is enough; out of line,
+// so that the pack kernel's paths for other classes keep their code size.
+__device__ __noinline__ uint32_t ext_fit_word(const DevCatalog& c, const int64_t* node, const int64_t* pod, uint32_t present, uint32_t word, int w) {
+  uint32_t out = word;
+  for (uint32_t m = word; m; m &= m - 1) {
+    const int b = __ffs(m) - 1;
+    const int64_t* a = c.alloc_ext + (size_t)(w * 32 + b) * c.n_res_ext;
+    for (uint32_t p = present; p; p &= p - 1) {
+      const int x = __ffs(p) - 1;
+      if ((node ? node[x] : 0) + pod[x] > a[x]) { out &= ~(1u << b); break; }
+    }
+  }
+  return out;
+}
 
 __device__ __forceinline__ KeyMeta key_meta(const DevCatalog& c, int k) {
   return KeyMeta{c.keys[k].int_mask, c.key_int_values ? c.key_int_values + (size_t)k * 64 : nullptr, c.key_regions ? c.key_regions + k : nullptr};

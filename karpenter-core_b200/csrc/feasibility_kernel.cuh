@@ -58,6 +58,8 @@ struct K1Params {
   long long* dbg;              // optional cycle counters (KSCHED_PROFILE_K1)
   int tables_in_smem;          // valset / absent / negempty / offset / anyoffer / member are staged too
   int n_valrows, n_offrows;
+  const int64_t* cls_req_ext;        // [n_pods = classes][n_res_ext] or nullptr (ksched.h: ksched_problem.class_requests_ext)
+  const uint32_t* cls_ext_present;   // [classes] or nullptr
 };
 
 // Parameters in constant memory and the CTA's catalog view (table pointers redirected to the staged shared-memory
@@ -151,6 +153,10 @@ __device__ __noinline__ unsigned long long k1_compute_row(int j, uint64_t word, 
           if (w < W32) fit &= c.fitset[((size_t)r * (T + 1) + rk) * W32 + w];
         }
         s &= fit;
+        if (s && p.cls_ext_present) {  // the rows are the class table: row j is class j
+          const uint32_t xp = p.cls_ext_present[j];
+          if (xp) s = ext_fit_word(c, nullptr, p.cls_req_ext + (size_t)j * c.n_res_ext, xp, s, w);
+        }
         if (s && itype_req != KSCHED_NONE) s &= p.itype_sets[(size_t)itype_req * W32 + w];
         if (mine) out[w] = s;
         if (cacheable) cache[v * wpl + wi] = s;
@@ -259,7 +265,8 @@ __global__ void __launch_bounds__(kK1Threads, 1) class_feasibility_kernel() {
   const int wpl = (W32 + 31) >> 5;  // column words per lane
   const bool cacheable = V * wpl <= kK1Cache;
   // fields of the row that feasibility depends on (requests, requirement masks, meta, tolerations, res_present, itype_req)
-  const uint64_t cmp_mask = lane <= 25 ? ~0ull : ((lane == 28 || lane == 29) ? 0xFFFFFFFFull : 0ull);
+  // With ext resources the class index (word 31) as well: two classes may differ in an ext request only.
+  const uint64_t cmp_mask = lane <= 25 ? ~0ull : ((lane == 28 || lane == 29) ? 0xFFFFFFFFull : ((lane == 31 && p.cls_ext_present) ? ~0ull : 0ull));
   uint32_t cache[kK1Cache];
   unsigned long long best_prev = kNoBest;
   uint64_t prev_word = 0;

@@ -162,6 +162,9 @@ struct ksched_handle {
   DevBuf<int32_t> d_cls_cursor;
   DevBuf<uint64_t> d_cls_tol_ext;  // [n_classes][tol_ext_words] taint sets from id 64 on (ksched_problem.class_tolerated_ext)
   int tol_ext_words = 0;
+  // ext resources (ksched.h: ksched_catalog.n_res_ext); allocated only when the catalog has some
+  DevBuf<int64_t> d_alloc_ext, d_cls_req_ext, d_ex_avail_ext, d_ex_req_ext, d_nn_req_ext;
+  DevBuf<uint32_t> d_cls_ext_present, d_nn_ext_present;
   // device-resident cluster snapshot (ksched_load_cluster)
   bool have_cluster = false;
   int stop_new_nodes = 0;
@@ -289,7 +292,8 @@ int ksched_create(int device_ordinal, ksched_handle** out) {
   {
     // CUDA loads kernels lazily on first launch: pull ours in here, not inside the first Solve
     cudaFuncAttributes fa;
-    cudaFuncGetAttributes(&fa, pack_kernel);
+    cudaFuncGetAttributes(&fa, pack_kernel<false>);
+    cudaFuncGetAttributes(&fa, pack_kernel<true>);
     cudaFuncGetAttributes(&fa, feasibility_kernel);
     cudaFuncGetAttributes(&fa, class_feasibility_kernel);
     cudaFuncGetAttributes(&fa, finalize_options_kernel);
@@ -317,6 +321,10 @@ int ksched_load_catalog(ksched_handle* h, const ksched_catalog* cat) {
   if (!h || !cat) return KSCHED_ERR_INVALID;
   if (cat->n_keys > KSCHED_MAX_KEYS || cat->n_res > KSCHED_MAX_RES || cat->n_templates > KSCHED_MAX_TEMPLATES || cat->n_templates < 1 ||
       cat->n_types < 0) { h->err = "catalog dimensions out of range"; return KSCHED_ERR_INVALID; }
+  if (cat->n_res_ext < 0 || cat->n_res_ext > KSCHED_MAX_RES_EXT || (cat->n_res_ext > 0 && (cat->n_res != KSCHED_MAX_RES || !cat->type_alloc_ext))) {
+    h->err = "inconsistent ext resources: n_res_ext in [0, 24], and with ext resources n_res == 8 and type_alloc_ext set";
+    return KSCHED_ERR_INVALID;
+  }
   // Gt/Lt cross the ABI in region form (ksched_key_regions): a requirement set that still carries gt / lt is a caller bug
   if (cat->type_bounds || cat->template_bounds) { h->err = "bounds arrays must be NULL: Gt/Lt requirements are passed in region form (ksched_key_regions)"; return KSCHED_ERR_INVALID; }
   for (int v = 0; v < cat->n_templates; ++v) {
@@ -351,6 +359,8 @@ int ksched_load_catalog(ksched_handle* h, const ksched_catalog* cat) {
     put(cat->types, sizeof(ksched_type_row) * (size_t)T);
     put(cat->type_capacity, sizeof(int64_t) * (size_t)T * KSCHED_MAX_RES);
     if (has_off) put(cat->offering_keys, sizeof(uint64_t) * (size_t)T * 64);
+    put(&cat->n_res_ext, sizeof cat->n_res_ext);
+    if (cat->n_res_ext) put(cat->type_alloc_ext, sizeof(int64_t) * (size_t)T * cat->n_res_ext);
     if (h->have_catalog && blob == h->catalog_blob) {
       // same instance types: only the templates can differ (remaining provisioner limits move between solves, daemonset
       // overhead with the daemonsets) - they are small, re-upload them when they changed
@@ -498,6 +508,13 @@ int ksched_load_catalog(ksched_handle* h, const ksched_catalog* cat) {
   c.perm_desc = h->d_perm_desc.ptr; c.alloc_rt = h->d_alloc_rt.ptr; c.domset = h->d_domset.ptr;
   c.offer_keys = nullptr;
   c.input_index = nullptr;
+  c.n_res_ext = cat->n_res_ext;
+  c.alloc_ext = nullptr;
+  if (cat->n_res_ext > 0 && T > 0) {
+    CUDA_TRY(h, upload(h, h->d_alloc_ext, cat->type_alloc_ext, (size_t)T * cat->n_res_ext));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    c.alloc_ext = h->d_alloc_ext.ptr;
+  }
   if (cat->offering_keys && T > 0) {
     std::vector<uint32_t> input_index(T);
     for (int t = 0; t < T; ++t) input_index[t] = cat->types[t].input_index;
@@ -639,6 +656,17 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
         return KSCHED_ERR_INVALID;
       }
   }
+  {
+    // ext resources: the tables exist exactly when the catalog has ext resources, and name no resource beyond them
+    const int X = h->cat.n_res_ext;
+    const bool any = pb->class_requests_ext || pb->class_res_ext_present || pb->existing_available_ext;
+    if (X > 0 ? !(pb->class_requests_ext && pb->class_res_ext_present && (pb->existing_available_ext || pb->n_existing == 0)) : any) {
+      h->err = "ext resource tables must be set exactly when the catalog has ext resources";
+      return KSCHED_ERR_INVALID;
+    }
+    for (int c2 = 0; c2 < (X > 0 ? pb->n_classes : 0); ++c2)
+      if (pb->class_res_ext_present[c2] >> X) { h->err = "class_res_ext_present names an ext resource beyond n_res_ext"; return KSCHED_ERR_INVALID; }
+  }
   CUDA_TRY(h, cudaSetDevice(h->device));
   // the superset buffers ksched_load_cluster filled are about to be overwritten: simulations need a new ksched_load_cluster
   h->have_cluster = false;
@@ -672,6 +700,19 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
   CUDA_TRY(h, upload(h, h->d_classes, pb->classes, (size_t)NC));
   h->tol_ext_words = pb->class_tolerated_ext ? pb->n_tolerated_ext_words : 0;
   if (h->tol_ext_words > 0) CUDA_TRY(h, upload(h, h->d_cls_tol_ext, pb->class_tolerated_ext, (size_t)NC * h->tol_ext_words));
+  if (const int X = c.n_res_ext) {
+    CUDA_TRY(h, upload(h, h->d_cls_req_ext, pb->class_requests_ext, (size_t)NC * X));
+    CUDA_TRY(h, upload(h, h->d_cls_ext_present, pb->class_res_ext_present, (size_t)NC));
+    // existing nodes: [x][n_existing] (the scan reads one resource of consecutive nodes)
+    std::vector<int64_t> avail((size_t)X * std::max(NE, 1), 0);
+    for (int e = 0; e < NE; ++e)
+      for (int x = 0; x < X; ++x) avail[(size_t)x * NE + e] = pb->existing_available_ext[(size_t)e * X + x];
+    CUDA_TRY(h, upload_vec(h, h->d_ex_avail_ext, avail));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    CUDA_TRY(h, h->d_ex_req_ext.ensure((size_t)X * std::max(NE, 1)));
+    CUDA_TRY(h, h->d_nn_req_ext.ensure((size_t)X * MAXN));
+    CUDA_TRY(h, h->d_nn_ext_present.ensure((size_t)MAXN));
+  }
   {
     // queue.go:82-108 orders by cpu desc, memory desc, timestamp asc, UID asc. (cpu, memory) is a property of the class: rank
     // the classes once here, and the whole order is one packed key when rank, timestamp span and UID rank fit 64 bits.
@@ -904,6 +945,9 @@ static void fill_k1(ksched_handle* h, K1Params& k1) {
   k1.itype_sets = h->d_itype_sets.ptr;
   k1.F = h->d_Fclass.ptr;
   k1.best = h->d_best_class.ptr;
+  const bool ext = h->cat.n_res_ext > 0;
+  k1.cls_req_ext = ext ? h->d_cls_req_ext.ptr : nullptr;
+  k1.cls_ext_present = ext ? h->d_cls_ext_present.ptr : nullptr;
   const int W32 = h->cat.W32;
   if (h->world > 1) {
     ksched_shard_range(W32, h->rank, h->world, &k1.word_begin, &k1.word_end);
@@ -1016,6 +1060,11 @@ static int reset_state(ksched_handle* h, const int64_t* d_remaining_src = nullpt
   add(h->d_ex_closed.ptr, nullptr, (size_t)NE);
   add(h->d_cls_cursor.ptr, nullptr, (size_t)std::max(h->n_classes, 1) * 4);
   if (h->have_volumes) add(h->d_ex_vol.ptr, h->d_ex_vol0.ptr, (size_t)h->n_existing * sizeof(ksched_node_volumes));
+  if (h->cat.n_res_ext) {  // ext sums of existing and new nodes: every mode that opens a node relies on zeros here
+    add(h->d_ex_req_ext.ptr, nullptr, (size_t)h->cat.n_res_ext * NE * 8);
+    add(h->d_nn_req_ext.ptr, nullptr, (size_t)h->cat.n_res_ext * h->max_new * 8);
+    add(h->d_nn_ext_present.ptr, nullptr, (size_t)h->max_new * 4);
+  }
   add(h->d_grp_cnt.ptr, h->d_grp_cnt0.ptr, (size_t)NG * 64 * 4);
   add(h->d_grp_registered.ptr, h->d_grp_registered0.ptr, (size_t)NG * 8);
   add(h->d_grp_host_total.ptr, h->d_grp_host_total0.ptr, (size_t)NG * 4);
@@ -1065,6 +1114,10 @@ static int run_pack(ksched_handle* h) {
   s.ex_hp = h->d_ex_hp.ptr; s.ex_closed = h->d_ex_closed.ptr;
   s.cls_cursor = h->d_cls_cursor.ptr;
   s.cls_tol_ext = h->tol_ext_words > 0 ? h->d_cls_tol_ext.ptr : nullptr; s.tol_ext_words = h->tol_ext_words;
+  const bool ext = h->cat.n_res_ext > 0;
+  s.cls_req_ext = ext ? h->d_cls_req_ext.ptr : nullptr; s.cls_ext_present = ext ? h->d_cls_ext_present.ptr : nullptr;
+  s.ex_avail_ext = ext ? h->d_ex_avail_ext.ptr : nullptr; s.ex_req_ext = ext ? h->d_ex_req_ext.ptr : nullptr;
+  s.nn_req_ext = ext ? h->d_nn_req_ext.ptr : nullptr; s.nn_ext_present = ext ? h->d_nn_ext_present.ptr : nullptr;
   s.cls_vol = h->have_volumes ? h->d_cls_vol.ptr : nullptr; s.ex_vol = h->have_volumes ? h->d_ex_vol.ptr : nullptr;
   for (int d = 0; d < KSCHED_MAX_VOLUME_DRIVERS; ++d) s.vol_mask[d] = h->vol_mask[d];
   s.nn_tmpl = h->d_nn_tmpl.ptr; s.nn_count = h->d_nn_count.ptr; s.nn_tb = h->d_nn_tb.ptr; s.nn_req = h->d_nn_req.ptr;
@@ -1111,8 +1164,9 @@ static int run_pack(ksched_handle* h) {
     CUDA_TRY(h, cudaStreamWaitEvent(h->stream, done, 0));  // no-op for an event that was never recorded
     CUDA_TRY(h, cudaMemcpyToSymbolAsync(g_k2, &k2, sizeof(K2Params), 0, cudaMemcpyHostToDevice, h->stream));
     // the attribute belongs to the function, not to the handle: set it under the same lock as the launch
-    CUDA_TRY(h, cudaFuncSetAttribute(pack_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    pack_kernel<<<1, threads, smem, h->stream>>>();
+    void (*kern)() = h->cat.n_res_ext > 0 ? pack_kernel<true> : pack_kernel<false>;
+    CUDA_TRY(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<1, threads, smem, h->stream>>>();
     CUDA_TRY(h, cudaGetLastError());
     CUDA_TRY(h, cudaEventRecord(done, h->stream));
   }
@@ -1263,6 +1317,13 @@ int ksched_download(ksched_handle* h, const ksched_problem* pb, ksched_result* r
       uint32_t* dst = reinterpret_cast<uint32_t*>(res->new_node_types + (size_t)n * W64);
       for (int w = 0; w < W32; ++w) dst[w] = opts[(size_t)w * n_new + n];
       if (W32 & 1) dst[W32] = 0;  // the row is W64 64-bit words: the caller's buffer need not be cleared
+    }
+    if (const int X = h->cat.n_res_ext) {
+      if (res->new_node_requests_ext)
+        CUDA_TRY(h, cudaMemcpyAsync(res->new_node_requests_ext, h->d_nn_req_ext.ptr, (size_t)n_new * X * 8, cudaMemcpyDeviceToHost, h->stream));
+      if (res->new_node_requests_ext_present)
+        CUDA_TRY(h, cudaMemcpyAsync(res->new_node_requests_ext_present, h->d_nn_ext_present.ptr, (size_t)n_new * 4, cudaMemcpyDeviceToHost, h->stream));
+      CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     }
   }
   if (res->launch && n_new > 0) {

@@ -301,6 +301,11 @@ __device__ __forceinline__ PodRegs load_pod_regs(const ksched_pod_row* row, uint
   return r;
 }
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
+// Ext resources the class requests (DESIGN.md §3). Such classes take the generic step only: every closed-form mode below
+// reads the 8 row slots alone, and the variant store's key and row compare cannot see an ext amount.
+__device__ __forceinline__ uint32_t class_ext(const PackState& s, unsigned cls) {
+  return s.cls_ext_present ? s.cls_ext_present[cls] : 0u;
+}
 
 // Slow part of a candidate check (requirement keys / topology / instance-type words), kept out of line so that the
 // common path (no requirement can change, dominant option fits) stays in registers.
@@ -313,16 +318,17 @@ struct SlowEval {
   bool need_types;  // with_types == false: the instance-type options still have to be checked (by the whole CTA, for the winner only)
 };
 // `t` receives the touched requirement keys: the thread's own e.t, or the CTA's shared Touched when the caller is the argmin winner
+template <bool kExt>
 __device__ __noinline__ bool evaluate_slow(bool plain,
                                            int n, unsigned short fl, const long long* q_hot, const int64_t* alloc_sorted, bool with_types, Touched& t,
                                            SlowEval& e) {
   KS_K2
   KS_ROW
   const int MAXN = s.max_new, NE = s.n_existing, R = c.n_res, W32 = c.W32;
-  const uint32_t p_res = row.res_present;
+  const uint32_t p_res = row.res_present, p_ext = kExt ? class_ext(s, (unsigned)row.reserved) : 0u;
   t.n = 0;
   e.changed = false;
-  bool need_types = !(fl & 1) || row.itype_req != KSCHED_NONE;
+  bool need_types = !(fl & 1) || row.itype_req != KSCHED_NONE || p_ext;
   if (!plain) {
     if (!requirements_phase(s.nn_vals, s.nn_meta[n], MAXN, n, NE + n, false, t)) return false;
     for (int i = 0; i < t.n; ++i) e.changed = e.changed || t.changed[i];
@@ -336,7 +342,10 @@ __device__ __noinline__ bool evaluate_slow(bool plain,
   build_type_ctx(t, e.q, e.qp, s.nn_vals, s.nn_meta[n], MAXN, n, false, alloc_sorted, e.x);
   for (int w = 0; w < W32; ++w) {
     const uint32_t base = s.nn_opts[(size_t)w * MAXN + n];
-    if (base && type_word(c, s, e.x, base, w)) return true;
+    uint32_t sw = base ? type_word(c, s, e.x, base, w) : 0;
+    if (sw && p_ext)
+      sw = ext_fit_word(c, s.nn_req_ext + (size_t)n * c.n_res_ext, s.cls_req_ext + (size_t)row.reserved * c.n_res_ext, p_ext, sw, w);
+    if (sw) return true;
   }
   return false;
 }
@@ -359,16 +368,21 @@ __device__ __forceinline__ uint64_t commit_reqs(int n, const Touched& t) {
 }
 // Requirement-changing commit done by ONE thread (fallback mode): new masks, requirement-driven narrowing of the stored
 // options, new bounds.
+template <bool kExt>
 __device__ __noinline__ void commit_slow(int n, SlowEval& e, long long* bound,
                                          long long* bound2, unsigned short* front_bits, uint64_t* meta_out) {
   KS_K2
   KS_ROW
   const int MAXN = s.max_new, W32 = c.W32;
   *meta_out = commit_reqs(n, e.t);
-  e.x.res_mask = 0;  // resources stay lazy (finalize_options_kernel)
+  e.x.res_mask = 0;  // resources stay lazy (finalize_options_kernel), except ext resources: narrowed eagerly (DESIGN.md §3)
+  const uint32_t p_ext = kExt ? class_ext(s, (unsigned)row.reserved) : 0u;
   for (int w = 0; w < W32; ++w) {
     const uint32_t base = s.nn_opts[(size_t)w * MAXN + n];
-    if (base) s.nn_opts[(size_t)w * MAXN + n] = type_word(c, s, e.x, base, w);
+    uint32_t sw = base ? type_word(c, s, e.x, base, w) : 0;
+    if (sw && p_ext)
+      sw = ext_fit_word(c, s.nn_req_ext + (size_t)n * c.n_res_ext, s.cls_req_ext + (size_t)row.reserved * c.n_res_ext, p_ext, sw, w);
+    if (base) s.nn_opts[(size_t)w * MAXN + n] = sw;
   }
   compute_front(s.nn_opts, MAXN, n, bound, bound2, front_bits);
 }
@@ -515,6 +529,8 @@ __device__ __noinline__ void existing_run(const PodRegs& first) {
 // One full Scheduler.add for one pod (existing nodes -> in-flight nodes -> new node -> relax/requeue). Every thread of
 // the CTA calls it together. Kept out of line: the steady-state path in pack_kernel must stay a few KB of code, because a
 // single resident CTA runs straight out of the instruction cache hierarchy (L0 ~6 KB, L1.5 32 KB).
+// kExt: the problem has ext resources (DESIGN.md §3); without them every ext branch is compiled out.
+template <bool kExt>
 __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, int fpos_first, LoopVars& L) {
   KS_K2
   const int tid = threadIdx.x, lane = tid & 31;
@@ -577,8 +593,12 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
         if (pt.overflow) { fatal = KSCHED_ERR_UNSUPPORTED; return; }
       }
     }
-    const bool plain = p_keys == 0 && !pt_nonempty && p_itype == KSCHED_NONE && p_hostname == KSCHED_NONE;  // no requirement can change
-    const bool simple = !has_topo && p_hpc == 0 && p_hpe == 0;  // the requirement verdict memo (HotSmem::absorbed/rejected) applies
+    // ext resources (DESIGN.md §3): checked on every node this class is placed on, narrowed eagerly into new nodes' options.
+    // A class that requests one is neither plain nor simple: no in-flight node accepts it without the full check.
+    const uint32_t p_ext = kExt ? class_ext(s, cls) : 0u;
+    const int X = c.n_res_ext;
+    const bool plain = p_keys == 0 && !pt_nonempty && p_itype == KSCHED_NONE && p_hostname == KSCHED_NONE && !p_ext;  // no requirement can change
+    const bool simple = !has_topo && p_hpc == 0 && p_hpe == 0 && !p_ext;  // the requirement verdict memo (HotSmem::absorbed/rejected) applies
 
     bool placed = false;
     ksched_class_volumes p_vol{};
@@ -617,6 +637,10 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
           long long q = s.ex_req[(size_t)r * NE + e] + (((p_res >> r) & 1) ? row.requests[r] : 0);
           long long a = ((s.ex_avail_present[e] >> r) & 1) ? s.ex_avail[(size_t)r * NE + e] : 0;
           ok = q <= a;
+        }
+        for (uint32_t m = p_ext; m && ok; m &= m - 1) {
+          const int x = __ffs(m) - 1;
+          ok = s.ex_req_ext[(size_t)x * NE + e] + s.cls_req_ext[(size_t)cls * X + x] <= s.ex_avail_ext[(size_t)x * NE + e];
         }
         if (!ok) continue;
         if (soft == ~0u) soft = (unsigned)e;
@@ -657,6 +681,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
             if (s.min_req[r] > 0 && s.ex_req[(size_t)r * NE + e] + s.min_req[r] > a) closed = true;
           }
           s.ex_req_present[e] |= p_res;
+          for (uint32_t m = p_ext; m; m &= m - 1) { const int x = __ffs(m) - 1; s.ex_req_ext[(size_t)x * NE + e] += s.cls_req_ext[(size_t)cls * X + x]; }
           if (p_hpe) s.ex_hp[e] |= p_hpe;
           if (has_vol) {  // volumeUsage.Add existingnode.go:128
             ksched_node_volumes nv = s.ex_vol[e];
@@ -719,7 +744,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
               if (!topo_prefilter(s.nn_vals, s.nn_meta[n], MAXN, n, NE + n)) continue;
             } else {
               last_slow = a;
-              if (!evaluate_slow(plain, H.node(a), fl, q, alloc_sorted, full_eval, ev.t, ev)) {
+              if (!evaluate_slow<kExt>(plain, H.node(a), fl, q, alloc_sorted, full_eval, ev.t, ev)) {
                 if (simple) H.rejected(a) = cls;
                 continue;
               }
@@ -744,13 +769,13 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
           if (best_slow && last_slow != a) {
             // without the instance-type part the touched keys go straight into the CTA's shared Touched
             in_shared = !full_eval;
-            okw = evaluate_slow(plain, H.node(a), H.flags(a), bq, alloc_sorted, full_eval, in_shared ? fresh_t : ev.t, ev);
+            okw = evaluate_slow<kExt>(plain, H.node(a), H.flags(a), bq, alloc_sorted, full_eval, in_shared ? fresh_t : ev.t, ev);
           }
           sh.win_a = a;
           sh.win_n = H.node(a);
           sh.win_fail = okw ? 0 : 1;
           sh.win_need = (okw && best_slow && ev.need_types) ? 1 : 0;
-          sh.win_commit = (okw && best_slow && (ev.changed || p_itype != KSCHED_NONE)) ? 1 : 0;
+          sh.win_commit = (okw && best_slow && (ev.changed || p_itype != KSCHED_NONE || p_ext)) ? 1 : 0;
           if (sh.win_need) {
             if (!in_shared) fresh_t = ev.t;
             for (int r = 0; r < KSCHED_MAX_RES; ++r) sh.q[r] = r < R ? ev.q[r] : 0;
@@ -783,10 +808,12 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
           // one pass: requirement-narrowed word kept in a register, resource test on top of it
           uint32_t keep_base = 0, keep = 0;
           int local_any = 0;
+          const int64_t* wn_ext = p_ext ? s.nn_req_ext + (size_t)wn * X : nullptr;
           for (int w = tid; w < W32; w += blockDim.x) {
             const uint32_t base = s.nn_opts[(size_t)w * MAXN + wn];
             if (!base) continue;
-            const uint32_t sw = type_word_keys(c, s, fresh_x, base, w);
+            uint32_t sw = type_word_keys(c, s, fresh_x, base, w);
+            if (sw && p_ext) sw = ext_fit_word(c, wn_ext, s.cls_req_ext + (size_t)cls * X, p_ext, sw, w);
             if (w == tid) { keep_base = base; keep = sw; }
             if (sw && type_word_res(c, fresh_x, sw, w)) local_any = 1;
           }
@@ -806,7 +833,8 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
             for (int w = tid + blockDim.x; w < W32; w += blockDim.x) {
               const uint32_t base = s.nn_opts[(size_t)w * MAXN + wn];
               if (!base) continue;
-              const uint32_t sw = type_word_keys(c, s, fresh_x, base, w);
+              uint32_t sw = type_word_keys(c, s, fresh_x, base, w);
+              if (sw && p_ext) sw = ext_fit_word(c, wn_ext, s.cls_req_ext + (size_t)cls * X, p_ext, sw, w);
               if (sw != base) { s.nn_opts[(size_t)w * MAXN + wn] = sw; local_changed = 1; }
             }
             opts_changed = __syncthreads_or(local_changed) != 0;
@@ -840,7 +868,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
           s.nn_count[n] = count;
           s.nn_tb[n] = -(tick + 1);  // front of the next pod-count block under a stable sort
           H.key(a) = order_key(count, -(tick + 1));
-          if (best_slow && (ev.changed || p_itype != KSCHED_NONE)) {
+          if (best_slow && (ev.changed || p_itype != KSCHED_NONE || p_ext)) {
             long long nb1[kHotRes], nb2[kHotRes];
             unsigned short fb;
             bool new_front = true;
@@ -850,13 +878,17 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
               else new_front = false;  // same option set, same Pareto front
             } else {
               uint64_t meta;
-              commit_slow(n, ev, nb1, nb2, &fb, &meta);
+              commit_slow<kExt>(n, ev, nb1, nb2, &fb, &meta);
             }
             if (new_front) {
 #pragma unroll
               for (int r = 0; r < kHotRes; ++r) { H.bound(r, a) = nb1[r]; H.bound2(r, a) = nb2[r]; }
               fl = (unsigned short)((fl & ~(kFlExact | kFlTwo)) | fb);
             }
+          }
+          if (p_ext) {  // after the narrowing above, which read the node's sums before this pod
+            for (uint32_t m = p_ext; m; m &= m - 1) { const int x = __ffs(m) - 1; s.nn_req_ext[(size_t)n * X + x] += s.cls_req_ext[(size_t)cls * X + x]; }
+            s.nn_ext_present[n] |= p_ext;
           }
           H.flags(a) = fl;
           H.rejected(a) = KSCHED_NONE;
@@ -993,6 +1025,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
             uint32_t sw = 0;
             if (path == kPathDynCached) sw = s.fd_opts[(size_t)fd_slot * W32 + w];
             else if (base) sw = path == kPathRow ? (base & s.F[((size_t)fpos * V + v) * W32 + w]) : type_word(c, s, fresh_x, base, w);
+            if (sw && p_ext && path == kPathDynamic) sw = ext_fit_word(c, nullptr, s.cls_req_ext + (size_t)cls * X, p_ext, sw, w);  // (F has them)
             s.nn_opts[(size_t)w * MAXN + n] = sw;
             if (memo) s.fc_opts[fc * W32 + w] = sw;
             if (path == kPathDynamic && fd_slot >= 0) s.fd_opts[(size_t)fd_slot * W32 + w] = sw;
@@ -1062,6 +1095,10 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
           s.nn_tmpl[n] = (uint8_t)v;
           for (int r = 0; r < KSCHED_MAX_RES; ++r) s.nn_req[(size_t)r * MAXN + n] = sh.q[r];
           s.nn_req_present[n] = sh.qp;
+          if (kExt) {  // a fresh node's ext sums are the pod's: no daemonset requests an ext resource
+            for (int x = 0; x < X; ++x) s.nn_req_ext[(size_t)n * X + x] = ((p_ext >> x) & 1) ? s.cls_req_ext[(size_t)cls * X + x] : 0;
+            s.nn_ext_present[n] = p_ext;
+          }
           s.nn_hp[n] = p_hpe;
           s.nn_count[n] = 1;
           s.nn_tb[n] = tick + 1;  // appended: last of the one-pod block
@@ -1187,7 +1224,7 @@ __device__ __noinline__ void warp_resident_loop(WarpIO* io) {
   for (int r = 0; r < kHotRes; ++r) min_req[r] = r < RH ? s.min_req[r] : 0;
 
   while (true) {
-    if (!simple_pod_regs(cur)) break;  // this pod takes the block-wide path
+    if (!simple_pod_regs(cur) || class_ext(s, (unsigned)cur.cls64)) break;  // this pod takes the block-wide path
     const bool plain = plain_pod_regs(cur);
     const unsigned cls = (unsigned)cur.cls64;
     const bool cand = live && rejected != cls && ((cur.tol >> tmpl_taintset[fl >> 8]) & 1);
@@ -2953,6 +2990,8 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
 #define PK_T(i)
 #endif
 
+// kExt: the problem has ext resources (DESIGN.md §3). Without them the kernel is compiled without any ext gate.
+template <bool kExt>
 __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
 #ifdef KSCHED_PROFILE_PACK
   long long pk_acc[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
@@ -3044,7 +3083,8 @@ __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
       }
     }
     // ---- register-resident mode (see warp_resident_loop): entered when the next pod is plain and <= 32 nodes are open
-    if (fast_allowed && s.use_warp_loop && !fresh_valid && qi < s.n_pods && n_active > 0 && n_active <= 32 && simple_pod_regs(nxt)) {
+    if (fast_allowed && s.use_warp_loop && !fresh_valid && qi < s.n_pods && n_active > 0 && n_active <= 32 && simple_pod_regs(nxt) &&
+        !(kExt && class_ext(s, (unsigned)nxt.cls64))) {
       __syncthreads();
       if (tid == 0) { wio.qi = qi; wio.head = head; wio.qlen = qlen; wio.tick = tick; wio.seq = seq; wio.n_active = n_active; wio.add_calls = add_calls; }
       __syncthreads();
@@ -3060,7 +3100,7 @@ __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
     bool skip_run = true;
     if (fast_allowed && s.use_class_run && qi < s.n_pods && n_active <= kActCap) {
       const bool topo_cls = nxt.topo_begin != nxt.topo_end;
-      const bool shape_ok = nxt.hpc == 0 && nxt.hpe == 0 && (nxt.res >> kHotRes) == 0 &&
+      const bool shape_ok = nxt.hpc == 0 && nxt.hpe == 0 && (nxt.res >> kHotRes) == 0 && !(kExt && class_ext(s, (unsigned)nxt.cls64)) &&
                             (!topo_cls || (((nxt.meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF) == 0 && nxt.itype == KSCHED_NONE && nxt.hostname == KSCHED_NONE));
       if (shape_ok && (unsigned)nxt.cls64 != run_block_cls) {
         if (fresh_valid && fresh_cls == (unsigned)nxt.cls64) skip_run = false;  // a fresh node of this class to capture
@@ -3113,7 +3153,8 @@ __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
     // ---- existing-node run (see existing_run): identical plain pods take the existing nodes in one prefix-sum pass
     if (NE > 0 && !s.count_visited && qi < s.n_pods && (unsigned)nxt.cls64 != xrun_block_cls &&
         ((nxt.meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF) == 0 && nxt.topo_begin == nxt.topo_end && nxt.itype == KSCHED_NONE &&
-        nxt.hostname == KSCHED_NONE && nxt.hpc == 0 && nxt.hpe == 0 && (nxt.res >> kHotRes) == 0 && !class_has_volumes(s, (unsigned)nxt.cls64)) {
+        nxt.hostname == KSCHED_NONE && nxt.hpc == 0 && nxt.hpe == 0 && (nxt.res >> kHotRes) == 0 && !class_has_volumes(s, (unsigned)nxt.cls64) &&
+        !(kExt && class_ext(s, (unsigned)nxt.cls64))) {
       __syncthreads();
       if (tid == 0) { ExRunIO& io = g_xio; io.qi = qi; io.head = head; io.qlen = qlen; io.seq = seq; io.parity = parity; io.add_calls = add_calls; io.placed = 0; }
       __syncthreads();
@@ -3153,7 +3194,7 @@ __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
     if (tid == 0) s.counters[8 + 9] += 1;
 #endif
     LoopVars L{head, qlen, n_new, n_active, tick, seq, parity, fatal, epoch, pt_nonempty, nodes_visited, pt_class, row_class, 0, 0, KSCHED_NONE, 0};
-    generic_step(cur, first_pass, fpos_first, L);
+    generic_step<kExt>(cur, first_pass, fpos_first, L);
     if (L.fail_memo) { fail_cls = (unsigned)cur.cls64; fail_seq = L.seq; fail_epoch = L.epoch; } else fail_cls = KSCHED_NONE;
     head = L.head; qlen = L.qlen; n_new = L.n_new; n_active = L.n_active; tick = L.tick; seq = L.seq; parity = L.parity; fatal = L.fatal;
     epoch = L.epoch; pt_nonempty = L.pt_nonempty; nodes_visited = L.nodes_visited; pt_class = L.pt_class; row_class = L.row_class;

@@ -127,6 +127,13 @@ struct PackState {
   // taint sets from id 64 on, existing nodes only (ksched.h: class_tolerated_ext)
   const uint64_t* cls_tol_ext;       // [n_classes][tol_ext_words], or nullptr
   int tol_ext_words;
+  // ext resources (ksched.h: ksched_catalog.n_res_ext; DESIGN.md §3), all nullptr without them
+  const int64_t* cls_req_ext;        // [n_classes][n_res_ext]
+  const uint32_t* cls_ext_present;   // [n_classes]
+  const int64_t* ex_avail_ext;       // [n_res_ext][n_existing]
+  int64_t* ex_req_ext;               // [n_res_ext][n_existing] what the batch's pods placed there request
+  int64_t* nn_req_ext;               // [max_new][n_res_ext]
+  uint32_t* nn_ext_present;          // [max_new]
 };
 
 struct K2Params {

@@ -505,8 +505,21 @@ struct Builder {
     for (auto& kv : r) {
       if (res_pruned && !res_id.count(kv.first)) continue;  // no request or limit reads it: it cannot change an answer
       int id = resource(kv.first);
+      if (id >= KSCHED_MAX_RES) continue;  // an ext resource: fill_ext
       out[id] = kv.second;
       present |= 1u << id;
+    }
+    return present;
+  }
+  // ext resources (ids from KSCHED_MAX_RES on) of r into out[E.n_res_ext]; bit x of the result: ext resource x is a key of r
+  uint32_t fill_ext(const ResourceList& r, int64_t* out) const {
+    uint32_t present = 0;
+    for (int i = 0; i < E.n_res_ext; ++i) out[i] = 0;
+    for (auto& kv : r) {
+      auto it = res_id.find(kv.first);
+      if (it == res_id.end() || it->second < KSCHED_MAX_RES) continue;
+      out[it->second - KSCHED_MAX_RES] = kv.second;
+      present |= 1u << (it->second - KSCHED_MAX_RES);
     }
     return present;
   }
@@ -1059,7 +1072,26 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
       for (auto& n : read) if (n != "cpu" && n != "memory" && n != "pods") E.res_names.push_back(n);
       B.res_pruned = true;
     }
-    if (E.res_names.size() > KSCHED_MAX_RES) unsupported("more than 8 distinct resources");
+    if (E.res_names.size() > KSCHED_MAX_RES) {
+      // Ext resources (DESIGN.md §3): the 8 row slots take cpu, memory, pods and every resource a daemonset requests or a
+      // provisioner limit names, then the other read resources by descending number of requesting pods (ties by name).
+      // The rest is requested by pod classes only, and only the classes requesting it ever read it.
+      std::set<std::string> bound = {"cpu", "memory", "pods"};
+      for (auto& d : daemons) for (auto& kv : pod_requests(d)) bound.insert(kv.first);
+      for (auto& pr : P.provisioners) for (auto& kv : pr.limits) bound.insert(kv.first);
+      if (bound.size() > KSCHED_MAX_RES) unsupported("more than 8 resources that a daemonset requests or a provisioner limit names");
+      if (E.res_names.size() > KSCHED_MAX_RES + KSCHED_MAX_RES_EXT) unsupported("more than 32 resources that a pod requests or a limit names");
+      std::map<std::string, size_t> requesting;
+      for (size_t i = 0; i < NP; ++i) for (auto& kv : specs[E.pod_class[i]].req) ++requesting[kv.first];
+      std::vector<std::string> rest;
+      for (size_t i = 3; i < E.res_names.size(); ++i) if (!bound.count(E.res_names[i])) rest.push_back(E.res_names[i]);
+      std::stable_sort(rest.begin(), rest.end(), [&](const std::string& a, const std::string& b) { return requesting[a] > requesting[b]; });
+      std::vector<std::string> order = {"cpu", "memory", "pods"};
+      for (auto& n : bound) if (n != "cpu" && n != "memory" && n != "pods") order.push_back(n);
+      order.insert(order.end(), rest.begin(), rest.end());
+      E.res_names = order;
+      E.n_res_ext = (int)E.res_names.size() - KSCHED_MAX_RES;
+    }
     for (size_t i = 0; i < E.res_names.size(); ++i) B.res_id[E.res_names[i]] = (int)i;
   }
 
@@ -1078,6 +1110,7 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
     std::stable_sort(E.type_input_index.begin(), E.type_input_index.end(), [&](int a, int b) { return min_price[a] < min_price[b]; });
     E.types.resize(NT);
     E.type_capacity.assign((size_t)NT * KSCHED_MAX_RES, 0);
+    E.type_alloc_ext.assign((size_t)NT * E.n_res_ext, 0);
     // launch-choice table: exact price order through ranks of the distinct (double) prices
     {
       std::set<double> prices;
@@ -1113,6 +1146,7 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
       for (auto& kv : alloc) { auto o = overhead.find(kv.first); if (o != overhead.end()) kv.second -= o->second; }
       row.res_present = B.fill_resources(alloc, row.allocatable);
       B.fill_resources(it.capacity, &E.type_capacity[(size_t)c * KSCHED_MAX_RES]);
+      if (E.n_res_ext) B.fill_ext(alloc, &E.type_alloc_ext[(size_t)c * E.n_res_ext]);
       for (size_t oi = 0; oi < it.offerings.size(); ++oi) {
         const Offering& o = it.offerings[oi];
         if (!o.available) continue;
@@ -1271,6 +1305,10 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
     for (auto& kv : avail) { auto f = pod_req.find(kv.first); if (f != pod_req.end()) kv.second -= f->second; }
     e.available_present = B.fill_resources(avail, e.available);
     e.requests_present = B.fill_resources(rem, e.requests);
+    if (E.n_res_ext) {
+      E.existing_available_ext.resize(E.existing_available_ext.size() + E.n_res_ext);
+      B.fill_ext(avail, &E.existing_available_ext[E.existing_available_ext.size() - E.n_res_ext]);
+    }
     e.taintset = (uint32_t)B.taintset(nf.taints);
     e.itype = KSCHED_NONE;
     auto itl = n.labels.find(kInstanceType);
@@ -1643,12 +1681,15 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
       }
   });
   phase("  class relations");
+  E.class_requests_ext.assign((size_t)NC * E.n_res_ext, 0);
+  E.class_res_ext_present.assign(E.n_res_ext ? NC : 0, 0);
   for (int c = 0; c < NC; ++c) {
     const Pod& p = specs[c].pod;
     ksched_pod_row& row = E.classes[c];
     std::memset(&row, 0, sizeof row);
     std::memset(&E.class_bounds[c], 0, sizeof(ksched_bounds));
     row.res_present = B.fill_resources(specs[c].req, row.requests);
+    if (E.n_res_ext) E.class_res_ext_present[c] = B.fill_ext(specs[c].req, &E.class_requests_ext[(size_t)c * E.n_res_ext]);
     ksched_reqset rs{};
     Builder::Special sp;
     B.pod_requirements(p, rs, E.class_bounds[c], &sp);
@@ -1764,7 +1805,9 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
   phase("queue keys");
   // ------------------------------------------------------------------ wire up the flat structs
   ksched_catalog& cat = E.catalog;
-  cat.n_keys = NK; cat.n_res = (int)E.res_names.size(); cat.n_types = NT; cat.n_templates = NV;
+  cat.n_keys = NK; cat.n_res = (int)E.res_names.size() - E.n_res_ext; cat.n_types = NT; cat.n_templates = NV;
+  cat.n_res_ext = E.n_res_ext;
+  cat.type_alloc_ext = E.n_res_ext ? E.type_alloc_ext.data() : nullptr;
   cat.keys = E.keys.data();
   cat.key_int_values = E.key_int_values.data();
   cat.types = E.types.data();
@@ -1803,6 +1846,11 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
   }
   pr.class_tolerated_ext = E.class_tolerated_ext.empty() ? nullptr : E.class_tolerated_ext.data();
   pr.n_tolerated_ext_words = E.tolerated_ext_words;
+  if (E.n_res_ext) {
+    pr.class_requests_ext = E.class_requests_ext.data();
+    pr.class_res_ext_present = E.class_res_ext_present.data();
+    pr.existing_available_ext = E.existing_available_ext.data();
+  }
   pr.count_nodes_visited = 0;  // the exact nodes_visited statistic is opt-in (kh_set_count_visited / tests): it turns the pack kernel's steady-state paths off
   // Gt/Lt leave the host algebra here: templates and pod classes in region form (types and filter terms already are)
   for (int v = 0; v < NV; ++v) B.to_region_form(E.templates[v].reqs, tb[v]);

@@ -42,7 +42,7 @@ struct Encoded {
   std::vector<std::string> folded_keys;               // template-only keys folded into template_members (DESIGN.md §3), ascending
   std::vector<std::map<std::string, std::string>> template_folded;  // per template (empty when nothing is folded): folded key ->
                                                       // the template's requirement on it, rendered as render_requirement does
-  std::vector<std::string> res_names;                 // resource ids: cpu, memory, pods, then ascending
+  std::vector<std::string> res_names;                 // resource ids: cpu, memory, pods, then ascending; beyond 8: DESIGN.md §3
   // ---- which objects take part (provisioner.go:119-144 / deprovisioning/helpers.go:42-93)
   std::vector<const kmodel::Pod*> pods;               // Solve's pod list
   std::vector<int> existing_state_index;              // existing slot -> Problem.nodes index
@@ -92,6 +92,11 @@ struct Encoded {
   int n_taintsets = 0;                                // distinct taint sets of templates and existing nodes
   std::vector<uint64_t> class_tolerated_ext;          // [n_classes][tolerated_ext_words] sets from id 64 on (ksched.h); empty with <= 64 sets
   int tolerated_ext_words = 0;
+  int n_res_ext = 0;                                  // ext resources: res_names from index 8 on (ksched.h); 0 with <= 8 read resources
+  std::vector<int64_t> type_alloc_ext;                // [n_types][n_res_ext]
+  std::vector<int64_t> class_requests_ext;            // [n_classes][n_res_ext]
+  std::vector<uint32_t> class_res_ext_present;        // [n_classes]
+  std::vector<int64_t> existing_available_ext;        // [n_existing][n_res_ext]
 
   ksched_catalog catalog{};
   ksched_problem problem{};

@@ -66,6 +66,8 @@ struct ResultBuffers {
   std::vector<uint64_t> feasibility;
   std::vector<uint64_t> best;
   std::vector<ksched_launch_choice> launch;
+  std::vector<int64_t> ext;          // [max_new_nodes][n_res_ext] ext resources of the new nodes
+  std::vector<uint32_t> ext_present;
   ksched_result r{};
   // ksched_solve overwrites every per-pod entry and the rows of the nodes it reports (ksched_download), decode reads nothing
   // else: the buffers are sized, not cleared - kh_scheduler_solve keeps one set per thread, so a 100 000-pod Solve does not
@@ -87,6 +89,12 @@ struct ResultBuffers {
     r.existing_reqs = existing_reqs.data();
     launch.resize(nodes.size());
     r.launch = launch.data();
+    if (E.n_res_ext) {
+      ext.resize(N * E.n_res_ext);
+      ext_present.resize(N);
+      r.new_node_requests_ext = ext.data();
+      r.new_node_requests_ext_present = ext_present.data();
+    }
     r.feasibility = nullptr;
     r.best_column = nullptr;
     if (want_feasibility) {
@@ -174,8 +182,10 @@ void decode(const Encoded& E, const ResultBuffers& B, Result& out) {
       const ksched_new_node& src = B.nodes[n];
       NewNodeResult& dst = out.new_nodes[n];
       dst.provisioner = src.template_index;
-      for (size_t r = 0; r < E.res_names.size(); ++r)
+      for (size_t r = 0; r < E.res_names.size() && r < KSCHED_MAX_RES; ++r)
         if ((src.requests_present >> r) & 1) dst.requests[E.res_names[r]] = src.requests[r];
+      for (int x = 0; x < E.n_res_ext; ++x)  // ext resources (DESIGN.md §3)
+        if ((B.ext_present[n] >> x) & 1) dst.requests[E.res_names[(size_t)KSCHED_MAX_RES + x]] = B.ext[n * (size_t)E.n_res_ext + x];
       for (size_t k = 0; k < E.key_names.size(); ++k)
         if ((src.reqs.meta >> (KSCHED_META_PRESENT_SHIFT + k)) & 1) {
           const uint64_t memo_key = src.reqs.values[k] ^ (((src.reqs.meta >> (KSCHED_META_COMPLEMENT_SHIFT + k)) & 1) << 63);  // <= 63 values per key
@@ -339,12 +349,12 @@ void kh_encoded_free(Encoded* E) {
   if (E == g_gpu_encoded) { g_gpu_encoded = nullptr; g_gpu_current = false; }
   delete E;
 }
-// dims: [pods, classes, existing, groups, types, templates, keys, resources, type_words, class_topo, taintsets]
+// dims: [pods, classes, existing, groups, types, templates, keys, resources, type_words, class_topo, taintsets, resources_ext]
 void kh_encoded_dims(const Encoded* E, long long* out) {
   out[0] = (long long)E->pods.size(); out[1] = (long long)E->classes.size(); out[2] = (long long)E->existing.size();
   out[3] = (long long)E->groups.size(); out[4] = (long long)E->types.size(); out[5] = (long long)E->templates.size();
-  out[6] = (long long)E->key_names.size(); out[7] = (long long)E->res_names.size(); out[8] = E->type_words;
-  out[9] = (long long)E->class_topo.size(); out[10] = E->n_taintsets;
+  out[6] = (long long)E->key_names.size(); out[7] = (long long)E->res_names.size() - E->n_res_ext; out[8] = E->type_words;
+  out[9] = (long long)E->class_topo.size(); out[10] = E->n_taintsets; out[11] = E->n_res_ext;
 }
 void kh_encoded_set_count_visited(Encoded* E, int on) { E->problem.count_nodes_visited = on; }
 const ksched_catalog* kh_encoded_catalog(const Encoded* E) { return &E->catalog; }
@@ -1288,6 +1298,10 @@ extern "C" unsigned long long kh_encoded_digest(const Encoded* E) {
   vec(E->group_existing_counts); vec(E->class_topo); vec(E->filter_terms); vec(E->itype_req_sets); vec(E->itype_req_complement); vec(E->hostname_reqs);
   if (!E->class_volumes.empty()) { vec(E->class_volumes); vec(E->existing_volumes); bytes(E->volume_driver_mask, sizeof E->volume_driver_mask); }
   if (!E->class_tolerated_ext.empty()) vec(E->class_tolerated_ext);  // absent with at most 64 taint sets: those digests predate it
+  if (E->n_res_ext) {  // absent with at most 8 read resources: those digests predate ext resources
+    bytes(&E->n_res_ext, sizeof E->n_res_ext);
+    vec(E->type_alloc_ext); vec(E->class_requests_ext); vec(E->class_res_ext_present); vec(E->existing_available_ext);
+  }
   if (!E->folded_keys.empty()) {  // absent when nothing is folded: those digests predate template-only keys
     for (auto& k : E->folded_keys) str(k);
     for (auto& m : E->template_folded) { size_t n = m.size(); bytes(&n, sizeof n); for (auto& kv : m) { str(kv.first); str(kv.second); } }
@@ -1606,6 +1620,13 @@ int kh_encoded_key_info(const Encoded* E, const char* key, long long* out) {
     out[2] = E->key_regions.empty() ? 0 : E->key_regions[k].n_thresholds;
     return 0;
   }
+  return -1;
+}
+// Id of a resource in an encoding (tests): a row slot below 8, an ext resource from 8 on (DESIGN.md §3); -1 when the
+// encoding does not carry it.
+int kh_encoded_resource_id(const Encoded* E, const char* name) {
+  for (size_t r = 0; r < E->res_names.size(); ++r)
+    if (E->res_names[r] == name) return (int)r;
   return -1;
 }
 }

@@ -49,7 +49,7 @@ constexpr int kMaxCG = 8;        // topology groups that may constrain one pod c
 constexpr int kMaxTouched = 8;   // requirement keys one Add may touch (pod keys + topology keys)
 constexpr int kPackThreads = 512;
 constexpr int kFreshMemoSlots = 8192;  // PackState::fd_*
-constexpr int kNumCounters = 64;       // PackState::counters
+constexpr int kNumCounters = 96;      // PackState::counters
 constexpr uint64_t kNoBest = ~0ull;
 
 #include "catalog.cuh"
@@ -1151,6 +1151,7 @@ static int run_pack(ksched_handle* h) {
   s.use_mask_run = std::getenv("KSCHED_NO_MASKRUN") ? 0 : 1;
   s.use_level_warp = std::getenv("KSCHED_NO_LEVELWARP") ? 0 : 1;
   s.use_varstore = std::getenv("KSCHED_NO_VARSTORE") ? 0 : 1;
+  s.use_round_stretch = std::getenv("KSCHED_NO_ROUNDSTRETCH") ? 0 : 1;
   s.vstore = h->d_vstore.ptr;
   // block size: the chain is latency-bound on ONE thread's commit; more warps only help when there are many candidate
   // nodes to examine per pod (existing nodes, large in-flight sets)
@@ -1259,6 +1260,14 @@ static void print_pack_profile(const long long* counters) {
   fprintf(stderr, "[pack profile] mask run: single steps on the unpinned head=%lld | pin steps=%lld pods=%lld ended by "
                   "[staged entries,count,key,refused,end of list or 32 pods]=%lld,%lld,%lld,%lld,%lld\n",
           counters[48], counters[49], counters[50], counters[51], counters[52], counters[53], counters[54], counters[55]);
+  fprintf(stderr, "[pack profile] mask run rounds: iterations=%lld pods=%lld cycles=%lld | stretch length R (rounds a step could place, "
+                  "1..16) [pinned] [fresh]:", counters[62], counters[63], counters[61]);
+  for (int k = 0; k < 2; ++k) {
+    fprintf(stderr, " [");
+    for (int r = 0; r < 16; ++r) fprintf(stderr, r ? ",%lld" : "%lld", counters[64 + 16 * k + r]);
+    fprintf(stderr, "]");
+  }
+  fprintf(stderr, "\n");
   fprintf(stderr, "[pack profile] class_run without mask-key spread: cycles=%lld pods=%lld level+fill iterations=%lld (fill %lld) fresh=%lld per-pod=%lld | with: cycles=%lld pods=%lld fresh=%lld per-pod=%lld\n",
           counters[32], counters[33], counters[34], counters[46], counters[35], counters[44], counters[36], counters[37], counters[39], counters[45]);
 }

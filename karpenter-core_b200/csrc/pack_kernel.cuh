@@ -1527,12 +1527,15 @@ struct M1Ctx {
   uint16_t head[kM1Lists];            // first node of the list (between two entries of the warp loop)
   uint16_t ap[kM1Lv][kM1Lists];       // build: the bucket is arr[ap .. ae)
   uint16_t ae[kM1Lv][kM1Lists];
-  int bcnt[kM1Lv * kM1Lists];         // build: members per bucket (bucket = list * kM1Lv + count)
+  union {
+    int bcnt[kM1Lv * kM1Lists];       // build: members per bucket (bucket = list * kM1Lv + count)
+    unsigned long long rk[32];        // round stretch (after the build): the key of each node, round by round
+  };
   int bad;                            // build: a node the lists cannot represent
   int upos;                           // position of the unpinned list's head in arr: that list never gains a member (a node
                                       // leaves it when a pod pins it, fresh nodes are pinned), so it is the rest of the
                                       // segment the build sorted, and the pin step reads its next members without the links
-  uint16_t ps[32];                    // pin step: the node of each pod
+  uint16_t ps[32];                    // pin step: the node of each pod; round stretch: the node of each (round, domain)
   int out_adv, out_reason, out_tick, out_n_new, out_n_active;
   int n_fresh;                        // nodes created by this entry of the warp loop: slot | variant << 16; their global
   uint32_t fr[kRunChunk];             // state (option words, requirement values, requests, ...) is stored by the CTA afterwards
@@ -2029,6 +2032,35 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
         // smallest head key first - a whole round is committed at once, every lane its own domain
         const bool rounds = m_rec0 && m_bias0 == 0;
         int li = i, ltick = tick, lnew = n_new, lact = n_active, nfr = 0;
+        // a round's commit of one pod on the pinned node a (pod count c, room word rp) with tick mytick, staged entry q:
+        // Topology.Record, the node's new key and room word (returned); closed: the class no longer fits anywhere on it
+        auto commit_round = [&](int a, uint32_t rp, int c, int mytick, int q, bool& closed) -> uint32_t {
+          uint32_t rp2 = rp - 1 + (1u << 16);
+          for (int j = 0; j < n_host; ++j) {  // Topology.Record, hostname groups
+            const int times = rc.h_times[j];
+            const int old = hc[j * kTopoCap + a];
+            const int now = old + times > 0xFFFF ? 0xFFFF : old + times;
+            if (times) hc[j * kTopoCap + a] = (uint16_t)now;
+            if (now > rc.h_lim[j]) rp2 |= kRpDead;
+          }
+          unsigned long long skey = order_key(c + 1, -(mytick + 1));
+          rc.q_node[buf][q] = -(a + 2);
+          if ((rp2 & 0xFFFF) == 0) {  // the class no longer fits by resources: does anything? (node_closed)
+            const int placed = (rp2 >> 16) & 0x7FFF;
+            long long nq[kHotRes], cb1[kHotRes], cb2[kHotRes];
+#pragma unroll
+            for (int r = 0; r < kHotRes; ++r) { nq[r] = hs->q[r][a] + placed * p_req[r]; cb1[r] = hs->bound[r][a]; cb2[r] = hs->bound2[r][a]; }
+            const unsigned short fl = (unsigned short)(hs->flags[a] | ((p_res & 0xF) << 1));
+            if (node_closed(nq, min_req, RH, cb1, cb2, fl)) {
+              skey = ~0ull;
+              hs->nn_last[a] = ((unsigned long long)(unsigned)(c + 1) << 32) | (unsigned)(-(mytick + 1));
+              closed = true;
+            }
+          }
+          hs->key[a] = skey;
+          rpv[a] = rp2;
+          return rp2;
+        };
         unsigned fr_used = 0;  // ring slots the nodes created in this entry replay: a store fetch must not overwrite them
         int i_end = rc.q_end[buf];
         if (i + qlen < i_end) i_end = i + qlen;
@@ -2037,6 +2069,9 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
         // or more admits every domain exactly like the 64-bit form of the per-pod loop
         const int slack = m_bias0 < -(1 << 30) ? (1 << 30) : -m_bias0;
         while (li < i_end) {
+#ifdef KSCHED_PROFILE_PACK
+          const long long it0 = clock64();
+#endif
           const int mn = __reduce_min_sync(FULL, valid ? cnt_d : INT32_MAX);
           const bool allowed = valid && cnt_d - mn <= slack;
           const unsigned okm = __ballot_sync(FULL, allowed);
@@ -2063,6 +2098,117 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
               const unsigned hv = __ballot_sync(FULL, hd), fv = okm & ~hv;  // fv: domains that get a fresh node (no pinned node at hand)
               const bool bad_l = hd && ((hr & 0xFFFF) == kRoomSlow || (int)(hk >> 32) + 1 >= kM1Lv);
               const unsigned long long ukey = __shfl_sync(FULL, hk, kM1Dom);
+              // ---- round stretch: when every registered domain admits a pod (all counts are equal), each round gives every
+              // domain one pod, so the counts stay equal and the round's shape repeats. R rounds are placed in one step
+              // while R single rounds would take the same nodes (DESIGN.md section 4): pinned, the r-th members of each
+              // head's bucket; fresh, R fresh nodes per domain that take no second pod.
+              int R = 0, vi_s = -1;
+              const bool pinned = hv == okm;
+              const int jd = __popc(okm & ((1u << L) - 1u));  // act: this domain's place among the round's domains
+#ifdef KSCHED_PROFILE_PACK
+              if (okm == m_reg0 && 2 * na <= i_end - li && 2 * na <= 32) {
+#else
+              if (s.use_round_stretch && okm == m_reg0 && 2 * na <= i_end - li && 2 * na <= 32) {
+#endif
+                const int cap = (i_end - li) / na < 32 / na ? (i_end - li) / na : 32 / na;
+                if (pinned) {  // the bucket's keys ascend; nodes re-entering at count + 1 lie behind it
+                  int rd = 0;
+                  if (act) {
+                    const int c = (int)(hk >> 32);
+                    int a = h;
+                    unsigned long long k = hk;
+                    uint32_t rp = hr;
+                    while (rd < cap && (int)(k >> 32) == c && k < ukey && (rp & 0xFFFF) != kRoomSlow && c + 1 < kM1Lv) {
+                      m1.ps[rd * na + jd] = (uint16_t)a;
+                      m1.rk[rd * na + jd] = k;
+                      ++rd;
+                      a = nxt_of(a);
+                      if (a < 0) break;
+                      k = hs->key[a];
+                      rp = rpv[a];
+                    }
+                  }
+                  R = __reduce_min_sync(FULL, act ? rd : 32);
+                } else if (hv == 0 && ukey == ~0ull && (okm & ~rc.m_tallow[0]) == 0) {  // fresh nodes that never re-enter a list
+                  if (act) for (int v2 = 0; v2 < rc.n_var && vi_s < 0; ++v2) if (rc.var[v2].dom[0] == L) vi_s = v2;
+                  const bool shut = vi_s >= 0 && ((rc.var[vi_s].rp & 0xFFFF) == 0 || (rc.var[vi_s].rp & kRpDead));
+                  bool ok = !__any_sync(FULL, act && !shut);
+                  for (int j = 0; j < n_host; ++j) ok = ok && rc.h_lim[j] >= 0;
+                  int room = MAXN - lnew;
+                  if (kActCap - lact < room) room = kActCap - lact;
+                  if (kTopoCap - lact < room) room = kTopoCap - lact;
+                  R = !ok ? 0 : room / na < cap ? room / na : cap;
+                }
+#ifdef KSCHED_PROFILE_PACK
+                if (L == 0 && R > 0) s.counters[64 + (pinned ? 0 : 16) + (R > 16 ? 16 : R) - 1] += 1;
+                if (!s.use_round_stretch) R = 0;
+#endif
+              }
+              if (R >= 2) {
+                const int np = R * na;
+                if (pinned) {
+                  const int c = (int)(hk >> 32);
+                  if (act) for (int r = 0; r < R; ++r) pop_head(c);  // (reads the keys of the bucket before they change)
+                  __syncwarp();
+                  bool closed_l = false;
+                  if (L < np) {  // pod L: round L / na, the node whose key has rank L % na in that round
+                    const int r = L / na, a = m1.ps[L];
+                    const unsigned long long k = m1.rk[L];
+                    int p = r * na;
+                    for (int j = 0; j < na; ++j) p += m1.rk[r * na + j] < k;
+                    commit_round(a, rpv[a], (int)(k >> 32), ltick + p, li + p, closed_l);
+                  }
+                  const unsigned tb = __ballot_sync(FULL, closed_l);
+                  if (L == 0 && tb) rc.tomb = rc.tomb + __popc(tb);
+                  __syncwarp();  // key and room words
+                  if (act) {  // the nodes that still accept enter the front of block c + 1, round by round
+                    for (int r = 0; r < R; ++r) {
+                      const int a = m1.ps[r * na + jd];
+                      const uint32_t rp2 = rpv[a];
+                      if ((rp2 & 0xFFFF) != 0 && !(rp2 & kRpDead)) insert_front(a, c + 1, hs->key[a], rp2);
+                    }
+                    cnt_d += R;
+                  }
+                } else {
+                  fr_used |= __reduce_or_sync(FULL, act ? 1u << vi_s : 0u);
+                  unsigned m = okm;  // pod L: round L / na, the (L % na)-th domain in id order
+                  for (int j = L % na; j > 0; --j) m &= m - 1;
+                  const int d = __ffs(m) - 1;
+                  const int vi = __shfl_sync(FULL, vi_s, d);
+                  if (L < np) {  // NewNode + Add replayed from the variant of the domain
+                    const RunVariant& v = rc.var[vi];
+                    const int n = lnew + L, a = lact + L;
+                    for (int j = 0; j < n_host; ++j) {
+                      const int times = rc.h_times[j];
+                      hc[j * kTopoCap + a] = (uint16_t)times;
+                      if (times) s.grp_host[(size_t)rc.h_row[j] * hstride + NE + n] = (uint16_t)times;
+                    }
+                    hs->key[a] = order_key(1, ltick + L + 1);
+#pragma unroll
+                    for (int r = 0; r < kHotRes; ++r) { hs->q[r][a] = v.q[r]; hs->bound[r][a] = v.b1[r]; hs->bound2[r][a] = v.b2[r]; }
+                    hs->node[a] = n;
+                    hs->flags[a] = v.fl;
+                    hs->absorbed[a] = simple ? cls : KSCHED_NONE;
+                    hs->rejected[a] = KSCHED_NONE;
+                    rpv[a] = v.rp;
+                    rc.q_node[buf][li + L] = NE + n;
+                    zv[a] = (1u << d) | (3u << 16);
+                    m1.fr[nfr + L] = (uint32_t)a | ((uint32_t)vi << 16);
+                  }
+                  if (L < n_host && rc.h_times[L]) rc.h_inc[L] = rc.h_inc[L] + np;
+                  if (act) cnt_d += R;
+                  lnew += np;
+                  lact += np;
+                  nfr += np;
+                }
+#ifdef KSCHED_PROFILE_PACK
+                if (L == 0) { s.counters[61] += clock64() - it0; s.counters[62] += 1; s.counters[63] += np; }
+#endif
+                ltick += np;
+                li += np;
+                __syncwarp();
+                continue;
+              }
               const unsigned hi = hd ? (unsigned)(hk >> 32) : 0u;
               const unsigned mhi = __reduce_max_sync(FULL, hi);
               const unsigned mlo = __reduce_max_sync(FULL, (hd && hi == mhi) ? (unsigned)hk : 0u);
@@ -2093,32 +2239,8 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
                   const int c = (int)(hk >> 32);
                   const int mytick = ltick + rank;
                   pop_head(c);
-                  uint32_t rp2 = rp - 1 + (1u << 16);
-                  for (int j = 0; j < n_host; ++j) {  // Topology.Record, hostname groups
-                    const int times = rc.h_times[j];
-                    const int old = hc[j * kTopoCap + a];
-                    const int now = old + times > 0xFFFF ? 0xFFFF : old + times;
-                    if (times) hc[j * kTopoCap + a] = (uint16_t)now;
-                    if (now > rc.h_lim[j]) rp2 |= kRpDead;
-                  }
-                  const unsigned long long nkey = order_key(c + 1, -(mytick + 1));
-                  unsigned long long skey = nkey;
-                  rc.q_node[buf][li + rank] = -(a + 2);
-                  if ((rp2 & 0xFFFF) == 0) {  // the class no longer fits by resources: does anything? (node_closed)
-                    const int placed = (rp2 >> 16) & 0x7FFF;
-                    long long nq[kHotRes], cb1[kHotRes], cb2[kHotRes];
-#pragma unroll
-                    for (int r = 0; r < kHotRes; ++r) { nq[r] = hs->q[r][a] + placed * p_req[r]; cb1[r] = hs->bound[r][a]; cb2[r] = hs->bound2[r][a]; }
-                    const unsigned short fl = (unsigned short)(hs->flags[a] | ((p_res & 0xF) << 1));
-                    if (node_closed(nq, min_req, RH, cb1, cb2, fl)) {
-                      skey = ~0ull;
-                      hs->nn_last[a] = ((unsigned long long)(unsigned)(c + 1) << 32) | (unsigned)(-(mytick + 1));
-                      closed_l = true;
-                    }
-                  }
-                  hs->key[a] = skey;
-                  rpv[a] = rp2;
-                  if ((rp2 & 0xFFFF) != 0 && !(rp2 & kRpDead)) insert_front(a, c + 1, nkey, rp2);
+                  const uint32_t rp2 = commit_round(a, rp, c, mytick, li + rank, closed_l);
+                  if ((rp2 & 0xFFFF) != 0 && !(rp2 & kRpDead)) insert_front(a, c + 1, order_key(c + 1, -(mytick + 1)), rp2);
                   ++cnt_d;
                 } else if (act) {  // NewNode + Add replayed from the variant of this lane's domain
                   const RunVariant& v = rc.var[vi_l];
@@ -2148,6 +2270,9 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
                 if (nf && L < n_host && rc.h_times[L]) rc.h_inc[L] = rc.h_inc[L] + nf;
                 const unsigned tb = __ballot_sync(FULL, closed_l);
                 if (L == 0 && tb) rc.tomb = rc.tomb + __popc(tb);
+#ifdef KSCHED_PROFILE_PACK
+                if (L == 0) { s.counters[61] += clock64() - it0; s.counters[62] += 1; s.counters[63] += na; }
+#endif
                 lnew += nf;
                 lact += nf;
                 nfr += nf;

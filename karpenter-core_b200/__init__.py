@@ -305,7 +305,7 @@ class Scheduler:
 
     def solve(self, candidates=(), count_visited=True):
         """count_visited=False is the production setting: the exact nodes_visited statistic is dropped and the pack
-        kernel may use its steady-state paths (register-resident warp loop, block-wide fast path)."""
+        kernel may use its steady-state paths (failure memo, class run, existing-node run)."""
         lib().kh_set_count_visited(int(count_visited))
         res = Result()
         arr, n = _cand_array(list(candidates))

@@ -1144,9 +1144,7 @@ static int run_pack(ksched_handle* h) {
   const size_t smem = sizeof(HotSmem) + (size_t)s.run_off + kRunArrayBytes;
   s.any_limits = 0;
   for (const ksched_template& tm : h->h_templates) if (tm.has_limits && tm.limit_present) s.any_limits = 1;
-  s.use_warp_loop = getenv("KSCHED_WARPLOOP") ? 1 : 0;  // superseded by the class-run loop (kept for A/B timing)
   s.use_class_run = getenv("KSCHED_NO_CLASSRUN") ? 0 : 1;
-  s.use_level_step = std::getenv("KSCHED_NO_LEVELSTEP") ? 0 : 1;
   s.use_level_run = std::getenv("KSCHED_NO_LEVELRUN") ? 0 : 1;
   s.use_mask_run = std::getenv("KSCHED_NO_MASKRUN") ? 0 : 1;
   s.use_level_warp = std::getenv("KSCHED_NO_LEVELWARP") ? 0 : 1;

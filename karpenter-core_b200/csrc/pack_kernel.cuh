@@ -1,9 +1,10 @@
 // K2 — pack_kernel: Scheduler.add's sequential first-fit (scheduler.go:174-219) in one persistent CTA.
 //
 // Design (latency-bound integer work; DESIGN.md section 4 has the long form):
-//  * one CTA (128..512 threads), one pod per iteration, three speeds: a register-resident warp loop when at most 32
-//    nodes are open and the pod cannot change any requirement (warp_resident_loop), a block-wide fast path over the
-//    shared-memory window of open nodes, and the out-of-line generic step (existing nodes, requirement / topology
+//  * one CTA (128..512 threads), four modes: the failure memo (pods of the class that has just failed are requeued in
+//    one step), the class run over the shared-memory window of open nodes (consecutive pods of one class whose accept
+//    test is exact there; class_run), the existing-node run (identical plain pods fill the existing nodes in one
+//    prefix-sum pass; existing_run), and the out-of-line generic step (existing nodes, requirement / topology
 //    evaluation, fresh nodes, relaxation);
 //  * candidate nodes are examined one per thread and the reference's scan order is recovered by an argmin over
 //    (pod count, stable tie-break) = the position under sort.Slice(newNodes, len(Pods)<) treated as a stable sort;
@@ -1175,174 +1176,9 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
     }
   }
 
-// ---- register-resident steady state -----------------------------------------------------------------------------
-// When at most 32 in-flight nodes are open, warp 0 keeps one node per lane IN REGISTERS and places consecutive
-// "plain" pods (no requirement can change, no host ports) without touching shared or global node state: R compares per
-// lane, a 2-REDUX argmin, the winning lane updates its own registers. The other warps wait at a block barrier.
-struct WarpIO {
-  int qi, head, qlen, tick, seq, n_active;
-  long long add_calls;
-};
-
+// no requirement of the pod can change a node's requirements
 __device__ __forceinline__ bool plain_pod_regs(const PodRegs& r) {
   return ((r.meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF) == 0 && r.itype == KSCHED_NONE && r.hostname == KSCHED_NONE && r.topo_begin == r.topo_end;
-}
-// topology-free, no host ports, resources within the hot vectors: the requirement verdict memo applies
-__device__ __forceinline__ bool simple_pod_regs(const PodRegs& r) {
-  return r.topo_begin == r.topo_end && r.hpc == 0 && r.hpe == 0 && (r.res >> kHotRes) == 0;
-}
-
-__device__ __noinline__ void warp_resident_loop(WarpIO* io) {
-  KS_K2
-  HotSmem* hs = reinterpret_cast<HotSmem*>(dyn_smem);
-  const uint32_t* tmpl_taintset = g_tmpl_taintset;
-  const int lane = threadIdx.x & 31;
-  const int NE = s.n_existing, MAXN = s.max_new;
-  const int RH = c.n_res < kHotRes ? c.n_res : kHotRes;
-  const int qcap = s.n_pods + 1;
-  int qi = io->qi, head = io->head, qlen = io->qlen, tick = io->tick, seq = io->seq;
-  long long add_calls = io->add_calls;
-  const int n_active = io->n_active;
-  // lane state
-  bool live = lane < n_active, dirty = false;
-  unsigned long long key = live ? hs->key[lane] : ~0ull;
-  long long q[kHotRes], b[kHotRes], b2[kHotRes];
-#pragma unroll
-  for (int r = 0; r < kHotRes; ++r) { q[r] = live ? hs->q[r][lane] : 0; b[r] = live ? hs->bound[r][lane] : 0; b2[r] = live ? hs->bound2[r][lane] : 0; }
-  const int node = live ? hs->node[lane] : 0;
-  unsigned short fl = live ? hs->flags[lane] : 0;
-  unsigned absorbed = live ? hs->absorbed[lane] : KSCHED_NONE, rejected = live ? hs->rejected[lane] : KSCHED_NONE;
-  const ksched_pod_row* ffd_rows = reinterpret_cast<const ksched_pod_row*>(s.rows);
-  // Consecutive pods of the queue usually belong to the same class (identical row): only the next pod's id and class are
-  // prefetched; the row's words are reloaded on a class change.
-  PodRegs cur = load_pod_regs(ffd_rows + qi, s.order[qi]);
-  uint32_t npod = 0;
-  uint64_t ncls = ~0ull;
-  if (qi + 1 < s.n_pods) { npod = s.order[qi + 1]; ncls = ffd_rows[qi + 1].reserved; }
-  long long min_req[kHotRes];
-#pragma unroll
-  for (int r = 0; r < kHotRes; ++r) min_req[r] = r < RH ? s.min_req[r] : 0;
-
-  while (true) {
-    if (!simple_pod_regs(cur) || class_ext(s, (unsigned)cur.cls64)) break;  // this pod takes the block-wide path
-    const bool plain = plain_pod_regs(cur);
-    const unsigned cls = (unsigned)cur.cls64;
-    const bool cand = live && rejected != cls && ((cur.tol >> tmpl_taintset[fl >> 8]) & 1);
-    const uint32_t qp = ((fl >> 1) & 0xF) | cur.res;
-    long long nq[kHotRes];
-#pragma unroll
-    for (int r = 0; r < kHotRes; ++r) nq[r] = q[r] + cur.req[r];
-    const int qf = cand ? quick_fit(nq, qp, RH, b, b2, fl) : 0;
-    const bool ok = qf != 0;
-    // a candidate whose resource test is not exact, or whose requirement verdict for this class is unknown, needs the full check
-    if (__any_sync(0xffffffffu, ok && (qf == 2 || !(plain || absorbed == cls)))) break;
-    const unsigned long long wkey = warp_min_u64(ok ? key : ~0ull);
-    if (wkey == ~0ull) break;  // nobody accepts: a new node has to be opened
-    // ---- level step. The accepting nodes with the FEWEST pods (count L) take the next pods one each, in tie order: a node
-    // that accepts moves to the front of block L+1 (scheduler.go:183 re-sort), i.e. behind every node still in block L. With
-    // t identical pods ahead, the first t members of the block take them - t iterations of this loop in one.
-    const unsigned members = __ballot_sync(0xffffffffu, ok && (key >> 32) == (wkey >> 32));
-    if (s.use_level_step && (members & (members - 1)) && ncls == cur.cls64) {
-      const bool same = qi + lane < s.n_pods && (lane == 0 || ffd_rows[qi + lane].reserved == cur.cls64);
-      const unsigned sm = __ballot_sync(0xffffffffu, same);
-      const int run_len = sm == 0xffffffffu ? 32 : __ffs(~sm) - 1;
-      const int k = __popc(members);
-      const int t = k < run_len ? k : run_len;
-      if (t > 1) {
-        int rank = 0;
-        for (unsigned mm = members; mm; mm &= mm - 1) {
-          const unsigned long long k2 = __shfl_sync(0xffffffffu, key, __ffs(mm) - 1);
-          rank += k2 < key ? 1 : 0;
-        }
-        if (((members >> lane) & 1) && rank < t) {
-          const uint32_t pod = s.order[qi + rank];
-#pragma unroll
-          for (int r = 0; r < kHotRes; ++r) q[r] = nq[r];
-          const int count = (int)(wkey >> 32) + 1;
-          key = order_key(count, -(tick + 1 + rank));
-          if ((cur.res & 0xF) & ~((fl >> 1) & 0xF)) {
-            s.nn_req_present[node] |= cur.res;
-            fl |= (unsigned short)((cur.res & 0xF) << 1);
-          }
-          dirty = true;
-          rejected = KSCHED_NONE;
-          s.assign[pod] = NE + node;
-          s.place_seq[pod] = seq + rank;
-          if (node_closed(q, min_req, RH, b, b2, fl)) {  // the node leaves the active set
-            for (int r = 0; r < RH; ++r) s.nn_req[(size_t)r * MAXN + node] = q[r];
-            s.nn_count[node] = count;
-            s.nn_tb[node] = -(tick + 1 + rank);
-            live = false;
-            dirty = false;
-            key = ~0ull;
-          }
-        }
-        tick += t; seq += t; qi += t; add_calls += t;
-        head += t; if (head >= qcap) head -= qcap;
-        qlen -= t;
-        if (qi >= s.n_pods || qlen == 0) break;
-        if (run_len > t) { cur.pod = s.order[qi]; cur.row = ffd_rows + qi; }
-        else cur = load_pod_regs(ffd_rows + qi, s.order[qi]);
-        if (qi + 1 < s.n_pods) { npod = s.order[qi + 1]; ncls = ffd_rows[qi + 1].reserved; } else ncls = ~0ull;
-        if (lane == 0 && qi + 32 < s.n_pods) prefetch_l2(reinterpret_cast<const char*>(ffd_rows + qi + 32) + 128);
-        if (lane == 2 && qi + 96 < s.n_pods) prefetch_l2(s.order + qi + 96);
-        continue;
-      }
-    }
-    if (ok && key == wkey) {
-#pragma unroll
-      for (int r = 0; r < kHotRes; ++r) q[r] = nq[r];
-      const int count = (int)(wkey >> 32) + 1;
-      key = order_key(count, -(tick + 1));
-      if ((cur.res & 0xF) & ~((fl >> 1) & 0xF)) {
-        s.nn_req_present[node] |= cur.res;
-        fl |= (unsigned short)((cur.res & 0xF) << 1);
-      }
-      dirty = true;
-      rejected = KSCHED_NONE;
-      s.assign[cur.pod] = NE + node;
-      s.place_seq[cur.pod] = seq;
-      const bool closed = node_closed(q, min_req, RH, b, b2, fl);
-      if (closed) {  // the node leaves the active set
-        for (int r = 0; r < RH; ++r) s.nn_req[(size_t)r * MAXN + node] = q[r];
-        s.nn_count[node] = count;
-        s.nn_tb[node] = -(tick + 1);
-        live = false;
-        dirty = false;
-        key = ~0ull;
-      }
-    }
-    ++tick; ++seq; ++qi; ++add_calls;
-    head = head + 1 == qcap ? 0 : head + 1;
-    --qlen;
-    if (qi >= s.n_pods || qlen == 0) break;
-    if (ncls == cur.cls64) { cur.pod = npod; cur.row = ffd_rows + qi; }
-    else cur = load_pod_regs(ffd_rows + qi, npod);
-    if (qi + 1 < s.n_pods) { npod = s.order[qi + 1]; ncls = ffd_rows[qi + 1].reserved; }
-    if (lane == 0 && qi + 32 < s.n_pods) prefetch_l2(reinterpret_cast<const char*>(ffd_rows + qi + 32) + 128);  // the line holding `reserved`
-    if (lane == 2 && (qi & 31) == 0 && qi + 96 < s.n_pods) prefetch_l2(s.order + qi + 96);
-  }
-  // write the lanes back, compacted
-  const unsigned livemask = __ballot_sync(0xffffffffu, live);
-  const int slot = __popc(livemask & ((1u << lane) - 1));
-  __syncwarp();
-  if (live) {
-    hs->key[slot] = key;
-#pragma unroll
-    for (int r = 0; r < kHotRes; ++r) { hs->q[r][slot] = q[r]; hs->bound[r][slot] = b[r]; hs->bound2[r][slot] = b2[r]; }
-    hs->node[slot] = node;
-    hs->flags[slot] = fl;
-    hs->absorbed[slot] = absorbed;
-    hs->rejected[slot] = rejected;
-    if (dirty) {
-      s.nn_count[node] = (int)(key >> 32);
-      s.nn_tb[node] = (int)((unsigned)key ^ 0x80000000u);
-    }
-  }
-  if (lane == 0) {
-    io->qi = qi; io->head = head; io->qlen = qlen; io->tick = tick; io->seq = seq; io->n_active = __popc(livemask);
-    io->add_calls = add_calls;
-  }
 }
 
 // ---- class-run loop ------------------------------------------------------------------------------------------------
@@ -1524,7 +1360,7 @@ constexpr int kM1Lv = 12;             // pod counts < kM1Lv
 constexpr uint16_t kM1None = 0xFFFF;
 struct M1Ctx {
   uint16_t tl[kM1Lv][kM1Lists];       // last node of the bucket (kM1None: empty)
-  uint16_t head[kM1Lists];            // first node of the list (between two entries of the warp loop)
+  uint16_t head[kM1Lists];            // first node of the list (between two entries of the mask run)
   uint16_t ap[kM1Lv][kM1Lists];       // build: the bucket is arr[ap .. ae)
   uint16_t ae[kM1Lv][kM1Lists];
   union {
@@ -1537,7 +1373,7 @@ struct M1Ctx {
                                       // segment the build sorted, and the pin step reads its next members without the links
   uint16_t ps[32];                    // pin step: the node of each pod; round stretch: the node of each (round, domain)
   int out_adv, out_reason, out_tick, out_n_new, out_n_active;
-  int n_fresh;                        // nodes created by this entry of the warp loop: slot | variant << 16; their global
+  int n_fresh;                        // nodes created by this entry of the mask run: slot | variant << 16; their global
   uint32_t fr[kRunChunk];             // state (option words, requirement values, requests, ...) is stored by the CTA afterwards
 };
 __shared__ M1Ctx g_m1;
@@ -1587,6 +1423,32 @@ __device__ __noinline__ unsigned run_room(const HotSmem* hs, int a, const long l
   }
   if (!(fl & kFlExact)) return inexact_ok ? kRoomSlow : 0;  // per-resource maxima only: a necessary test
   return (unsigned)best;
+}
+// A commit's Topology.Record for the class's hostname groups: t more pods on the node at slot a (counters saturate at
+// 0xFFFF). Returns the room word rp with t pods moved from room to placed, dead once a group no longer admits the node.
+__device__ __forceinline__ uint32_t run_record_host(const RunCtx& rc, uint16_t* hc, int n_host, int a, uint32_t rp, int t) {
+  uint32_t rp2 = rp - (uint32_t)t + ((uint32_t)t << 16);
+#pragma unroll
+  for (int j = 0; j < kRunHost; ++j) {
+    if (j >= n_host) break;
+    const int times = rc.h_times[j];
+    const int old = hc[j * kTopoCap + a];
+    const int now = old + t * times > 0xFFFF ? 0xFFFF : old + t * times;
+    if (times) hc[j * kTopoCap + a] = (uint16_t)now;
+    if (now > rc.h_lim[j]) rp2 |= kRpDead;
+  }
+  return rp2;
+}
+// A commit left the node at slot a no room for the class (room word rp, room 0): true when no pod of the batch fits it
+// any more either (node_closed on the run's start requests plus the placed pods) - the node leaves the active set. The
+// callers test the room first, in their own condition: a bool merged from an early return here costs the one-warp
+// level / fill loop a branch and a convergence barrier per commit.
+__device__ __forceinline__ bool run_closes(const HotSmem* hs, int a, uint32_t rp, const long long* p_req, const long long* min_req, int RH) {
+  const int placed = (rp >> 16) & 0x7FFF;
+  long long nq[kHotRes], b1[kHotRes], b2[kHotRes];
+#pragma unroll
+  for (int r = 0; r < kHotRes; ++r) { nq[r] = hs->q[r][a] + placed * p_req[r]; b1[r] = hs->bound[r][a]; b2[r] = hs->bound2[r][a]; }
+  return node_closed(nq, min_req, RH, b1, b2, hs->flags[a]);
 }
 
 __device__ __noinline__ void class_run(const PodRegs& first_in) {
@@ -2035,27 +1897,13 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
         // a round's commit of one pod on the pinned node a (pod count c, room word rp) with tick mytick, staged entry q:
         // Topology.Record, the node's new key and room word (returned); closed: the class no longer fits anywhere on it
         auto commit_round = [&](int a, uint32_t rp, int c, int mytick, int q, bool& closed) -> uint32_t {
-          uint32_t rp2 = rp - 1 + (1u << 16);
-          for (int j = 0; j < n_host; ++j) {  // Topology.Record, hostname groups
-            const int times = rc.h_times[j];
-            const int old = hc[j * kTopoCap + a];
-            const int now = old + times > 0xFFFF ? 0xFFFF : old + times;
-            if (times) hc[j * kTopoCap + a] = (uint16_t)now;
-            if (now > rc.h_lim[j]) rp2 |= kRpDead;
-          }
+          const uint32_t rp2 = run_record_host(rc, hc, n_host, a, rp, 1);
           unsigned long long skey = order_key(c + 1, -(mytick + 1));
           rc.q_node[buf][q] = -(a + 2);
-          if ((rp2 & 0xFFFF) == 0) {  // the class no longer fits by resources: does anything? (node_closed)
-            const int placed = (rp2 >> 16) & 0x7FFF;
-            long long nq[kHotRes], cb1[kHotRes], cb2[kHotRes];
-#pragma unroll
-            for (int r = 0; r < kHotRes; ++r) { nq[r] = hs->q[r][a] + placed * p_req[r]; cb1[r] = hs->bound[r][a]; cb2[r] = hs->bound2[r][a]; }
-            const unsigned short fl = (unsigned short)(hs->flags[a] | ((p_res & 0xF) << 1));
-            if (node_closed(nq, min_req, RH, cb1, cb2, fl)) {
-              skey = ~0ull;
-              hs->nn_last[a] = ((unsigned long long)(unsigned)(c + 1) << 32) | (unsigned)(-(mytick + 1));
-              closed = true;
-            }
+          if ((rp2 & 0xFFFF) == 0 && run_closes(hs, a, rp2, p_req, min_req, RH)) {
+            skey = ~0ull;
+            hs->nn_last[a] = ((unsigned long long)(unsigned)(c + 1) << 32) | (unsigned)(-(mytick + 1));
+            closed = true;
           }
           hs->key[a] = skey;
           rpv[a] = rp2;
@@ -2336,14 +2184,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
                 bool closed_l = false;
                 if (L < J) {  // the single step's commit for pod L on node a_t, pinned to d_t
                   const int a = a_t, mytick = ltick + L;
-                  uint32_t rp2 = rp_t - 1 + (1u << 16);
-                  for (int j = 0; j < n_host; ++j) {  // Topology.Record, hostname groups
-                    const int times = rc.h_times[j];
-                    const int old = hc[j * kTopoCap + a];
-                    const int now = old + times > 0xFFFF ? 0xFFFF : old + times;
-                    if (times) hc[j * kTopoCap + a] = (uint16_t)now;
-                    if (now > rc.h_lim[j]) rp2 |= kRpDead;
-                  }
+                  const uint32_t rp2 = run_record_host(rc, hc, n_host, a, rp_t, 1);
                   const int n = hs->node[a], k = rc.m_key[0];
                   zv[a] = (1u << d_t) | (3u << 16);
                   s.nn_vals[(size_t)k * MAXN + n] = 1ull << d_t;
@@ -2351,17 +2192,10 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
                   atomicAnd(reinterpret_cast<unsigned long long*>(&s.nn_meta[n]), ~(1ull << (KSCHED_META_COMPLEMENT_SHIFT + k)));
                   rc.q_node[buf][li + L] = -(a + 2);
                   unsigned long long skey = order_key(c + 1, -(mytick + 1));
-                  if ((rp2 & 0xFFFF) == 0) {  // the class no longer fits by resources: does anything? (node_closed)
-                    const int placed = (rp2 >> 16) & 0x7FFF;
-                    long long nq[kHotRes], cb1[kHotRes], cb2[kHotRes];
-#pragma unroll
-                    for (int r = 0; r < kHotRes; ++r) { nq[r] = hs->q[r][a] + placed * p_req[r]; cb1[r] = hs->bound[r][a]; cb2[r] = hs->bound2[r][a]; }
-                    const unsigned short fl = (unsigned short)(hs->flags[a] | ((p_res & 0xF) << 1));
-                    if (node_closed(nq, min_req, RH, cb1, cb2, fl)) {
-                      skey = ~0ull;
-                      hs->nn_last[a] = ((unsigned long long)(unsigned)(c + 1) << 32) | (unsigned)(-(mytick + 1));
-                      closed_l = true;
-                    }
+                  if ((rp2 & 0xFFFF) == 0 && run_closes(hs, a, rp2, p_req, min_req, RH)) {
+                    skey = ~0ull;
+                    hs->nn_last[a] = ((unsigned long long)(unsigned)(c + 1) << 32) | (unsigned)(-(mytick + 1));
+                    closed_l = true;
                   }
                   hs->key[a] = skey;
                   rpv[a] = rp2;
@@ -2442,17 +2276,10 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
                 atomicAnd(reinterpret_cast<unsigned long long*>(&s.nn_meta[n]), ~(1ull << (KSCHED_META_COMPLEMENT_SHIFT + k)));
               }
               rc.q_node[buf][li] = -(a + 2);  // the slot: translated to the node when the chunk is stored
-              if ((rp2 & 0xFFFF) == 0) {  // the class no longer fits by resources: does anything? (node_closed)
-                const int placed = (rp2 >> 16) & 0x7FFF;
-                long long nq[kHotRes], cb1[kHotRes], cb2[kHotRes];
-#pragma unroll
-                for (int r = 0; r < kHotRes; ++r) { nq[r] = hs->q[r][a] + placed * p_req[r]; cb1[r] = hs->bound[r][a]; cb2[r] = hs->bound2[r][a]; }
-                const unsigned short fl = (unsigned short)(hs->flags[a] | ((p_res & 0xF) << 1));
-                if (node_closed(nq, min_req, RH, cb1, cb2, fl)) {
-                  skey = ~0ull;
-                  hs->nn_last[a] = ((unsigned long long)(unsigned)(c + 1) << 32) | (unsigned)(-(ltick + 1));
-                  rc.tomb = rc.tomb + 1;
-                }
+              if ((rp2 & 0xFFFF) == 0 && run_closes(hs, a, rp2, p_req, min_req, RH)) {
+                skey = ~0ull;
+                hs->nn_last[a] = ((unsigned long long)(unsigned)(c + 1) << 32) | (unsigned)(-(ltick + 1));
+                rc.tomb = rc.tomb + 1;
               }
               hs->key[a] = skey;
               rpv[a] = rp2;
@@ -2528,7 +2355,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
         if (L == 0) { m1.out_adv = li - i; m1.out_reason = reason; m1.out_tick = ltick; m1.out_n_new = lnew; m1.out_n_active = lact; m1.n_fresh = nfr; }
       }
       __syncthreads();
-      {  // the global state of the nodes the warp loop created, 64 words per node across the CTA
+      {  // the global state of the nodes the mask run created, 64 words per node across the CTA
         const int nfr = m1.n_fresh;
         for (int e = tid; e < nfr * 64; e += T) {
           const uint32_t rec = m1.fr[e >> 6];
@@ -2610,30 +2437,16 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
             adv_w = n_s < k_av ? n_s : k_av;
           }
           if (mem && rank < adv_w) {  // (fill: rank 0 < t)
-            uint32_t rp2 = rp - (uint32_t)t + ((uint32_t)t << 16);
-            for (int j = 0; j < n_host; ++j) {  // Topology.Record, hostname groups
-              const int times = rc.h_times[j];
-              const int old = hc[j * kTopoCap + a];
-              const int now = old + t * times > 0xFFFF ? 0xFFFF : old + t * times;
-              if (times) hc[j * kTopoCap + a] = (uint16_t)now;
-              if (now > rc.h_lim[j]) rp2 |= kRpDead;
-            }
+            const uint32_t rp2 = run_record_host(rc, hc, n_host, a, rp, t);
             const int count = (int)c_min + t;
             const int tb = -(ltick + rank + t);
             unsigned long long nkey = order_key(count, tb);
             const int nd = NE + hs->node[a];
             for (int e = 0; e < t; ++e) rc.q_node[buf][li + rank + e] = nd;
-            if ((rp2 & 0xFFFF) == 0) {  // the class no longer fits by resources: does anything? (node_closed)
-              const int placed = (rp2 >> 16) & 0x7FFF;
-              long long nq[kHotRes], cb1[kHotRes], cb2[kHotRes];
-#pragma unroll
-              for (int r = 0; r < kHotRes; ++r) { nq[r] = hs->q[r][a] + placed * p_req[r]; cb1[r] = hs->bound[r][a]; cb2[r] = hs->bound2[r][a]; }
-              const unsigned short fl = (unsigned short)(hs->flags[a] | ((p_res & 0xF) << 1));
-              if (node_closed(nq, min_req, RH, cb1, cb2, fl)) {
-                nkey = ~0ull;
-                hs->nn_last[a] = ((unsigned long long)(unsigned)count << 32) | (unsigned)tb;
-                atomicAdd(&rc.tomb, 1);
-              }
+            if ((rp2 & 0xFFFF) == 0 && run_closes(hs, a, rp2, p_req, min_req, RH)) {
+              nkey = ~0ull;
+              hs->nn_last[a] = ((unsigned long long)(unsigned)count << 32) | (unsigned)tb;
+              atomicAdd(&rc.tomb, 1);
             }
             hs->key[a] = nkey;
             rpv[a] = rp2;
@@ -2747,30 +2560,16 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
             }
             // the owner commits: pods i + rank .. i + rank + t - 1 of the chunk
             const int t = t_fill;
-            uint32_t rp2 = rp - (uint32_t)t + ((uint32_t)t << 16);
-            for (int j = 0; j < n_host; ++j) {  // Topology.Record, hostname groups
-              const int times = rc.h_times[j];
-              const int old = hc[j * kTopoCap + a];
-              const int now = old + t * times > 0xFFFF ? 0xFFFF : old + t * times;
-              if (times) hc[j * kTopoCap + a] = (uint16_t)now;
-              if (now > rc.h_lim[j]) rp2 |= kRpDead;
-            }
+            const uint32_t rp2 = run_record_host(rc, hc, n_host, a, rp, t);
             const int count = (int)c_min + t;
             const int tb = -(tick + rank + t);
             unsigned long long nkey = order_key(count, tb);
             const int nd = NE + hs->node[a];
             for (int e = 0; e < t; ++e) rc.q_node[buf][i + rank + e] = nd;
-            if ((rp2 & 0xFFFF) == 0) {  // the class no longer fits by resources: does anything? (node_closed)
-              const int placed = (rp2 >> 16) & 0x7FFF;
-              long long nq[kHotRes], cb1[kHotRes], cb2[kHotRes];
-#pragma unroll
-              for (int r = 0; r < kHotRes; ++r) { nq[r] = hs->q[r][a] + placed * p_req[r]; cb1[r] = hs->bound[r][a]; cb2[r] = hs->bound2[r][a]; }
-              const unsigned short fl = (unsigned short)(hs->flags[a] | ((p_res & 0xF) << 1));
-              if (node_closed(nq, min_req, RH, cb1, cb2, fl)) {
-                nkey = ~0ull;
-                hs->nn_last[a] = ((unsigned long long)(unsigned)count << 32) | (unsigned)tb;
-                atomicAdd(&rc.tomb, 1);
-              }
+            if ((rp2 & 0xFFFF) == 0 && run_closes(hs, a, rp2, p_req, min_req, RH)) {
+              nkey = ~0ull;
+              hs->nn_last[a] = ((unsigned long long)(unsigned)count << 32) | (unsigned)tb;
+              atomicAdd(&rc.tomb, 1);
             }
             hs->key[a] = nkey;
             rpv[a] = rp2;
@@ -2854,18 +2653,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
       fd1 = (wp >> 19) & 0xF;
       if (mine == wkey) {  // the owner commits its node: a handful of shared-memory stores
         const int a = best_a;
-        uint32_t rp = best_rp - 1 + (1u << 16);
-        bool host_first = false;
-#pragma unroll
-        for (int j = 0; j < kRunHost; ++j) {  // Topology.Record, hostname groups
-          if (j >= n_host) continue;
-          const int times = rc.h_times[j];
-          const int old = hc[j * kTopoCap + a];
-          const int now = old + times > 0xFFFF ? 0xFFFF : old + times;
-          if (times) hc[j * kTopoCap + a] = (uint16_t)now;
-          if (now > rc.h_lim[j]) rp |= kRpDead;  // no further pod of the class here
-          host_first = host_first || (times && old == 0);
-        }
+        const uint32_t rp = run_record_host(rc, hc, n_host, a, best_rp, 1);
         if (pay & (3u << 13)) {  // requirements.Add(In{d}) on the node: once per node and key
           const int n = hs->node[a];
           for (int j = 0; j < n_mask; ++j) {
@@ -2879,21 +2667,13 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
         const int count = (int)(wkey >> 32) + 1;
         unsigned long long nkey = order_key(count, -(tick + 1));
         rc.q_node[buf][i] = NE + hs->node[a];
-        if ((rp & 0xFFFF) == 0) {  // the class no longer fits by resources: does anything? (node_closed)
-          const int placed = (rp >> 16) & 0x7FFF;
-          long long nq[kHotRes], cb1[kHotRes], cb2[kHotRes];
-#pragma unroll
-          for (int r = 0; r < kHotRes; ++r) { nq[r] = hs->q[r][a] + placed * p_req[r]; cb1[r] = hs->bound[r][a]; cb2[r] = hs->bound2[r][a]; }
-          const unsigned short fl = (unsigned short)(hs->flags[a] | ((p_res & 0xF) << 1));
-          if (node_closed(nq, min_req, RH, cb1, cb2, fl)) {  // leaves the active set: tombstone, compacted when the run ends
-            nkey = ~0ull;
-            hs->nn_last[a] = ((unsigned long long)(unsigned)count << 32) | (unsigned)(-(tick + 1));
-            rc.tomb = rc.tomb + 1;
-          }
+        if ((rp & 0xFFFF) == 0 && run_closes(hs, a, rp, p_req, min_req, RH)) {  // tombstone, compacted when the run ends
+          nkey = ~0ull;
+          hs->nn_last[a] = ((unsigned long long)(unsigned)count << 32) | (unsigned)(-(tick + 1));
+          rc.tomb = rc.tomb + 1;
         }
         hs->key[a] = nkey;
         rpv[a] = rp;
-        (void)host_first;
       }
       if (n_mask > 0) {  // every warp keeps its copy of the spread counters in step (the node's domain is the single value d)
         if (lane == 0) {
@@ -3000,16 +2780,11 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
           if (t > 0 && now > rc.h_lim[jj]) rp2 |= kRpDead;
         }
         unsigned long long nkey = t > 0 ? order_key(1 + t, -(tk + 1 + t)) : order_key(1, tk + 1);
-        if (t > 0 && (rp2 & 0xFFFF) == 0) {  // full for the class: closed for every class? (same test as the accept that fills a node)
-          long long nq[kHotRes], cb1[kHotRes], cb2[kHotRes];
-#pragma unroll
-          for (int r = 0; r < kHotRes; ++r) { nq[r] = v.q[r] + t * p_req[r]; cb1[r] = v.b1[r]; cb2[r] = v.b2[r]; }
-          const unsigned short fl = (unsigned short)(v.fl | ((p_res & 0xF) << 1));
-          if (node_closed(nq, min_req, RH, cb1, cb2, fl)) {
-            nkey = ~0ull;
-            hs->nn_last[a] = ((unsigned long long)(unsigned)(1 + t) << 32) | (unsigned)(-(tk + 1 + t));
-            atomicAdd(&rc.tomb, 1);
-          }
+        // (the slot holds the variant's requests and front, and rp2 has t pods placed: v.rp carries none)
+        if (t > 0 && (rp2 & 0xFFFF) == 0 && run_closes(hs, a, rp2, p_req, min_req, RH)) {
+          nkey = ~0ull;
+          hs->nn_last[a] = ((unsigned long long)(unsigned)(1 + t) << 32) | (unsigned)(-(tk + 1 + t));
+          atomicAdd(&rc.tomb, 1);
         }
         hs->key[a] = nkey;
         rpv[a] = rp2;
@@ -3136,7 +2911,6 @@ __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
 
   PodTopo& pt = g_pt;
   uint32_t* tmpl_taintset = g_tmpl_taintset;
-  __shared__ WarpIO wio;
   for (int v = tid; v < c.n_templates; v += blockDim.x) tmpl_taintset[v] = c.templates[v].taintset;
   if (tid == 0) { pt.n = 0; g_rc.cls = KSCHED_NONE; g_rc.eligible = 0; g_rc.vs_n = 0; }
 
@@ -3206,19 +2980,6 @@ __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
         if (qi < s.n_pods) nxt = load_pod_regs(ffd_rows + qi, s.order[qi]);
         continue;
       }
-    }
-    // ---- register-resident mode (see warp_resident_loop): entered when the next pod is plain and <= 32 nodes are open
-    if (fast_allowed && s.use_warp_loop && !fresh_valid && qi < s.n_pods && n_active > 0 && n_active <= 32 && simple_pod_regs(nxt) &&
-        !(kExt && class_ext(s, (unsigned)nxt.cls64))) {
-      __syncthreads();
-      if (tid == 0) { wio.qi = qi; wio.head = head; wio.qlen = qlen; wio.tick = tick; wio.seq = seq; wio.n_active = n_active; wio.add_calls = add_calls; }
-      __syncthreads();
-      if (tid < 32) warp_resident_loop(&wio);
-      __syncthreads();
-      qi = wio.qi; head = wio.head; qlen = wio.qlen; tick = wio.tick; seq = wio.seq; n_active = wio.n_active; add_calls = wio.add_calls;
-      if (qlen == 0) break;
-      if (qi < s.n_pods) nxt = load_pod_regs(ffd_rows + qi, s.order[qi]);
-      // the pod the warp loop stopped at (new node needed, non-plain pod, end of the first pass) takes the block-wide path
     }
     PK_T(0)
     // ---- class-run mode (see class_run): first-pass pods of a class whose accept test is exact from shared memory

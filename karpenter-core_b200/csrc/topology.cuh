@@ -105,12 +105,11 @@ struct PackState {
   int alloc_in_smem;
   int run_off;                       // byte offset (after HotSmem) of the class-run loop's per-node arrays in dynamic shared memory
   int any_limits;                    // some template has active provisioner limits (fresh nodes are then never replayed from a variant)
-  int use_warp_loop;                 // register-resident warp loop enabled (KSCHED_NO_WARPLOOP=1 turns it off for A/B timing)
-  int use_class_run;                 // class-run loop enabled (KSCHED_NO_CLASSRUN=1 turns it off for A/B timing)
-  int use_level_step;                // level step of the warp loop enabled (KSCHED_NO_LEVELSTEP=1 turns it off for A/B timing)
+  // Mode switches, read from the environment per Solve: the tests turn each step off to compare it with the generic step.
+  int use_class_run;                 // class-run loop (KSCHED_NO_CLASSRUN=1: off)
   int use_level_run;                 // class_run: level / fill steps for classes without mask-key spread (KSCHED_NO_LEVELRUN=1: off)
   int use_level_warp;                // class_run: the level / fill steps on one warp while at most 32 nodes are open (KSCHED_NO_LEVELWARP=1: off)
-  int use_mask_run;                  // class_run: list-driven warp loop for one mask-key spread relation (KSCHED_NO_MASKRUN=1: off)
+  int use_mask_run;                  // class_run: list-driven loop on warp 0 for one mask-key spread relation (KSCHED_NO_MASKRUN=1: off)
   int use_varstore;                  // class_run: fresh-node variants shared by classes of one shape (KSCHED_NO_VARSTORE=1: off)
   int use_round_stretch;             // mask run: several rounds of a zone spread in one step (KSCHED_NO_ROUNDSTRETCH=1: off)
   struct VarStoreEntry* vstore;      // [kVarStore] (pack_kernel.cuh); valid entries: RunCtx::vs_n, reset per Solve

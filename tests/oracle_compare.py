@@ -1,8 +1,25 @@
-"""The GPU path's Solve against the oracle's, field by field: shared by the GPU differential tests (test_gpu_parity,
-test_gpu_fuzz, test_gpu_runs)."""
+"""The GPU path's Solve against the oracle's, field by field, and the pack kernel's mode switches: shared by the GPU
+differential tests (test_gpu_parity, test_gpu_fuzz, test_gpu_runs, ...)."""
 import pytest
 
 INSTANCE_TYPE = "node.kubernetes.io/instance-type"
+
+# Each switch turns off one closed-form mode of the pack kernel, the class-run loop or one of its steps (read per Solve,
+# csrc/ksched.cu): the per-pod loop or the generic step then places the same pods one at a time, with the same result.
+MODE_SWITCHES = ("KSCHED_NO_CLASSRUN", "KSCHED_NO_LEVELRUN", "KSCHED_NO_LEVELWARP", "KSCHED_NO_MASKRUN", "KSCHED_NO_VARSTORE",
+                 "KSCHED_NO_ROUNDSTRETCH")
+
+
+def set_modes(monkeypatch, *specs):
+    """Clear every mode switch and KSCHED_PACK_THREADS, then set the variables the specs name: each spec is a comma-separated
+    list of NAME (set to 1) or NAME=value; empty specs set nothing."""
+    for v in MODE_SWITCHES + ("KSCHED_PACK_THREADS",):
+        monkeypatch.delenv(v, raising=False)
+    for spec in specs:
+        for kv in (spec or "").split(","):
+            if kv:
+                k, _, v = kv.partition("=")
+                monkeypatch.setenv(k, v or "1")
 
 
 def compare(pkg, oracle, problem, candidates=(), add_calls=True, refusal_skips=False):

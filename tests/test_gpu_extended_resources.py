@@ -6,27 +6,26 @@ import pytest
 
 import extended_resource_problems as xp
 import validation_oracle as vo
-from oracle_compare import compare
+from oracle_compare import MODE_SWITCHES, compare, set_modes
 
 pytestmark = pytest.mark.gpu
 
 CORPUS = xp.corpus()
 IDS = [c[0] for c in CORPUS]
-SWITCHES = ["KSCHED_NO_CLASSRUN", "KSCHED_NO_LEVELSTEP", "KSCHED_NO_LEVELRUN", "KSCHED_NO_MASKRUN", "KSCHED_NO_LEVELWARP", "KSCHED_NO_VARSTORE"]
 
 
 @pytest.mark.parametrize("threads", [32, 128, 512])
 @pytest.mark.parametrize("name,prob", CORPUS, ids=IDS)
 def test_extended_resources_equal_oracle(pkg, oracle, monkeypatch, name, prob, threads):
-    monkeypatch.setenv("KSCHED_PACK_THREADS", str(threads))
+    set_modes(monkeypatch, f"KSCHED_PACK_THREADS={threads}")
     got, _ = compare(pkg, oracle, pkg.Problem.from_dict(prob), refusal_skips=False)
     assert _ext_on_new_nodes(got) > 0
 
 
-@pytest.mark.parametrize("switch", SWITCHES)
+@pytest.mark.parametrize("switch", MODE_SWITCHES)
 @pytest.mark.parametrize("name,prob", CORPUS[::2], ids=IDS[::2])
 def test_extended_resources_with_a_step_switched_off(pkg, oracle, monkeypatch, name, prob, switch):
-    monkeypatch.setenv(switch, "1")
+    set_modes(monkeypatch, switch)
     compare(pkg, oracle, pkg.Problem.from_dict(prob), refusal_skips=False)
 
 
@@ -37,15 +36,13 @@ def _ext_on_new_nodes(got):
     return sum(1 for n in got.to_dict()["newNodes"] if any(k in xp.EXT_RESOURCES for k in n["requests"]))
 
 
-@pytest.mark.parametrize("switch", [None] + SWITCHES)
+@pytest.mark.parametrize("switch", (None,) + MODE_SWITCHES)
 @pytest.mark.parametrize("threads", [32, 128, 512])
 def test_fresh_fleets_back_to_back_equal_oracle(pkg, oracle, monkeypatch, threads, switch):
     """no existing nodes: the closed-form modes place the classes that request no ext resource and open nodes of their
     own between the generic steps of those that do. Different problems run one after the other on the same device state,
     so a node slot that keeps an earlier problem's ext sums would show."""
-    monkeypatch.setenv("KSCHED_PACK_THREADS", str(threads))
-    if switch:
-        monkeypatch.setenv(switch, "1")
+    set_modes(monkeypatch, f"KSCHED_PACK_THREADS={threads}", switch)
     for name, prob in FRESH + CORPUS[:1] + FRESH[::-1]:
         got, _ = compare(pkg, oracle, pkg.Problem.from_dict(prob), refusal_skips=False)
         assert _ext_on_new_nodes(got) > 0, name

@@ -6,27 +6,26 @@ import pytest
 
 import provisioner_problems as pp
 import validation_oracle as vo
-from oracle_compare import compare
+from oracle_compare import MODE_SWITCHES, compare, set_modes
 
 pytestmark = pytest.mark.gpu
 
 CORPUS = pp.corpus()
-SWITCHES = ["KSCHED_NO_CLASSRUN", "KSCHED_NO_LEVELSTEP", "KSCHED_NO_LEVELRUN", "KSCHED_NO_MASKRUN", "KSCHED_NO_LEVELWARP", "KSCHED_NO_VARSTORE"]
 
 
 @pytest.mark.parametrize("threads", [32, 128, 512])
 @pytest.mark.parametrize("name,prob", CORPUS, ids=[c[0] for c in CORPUS])
 def test_many_provisioners_equal_oracle(pkg, oracle, monkeypatch, name, prob, threads):
-    monkeypatch.setenv("KSCHED_PACK_THREADS", str(threads))
+    set_modes(monkeypatch, f"KSCHED_PACK_THREADS={threads}")
     got, _ = compare(pkg, oracle, pkg.Problem.from_dict(prob), refusal_skips=False)
     folded = pp.template_keys(prob) - pp.pod_side_keys(prob)
     assert any(k in n["requirements"] for n in got.to_dict()["newNodes"] for k in folded), "no folded requirement was rendered"
 
 
-@pytest.mark.parametrize("switch", SWITCHES)
+@pytest.mark.parametrize("switch", MODE_SWITCHES)
 @pytest.mark.parametrize("name,prob", CORPUS[::3], ids=[c[0] for c in CORPUS[::3]])
 def test_many_provisioners_with_a_step_switched_off(pkg, oracle, monkeypatch, name, prob, switch):
-    monkeypatch.setenv(switch, "1")
+    set_modes(monkeypatch, switch)
     compare(pkg, oracle, pkg.Problem.from_dict(prob), refusal_skips=False)
 
 

@@ -4,7 +4,7 @@ Compared per problem: the pod->node assignment vector, relaxation levels, and fo
 provisioner, pods in Add order, surviving instance-type options, requests and final requirements."""
 import pytest
 
-from oracle_compare import compare
+from oracle_compare import MODE_SWITCHES, compare, set_modes
 
 pytestmark = pytest.mark.gpu
 
@@ -143,9 +143,6 @@ def test_consolidation_known_answers_match_oracle(pkg, oracle, name, ref, build)
     check(probe, search)
 
 
-CLASS_RUN_SWITCHES = ("KSCHED_NO_LEVELWARP", "KSCHED_NO_MASKRUN", "KSCHED_NO_LEVELRUN", "KSCHED_NO_CLASSRUN", "KSCHED_NO_LEVELSTEP", "KSCHED_WARPLOOP")
-
-
 @pytest.mark.parametrize("config,pods,types,seed", [(4, 6000, 1000, 7), (4, 2500, 1000, 3), (3, 5000, 1000, 7), (2, 3000, 500, 7), (2, 4000, 40, 9)])
 def test_class_run_modes_agree(pkg, monkeypatch, config, pods, types, seed):
     """The closed-form steps of the class-run loop (level / fill steps and fresh nodes in bulk, their one-warp form, the mask
@@ -157,16 +154,10 @@ def test_class_run_modes_agree(pkg, monkeypatch, config, pods, types, seed):
     rs.set_count_visited(False)
     rs.load()
     digests = {}
-    for off in ("", "KSCHED_NO_LEVELWARP", "KSCHED_NO_MASKRUN", "KSCHED_NO_LEVELRUN,KSCHED_NO_MASKRUN", "KSCHED_NO_CLASSRUN", "KSCHED_NO_LEVELSTEP",
-                "KSCHED_WARPLOOP"):
-        for v in CLASS_RUN_SWITCHES:
-            monkeypatch.delenv(v, raising=False)
-        for v in off.split(","):
-            if v:
-                monkeypatch.setenv(v, "1")
+    for off in ("",) + MODE_SWITCHES + ("KSCHED_NO_LEVELRUN,KSCHED_NO_MASKRUN",):
+        set_modes(monkeypatch, off)
         rs.run()
         res = rs.download()
         digests[off or "all on"] = (int(res.digest()), int(res.num_new_nodes), int((res.assign >= 0).sum()))
-    for v in CLASS_RUN_SWITCHES:
-        monkeypatch.delenv(v, raising=False)
+    set_modes(monkeypatch)
     assert len(set(digests.values())) == 1, digests

@@ -5,13 +5,12 @@ mode switch of the class-run loop, and the result at every block size the pack k
 import pytest
 
 import run_problems as rp
-from oracle_compare import compare
+from oracle_compare import MODE_SWITCHES, compare, set_modes
 
 pytestmark = pytest.mark.gpu
 
 IDS = [f"{n}-{s}" for n, s in rp.CORPUS]
-SWITCHES = ("KSCHED_NO_CLASSRUN", "KSCHED_NO_LEVELRUN", "KSCHED_NO_LEVELWARP", "KSCHED_NO_MASKRUN", "KSCHED_NO_LEVELSTEP", "KSCHED_WARPLOOP")
-MODES = ("",) + SWITCHES + ("KSCHED_NO_LEVELRUN,KSCHED_NO_MASKRUN",)
+MODES = ("",) + MODE_SWITCHES + ("KSCHED_NO_LEVELRUN,KSCHED_NO_MASKRUN",)
 BLOCK_SIZES = (32, 64, 128, 256, 512)  # ksched.cu picks 128 / 256 / 512 by existing-node count; KSCHED_PACK_THREADS overrides it
 
 
@@ -27,17 +26,9 @@ def _check(res, want, label):
     assert res.digest() == want.digest(), f"{label}: same placements, different nodes (options / requests / requirements)"
 
 
-def _set_env(monkeypatch, names):
-    for v in SWITCHES + ("KSCHED_PACK_THREADS",):
-        monkeypatch.delenv(v, raising=False)
-    for kv in names:
-        k, _, v = kv.partition("=")
-        monkeypatch.setenv(k, v or "1")
-
-
 @pytest.mark.parametrize("name,seed", rp.CORPUS, ids=IDS)
 def test_run_corpus_matches_oracle(pkg, oracle, monkeypatch, name, seed):
-    _set_env(monkeypatch, [])
+    set_modes(monkeypatch)
     compare(pkg, oracle, pkg.Problem.from_dict(rp.build(name, seed)[0]))
 
 
@@ -50,10 +41,10 @@ def test_every_mode_switch_matches_oracle(pkg, oracle, monkeypatch, name, seed):
     rs.set_count_visited(False)
     rs.load()
     for mode in MODES:
-        _set_env(monkeypatch, [m for m in mode.split(",") if m])
+        set_modes(monkeypatch, mode)
         rs.run()
         _check(rs.download(), want, mode or "default")
-    _set_env(monkeypatch, [])
+    set_modes(monkeypatch)
 
 
 FIRST_SEEDS = [(n, s) for n, s in rp.CORPUS if s == rp.SEEDS.get(n, (0,))[0]]
@@ -69,10 +60,10 @@ def test_every_block_size_matches_oracle(pkg, oracle, monkeypatch, name, seed):
         rs.set_count_visited(count_visited)  # taken when the problem is loaded
         rs.load()
         for threads in BLOCK_SIZES:
-            _set_env(monkeypatch, [f"KSCHED_PACK_THREADS={threads}"])
+            set_modes(monkeypatch, f"KSCHED_PACK_THREADS={threads}")
             rs.run()
             res = rs.download()
             _check(res, want, f"{threads} threads, count_visited={count_visited}")
             if count_visited:
                 assert res.nodes_visited == want.nodes_visited, threads
-    _set_env(monkeypatch, [])
+    set_modes(monkeypatch)

@@ -5,13 +5,12 @@ import pytest
 
 import taint_problems as tp
 import validation_oracle as vo
-from oracle_compare import compare
+from oracle_compare import MODE_SWITCHES, compare, set_modes
 
 pytestmark = pytest.mark.gpu
 
 CORPUS = tp.corpus()
 IDS = [c[0] for c in CORPUS]
-SWITCHES = ["KSCHED_NO_CLASSRUN", "KSCHED_NO_LEVELSTEP", "KSCHED_NO_LEVELRUN", "KSCHED_NO_MASKRUN", "KSCHED_NO_LEVELWARP", "KSCHED_NO_VARSTORE"]
 
 
 def _beyond_template_sets(prob, got):
@@ -24,15 +23,15 @@ def _beyond_template_sets(prob, got):
 @pytest.mark.parametrize("threads", [32, 128, 512])
 @pytest.mark.parametrize("name,prob", CORPUS, ids=IDS)
 def test_taint_sets_equal_oracle(pkg, oracle, monkeypatch, name, prob, threads):
-    monkeypatch.setenv("KSCHED_PACK_THREADS", str(threads))
+    set_modes(monkeypatch, f"KSCHED_PACK_THREADS={threads}")
     got, _ = compare(pkg, oracle, pkg.Problem.from_dict(prob), refusal_skips=False)
     assert _beyond_template_sets(prob, got) > 0
 
 
-@pytest.mark.parametrize("switch", SWITCHES)
+@pytest.mark.parametrize("switch", MODE_SWITCHES)
 @pytest.mark.parametrize("name,prob", CORPUS[::2], ids=IDS[::2])
 def test_taint_sets_with_a_step_switched_off(pkg, oracle, monkeypatch, name, prob, switch):
-    monkeypatch.setenv(switch, "1")
+    set_modes(monkeypatch, switch)
     compare(pkg, oracle, pkg.Problem.from_dict(prob), refusal_skips=False)
 
 

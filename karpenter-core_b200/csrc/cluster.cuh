@@ -89,9 +89,9 @@ __global__ void cluster_collect_kernel(const long long* __restrict__ counters, i
   const int tid = threadIdx.x;
   if (tid == 0) {
     out->n_pods = n_pods;
-    out->n_new_nodes = (int32_t)counters[0];
-    out->n_unscheduled = (int32_t)counters[1];
-    out->error = (int32_t)counters[4];
+    out->n_new_nodes = (int32_t)counters[kCtrNewNodes];
+    out->n_unscheduled = (int32_t)counters[kCtrUnscheduled];
+    out->error = (int32_t)counters[kCtrError];
     out->template_index = nn_tmpl[0];
     out->pod_count = nn_count[0];
     out->requests_present = nn_req_present[0];

@@ -49,7 +49,30 @@ constexpr int kMaxCG = 8;        // topology groups that may constrain one pod c
 constexpr int kMaxTouched = 8;   // requirement keys one Add may touch (pod keys + topology keys)
 constexpr int kPackThreads = 512;
 constexpr int kFreshMemoSlots = 8192;  // PackState::fd_*
-constexpr int kNumCounters = 96;      // PackState::counters
+// PackState::counters: the results of a Solve, then the KSCHED_PROFILE_PACK profile (print_pack_profile)
+enum Counter : int {
+  kCtrNewNodes, kCtrUnscheduled, kCtrNodesVisited, kCtrAddCalls, kCtrError, kCtrSteps,
+  kCtrMaskCycles, kCtrMaskPods,  // mask run: cycles of its walks and stores, pods
+  // generic_step (GK_T / GK_C): cycles per phase, then counts
+  kCtrGenTopo, kCtrGenExisting, kCtrGenEval, kCtrGenCommit, kCtrGenFresh, kCtrGenFail,
+  kCtrRunCallCycles, kCtrGenCallCycles,  // cycles inside class_run / generic_step calls
+  kCtrMaskEntries,
+  kCtrGenSteps, kCtrGenInflightPlaced, kCtrGenFreshSteps, kCtrGenFailures,
+  kCtrGenPath,  // 5 paths: rejected, cached, row, dyn, cached empty
+  kCtrGenFreshDecide = kCtrGenPath + 5, kCtrGenFreshWords, kCtrGenFreshCommit, kCtrGenInflightVerify,
+  kCtrGenInflightWinner, kCtrGenInflightRecord,
+  // class_run, classes without mask-key spread in level mode (RunLv) and all others (Run)
+  kCtrRunLvCycles, kCtrRunLvPods, kCtrRunLvSteps, kCtrRunLvFresh, kCtrRunCycles, kCtrRunPods,
+  kCtrMaskBuildCycles,
+  kCtrRunFresh, kCtrRunCalls, kCtrRunPlaced, kCtrRunBails, kCtrRunIneligible, kCtrRunLvPerPod, kCtrRunPerPod, kCtrRunLvFills,
+  kCtrMaskBuildRefused, kCtrMaskUnpinnedSingle,
+  kCtrPinSteps, kCtrPinPods, kCtrPinEndStaged, kCtrPinEndCount, kCtrPinEndKey, kCtrPinEndRefused, kCtrPinEndList,
+  kCtrRoundTripCycles, kCtrNoVariantStops, kCtrNoVariantTripCycles, kCtrVarStoreHits, kCtrVarStoreEntries,
+  kCtrRoundCycles, kCtrRounds, kCtrRoundPods,
+  kCtrStretchPinned, kCtrStretchFresh = kCtrStretchPinned + 16,  // round stretches by length 1..16
+  kCtrMaskSteps = kCtrStretchFresh + 16, kCtrMaskMultiDomain, kCtrMaskRoundable,
+  kNumCounters
+};
 constexpr uint64_t kNoBest = ~0ull;
 
 #include "catalog.cuh"
@@ -66,7 +89,7 @@ namespace {
 // Launch choice per finished new node (launch.cuh): one warp per node, lanes over the words of its final option set.
 __global__ void launch_choice_kernel(DevCatalog c, const long long* counters, const uint64_t* nn_vals, const uint64_t* nn_meta,
                                      const uint32_t* nn_opts, int max_new, ksched_launch_choice* out) {
-  const int n_new = (int)counters[0];
+  const int n_new = (int)counters[kCtrNewNodes];
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
   for (int n = warp; n < n_new; n += nwarps) {
@@ -235,7 +258,7 @@ struct ksched_handle {
   DevBuf<uint64_t> d_ex_vals, d_ex_vals0, d_ex_meta, d_ex_meta0, d_ex_hp, d_ex_hp0, d_nn_vals, d_nn_meta, d_nn_hp, d_grp_registered,
       d_grp_registered0;
   DevBuf<uint16_t> d_grp_host, d_grp_host0;
-  DevBuf<long long> d_counters, d_k1dbg;  // d_counters: kNumCounters entries (0..5 results, the rest KSCHED_PROFILE_PACK)
+  DevBuf<long long> d_counters, d_k1dbg;  // d_counters: kNumCounters entries (Counter)
   DevBuf<uint32_t> d_flush;
   size_t cub_tmp_bytes = 0;
   // one-pass queue order (feasibility_kernel.cuh: sort_key1_kernel): total key bits, 0 = the three-key path
@@ -1241,33 +1264,40 @@ int ksched_run_feasibility_only(ksched_handle* h, int do_flush, float* elapsed_u
 
 #ifdef KSCHED_PROFILE_PACK
 static void print_pack_profile(const long long* counters) {
+  const long long* c = counters;
   fprintf(stderr, "[pack profile] generic: topo=%lld existing=%lld eval=%lld commit=%lld fresh=%lld fail=%lld | fastblock=%lld genericcall=%lld | "
                   "n_generic=%lld inflight_placed=%lld fresh_steps=%lld failures=%lld paths[rej,cached,row,dyn,cachedempty]=%lld,%lld,%lld,%lld,%lld steps=%lld\n",
-          counters[8], counters[9], counters[10], counters[11], counters[12], counters[13], counters[14], counters[15], counters[17], counters[18],
-          counters[19], counters[20], counters[21], counters[22], counters[23], counters[24], counters[25], counters[5]);
-  fprintf(stderr, "[pack profile] fresh: decide=%lld words=%lld commit=%lld rest=%lld | in-flight verify=%lld\n", counters[26], counters[27], counters[28],
-          counters[12], counters[29]);
-  fprintf(stderr, "[pack profile] in-flight commit: winner+barrier=%lld record=%lld rest=%lld\n", counters[30], counters[31], counters[11]);
-  fprintf(stderr, "[pack profile] class_run: calls=%lld pods=%lld bails=%lld ineligible=%lld cycles=%lld\n", counters[40], counters[41], counters[42], counters[43],
-          counters[14]);
+          c[kCtrGenTopo], c[kCtrGenExisting], c[kCtrGenEval], c[kCtrGenCommit], c[kCtrGenFresh], c[kCtrGenFail], c[kCtrRunCallCycles],
+          c[kCtrGenCallCycles], c[kCtrGenSteps], c[kCtrGenInflightPlaced], c[kCtrGenFreshSteps], c[kCtrGenFailures], c[kCtrGenPath],
+          c[kCtrGenPath + 1], c[kCtrGenPath + 2], c[kCtrGenPath + 3], c[kCtrGenPath + 4], c[kCtrSteps]);
+  fprintf(stderr, "[pack profile] fresh: decide=%lld words=%lld commit=%lld rest=%lld | in-flight verify=%lld\n", c[kCtrGenFreshDecide],
+          c[kCtrGenFreshWords], c[kCtrGenFreshCommit], c[kCtrGenFresh], c[kCtrGenInflightVerify]);
+  fprintf(stderr, "[pack profile] in-flight commit: winner+barrier=%lld record=%lld rest=%lld\n", c[kCtrGenInflightWinner], c[kCtrGenInflightRecord],
+          c[kCtrGenCommit]);
+  fprintf(stderr, "[pack profile] class_run: calls=%lld pods=%lld bails=%lld ineligible=%lld cycles=%lld\n", c[kCtrRunCalls], c[kCtrRunPlaced],
+          c[kCtrRunBails], c[kCtrRunIneligible], c[kCtrRunCallCycles]);
   fprintf(stderr, "[pack profile] class_run round trips (status-1 stop -> entry of the next call that places pods): cycles=%lld | "
                   "stops for want of a variant=%lld, their round trips' cycles=%lld | variant store: hits=%lld entries=%lld\n",
-          counters[56], counters[57], counters[58], counters[59], counters[60]);
-  fprintf(stderr, "[pack profile] mask run steps=%lld with >1 admissible domain=%lld round-able=%lld (counters shared with generic n/fresh: ignore there)\n", counters[18], counters[19], counters[17]);
-  fprintf(stderr, "[pack profile] mask run: build cycles=%lld (refused %lld) loop cycles=%lld pods=%lld entries=%lld\n", counters[38], counters[47], counters[6], counters[7], counters[16]);
+          c[kCtrRoundTripCycles], c[kCtrNoVariantStops], c[kCtrNoVariantTripCycles], c[kCtrVarStoreHits], c[kCtrVarStoreEntries]);
+  fprintf(stderr, "[pack profile] mask run steps=%lld with >1 admissible domain=%lld round-able=%lld\n", c[kCtrMaskSteps], c[kCtrMaskMultiDomain],
+          c[kCtrMaskRoundable]);
+  fprintf(stderr, "[pack profile] mask run: build cycles=%lld (refused %lld) loop cycles=%lld pods=%lld entries=%lld\n", c[kCtrMaskBuildCycles],
+          c[kCtrMaskBuildRefused], c[kCtrMaskCycles], c[kCtrMaskPods], c[kCtrMaskEntries]);
   fprintf(stderr, "[pack profile] mask run: single steps on the unpinned head=%lld | pin steps=%lld pods=%lld ended by "
                   "[staged entries,count,key,refused,end of list or 32 pods]=%lld,%lld,%lld,%lld,%lld\n",
-          counters[48], counters[49], counters[50], counters[51], counters[52], counters[53], counters[54], counters[55]);
+          c[kCtrMaskUnpinnedSingle], c[kCtrPinSteps], c[kCtrPinPods], c[kCtrPinEndStaged], c[kCtrPinEndCount], c[kCtrPinEndKey],
+          c[kCtrPinEndRefused], c[kCtrPinEndList]);
   fprintf(stderr, "[pack profile] mask run rounds: iterations=%lld pods=%lld cycles=%lld | stretch length R (rounds a step could place, "
-                  "1..16) [pinned] [fresh]:", counters[62], counters[63], counters[61]);
-  for (int k = 0; k < 2; ++k) {
+                  "1..16) [pinned] [fresh]:", c[kCtrRounds], c[kCtrRoundPods], c[kCtrRoundCycles]);
+  for (const int k : {kCtrStretchPinned, kCtrStretchFresh}) {
     fprintf(stderr, " [");
-    for (int r = 0; r < 16; ++r) fprintf(stderr, r ? ",%lld" : "%lld", counters[64 + 16 * k + r]);
+    for (int r = 0; r < 16; ++r) fprintf(stderr, r ? ",%lld" : "%lld", c[k + r]);
     fprintf(stderr, "]");
   }
   fprintf(stderr, "\n");
   fprintf(stderr, "[pack profile] class_run without mask-key spread: cycles=%lld pods=%lld level+fill iterations=%lld (fill %lld) fresh=%lld per-pod=%lld | with: cycles=%lld pods=%lld fresh=%lld per-pod=%lld\n",
-          counters[32], counters[33], counters[34], counters[46], counters[35], counters[44], counters[36], counters[37], counters[39], counters[45]);
+          c[kCtrRunLvCycles], c[kCtrRunLvPods], c[kCtrRunLvSteps], c[kCtrRunLvFills], c[kCtrRunLvFresh], c[kCtrRunLvPerPod], c[kCtrRunCycles],
+          c[kCtrRunPods], c[kCtrRunFresh], c[kCtrRunPerPod]);
 }
 #endif
 
@@ -1281,20 +1311,20 @@ int ksched_download(ksched_handle* h, const ksched_problem* pb, ksched_result* r
 #ifdef KSCHED_PROFILE_PACK
   print_pack_profile(counters);
 #endif
-  if (counters[4] != 0) {
-    h->err = counters[4] == KSCHED_ERR_OVERFLOW ? "new-node capacity exceeded" : "a pod is constrained by more topology groups than the kernel supports";
-    return (int)counters[4];
+  if (counters[kCtrError] != 0) {
+    h->err = counters[kCtrError] == KSCHED_ERR_OVERFLOW ? "new-node capacity exceeded" : "a pod is constrained by more topology groups than the kernel supports";
+    return (int)counters[kCtrError];
   }
-  const int n_new = (int)counters[0];
+  const int n_new = (int)counters[kCtrNewNodes];
   h->tm.d2h_bytes = (int64_t)sizeof counters + (int64_t)P * 4 * ((res->assign != nullptr) + (res->relax_level != nullptr) + (res->place_seq != nullptr)) +
                     (int64_t)n_new * (1 + 4 + 4 + 8 + 64 + 128 + (int64_t)W32 * 4) + (res->existing_reqs ? (int64_t)NE * 136 : 0) +
                     (res->launch ? (int64_t)n_new * (int64_t)sizeof(ksched_launch_choice) : 0) +
                     (res->feasibility ? (int64_t)P * V * W32 * 4 + (int64_t)P * 4 : 0) + (res->best_column ? (int64_t)P * 12 : 0);
   res->n_new_nodes = n_new;
-  res->n_unscheduled = (int)counters[1];
-  res->nodes_visited = counters[2];
-  res->add_calls = counters[3];
-  h->tm.pack_steps = counters[5];
+  res->n_unscheduled = (int)counters[kCtrUnscheduled];
+  res->nodes_visited = counters[kCtrNodesVisited];
+  res->add_calls = counters[kCtrAddCalls];
+  h->tm.pack_steps = counters[kCtrSteps];
   if (res->assign) CUDA_TRY(h, cudaMemcpyAsync(res->assign, h->d_assign.ptr, (size_t)P * 4, cudaMemcpyDeviceToHost, h->stream));
   if (res->relax_level) CUDA_TRY(h, cudaMemcpyAsync(res->relax_level, h->d_relax.ptr, (size_t)P * 4, cudaMemcpyDeviceToHost, h->stream));
   if (res->place_seq) CUDA_TRY(h, cudaMemcpyAsync(res->place_seq, h->d_place_seq.ptr, (size_t)P * 4, cudaMemcpyDeviceToHost, h->stream));

@@ -553,8 +553,8 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
   uint32_t& pt_class = L.pt_class;
 #ifdef KSCHED_PROFILE_PACK
   long long gk_last = clock64();
-#define GK_T(i) { if (tid == 0) { long long _n = clock64(); s.counters[8 + (i)] += _n - gk_last; gk_last = _n; } }
-#define GK_C(i) { if (tid == 0) s.counters[8 + (i)] += 1; }
+#define GK_T(i) { if (tid == 0) { long long _n = clock64(); s.counters[i] += _n - gk_last; gk_last = _n; } }
+#define GK_C(i) { if (tid == 0) s.counters[i] += 1; }
 #else
 #define GK_T(i)
 #define GK_C(i)
@@ -608,7 +608,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
       p_vol = s.cls_vol[cls];
       has_vol = (p_vol.shared | p_vol.priv[0] | p_vol.priv[1] | p_vol.priv[2] | p_vol.priv[3]) != 0;
     }
-    GK_T(0)
+    GK_T(kCtrGenTopo)
     // ------------------------------------------------------------ 1) existing nodes in caller order (scheduler.go:176-180)
     if (NE > 0) {
       // Every existing node below the class's cursor refuses this class for good: it is closed, its taints are not
@@ -703,7 +703,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
         nodes_visited += NE;
       }
     }
-    GK_T(1)
+    GK_T(kCtrGenExisting)
     // ------------------------------------------------------------ 2) in-flight nodes, fewest pods first (scheduler.go:183-190)
     // Every thread checks candidates for everything except the instance-type options (requirements, topology, the
     // resource pre-test); the block argmin picks the first such node in the reference's order; the whole CTA then
@@ -757,7 +757,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
 #pragma unroll
           for (int r = 0; r < kHotRes; ++r) bq[r] = q[r];
         }
-        GK_T(2)
+        GK_T(kCtrGenEval)
         const unsigned long long wkey = block_min_u64_db(mine, red, parity);
         if (wkey == ~0ull) {
           nodes_visited += n_new;
@@ -841,8 +841,8 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
             opts_changed = __syncthreads_or(local_changed) != 0;
           }
         }
-        GK_T(21)
-        GK_C(10)
+        GK_T(kCtrGenInflightVerify)
+        GK_C(kCtrGenInflightPlaced)
         if (s.count_visited) {  // rank of the winner among ALL in-flight nodes (the reference also walks the full ones)
           int less = 0;
           for (int i = tid; i < n_new; i += blockDim.x) less += order_key(s.nn_count[i], s.nn_tb[i]) < wkey;
@@ -910,19 +910,19 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
         ++seq;
         placed = true;
         __syncthreads();
-        GK_T(22)
+        GK_T(kCtrGenInflightWinner)
         if (sh.placed_closed) --n_active;
         if (has_topo) topo_record_block(s.nn_vals, s.nn_meta[wn], MAXN, wn, NE + wn);  // Topology.Record, one relation per thread
-        GK_T(23)
+        GK_T(kCtrGenInflightRecord)
         break;
       }
     } else if (!placed) {
       nodes_visited += n_new;  // every in-flight node is full; the reference still walks them
     }
-    GK_T(3)
+    GK_T(kCtrGenCommit)
     // ------------------------------------------------------------ 3) open a new node, templates in weight order (scheduler.go:194-217)
     if (!placed) {
-      GK_C(11)
+      GK_C(kCtrGenFreshSteps)
       const bool f_valid = s.use_F && (first_pass || s.relax_level[pod] == 0);  // K1's row is valid while the pod has its original class
       const uint32_t fpos = first_pass ? (uint32_t)fpos_first : s.pod_pos[pod];
       const bool no_column = f_valid && s.best[fpos] == kNoBest;  // no feasible (template, type) column at all
@@ -1001,8 +1001,8 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
         }
         __syncthreads();
         const int path = sh.path;
-        GK_C(13 + (path > 4 ? 4 : path))
-        GK_T(18)
+        GK_C(kCtrGenPath + (path > 4 ? 4 : path))
+        GK_T(kCtrGenFreshDecide)
         if (path == kPathReject || path == kPathCachedEmpty || path == kPathDynEmpty) continue;
         const int fd_slot = (path == kPathDynamic || path == kPathDynCached) ? sh.fd_slot : -1;
         const int a = n_active;
@@ -1046,7 +1046,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
             continue;
           }
         }
-        GK_T(19)
+        GK_T(kCtrGenFreshWords)
         // the Pareto front of a new option set, with every thread (the words were stored before the barrier above)
         const bool front_memo_hit = path == kPathRow && !limits_active && s.fc_front_state[fc];
         const bool front_fresh = path != kPathCached && path != kPathDynCached && !front_memo_hit;
@@ -1139,14 +1139,14 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
         ++n_new;
         if (!sh.placed_closed) { L.fresh_valid = 1; L.fresh_a = n_active; L.fresh_cls = cls; ++n_active; }
         placed = true;
-        GK_T(20)
+        GK_T(kCtrGenFreshCommit)
       }
       if (fatal) return;
     }
-    GK_T(4)
+    GK_T(kCtrGenFresh)
     // ------------------------------------------------------------ failure: relax + requeue (scheduler.go:117-123, queue.go:61-68)
     if (!placed) {
-      GK_C(12)
+      GK_C(kCtrGenFailures)
       const uint32_t nx = row.relax_next;
       int tail = head + qlen;
       if (tail >= qcap) tail -= qcap;
@@ -1338,7 +1338,7 @@ __device__ int vs_fetch(RunCtx& rc, unsigned cls, uint32_t pat, int lane) {
     rc.var_next = (slot + 1) % kRunVariants;
     if (rc.n_var < kRunVariants) rc.n_var++;
 #ifdef KSCHED_PROFILE_PACK
-    s.counters[59] += 1;
+    s.counters[kCtrVarStoreHits] += 1;
 #endif
   }
   __syncwarp();
@@ -1388,6 +1388,7 @@ struct RunIO {
 };
 __shared__ RunIO g_rio;
 
+constexpr unsigned kFull = 0xffffffffu;
 // first domain in (count, id) order among `cand` (non-empty)
 __device__ __forceinline__ int run_pick(uint32_t cand, const int32_t* cn) {
   int d = __ffs(cand) - 1;
@@ -1399,6 +1400,11 @@ __device__ __forceinline__ int run_pick(uint32_t cand, const int32_t* cn) {
     if (cn[e] < best) { best = cn[e]; d = e; }
   }
   return d;
+}
+// run_pick with one domain per lane (warp-wide): the lowest lane among those `in` with the fewest count
+__device__ __forceinline__ int warp_pick(bool in, int cnt) {
+  const int mc = __reduce_min_sync(0xffffffffu, in ? cnt : INT32_MAX);
+  return __ffs(__ballot_sync(0xffffffffu, in && cnt == mc)) - 1;
 }
 // How many more pods with request vector `req` (keys `res`) the node at slot a can take: exact by the Pareto front of its
 // options (quick_fit for the k-th pod <=> k <= room); kRoomSlow when the front is not exact.
@@ -1451,6 +1457,1055 @@ __device__ __forceinline__ bool run_closes(const HotSmem* hs, int a, uint32_t rp
   return node_closed(nq, min_req, RH, b1, b2, hs->flags[a]);
 }
 
+// The class run's constants for one call, shared by its steps (all inlined into class_run)
+struct RunEnv {
+  HotSmem* hs;
+  uint32_t* zv;   // [kRunMask][kTopoCap] bits 0..15 admitted domains, 16 exact (In), 17 present
+  uint32_t* rpv;  // [kActCap] room | placed << 16 | dead
+  uint16_t* hc;   // [kRunHost][kTopoCap] the hostname groups' counts
+  int NE, MAXN, W32, RH, hstride, n_host, n_mask;
+  unsigned cls;
+  bool topo, simple;
+  long long p_req[kHotRes], min_req[kHotRes];
+  // relation constants of the commit
+  uint32_t m_reg0, m_reg1;
+  int m_bias0, m_bias1;
+  bool m_rec0, m_rec1;
+  // mask run: its lists live in the second mask relation's plane, which is unused (n_mask == 1)
+  __device__ __forceinline__ uint16_t* m1_arr() const { return reinterpret_cast<uint16_t*>(zv + kTopoCap); }
+  __device__ __forceinline__ uint16_t* m1_nxt() const { return m1_arr() + kTopoCap; }
+};
+
+// A commit settles the node at slot a with room word rp2 and order (count, tb): the new order key, or - once the class no
+// longer fits anywhere on it (run_closes) - the tombstone key ~0 with the order kept in nn_last. Returns whether the node
+// closed; the caller counts the tombstone.
+__device__ __forceinline__ bool run_settle(const RunEnv& e, int a, uint32_t rp2, int count, int tb) {
+  unsigned long long key = order_key(count, tb);
+  bool closed = false;
+  if ((rp2 & 0xFFFF) == 0 && run_closes(e.hs, a, rp2, e.p_req, e.min_req, e.RH)) {
+    key = ~0ull;
+    e.hs->nn_last[a] = ((unsigned long long)(unsigned)count << 32) | (unsigned)tb;
+    closed = true;
+  }
+  e.hs->key[a] = key;
+  e.rpv[a] = rp2;
+  return closed;
+}
+// NewNode + Add replayed from variant v on the fresh slot a (node n) with order (1, tb): hot state, room word and the
+// hostname counts of its one pod (grp_host now; the run's write-back stores the counts of later pods)
+__device__ __forceinline__ void run_fresh(const RunEnv& e, const RunVariant& v, int a, int n, int tb) {
+  KS_K2
+  const RunCtx& rc = g_rc;
+  HotSmem* hs = e.hs;
+  for (int j = 0; j < e.n_host; ++j) {
+    const int times = rc.h_times[j];
+    e.hc[j * kTopoCap + a] = (uint16_t)times;
+    if (times) s.grp_host[(size_t)rc.h_row[j] * e.hstride + e.NE + n] = (uint16_t)times;
+  }
+  hs->key[a] = order_key(1, tb);
+#pragma unroll
+  for (int r = 0; r < kHotRes; ++r) { hs->q[r][a] = v.q[r]; hs->bound[r][a] = v.b1[r]; hs->bound2[r][a] = v.b2[r]; }
+  hs->node[a] = n;
+  hs->flags[a] = v.fl;
+  hs->absorbed[a] = e.simple ? e.cls : KSCHED_NONE;
+  hs->rejected[a] = KSCHED_NONE;
+  e.rpv[a] = v.rp;
+}
+// requirements.Add(In{d}) of spread relation j on the node at slot a. Two reductions instead of a read-modify-write of
+// nn_meta: the load would stall the commit for an L2 round trip (a node has one writer, and nothing in the run reads it).
+__device__ __forceinline__ void run_pin(const RunEnv& e, int j, int a, int d) {
+  KS_K2
+  const int n = e.hs->node[a], k = g_rc.m_key[j];
+  e.zv[j * kTopoCap + a] = (1u << d) | (3u << 16);
+  s.nn_vals[(size_t)k * e.MAXN + n] = 1ull << d;
+  atomicOr(reinterpret_cast<unsigned long long*>(&s.nn_meta[n]), 1ull << (KSCHED_META_PRESENT_SHIFT + k));
+  atomicAnd(reinterpret_cast<unsigned long long*>(&s.nn_meta[n]), ~(1ull << (KSCHED_META_COMPLEMENT_SHIFT + k)));
+}
+// the ring slot of the variant whose spread relations pinned domain d0 (and d1), or -1
+__device__ __forceinline__ int run_ring_find(const RunCtx& rc, int n_mask, int d0, int d1) {
+  int vi = -1;
+  for (int v2 = 0; v2 < rc.n_var && vi < 0; ++v2)
+    if ((n_mask < 1 || rc.var[v2].dom[0] == d0) && (n_mask < 2 || rc.var[v2].dom[1] == d1)) vi = v2;
+  return vi;
+}
+// fill step: the pods the node at slot a takes before it refuses - its room `cap`, cut by the hostname limits
+__device__ __forceinline__ int run_fill_cap(const RunEnv& e, int a, int cap) {
+  const RunCtx& rc = g_rc;
+  for (int j = 0; j < e.n_host; ++j) {
+    const int times = rc.h_times[j], lim = rc.h_lim[j];
+    if (!times || lim >= 0x10000) continue;
+    if (lim >= 0xFFF0) { cap = 1; continue; }  // saturating counters nearby: one pod at a time
+    const int td = (lim - (int)e.hc[j * kTopoCap + a]) / times + 1;
+    cap = td < cap ? td : cap;
+  }
+  return cap;
+}
+// the assignments of staged entries 0 .. n - 1 of buffer buf, placed from sequence number seq on
+__device__ __forceinline__ void run_store_chunk(const RunEnv& e, int buf, int n, int seq) {
+  KS_K2
+  const int tid = threadIdx.x;
+  if (tid < n) {
+    const uint32_t pd = g_rc.q_pod[buf][tid];
+    int nd = g_rc.q_node[buf][tid];
+    if (nd < -1) nd = e.NE + e.hs->node[-nd - 2];  // the mask run stores the slot
+    s.assign[pd] = nd;
+    s.place_seq[pd] = seq + tid;
+  }
+}
+
+// ---- mask run, list build (block, once per call): sorts the accepting nodes into the lists of M1Ctx. Nothing of this
+// call has been committed yet, so nn_last is free as scratch. False: a node the lists cannot represent (per-pod loop).
+__device__ __forceinline__ bool m1_build(const RunEnv& e, int n_active) {
+  M1Ctx& m1 = g_m1;
+  const HotSmem* hs = e.hs;
+  const int tid = threadIdx.x, T = blockDim.x, lane = tid & 31, warp = tid >> 5;
+  uint16_t* m1_arr = e.m1_arr();
+  uint16_t* m1_nxt = e.m1_nxt();
+  uint8_t* t_b = reinterpret_cast<uint8_t*>(e.hs->nn_last);            // bucket of slot a (0xFF: not a member)
+  uint16_t* t_pos = reinterpret_cast<uint16_t*>(t_b + kTopoCap);        // its arrival order inside the bucket
+  uint16_t* t_slot = t_pos + kTopoCap;                                  // members, bucket by bucket, unsorted
+  uint32_t* t_tie = reinterpret_cast<uint32_t*>(t_slot + kTopoCap);     // their tie-breaks
+  for (int b = tid; b < kM1Lv * kM1Lists; b += T) m1.bcnt[b] = 0;
+  if (tid == 0) m1.bad = 0;
+  __syncthreads();
+  for (int a = tid; a < n_active; a += T) {
+    const uint32_t rp = e.rpv[a];
+    int b = 0xFF;
+    if ((rp & 0xFFFF) != 0 && !(rp & kRpDead)) {
+      const uint32_t z = e.zv[a], adm = z & 0xFFFF;
+      const unsigned cn = (unsigned)(hs->key[a] >> 32);
+      int list = -1;
+      if (adm && !(adm & (adm - 1)) && (z & (1u << 16))) {  // pinned to one domain
+        if (adm & e.m_reg0) list = __ffs(adm) - 1;           // (a domain that is not registered never admits a pod)
+      } else if ((adm & e.m_reg0) == e.m_reg0) list = kM1Dom;  // admits every registered domain
+      else if (adm & e.m_reg0) m1.bad = 1;                    // some of them: per-pod loop
+      if (list >= 0) {
+        if (cn >= (unsigned)kM1Lv) m1.bad = 1;
+        else { b = list * kM1Lv + (int)cn; t_pos[a] = (uint16_t)atomicAdd(&m1.bcnt[b], 1); }
+      }
+    }
+    t_b[a] = (uint8_t)b;
+  }
+  __syncthreads();
+  if (warp == 0) {  // exclusive scan of the bucket sizes -> arr segments
+    int run = 0;
+    for (int b0 = 0; b0 < kM1Lv * kM1Lists; b0 += 32) {
+      const int b = b0 + lane;
+      const int v = b < kM1Lv * kM1Lists ? m1.bcnt[b] : 0;
+      int inc = v;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
+      if (b < kM1Lv * kM1Lists) {
+        const int list = b / kM1Lv, lv = b - list * kM1Lv;
+        m1.ap[lv][list] = (uint16_t)(run + inc - v);
+        m1.ae[lv][list] = (uint16_t)(run + inc);
+      }
+      run += __shfl_sync(0xffffffffu, inc, 31);
+    }
+  }
+  __syncthreads();
+  const bool bad = m1.bad != 0;
+  if (!bad) {
+    for (int a = tid; a < n_active; a += T) {
+      const int b = t_b[a];
+      if (b == 0xFF) continue;
+      const int list = b / kM1Lv, lv = b - list * kM1Lv;
+      const int j = m1.ap[lv][list] + t_pos[a];
+      t_slot[j] = (uint16_t)a;
+      t_tie[j] = (uint32_t)hs->key[a];
+    }
+  }
+  __syncthreads();
+  if (!bad) {
+    for (int a = tid; a < n_active; a += T) {
+      const int b = t_b[a];
+      if (b == 0xFF) continue;
+      const int list = b / kM1Lv, lv = b - list * kM1Lv;
+      const int p0 = m1.ap[lv][list], p1 = m1.ae[lv][list];
+      const uint32_t tie = (uint32_t)hs->key[a];
+      int rank = 0;
+      for (int j = p0; j < p1; ++j) rank += t_tie[j] < tie;
+      m1_arr[p0 + rank] = (uint16_t)a;
+      t_pos[a] = (uint16_t)(p0 + rank);
+    }
+  }
+  __syncthreads();
+  if (!bad) {  // link every list (its buckets are contiguous in arr), tails and heads
+    for (int a = tid; a < n_active; a += T) {
+      const int b = t_b[a];
+      if (b == 0xFF) continue;
+      const int list = b / kM1Lv, gp = t_pos[a];
+      m1_nxt[a] = gp + 1 < (int)m1.ae[kM1Lv - 1][list] ? m1_arr[gp + 1] : kM1None;
+    }
+    for (int b = tid; b < kM1Lv * kM1Lists; b += T) {
+      const int list = b / kM1Lv, lv = b - list * kM1Lv;
+      m1.tl[lv][list] = m1.ae[lv][list] > m1.ap[lv][list] ? m1_arr[m1.ae[lv][list] - 1] : kM1None;
+    }
+    if (tid < kM1Lists) m1.head[tid] = m1.ae[kM1Lv - 1][tid] > m1.ap[0][tid] ? m1_arr[m1.ap[0][tid]] : kM1None;
+    if (tid == 0) m1.upos = m1.ap[0][kM1Dom];
+  }
+  __syncthreads();
+  return !bad;
+}
+
+// ---- mask run, warp 0: lane L < kM1Lists holds list L - its head (slot, key, room word), the node after it, the tail of
+// the head's bucket, the first node behind that bucket and its pod count
+struct M1Lane {
+  int L;
+  int h = -1, n1 = -1, tcur = -1, bn = -1, bnc = 0;
+  unsigned long long hk = ~0ull, nk = ~0ull;
+  uint32_t hr = 0, nr = 0;
+
+  __device__ __forceinline__ int nxt_of(const RunEnv& e, int sl) const { const uint16_t v = e.m1_nxt()[sl]; return v == kM1None ? -1 : (int)v; }
+  __device__ __forceinline__ void level_state(const RunEnv& e) {
+    if (h < 0) { tcur = -1; bn = -1; bnc = 0; return; }
+    tcur = g_m1.tl[(int)(hk >> 32)][L];
+    bn = nxt_of(e, tcur);
+    bnc = bn >= 0 ? (int)(e.hs->key[bn] >> 32) : 0;
+  }
+  // the list's head is slot a (-1: empty): it and the node behind it are read
+  __device__ __forceinline__ void set_head(const RunEnv& e, int a) {
+    h = a; hk = ~0ull; hr = 0; n1 = -1; nk = ~0ull; nr = 0;
+    if (h >= 0) {
+      hk = e.hs->key[h]; hr = e.rpv[h]; n1 = nxt_of(e, h);
+      if (n1 >= 0) { nk = e.hs->key[n1]; nr = e.rpv[n1]; }
+    }
+  }
+  // the head has left the bucket of count c: when that bucket is exhausted, its tail goes and the next bucket is read
+  __device__ __forceinline__ void bucket_left(const RunEnv& e, int c) {
+    if (h < 0 || (int)(hk >> 32) != c) { g_m1.tl[c][L] = kM1None; level_state(e); }
+  }
+  // node a (key ak, room word ar) enters this lane's list at the FRONT of the block of count La
+  __device__ __forceinline__ void insert_front(const RunEnv& e, int a, int La, unsigned long long ak, uint32_t ar) {
+    M1Ctx& m1 = g_m1;
+    uint16_t* m1_nxt = e.m1_nxt();
+    const int hl = h >= 0 ? (int)(hk >> 32) : 0x7fffffff;
+    if (hl >= La) {  // nothing lies below: the new head
+      m1_nxt[a] = h >= 0 ? (uint16_t)h : kM1None;
+      if (hl > La) { m1.tl[La][L] = (uint16_t)a; tcur = a; bn = h; bnc = hl; }
+      n1 = h; nk = hk; nr = hr;
+      h = a; hk = ak; hr = ar;
+    } else if (bn < 0 || bnc >= La) {  // right behind the head's bucket
+      m1_nxt[a] = bn >= 0 ? (uint16_t)bn : kM1None;
+      m1_nxt[tcur] = (uint16_t)a;
+      if (bn < 0 || bnc > La) m1.tl[La][L] = (uint16_t)a;
+      if (tcur == h) { n1 = a; nk = ak; nr = ar; }
+      bn = a; bnc = La;
+    } else {  // behind the last bucket below La (the head's level is not the one)
+      int lv = La - 1;
+      while (m1.tl[lv][L] == kM1None) --lv;
+      const int pred = m1.tl[lv][L];
+      m1_nxt[a] = m1_nxt[pred];
+      m1_nxt[pred] = (uint16_t)a;
+      if (m1.tl[La][L] == kM1None) m1.tl[La][L] = (uint16_t)a;
+      if (pred == h) { n1 = a; nk = ak; nr = ar; }
+      if (pred == tcur) { bn = a; bnc = La; }
+    }
+  }
+  // a fresh node (count 1, the largest tie-break so far) enters at the END of the block of count 1
+  __device__ __forceinline__ void insert_back1(const RunEnv& e, int a, unsigned long long ak, uint32_t ar) {
+    M1Ctx& m1 = g_m1;
+    uint16_t* m1_nxt = e.m1_nxt();
+    const int hl = h >= 0 ? (int)(hk >> 32) : 0x7fffffff;
+    if (hl > 1) {
+      m1_nxt[a] = h >= 0 ? (uint16_t)h : kM1None;
+      m1.tl[1][L] = (uint16_t)a;
+      tcur = a; bn = h; bnc = hl;
+      n1 = h; nk = hk; nr = hr;
+      h = a; hk = ak; hr = ar;
+    } else if (hl == 1) {
+      m1_nxt[a] = bn >= 0 ? (uint16_t)bn : kM1None;
+      m1_nxt[tcur] = (uint16_t)a;
+      m1.tl[1][L] = (uint16_t)a;
+      if (tcur == h) { n1 = a; nk = ak; nr = ar; }
+      tcur = a;
+    } else {  // nodes without pods in front (not produced by the scheduler, kept exact anyway)
+      int lv = 1;
+      while (m1.tl[lv][L] == kM1None) --lv;
+      const int pred = m1.tl[lv][L];
+      m1_nxt[a] = m1_nxt[pred];
+      m1_nxt[pred] = (uint16_t)a;
+      m1.tl[1][L] = (uint16_t)a;
+      if (pred == h) { n1 = a; nk = ak; nr = ar; }
+      if (pred == tcur) { bn = a; bnc = 1; }
+    }
+  }
+  // the head (pod count c) leaves this lane's list: the node behind it moves up, the one behind that is fetched (it is used
+  // at this list's next pop)
+  __device__ __forceinline__ void pop_head(const RunEnv& e, int c) {
+    h = n1; hk = nk; hr = nr;
+    n1 = -1; nk = ~0ull; nr = 0;
+    if (h >= 0) {
+      n1 = nxt_of(e, h);
+      if (n1 >= 0) { nk = e.hs->key[n1]; nr = e.rpv[n1]; }
+    }
+    bucket_left(e, c);
+  }
+};
+// warp 0's place in the mask run: staged entry, tick, new nodes and slots, fr entries, ring slots the nodes created in this
+// entry replay (a store fetch must not overwrite them), and the spread count of this lane's domain
+struct M1Walk { int li, ltick, lnew, lact, nfr, cnt_d; unsigned fr_used; };
+
+// a mask-run commit of one pod on the pinned node a (pod count c, room word rp) with tick `tick`, staged entry q:
+// Topology.Record, the node's new key and room word (returned); closed: the class no longer fits anywhere on it
+__device__ __forceinline__ uint32_t m1_commit(const RunEnv& e, int buf, int a, uint32_t rp, int c, int tick, int q, bool& closed) {
+  RunCtx& rc = g_rc;
+  const uint32_t rp2 = run_record_host(rc, e.hc, e.n_host, a, rp, 1);
+  rc.q_node[buf][q] = -(a + 2);  // the slot: translated to the node when the chunk is stored
+  closed = run_settle(e, a, rp2, c + 1, -(tick + 1));
+  return rp2;
+}
+// a mask-run fresh node from ring slot vi on slot a (node n) with order (1, tb) for staged entry q, pinned to domain d;
+// its global state is stored by the CTA after the walk (fr entry f)
+__device__ __forceinline__ void m1_fresh(const RunEnv& e, int buf, int vi, int a, int n, int tb, int q, int d, int f) {
+  run_fresh(e, g_rc.var[vi], a, n, tb);
+  g_rc.q_node[buf][q] = e.NE + n;
+  e.zv[a] = (1u << d) | (3u << 16);
+  g_m1.fr[f] = (uint32_t)a | ((uint32_t)vi << 16);
+}
+
+// ---- round / round stretch. Skew 1 with a self-matching selector: only the domains with the fewest pods admit a pod, so
+// once every one of them has a pinned node at hand and the unpinned nodes come later in the order, the next pods go one to
+// each of these domains, smallest head key first - a whole round is committed at once, every lane its own domain. Returns
+// the pods placed (0: no round applies).
+__device__ __forceinline__ int m1_round(const RunEnv& e, int buf, M1Lane& l, M1Walk& w, int i_end, bool allowed, unsigned okm) {
+  KS_K2
+  RunCtx& rc = g_rc;
+  M1Ctx& m1 = g_m1;
+  HotSmem* hs = e.hs;
+  const int L = l.L;
+  const int na = __popc(okm);
+  if (na <= 1 || i_end - w.li < na) return 0;
+  const bool act = L < kM1Dom && allowed;
+  const bool hd = act && l.h >= 0;                       // this domain's pod goes to the head of its list
+  const unsigned hv = __ballot_sync(kFull, hd), fv = okm & ~hv;  // fv: domains that get a fresh node (no pinned node at hand)
+  const bool bad_l = hd && ((l.hr & 0xFFFF) == kRoomSlow || (int)(l.hk >> 32) + 1 >= kM1Lv);
+  const unsigned long long ukey = __shfl_sync(kFull, l.hk, kM1Dom);
+  // ---- round stretch: when every registered domain admits a pod (all counts are equal), each round gives every domain
+  // one pod, so the counts stay equal and the round's shape repeats. R rounds are placed in one step while R single rounds
+  // would take the same nodes (DESIGN.md section 4): pinned, the r-th members of each head's bucket; fresh, R fresh nodes
+  // per domain that take no second pod.
+  int R = 0, vi_s = -1;
+  const bool pinned = hv == okm;
+  const int jd = __popc(okm & ((1u << L) - 1u));  // act: this domain's place among the round's domains
+#ifdef KSCHED_PROFILE_PACK
+  if (okm == e.m_reg0 && 2 * na <= i_end - w.li && 2 * na <= 32) {
+#else
+  if (s.use_round_stretch && okm == e.m_reg0 && 2 * na <= i_end - w.li && 2 * na <= 32) {
+#endif
+    const int cap = (i_end - w.li) / na < 32 / na ? (i_end - w.li) / na : 32 / na;
+    if (pinned) {  // the bucket's keys ascend; nodes re-entering at count + 1 lie behind it
+      int rd = 0;
+      if (act) {
+        const int c = (int)(l.hk >> 32);
+        int a = l.h;
+        unsigned long long k = l.hk;
+        uint32_t rp = l.hr;
+        while (rd < cap && (int)(k >> 32) == c && k < ukey && (rp & 0xFFFF) != kRoomSlow && c + 1 < kM1Lv) {
+          m1.ps[rd * na + jd] = (uint16_t)a;
+          m1.rk[rd * na + jd] = k;
+          ++rd;
+          a = l.nxt_of(e, a);
+          if (a < 0) break;
+          k = hs->key[a];
+          rp = e.rpv[a];
+        }
+      }
+      R = __reduce_min_sync(kFull, act ? rd : 32);
+    } else if (hv == 0 && ukey == ~0ull && (okm & ~rc.m_tallow[0]) == 0) {  // fresh nodes that never re-enter a list
+      if (act) vi_s = run_ring_find(rc, 1, L, 0);
+      const bool shut = vi_s >= 0 && ((rc.var[vi_s].rp & 0xFFFF) == 0 || (rc.var[vi_s].rp & kRpDead));
+      bool ok = !__any_sync(kFull, act && !shut);
+      for (int j = 0; j < e.n_host; ++j) ok = ok && rc.h_lim[j] >= 0;
+      int room = e.MAXN - w.lnew;
+      if (kActCap - w.lact < room) room = kActCap - w.lact;
+      if (kTopoCap - w.lact < room) room = kTopoCap - w.lact;
+      R = !ok ? 0 : room / na < cap ? room / na : cap;
+    }
+#ifdef KSCHED_PROFILE_PACK
+    if (L == 0 && R > 0) s.counters[(pinned ? kCtrStretchPinned : kCtrStretchFresh) + (R > 16 ? 16 : R) - 1] += 1;
+    if (!s.use_round_stretch) R = 0;
+#endif
+  }
+  if (R >= 2) {
+    const int np = R * na;
+    if (pinned) {
+      const int c = (int)(l.hk >> 32);
+      if (act) for (int r = 0; r < R; ++r) l.pop_head(e, c);  // (reads the keys of the bucket before they change)
+      __syncwarp();
+      bool closed_l = false;
+      if (L < np) {  // pod L: round L / na, the node whose key has rank L % na in that round
+        const int r = L / na, a = m1.ps[L];
+        const unsigned long long k = m1.rk[L];
+        int p = r * na;
+        for (int j = 0; j < na; ++j) p += m1.rk[r * na + j] < k;
+        m1_commit(e, buf, a, e.rpv[a], (int)(k >> 32), w.ltick + p, w.li + p, closed_l);
+      }
+      const unsigned tb = __ballot_sync(kFull, closed_l);
+      if (L == 0 && tb) rc.tomb = rc.tomb + __popc(tb);
+      __syncwarp();  // key and room words
+      if (act) {  // the nodes that still accept enter the front of block c + 1, round by round
+        for (int r = 0; r < R; ++r) {
+          const int a = m1.ps[r * na + jd];
+          const uint32_t rp2 = e.rpv[a];
+          if ((rp2 & 0xFFFF) != 0 && !(rp2 & kRpDead)) l.insert_front(e, a, c + 1, hs->key[a], rp2);
+        }
+        w.cnt_d += R;
+      }
+    } else {
+      w.fr_used |= __reduce_or_sync(kFull, act ? 1u << vi_s : 0u);
+      unsigned m = okm;  // pod L: round L / na, the (L % na)-th domain in id order
+      for (int j = L % na; j > 0; --j) m &= m - 1;
+      const int d = __ffs(m) - 1;
+      const int vi = __shfl_sync(kFull, vi_s, d);
+      if (L < np) m1_fresh(e, buf, vi, w.lact + L, w.lnew + L, w.ltick + L + 1, w.li + L, d, w.nfr + L);
+      if (L < e.n_host && rc.h_times[L]) rc.h_inc[L] = rc.h_inc[L] + np;
+      if (act) w.cnt_d += R;
+      w.lnew += np;
+      w.lact += np;
+      w.nfr += np;
+    }
+    return np;
+  }
+  const unsigned hi = hd ? (unsigned)(l.hk >> 32) : 0u;
+  const unsigned mhi = __reduce_max_sync(kFull, hi);
+  const unsigned mlo = __reduce_max_sync(kFull, (hd && hi == mhi) ? (unsigned)l.hk : 0u);
+  const unsigned long long mx = ((unsigned long long)mhi << 32) | mlo;  // largest head key of the round
+  // fresh nodes come last in a round, lowest domain id first (every admissible domain has the same count: run_pick takes
+  // the lowest id), and only when no unpinned node is left (it would be taken first)
+  int vi_l = -1;
+  const int nf = __popc(fv);
+  bool fresh_ok = true;
+  if (fv) {
+    const bool fl = act && l.h < 0;
+    if (fl) vi_l = run_ring_find(rc, 1, L, 0);
+    fresh_ok = ukey == ~0ull && (fv & ~rc.m_tallow[0]) == 0 && !__any_sync(kFull, fl && vi_l < 0) && w.lnew + nf <= e.MAXN &&
+               w.lact + nf <= kActCap && w.lact + nf <= kTopoCap;
+    for (int j = 0; j < e.n_host; ++j) fresh_ok = fresh_ok && rc.h_lim[j] >= 0;
+  }
+  if (!fresh_ok || __any_sync(kFull, bad_l) || (hv != 0 && ukey <= mx)) return 0;
+  w.fr_used |= __reduce_or_sync(kFull, (act && !hd) ? 1u << vi_l : 0u);
+  int rank = 0;  // position of this lane's node in the round
+  for (unsigned m = hv; m; m &= m - 1) {
+    const unsigned long long k2 = __shfl_sync(kFull, l.hk, __ffs(m) - 1);
+    rank += k2 < l.hk;
+  }
+  bool closed_l = false;
+  if (hd) {
+    const int a = l.h;
+    const uint32_t rp = l.hr;
+    const int c = (int)(l.hk >> 32);
+    const int mytick = w.ltick + rank;
+    l.pop_head(e, c);
+    const uint32_t rp2 = m1_commit(e, buf, a, rp, c, mytick, w.li + rank, closed_l);
+    if ((rp2 & 0xFFFF) != 0 && !(rp2 & kRpDead)) l.insert_front(e, a, c + 1, order_key(c + 1, -(mytick + 1)), rp2);
+    ++w.cnt_d;
+  } else if (act) {  // NewNode + Add replayed from the variant of this lane's domain
+    const RunVariant& v = rc.var[vi_l];
+    const int idx = __popc(fv & ((1u << L) - 1u));
+    const int mytick = w.ltick + __popc(hv) + idx;
+    m1_fresh(e, buf, vi_l, w.lact + idx, w.lnew + idx, mytick + 1, w.li + __popc(hv) + idx, L, w.nfr + idx);
+    if ((v.rp & 0xFFFF) != 0 && !(v.rp & kRpDead)) l.insert_back1(e, w.lact + idx, order_key(1, mytick + 1), v.rp);
+    ++w.cnt_d;
+  }
+  if (nf && L < e.n_host && rc.h_times[L]) rc.h_inc[L] = rc.h_inc[L] + nf;
+  const unsigned tb = __ballot_sync(kFull, closed_l);
+  if (L == 0 && tb) rc.tomb = rc.tomb + __popc(tb);
+  w.lnew += nf;
+  w.lact += nf;
+  w.nfr += nf;
+  return na;
+}
+
+// ---- pin step: the unpinned head (key wkey) wins, so the next pods take the next unpinned nodes one each, in list order
+// (lane t: pod t), as long as no node of a domain list can come first: every member of the stretch has the first one's pod
+// count c and a key below every pinned head (a node pinned by the stretch re-enters at c + 1). Pod t's domain is the t-th
+// pick of run_pick's (count, id) order while the counts advance. Returns the pods placed.
+__device__ __forceinline__ int m1_pin_step(const RunEnv& e, int buf, M1Lane& l, M1Walk& w, int i_end, unsigned long long wkey, int mn, bool valid) {
+  const PackState& s = g_k2.st; (void)s;  // (c: the pod count below)
+  RunCtx& rc = g_rc;
+  M1Ctx& m1 = g_m1;
+  const int L = l.L;
+  const uint16_t* m1_arr = e.m1_arr();
+  const int c = (int)(wkey >> 32);
+  const int upos = m1.upos;
+  int lim = i_end - w.li < 32 ? i_end - w.li : 32;
+  if (m1.ae[kM1Lv - 1][kM1Dom] - upos < lim) lim = m1.ae[kM1Lv - 1][kM1Dom] - upos;
+  const unsigned long long pmin = warp_min_u64(L < kM1Dom ? l.hk : ~0ull);
+  const bool in = L < lim;
+  const int a_t = in ? (int)m1_arr[upos + L] : 0;
+  const unsigned long long k_t = in ? e.hs->key[a_t] : ~0ull;
+  const uint32_t rp_t = in ? e.rpv[a_t] : 0u;
+  const uint32_t z_t = in ? e.zv[a_t] : 0u;
+  int d_t;
+  {
+    // domain e has a slot on every level >= its count; pod t takes the t-th slot in (level, id) order (without Record the
+    // counts stay, and every pod takes the first pick). Levels are counted from mn: pod t's level is at most t, so a domain
+    // more than 31 pods above mn never gets one. Byte e of dw: domain e's level.
+    const unsigned dl = !valid ? 0xFFu : (unsigned)(w.cnt_d - mn < 32 ? w.cnt_d - mn : 32);
+    const unsigned dw0 = __reduce_or_sync(kFull, L < 4 ? dl << (8 * L) : 0u);
+    const unsigned dw1 = __reduce_or_sync(kFull, L >= 4 && L < kM1Dom ? dl << (8 * (L - 4)) : 0u);
+    unsigned y = 0, r = e.m_rec0 ? L : 0, am;
+    while (true) {
+      const unsigned yy = y * 0x01010101u;  // bit 0 of every byte of the compares -> bits 24..27 (no carries)
+      am = (((__vcmpleu4(dw0, yy) & 0x01010101u) * 0x01020408u) >> 24) & 0xFu;
+      am |= (((__vcmpleu4(dw1, yy) & 0x01010101u) * 0x01020408u) >> 20) & 0xF0u;
+      const unsigned k = __popc(am);
+      if (am == e.m_reg0) { r %= k; break; }  // every domain has a slot on every level from here on
+      if (r < k) break;
+      r -= k;
+      ++y;
+    }
+    for (; r > 0; --r) am &= am - 1;
+    d_t = __ffs(am) - 1;
+  }
+  const bool same_c = (int)(k_t >> 32) == c, below = k_t < pmin;
+  const bool ok_t = in && same_c && below && (rp_t & 0xFFFF) != kRoomSlow && c + 1 < kM1Lv &&
+                    ((rc.m_neutral[0] >> d_t) & 1) && ((z_t & (1u << 17)) || rc.m_wk[0]);
+  const unsigned okb = __ballot_sync(kFull, ok_t);
+  const int J = okb == kFull ? 32 : __ffs(~okb) - 1;
+#ifdef KSCHED_PROFILE_PACK
+  if (J > 0 && L == J)
+    s.counters[!in ? (lim == i_end - w.li ? kCtrPinEndStaged : kCtrPinEndList) : !same_c ? kCtrPinEndCount : !below ? kCtrPinEndKey : kCtrPinEndRefused] += 1;
+  if (J == 32 && L == 0) s.counters[kCtrPinEndList] += 1;
+  if (J > 0 && L == 0) { s.counters[kCtrPinSteps] += 1; s.counters[kCtrPinPods] += J; }
+#endif
+  if (J == 0) return 0;
+  bool closed_l = false;
+  if (L < J) {  // the single step's commit for pod L on node a_t, pinned to d_t
+    run_pin(e, 0, a_t, d_t);
+    m1_commit(e, buf, a_t, rp_t, c, w.ltick + L, w.li + L, closed_l);
+    m1.ps[L] = (uint16_t)a_t;
+  }
+  const unsigned tb = __ballot_sync(kFull, closed_l);
+  if (L == 0 && tb) rc.tomb = rc.tomb + __popc(tb);
+  unsigned mine = 0;  // the pods of this lane's domain
+#pragma unroll
+  for (int d = 0; d < kM1Dom; ++d) {
+    const unsigned b = __ballot_sync(kFull, L < J && d_t == d);
+    if (L == d) mine = b;
+  }
+  __syncwarp();  // ps, key and room words
+  // the nodes that still accept enter their domain's list at the front of block c + 1, in pod order: the last one ends up
+  // first (the smallest tie-break)
+  for (unsigned m = mine; m; m &= m - 1) {
+    const int t = __ffs(m) - 1, a = m1.ps[t];
+    const uint32_t rp2 = e.rpv[a];
+    if ((rp2 & 0xFFFF) != 0 && !(rp2 & kRpDead)) l.insert_front(e, a, c + 1, order_key(c + 1, -(w.ltick + t + 1)), rp2);
+  }
+  if (e.m_rec0) w.cnt_d += __popc(mine);
+  if (L == 0) m1.upos = upos + J;
+  if (L == kM1Dom) {  // the unpinned list's new head and the node behind it
+    l.set_head(e, upos + J < (int)m1.ae[kM1Lv - 1][kM1Dom] ? (int)m1_arr[upos + J] : -1);
+    l.bucket_left(e, c);
+  }
+  return J;
+}
+
+// ---- single step: the pod goes to the head of list wl (key wkey); the per-pod loop's commit, relation by relation on the
+// first lanes. Returns 0, or the reason the walk ends: 1 the pod needs generic_step, 2 per-pod loop from the next pod on.
+__device__ __forceinline__ int m1_single(const RunEnv& e, int buf, M1Lane& l, M1Walk& w, unsigned long long wkey, int wl, bool allowed) {
+  const PackState& s = g_k2.st; (void)s;  // (c: the pod count below)
+  RunCtx& rc = g_rc;
+  const int L = l.L;
+  const int a = __shfl_sync(kFull, l.h, wl);
+  const uint32_t rp = __shfl_sync(kFull, l.hr, wl);
+  if ((rp & 0xFFFF) == kRoomSlow) return 1;  // the winner needs the full evaluation
+  int d = wl;
+  const bool pin = wl == kM1Dom;
+  if (pin) {  // the placement pins the node's domain: fewest pods, lowest id among the admissible ones (run_pick)
+    d = warp_pick(allowed, w.cnt_d);
+    if (!((rc.m_neutral[0] >> d) & 1) || !((e.zv[a] & (1u << 17)) || rc.m_wk[0])) return 1;
+#ifdef KSCHED_PROFILE_PACK
+    if (L == 0) s.counters[kCtrMaskUnpinnedSingle] += 1;
+#endif
+  }
+  const int c = (int)(wkey >> 32);
+  if (L == wl) l.pop_head(e, c);
+  if (pin && L == 0) g_m1.upos = g_m1.upos + 1;  // (read by the next pin step after the __syncwarp below)
+  uint32_t rp2 = rp - 1 + (1u << 16);
+  bool dead_l = false;
+  if (L < e.n_host) {  // Topology.Record, hostname groups
+    const int times = rc.h_times[L];
+    const int old = e.hc[L * kTopoCap + a];
+    const int now = old + times > 0xFFFF ? 0xFFFF : old + times;
+    if (times) e.hc[L * kTopoCap + a] = (uint16_t)now;
+    dead_l = now > rc.h_lim[L];
+  }
+  if (e.n_host > 0 && __any_sync(kFull, dead_l)) rp2 |= kRpDead;
+  if (L == 0) {
+    if (pin) run_pin(e, 0, a, d);
+    rc.q_node[buf][w.li] = -(a + 2);  // the slot: translated to the node when the chunk is stored
+    if (run_settle(e, a, rp2, c + 1, -(w.ltick + 1))) rc.tomb = rc.tomb + 1;
+  }
+  int reason = 0;
+  if ((rp2 & 0xFFFF) != 0 && !(rp2 & kRpDead)) {  // still accepts the class: front of the block of count + 1
+    if (c + 1 >= kM1Lv) reason = 2;
+    else if (L == d) l.insert_front(e, a, c + 1, order_key(c + 1, -(w.ltick + 1)), rp2);
+  }
+  if (e.m_rec0 && L == d) ++w.cnt_d;
+  ++w.ltick;
+  ++w.li;
+  __syncwarp();  // lane 0's key / room words before a later pop fetches them
+  return reason;
+}
+
+// ---- single step when nobody accepts: NewNode + Add replayed from the variant of the domain a fresh node gets. Returns 0,
+// or 1 when the pod needs generic_step (novar: for want of a variant).
+__device__ __forceinline__ int m1_single_fresh(const RunEnv& e, int buf, M1Lane& l, M1Walk& w, unsigned okm, int& novar) {
+  RunCtx& rc = g_rc;
+  const int L = l.L;
+  if (w.lnew >= e.MAXN || w.lact >= kActCap || w.lact >= kTopoCap) return 1;
+  bool ok = true;
+  for (int j = 0; j < e.n_host; ++j) ok = ok && rc.h_lim[j] >= 0;
+  const unsigned cand = rc.m_tallow[0] & okm;
+  if (!ok || !cand) return 1;
+  const int fd = warp_pick((cand >> L) & 1, w.cnt_d);  // (cand is a subset of okm: lanes below kM1Dom)
+  int vi = run_ring_find(rc, 1, fd, 0);
+  if (vi < 0 && rc.vs_ok && !((w.fr_used >> rc.var_next) & 1))
+    vi = vs_fetch(rc, e.cls, vs_pattern(1, rc.m_key, fd, 0), L);
+  if (vi < 0) { novar = 1; return 1; }
+  const RunVariant& v = rc.var[vi];
+  w.fr_used |= 1u << vi;
+  if (L < e.n_host && rc.h_times[L]) rc.h_inc[L] = rc.h_inc[L] + 1;
+  if (L == 0) m1_fresh(e, buf, vi, w.lact, w.lnew, w.ltick + 1, w.li, fd, w.nfr);  // nothing in this loop reads the node's global state
+  ++w.nfr;
+  if (L == fd) {
+    if ((v.rp & 0xFFFF) != 0 && !(v.rp & kRpDead)) l.insert_back1(e, w.lact, order_key(1, w.ltick + 1), v.rp);  // accepts further pods of the class
+    if (e.m_rec0) ++w.cnt_d;
+  }
+  ++w.ltick; ++w.lnew; ++w.lact; ++w.li;
+  __syncwarp();
+  return 0;
+}
+
+// ---- mask run, warp 0's steps from staged entry i on: each pod's node is the smallest head key over the lists of the
+// admissible domains. The outcome goes to g_m1.out_*.
+__device__ __forceinline__ void m1_walk(const RunEnv& e, int buf, int i, int qlen, int tick, int n_new, int n_active, int& novar) {
+  KS_K2
+  RunCtx& rc = g_rc;
+  M1Ctx& m1 = g_m1;
+  const int L = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+  const bool valid = L < kM1Dom && ((e.m_reg0 >> L) & 1);
+  M1Lane l;
+  l.L = L;
+  if (L < kM1Lists) {
+    l.set_head(e, m1.head[L] == kM1None ? -1 : (int)m1.head[L]);
+    l.level_state(e);
+  }
+  M1Walk w{i, tick, n_new, n_active, 0, L < kM1Dom ? rc.cnt[0][0][L] : 0, 0u};
+  const bool rounds = e.m_rec0 && e.m_bias0 == 0;
+  int i_end = rc.q_end[buf];
+  if (i + qlen < i_end) i_end = i + qlen;
+  int reason = 0;  // 0: the staged entries of the class are consumed; 1: the pod at li needs generic_step; 2: per-pod loop from li on
+  // count + self - min <= maxSkew as count - min <= slack in 32 bits: counts are pod counts (< 2^30), so a slack of 2^30 or
+  // more admits every domain exactly like the 64-bit form of the per-pod loop
+  const int slack = e.m_bias0 < -(1 << 30) ? (1 << 30) : -e.m_bias0;
+  while (w.li < i_end) {
+#ifdef KSCHED_PROFILE_PACK
+    const long long it0 = clock64();
+#endif
+    const int mn = __reduce_min_sync(kFull, valid ? w.cnt_d : INT32_MAX);
+    const bool allowed = valid && w.cnt_d - mn <= slack;
+    const unsigned okm = __ballot_sync(kFull, allowed);
+    const bool cand_ok = L < kM1Dom ? allowed : (L == kM1Dom && okm != 0);  // an empty list keeps hk = ~0
+    const unsigned long long key = cand_ok ? l.hk : ~0ull;
+    const unsigned long long wkey = warp_min_u64(key);
+#ifdef KSCHED_PROFILE_PACK
+    {  // how often a whole round (one pod per admissible domain, all from pinned lists) could be placed at once
+      const unsigned have = __ballot_sync(kFull, L < kM1Dom && allowed && l.h >= 0);
+      const unsigned long long ukey = __shfl_sync(kFull, l.hk, kM1Dom);
+      unsigned long long mx = (L < kM1Dom && allowed && l.h >= 0) ? l.hk : 0ull;
+      for (int o = 16; o; o >>= 1) { const unsigned long long t = __shfl_xor_sync(kFull, mx, o); mx = t > mx ? t : mx; }
+      const int na = __popc(okm);
+      if (L == 0 && na > 1 && have == okm && ukey > mx && i_end - w.li >= na) s.counters[kCtrMaskRoundable] += 1;
+      if (L == 0) s.counters[kCtrMaskSteps] += 1;
+      if (L == 0 && na > 1) s.counters[kCtrMaskMultiDomain] += 1;
+    }
+#endif
+    if (rounds) {
+      const int np = m1_round(e, buf, l, w, i_end, allowed, okm);
+      if (np > 0) {
+#ifdef KSCHED_PROFILE_PACK
+        if (L == 0) { s.counters[kCtrRoundCycles] += clock64() - it0; s.counters[kCtrRounds] += 1; s.counters[kCtrRoundPods] += np; }
+#endif
+        w.ltick += np;
+        w.li += np;
+        __syncwarp();
+        continue;
+      }
+    }
+    if (wkey != ~0ull) {
+      const int wl = __ffs(__ballot_sync(kFull, key == wkey)) - 1;
+      if (wl == kM1Dom) {
+        const int J = m1_pin_step(e, buf, l, w, i_end, wkey, mn, valid);
+        if (J > 0) {
+          w.ltick += J;
+          w.li += J;
+          __syncwarp();
+          continue;
+        }
+      }
+      reason = m1_single(e, buf, l, w, wkey, wl, allowed);
+    } else reason = m1_single_fresh(e, buf, l, w, okm, novar);
+    if (reason) break;
+  }
+  __syncwarp();
+  // every warp's copy of the spread counters follows (the per-pod loop and the write-back read them)
+  if (L < kM1Dom) for (int wi = 0; wi < nwarps; ++wi) rc.cnt[wi][0][L] = w.cnt_d;
+  if (L < kM1Lists) m1.head[L] = l.h >= 0 ? (uint16_t)l.h : kM1None;
+  if (L == 0) { m1.out_adv = w.li - i; m1.out_reason = reason; m1.out_tick = w.ltick; m1.out_n_new = w.lnew; m1.out_n_active = w.lact; m1.n_fresh = w.nfr; }
+}
+
+// ---- mask run, fresh-node store (block): the global state of the nodes the walk created, 64 words per node across the CTA
+__device__ __forceinline__ void m1_store_fresh(const RunEnv& e) {
+  KS_K2
+  const int tid = threadIdx.x, T = blockDim.x;
+  const int nfr = g_m1.n_fresh;
+  for (int x = tid; x < nfr * 64; x += T) {
+    const uint32_t rec = g_m1.fr[x >> 6];
+    const int a = (int)(rec & 0xFFFF), w = x & 63;
+    const RunVariant& v = g_rc.var[rec >> 16];
+    const int n = e.hs->node[a];
+    if (w < e.W32) s.nn_opts[(size_t)w * e.MAXN + n] = v.opts[w];
+    if (w < c.n_keys) s.nn_vals[(size_t)w * e.MAXN + n] = v.vals[w];
+    if (w < KSCHED_MAX_RES) s.nn_req[(size_t)w * e.MAXN + n] = v.q[w];
+    if (w == 0) {
+      s.nn_meta[n] = v.meta;
+      s.nn_tmpl[n] = (uint8_t)(v.fl >> 8);
+      s.nn_req_present[n] = v.qp;
+      s.nn_hp[n] = 0;
+      if (((e.rpv[a] >> 16) & 0x7FFF) == 0) {  // no further pod so far: (1, creation tick); otherwise the run's write-back stores them
+        s.nn_count[n] = 1;
+        s.nn_tb[n] = (int)((unsigned)e.hs->key[a] ^ 0x80000000u);
+      }
+    }
+  }
+}
+
+// ---- warp level / fill: at most 32 open nodes, the level / fill steps of run_level_block with ONE node per lane of warp 0
+// and no block barrier (slot a belongs to thread a, as in the block-wide form). Fresh nodes and winners that need the full
+// evaluation go to the block-wide steps. The outcome goes to g_m1.out_*.
+__device__ __forceinline__ void run_level_warp(const RunEnv& e, int buf, int i, int qlen, int tick, int n_active) {
+  RunCtx& rc = g_rc;
+  HotSmem* hs = e.hs;
+  const int lane = threadIdx.x & 31;
+  const int a = lane;
+  const bool mine = a < n_active;
+  int li = i, ltick = tick, reason = 0;
+  int i_end = rc.q_end[buf];
+  if (i + qlen < i_end) i_end = i + qlen;
+  while (li < i_end) {
+    const uint32_t rp = mine ? e.rpv[a] : 0u;
+    const unsigned long long key = mine ? hs->key[a] : ~0ull;
+    const bool el = mine && (rp & 0xFFFF) != 0 && !(rp & kRpDead);
+    const unsigned elm = __ballot_sync(kFull, el);
+    if (!elm || __any_sync(kFull, el && (rp & 0xFFFF) == kRoomSlow)) { reason = 1; break; }
+    const unsigned cn = el ? (unsigned)(key >> 32) : 0xFFFFFFFFu;
+    const unsigned c_min = __reduce_min_sync(kFull, cn);
+    const bool mem = el && cn == c_min;
+    const unsigned memm = __ballot_sync(kFull, mem);
+    const int k_av = i_end - li;
+    int t = 1, rank = 0, adv_w;
+    if (!(elm & (elm - 1))) {  // fill: the only accepting node takes pods until it refuses
+      int cap = (int)(rp & 0xFFFF);
+      if (mem) cap = run_fill_cap(e, a, cap);
+      t = __shfl_sync(kFull, cap, __ffs(memm) - 1);
+      t = t < k_av ? t : k_av;
+      adv_w = t;
+    } else {  // level: the accepting nodes with the fewest pods, one pod each in tie order
+      const unsigned tie = (unsigned)key;
+      for (unsigned m = memm; m; m &= m - 1) {
+        const unsigned tm = __shfl_sync(kFull, tie, __ffs(m) - 1);
+        rank += tm < tie;
+      }
+      const int n_s = __popc(memm);
+      adv_w = n_s < k_av ? n_s : k_av;
+    }
+    if (mem && rank < adv_w) {  // (fill: rank 0 < t)
+      const uint32_t rp2 = run_record_host(rc, e.hc, e.n_host, a, rp, t);
+      const int nd = e.NE + hs->node[a];
+      for (int x = 0; x < t; ++x) rc.q_node[buf][li + rank + x] = nd;
+      if (run_settle(e, a, rp2, (int)c_min + t, -(ltick + rank + t))) atomicAdd(&rc.tomb, 1);
+    }
+    ltick += adv_w;
+    li += adv_w;
+  }
+  if (lane == 0) { g_m1.out_adv = li - i; g_m1.out_reason = reason; g_m1.out_tick = ltick; }
+}
+
+// ---- block level / fill, for classes without mask-key spread: a node's verdict depends on the node alone, so
+//  * level step: the n accepting nodes with the fewest pods take the next n pods one each, in tie order (each leaves for the
+//    block of count + 1, behind every node of the level);
+//  * fill step: the only accepting node takes pods until it refuses (resources / hostname limits);
+//  * a fresh node is filled the same way in the step that creates it (run_fresh_step).
+// Returns 0 when a node needs the full evaluation (per-pod argmin step), 1 when `adv` pods are placed (fill: by a fill
+// step), 2 when nobody accepts.
+__device__ __forceinline__ int run_level_block(const RunEnv& e, int buf, int i, int k_avail, int n_active, int& tick, int& parity, int& lvp,
+                                               int& adv, bool& fill) {
+  RunCtx& rc = g_rc;
+  HotSmem* hs = e.hs;
+  const int tid = threadIdx.x, T = blockDim.x, lane = tid & 31, warp = tid >> 5, nwarps = T >> 5;
+  uint32_t* lvt = e.zv;  // tie-breaks of the level's members (the zone words are unused when n_mask == 0)
+  unsigned cmin = 0xFFFFFFFFu;
+  int ne = 0;
+  bool slow = false;
+  for (int a = tid; a < n_active; a += T) {
+    const uint32_t rp = e.rpv[a];
+    if ((rp & 0xFFFF) != 0 && !(rp & kRpDead)) {  // tombstones have no room
+      const unsigned cn = (unsigned)(hs->key[a] >> 32);
+      cmin = cn < cmin ? cn : cmin;
+      ++ne;
+      slow = slow || (rp & 0xFFFF) == kRoomSlow;
+    }
+  }
+  const unsigned wc = __reduce_min_sync(0xffffffffu, cmin);
+  const unsigned wn = __reduce_add_sync(0xffffffffu, (unsigned)ne) | (__any_sync(0xffffffffu, slow) ? 0x80000000u : 0u);
+  if (lane == 0) rc.red_key[parity][warp] = ((unsigned long long)wc << 32) | wn;
+  __syncthreads();
+  const unsigned long long rr = lane < nwarps ? rc.red_key[parity][lane] : 0xFFFFFFFF00000000ull;
+  parity ^= 1;
+  const unsigned c_min = __reduce_min_sync(0xffffffffu, (unsigned)(rr >> 32));
+  const int n_el = (int)__reduce_add_sync(0xffffffffu, (unsigned)rr & 0x7FFFFFFFu);
+  const bool any_slow = __any_sync(0xffffffffu, ((unsigned)rr >> 31) != 0);
+  if (any_slow) return 0;
+  if (n_el == 0) return 2;
+  const int lp = lvp;
+  lvp ^= 1;
+  if (tid == 0) rc.lv_cnt[lp ^ 1] = 0;  // last read before this step's first barrier
+  // the level's members append their tie-breaks to the list (any order)
+  for (int base = 0; base < n_active; base += T) {
+    const int a = base + tid;
+    bool mem = false;
+    unsigned tie = 0;
+    if (a < n_active) {
+      const uint32_t rp = e.rpv[a];
+      const unsigned long long key = hs->key[a];
+      mem = (rp & 0xFFFF) != 0 && !(rp & kRpDead) && (unsigned)(key >> 32) == c_min;
+      tie = (unsigned)key;
+      if (mem && n_el == 1) {  // fill: how many pods this node takes before it refuses
+        const int cap = run_fill_cap(e, a, (int)(rp & 0xFFFF));
+        rc.lv_fill[lp] = cap < k_avail ? cap : k_avail;
+      }
+    }
+    const unsigned bal = __ballot_sync(0xffffffffu, mem);
+    if (bal) {
+      const int src = __ffs(bal) - 1;
+      int pos0 = 0;
+      if (lane == src) pos0 = atomicAdd(&rc.lv_cnt[lp], __popc(bal));
+      pos0 = __shfl_sync(0xffffffffu, pos0, src);
+      if (mem) lvt[pos0 + __popc(bal & ((1u << lane) - 1u))] = tie;
+    }
+  }
+  __syncthreads();
+  const int n_s = rc.lv_cnt[lp];
+  const int t_fill = n_el == 1 ? rc.lv_fill[lp] : 1;
+  const int k_lvl = n_el == 1 ? 1 : (n_s < k_avail ? n_s : k_avail);
+  fill = n_el == 1;
+  adv = n_el == 1 ? t_fill : k_lvl;
+  for (int a = tid; a < n_active; a += T) {
+    const uint32_t rp = e.rpv[a];
+    const unsigned long long key = hs->key[a];
+    if (!((rp & 0xFFFF) != 0 && !(rp & kRpDead) && (unsigned)(key >> 32) == c_min)) continue;
+    const unsigned tie = (unsigned)key;
+    int rank = 0;
+    if (n_el != 1) {
+      int j = 0;
+      for (; j + 4 <= n_s; j += 4) {
+        const uint4 v = *reinterpret_cast<const uint4*>(lvt + j);
+        rank += (v.x < tie) + (v.y < tie) + (v.z < tie) + (v.w < tie);
+      }
+      for (; j < n_s; ++j) rank += lvt[j] < tie;
+      if (rank >= k_lvl) continue;
+    }
+    // the owner commits: pods i + rank .. i + rank + t - 1 of the chunk
+    const int t = t_fill;
+    const uint32_t rp2 = run_record_host(rc, e.hc, e.n_host, a, rp, t);
+    const int nd = e.NE + hs->node[a];
+    for (int x = 0; x < t; ++x) rc.q_node[buf][i + rank + x] = nd;
+    if (run_settle(e, a, rp2, (int)c_min + t, -(tick + rank + t))) atomicAdd(&rc.tomb, 1);
+  }
+  tick += adv;
+  return 1;
+}
+
+// ---- per-pod argmin step: the node the reference's scan takes, by a block argmin on the order key over the accepting
+// nodes (their admissible domains included), committed by its owner. Returns 0 when the pod is placed, 1 when the winner
+// needs the full evaluation, 2 when nobody accepts; okm0 / okm1: the admissible domains of each spread relation.
+__device__ __forceinline__ int run_argmin_step(const RunEnv& e, int buf, int i, int n_active, int& tick, int& parity, uint32_t& okm0, uint32_t& okm1) {
+  RunCtx& rc = g_rc;
+  HotSmem* hs = e.hs;
+  const int tid = threadIdx.x, T = blockDim.x, lane = tid & 31, warp = tid >> 5, nwarps = T >> 5;
+  const int n_mask = e.n_mask;
+  // node-independent half of nextDomainTopologySpread, one domain per lane: min count over the pod's domains, the
+  // domains within max-skew (count + self - min <= maxSkew)
+#pragma unroll
+  for (int j = 0; j < kRunMask; ++j) {
+    if (j >= n_mask) break;
+    const bool valid = ((j ? e.m_reg1 : e.m_reg0) >> lane) & 1;  // registered domains have ids < kRunDom
+    const int cn = rc.cnt[warp][j][lane & (kRunDom - 1)];
+    const int mn = __reduce_min_sync(0xffffffffu, valid ? cn : INT32_MAX);
+    (j ? okm1 : okm0) = __ballot_sync(0xffffffffu, valid && (long long)cn + (j ? e.m_bias1 : e.m_bias0) <= (long long)mn);
+  }
+  // ---- scan the slots this thread owns: key, rp and (topology classes) the admissible domains
+  unsigned long long mine = ~0ull;
+  int best_a = 0;
+  uint32_t best_rp = 0, best_z0 = 0, best_z1 = 0;
+  for (int a = tid; a < n_active; a += T) {
+    const unsigned long long key = hs->key[a];
+    const uint32_t rp = e.rpv[a];
+    uint32_t z0 = 0, z1 = 0;
+    bool ok = key < mine && (rp & 0xFFFF) != 0 && !(rp & kRpDead);  // tombstones carry key = ~0
+    if (n_mask > 0) { z0 = e.zv[a]; ok = ok && (z0 & okm0) != 0; }
+    if (n_mask > 1) { z1 = e.zv[kTopoCap + a]; ok = ok && (z1 & okm1) != 0; }
+    if (ok) { mine = key; best_a = a; best_rp = rp; best_z0 = z0; best_z1 = z1; }
+  }
+  // payload of this thread's candidate: slot | slow << 11 | pin bits << 13 | domains << 15 / 19
+  unsigned pay = (unsigned)best_a;
+  if (mine != ~0ull) {
+    if ((best_rp & 0xFFFF) == kRoomSlow) pay |= 1u << 11;
+#pragma unroll
+    for (int j = 0; j < kRunMask; ++j) {
+      if (j >= n_mask) break;
+      const uint32_t z = j ? best_z1 : best_z0, cand = z & (j ? okm1 : okm0);
+      int d;
+      if (!(z & 0xFFFF & ((z & 0xFFFF) - 1)) && (z & (1u << 16))) d = __ffs(cand) - 1;  // pinned already
+      else {  // the placement pins the node's domain
+        d = run_pick(cand, rc.cnt[warp][j]);
+        pay |= 1u << (13 + j);
+        if (!((rc.m_neutral[j] >> d) & 1) || !((z & (1u << 17)) || rc.m_wk[j])) pay |= 1u << 11;
+      }
+      pay |= (unsigned)d << (15 + 4 * j);
+    }
+  }
+  // ---- block argmin with payload: ONE barrier (double-buffered scratch)
+  const unsigned long long wmin = warp_min_u64(mine);
+  if (mine == wmin && mine != ~0ull) { rc.red_key[parity][warp] = wmin; rc.red_pay[parity][warp] = pay; }
+  else if (lane == 0 && wmin == ~0ull) rc.red_key[parity][warp] = ~0ull;
+  __syncthreads();
+  const unsigned long long rk = lane < nwarps ? rc.red_key[parity][lane] : ~0ull;
+  const unsigned rp_l = lane < nwarps ? rc.red_pay[parity][lane] : 0;
+  parity ^= 1;
+  const unsigned long long wkey = warp_min_u64(rk);
+  if (wkey == ~0ull) return 2;
+  const unsigned src = __ballot_sync(0xffffffffu, rk == wkey);
+  const unsigned wp = __shfl_sync(0xffffffffu, rp_l, __ffs(src) - 1);
+  if (wp & (1u << 11)) return 1;  // the winner needs the full evaluation
+  const int fd0 = (wp >> 15) & 0xF, fd1 = (wp >> 19) & 0xF;
+  if (mine == wkey) {  // the owner commits its node: a handful of shared-memory stores
+    const int a = best_a;
+    const uint32_t rp = run_record_host(rc, e.hc, e.n_host, a, best_rp, 1);
+    for (int j = 0; j < n_mask; ++j)  // requirements.Add(In{d}) on the node: once per node and key
+      if ((pay >> (13 + j)) & 1) run_pin(e, j, a, j ? fd1 : fd0);
+    rc.q_node[buf][i] = e.NE + hs->node[a];
+    if (run_settle(e, a, rp, (int)(wkey >> 32) + 1, -(tick + 1))) rc.tomb = rc.tomb + 1;  // tombstone, compacted when the run ends
+  }
+  if (n_mask > 0) {  // every warp keeps its copy of the spread counters in step (the node's domain is the single value d)
+    if (lane == 0) {
+      if (e.m_rec0) rc.cnt[warp][0][fd0]++;
+      if (e.m_rec1) rc.cnt[warp][1][fd1]++;
+    }
+    __syncwarp();
+  }
+  ++tick;
+  return 0;
+}
+
+// ---- fresh-node step: nobody accepts, so NewNode + Add is replayed from a variant (templates: the one the variant was
+// created from). Fill step on the fresh node: it takes `cap` further pods of the class while it is the only accepting node
+// and then refuses (room 0 or a hostname limit reached). With an exact cap the run needs F such nodes in a row, m = 1 + cap
+// pods each: all of them are created in this step, one per thread (slot a belongs to thread a % T as everywhere). Returns
+// false when the pod needs generic_step (novar: for want of a variant); else `adv` pods are placed.
+__device__ __forceinline__ bool run_fresh_step(const RunEnv& e, int buf, int i, int k_avail, bool lvl, uint32_t okm0, uint32_t okm1,
+                                               int& tick, int& n_new, int& n_active, int& adv, int& novar) {
+  KS_K2
+  RunCtx& rc = g_rc;
+  const int tid = threadIdx.x, T = blockDim.x, lane = tid & 31, warp = tid >> 5;
+  const int n_mask = e.n_mask, MAXN = e.MAXN;
+  if (n_new >= MAXN || n_active >= kActCap || (e.topo && n_active >= kTopoCap)) return false;
+  bool ok = true;
+#pragma unroll
+  for (int j = 0; j < kRunHost; ++j) ok = ok && (j >= e.n_host || rc.h_lim[j] >= 0);  // a fresh hostname has count 0
+  int fd0 = 0, fd1 = 0;
+  if (n_mask > 0 && ok) {
+    const uint32_t cand = rc.m_tallow[0] & okm0;
+    if (!cand) ok = false; else fd0 = run_pick(cand, rc.cnt[warp][0]);
+  }
+  if (n_mask > 1 && ok) {
+    const uint32_t cand = rc.m_tallow[1] & okm1;
+    if (!cand) ok = false; else fd1 = run_pick(cand, rc.cnt[warp][1]);
+  }
+  int vi = ok ? run_ring_find(rc, n_mask, fd0, fd1) : -1;
+  const uint32_t pat = vs_pattern(n_mask, rc.m_key, fd0, fd1);
+  if (vi < 0 && ok && rc.vs_ok && vs_maybe(rc, vs_tag(rc.sig, pat), lane)) {  // (every warp finds the same answer)
+    __syncthreads();  // every warp has scanned the ring
+    if (warp == 0) {
+      const int got = vs_fetch(rc, e.cls, pat, lane);
+      if (lane == 0) rc.vs_got = got;
+    }
+    __syncthreads();
+    vi = rc.vs_got;
+  }
+  if (vi < 0) { novar = ok; return false; }
+  const RunVariant& v = rc.var[vi];
+  int cap = 0, F = 1;
+  bool cap_exact = false;
+  if (lvl && (v.rp & 0xFFFF) != kRoomSlow) {
+    cap_exact = true;
+    if (!(v.rp & kRpDead)) {
+      cap = (int)(v.rp & 0xFFFF);
+      for (int j = 0; j < e.n_host; ++j) {
+        const int times = rc.h_times[j], lim = rc.h_lim[j];
+        if (!times || lim >= 0x10000) continue;
+        if (lim >= 0xFFF0) { cap = 0; cap_exact = false; continue; }  // saturating counters nearby: one pod at a time
+        const int td = (lim - times) / times + 1;  // the count is `times` after the first pod
+        cap = td < cap ? td : cap;
+      }
+    }
+  }
+  const int m = 1 + cap;
+  if (cap_exact) {
+    F = (k_avail + m - 1) / m;
+    if (F > MAXN - n_new) F = MAXN - n_new;
+    if (F > kActCap - n_active) F = kActCap - n_active;
+    if (e.topo && F > kTopoCap - n_active) F = kTopoCap - n_active;
+  }
+  const int K = k_avail < F * m ? k_avail : F * m;  // pods consumed (k_avail is 1 outside level mode: F = m = K = 1)
+  for (int idx = tid; idx < e.W32 * F; idx += T) { const int w = idx / F, j = idx - w * F; s.nn_opts[(size_t)w * MAXN + n_new + j] = v.opts[w]; }
+  for (int idx = tid; idx < c.n_keys * F; idx += T) { const int k = idx / F, j = idx - k * F; s.nn_vals[(size_t)k * MAXN + n_new + j] = v.vals[k]; }
+  for (int idx = tid; idx < KSCHED_MAX_RES * F; idx += T) { const int r = idx / F, j = idx - r * F; s.nn_req[(size_t)r * MAXN + n_new + j] = v.q[r]; }
+  for (int x = tid; x < K; x += T) rc.q_node[buf][i + x] = e.NE + n_new + x / m;
+  if (tid == 0) for (int j = 0; j < e.n_host; ++j) if (rc.h_times[j]) rc.h_inc[j] = rc.h_inc[j] + F;
+  for (int j = (tid + T - n_active % T) % T; j < F; j += T) {  // the new slots this thread owns
+    const int a = n_active + j, n = n_new + j;
+    const int t = (K - j * m < m ? K - j * m : m) - 1;  // further pods on this node (the last one may get fewer)
+    const int tk = tick + j * m;                          // tick of its first pod
+    run_fresh(e, v, a, n, tk + 1);
+    s.nn_meta[n] = v.meta;
+    s.nn_tmpl[n] = (uint8_t)(v.fl >> 8);
+    s.nn_req_present[n] = v.qp;
+    s.nn_hp[n] = 0;
+    s.nn_count[n] = 1;
+    s.nn_tb[n] = tk + 1;
+    if (n_mask > 0) e.zv[a] = (1u << fd0) | (3u << 16);
+    if (n_mask > 1) e.zv[kTopoCap + a] = (1u << fd1) | (3u << 16);
+    // the fill's t further pods (the slot holds the variant's requests and front, and v.rp carries no placed pod)
+    if (t > 0 && run_settle(e, a, run_record_host(rc, e.hc, e.n_host, a, v.rp, t), 1 + t, -(tk + 1 + t))) atomicAdd(&rc.tomb, 1);
+  }
+  if (n_mask > 0) {
+    if (lane == 0) {
+      if (e.m_rec0) rc.cnt[warp][0][fd0]++;
+      if (e.m_rec1) rc.cnt[warp][1][fd1]++;
+    }
+    __syncwarp();
+  }
+  adv = K;
+  tick += K;
+  n_new += F;
+  n_active += F;
+  return true;
+}
+
 __device__ __noinline__ void class_run(const PodRegs& first_in) {
   KS_K2
   RunCtx& rc = g_rc;
@@ -1460,7 +2515,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
   uint32_t* rpv = zv + (size_t)kRunMask * kTopoCap;                                      // [kActCap] room | placed << 16 | dead
   uint16_t* hc = reinterpret_cast<uint16_t*>(rpv + kActCap);                             // [kRunHost][kTopoCap]
   const uint32_t* tmpl_taintset = g_tmpl_taintset;
-  const int tid = threadIdx.x, T = blockDim.x, lane = tid & 31, warp = tid >> 5, nwarps = T >> 5;
+  const int tid = threadIdx.x, T = blockDim.x, lane = tid & 31, warp = tid >> 5;
   const int NE = s.n_existing, MAXN = s.max_new, W32 = c.W32;
   const int RH = c.n_res < kHotRes ? c.n_res : kHotRes;
   const int hstride = s.n_existing + s.max_new;
@@ -1541,15 +2596,18 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
   const ksched_pod_row* ffd_rows = reinterpret_cast<const ksched_pod_row*>(s.rows);
   int cb = qi, buf = 0;
   uint32_t nx_pod = 0, nx_cls = KSCHED_NONE;
+  auto stage = [&](int b, uint32_t pd, uint32_t pc) {  // thread tid < CH: entry cb + tid into buffer b, entry cb + CH + tid into registers
+    rc.q_pod[b][tid] = pd; rc.q_cls[b][tid] = pc;
+    const unsigned mm = __ballot_sync(0xffffffffu, pc != cls);  // CH is a multiple of 32: whole warps
+    if (lane == 0 && mm) atomicMin(&rc.q_end[b], (tid & ~31) + __ffs(mm) - 1);
+    const int idx2 = cb + CH + tid;
+    nx_cls = KSCHED_NONE;
+    if (idx2 < s.n_pods) { nx_pod = s.order[idx2]; nx_cls = (uint32_t)ffd_rows[idx2].reserved; }
+  };
   if (tid < CH) {
     const int idx = cb + tid;
-    uint32_t pd = 0, pc = KSCHED_NONE;
-    if (idx < s.n_pods) { pd = s.order[idx]; pc = (uint32_t)ffd_rows[idx].reserved; }
-    rc.q_pod[0][tid] = pd; rc.q_cls[0][tid] = pc;
-    const unsigned mm = __ballot_sync(0xffffffffu, pc != cls);  // CH is a multiple of 32: whole warps
-    if (lane == 0 && mm) atomicMin(&rc.q_end[0], (tid & ~31) + __ffs(mm) - 1);
-    const int idx2 = idx + CH;
-    if (idx2 < s.n_pods) { nx_pod = s.order[idx2]; nx_cls = (uint32_t)ffd_rows[idx2].reserved; }
+    const bool in = idx < s.n_pods;
+    stage(0, in ? s.order[idx] : 0, in ? (uint32_t)ffd_rows[idx].reserved : KSCHED_NONE);
   }
   // ---- per-run state: spread counters (one copy per warp), per-node inputs (each thread fills the slots it owns)
   if (tid == 0) rc.tomb = 0;
@@ -1637,7 +2695,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
           rc.vs_tag[e] = vs_tag(rc.sig, pat);
           rc.vs_n = e + 1;
 #ifdef KSCHED_PROFILE_PACK
-          s.counters[60] += 1;
+          s.counters[kCtrVarStoreEntries] += 1;
 #endif
         }
         __syncwarp();
@@ -1645,30 +2703,22 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
     }
   }
 
-  long long min_req[kHotRes];
+  RunEnv e{hs, zv, rpv, hc, NE, MAXN, W32, RH, hstride, n_host, n_mask, cls, topo, simple};
 #pragma unroll
-  for (int r = 0; r < kHotRes; ++r) min_req[r] = r < RH ? s.min_req[r] : 0;
-  // relation constants of the commit, in registers
-  int h_times_sum = 0;
-#pragma unroll
-  for (int j = 0; j < kRunHost; ++j) if (j < n_host) h_times_sum += rc.h_times[j];
-  const uint32_t m_reg0 = n_mask > 0 ? rc.m_registered[0] : 0, m_reg1 = n_mask > 1 ? rc.m_registered[1] : 0;
-  const int m_bias0 = n_mask > 0 ? (int)rc.m_self[0] - rc.m_skew[0] : 0, m_bias1 = n_mask > 1 ? (int)rc.m_self[1] - rc.m_skew[1] : 0;
-  const bool m_rec0 = n_mask > 0 && rc.m_rec[0], m_rec1 = n_mask > 1 && rc.m_rec[1];
+  for (int r = 0; r < kHotRes; ++r) { e.p_req[r] = p_req[r]; e.min_req[r] = r < RH ? s.min_req[r] : 0; }
+  e.m_reg0 = n_mask > 0 ? rc.m_registered[0] : 0; e.m_reg1 = n_mask > 1 ? rc.m_registered[1] : 0;
+  e.m_bias0 = n_mask > 0 ? (int)rc.m_self[0] - rc.m_skew[0] : 0; e.m_bias1 = n_mask > 1 ? (int)rc.m_self[1] - rc.m_skew[1] : 0;
+  e.m_rec0 = n_mask > 0 && rc.m_rec[0]; e.m_rec1 = n_mask > 1 && rc.m_rec[1];
   int status = 0;
+  int novar = 0;  // the run stopped because no variant was known for the fresh node's domain (profile)
   const bool lvl = s.use_level_run && n_mask == 0;
   // mask run (see M1Ctx): one mask-key spread relation, domains and counts small enough for the lists
-  M1Ctx& m1 = g_m1;
-  bool m1_ok = s.use_mask_run && n_mask == 1 && (m_reg0 >> kM1Dom) == 0;
+  bool m1_ok = s.use_mask_run && n_mask == 1 && (e.m_reg0 >> kM1Dom) == 0;
   bool m1_built = false;
-  uint16_t* m1_arr = reinterpret_cast<uint16_t*>(zv + kTopoCap);  // the second mask relation's plane is unused (n_mask == 1)
-  uint16_t* m1_nxt = m1_arr + kTopoCap;
-  uint32_t* lvt = zv;  // level step: tie-breaks of the level's members (the zone words are unused when n_mask == 0)
   int lvp = 0;
 #ifdef KSCHED_PROFILE_PACK
   const long long cr_t0 = clock64();
   int cr_it[4] = {0, 0, 0, 0};  // iterations: level, fill, fresh, per-pod argmin
-  int cr_novar = 0;             // the run stopped because no variant was known for the fresh node's domain
 #define CR_IT(k) { ++cr_it[k]; }
 #else
 #define CR_IT(k)
@@ -1678,712 +2728,39 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
     int i = qi - cb;
     if (i == CH) {  // chunk consumed: store its assignments, registers -> the other buffer, fetch the chunk after
       __syncthreads();  // the last commit's q_node entry is visible
-      if (tid < CH) {
-        const uint32_t pd = rc.q_pod[buf][tid];
-        int nd = rc.q_node[buf][tid];
-        if (nd < -1) nd = NE + hs->node[-nd - 2];  // the mask run stores the slot
-        s.assign[pd] = nd;
-        s.place_seq[pd] = seq0 + (cb - qi0) + tid;
-      }
+      run_store_chunk(e, buf, CH, seq0 + (cb - qi0));
       buf ^= 1;
       cb += CH;
       i = 0;
-      if (tid < CH) {
-        rc.q_pod[buf][tid] = nx_pod; rc.q_cls[buf][tid] = nx_cls;
-        const unsigned mm = __ballot_sync(0xffffffffu, nx_cls != cls);
-        if (lane == 0 && mm) atomicMin(&rc.q_end[buf], (tid & ~31) + __ffs(mm) - 1);
-        const int idx2 = cb + CH + tid;
-        nx_cls = KSCHED_NONE;
-        if (idx2 < s.n_pods) { nx_pod = s.order[idx2]; nx_cls = (uint32_t)ffd_rows[idx2].reserved; }
-      }
+      if (tid < CH) stage(buf, nx_pod, nx_cls);
       __syncthreads();
       if (tid == 0) rc.q_end[buf ^ 1] = CH;  // the consumed buffer: its next atomicMin comes after the next chunk's first barrier
     }
     if (rc.q_cls[buf][i] != cls) break;  // class change or end of the first pass
+    if (m1_ok && !m1_built) {
 #ifdef KSCHED_PROFILE_PACK
-    const long long m1_t0 = clock64();
+      const long long m1_t0 = clock64();
 #endif
-    if (m1_ok) {
-      if (!m1_built) {
-        // ---- build the lists (once per call; nothing of this call has been committed yet, so nn_last is free as scratch)
-        m1_built = true;
-        uint8_t* t_b = reinterpret_cast<uint8_t*>(hs->nn_last);              // bucket of slot a (0xFF: not a member)
-        uint16_t* t_pos = reinterpret_cast<uint16_t*>(t_b + kTopoCap);        // its arrival order inside the bucket
-        uint16_t* t_slot = t_pos + kTopoCap;                                  // members, bucket by bucket, unsorted
-        uint32_t* t_tie = reinterpret_cast<uint32_t*>(t_slot + kTopoCap);     // their tie-breaks
-        for (int b = tid; b < kM1Lv * kM1Lists; b += T) m1.bcnt[b] = 0;
-        if (tid == 0) m1.bad = 0;
-        __syncthreads();
-        for (int a = tid; a < n_active; a += T) {
-          const uint32_t rp = rpv[a];
-          int b = 0xFF;
-          if ((rp & 0xFFFF) != 0 && !(rp & kRpDead)) {
-            const uint32_t z = zv[a], adm = z & 0xFFFF;
-            const unsigned cn = (unsigned)(hs->key[a] >> 32);
-            int list = -1;
-            if (adm && !(adm & (adm - 1)) && (z & (1u << 16))) {  // pinned to one domain
-              if (adm & m_reg0) list = __ffs(adm) - 1;             // (a domain that is not registered never admits a pod)
-            } else if ((adm & m_reg0) == m_reg0) list = kM1Dom;     // admits every registered domain
-            else if (adm & m_reg0) m1.bad = 1;                      // some of them: per-pod loop
-            if (list >= 0) {
-              if (cn >= (unsigned)kM1Lv) m1.bad = 1;
-              else { b = list * kM1Lv + (int)cn; t_pos[a] = (uint16_t)atomicAdd(&m1.bcnt[b], 1); }
-            }
-          }
-          t_b[a] = (uint8_t)b;
-        }
-        __syncthreads();
-        if (warp == 0) {  // exclusive scan of the bucket sizes -> arr segments
-          int run = 0;
-          for (int b0 = 0; b0 < kM1Lv * kM1Lists; b0 += 32) {
-            const int b = b0 + lane;
-            const int v = b < kM1Lv * kM1Lists ? m1.bcnt[b] : 0;
-            int inc = v;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
-            if (b < kM1Lv * kM1Lists) {
-              const int list = b / kM1Lv, lv = b - list * kM1Lv;
-              m1.ap[lv][list] = (uint16_t)(run + inc - v);
-              m1.ae[lv][list] = (uint16_t)(run + inc);
-            }
-            run += __shfl_sync(0xffffffffu, inc, 31);
-          }
-        }
-        __syncthreads();
-        const bool bad = m1.bad != 0;
-        if (!bad) {
-          for (int a = tid; a < n_active; a += T) {
-            const int b = t_b[a];
-            if (b == 0xFF) continue;
-            const int list = b / kM1Lv, lv = b - list * kM1Lv;
-            const int j = m1.ap[lv][list] + t_pos[a];
-            t_slot[j] = (uint16_t)a;
-            t_tie[j] = (uint32_t)hs->key[a];
-          }
-        }
-        __syncthreads();
-        if (!bad) {
-          for (int a = tid; a < n_active; a += T) {
-            const int b = t_b[a];
-            if (b == 0xFF) continue;
-            const int list = b / kM1Lv, lv = b - list * kM1Lv;
-            const int p0 = m1.ap[lv][list], p1 = m1.ae[lv][list];
-            const uint32_t tie = (uint32_t)hs->key[a];
-            int rank = 0;
-            for (int j = p0; j < p1; ++j) rank += t_tie[j] < tie;
-            m1_arr[p0 + rank] = (uint16_t)a;
-            t_pos[a] = (uint16_t)(p0 + rank);
-          }
-        }
-        __syncthreads();
-        if (!bad) {  // link every list (its buckets are contiguous in arr), tails and heads
-          for (int a = tid; a < n_active; a += T) {
-            const int b = t_b[a];
-            if (b == 0xFF) continue;
-            const int list = b / kM1Lv, gp = t_pos[a];
-            m1_nxt[a] = gp + 1 < (int)m1.ae[kM1Lv - 1][list] ? m1_arr[gp + 1] : kM1None;
-          }
-          for (int b = tid; b < kM1Lv * kM1Lists; b += T) {
-            const int list = b / kM1Lv, lv = b - list * kM1Lv;
-            m1.tl[lv][list] = m1.ae[lv][list] > m1.ap[lv][list] ? m1_arr[m1.ae[lv][list] - 1] : kM1None;
-          }
-          if (tid < kM1Lists) m1.head[tid] = m1.ae[kM1Lv - 1][tid] > m1.ap[0][tid] ? m1_arr[m1.ap[0][tid]] : kM1None;
-          if (tid == 0) m1.upos = m1.ap[0][kM1Dom];
-        }
-        __syncthreads();
-        if (bad) m1_ok = false;
+      m1_built = true;
+      m1_ok = m1_build(e, n_active);
 #ifdef KSCHED_PROFILE_PACK
-        if (tid == 0) { s.counters[38] += clock64() - m1_t0; s.counters[47] += bad ? 1 : 0; }
+      if (tid == 0) { s.counters[kCtrMaskBuildCycles] += clock64() - m1_t0; s.counters[kCtrMaskBuildRefused] += m1_ok ? 0 : 1; }
 #endif
-      }
     }
-#ifdef KSCHED_PROFILE_PACK
-    const long long m1_t1 = clock64();
-#endif
     if (m1_ok) {
-      if (warp == 0) {
-        const int L = lane;
-        const unsigned FULL = 0xffffffffu;
-        int cnt_d = L < kM1Dom ? rc.cnt[0][0][L] : 0;
-        const bool valid = L < kM1Dom && ((m_reg0 >> L) & 1);
-        // this lane's list: head (slot, key, room word), the node after it, the tail of the head's bucket, the first node
-        // behind that bucket and its pod count
-        int h = -1, n1 = -1, tcur = -1, bn = -1, bnc = 0;
-        unsigned long long hk = ~0ull, nk = ~0ull;
-        uint32_t hr = 0, nr = 0;
-        auto nxt_of = [&](int sl) -> int { const uint16_t v = m1_nxt[sl]; return v == kM1None ? -1 : (int)v; };
-        auto level_state = [&]() {
-          if (h < 0) { tcur = -1; bn = -1; bnc = 0; return; }
-          tcur = m1.tl[(int)(hk >> 32)][L];
-          bn = nxt_of(tcur);
-          bnc = bn >= 0 ? (int)(hs->key[bn] >> 32) : 0;
-        };
-        if (L < kM1Lists) {
-          h = m1.head[L] == kM1None ? -1 : (int)m1.head[L];
-          if (h >= 0) { hk = hs->key[h]; hr = rpv[h]; n1 = nxt_of(h); }
-          if (n1 >= 0) { nk = hs->key[n1]; nr = rpv[n1]; }
-          level_state();
-        }
-        // node a (key ak, room word ar) enters this lane's list at the FRONT of the block of count La
-        auto insert_front = [&](int a, int La, unsigned long long ak, uint32_t ar) {
-          const int hl = h >= 0 ? (int)(hk >> 32) : 0x7fffffff;
-          if (hl >= La) {  // nothing lies below: the new head
-            m1_nxt[a] = h >= 0 ? (uint16_t)h : kM1None;
-            if (hl > La) { m1.tl[La][L] = (uint16_t)a; tcur = a; bn = h; bnc = hl; }
-            n1 = h; nk = hk; nr = hr;
-            h = a; hk = ak; hr = ar;
-          } else if (bn < 0 || bnc >= La) {  // right behind the head's bucket
-            m1_nxt[a] = bn >= 0 ? (uint16_t)bn : kM1None;
-            m1_nxt[tcur] = (uint16_t)a;
-            if (bn < 0 || bnc > La) m1.tl[La][L] = (uint16_t)a;
-            if (tcur == h) { n1 = a; nk = ak; nr = ar; }
-            bn = a; bnc = La;
-          } else {  // behind the last bucket below La (the head's level is not the one)
-            int lv = La - 1;
-            while (m1.tl[lv][L] == kM1None) --lv;
-            const int pred = m1.tl[lv][L];
-            m1_nxt[a] = m1_nxt[pred];
-            m1_nxt[pred] = (uint16_t)a;
-            if (m1.tl[La][L] == kM1None) m1.tl[La][L] = (uint16_t)a;
-            if (pred == h) { n1 = a; nk = ak; nr = ar; }
-            if (pred == tcur) { bn = a; bnc = La; }
-          }
-        };
-        // a fresh node (count 1, the largest tie-break so far) enters at the END of the block of count 1
-        auto insert_back1 = [&](int a, unsigned long long ak, uint32_t ar) {
-          const int hl = h >= 0 ? (int)(hk >> 32) : 0x7fffffff;
-          if (hl > 1) {
-            m1_nxt[a] = h >= 0 ? (uint16_t)h : kM1None;
-            m1.tl[1][L] = (uint16_t)a;
-            tcur = a; bn = h; bnc = hl;
-            n1 = h; nk = hk; nr = hr;
-            h = a; hk = ak; hr = ar;
-          } else if (hl == 1) {
-            m1_nxt[a] = bn >= 0 ? (uint16_t)bn : kM1None;
-            m1_nxt[tcur] = (uint16_t)a;
-            m1.tl[1][L] = (uint16_t)a;
-            if (tcur == h) { n1 = a; nk = ak; nr = ar; }
-            tcur = a;
-          } else {  // nodes without pods in front (not produced by the scheduler, kept exact anyway)
-            int lv = 1;
-            while (m1.tl[lv][L] == kM1None) --lv;
-            const int pred = m1.tl[lv][L];
-            m1_nxt[a] = m1_nxt[pred];
-            m1_nxt[pred] = (uint16_t)a;
-            m1.tl[1][L] = (uint16_t)a;
-            if (pred == h) { n1 = a; nk = ak; nr = ar; }
-            if (pred == tcur) { bn = a; bnc = 1; }
-          }
-        };
-        // the head (pod count c) leaves this lane's list: the node behind it moves up, the one behind that is fetched (it is used
-        // at this list's next pop)
-        auto pop_head = [&](int c) {
-          h = n1; hk = nk; hr = nr;
-          n1 = -1; nk = ~0ull; nr = 0;
-          if (h >= 0) {
-            n1 = nxt_of(h);
-            if (n1 >= 0) { nk = hs->key[n1]; nr = rpv[n1]; }
-          }
-          if (h < 0 || (int)(hk >> 32) != c) {  // the bucket of count c is exhausted
-            m1.tl[c][L] = kM1None;
-            level_state();
-          }
-        };
-        // skew 1 with a self-matching selector: only the domains with the fewest pods admit a pod, so once every one of them has
-        // a pinned node at hand and the unpinned nodes come later in the order, the next pods go one to each of these domains,
-        // smallest head key first - a whole round is committed at once, every lane its own domain
-        const bool rounds = m_rec0 && m_bias0 == 0;
-        int li = i, ltick = tick, lnew = n_new, lact = n_active, nfr = 0;
-        // a round's commit of one pod on the pinned node a (pod count c, room word rp) with tick mytick, staged entry q:
-        // Topology.Record, the node's new key and room word (returned); closed: the class no longer fits anywhere on it
-        auto commit_round = [&](int a, uint32_t rp, int c, int mytick, int q, bool& closed) -> uint32_t {
-          const uint32_t rp2 = run_record_host(rc, hc, n_host, a, rp, 1);
-          unsigned long long skey = order_key(c + 1, -(mytick + 1));
-          rc.q_node[buf][q] = -(a + 2);
-          if ((rp2 & 0xFFFF) == 0 && run_closes(hs, a, rp2, p_req, min_req, RH)) {
-            skey = ~0ull;
-            hs->nn_last[a] = ((unsigned long long)(unsigned)(c + 1) << 32) | (unsigned)(-(mytick + 1));
-            closed = true;
-          }
-          hs->key[a] = skey;
-          rpv[a] = rp2;
-          return rp2;
-        };
-        unsigned fr_used = 0;  // ring slots the nodes created in this entry replay: a store fetch must not overwrite them
-        int i_end = rc.q_end[buf];
-        if (i + qlen < i_end) i_end = i + qlen;
-        int reason = 0;  // 0: the staged entries of the class are consumed; 1: the pod at li needs generic_step; 2: per-pod loop from li on
-        // count + self - min <= maxSkew as count - min <= slack in 32 bits: counts are pod counts (< 2^30), so a slack of 2^30
-        // or more admits every domain exactly like the 64-bit form of the per-pod loop
-        const int slack = m_bias0 < -(1 << 30) ? (1 << 30) : -m_bias0;
-        while (li < i_end) {
 #ifdef KSCHED_PROFILE_PACK
-          const long long it0 = clock64();
+      const long long m1_t1 = clock64();
 #endif
-          const int mn = __reduce_min_sync(FULL, valid ? cnt_d : INT32_MAX);
-          const bool allowed = valid && cnt_d - mn <= slack;
-          const unsigned okm = __ballot_sync(FULL, allowed);
-          const bool cand_ok = L < kM1Dom ? allowed : (L == kM1Dom && okm != 0);  // an empty list keeps hk = ~0
-          const unsigned long long key = cand_ok ? hk : ~0ull;
-          const unsigned long long wkey = warp_min_u64(key);
-#ifdef KSCHED_PROFILE_PACK
-          {  // how often a whole round (one pod per admissible domain, all from pinned lists) could be placed at once
-            const unsigned have = __ballot_sync(FULL, L < kM1Dom && allowed && h >= 0);
-            const unsigned long long ukey = __shfl_sync(FULL, hk, kM1Dom);
-            unsigned long long mx = (L < kM1Dom && allowed && h >= 0) ? hk : 0ull;
-            for (int o = 16; o; o >>= 1) { const unsigned long long t = __shfl_xor_sync(FULL, mx, o); mx = t > mx ? t : mx; }
-            const int na = __popc(okm);
-            if (L == 0 && na > 1 && have == okm && ukey > mx && i_end - li >= na) s.counters[17] += 1;
-            if (L == 0) s.counters[18] += 1;
-            if (L == 0 && na > 1) s.counters[19] += 1;
-          }
-#endif
-          if (rounds) {
-            const int na = __popc(okm);
-            if (na > 1 && i_end - li >= na) {
-              const bool act = L < kM1Dom && allowed;
-              const bool hd = act && h >= 0;                       // this domain's pod goes to the head of its list
-              const unsigned hv = __ballot_sync(FULL, hd), fv = okm & ~hv;  // fv: domains that get a fresh node (no pinned node at hand)
-              const bool bad_l = hd && ((hr & 0xFFFF) == kRoomSlow || (int)(hk >> 32) + 1 >= kM1Lv);
-              const unsigned long long ukey = __shfl_sync(FULL, hk, kM1Dom);
-              // ---- round stretch: when every registered domain admits a pod (all counts are equal), each round gives every
-              // domain one pod, so the counts stay equal and the round's shape repeats. R rounds are placed in one step
-              // while R single rounds would take the same nodes (DESIGN.md section 4): pinned, the r-th members of each
-              // head's bucket; fresh, R fresh nodes per domain that take no second pod.
-              int R = 0, vi_s = -1;
-              const bool pinned = hv == okm;
-              const int jd = __popc(okm & ((1u << L) - 1u));  // act: this domain's place among the round's domains
-#ifdef KSCHED_PROFILE_PACK
-              if (okm == m_reg0 && 2 * na <= i_end - li && 2 * na <= 32) {
-#else
-              if (s.use_round_stretch && okm == m_reg0 && 2 * na <= i_end - li && 2 * na <= 32) {
-#endif
-                const int cap = (i_end - li) / na < 32 / na ? (i_end - li) / na : 32 / na;
-                if (pinned) {  // the bucket's keys ascend; nodes re-entering at count + 1 lie behind it
-                  int rd = 0;
-                  if (act) {
-                    const int c = (int)(hk >> 32);
-                    int a = h;
-                    unsigned long long k = hk;
-                    uint32_t rp = hr;
-                    while (rd < cap && (int)(k >> 32) == c && k < ukey && (rp & 0xFFFF) != kRoomSlow && c + 1 < kM1Lv) {
-                      m1.ps[rd * na + jd] = (uint16_t)a;
-                      m1.rk[rd * na + jd] = k;
-                      ++rd;
-                      a = nxt_of(a);
-                      if (a < 0) break;
-                      k = hs->key[a];
-                      rp = rpv[a];
-                    }
-                  }
-                  R = __reduce_min_sync(FULL, act ? rd : 32);
-                } else if (hv == 0 && ukey == ~0ull && (okm & ~rc.m_tallow[0]) == 0) {  // fresh nodes that never re-enter a list
-                  if (act) for (int v2 = 0; v2 < rc.n_var && vi_s < 0; ++v2) if (rc.var[v2].dom[0] == L) vi_s = v2;
-                  const bool shut = vi_s >= 0 && ((rc.var[vi_s].rp & 0xFFFF) == 0 || (rc.var[vi_s].rp & kRpDead));
-                  bool ok = !__any_sync(FULL, act && !shut);
-                  for (int j = 0; j < n_host; ++j) ok = ok && rc.h_lim[j] >= 0;
-                  int room = MAXN - lnew;
-                  if (kActCap - lact < room) room = kActCap - lact;
-                  if (kTopoCap - lact < room) room = kTopoCap - lact;
-                  R = !ok ? 0 : room / na < cap ? room / na : cap;
-                }
-#ifdef KSCHED_PROFILE_PACK
-                if (L == 0 && R > 0) s.counters[64 + (pinned ? 0 : 16) + (R > 16 ? 16 : R) - 1] += 1;
-                if (!s.use_round_stretch) R = 0;
-#endif
-              }
-              if (R >= 2) {
-                const int np = R * na;
-                if (pinned) {
-                  const int c = (int)(hk >> 32);
-                  if (act) for (int r = 0; r < R; ++r) pop_head(c);  // (reads the keys of the bucket before they change)
-                  __syncwarp();
-                  bool closed_l = false;
-                  if (L < np) {  // pod L: round L / na, the node whose key has rank L % na in that round
-                    const int r = L / na, a = m1.ps[L];
-                    const unsigned long long k = m1.rk[L];
-                    int p = r * na;
-                    for (int j = 0; j < na; ++j) p += m1.rk[r * na + j] < k;
-                    commit_round(a, rpv[a], (int)(k >> 32), ltick + p, li + p, closed_l);
-                  }
-                  const unsigned tb = __ballot_sync(FULL, closed_l);
-                  if (L == 0 && tb) rc.tomb = rc.tomb + __popc(tb);
-                  __syncwarp();  // key and room words
-                  if (act) {  // the nodes that still accept enter the front of block c + 1, round by round
-                    for (int r = 0; r < R; ++r) {
-                      const int a = m1.ps[r * na + jd];
-                      const uint32_t rp2 = rpv[a];
-                      if ((rp2 & 0xFFFF) != 0 && !(rp2 & kRpDead)) insert_front(a, c + 1, hs->key[a], rp2);
-                    }
-                    cnt_d += R;
-                  }
-                } else {
-                  fr_used |= __reduce_or_sync(FULL, act ? 1u << vi_s : 0u);
-                  unsigned m = okm;  // pod L: round L / na, the (L % na)-th domain in id order
-                  for (int j = L % na; j > 0; --j) m &= m - 1;
-                  const int d = __ffs(m) - 1;
-                  const int vi = __shfl_sync(FULL, vi_s, d);
-                  if (L < np) {  // NewNode + Add replayed from the variant of the domain
-                    const RunVariant& v = rc.var[vi];
-                    const int n = lnew + L, a = lact + L;
-                    for (int j = 0; j < n_host; ++j) {
-                      const int times = rc.h_times[j];
-                      hc[j * kTopoCap + a] = (uint16_t)times;
-                      if (times) s.grp_host[(size_t)rc.h_row[j] * hstride + NE + n] = (uint16_t)times;
-                    }
-                    hs->key[a] = order_key(1, ltick + L + 1);
-#pragma unroll
-                    for (int r = 0; r < kHotRes; ++r) { hs->q[r][a] = v.q[r]; hs->bound[r][a] = v.b1[r]; hs->bound2[r][a] = v.b2[r]; }
-                    hs->node[a] = n;
-                    hs->flags[a] = v.fl;
-                    hs->absorbed[a] = simple ? cls : KSCHED_NONE;
-                    hs->rejected[a] = KSCHED_NONE;
-                    rpv[a] = v.rp;
-                    rc.q_node[buf][li + L] = NE + n;
-                    zv[a] = (1u << d) | (3u << 16);
-                    m1.fr[nfr + L] = (uint32_t)a | ((uint32_t)vi << 16);
-                  }
-                  if (L < n_host && rc.h_times[L]) rc.h_inc[L] = rc.h_inc[L] + np;
-                  if (act) cnt_d += R;
-                  lnew += np;
-                  lact += np;
-                  nfr += np;
-                }
-#ifdef KSCHED_PROFILE_PACK
-                if (L == 0) { s.counters[61] += clock64() - it0; s.counters[62] += 1; s.counters[63] += np; }
-#endif
-                ltick += np;
-                li += np;
-                __syncwarp();
-                continue;
-              }
-              const unsigned hi = hd ? (unsigned)(hk >> 32) : 0u;
-              const unsigned mhi = __reduce_max_sync(FULL, hi);
-              const unsigned mlo = __reduce_max_sync(FULL, (hd && hi == mhi) ? (unsigned)hk : 0u);
-              const unsigned long long mx = ((unsigned long long)mhi << 32) | mlo;  // largest head key of the round
-              // fresh nodes come last in a round, lowest domain id first (every admissible domain has the same count: run_pick
-              // takes the lowest id), and only when no unpinned node is left (it would be taken first)
-              int vi_l = -1;
-              const int nf = __popc(fv);
-              bool fresh_ok = true;
-              if (fv) {
-                const bool fl = act && h < 0;
-                if (fl) for (int v2 = 0; v2 < rc.n_var && vi_l < 0; ++v2) if (rc.var[v2].dom[0] == L) vi_l = v2;
-                fresh_ok = ukey == ~0ull && (fv & ~rc.m_tallow[0]) == 0 && !__any_sync(FULL, fl && vi_l < 0) && lnew + nf <= MAXN &&
-                           lact + nf <= kActCap && lact + nf <= kTopoCap;
-                for (int j = 0; j < n_host; ++j) fresh_ok = fresh_ok && rc.h_lim[j] >= 0;
-              }
-              if (fresh_ok && !__any_sync(FULL, bad_l) && (hv == 0 || ukey > mx)) {
-                fr_used |= __reduce_or_sync(FULL, (act && !hd) ? 1u << vi_l : 0u);
-                int rank = 0;  // position of this lane's node in the round
-                for (unsigned m = hv; m; m &= m - 1) {
-                  const unsigned long long k2 = __shfl_sync(FULL, hk, __ffs(m) - 1);
-                  rank += k2 < hk;
-                }
-                bool closed_l = false;
-                if (hd) {
-                  const int a = h;
-                  const uint32_t rp = hr;
-                  const int c = (int)(hk >> 32);
-                  const int mytick = ltick + rank;
-                  pop_head(c);
-                  const uint32_t rp2 = commit_round(a, rp, c, mytick, li + rank, closed_l);
-                  if ((rp2 & 0xFFFF) != 0 && !(rp2 & kRpDead)) insert_front(a, c + 1, order_key(c + 1, -(mytick + 1)), rp2);
-                  ++cnt_d;
-                } else if (act) {  // NewNode + Add replayed from the variant of this lane's domain
-                  const RunVariant& v = rc.var[vi_l];
-                  const int idx = __popc(fv & ((1u << L) - 1u));
-                  const int n = lnew + idx, a = lact + idx;
-                  const int mytick = ltick + __popc(hv) + idx;
-                  for (int j = 0; j < n_host; ++j) {
-                    const int times = rc.h_times[j];
-                    hc[j * kTopoCap + a] = (uint16_t)times;
-                    if (times) s.grp_host[(size_t)rc.h_row[j] * hstride + NE + n] = (uint16_t)times;
-                  }
-                  const unsigned long long fkey = order_key(1, mytick + 1);
-                  hs->key[a] = fkey;
-#pragma unroll
-                  for (int r = 0; r < kHotRes; ++r) { hs->q[r][a] = v.q[r]; hs->bound[r][a] = v.b1[r]; hs->bound2[r][a] = v.b2[r]; }
-                  hs->node[a] = n;
-                  hs->flags[a] = v.fl;
-                  hs->absorbed[a] = simple ? cls : KSCHED_NONE;
-                  hs->rejected[a] = KSCHED_NONE;
-                  rpv[a] = v.rp;
-                  rc.q_node[buf][li + __popc(hv) + idx] = NE + n;
-                  zv[a] = (1u << L) | (3u << 16);
-                  m1.fr[nfr + idx] = (uint32_t)a | ((uint32_t)vi_l << 16);
-                  if ((v.rp & 0xFFFF) != 0 && !(v.rp & kRpDead)) insert_back1(a, fkey, v.rp);
-                  ++cnt_d;
-                }
-                if (nf && L < n_host && rc.h_times[L]) rc.h_inc[L] = rc.h_inc[L] + nf;
-                const unsigned tb = __ballot_sync(FULL, closed_l);
-                if (L == 0 && tb) rc.tomb = rc.tomb + __popc(tb);
-#ifdef KSCHED_PROFILE_PACK
-                if (L == 0) { s.counters[61] += clock64() - it0; s.counters[62] += 1; s.counters[63] += na; }
-#endif
-                lnew += nf;
-                lact += nf;
-                nfr += nf;
-                ltick += na;
-                li += na;
-                __syncwarp();
-                continue;
-              }
-            }
-          }
-          if (wkey != ~0ull) {
-            const int wl = __ffs(__ballot_sync(FULL, key == wkey)) - 1;
-            if (wl == kM1Dom) {
-              // ---- pin step: the unpinned head wins, so the next pods take the next unpinned nodes one each, in list order
-              // (lane t: pod t), as long as no node of a domain list can come first: every member of the stretch has the
-              // first one's pod count c and a key below every pinned head (a node pinned by the stretch re-enters at c + 1).
-              // Pod t's domain is the t-th pick of run_pick's (count, id) order while the counts advance.
-              const int c = (int)(wkey >> 32);
-              const int upos = m1.upos;
-              int lim = i_end - li < 32 ? i_end - li : 32;
-              if (m1.ae[kM1Lv - 1][kM1Dom] - upos < lim) lim = m1.ae[kM1Lv - 1][kM1Dom] - upos;
-              const unsigned long long pmin = warp_min_u64(L < kM1Dom ? hk : ~0ull);
-              const bool in = L < lim;
-              const int a_t = in ? (int)m1_arr[upos + L] : 0;
-              const unsigned long long k_t = in ? hs->key[a_t] : ~0ull;
-              const uint32_t rp_t = in ? rpv[a_t] : 0u;
-              const uint32_t z_t = in ? zv[a_t] : 0u;
-              int d_t;
-              {
-                // domain e has a slot on every level >= its count; pod t takes the t-th slot in (level, id) order (without
-                // Record the counts stay, and every pod takes the first pick). Levels are counted from mn: pod t's level is
-                // at most t, so a domain more than 31 pods above mn never gets one. Byte e of dw: domain e's level.
-                const unsigned dl = !valid ? 0xFFu : (unsigned)(cnt_d - mn < 32 ? cnt_d - mn : 32);
-                const unsigned dw0 = __reduce_or_sync(FULL, L < 4 ? dl << (8 * L) : 0u);
-                const unsigned dw1 = __reduce_or_sync(FULL, L >= 4 && L < kM1Dom ? dl << (8 * (L - 4)) : 0u);
-                unsigned y = 0, r = m_rec0 ? L : 0, am;
-                while (true) {
-                  const unsigned yy = y * 0x01010101u;  // bit 0 of every byte of the compares -> bits 24..27 (no carries)
-                  am = (((__vcmpleu4(dw0, yy) & 0x01010101u) * 0x01020408u) >> 24) & 0xFu;
-                  am |= (((__vcmpleu4(dw1, yy) & 0x01010101u) * 0x01020408u) >> 20) & 0xF0u;
-                  const unsigned k = __popc(am);
-                  if (am == m_reg0) { r %= k; break; }  // every domain has a slot on every level from here on
-                  if (r < k) break;
-                  r -= k;
-                  ++y;
-                }
-                for (; r > 0; --r) am &= am - 1;
-                d_t = __ffs(am) - 1;
-              }
-              const bool same_c = (int)(k_t >> 32) == c, below = k_t < pmin;
-              const bool ok_t = in && same_c && below && (rp_t & 0xFFFF) != kRoomSlow && c + 1 < kM1Lv &&
-                                ((rc.m_neutral[0] >> d_t) & 1) && ((z_t & (1u << 17)) || rc.m_wk[0]);
-              const unsigned okb = __ballot_sync(FULL, ok_t);
-              const int J = okb == FULL ? 32 : __ffs(~okb) - 1;
-#ifdef KSCHED_PROFILE_PACK
-              if (J > 0 && L == J) s.counters[!in ? (lim == i_end - li ? 51 : 55) : !same_c ? 52 : !below ? 53 : 54] += 1;
-              if (J == 32 && L == 0) s.counters[55] += 1;
-              if (J > 0 && L == 0) { s.counters[49] += 1; s.counters[50] += J; }
-#endif
-              if (J > 0) {
-                bool closed_l = false;
-                if (L < J) {  // the single step's commit for pod L on node a_t, pinned to d_t
-                  const int a = a_t, mytick = ltick + L;
-                  const uint32_t rp2 = run_record_host(rc, hc, n_host, a, rp_t, 1);
-                  const int n = hs->node[a], k = rc.m_key[0];
-                  zv[a] = (1u << d_t) | (3u << 16);
-                  s.nn_vals[(size_t)k * MAXN + n] = 1ull << d_t;
-                  atomicOr(reinterpret_cast<unsigned long long*>(&s.nn_meta[n]), 1ull << (KSCHED_META_PRESENT_SHIFT + k));
-                  atomicAnd(reinterpret_cast<unsigned long long*>(&s.nn_meta[n]), ~(1ull << (KSCHED_META_COMPLEMENT_SHIFT + k)));
-                  rc.q_node[buf][li + L] = -(a + 2);
-                  unsigned long long skey = order_key(c + 1, -(mytick + 1));
-                  if ((rp2 & 0xFFFF) == 0 && run_closes(hs, a, rp2, p_req, min_req, RH)) {
-                    skey = ~0ull;
-                    hs->nn_last[a] = ((unsigned long long)(unsigned)(c + 1) << 32) | (unsigned)(-(mytick + 1));
-                    closed_l = true;
-                  }
-                  hs->key[a] = skey;
-                  rpv[a] = rp2;
-                  m1.ps[L] = (uint16_t)a;
-                }
-                const unsigned tb = __ballot_sync(FULL, closed_l);
-                if (L == 0 && tb) rc.tomb = rc.tomb + __popc(tb);
-                unsigned mine = 0;  // the pods of this lane's domain
-#pragma unroll
-                for (int e = 0; e < kM1Dom; ++e) {
-                  const unsigned b = __ballot_sync(FULL, L < J && d_t == e);
-                  if (L == e) mine = b;
-                }
-                __syncwarp();  // ps, key and room words
-                // the nodes that still accept enter their domain's list at the front of block c + 1, in pod order: the
-                // last one ends up first (the smallest tie-break)
-                for (unsigned m = mine; m; m &= m - 1) {
-                  const int t = __ffs(m) - 1, a = m1.ps[t];
-                  const uint32_t rp2 = rpv[a];
-                  if ((rp2 & 0xFFFF) != 0 && !(rp2 & kRpDead)) insert_front(a, c + 1, order_key(c + 1, -(ltick + t + 1)), rp2);
-                }
-                if (m_rec0) cnt_d += __popc(mine);
-                if (L == 0) m1.upos = upos + J;
-                if (L == kM1Dom) {  // the unpinned list's new head and the node behind it
-                  h = upos + J < (int)m1.ae[kM1Lv - 1][kM1Dom] ? (int)m1_arr[upos + J] : -1;
-                  hk = ~0ull; hr = 0; n1 = -1; nk = ~0ull; nr = 0;
-                  if (h >= 0) {
-                    hk = hs->key[h]; hr = rpv[h]; n1 = nxt_of(h);
-                    if (n1 >= 0) { nk = hs->key[n1]; nr = rpv[n1]; }
-                  }
-                  if (h < 0 || (int)(hk >> 32) != c) {  // the bucket of count c is exhausted
-                    m1.tl[c][L] = kM1None;
-                    level_state();
-                  }
-                }
-                ltick += J;
-                li += J;
-                __syncwarp();
-                continue;
-              }
-            }
-            const int a = __shfl_sync(FULL, h, wl);
-            const uint32_t rp = __shfl_sync(FULL, hr, wl);
-            if ((rp & 0xFFFF) == kRoomSlow) { reason = 1; break; }  // the winner needs the full evaluation
-            int d = wl;
-            const bool pin = wl == kM1Dom;
-            if (pin) {  // the placement pins the node's domain: fewest pods, lowest id among the admissible ones (run_pick)
-              const int mc = __reduce_min_sync(FULL, allowed ? cnt_d : INT32_MAX);
-              d = __ffs(__ballot_sync(FULL, allowed && cnt_d == mc)) - 1;
-              if (!((rc.m_neutral[0] >> d) & 1) || !((zv[a] & (1u << 17)) || rc.m_wk[0])) { reason = 1; break; }
-#ifdef KSCHED_PROFILE_PACK
-              if (L == 0) s.counters[48] += 1;
-#endif
-            }
-            const int c = (int)(wkey >> 32);
-            if (L == wl) pop_head(c);
-            if (pin && L == 0) m1.upos = m1.upos + 1;  // (read by the next pin step after the __syncwarp below)
-            // ---- commit (the per-pod loop's commit, relation by relation on the first lanes)
-            uint32_t rp2 = rp - 1 + (1u << 16);
-            bool dead_l = false;
-            if (L < n_host) {  // Topology.Record, hostname groups
-              const int times = rc.h_times[L];
-              const int old = hc[L * kTopoCap + a];
-              const int now = old + times > 0xFFFF ? 0xFFFF : old + times;
-              if (times) hc[L * kTopoCap + a] = (uint16_t)now;
-              dead_l = now > rc.h_lim[L];
-            }
-            if (n_host > 0 && __any_sync(FULL, dead_l)) rp2 |= kRpDead;
-            const unsigned long long nkey = order_key(c + 1, -(ltick + 1));
-            if (L == 0) {
-              unsigned long long skey = nkey;
-              if (pin) {  // requirements.Add(In{d}) on the node
-                const int n = hs->node[a], k = rc.m_key[0];
-                zv[a] = (1u << d) | (3u << 16);
-                s.nn_vals[(size_t)k * MAXN + n] = 1ull << d;
-                // two reductions instead of a read-modify-write: the load would stall the whole chain for an L2 round trip
-                atomicOr(reinterpret_cast<unsigned long long*>(&s.nn_meta[n]), 1ull << (KSCHED_META_PRESENT_SHIFT + k));
-                atomicAnd(reinterpret_cast<unsigned long long*>(&s.nn_meta[n]), ~(1ull << (KSCHED_META_COMPLEMENT_SHIFT + k)));
-              }
-              rc.q_node[buf][li] = -(a + 2);  // the slot: translated to the node when the chunk is stored
-              if ((rp2 & 0xFFFF) == 0 && run_closes(hs, a, rp2, p_req, min_req, RH)) {
-                skey = ~0ull;
-                hs->nn_last[a] = ((unsigned long long)(unsigned)(c + 1) << 32) | (unsigned)(-(ltick + 1));
-                rc.tomb = rc.tomb + 1;
-              }
-              hs->key[a] = skey;
-              rpv[a] = rp2;
-            }
-            if ((rp2 & 0xFFFF) != 0 && !(rp2 & kRpDead)) {  // still accepts the class: front of the block of count + 1
-              if (c + 1 >= kM1Lv) reason = 2;
-              else if (L == d) insert_front(a, c + 1, nkey, rp2);
-            }
-            if (m_rec0 && L == d) ++cnt_d;
-            ++ltick;
-            ++li;
-            __syncwarp();  // lane 0's key / room words before a later pop fetches them
-            if (reason == 2) break;
-          } else {
-            // ---- nobody accepts: NewNode + Add replayed from the variant of the domain a fresh node gets
-            if (lnew >= MAXN || lact >= kActCap || lact >= kTopoCap) { reason = 1; break; }
-            bool ok = true;
-            for (int j = 0; j < n_host; ++j) ok = ok && rc.h_lim[j] >= 0;
-            const unsigned cand = rc.m_tallow[0] & okm;
-            if (!ok || !cand) { reason = 1; break; }
-            const bool in_c = (cand >> L) & 1;  // (cand is a subset of okm: lanes below kM1Dom)
-            const int mc = __reduce_min_sync(FULL, in_c ? cnt_d : INT32_MAX);
-            const int fd = __ffs(__ballot_sync(FULL, in_c && cnt_d == mc)) - 1;
-            int vi = -1;
-            for (int v2 = 0; v2 < rc.n_var && vi < 0; ++v2) if (rc.var[v2].dom[0] == fd) vi = v2;
-            if (vi < 0 && rc.vs_ok && !((fr_used >> rc.var_next) & 1))
-              vi = vs_fetch(rc, cls, vs_pattern(1, rc.m_key, fd, 0), L);
-            if (vi < 0) {
-              reason = 1;
-#ifdef KSCHED_PROFILE_PACK
-              cr_novar = 1;
-#endif
-              break;
-            }
-            const RunVariant& v = rc.var[vi];
-            fr_used |= 1u << vi;
-            const int n = lnew, a = lact;
-            if (L < n_host) {
-              const int times = rc.h_times[L];
-              hc[L * kTopoCap + a] = (uint16_t)times;
-              if (times) {
-                s.grp_host[(size_t)rc.h_row[L] * hstride + NE + n] = (uint16_t)times;
-                rc.h_inc[L] = rc.h_inc[L] + 1;
-              }
-            }
-            const unsigned long long fkey = order_key(1, ltick + 1);
-            if (L == 0) {
-              hs->key[a] = fkey;
-#pragma unroll
-              for (int r = 0; r < kHotRes; ++r) { hs->q[r][a] = v.q[r]; hs->bound[r][a] = v.b1[r]; hs->bound2[r][a] = v.b2[r]; }
-              hs->node[a] = n;
-              hs->flags[a] = v.fl;
-              hs->absorbed[a] = simple ? cls : KSCHED_NONE;
-              hs->rejected[a] = KSCHED_NONE;
-              rpv[a] = v.rp;
-              rc.q_node[buf][li] = NE + n;
-              zv[a] = (1u << fd) | (3u << 16);
-              m1.fr[nfr] = (uint32_t)a | ((uint32_t)vi << 16);  // nothing in this loop reads the node's global state
-            }
-            ++nfr;
-            if (L == fd) {
-              if ((v.rp & 0xFFFF) != 0 && !(v.rp & kRpDead)) insert_back1(a, fkey, v.rp);  // accepts further pods of the class
-              if (m_rec0) ++cnt_d;
-            }
-            ++ltick; ++lnew; ++lact; ++li;
-            __syncwarp();
-          }
-        }
-        __syncwarp();
-        // every warp's copy of the spread counters follows (the per-pod loop and the write-back read them)
-        if (L < kM1Dom) for (int w = 0; w < nwarps; ++w) rc.cnt[w][0][L] = cnt_d;
-        if (L < kM1Lists) m1.head[L] = h >= 0 ? (uint16_t)h : kM1None;
-        if (L == 0) { m1.out_adv = li - i; m1.out_reason = reason; m1.out_tick = ltick; m1.out_n_new = lnew; m1.out_n_active = lact; m1.n_fresh = nfr; }
-      }
+      if (warp == 0) m1_walk(e, buf, i, qlen, tick, n_new, n_active, novar);
       __syncthreads();
-      {  // the global state of the nodes the mask run created, 64 words per node across the CTA
-        const int nfr = m1.n_fresh;
-        for (int e = tid; e < nfr * 64; e += T) {
-          const uint32_t rec = m1.fr[e >> 6];
-          const int a = (int)(rec & 0xFFFF), w = e & 63;
-          const RunVariant& v = rc.var[rec >> 16];
-          const int n = hs->node[a];
-          if (w < W32) s.nn_opts[(size_t)w * MAXN + n] = v.opts[w];
-          if (w < c.n_keys) s.nn_vals[(size_t)w * MAXN + n] = v.vals[w];
-          if (w < KSCHED_MAX_RES) s.nn_req[(size_t)w * MAXN + n] = v.q[w];
-          if (w == 0) {
-            s.nn_meta[n] = v.meta;
-            s.nn_tmpl[n] = (uint8_t)(v.fl >> 8);
-            s.nn_req_present[n] = v.qp;
-            s.nn_hp[n] = 0;
-            if (((rpv[a] >> 16) & 0x7FFF) == 0) {  // no further pod so far: (1, creation tick); otherwise the run's write-back stores them
-              s.nn_count[n] = 1;
-              s.nn_tb[n] = (int)((unsigned)hs->key[a] ^ 0x80000000u);
-            }
-          }
-        }
-      }
-      const int m_adv = m1.out_adv, m_reason = m1.out_reason;
-      tick = m1.out_tick; n_new = m1.out_n_new; n_active = m1.out_n_active;
+      m1_store_fresh(e);
+      const int m_adv = g_m1.out_adv, m_reason = g_m1.out_reason;
+      tick = g_m1.out_tick; n_new = g_m1.out_n_new; n_active = g_m1.out_n_active;
       qi += m_adv;
       qlen -= m_adv;
       __syncthreads();  // out_* are rewritten by the next entry
 #ifdef KSCHED_PROFILE_PACK
-      if (tid == 0) { s.counters[6] += clock64() - m1_t1; s.counters[7] += m_adv; s.counters[16] += 1; }
+      if (tid == 0) { s.counters[kCtrMaskCycles] += clock64() - m1_t1; s.counters[kCtrMaskPods] += m_adv; s.counters[kCtrMaskEntries] += 1; }
 #endif
       if (m_reason == 1) { status = 1; break; }
       if (qlen == 0) break;
@@ -2391,71 +2768,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
       continue;
     }
     if (lvl && n_active > 0 && n_active <= 32 && s.use_level_warp) {
-      // ---- at most 32 open nodes: the level / fill steps of the block below with ONE node per lane of warp 0 and no block
-      // barrier (slot a belongs to thread a, as in the block-wide form). Fresh nodes and winners that need the full evaluation
-      // go to the block-wide iteration below.
-      if (warp == 0) {
-        const unsigned FULL = 0xffffffffu;
-        const int a = lane;
-        const bool mine = a < n_active;
-        int li = i, ltick = tick, reason = 0;
-        int i_end = rc.q_end[buf];
-        if (i + qlen < i_end) i_end = i + qlen;
-        while (li < i_end) {
-          const uint32_t rp = mine ? rpv[a] : 0u;
-          const unsigned long long key = mine ? hs->key[a] : ~0ull;
-          const bool el = mine && (rp & 0xFFFF) != 0 && !(rp & kRpDead);
-          const unsigned elm = __ballot_sync(FULL, el);
-          if (!elm || __any_sync(FULL, el && (rp & 0xFFFF) == kRoomSlow)) { reason = 1; break; }
-          const unsigned cn = el ? (unsigned)(key >> 32) : 0xFFFFFFFFu;
-          const unsigned c_min = __reduce_min_sync(FULL, cn);
-          const bool mem = el && cn == c_min;
-          const unsigned memm = __ballot_sync(FULL, mem);
-          const int k_av = i_end - li;
-          int t = 1, rank = 0, adv_w;
-          if (!(elm & (elm - 1))) {  // fill: the only accepting node takes pods until it refuses
-            int cap = (int)(rp & 0xFFFF);
-            if (mem) {
-              for (int j = 0; j < n_host; ++j) {
-                const int times = rc.h_times[j], lim = rc.h_lim[j];
-                if (!times || lim >= 0x10000) continue;
-                if (lim >= 0xFFF0) { cap = 1; continue; }
-                const int td = (lim - (int)hc[j * kTopoCap + a]) / times + 1;
-                cap = td < cap ? td : cap;
-              }
-            }
-            t = __shfl_sync(FULL, cap, __ffs(memm) - 1);
-            t = t < k_av ? t : k_av;
-            adv_w = t;
-          } else {  // level: the accepting nodes with the fewest pods, one pod each in tie order
-            const unsigned tie = (unsigned)key;
-            for (unsigned m = memm; m; m &= m - 1) {
-              const unsigned tm = __shfl_sync(FULL, tie, __ffs(m) - 1);
-              rank += tm < tie;
-            }
-            const int n_s = __popc(memm);
-            adv_w = n_s < k_av ? n_s : k_av;
-          }
-          if (mem && rank < adv_w) {  // (fill: rank 0 < t)
-            const uint32_t rp2 = run_record_host(rc, hc, n_host, a, rp, t);
-            const int count = (int)c_min + t;
-            const int tb = -(ltick + rank + t);
-            unsigned long long nkey = order_key(count, tb);
-            const int nd = NE + hs->node[a];
-            for (int e = 0; e < t; ++e) rc.q_node[buf][li + rank + e] = nd;
-            if ((rp2 & 0xFFFF) == 0 && run_closes(hs, a, rp2, p_req, min_req, RH)) {
-              nkey = ~0ull;
-              hs->nn_last[a] = ((unsigned long long)(unsigned)count << 32) | (unsigned)tb;
-              atomicAdd(&rc.tomb, 1);
-            }
-            hs->key[a] = nkey;
-            rpv[a] = rp2;
-          }
-          ltick += adv_w;
-          li += adv_w;
-        }
-        if (lane == 0) { g_m1.out_adv = li - i; g_m1.out_reason = reason; g_m1.out_tick = ltick; }
-      }
+      if (warp == 0) run_level_warp(e, buf, i, qlen, tick, n_active);
       __syncthreads();
       const int w_adv = g_m1.out_adv, w_reason = g_m1.out_reason;
       tick = g_m1.out_tick;
@@ -2465,341 +2778,28 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
       __syncthreads();  // out_* are rewritten by the next entry
       if (qlen == 0) break;
       if (w_reason == 0) continue;  // the staged entries of the class are consumed
-      // w_reason == 1: the pod at i takes the block-wide iteration (fresh nodes / full evaluation)
+      // w_reason == 1: the pod at i takes the block-wide steps (fresh nodes / full evaluation)
     }
     int adv = 1;       // pods this iteration consumes
-    int mode = 0;      // 0: per-pod argmin below; 1: placed by a level / fill step; 2: nobody accepts (fresh node)
+    int mode = 0;      // 0: per-pod argmin step; 1: placed by a level / fill step; 2: nobody accepts (fresh node)
     int k_avail = 1;   // pods of the class that may be consumed now: staged, same class, still queued
     if (lvl) {
-      // ---- classes without mask-key spread: a node's verdict depends on the node alone, so
-      //  * level step: the n accepting nodes with the fewest pods take the next n pods one each, in tie order (each leaves
-      //    for the block of count + 1, behind every node of the level);
-      //  * fill step: the only accepting node takes pods until it refuses (resources / hostname limits);
-      //  * a fresh node is filled the same way in the iteration that creates it.
       k_avail = rc.q_end[buf] - i;
       k_avail = k_avail < qlen ? k_avail : qlen;
-      unsigned cmin = 0xFFFFFFFFu;
-      int ne = 0;
-      bool slow = false;
-      for (int a = tid; a < n_active; a += T) {
-        const uint32_t rp = rpv[a];
-        if ((rp & 0xFFFF) != 0 && !(rp & kRpDead)) {  // tombstones have no room
-          const unsigned cn = (unsigned)(hs->key[a] >> 32);
-          cmin = cn < cmin ? cn : cmin;
-          ++ne;
-          slow = slow || (rp & 0xFFFF) == kRoomSlow;
-        }
-      }
-      const unsigned wc = __reduce_min_sync(0xffffffffu, cmin);
-      const unsigned wn = __reduce_add_sync(0xffffffffu, (unsigned)ne) | (__any_sync(0xffffffffu, slow) ? 0x80000000u : 0u);
-      if (lane == 0) rc.red_key[parity][warp] = ((unsigned long long)wc << 32) | wn;
-      __syncthreads();
-      const unsigned long long rr = lane < nwarps ? rc.red_key[parity][lane] : 0xFFFFFFFF00000000ull;
-      parity ^= 1;
-      const unsigned c_min = __reduce_min_sync(0xffffffffu, (unsigned)(rr >> 32));
-      const int n_el = (int)__reduce_add_sync(0xffffffffu, (unsigned)rr & 0x7FFFFFFFu);
-      const bool any_slow = __any_sync(0xffffffffu, ((unsigned)rr >> 31) != 0);
-      if (!any_slow) {
-        if (n_el == 0) mode = 2;
-        else {
-          mode = 1;
-          const int lp = lvp;
-          lvp ^= 1;
-          if (tid == 0) rc.lv_cnt[lp ^ 1] = 0;  // last read before this iteration's first barrier
-          // the level's members append their tie-breaks to the list (any order)
-          for (int base = 0; base < n_active; base += T) {
-            const int a = base + tid;
-            bool mem = false;
-            unsigned tie = 0;
-            if (a < n_active) {
-              const uint32_t rp = rpv[a];
-              const unsigned long long key = hs->key[a];
-              mem = (rp & 0xFFFF) != 0 && !(rp & kRpDead) && (unsigned)(key >> 32) == c_min;
-              tie = (unsigned)key;
-              if (mem && n_el == 1) {  // fill: how many pods this node takes before it refuses
-                int cap = (int)(rp & 0xFFFF);
-                for (int j = 0; j < n_host; ++j) {
-                  const int times = rc.h_times[j], lim = rc.h_lim[j];
-                  if (!times || lim >= 0x10000) continue;
-                  if (lim >= 0xFFF0) { cap = 1; continue; }  // saturating counters nearby: one pod at a time
-                  const int td = (lim - (int)hc[j * kTopoCap + a]) / times + 1;
-                  cap = td < cap ? td : cap;
-                }
-                rc.lv_fill[lp] = cap < k_avail ? cap : k_avail;
-              }
-            }
-            const unsigned bal = __ballot_sync(0xffffffffu, mem);
-            if (bal) {
-              const int src = __ffs(bal) - 1;
-              int pos0 = 0;
-              if (lane == src) pos0 = atomicAdd(&rc.lv_cnt[lp], __popc(bal));
-              pos0 = __shfl_sync(0xffffffffu, pos0, src);
-              if (mem) lvt[pos0 + __popc(bal & ((1u << lane) - 1u))] = tie;
-            }
-          }
-          __syncthreads();
-          const int n_s = rc.lv_cnt[lp];
-          const int t_fill = n_el == 1 ? rc.lv_fill[lp] : 1;
-          const int k_lvl = n_el == 1 ? 1 : (n_s < k_avail ? n_s : k_avail);
-          adv = n_el == 1 ? t_fill : k_lvl;
-          CR_IT(n_el == 1 ? 1 : 0)
-          for (int a = tid; a < n_active; a += T) {
-            const uint32_t rp = rpv[a];
-            const unsigned long long key = hs->key[a];
-            if (!((rp & 0xFFFF) != 0 && !(rp & kRpDead) && (unsigned)(key >> 32) == c_min)) continue;
-            const unsigned tie = (unsigned)key;
-            int rank = 0;
-            if (n_el != 1) {
-              int j = 0;
-              for (; j + 4 <= n_s; j += 4) {
-                const uint4 v = *reinterpret_cast<const uint4*>(lvt + j);
-                rank += (v.x < tie) + (v.y < tie) + (v.z < tie) + (v.w < tie);
-              }
-              for (; j < n_s; ++j) rank += lvt[j] < tie;
-              if (rank >= k_lvl) continue;
-            }
-            // the owner commits: pods i + rank .. i + rank + t - 1 of the chunk
-            const int t = t_fill;
-            const uint32_t rp2 = run_record_host(rc, hc, n_host, a, rp, t);
-            const int count = (int)c_min + t;
-            const int tb = -(tick + rank + t);
-            unsigned long long nkey = order_key(count, tb);
-            const int nd = NE + hs->node[a];
-            for (int e = 0; e < t; ++e) rc.q_node[buf][i + rank + e] = nd;
-            if ((rp2 & 0xFFFF) == 0 && run_closes(hs, a, rp2, p_req, min_req, RH)) {
-              nkey = ~0ull;
-              hs->nn_last[a] = ((unsigned long long)(unsigned)count << 32) | (unsigned)tb;
-              atomicAdd(&rc.tomb, 1);
-            }
-            hs->key[a] = nkey;
-            rpv[a] = rp2;
-          }
-          tick += adv;
-        }
-      }
+      bool fill = false;
+      mode = run_level_block(e, buf, i, k_avail, n_active, tick, parity, lvp, adv, fill);
+      if (mode == 1) { CR_IT(fill ? 1 : 0) }
     }
-    // node-independent half of nextDomainTopologySpread, one domain per lane: min count over the pod's domains, the
-    // domains within max-skew (count + self - min <= maxSkew)
     uint32_t okm0 = 0, okm1 = 0;
-    int fd0 = 0, fd1 = 0;
     if (mode == 0) {
-    CR_IT(3)
-    if (n_mask > 0) {
-      const bool valid = (m_reg0 >> lane) & 1;  // registered domains have ids < kRunDom
-      const int cn = rc.cnt[warp][0][lane & (kRunDom - 1)];
-      const int mn = __reduce_min_sync(0xffffffffu, valid ? cn : INT32_MAX);
-      okm0 = __ballot_sync(0xffffffffu, valid && (long long)cn + m_bias0 <= (long long)mn);
-      if (n_mask > 1) {
-        const bool valid1 = (m_reg1 >> lane) & 1;
-        const int cn1 = rc.cnt[warp][1][lane & (kRunDom - 1)];
-        const int mn1 = __reduce_min_sync(0xffffffffu, valid1 ? cn1 : INT32_MAX);
-        okm1 = __ballot_sync(0xffffffffu, valid1 && (long long)cn1 + m_bias1 <= (long long)mn1);
-      }
-    }
-    // ---- scan the slots this thread owns: key, rp and (topology classes) the admissible domains
-    unsigned long long mine = ~0ull;
-    int best_a = 0;
-    uint32_t best_rp = 0, best_z0 = 0, best_z1 = 0;
-    for (int a = tid; a < n_active; a += T) {
-      const unsigned long long key = hs->key[a];
-      const uint32_t rp = rpv[a];
-      uint32_t z0 = 0, z1 = 0;
-      bool ok = key < mine && (rp & 0xFFFF) != 0 && !(rp & kRpDead);  // tombstones carry key = ~0
-      if (n_mask > 0) { z0 = zv[a]; ok = ok && (z0 & okm0) != 0; }
-      if (n_mask > 1) { z1 = zv[kTopoCap + a]; ok = ok && (z1 & okm1) != 0; }
-      if (ok) { mine = key; best_a = a; best_rp = rp; best_z0 = z0; best_z1 = z1; }
-    }
-    // payload of this thread's candidate: slot | slow << 11 | pin bits << 13 | domains << 15 / 19
-    unsigned pay = (unsigned)best_a;
-    if (mine != ~0ull) {
-      if ((best_rp & 0xFFFF) == kRoomSlow) pay |= 1u << 11;
-      if (n_mask > 0) {
-        const uint32_t cand = best_z0 & okm0;
-        int d;
-        if (!(best_z0 & 0xFFFF & ((best_z0 & 0xFFFF) - 1)) && (best_z0 & (1u << 16))) d = __ffs(cand) - 1;  // pinned already
-        else {  // the placement pins the node's domain
-          d = run_pick(cand, rc.cnt[warp][0]);
-          pay |= 1u << 13;
-          if (!((rc.m_neutral[0] >> d) & 1) || !((best_z0 & (1u << 17)) || rc.m_wk[0])) pay |= 1u << 11;
-        }
-        pay |= (unsigned)d << 15;
-      }
-      if (n_mask > 1) {
-        const uint32_t cand = best_z1 & okm1;
-        int d;
-        if (!(best_z1 & 0xFFFF & ((best_z1 & 0xFFFF) - 1)) && (best_z1 & (1u << 16))) d = __ffs(cand) - 1;
-        else {
-          d = run_pick(cand, rc.cnt[warp][1]);
-          pay |= 1u << 14;
-          if (!((rc.m_neutral[1] >> d) & 1) || !((best_z1 & (1u << 17)) || rc.m_wk[1])) pay |= 1u << 11;
-        }
-        pay |= (unsigned)d << 19;
-      }
-    }
-    // ---- block argmin with payload: ONE barrier (double-buffered scratch)
-    const unsigned long long wmin = warp_min_u64(mine);
-    if (mine == wmin && mine != ~0ull) { rc.red_key[parity][warp] = wmin; rc.red_pay[parity][warp] = pay; }
-    else if (lane == 0 && wmin == ~0ull) rc.red_key[parity][warp] = ~0ull;
-    __syncthreads();
-    const unsigned long long rk = lane < nwarps ? rc.red_key[parity][lane] : ~0ull;
-    const unsigned rp_l = lane < nwarps ? rc.red_pay[parity][lane] : 0;
-    parity ^= 1;
-    const unsigned long long wkey = warp_min_u64(rk);
-    if (wkey != ~0ull) {
-      const unsigned src = __ballot_sync(0xffffffffu, rk == wkey);
-      const unsigned wp = __shfl_sync(0xffffffffu, rp_l, __ffs(src) - 1);
-      if (wp & (1u << 11)) { status = 1; break; }  // the winner needs the full evaluation
-      fd0 = (wp >> 15) & 0xF;
-      fd1 = (wp >> 19) & 0xF;
-      if (mine == wkey) {  // the owner commits its node: a handful of shared-memory stores
-        const int a = best_a;
-        const uint32_t rp = run_record_host(rc, hc, n_host, a, best_rp, 1);
-        if (pay & (3u << 13)) {  // requirements.Add(In{d}) on the node: once per node and key
-          const int n = hs->node[a];
-          for (int j = 0; j < n_mask; ++j) {
-            if (!((pay >> (13 + j)) & 1)) continue;
-            const int d = j ? fd1 : fd0, k = rc.m_key[j];
-            zv[j * kTopoCap + a] = (1u << d) | (3u << 16);
-            s.nn_vals[(size_t)k * MAXN + n] = 1ull << d;
-            s.nn_meta[n] = (s.nn_meta[n] | (1ull << (KSCHED_META_PRESENT_SHIFT + k))) & ~(1ull << (KSCHED_META_COMPLEMENT_SHIFT + k));
-          }
-        }
-        const int count = (int)(wkey >> 32) + 1;
-        unsigned long long nkey = order_key(count, -(tick + 1));
-        rc.q_node[buf][i] = NE + hs->node[a];
-        if ((rp & 0xFFFF) == 0 && run_closes(hs, a, rp, p_req, min_req, RH)) {  // tombstone, compacted when the run ends
-          nkey = ~0ull;
-          hs->nn_last[a] = ((unsigned long long)(unsigned)count << 32) | (unsigned)(-(tick + 1));
-          rc.tomb = rc.tomb + 1;
-        }
-        hs->key[a] = nkey;
-        rpv[a] = rp;
-      }
-      if (n_mask > 0) {  // every warp keeps its copy of the spread counters in step (the node's domain is the single value d)
-        if (lane == 0) {
-          if (m_rec0) rc.cnt[warp][0][fd0]++;
-          if (m_rec1) rc.cnt[warp][1][fd1]++;
-        }
-        __syncwarp();
-      }
-      ++tick;
-    } else mode = 2;
+      CR_IT(3)
+      const int r = run_argmin_step(e, buf, i, n_active, tick, parity, okm0, okm1);
+      if (r == 1) { status = 1; break; }
+      if (r == 2) mode = 2;
     }
     if (mode == 2) {
-      // ---- nobody accepts: NewNode + Add replayed from a variant (templates: the one the variant was created from)
-      if (n_new >= MAXN || n_active >= kActCap || (topo && n_active >= kTopoCap)) { status = 1; break; }
-      bool ok = true;
-#pragma unroll
-      for (int j = 0; j < kRunHost; ++j) ok = ok && (j >= n_host || rc.h_lim[j] >= 0);  // a fresh hostname has count 0
-      if (n_mask > 0 && ok) {
-        const uint32_t cand = rc.m_tallow[0] & okm0;
-        if (!cand) ok = false; else fd0 = run_pick(cand, rc.cnt[warp][0]);
-      }
-      if (n_mask > 1 && ok) {
-        const uint32_t cand = rc.m_tallow[1] & okm1;
-        if (!cand) ok = false; else fd1 = run_pick(cand, rc.cnt[warp][1]);
-      }
-      int vi = -1;
-      for (int v2 = 0; v2 < rc.n_var && ok && vi < 0; ++v2)
-        if ((n_mask < 1 || rc.var[v2].dom[0] == fd0) && (n_mask < 2 || rc.var[v2].dom[1] == fd1)) vi = v2;
-      const uint32_t pat = vs_pattern(n_mask, rc.m_key, fd0, fd1);
-      if (vi < 0 && ok && rc.vs_ok && vs_maybe(rc, vs_tag(rc.sig, pat), lane)) {  // (every warp finds the same answer)
-        __syncthreads();  // every warp has scanned the ring
-        if (warp == 0) {
-          const int got = vs_fetch(rc, cls, pat, lane);
-          if (lane == 0) rc.vs_got = got;
-        }
-        __syncthreads();
-        vi = rc.vs_got;
-      }
-      if (vi < 0) {
-        status = 1;
-#ifdef KSCHED_PROFILE_PACK
-        cr_novar = ok;
-#endif
-        break;
-      }
-      const RunVariant& v = rc.var[vi];
+      if (!run_fresh_step(e, buf, i, k_avail, lvl, okm0, okm1, tick, n_new, n_active, adv, novar)) { status = 1; break; }
       CR_IT(2)
-      // Fill step on the fresh node: it takes `cap` further pods of the class while it is the only accepting node and then
-      // refuses (room 0 or a hostname limit reached). With an exact cap the run needs F such nodes in a row, m = 1 + cap pods
-      // each: all of them are created in this iteration, one per thread (slot a belongs to thread a % T as everywhere).
-      int cap = 0, F = 1;
-      bool cap_exact = false;
-      if (lvl && (v.rp & 0xFFFF) != kRoomSlow) {
-        cap_exact = true;
-        if (!(v.rp & kRpDead)) {
-          cap = (int)(v.rp & 0xFFFF);
-          for (int j = 0; j < n_host; ++j) {
-            const int times = rc.h_times[j], lim = rc.h_lim[j];
-            if (!times || lim >= 0x10000) continue;
-            if (lim >= 0xFFF0) { cap = 0; cap_exact = false; continue; }  // saturating counters nearby: one pod at a time
-            const int td = (lim - times) / times + 1;  // the count is `times` after the first pod
-            cap = td < cap ? td : cap;
-          }
-        }
-      }
-      const int m = 1 + cap;
-      if (cap_exact) {
-        F = (k_avail + m - 1) / m;
-        if (F > MAXN - n_new) F = MAXN - n_new;
-        if (F > kActCap - n_active) F = kActCap - n_active;
-        if (topo && F > kTopoCap - n_active) F = kTopoCap - n_active;
-      }
-      const int K = k_avail < F * m ? k_avail : F * m;  // pods consumed (k_avail is 1 outside level mode: F = m = K = 1)
-      for (int idx = tid; idx < W32 * F; idx += T) { const int w = idx / F, j = idx - w * F; s.nn_opts[(size_t)w * MAXN + n_new + j] = v.opts[w]; }
-      for (int idx = tid; idx < c.n_keys * F; idx += T) { const int k = idx / F, j = idx - k * F; s.nn_vals[(size_t)k * MAXN + n_new + j] = v.vals[k]; }
-      for (int idx = tid; idx < KSCHED_MAX_RES * F; idx += T) { const int r = idx / F, j = idx - r * F; s.nn_req[(size_t)r * MAXN + n_new + j] = v.q[r]; }
-      for (int e = tid; e < K; e += T) rc.q_node[buf][i + e] = NE + n_new + e / m;
-      if (tid == 0)
-        for (int j = 0; j < n_host; ++j) if (rc.h_times[j]) rc.h_inc[j] = rc.h_inc[j] + F;
-      for (int j = (tid + T - n_active % T) % T; j < F; j += T) {  // the new slots this thread owns
-        const int a = n_active + j, n = n_new + j;
-        const int t = (K - j * m < m ? K - j * m : m) - 1;  // further pods on this node (the last one may get fewer)
-        const int tk = tick + j * m;                          // tick of its first pod
-#pragma unroll
-        for (int r = 0; r < kHotRes; ++r) { hs->q[r][a] = v.q[r]; hs->bound[r][a] = v.b1[r]; hs->bound2[r][a] = v.b2[r]; }
-        hs->node[a] = n;
-        hs->flags[a] = v.fl;
-        hs->absorbed[a] = simple ? cls : KSCHED_NONE;
-        hs->rejected[a] = KSCHED_NONE;
-        s.nn_meta[n] = v.meta;
-        s.nn_tmpl[n] = (uint8_t)(v.fl >> 8);
-        s.nn_req_present[n] = v.qp;
-        s.nn_hp[n] = 0;
-        s.nn_count[n] = 1;
-        s.nn_tb[n] = tk + 1;
-        if (n_mask > 0) zv[a] = (1u << fd0) | (3u << 16);
-        if (n_mask > 1) zv[kTopoCap + a] = (1u << fd1) | (3u << 16);
-        uint32_t rp2 = t > 0 ? v.rp - (uint32_t)t + ((uint32_t)t << 16) : v.rp;
-        for (int jj = 0; jj < n_host; ++jj) {
-          const int times = rc.h_times[jj];
-          const int now = times + t * times > 0xFFFF ? 0xFFFF : times + t * times;
-          hc[jj * kTopoCap + a] = (uint16_t)now;
-          if (times) s.grp_host[(size_t)rc.h_row[jj] * hstride + NE + n] = (uint16_t)times;  // (the run's write-back stores the final count)
-          if (t > 0 && now > rc.h_lim[jj]) rp2 |= kRpDead;
-        }
-        unsigned long long nkey = t > 0 ? order_key(1 + t, -(tk + 1 + t)) : order_key(1, tk + 1);
-        // (the slot holds the variant's requests and front, and rp2 has t pods placed: v.rp carries none)
-        if (t > 0 && (rp2 & 0xFFFF) == 0 && run_closes(hs, a, rp2, p_req, min_req, RH)) {
-          nkey = ~0ull;
-          hs->nn_last[a] = ((unsigned long long)(unsigned)(1 + t) << 32) | (unsigned)(-(tk + 1 + t));
-          atomicAdd(&rc.tomb, 1);
-        }
-        hs->key[a] = nkey;
-        rpv[a] = rp2;
-      }
-      if (n_mask > 0) {
-        if (lane == 0) {
-          if (m_rec0) rc.cnt[warp][0][fd0]++;
-          if (m_rec1) rc.cnt[warp][1][fd1]++;
-        }
-        __syncwarp();
-      }
-      adv = K;
-      tick += K;
-      n_new += F;
-      n_active += F;
     }
     // ---- the pods are placed: pop them
     qi += adv;
@@ -2809,13 +2809,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
   __syncthreads();
   // ---- the run is over: write back what the commits deferred
   const int placed_total = qi - qi0;
-  if (tid < CH && tid < qi - cb) {  // assignments of the partly consumed chunk
-    const uint32_t pd = rc.q_pod[buf][tid];
-    int nd = rc.q_node[buf][tid];
-    if (nd < -1) nd = NE + hs->node[-nd - 2];  // the mask run stores the slot
-    s.assign[pd] = nd;
-    s.place_seq[pd] = seq0 + (cb - qi0) + tid;
-  }
+  run_store_chunk(e, buf, qi - cb < CH ? qi - cb : CH, seq0 + (cb - qi0));  // assignments of the partly consumed chunk
   for (int a = tid; a < n_active; a += T) {  // requests, order statistics, hostname counters of the nodes that took pods
     const uint32_t rp = rpv[a];
     const int placed = (rp >> 16) & 0x7FFF;
@@ -2868,11 +2862,15 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
   }
 #ifdef KSCHED_PROFILE_PACK
   if (tid == 0) {
-    const int b = lvl ? 32 : 36;  // [cycles, pods, level+fill iterations, fresh iterations] ; per-pod iterations go to 44 / 45
-    s.counters[b] += clock64() - cr_t0; s.counters[b + 1] += placed_total; s.counters[b + 2] += cr_it[0] + cr_it[1]; s.counters[b + 3] += cr_it[2];
-    s.counters[lvl ? 44 : 45] += cr_it[3];
-    s.counters[46] += cr_it[1];
-    if (status == 1 && cr_novar) s.counters[57] += 1;
+    if (lvl) {
+      s.counters[kCtrRunLvCycles] += clock64() - cr_t0; s.counters[kCtrRunLvPods] += placed_total;
+      s.counters[kCtrRunLvSteps] += cr_it[0] + cr_it[1]; s.counters[kCtrRunLvFresh] += cr_it[2]; s.counters[kCtrRunLvPerPod] += cr_it[3];
+    } else {
+      s.counters[kCtrRunCycles] += clock64() - cr_t0; s.counters[kCtrRunPods] += placed_total;
+      s.counters[kCtrRunFresh] += cr_it[2]; s.counters[kCtrRunPerPod] += cr_it[3];
+    }
+    s.counters[kCtrRunLvFills] += cr_it[1];
+    if (status == 1 && novar) s.counters[kCtrNoVariantStops] += 1;
   }
 #endif
   if (tid == 0) {
@@ -3005,7 +3003,7 @@ __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
       __syncthreads();
 #ifdef KSCHED_PROFILE_PACK
       const long long pk_entry = clock64();
-      const long long pk_novar0 = tid == 0 ? s.counters[57] : 0;
+      const long long pk_novar0 = tid == 0 ? s.counters[kCtrNoVariantStops] : 0;
 #endif
       class_run(nxt);
       const RunIO& io = g_rio;
@@ -3015,14 +3013,14 @@ __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
       fresh_valid = 0;
 #ifdef KSCHED_PROFILE_PACK
       if (tid == 0) {
-        s.counters[40] += 1; s.counters[41] += placed; s.counters[42] += status == 1; s.counters[43] += status == 2;
+        s.counters[kCtrRunCalls] += 1; s.counters[kCtrRunPlaced] += placed; s.counters[kCtrRunBails] += status == 1; s.counters[kCtrRunIneligible] += status == 2;
         // round trips: from a call that stopped with status 1 to the entry of the next call that places pods
         if (placed > 0 && pk_bail >= 0) {
-          s.counters[56] += pk_entry - pk_bail;
-          if (pk_bail_novar) s.counters[58] += pk_entry - pk_bail;
+          s.counters[kCtrRoundTripCycles] += pk_entry - pk_bail;
+          if (pk_bail_novar) s.counters[kCtrNoVariantTripCycles] += pk_entry - pk_bail;
           pk_bail = -1;
         }
-        if (status == 1 && pk_bail < 0) { pk_bail = clock64(); pk_bail_novar = s.counters[57] != pk_novar0; }
+        if (status == 1 && pk_bail < 0) { pk_bail = clock64(); pk_bail_novar = s.counters[kCtrNoVariantStops] != pk_novar0; }
       }
 #endif
       if (status == 2) run_block_cls = (unsigned)nxt.cls64;
@@ -3077,7 +3075,7 @@ __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
     --qlen;
     ++add_calls;
 #ifdef KSCHED_PROFILE_PACK
-    if (tid == 0) s.counters[8 + 9] += 1;
+    if (tid == 0) s.counters[kCtrGenSteps] += 1;
 #endif
     LoopVars L{head, qlen, n_new, n_active, tick, seq, parity, fatal, epoch, pt_nonempty, nodes_visited, pt_class, row_class, 0, 0, KSCHED_NONE, 0};
     generic_step<kExt>(cur, first_pass, fpos_first, L);
@@ -3094,15 +3092,15 @@ __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
     for (int r = 0; r < RH; ++r) s.nn_req[(size_t)r * MAXN + n] = H.q(r, a);
   }
   if (tid == 0) {
-    s.counters[0] = n_new;
-    s.counters[1] = qlen;
-    s.counters[2] = nodes_visited;
-    s.counters[3] = add_calls;
-    s.counters[4] = fatal;
-    s.counters[5] = add_calls;
+    s.counters[kCtrNewNodes] = n_new;
+    s.counters[kCtrUnscheduled] = qlen;
+    s.counters[kCtrNodesVisited] = nodes_visited;
+    s.counters[kCtrAddCalls] = add_calls;
+    s.counters[kCtrError] = fatal;
+    s.counters[kCtrSteps] = add_calls;
 #ifdef KSCHED_PROFILE_PACK
-    s.counters[8 + 6] = pk_acc[1];  // cycles inside class_run calls
-    s.counters[8 + 7] = pk_acc[5];  // cycles inside generic calls (incl. call)
+    s.counters[kCtrRunCallCycles] = pk_acc[1];
+    s.counters[kCtrGenCallCycles] = pk_acc[5];  // (incl. the call)
 #endif
   }
 }
@@ -3110,7 +3108,7 @@ __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
 // options_true = options_stored AND Fits(requests): one warp per new node (resources.Fits, utils/resources/resources.go:138).
 __global__ void finalize_options_kernel(DevCatalog c, const long long* counters, const int64_t* nn_req, const uint32_t* nn_req_present,
                                         uint32_t* nn_opts, int max_new) {
-  const int n_new = (int)counters[0];
+  const int n_new = (int)counters[kCtrNewNodes];
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
   for (int n = warp; n < n_new; n += nwarps) {

@@ -122,7 +122,7 @@ struct PackState {
   uint8_t* grp_active;               // [n_groups] 0 while a relaxation-created group does not exist yet (topology.go:86-117)
   int32_t* grp_min_slot;             // [n_groups] hostname slots below this were never Register()ed with the group
   int64_t* remaining;                // [V][8] provisioner limits
-  // outputs / counters: [0]=n_new [1]=n_unscheduled [2]=nodes_visited [3]=add_calls [4]=error [5]=steps
+  // outputs and profile, indexed by Counter (ksched.cu)
   long long* counters;
   // taint sets from id 64 on, existing nodes only (ksched.h: class_tolerated_ext)
   const uint64_t* cls_tol_ext;       // [n_classes][tol_ext_words], or nullptr

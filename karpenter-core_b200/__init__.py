@@ -120,6 +120,8 @@ def lib():
     L.kh_scheduler_solve_timed.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.c_int, C.c_void_p, C.POINTER(C.c_double)]
     L.kh_encode.restype = C.c_void_p
     L.kh_encode.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.c_int]
+    L.kh_encode_cluster.restype = C.c_void_p
+    L.kh_encode_cluster.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.c_int]
     L.kh_encoded_free.argtypes = [C.c_void_p]
     L.kh_encoded_dims.argtypes = [C.c_void_p, C.POINTER(C.c_longlong)]
     L.kh_encoded_key_info.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(C.c_longlong)]

@@ -13,7 +13,6 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <functional>
 #include <limits>
 #include <tuple>
 #include <unordered_map>
@@ -64,6 +63,16 @@ bool parse_int(const std::string& s, int64_t* out) {  // strconv.Atoi: optional 
   }
   *out = neg ? (int64_t)(0 - (uint64_t)v) : (int64_t)v;
   return true;
+}
+
+// NewRequirement (requirement.go:44-68) on a dictionary: id maps a value to its bit
+Req new_requirement(Op op, const std::vector<std::string>& values, const std::map<std::string, int>& id) {
+  Req r{0, 0, 0, true, !(op == Op::In || op == Op::DoesNotExist), false, false};
+  if (op == Op::In || op == Op::NotIn)
+    for (auto& v : values) r.values |= 1ull << id.at(v);
+  if (op == Op::Gt) { r.has_gt = true; parse_int(values.at(0), &r.gt); }
+  if (op == Op::Lt) { r.has_lt = true; parse_int(values.at(0), &r.lt); }
+  return r;
 }
 
 // ---- resources (utils/resources/resources.go)
@@ -337,6 +346,43 @@ std::vector<HostPortEntry> host_ports(const Pod& p) {  // hostportusage.go:118-1
   return out;
 }
 
+std::vector<NodeSelectorRequirement> label_reqs(const Labels& l) {  // NewLabelRequirements requirements.go:54-59
+  std::vector<NodeSelectorRequirement> out;
+  for (auto& kv : l) out.push_back({kv.first, Op::In, {kv.second}});
+  return out;
+}
+Labels template_labels(const Provisioner& pr) {  // NewMachineTemplate's labels (machinetemplate.go:46-62)
+  Labels l = pr.labels;
+  l[kProvisionerName] = pr.name;
+  return l;
+}
+// The requirement lists a pod can put into a node's requirements (NewPodRequirements, requirements.go:61-78): its node
+// selector as labels, every required term and every preferred term.
+template <class F>
+void pod_requirement_lists(const Pod& p, F f) {
+  f(label_reqs(p.node_selector));
+  for (auto& t : p.required_node_terms) f(t);
+  for (auto& t : p.preferred_node_terms) f(t.preference);
+}
+// The topology terms of a pod, in the order newForTopologies + newForAffinities make groups of them (topology.go:278-322):
+// f(type, topology key, namespaces, selector, max skew) with type 0 spread, 1 affinity, 2 anti-affinity. Empty namespaces
+// stand for the pod's own.
+template <class F>
+void pod_topology_terms(const Pod& p, F f) {
+  static const std::vector<std::string> own;
+  for (auto& t : p.topology_spread) f(0, t.topology_key, own, t.selector, t.max_skew);
+  for (auto& t : p.pod_affinity_required) f(1, t.topology_key, t.namespaces, t.selector, INT32_MAX);
+  for (auto& t : p.pod_affinity_preferred) f(1, t.term.topology_key, t.term.namespaces, t.term.selector, INT32_MAX);
+  for (auto& t : p.pod_anti_affinity_required) f(2, t.topology_key, t.namespaces, t.selector, INT32_MAX);
+  for (auto& t : p.pod_anti_affinity_preferred) f(2, t.term.topology_key, t.term.namespaces, t.term.selector, INT32_MAX);
+}
+// Resource ids: cpu, memory and pods first, then the other names in order.
+std::vector<std::string> resource_order(const std::set<std::string>& names) {
+  std::vector<std::string> out = {"cpu", "memory", "pods"};
+  for (auto& n : names) if (std::find(out.begin(), out.begin() + 3, n) == out.begin() + 3) out.push_back(n);
+  return out;
+}
+
 // Facts about the cluster state that do not depend on which nodes are consolidation candidates nor on the dictionary:
 // computed once per Problem (a consolidation pass encodes the same Problem once per probe), by exactly the code the
 // encoder used to run per node on every call, so the encoding stays byte-identical (tests/test_encoding_digests.py).
@@ -368,22 +414,18 @@ const ClusterFacts& cluster_facts(const Problem& P) {
       for (auto& p : n.pods) {
         const ResourceList r = pod_requests(p);
         for (auto& kv : r) { f->res_names.insert(kv.first); f->req_names.insert(kv.first); }
-        auto name = [&](const std::vector<NodeSelectorRequirement>& rs) {
+        pod_requirement_lists(p, [&](const std::vector<NodeSelectorRequirement>& rs) {
           for (auto& q : rs)
             if (q.op == Op::In || q.op == Op::NotIn)
               for (auto& v : q.values) f->named_pairs.insert({normalize_key(q.key), v});
-        };
-        for (auto& kv : p.node_selector) f->named_pairs.insert({normalize_key(kv.first), kv.second});
-        for (auto& t : p.required_node_terms) name(t);
-        for (auto& t : p.preferred_node_terms) name(t.preference);
+        });
         nf.pod_req = merge(nf.pod_req, r);
         if (p.is_daemonset) nf.ds_req = merge(nf.ds_req, r);
         for (auto& hp : host_ports(p)) nf.hostports.push_back(hp);
-      }
-      for (auto& kv : n.labels) nf.label_reqs.push_back({kv.first, Op::In, {kv.second}});
-      nf.taints = state_node_taints(n);
-      for (auto& p : n.pods)
         for (auto& t : p.pod_anti_affinity_required) f->anti_keys.insert(t.topology_key);
+      }
+      nf.label_reqs = label_reqs(n.labels);
+      nf.taints = state_node_taints(n);
       for (auto& kv : n.labels) f->label_pairs.insert({kv.first, kv.second});
     }
     P.derived = f;
@@ -391,9 +433,35 @@ const ClusterFacts& cluster_facts(const Problem& P) {
   return static_cast<const ClusterFacts&>(*P.derived);
 }
 
+struct Profile {  // KSCHED_ENCODE_PROFILE: one line per phase of encode() on stderr
+  std::chrono::steady_clock::time_point last = std::chrono::steady_clock::now();
+  void operator()(const char* name) {
+    static const bool on = std::getenv("KSCHED_ENCODE_PROFILE") != nullptr;
+    if (!on) return;
+    auto now = std::chrono::steady_clock::now();
+    std::fprintf(stderr, "[encode] %-28s %8.2f ms\n", name, std::chrono::duration<double, std::milli>(now - last).count());
+    last = now;
+  }
+};
+
+struct Spec { Pod pod; ResourceList req; uint32_t next = KSCHED_NONE; };  // a pod class and the class its relaxation leads to
+// a daemonset pod's requirements (`special`: it has hostname / instance-type ones) and requests
+struct Daemon { const Pod* pod; ksched_reqset rs; ksched_bounds bd; bool special; ResourceList req; };
+
+// The encoder's state: what one phase of encode() hands to the next.
 struct Builder {
+  Profile phase;
   const Problem& P;
   Encoded& E;
+  const ClusterFacts& facts;
+  const bool superset;                                     // encode(..., cluster_superset)
+  std::vector<int> state_nodes;                            // Problem.nodes that stay existing nodes
+  bool tolerate_pns = false;                               // scheduler.go:49-56
+  bool uids_ascending = true;                              // the batch's UIDs: unique and already in rank order
+  std::vector<std::string> vol_drivers;                    // CSI drivers some owned state node limits
+  std::map<std::pair<std::string, std::string>, int> vol_tracked;  // (driver, claim) -> bit
+  std::vector<Spec> specs;                                 // pod classes, relaxed variants included (intern)
+  std::map<std::string, uint32_t> spec_id;
   std::set<std::string> well_known;
   std::map<std::string, int> key_id;                       // mask key -> id
   std::vector<std::map<std::string, int>> value_id;        // per key
@@ -404,23 +472,17 @@ struct Builder {
   std::vector<HostPortEntry> hp_entries;
   std::map<std::string, int> type_col;                     // instance type name -> column
   bool res_pruned = false;                                 // resource names no request reads were left out of res_id
+  std::vector<Daemon> daemons;
+  std::map<std::string, int> hostname_slot;                // hostname -> existing slot
 
-  Builder(const Problem& p, Encoded& e) : P(p), E(e) {}
+  Builder(const Problem& p, Encoded& e, bool cluster_superset) : P(p), E(e), facts(cluster_facts(p)), superset(cluster_superset) {}
 
   // ------------------------------------------------------------ requirement encoding
   int key_of(const std::string& k) const {
     auto it = key_id.find(normalize_key(k));
     return it == key_id.end() ? -1 : it->second;
   }
-  Req encode_req(int k, Op op, const std::vector<std::string>& values) const {  // NewRequirement requirement.go:44-68
-    Req r{0, 0, 0, true, true, false, false};
-    r.complement = !(op == Op::In || op == Op::DoesNotExist);
-    if (op == Op::In || op == Op::NotIn)
-      for (auto& v : values) r.values |= 1ull << value_id[k].at(v);
-    if (op == Op::Gt) { r.has_gt = true; parse_int(values.at(0), &r.gt); }
-    if (op == Op::Lt) { r.has_lt = true; parse_int(values.at(0), &r.lt); }
-    return r;
-  }
+  Req encode_req(int k, Op op, const std::vector<std::string>& values) const { return new_requirement(op, values, value_id[k]); }
   void add_req(ksched_reqset& rs, ksched_bounds& b, int k, const Req& r) const {  // Requirements.Add
     Req cur = ksched::req_load(rs, &b, k);
     ksched::req_store(rs, &b, k, ksched::key_add(cur, r, key_meta[k]));
@@ -438,11 +500,6 @@ struct Builder {
       if (k < 0) continue;  // key inactive: cannot influence any decision
       add_req(rs, b, k, encode_req(k, r.op, r.values));
     }
-  }
-  static std::vector<NodeSelectorRequirement> label_reqs(const Labels& l) {  // NewLabelRequirements requirements.go:54-59
-    std::vector<NodeSelectorRequirement> out;
-    for (auto& kv : l) out.push_back({kv.first, Op::In, {kv.second}});
-    return out;
   }
   // NewPodRequirements requirements.go:61-78 (the preferred-term sort is stable here)
   void pod_requirements(const Pod& pod, ksched_reqset& rs, ksched_bounds& b, Special* sp) const {
@@ -523,6 +580,61 @@ struct Builder {
     }
     return present;
   }
+
+  // ------------------------------------------------------------ CSI volume limits (ksched.h: ksched_class_volumes)
+  size_t driver_index(const std::string& driver) const {  // vol_drivers.size() when the driver has no limit
+    return (size_t)(std::find(vol_drivers.begin(), vol_drivers.end(), driver) - vol_drivers.begin());
+  }
+  std::map<std::string, std::set<std::string>> pod_claims(const Pod& p) const {  // VolumeUsage.validate: driver -> claims, limited drivers only
+    std::map<std::string, std::set<std::string>> m;
+    for (auto& v : p.volumes)
+      if (!v.driver.empty() && driver_index(v.driver) < vol_drivers.size()) m[v.driver].insert(v.pvc_id);
+    return m;
+  }
+  std::string volume_signature(const Pod& p, ksched_class_volumes* out) const {
+    ksched_class_volumes cv{};
+    if (!vol_drivers.empty())
+      for (auto& kv : pod_claims(p)) {
+        const size_t d = driver_index(kv.first);
+        for (auto& c : kv.second) {
+          auto t = vol_tracked.find({kv.first, c});
+          if (t != vol_tracked.end()) cv.shared |= 1ull << t->second;
+          else if (cv.priv[d] == 0xFFFF) unsupported("more than 65535 volume claims on one pod");
+          else cv.priv[d]++;
+        }
+      }
+    if (out) *out = cv;
+    char b[96];
+    std::snprintf(b, sizeof b, "|V=%llx:%u:%u:%u:%u", (unsigned long long)cv.shared, cv.priv[0], cv.priv[1], cv.priv[2], cv.priv[3]);
+    return (cv.shared | cv.priv[0] | cv.priv[1] | cv.priv[2] | cv.priv[3]) ? std::string(b) : std::string();
+  }
+
+  // ------------------------------------------------------------ pod classes and relaxation chains
+  uint32_t intern(const Pod& p) {
+    ResourceList req = pod_requests(p);
+    std::string k = class_key(p, req);
+    if (!p.volumes.empty()) k += volume_signature(p, nullptr);
+    auto it = spec_id.find(k);
+    if (it != spec_id.end()) return it->second;
+    uint32_t id = (uint32_t)specs.size();
+    spec_id[k] = id;
+    specs.push_back({p, req, KSCHED_NONE});
+    Pod relaxed = p;
+    // NewPodRequirements sorts the preferred terms in place before Relax ever runs (requirements.go:69)
+    std::stable_sort(relaxed.preferred_node_terms.begin(), relaxed.preferred_node_terms.end(),
+                     [](auto& a, auto& b) { return a.weight > b.weight; });
+    if (relax(relaxed, tolerate_pns)) {
+      uint32_t nx = intern(relaxed);
+      specs[id].next = nx;
+    }
+    return id;
+  }
+  // the pods whose requirements can reach a node: every pod class (relaxed variants included) and every daemonset pod
+  template <class F>
+  void for_class_and_daemon_pods(F f) const {
+    for (auto& s : specs) f(s.pod);
+    for (auto& d : P.daemonset_pods) f(d);
+  }
 };
 
 std::vector<Taint> state_node_taints(const StateNode& n) {  // state/node.go:61-78
@@ -600,14 +712,7 @@ struct FoldedKey {
   // NewRequirement (requirement.go:44-68) of every requirement, combined by Requirements.Add (requirements.go:87-94)
   Req req(const std::vector<NodeSelectorRequirement>& rs) const {
     Req cur = ksched::req_absent();
-    for (auto& r : rs) {
-      Req x{0, 0, 0, true, !(r.op == Op::In || r.op == Op::DoesNotExist), false, false};
-      if (r.op == Op::In || r.op == Op::NotIn)
-        for (auto& v : r.values) x.values |= 1ull << id.at(v);
-      if (r.op == Op::Gt) { x.has_gt = true; parse_int(r.values.at(0), &x.gt); }
-      if (r.op == Op::Lt) { x.has_lt = true; parse_int(r.values.at(0), &x.lt); }
-      cur = ksched::key_add(cur, x, meta());
-    }
+    for (auto& r : rs) cur = ksched::key_add(cur, new_requirement(r.op, r.values, id), meta());
     return cur;
   }
   std::string render(const Req& r) const {
@@ -634,51 +739,37 @@ std::map<std::string, std::string> value_classes(const std::set<std::string>& va
   return rep_of;
 }
 
-std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candidates, bool cluster_superset) {
-  static const bool prof = std::getenv("KSCHED_ENCODE_PROFILE") != nullptr;
-  auto t_last = std::chrono::steady_clock::now();
-  auto phase = [&](const char* name) {
-    if (!prof) return;
-    auto now = std::chrono::steady_clock::now();
-    std::fprintf(stderr, "[encode] %-28s %8.2f ms\n", name, std::chrono::duration<double, std::milli>(now - t_last).count());
-    t_last = now;
-  };
-  auto enc = std::make_unique<Encoded>();
-  Encoded& E = *enc;
-  E.problem_ref = &P;
-  Builder B(P, E);
-  const ClusterFacts& facts = cluster_facts(P);
+namespace {
 
-  // ------------------------------------------------------------------ who takes part
-  std::vector<int> state_nodes;
-  {
-    std::set<int> cand(candidates.begin(), candidates.end());
-    auto reschedulable = [](const Pod& p) { return !p.is_daemonset && !p.terminal && !p.terminating; };  // utils/node/node.go:30-50
+// ------------------------------------------------------------------ who takes part
+// The nodes that stay existing nodes, Solve's pod list (provisioner.go:119-144, deprovisioning/helpers.go:42-93), the
+// well-known keys and the template order.
+void participants(Builder& B, const std::vector<int>& candidates) {
+  const Problem& P = B.P;
+  Encoded& E = B.E;
+  std::set<int> cand(candidates.begin(), candidates.end());
+  auto reschedulable = [](const Pod& p) { return !p.is_daemonset && !p.terminal && !p.terminating; };  // utils/node/node.go:30-50
+  for (size_t i = 0; i < P.nodes.size(); ++i)
+    if ((B.superset || !cand.count((int)i)) && !P.nodes[i].marked_for_deletion) B.state_nodes.push_back((int)i);
+  for (auto& p : P.pods) E.pods.push_back(&p);
+  auto deleting_nodes_pods = [&] {  // pending in every simulation
     for (size_t i = 0; i < P.nodes.size(); ++i)
-      if ((cluster_superset || !cand.count((int)i)) && !P.nodes[i].marked_for_deletion) state_nodes.push_back((int)i);
-    for (auto& p : P.pods) E.pods.push_back(&p);
-    if (cluster_superset) {
-      // pending pods first (the pods of deleting nodes are pending in every simulation), then the candidates' pods node by node
-      for (size_t i = 0; i < P.nodes.size(); ++i)
-        if (!cand.count((int)i) && P.nodes[i].marked_for_deletion)
-          for (auto& p : P.nodes[i].pods) if (reschedulable(p)) E.pods.push_back(&p);
-      E.pod_node.assign(E.pods.size(), -1);
-      for (int c : candidates) {
-        if (P.nodes.at(c).marked_for_deletion) throw std::runtime_error("a candidate node is marked for deletion");
-        for (auto& p : P.nodes[c].pods) if (reschedulable(p)) { E.pods.push_back(&p); E.pod_node.push_back(-2 - c); }  // slot resolved below
-      }
-    } else {
-      for (int c : candidates)
-        for (auto& p : P.nodes.at(c).pods) if (reschedulable(p)) E.pods.push_back(&p);
-      for (size_t i = 0; i < P.nodes.size(); ++i)
-        if (!cand.count((int)i) && P.nodes[i].marked_for_deletion)
-          for (auto& p : P.nodes[i].pods) if (reschedulable(p)) E.pods.push_back(&p);
+      if (!cand.count((int)i) && P.nodes[i].marked_for_deletion)
+        for (auto& p : P.nodes[i].pods) if (reschedulable(p)) E.pods.push_back(&p);
+  };
+  if (B.superset) {
+    // pending pods first, then the candidates' pods node by node
+    deleting_nodes_pods();
+    E.pod_node.assign(E.pods.size(), -1);
+    for (int c : candidates) {
+      if (P.nodes.at(c).marked_for_deletion) throw std::runtime_error("a candidate node is marked for deletion");
+      for (auto& p : P.nodes[c].pods) if (reschedulable(p)) { E.pods.push_back(&p); E.pod_node.push_back(-2 - c); }  // slot resolved in existing_nodes
     }
+  } else {
+    for (int c : candidates)
+      for (auto& p : P.nodes.at(c).pods) if (reschedulable(p)) E.pods.push_back(&p);
+    deleting_nodes_pods();
   }
-  const size_t NP = E.pods.size();
-  // strictly ascending UIDs (the usual case: one informer list) are unique and already ranked; found out in the pass below
-  // that visits every pod anyway
-  bool uids_ascending = true;
   if (P.provisioners.empty()) throw std::runtime_error("no provisioners found");
   if (P.provisioners.size() > KSCHED_MAX_TEMPLATES) unsupported("more than 64 provisioners");
 
@@ -689,334 +780,232 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
   for (size_t i = 0; i < P.provisioners.size(); ++i) E.template_provisioner.push_back((int)i);
   std::stable_sort(E.template_provisioner.begin(), E.template_provisioner.end(),
                    [&](int a, int b) { return P.provisioners[a].weight > P.provisioners[b].weight; });
-  bool tolerate_pns = false;  // scheduler.go:49-56
   for (auto& pr : P.provisioners)
-    for (auto& t : pr.taints) if (t.effect == "PreferNoSchedule") tolerate_pns = true;
+    for (auto& t : pr.taints) if (t.effect == "PreferNoSchedule") B.tolerate_pns = true;
+}
 
-  phase("who takes part");
-  // ------------------------------------------------------------------ CSI volume limits (ksched.h: ksched_class_volumes)
-  // Drivers some owned state node limits; claims by how many pods (batch + bound) mount them: one -> counted, several -> tracked id.
-  std::vector<std::string> vol_drivers;
-  std::map<std::pair<std::string, std::string>, int> vol_tracked;  // (driver, claim) -> bit
-  auto pod_claims = [&](const Pod& p) {  // VolumeUsage.validate's result: driver -> claim set, limited drivers only
-    std::map<std::string, std::set<std::string>> m;
-    for (auto& v : p.volumes)
-      if (!v.driver.empty() && std::find(vol_drivers.begin(), vol_drivers.end(), v.driver) != vol_drivers.end()) m[v.driver].insert(v.pvc_id);
-    return m;
-  };
-  {
-    std::set<std::string> drivers;
-    for (int si : state_nodes) for (auto& kv : P.nodes[si].volume_limits) drivers.insert(kv.first);
-    vol_drivers.assign(drivers.begin(), drivers.end());
-    if (vol_drivers.size() > KSCHED_MAX_VOLUME_DRIVERS) unsupported("more than 4 CSI drivers with node volume limits");
-    if (!vol_drivers.empty()) {
-      std::map<std::pair<std::string, std::string>, int> refs;
-      auto count = [&](const Pod& p) { for (auto& kv : pod_claims(p)) for (auto& c : kv.second) refs[{kv.first, c}]++; };
-      for (auto* p : E.pods) count(*p);
-      for (int si : state_nodes) for (auto& p : P.nodes[si].pods) count(p);
-      for (auto& kv : refs)
-        if (kv.second > 1) {
-          if (vol_tracked.size() >= 64) unsupported("more than 64 volume claims shared between pods");
-          const int bit = (int)vol_tracked.size();
-          vol_tracked[kv.first] = bit;
-        }
+// ------------------------------------------------------------------ CSI volume limits (ksched.h: ksched_class_volumes)
+// Drivers some owned state node limits; claims by how many pods (batch + bound) mount them: one -> counted, several -> tracked id.
+void csi_volumes(Builder& B) {
+  std::set<std::string> drivers;
+  for (int si : B.state_nodes) for (auto& kv : B.P.nodes[si].volume_limits) drivers.insert(kv.first);
+  B.vol_drivers.assign(drivers.begin(), drivers.end());
+  if (B.vol_drivers.size() > KSCHED_MAX_VOLUME_DRIVERS) unsupported("more than 4 CSI drivers with node volume limits");
+  if (B.vol_drivers.empty()) return;
+  std::map<std::pair<std::string, std::string>, int> refs;
+  auto count = [&](const Pod& p) { for (auto& kv : B.pod_claims(p)) for (auto& c : kv.second) refs[{kv.first, c}]++; };
+  for (auto* p : B.E.pods) count(*p);
+  for (int si : B.state_nodes) for (auto& p : B.P.nodes[si].pods) count(p);
+  for (auto& kv : refs)
+    if (kv.second > 1) {
+      if (B.vol_tracked.size() >= 64) unsupported("more than 64 volume claims shared between pods");
+      const int bit = (int)B.vol_tracked.size();
+      B.vol_tracked[kv.first] = bit;
     }
-  }
-  auto volume_signature = [&](const Pod& p, ksched_class_volumes* out) {
-    ksched_class_volumes cv{};
-    if (!vol_drivers.empty())
-      for (auto& kv : pod_claims(p)) {
-        const size_t d = (size_t)(std::find(vol_drivers.begin(), vol_drivers.end(), kv.first) - vol_drivers.begin());
-        for (auto& c : kv.second) {
-          auto t = vol_tracked.find({kv.first, c});
-          if (t != vol_tracked.end()) cv.shared |= 1ull << t->second;
-          else if (cv.priv[d] == 0xFFFF) unsupported("more than 65535 volume claims on one pod");
-          else cv.priv[d]++;
-        }
-      }
-    if (out) *out = cv;
-    char b[96];
-    std::snprintf(b, sizeof b, "|V=%llx:%u:%u:%u:%u", (unsigned long long)cv.shared, cv.priv[0], cv.priv[1], cv.priv[2], cv.priv[3]);
-    return (cv.shared | cv.priv[0] | cv.priv[1] | cv.priv[2] | cv.priv[3]) ? std::string(b) : std::string();
-  };
+}
 
-  // ------------------------------------------------------------------ pod specs: classes and relaxation chains
-  struct Spec { Pod pod; ResourceList req; uint32_t next = KSCHED_NONE; };
-  std::vector<Spec> specs;
-  std::map<std::string, uint32_t> spec_id;
-  std::function<uint32_t(const Pod&)> intern = [&](const Pod& p) -> uint32_t {
-    ResourceList req = pod_requests(p);
-    std::string k = class_key(p, req);
-    if (!p.volumes.empty()) k += volume_signature(p, nullptr);
-    auto it = spec_id.find(k);
-    if (it != spec_id.end()) return it->second;
-    uint32_t id = (uint32_t)specs.size();
-    spec_id[k] = id;
-    specs.push_back({p, req, KSCHED_NONE});
-    Pod relaxed = p;
-    // NewPodRequirements sorts the preferred terms in place before Relax ever runs (requirements.go:69)
-    std::stable_sort(relaxed.preferred_node_terms.begin(), relaxed.preferred_node_terms.end(),
-                     [](auto& a, auto& b) { return a.weight > b.weight; });
-    if (relax(relaxed, tolerate_pns)) {
-      uint32_t nx = intern(relaxed);
-      specs[id].next = nx;
-    }
-    return id;
-  };
+// ------------------------------------------------------------------ pod specs: classes and relaxation chains
+void pod_classes(Builder& B) {
+  Encoded& E = B.E;
+  const size_t NP = E.pods.size();
   E.pod_class.resize(NP);
-  {
-    // "same deployment as the previous pod" is a pure comparison of two pods: every pair at once, on all cores; only the
-    // class boundaries (a few hundred in a 100 000-pod batch) take the keyed path, in order
-    std::vector<uint8_t> same(NP, 0), uid_order_broken((NP >> 12) + 2, 0);
-    std::vector<uint64_t> run_hash(NP, 0);  // spec_hash of the pods that start a run
-    E.pod_timestamp.resize(NP);
-    parallel_ranges(NP, 4096, [&](size_t b, size_t e) {
-      bool asc = true;
-      if (b == 0 && e > 0) { E.pod_timestamp[0] = E.pods[0]->creation_ts; run_hash[0] = spec_hash(*E.pods[0]); }
-      for (size_t i = std::max<size_t>(b, 1); i < e; ++i) {
-        const Pod& p = *E.pods[i];
-        const Pod& q = *E.pods[i - 1];
-        same[i] = same_spec(p, q) ? 1 : 0;
-        if (!same[i]) run_hash[i] = spec_hash(p);
-        asc = asc && q.uid < p.uid;
-        E.pod_timestamp[i] = p.creation_ts;  // queue.go:74-110 sorts by it (per-pod queue keys below)
-      }
-      if (!asc) uid_order_broken[b >> 12] = 1;  // (ranges start at multiples of >= 4096 pods or at 0: one flag each)
-    });
-    for (uint8_t f : uid_order_broken) uids_ascending = uids_ascending && !f;
-    if (!uids_ascending) {
-      std::unordered_set<std::string> uids;
-      uids.reserve(NP * 2);
-      for (auto* p : E.pods)
-        if (!uids.insert(p->uid).second) throw std::runtime_error("pods must have unique UIDs: " + p->uid);
-    }
-    phase("  same_spec pairs");
-    // a run's class: the class of an earlier run with the same spec (hash, then one same_spec against that class's first pod),
-    // else the keyed path (new classes, pods with volumes, pods whose containers differ but sum to the same requests)
-    std::unordered_map<uint64_t, std::vector<uint32_t>> by_hash;
-    for (size_t i = 0; i < NP; ++i) {
-      if (same[i]) { E.pod_class[i] = E.pod_class[i - 1]; continue; }
+  // "same deployment as the previous pod" is a pure comparison of two pods: every pair at once, on all cores; only the
+  // class boundaries (a few hundred in a 100 000-pod batch) take the keyed path, in order
+  std::vector<uint8_t> same(NP, 0), uid_order_broken((NP >> 12) + 2, 0);
+  std::vector<uint64_t> run_hash(NP, 0);  // spec_hash of the pods that start a run
+  E.pod_timestamp.resize(NP);
+  parallel_ranges(NP, 4096, [&](size_t b, size_t e) {
+    bool asc = true;
+    if (b == 0 && e > 0) { E.pod_timestamp[0] = E.pods[0]->creation_ts; run_hash[0] = spec_hash(*E.pods[0]); }
+    for (size_t i = std::max<size_t>(b, 1); i < e; ++i) {
       const Pod& p = *E.pods[i];
-      uint32_t id = KSCHED_NONE;
-      if (p.volumes.empty()) {
-        auto it = by_hash.find(run_hash[i]);
-        if (it != by_hash.end())
-          for (uint32_t cid : it->second)
-            if (same_spec(p, specs[cid].pod)) { id = cid; break; }
-      }
-      if (id == KSCHED_NONE) {
-        id = intern(p);
-        if (p.volumes.empty()) {
-          auto& v = by_hash[run_hash[i]];
-          if (std::find(v.begin(), v.end(), id) == v.end()) v.push_back(id);
-        }
-      }
-      E.pod_class[i] = id;
+      const Pod& q = *E.pods[i - 1];
+      same[i] = same_spec(p, q) ? 1 : 0;
+      if (!same[i]) run_hash[i] = spec_hash(p);
+      asc = asc && q.uid < p.uid;
+      E.pod_timestamp[i] = p.creation_ts;  // queue.go:74-110 sorts by it (per-pod queue keys)
     }
-    phase("  intern boundaries");
+    if (!asc) uid_order_broken[b >> 12] = 1;  // (ranges start at multiples of >= 4096 pods or at 0: one flag each)
+  });
+  // strictly ascending UIDs (the usual case: one informer list) are unique and already ranked
+  for (uint8_t f : uid_order_broken) B.uids_ascending = B.uids_ascending && !f;
+  if (!B.uids_ascending) {
+    std::unordered_set<std::string> uids;
+    uids.reserve(NP * 2);
+    for (auto* p : E.pods)
+      if (!uids.insert(p->uid).second) throw std::runtime_error("pods must have unique UIDs: " + p->uid);
   }
-  std::vector<Pod> daemons = P.daemonset_pods;
+  B.phase("  same_spec pairs");
+  // a run's class: the class of an earlier run with the same spec (hash, then one same_spec against that class's first pod),
+  // else the keyed path (new classes, pods with volumes, pods whose containers differ but sum to the same requests)
+  std::unordered_map<uint64_t, std::vector<uint32_t>> by_hash;
+  for (size_t i = 0; i < NP; ++i) {
+    if (same[i]) { E.pod_class[i] = E.pod_class[i - 1]; continue; }
+    const Pod& p = *E.pods[i];
+    uint32_t id = KSCHED_NONE;
+    if (p.volumes.empty()) {
+      auto it = by_hash.find(run_hash[i]);
+      if (it != by_hash.end())
+        for (uint32_t cid : it->second)
+          if (same_spec(p, B.specs[cid].pod)) { id = cid; break; }
+    }
+    if (id == KSCHED_NONE) {
+      id = B.intern(p);
+      if (p.volumes.empty()) {
+        auto& v = by_hash[run_hash[i]];
+        if (std::find(v.begin(), v.end(), id) == v.end()) v.push_back(id);
+      }
+    }
+    E.pod_class[i] = id;
+  }
+  B.phase("  intern boundaries");
+}
 
-  phase("pod classes");
-  // ------------------------------------------------------------------ active keys + dictionary
+// ------------------------------------------------------------------ active keys + dictionary
+// Active keys: everything that can appear in a node's requirements (template or pod side). Keys that only instance types
+// define can never meet a node requirement (Intersects walks keys present on BOTH sides, requirements.go:189-190) and are
+// dropped. Template-only keys (DESIGN.md §3) go to *foldable: no pod-side source names them, so a node's requirement on one is
+// always its template's own and the key only decides which instance types the template admits. Zone and capacity-type stay
+// mask keys: offerings, the launch choice and the price helpers read them.
+std::set<std::string> active_keys(const Builder& B, std::set<std::string>* foldable) {
   // pod-side keys: anything a pod / daemonset / topology group / node filter can put into a node's requirements
   std::set<std::string> pod_side;
-  auto note_reqs = [&](const std::vector<NodeSelectorRequirement>& rs) { for (auto& r : rs) pod_side.insert(normalize_key(r.key)); };
-  auto note_pod = [&](const Pod& p) {
-    for (auto& kv : p.node_selector) pod_side.insert(normalize_key(kv.first));
-    for (auto& t : p.required_node_terms) note_reqs(t);
-    for (auto& t : p.preferred_node_terms) note_reqs(t.preference);
-    for (auto& t : p.pod_affinity_required) pod_side.insert(t.topology_key);
-    for (auto& t : p.pod_affinity_preferred) pod_side.insert(t.term.topology_key);
-    for (auto& t : p.pod_anti_affinity_required) pod_side.insert(t.topology_key);
-    for (auto& t : p.pod_anti_affinity_preferred) pod_side.insert(t.term.topology_key);
-    for (auto& t : p.topology_spread) pod_side.insert(t.topology_key);
-  };
-  for (auto& s : specs) note_pod(s.pod);
-  for (auto& d : daemons) note_pod(d);
-  if (!P.empty_topology)
-    for (auto& k : facts.anti_keys) pod_side.insert(k);  // bound pods with required anti-affinity (ClusterFacts)
-  std::set<std::string> type_keys, template_keys;
-  for (auto& it : P.instance_types) for (auto& r : it.requirements) type_keys.insert(normalize_key(r.key));
-  for (auto& pr : P.provisioners) {
-    for (auto& r : pr.requirements) template_keys.insert(normalize_key(r.key));
-    for (auto& kv : pr.labels) template_keys.insert(normalize_key(kv.first));
-    template_keys.insert(kProvisionerName);
-  }
-  // Active keys: everything that can appear in a node's requirements (template or pod side). Keys that only
-  // instance types define can never meet a node requirement (Intersects walks keys present on BOTH sides,
-  // requirements.go:189-190) and are dropped.
+  B.for_class_and_daemon_pods([&](const Pod& p) {
+    pod_requirement_lists(p, [&](const std::vector<NodeSelectorRequirement>& rs) { for (auto& r : rs) pod_side.insert(normalize_key(r.key)); });
+    pod_topology_terms(p, [&](int, const std::string& key, auto&&...) { pod_side.insert(key); });
+  });
+  if (!B.P.empty_topology)
+    for (auto& k : B.facts.anti_keys) pod_side.insert(k);  // bound pods with required anti-affinity (ClusterFacts)
   std::set<std::string> active = pod_side;
-  active.insert(template_keys.begin(), template_keys.end());
-  (void)type_keys;
+  for (auto& pr : B.P.provisioners) {
+    for (auto& r : pr.requirements) active.insert(normalize_key(r.key));
+    for (auto& kv : template_labels(pr)) active.insert(normalize_key(kv.first));
+  }
   active.erase(kHostname);
   active.erase(kInstanceType);
-  // Template-only keys (DESIGN.md §3): no pod-side source names them, so a node's requirement on one is always its template's
-  // own and the key only decides which instance types the template admits. Zone and capacity-type stay mask keys: offerings,
-  // the launch choice and the price helpers read them.
-  std::set<std::string> foldable;
   for (auto& k : active)
-    if (!pod_side.count(k) && k != kZone && k != kCapacityType) foldable.insert(k);
-  // The dictionary of a set of mask keys: key ids, values, thresholds and value classes.
+    if (!pod_side.count(k) && k != kZone && k != kCapacityType) foldable->insert(k);
+  return active;
+}
+
+// The dictionary of a set of mask keys under construction: values, thresholds and value classes per key.
+struct Dictionary {
   std::vector<std::set<std::string>> vals;
   std::vector<std::set<int64_t>> thr;
-  std::vector<bool> type_complement;
+  std::vector<bool> type_complement;                       // an instance type has a complement requirement on the key
   std::vector<std::map<std::string, std::string>> rep_of;  // unnamed value -> its class's representative
-  auto dictionary = [&](const std::set<std::string>& keys) {
-    B.key_id.clear();
-    E.key_names.clear();
-    for (auto& k : keys) {
-      B.key_id[k] = (int)E.key_names.size();
-      E.key_names.push_back(k);
-    }
-    const int NK = (int)E.key_names.size();
-    vals.assign(NK, {});
-    auto note_vals = [&](const std::vector<NodeSelectorRequirement>& rs) {
-      for (auto& r : rs) {
-        int k = B.key_of(r.key);
-        if (k < 0) continue;
-        if (r.op == Op::In || r.op == Op::NotIn) vals[k].insert(r.values.begin(), r.values.end());
-      }
-    };
-    auto note_label_vals = [&](const Labels& l) {
-      for (auto& kv : l) { int k = B.key_of(kv.first); if (k >= 0) vals[k].insert(kv.second); }
-    };
-    auto note_pod_vals = [&](const Pod& p) {
-      note_label_vals(p.node_selector);
-      for (auto& t : p.required_node_terms) note_vals(t);
-      for (auto& t : p.preferred_node_terms) note_vals(t.preference);
-    };
-    for (auto& s : specs) note_pod_vals(s.pod);
-    for (auto& d : daemons) note_pod_vals(d);
-    for (auto& it : P.instance_types) note_vals(it.requirements);
-    // offerings name zones / capacity types too (a node without a requirement on the key admits all of them)
-    for (auto& it : P.instance_types)
-      for (auto& o : it.offerings) {
-        int kz = B.key_of(kZone), kc = B.key_of(kCapacityType);
-        if (kz >= 0) vals[kz].insert(o.zone);
-        if (kc >= 0) vals[kc].insert(o.capacity_type);
-      }
-    for (auto& pr : P.provisioners) {
-      note_vals(pr.requirements);
-      Labels l = pr.labels;
-      l[kProvisionerName] = pr.name;
-      note_label_vals(l);
-    }
-    for (auto& kv : facts.label_pairs) { int k = B.key_of(kv.first); if (k >= 0) vals[k].insert(kv.second); }  // every node's labels (ClusterFacts)
-    const int zone_key = B.key_of(kZone), ct_key = B.key_of(kCapacityType);
-    // Every threshold any requirement of this problem names, per key; a key also gets one region when an instance type has a
-    // complement requirement on it (region form below).
-    thr.assign(NK, {});
-    type_complement.assign(NK, false);
-    {
-      auto note_thr = [&](const std::vector<NodeSelectorRequirement>& rs, bool is_type) {
-        for (auto& r : rs) {
-          int k = B.key_of(r.key);
-          if (k < 0) continue;
-          if (r.op == Op::Gt || r.op == Op::Lt) { int64_t v = 0; if (!r.values.empty()) parse_int(r.values[0], &v); thr[k].insert(v); }
-          if (is_type && r.op != Op::In && r.op != Op::DoesNotExist) type_complement[k] = true;
-        }
-      };
-      auto note_pod_thr = [&](const Pod& p) {
-        for (auto& t : p.required_node_terms) note_thr(t, false);
-        for (auto& t : p.preferred_node_terms) note_thr(t.preference, false);
-      };
-      for (auto& sp : specs) note_pod_thr(sp.pod);
-      for (auto& d : daemons) note_pod_thr(d);
-      for (auto& it : P.instance_types) note_thr(it.requirements, true);
-      for (auto& pr : P.provisioners) note_thr(pr.requirements, false);
-    }
-    // Value classes (DESIGN.md §3). A key whose values do not fit the word keeps the values some requirement of the problem
-    // names, and one representative per class of the others: instance types' In values and node labels that no requirement
-    // tells apart. Keys that fit are encoded as they always were.
-    phase("  keys + thresholds");
-    E.key_representatives.assign(NK, 0);
-    rep_of.assign(NK, {});
-    {
-      std::vector<int> wide;
-      for (int k = 0; k < NK; ++k) {
-        const size_t nd = vals[k].size(), m = thr[k].size();
-        if (nd > 63 || ((m > 0 || type_complement[k]) && nd + m + 1 > 63)) wide.push_back(k);
-      }
-      if (!wide.empty()) {
-        std::vector<std::set<std::string>> named(NK);
-        std::vector<bool> all_named(NK, false);
-        auto name_vals = [&](const std::vector<NodeSelectorRequirement>& rs, bool complement_only) {
-          for (auto& r : rs) {
-            int k = B.key_of(r.key);
-            if (k < 0 || (complement_only && r.op == Op::In)) continue;
-            if (r.op == Op::In || r.op == Op::NotIn) named[k].insert(r.values.begin(), r.values.end());
-          }
-        };
-        auto name_labels = [&](const Labels& l) { for (auto& kv : l) { int k = B.key_of(kv.first); if (k >= 0) named[k].insert(kv.second); } };
-        auto name_pod = [&](const Pod& p) {  // topology node filters are built from the same node selector and required terms
-          name_labels(p.node_selector);
-          for (auto& t : p.required_node_terms) name_vals(t, false);
-          for (auto& t : p.preferred_node_terms) name_vals(t.preference, false);
-          auto topo = [&](const std::string& key) { int k = B.key_of(key); if (k >= 0) all_named[k] = true; };
-          for (auto& t : p.topology_spread) topo(t.topology_key);
-          for (auto& t : p.pod_affinity_required) topo(t.topology_key);
-          for (auto& t : p.pod_affinity_preferred) topo(t.term.topology_key);
-          for (auto& t : p.pod_anti_affinity_required) topo(t.topology_key);
-          for (auto& t : p.pod_anti_affinity_preferred) topo(t.term.topology_key);
-        };
-        for (auto& s : specs) name_pod(s.pod);
-        for (auto& d : daemons) name_pod(d);
-        for (auto& kv : facts.named_pairs) { int k = B.key_of(kv.first); if (k >= 0) named[k].insert(kv.second); }  // bound pods
-        for (auto& key : facts.anti_keys) { int k = B.key_of(key); if (k >= 0) all_named[k] = true; }  // inverse anti-affinity groups
-        for (auto& pr : P.provisioners) {
-          name_vals(pr.requirements, false);
-          Labels l = pr.labels;
-          l[kProvisionerName] = pr.name;
-          name_labels(l);
-        }
-        for (auto& it : P.instance_types) name_vals(it.requirements, true);
-        if (zone_key >= 0) all_named[zone_key] = true;  // offering slots: they feed the launch choice
-        if (ct_key >= 0) all_named[ct_key] = true;
-        for (int k : wide) {
-          if (all_named[k]) continue;  // refused below when it does not fit
-          rep_of[k] = value_classes(vals[k], named[k], thr[k]);
-          for (auto& kv : rep_of[k]) {
-            if (kv.first != kv.second) vals[k].erase(kv.first);
-            else E.key_representatives[k]++;
-          }
-        }
-      }
-    }
-  };
-  // What the checks of the dictionary below accept: a key that fails them is refused.
-  auto fits = [&](int k) {
+  bool fits(int k) const {  // what the checks of install_dictionary accept: a key that fails them is refused
     const size_t nd = vals[k].size(), m = thr[k].size();
     return nd <= 63 && m <= KSCHED_MAX_THRESHOLDS && !((m > 0 || type_complement[k]) && nd + m + 1 > 63);
-  };
-  // Folding is conditional, so that every problem that fits the word keeps its encoding byte for byte: the template-only keys
-  // are folded only when the problem would be refused otherwise, for more than 16 keys or for a template-only key whose values
-  // do not fit (karpenter.sh/provisioner-name with 64 provisioners).
-  bool fold = active.size() > KSCHED_MAX_KEYS;
-  if (!fold) {
-    dictionary(active);
-    for (auto& k : foldable) fold = fold || !fits(B.key_id.at(k));
   }
-  if (fold) {
-    for (auto& k : foldable) active.erase(k);
-    if (active.size() > KSCHED_MAX_KEYS) unsupported("more than 16 active label keys");
-    E.folded_keys.assign(foldable.begin(), foldable.end());
-    dictionary(active);
+};
+// Adds to out[k] the values that In / NotIn requirements of rs on mask key k name (NotIn only when complement_only).
+void note_values(const Builder& B, const std::vector<NodeSelectorRequirement>& rs, std::vector<std::set<std::string>>& out, bool complement_only = false) {
+  for (auto& r : rs) {
+    int k = B.key_of(r.key);
+    if (k < 0 || (complement_only && r.op == Op::In)) continue;
+    if (r.op == Op::In || r.op == Op::NotIn) out[k].insert(r.values.begin(), r.values.end());
+  }
+}
+
+// Value classes (DESIGN.md §3). A key whose values do not fit the word keeps the values some requirement of the problem
+// names, and one representative per class of the others: instance types' In values and node labels that no requirement
+// tells apart. Keys that fit are encoded as they always were.
+void collapse_value_classes(Builder& B, Dictionary& D) {
+  const int NK = (int)B.E.key_names.size();
+  std::vector<int> wide;
+  for (int k = 0; k < NK; ++k) {
+    const size_t nd = D.vals[k].size(), m = D.thr[k].size();
+    if (nd > 63 || ((m > 0 || D.type_complement[k]) && nd + m + 1 > 63)) wide.push_back(k);
+  }
+  if (wide.empty()) return;
+  std::vector<std::set<std::string>> named(NK);
+  std::vector<bool> all_named(NK, false);
+  auto name_key = [&](const std::string& key) { int k = B.key_of(key); if (k >= 0) all_named[k] = true; };
+  B.for_class_and_daemon_pods([&](const Pod& p) {  // topology node filters are built from the same node selector and required terms
+    pod_requirement_lists(p, [&](const std::vector<NodeSelectorRequirement>& rs) { note_values(B, rs, named); });
+    pod_topology_terms(p, [&](int, const std::string& key, auto&&...) { name_key(key); });
+  });
+  for (auto& kv : B.facts.named_pairs) { int k = B.key_of(kv.first); if (k >= 0) named[k].insert(kv.second); }  // bound pods
+  for (auto& key : B.facts.anti_keys) name_key(key);  // inverse anti-affinity groups
+  for (auto& pr : B.P.provisioners) {
+    note_values(B, pr.requirements, named);
+    note_values(B, label_reqs(template_labels(pr)), named);
+  }
+  for (auto& it : B.P.instance_types) note_values(B, it.requirements, named, true);
+  name_key(kZone);  // offering slots: they feed the launch choice
+  name_key(kCapacityType);
+  for (int k : wide) {
+    if (all_named[k]) continue;  // refused in install_dictionary when it does not fit
+    D.rep_of[k] = value_classes(D.vals[k], named[k], D.thr[k]);
+    for (auto& kv : D.rep_of[k]) {
+      if (kv.first != kv.second) D.vals[k].erase(kv.first);
+      else B.E.key_representatives[k]++;
+    }
+  }
+}
+Dictionary dictionary(Builder& B, const std::set<std::string>& keys) {
+  Encoded& E = B.E;
+  B.key_id.clear();
+  E.key_names.clear();
+  for (auto& k : keys) {
+    B.key_id[k] = (int)E.key_names.size();
+    E.key_names.push_back(k);
   }
   const int NK = (int)E.key_names.size();
-  const int zone_key = B.key_of(kZone), ct_key = B.key_of(kCapacityType);
-  phase("  value classes");
+  Dictionary D;
+  D.vals.assign(NK, {});
+  auto note_vals = [&](const std::vector<NodeSelectorRequirement>& rs) { note_values(B, rs, D.vals); };
+  B.for_class_and_daemon_pods([&](const Pod& p) { pod_requirement_lists(p, note_vals); });
+  for (auto& it : B.P.instance_types) note_vals(it.requirements);
+  // offerings name zones / capacity types too (a node without a requirement on the key admits all of them)
+  for (auto& it : B.P.instance_types)
+    for (auto& o : it.offerings) {
+      int kz = B.key_of(kZone), kc = B.key_of(kCapacityType);
+      if (kz >= 0) D.vals[kz].insert(o.zone);
+      if (kc >= 0) D.vals[kc].insert(o.capacity_type);
+    }
+  for (auto& pr : B.P.provisioners) {
+    note_vals(pr.requirements);
+    note_vals(label_reqs(template_labels(pr)));
+  }
+  for (auto& kv : B.facts.label_pairs) { int k = B.key_of(kv.first); if (k >= 0) D.vals[k].insert(kv.second); }  // every node's labels (ClusterFacts)
+  // Every threshold any requirement of this problem names, per key; a key also gets one region when an instance type has a
+  // complement requirement on it (region form in install_dictionary).
+  D.thr.assign(NK, {});
+  D.type_complement.assign(NK, false);
+  auto note_thr = [&](const std::vector<NodeSelectorRequirement>& rs, bool is_type) {
+    for (auto& r : rs) {
+      int k = B.key_of(r.key);
+      if (k < 0) continue;
+      if (r.op == Op::Gt || r.op == Op::Lt) { int64_t v = 0; if (!r.values.empty()) parse_int(r.values[0], &v); D.thr[k].insert(v); }
+      if (is_type && r.op != Op::In && r.op != Op::DoesNotExist) D.type_complement[k] = true;
+    }
+  };
+  B.for_class_and_daemon_pods([&](const Pod& p) { pod_requirement_lists(p, [&](const std::vector<NodeSelectorRequirement>& rs) { note_thr(rs, false); }); });
+  for (auto& it : B.P.instance_types) note_thr(it.requirements, true);
+  for (auto& pr : B.P.provisioners) note_thr(pr.requirements, false);
+  B.phase("  keys + thresholds");
+  E.key_representatives.assign(NK, 0);
+  D.rep_of.assign(NK, {});
+  collapse_value_classes(B, D);
+  return D;
+}
+// Value ids, key infos and the region form of Gt/Lt (ksched.h: ksched_key_regions) of the dictionary.
+void install_dictionary(Builder& B, const Dictionary& D) {
+  Encoded& E = B.E;
+  const int NK = (int)E.key_names.size();
   B.value_id.resize(NK);
   E.key_values.resize(NK);
   E.keys.resize(NK);
   E.key_int_values.assign((size_t)NK * 64, 0);
   B.key_meta.resize(NK);
   for (int k = 0; k < NK; ++k) {
-    if (vals[k].size() > 63) unsupported("label key " + E.key_names[k] + " has more than 63 distinct values");
+    if (D.vals[k].size() > 63) unsupported("label key " + E.key_names[k] + " has more than 63 distinct values");
     ksched_keyinfo& ki = E.keys[k];
     std::memset(&ki, 0, sizeof ki);
     int b = 0;
-    for (auto& v : vals[k]) {
+    for (auto& v : D.vals[k]) {
       B.value_id[k][v] = b;
       E.key_values[k].push_back(v);
       ki.dict_mask |= 1ull << b;
@@ -1025,185 +1014,211 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
       ++b;
     }
     // every requirement, label and domain table looks an unnamed value up under its representative's id
-    for (auto& kv : rep_of[k]) B.value_id[k][kv.first] = B.value_id[k].at(kv.second);
+    for (auto& kv : D.rep_of[k]) B.value_id[k][kv.first] = B.value_id[k].at(kv.second);
     ki.well_known = B.well_known.count(E.key_names[k]) ? 1 : 0;
     ki.is_zone = E.key_names[k] == kZone;
     ki.is_capacity_type = E.key_names[k] == kCapacityType;
   }
   for (int k = 0; k < NK; ++k) B.key_meta[k] = KeyMeta{E.keys[k].int_mask, &E.key_int_values[(size_t)k * 64], nullptr};
-  // Region form of Gt/Lt (ksched.h: ksched_key_regions).
-  {
-    bool any = false;
-    for (int k = 0; k < NK; ++k) any = any || !thr[k].empty() || type_complement[k];
-    if (any) {
-      E.key_regions.assign(NK, ksched_key_regions{});
-      for (int k = 0; k < NK; ++k) {
-        if (thr[k].empty() && !type_complement[k]) continue;
-        const int m = (int)thr[k].size(), nd = (int)E.key_values[k].size();
-        if (m > KSCHED_MAX_THRESHOLDS) unsupported("label key " + E.key_names[k] + " has more than 7 distinct Gt/Lt thresholds");
-        if (nd + m + 1 > 63) unsupported("label key " + E.key_names[k] + " has too many values for its Gt/Lt regions");
-        std::vector<int64_t> ts(thr[k].begin(), thr[k].end());
-        ksched::regions_build(&E.key_regions[k], ts.data(), m, nd, E.keys[k].dict_mask, B.key_meta[k]);
-      }
-    }
+  bool any = false;
+  for (int k = 0; k < NK; ++k) any = any || !D.thr[k].empty() || D.type_complement[k];
+  if (!any) return;
+  E.key_regions.assign(NK, ksched_key_regions{});
+  for (int k = 0; k < NK; ++k) {
+    if (D.thr[k].empty() && !D.type_complement[k]) continue;
+    const int m = (int)D.thr[k].size(), nd = (int)E.key_values[k].size();
+    if (m > KSCHED_MAX_THRESHOLDS) unsupported("label key " + E.key_names[k] + " has more than 7 distinct Gt/Lt thresholds");
+    if (nd + m + 1 > 63) unsupported("label key " + E.key_names[k] + " has too many values for its Gt/Lt regions");
+    std::vector<int64_t> ts(D.thr[k].begin(), D.thr[k].end());
+    ksched::regions_build(&E.key_regions[k], ts.data(), m, nd, E.keys[k].dict_mask, B.key_meta[k]);
   }
-
-  phase("keys + dictionary");
-  // ------------------------------------------------------------------ resources
-  {
-    std::set<std::string> names;
-    auto note = [&](const ResourceList& r) { for (auto& kv : r) names.insert(kv.first); };
-    for (auto& s : specs) note(s.req);
-    for (auto& d : daemons) note(pod_requests(d));
-    for (auto& it : P.instance_types) { note(it.capacity); }
-    for (auto& pr : P.provisioners) note(pr.limits);
-    for (auto& n : facts.res_names) names.insert(n);  // node allocatable / capacity / bound pods (ClusterFacts)
-    E.res_names = {"cpu", "memory", "pods"};
-    for (auto& n : names) if (n != "cpu" && n != "memory" && n != "pods") E.res_names.push_back(n);
-    if (E.res_names.size() > KSCHED_MAX_RES) {
-      // Fits reads the request's keys only (resources.go:138-145), the limits bookkeeping the limit's keys only
-      // (scheduler.go:284-303): a name that no pod requests and no limit names cannot change an answer. Left out.
-      std::set<std::string> read = facts.req_names;
-      auto note_read = [&](const ResourceList& r) { for (auto& kv : r) read.insert(kv.first); };
-      for (auto& s : specs) note_read(s.req);
-      for (auto& d : daemons) note_read(pod_requests(d));
-      for (auto& pr : P.provisioners) note_read(pr.limits);
-      E.res_names = {"cpu", "memory", "pods"};
-      for (auto& n : read) if (n != "cpu" && n != "memory" && n != "pods") E.res_names.push_back(n);
-      B.res_pruned = true;
-    }
-    if (E.res_names.size() > KSCHED_MAX_RES) {
-      // Ext resources (DESIGN.md §3): the 8 row slots take cpu, memory, pods and every resource a daemonset requests or a
-      // provisioner limit names, then the other read resources by descending number of requesting pods (ties by name).
-      // The rest is requested by pod classes only, and only the classes requesting it ever read it.
-      std::set<std::string> bound = {"cpu", "memory", "pods"};
-      for (auto& d : daemons) for (auto& kv : pod_requests(d)) bound.insert(kv.first);
-      for (auto& pr : P.provisioners) for (auto& kv : pr.limits) bound.insert(kv.first);
-      if (bound.size() > KSCHED_MAX_RES) unsupported("more than 8 resources that a daemonset requests or a provisioner limit names");
-      if (E.res_names.size() > KSCHED_MAX_RES + KSCHED_MAX_RES_EXT) unsupported("more than 32 resources that a pod requests or a limit names");
-      std::map<std::string, size_t> requesting;
-      for (size_t i = 0; i < NP; ++i) for (auto& kv : specs[E.pod_class[i]].req) ++requesting[kv.first];
-      std::vector<std::string> rest;
-      for (size_t i = 3; i < E.res_names.size(); ++i) if (!bound.count(E.res_names[i])) rest.push_back(E.res_names[i]);
-      std::stable_sort(rest.begin(), rest.end(), [&](const std::string& a, const std::string& b) { return requesting[a] > requesting[b]; });
-      std::vector<std::string> order = {"cpu", "memory", "pods"};
-      for (auto& n : bound) if (n != "cpu" && n != "memory" && n != "pods") order.push_back(n);
-      order.insert(order.end(), rest.begin(), rest.end());
-      E.res_names = order;
-      E.n_res_ext = (int)E.res_names.size() - KSCHED_MAX_RES;
-    }
-    for (size_t i = 0; i < E.res_names.size(); ++i) B.res_id[E.res_names[i]] = (int)i;
+}
+void keys_and_dictionary(Builder& B) {
+  std::set<std::string> foldable;
+  std::set<std::string> active = active_keys(B, &foldable);
+  // Folding is conditional, so that every problem that fits the word keeps its encoding byte for byte: the template-only keys
+  // are folded only when the problem would be refused otherwise, for more than 16 keys or for a template-only key whose values
+  // do not fit (karpenter.sh/provisioner-name with 64 provisioners).
+  bool fold = active.size() > KSCHED_MAX_KEYS;
+  Dictionary D;
+  if (!fold) {
+    D = dictionary(B, active);
+    for (auto& k : foldable) fold = fold || !D.fits(B.key_id.at(k));
   }
+  if (fold) {
+    for (auto& k : foldable) active.erase(k);
+    if (active.size() > KSCHED_MAX_KEYS) unsupported("more than 16 active label keys");
+    B.E.folded_keys.assign(foldable.begin(), foldable.end());
+    D = dictionary(B, active);
+  }
+  B.phase("  value classes");
+  install_dictionary(B, D);
+}
 
-  phase("resources");
-  // ------------------------------------------------------------------ instance types (columns, price order)
+// ------------------------------------------------------------------ resources
+void resources(Builder& B) {
+  const Problem& P = B.P;
+  Encoded& E = B.E;
+  // bound: what a daemonset requests or a provisioner limit names; read: that and what some pod requests; names: every
+  // resource name of the problem
+  std::set<std::string> bound, read = B.facts.req_names, names = B.facts.res_names;  // ClusterFacts: node allocatable / capacity / bound pods
+  for (auto& d : P.daemonset_pods) for (auto& kv : pod_requests(d)) bound.insert(kv.first);
+  for (auto& pr : P.provisioners) for (auto& kv : pr.limits) bound.insert(kv.first);
+  for (auto& s : B.specs) for (auto& kv : s.req) read.insert(kv.first);
+  read.insert(bound.begin(), bound.end());
+  names.insert(read.begin(), read.end());
+  for (auto& it : P.instance_types) for (auto& kv : it.capacity) names.insert(kv.first);
+  E.res_names = resource_order(names);
+  if (E.res_names.size() > KSCHED_MAX_RES) {
+    // Fits reads the request's keys only (resources.go:138-145), the limits bookkeeping the limit's keys only
+    // (scheduler.go:284-303): a name that no pod requests and no limit names cannot change an answer. Left out.
+    E.res_names = resource_order(read);
+    B.res_pruned = true;
+  }
+  if (E.res_names.size() > KSCHED_MAX_RES) {
+    // Ext resources (DESIGN.md §3): the 8 row slots take cpu, memory, pods and every resource a daemonset requests or a
+    // provisioner limit names, then the other read resources by descending number of requesting pods (ties by name).
+    // The rest is requested by pod classes only, and only the classes requesting it ever read it.
+    std::vector<std::string> order = resource_order(bound);
+    if (order.size() > KSCHED_MAX_RES) unsupported("more than 8 resources that a daemonset requests or a provisioner limit names");
+    if (E.res_names.size() > KSCHED_MAX_RES + KSCHED_MAX_RES_EXT) unsupported("more than 32 resources that a pod requests or a limit names");
+    std::map<std::string, size_t> requesting;
+    for (size_t i = 0; i < E.pods.size(); ++i) for (auto& kv : B.specs[E.pod_class[i]].req) ++requesting[kv.first];
+    std::vector<std::string> rest;
+    for (size_t i = 3; i < E.res_names.size(); ++i) if (!bound.count(E.res_names[i])) rest.push_back(E.res_names[i]);
+    std::stable_sort(rest.begin(), rest.end(), [&](const std::string& a, const std::string& b) { return requesting[a] > requesting[b]; });
+    order.insert(order.end(), rest.begin(), rest.end());
+    E.res_names = order;
+    E.n_res_ext = (int)E.res_names.size() - KSCHED_MAX_RES;
+  }
+  for (size_t i = 0; i < E.res_names.size(); ++i) B.res_id[E.res_names[i]] = (int)i;
+}
+
+// ------------------------------------------------------------------ instance types (columns, price order)
+void instance_types(Builder& B) {
+  const Problem& P = B.P;
+  Encoded& E = B.E;
   const int NT = (int)P.instance_types.size();
+  const int zone_key = B.key_of(kZone), ct_key = B.key_of(kCapacityType);
   E.type_words = (NT + 63) / 64;
   if (E.type_words == 0) E.type_words = 1;
-  {
-    std::vector<double> min_price(NT, std::numeric_limits<double>::infinity());
-    for (int i = 0; i < NT; ++i)
-      for (auto& o : P.instance_types[i].offerings)
-        if (o.available && o.price < min_price[i]) min_price[i] = o.price;
-    E.type_input_index.resize(NT);
-    for (int i = 0; i < NT; ++i) E.type_input_index[i] = i;
-    std::stable_sort(E.type_input_index.begin(), E.type_input_index.end(), [&](int a, int b) { return min_price[a] < min_price[b]; });
-    E.types.resize(NT);
-    E.type_capacity.assign((size_t)NT * KSCHED_MAX_RES, 0);
-    E.type_alloc_ext.assign((size_t)NT * E.n_res_ext, 0);
-    // launch-choice table: exact price order through ranks of the distinct (double) prices
-    {
-      std::set<double> prices;
-      for (auto& it : P.instance_types)
-        for (auto& o : it.offerings) if (o.available) prices.insert(o.price);
-      E.price_by_rank.assign(prices.begin(), prices.end());
-      E.offering_keys.assign((size_t)NT * 64, ~0ull);
-    }
-    for (int c = 0; c < NT; ++c) {
-      const InstanceType& it = P.instance_types[E.type_input_index[c]];
-      if (B.type_col.count(it.name)) unsupported("duplicate instance type name " + it.name);
-      B.type_col[it.name] = c;
-      ksched_type_row& row = E.types[c];
-      std::memset(&row, 0, sizeof row);
-      ksched_reqset rs{};
-      ksched_bounds bd{};
-      for (auto& r : it.requirements) {
-        std::string key = normalize_key(r.key);
-        if (key == kHostname) unsupported("instance type with a hostname requirement");
-        if (key == kInstanceType) {
-          if (!(r.op == Op::In && r.values.size() == 1 && r.values[0] == it.name)) unsupported("instance-type requirement of a type must be In [its own name]");
-          continue;
-        }
-        int k = B.key_of(key);
-        if (k < 0) continue;
-        B.add_req(rs, bd, k, B.encode_req(k, r.op, r.values));
+  std::vector<double> min_price(NT, std::numeric_limits<double>::infinity());
+  for (int i = 0; i < NT; ++i)
+    for (auto& o : P.instance_types[i].offerings)
+      if (o.available && o.price < min_price[i]) min_price[i] = o.price;
+  E.type_input_index.resize(NT);
+  for (int i = 0; i < NT; ++i) E.type_input_index[i] = i;
+  std::stable_sort(E.type_input_index.begin(), E.type_input_index.end(), [&](int a, int b) { return min_price[a] < min_price[b]; });
+  E.types.resize(NT);
+  E.type_capacity.assign((size_t)NT * KSCHED_MAX_RES, 0);
+  E.type_alloc_ext.assign((size_t)NT * E.n_res_ext, 0);
+  // launch-choice table: exact price order through ranks of the distinct (double) prices
+  std::set<double> prices;
+  for (auto& it : P.instance_types)
+    for (auto& o : it.offerings) if (o.available) prices.insert(o.price);
+  E.price_by_rank.assign(prices.begin(), prices.end());
+  E.offering_keys.assign((size_t)NT * 64, ~0ull);
+  for (int c = 0; c < NT; ++c) {
+    const InstanceType& it = P.instance_types[E.type_input_index[c]];
+    if (B.type_col.count(it.name)) unsupported("duplicate instance type name " + it.name);
+    B.type_col[it.name] = c;
+    ksched_type_row& row = E.types[c];
+    std::memset(&row, 0, sizeof row);
+    ksched_reqset rs{};
+    ksched_bounds bd{};
+    for (auto& r : it.requirements) {
+      std::string key = normalize_key(r.key);
+      if (key == kHostname) unsupported("instance type with a hostname requirement");
+      if (key == kInstanceType) {
+        if (!(r.op == Op::In && r.values.size() == 1 && r.values[0] == it.name)) unsupported("instance-type requirement of a type must be In [its own name]");
+        continue;
       }
-      B.to_region_form(rs, bd);
-      std::memcpy(row.values, rs.values, sizeof row.values);
-      row.meta = rs.meta;
-      ResourceList overhead = merge(merge(it.kube_reserved, it.system_reserved), it.eviction_threshold);
-      ResourceList alloc = it.capacity;  // resources.Subtract only over keys of capacity
-      for (auto& kv : alloc) { auto o = overhead.find(kv.first); if (o != overhead.end()) kv.second -= o->second; }
-      row.res_present = B.fill_resources(alloc, row.allocatable);
-      B.fill_resources(it.capacity, &E.type_capacity[(size_t)c * KSCHED_MAX_RES]);
-      if (E.n_res_ext) B.fill_ext(alloc, &E.type_alloc_ext[(size_t)c * E.n_res_ext]);
-      for (size_t oi = 0; oi < it.offerings.size(); ++oi) {
-        const Offering& o = it.offerings[oi];
-        if (!o.available) continue;
-        int z = 0, ct = 0;
-        if (zone_key >= 0) { auto f = B.value_id[zone_key].find(o.zone); if (f == B.value_id[zone_key].end()) continue; z = f->second; }
-        if (ct_key >= 0) { auto f = B.value_id[ct_key].find(o.capacity_type); if (f == B.value_id[ct_key].end()) continue; ct = f->second; }
-        if (z >= 16 || ct >= 4) unsupported("more than 16 zones or 4 capacity types");
-        row.offerings |= 1ull << (ct * 16 + z);
-        // (price rank, Offerings list position, slot): the smallest key of a slot wins when several offerings share it
-        if (oi > 255) unsupported("instance type " + it.name + " has more than 256 offerings");
-        const uint64_t rank = (uint64_t)(std::lower_bound(E.price_by_rank.begin(), E.price_by_rank.end(), o.price) - E.price_by_rank.begin());
-        const uint64_t key = (rank << 16) | ((uint64_t)oi << 8) | (uint64_t)(ct * 16 + z);
-        uint64_t& cell = E.offering_keys[(size_t)c * 64 + ct * 16 + z];
-        if (key < cell) cell = key;
-      }
-      row.min_price = min_price[E.type_input_index[c]];
-      row.input_index = (uint32_t)E.type_input_index[c];
+      int k = B.key_of(key);
+      if (k < 0) continue;
+      B.add_req(rs, bd, k, B.encode_req(k, r.op, r.values));
     }
+    B.to_region_form(rs, bd);
+    std::memcpy(row.values, rs.values, sizeof row.values);
+    row.meta = rs.meta;
+    ResourceList overhead = merge(merge(it.kube_reserved, it.system_reserved), it.eviction_threshold);
+    ResourceList alloc = it.capacity;  // resources.Subtract only over keys of capacity
+    for (auto& kv : alloc) { auto o = overhead.find(kv.first); if (o != overhead.end()) kv.second -= o->second; }
+    row.res_present = B.fill_resources(alloc, row.allocatable);
+    B.fill_resources(it.capacity, &E.type_capacity[(size_t)c * KSCHED_MAX_RES]);
+    if (E.n_res_ext) B.fill_ext(alloc, &E.type_alloc_ext[(size_t)c * E.n_res_ext]);
+    // offerings whose zone / capacity-type is not a dictionary value can never satisfy a *present* requirement; when the key
+    // is inactive every offering maps to z=0 / ct=0, which is exactly "key not constrained"
+    for (size_t oi = 0; oi < it.offerings.size(); ++oi) {
+      const Offering& o = it.offerings[oi];
+      if (!o.available) continue;
+      int z = 0, ct = 0;
+      if (zone_key >= 0) { auto f = B.value_id[zone_key].find(o.zone); if (f == B.value_id[zone_key].end()) continue; z = f->second; }
+      if (ct_key >= 0) { auto f = B.value_id[ct_key].find(o.capacity_type); if (f == B.value_id[ct_key].end()) continue; ct = f->second; }
+      if (z >= 16 || ct >= 4) unsupported("more than 16 zones or 4 capacity types");
+      row.offerings |= 1ull << (ct * 16 + z);
+      // (price rank, Offerings list position, slot): the smallest key of a slot wins when several offerings share it
+      if (oi > 255) unsupported("instance type " + it.name + " has more than 256 offerings");
+      const uint64_t rank = (uint64_t)(std::lower_bound(E.price_by_rank.begin(), E.price_by_rank.end(), o.price) - E.price_by_rank.begin());
+      const uint64_t key = (rank << 16) | ((uint64_t)oi << 8) | (uint64_t)(ct * 16 + z);
+      uint64_t& cell = E.offering_keys[(size_t)c * 64 + ct * 16 + z];
+      if (key < cell) cell = key;
+    }
+    row.min_price = min_price[E.type_input_index[c]];
+    row.input_index = (uint32_t)E.type_input_index[c];
   }
-  // offerings whose zone / capacity-type is not a dictionary value can never satisfy a *present* requirement,
-  // but they do satisfy an absent one: keep them visible through a catch-all bit when the key is inactive.
-  // (When zone/ct keys are inactive every offering maps to z=0/ct=0 above, which is exactly "key not constrained".)
+}
 
-  phase("instance types");
-  // ------------------------------------------------------------------ templates
-  const int NV = (int)E.template_provisioner.size();
+// The instance types that every one of a list of instance-type requirements admits, as (complement, names).
+std::pair<bool, std::set<std::string>> itype_intersection(const std::vector<NodeSelectorRequirement>& rs) {
+  bool comp = true;  // (true, {}): every type
+  std::set<std::string> names;
+  for (auto& r : rs) {
+    if (r.op == Op::Gt || r.op == Op::Lt) unsupported("Gt/Lt on instance-type");
+    bool rc = !(r.op == Op::In || r.op == Op::DoesNotExist);
+    std::set<std::string> rv;
+    if (r.op == Op::In || r.op == Op::NotIn) rv.insert(r.values.begin(), r.values.end());
+    std::set<std::string> nv;
+    if (comp && rc) { nv = names; nv.insert(rv.begin(), rv.end()); }
+    else if (comp && !rc) { for (auto& x : rv) if (!names.count(x)) nv.insert(x); }
+    else if (!comp && rc) { for (auto& x : names) if (!rv.count(x)) nv.insert(x); }
+    else { for (auto& x : names) if (rv.count(x)) nv.insert(x); }
+    comp = comp && rc;
+    names = nv;
+  }
+  return {comp, names};
+}
+// Its instance-type columns: bit col % 64 of word col / 64 is set when the type of column col is admitted.
+std::vector<uint64_t> itype_columns(const Builder& B, const std::pair<bool, std::set<std::string>>& set) {
+  std::vector<uint64_t> words((size_t)B.E.type_words, 0);
+  for (int col = 0; col < (int)B.E.types.size(); ++col) {
+    bool in = set.second.count(B.P.instance_types[B.E.type_input_index[col]].name) > 0;
+    if (set.first ? !in : in) words[col / 64] |= 1ull << (col % 64);
+  }
+  return words;
+}
+
+// ------------------------------------------------------------------ templates
+void templates(Builder& B) {
+  const Problem& P = B.P;
+  Encoded& E = B.E;
+  const int NV = (int)E.template_provisioner.size(), NT = (int)P.instance_types.size();
   E.templates.resize(NV);
   E.template_bounds.resize(NV);
-  std::vector<ksched_bounds> tb(NV);
   for (int v = 0; v < NV; ++v) {
     const Provisioner& pr = P.provisioners[E.template_provisioner[v]];
     ksched_template& t = E.templates[v];
     std::memset(&t, 0, sizeof t);
-    std::memset(&tb[v], 0, sizeof(ksched_bounds));
+    std::memset(&E.template_bounds[v], 0, sizeof(ksched_bounds));
     Builder::Special sp;
-    B.add_selector_reqs(t.reqs, tb[v], pr.requirements, &sp);  // NewMachineTemplate machinetemplate.go:46-62
-    Labels l = pr.labels;
-    l[kProvisionerName] = pr.name;
-    B.add_selector_reqs(t.reqs, tb[v], Builder::label_reqs(l), &sp);
+    B.add_selector_reqs(t.reqs, E.template_bounds[v], pr.requirements, &sp);  // NewMachineTemplate machinetemplate.go:46-62
+    B.add_selector_reqs(t.reqs, E.template_bounds[v], label_reqs(template_labels(pr)), &sp);
     if (!sp.hostname.empty()) unsupported("provisioner with a hostname requirement");
-    // instance-type requirement of the provisioner: fold into membership (types are singletons on that key)
-    std::vector<bool> allowed(NT, true);
-    for (auto& r : sp.itype) {
-      std::set<std::string> names(r.values.begin(), r.values.end());
-      for (int c = 0; c < NT; ++c) {
-        const std::string& name = P.instance_types[E.type_input_index[c]].name;
-        bool ok = true;
-        if (r.op == Op::In) ok = names.count(name) > 0;
-        else if (r.op == Op::NotIn) ok = !names.count(name);
-        else if (r.op == Op::DoesNotExist) ok = false;
-        else if (r.op == Op::Gt || r.op == Op::Lt) unsupported("Gt/Lt on instance-type");
-        allowed[c] = allowed[c] && ok;
-      }
-    }
+    // instance-type requirement of the provisioner: fold into membership (types are singletons on that key); without instance
+    // types nothing is folded (nor refused)
+    const std::vector<uint64_t> allowed = NT ? itype_columns(B, itype_intersection(sp.itype)) : std::vector<uint64_t>((size_t)E.type_words, 0);
     for (int idx : pr.instance_types) {
       int c = B.type_col.at(P.instance_types.at(idx).name);
-      if (allowed[c]) E.types[c].template_members |= 1ull << v;
+      if ((allowed[c / 64] >> (c % 64)) & 1) E.types[c].template_members |= 1ull << v;
     }
     t.taintset = (uint32_t)B.taintset(pr.taints);
     // at most KSCHED_MAX_TEMPLATES templates, encoded before any existing node: the template side reads only the 64-bit word
@@ -1212,7 +1227,6 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
     t.limit_present = B.fill_resources(pr.limits, t.remaining);
     if (t.reqs.meta >> KSCHED_META_HASGT_SHIFT) E.any_template_bounds = true;
   }
-  E.template_bounds = tb;
   // Template-only keys (DESIGN.md §3): filterInstanceTypesByRequirements (node.go:137-145) keeps a type only when its
   // requirements intersect the node's, and on such a key the node's requirement is always its template's
   // (NewMachineTemplate: provisioner requirements, then labels, machinetemplate.go:46-62). Types that fail it on some folded
@@ -1234,10 +1248,8 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
     }
     for (int v = 0; v < NV; ++v) {
       const Provisioner& pr = P.provisioners[E.template_provisioner[v]];
-      Labels l = pr.labels;
-      l[kProvisionerName] = pr.name;
       std::vector<NodeSelectorRequirement> tmpl = on_key(pr.requirements);
-      for (auto& r : on_key(Builder::label_reqs(l))) tmpl.push_back(r);
+      for (auto& r : on_key(label_reqs(template_labels(pr)))) tmpl.push_back(r);
       if (tmpl.empty()) continue;
       const FoldedKey own({&tmpl});
       E.template_folded[v][key] = own.render(own.req(tmpl));
@@ -1248,35 +1260,45 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
       }
     }
   }
+}
 
-  phase("templates");
-  // ------------------------------------------------------------------ daemonset overhead (scheduler.go:250-267)
-  auto daemon_reqs = [&](const Pod& d, ksched_reqset& rs, ksched_bounds& bd) {
-    Builder::Special sp;
-    B.pod_requirements(d, rs, bd, &sp);
-    return sp;
-  };
-  for (int v = 0; v < NV; ++v) {
-    const Provisioner& pr = P.provisioners[E.template_provisioner[v]];
-    ResourceList total;
-    int count = 0;
-    for (auto& d : daemons) {
-      if (!tolerates_all(pr.taints, d.tolerations)) continue;
-      ksched_reqset rs{}; ksched_bounds bd{};
-      auto sp = daemon_reqs(d, rs, bd);
-      if (!sp.hostname.empty() || !sp.itype.empty()) unsupported("daemonset pod with hostname / instance-type requirement");
-      if (!B.compatible(E.templates[v].reqs, tb[v], rs, bd)) continue;
-      total = merge(total, pod_requests(d));
-      ++count;
-    }
-    total["pods"] = (int64_t)count * 1000;
-    E.templates[v].daemon_res_present = B.fill_resources(total, E.templates[v].daemon_requests);
+// ------------------------------------------------------------------ daemonset overhead (scheduler.go:250-267)
+// The daemonset pods a node with these taints and requirements runs: their requests, and one pod each. A template refuses a
+// daemon that tolerates its taints and names a hostname or an instance type.
+ResourceList daemon_overhead(const Builder& B, const std::vector<Taint>& taints, const ksched_reqset& rs, const ksched_bounds& bd, bool is_template) {
+  ResourceList total;
+  int count = 0;
+  for (auto& d : B.daemons) {
+    if (!tolerates_all(taints, d.pod->tolerations)) continue;
+    if (is_template && d.special) unsupported("daemonset pod with hostname / instance-type requirement");
+    if (!B.compatible(rs, bd, d.rs, d.bd)) continue;
+    total = merge(total, d.req);
+    ++count;
   }
+  total["pods"] = (int64_t)count * 1000;
+  return total;
+}
+void daemonset_overhead(Builder& B) {
+  for (auto& d : B.P.daemonset_pods) {
+    Daemon x{&d, {}, {}, false, pod_requests(d)};
+    Builder::Special sp;
+    B.pod_requirements(d, x.rs, x.bd, &sp);
+    x.special = !sp.hostname.empty() || !sp.itype.empty();
+    B.daemons.push_back(x);
+  }
+  for (size_t v = 0; v < B.E.templates.size(); ++v) {
+    ksched_template& t = B.E.templates[v];
+    const ResourceList total = daemon_overhead(B, B.P.provisioners[B.E.template_provisioner[v]].taints, t.reqs, B.E.template_bounds[v], true);
+    t.daemon_res_present = B.fill_resources(total, t.daemon_requests);
+  }
+}
 
-  phase("daemonset overhead");
-  // ------------------------------------------------------------------ existing nodes (scheduler.go:221-248, existingnode.go:41-75)
-  std::map<std::string, int> hostname_slot;  // hostname -> existing slot
-  for (int si : state_nodes) {
+// ------------------------------------------------------------------ existing nodes (scheduler.go:221-248, existingnode.go:41-75)
+void existing_nodes(Builder& B) {
+  const Problem& P = B.P;
+  Encoded& E = B.E;
+  const int NV = (int)E.templates.size();
+  for (int si : B.state_nodes) {
     const StateNode& n = P.nodes[si];
     auto own = n.labels.find(kProvisionerName);
     if (own == n.labels.end() || own->second.empty()) continue;  // !node.Owned()
@@ -1284,25 +1306,13 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
     std::memset(&e, 0, sizeof e);
     ksched_bounds nb{};
     Builder::Special sp;
-    const NodeFacts& nf = facts.node[(size_t)si];
+    const NodeFacts& nf = B.facts.node[(size_t)si];
     B.add_selector_reqs(e.reqs, nb, nf.label_reqs, &sp);
-    ResourceList daemon_total;
-    int dcount = 0;
-    for (auto& d : daemons) {
-      if (!tolerates_all(n.taints, d.tolerations)) continue;  // raw Spec.Taints (scheduler.go:231)
-      ksched_reqset rs{}; ksched_bounds bd{};
-      daemon_reqs(d, rs, bd);
-      if (!B.compatible(e.reqs, nb, rs, bd)) continue;
-      daemon_total = merge(daemon_total, pod_requests(d));
-      ++dcount;
-    }
-    daemon_total["pods"] = (int64_t)dcount * 1000;
-    const ResourceList& pod_req = nf.pod_req;
-    const ResourceList& ds_req = nf.ds_req;
-    ResourceList rem = daemon_total;  // resources.Subtract over keys of lhs, clamped at 0
-    for (auto& kv : rem) { auto f = ds_req.find(kv.first); if (f != ds_req.end()) kv.second -= f->second; if (kv.second < 0) kv.second = 0; }
+    // the daemonsets' requests not yet bound: resources.Subtract over keys of lhs, clamped at 0
+    ResourceList rem = daemon_overhead(B, n.taints, e.reqs, nb, false);  // raw Spec.Taints (scheduler.go:231)
+    for (auto& kv : rem) { auto f = nf.ds_req.find(kv.first); if (f != nf.ds_req.end()) kv.second -= f->second; if (kv.second < 0) kv.second = 0; }
     ResourceList avail = n.allocatable;
-    for (auto& kv : avail) { auto f = pod_req.find(kv.first); if (f != pod_req.end()) kv.second -= f->second; }
+    for (auto& kv : avail) { auto f = nf.pod_req.find(kv.first); if (f != nf.pod_req.end()) kv.second -= f->second; }
     e.available_present = B.fill_resources(avail, e.available);
     e.requests_present = B.fill_resources(rem, e.requests);
     if (E.n_res_ext) {
@@ -1318,25 +1328,25 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
     auto h = n.labels.find(kHostname);
     if (h != n.labels.end()) hostname = h->second;
     if (hostname.empty()) hostname = n.name;
-    hostname_slot[hostname] = (int)E.existing.size();
+    B.hostname_slot[hostname] = (int)E.existing.size();
     E.existing_state_index.push_back(si);
     auto ini = n.labels.find(kInitialized);
     E.existing_initialized.push_back(ini != n.labels.end() && ini->second == "true");
-    if (!vol_drivers.empty()) {  // state.Node.VolumeUsage() / VolumeLimits() (state/cluster.go:292-303,340-347)
+    if (!B.vol_drivers.empty()) {  // state.Node.VolumeUsage() / VolumeLimits() (state/cluster.go:292-303,340-347)
       ksched_node_volumes nv{};
       std::map<std::string, std::set<std::string>> mounted;
-      for (auto& p : n.pods) for (auto& kv : pod_claims(p)) mounted[kv.first].insert(kv.second.begin(), kv.second.end());
+      for (auto& p : n.pods) for (auto& kv : B.pod_claims(p)) mounted[kv.first].insert(kv.second.begin(), kv.second.end());
       bool over = false;
       for (size_t d = 0; d < KSCHED_MAX_VOLUME_DRIVERS; ++d) {
         nv.limit[d] = -1;
-        if (d >= vol_drivers.size()) continue;
-        auto l = n.volume_limits.find(vol_drivers[d]);
+        if (d >= B.vol_drivers.size()) continue;
+        auto l = n.volume_limits.find(B.vol_drivers[d]);
         if (l != n.volume_limits.end()) nv.limit[d] = l->second;
         int total = 0;
-        for (auto& c : mounted[vol_drivers[d]]) {
+        for (auto& c : mounted[B.vol_drivers[d]]) {
           ++total;
-          auto t = vol_tracked.find({vol_drivers[d], c});
-          if (t != vol_tracked.end()) nv.mounted |= 1ull << t->second; else nv.used[d]++;
+          auto t = B.vol_tracked.find({B.vol_drivers[d], c});
+          if (t != B.vol_tracked.end()) nv.mounted |= 1ull << t->second; else nv.used[d]++;
         }
         if (nv.limit[d] >= 0 && total > nv.limit[d]) over = true;
       }
@@ -1355,61 +1365,67 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
           if ((E.templates[v].limit_present >> r) & 1 && (present >> r) & 1) { E.templates[v].remaining[r] -= cap[r]; charged_cap[r] = cap[r]; }
         charged = v;
       }
-    if (cluster_superset) {
+    if (B.superset) {
       E.existing_template.push_back(charged);
       E.existing_capacity.insert(E.existing_capacity.end(), charged_cap, charged_cap + KSCHED_MAX_RES);
     }
   }
-  if (cluster_superset) {
-    std::map<int, int> slot_of_state;
-    for (size_t e = 0; e < E.existing_state_index.size(); ++e) slot_of_state[E.existing_state_index[e]] = (int)e;
-    for (auto& pn : E.pod_node)
-      if (pn <= -2) {
-        auto f = slot_of_state.find(-2 - pn);
-        if (f == slot_of_state.end()) throw std::runtime_error("a candidate node is not owned by a provisioner");
-        pn = f->second;
-      }
-  }
-  const int NE = (int)E.existing.size();
+  if (!B.superset) return;
+  std::map<int, int> slot_of_state;
+  for (size_t e = 0; e < E.existing_state_index.size(); ++e) slot_of_state[E.existing_state_index[e]] = (int)e;
+  for (auto& pn : E.pod_node)
+    if (pn <= -2) {
+      auto f = slot_of_state.find(-2 - pn);
+      if (f == slot_of_state.end()) throw std::runtime_error("a candidate node is not owned by a provisioner");
+      pn = f->second;
+    }
+}
 
-  phase("existing nodes");
-  // ------------------------------------------------------------------ topology groups (topology.go)
+// ------------------------------------------------------------------ topology groups (topology.go)
+struct Topology {
+  const Builder& B;
   std::vector<Group> groups;
   std::map<std::string, size_t> group_of;          // hash -> index, non-inverse
   std::map<std::string, size_t> inverse_group_of;  // hash -> index, inverse
   // domain universe: provisioner.go:266-276 (requirement.Values() of every type + provisioner In requirements). Only topology
   // keys read it, and their values are never collapsed into classes, so the strings here are the dictionary's own.
   std::map<std::string, std::set<std::string>> universe;
-  for (int v = 0; v < NV; ++v) {
-    const Provisioner& pr = P.provisioners[E.template_provisioner[v]];
-    for (int idx : pr.instance_types)
-      for (auto& r : P.instance_types[idx].requirements)
-        if (r.op == Op::In || r.op == Op::NotIn) universe[normalize_key(r.key)].insert(r.values.begin(), r.values.end());
-    // NewNodeSelectorRequirements(provisioner.Spec.Requirements...) then Operator()==In
-    std::map<std::string, std::vector<NodeSelectorRequirement>> by_key;
-    for (auto& r : pr.requirements) by_key[normalize_key(r.key)].push_back(r);
-    for (auto& kv : by_key) {
-      int k = B.key_of(kv.first);
-      if (k < 0) {  // inactive key: only needed when a single In requirement exists
-        if (kv.second.size() == 1 && kv.second[0].op == Op::In) universe[kv.first].insert(kv.second[0].values.begin(), kv.second[0].values.end());
-        continue;
+  std::unordered_set<std::string> excluded;  // pods of the batch are not counted as cluster pods (topology.go:66-70)
+  explicit Topology(const Builder& b) : B(b) {
+    const Problem& P = B.P;
+    for (int pi : B.E.template_provisioner) {
+      const Provisioner& pr = P.provisioners[pi];
+      for (int idx : pr.instance_types)
+        for (auto& r : P.instance_types[idx].requirements)
+          if (r.op == Op::In || r.op == Op::NotIn) universe[normalize_key(r.key)].insert(r.values.begin(), r.values.end());
+      // NewNodeSelectorRequirements(provisioner.Spec.Requirements...) then Operator()==In
+      std::map<std::string, std::vector<NodeSelectorRequirement>> by_key;
+      for (auto& r : pr.requirements) by_key[normalize_key(r.key)].push_back(r);
+      for (auto& kv : by_key) {
+        int k = B.key_of(kv.first);
+        if (k < 0) {  // inactive key: only needed when a single In requirement exists
+          if (kv.second.size() == 1 && kv.second[0].op == Op::In) universe[kv.first].insert(kv.second[0].values.begin(), kv.second[0].values.end());
+          continue;
+        }
+        ksched_reqset rs{}; ksched_bounds bd{};
+        B.add_selector_reqs(rs, bd, kv.second, nullptr);
+        Req r = ksched::req_load(rs, &bd, k);
+        if (!r.complement && r.values)
+          for (int b = 0; b < 64; ++b) if ((r.values >> b) & 1) universe[kv.first].insert(B.E.key_values[k][b]);
       }
-      ksched_reqset rs{}; ksched_bounds bd{};
-      B.add_selector_reqs(rs, bd, kv.second, nullptr);
-      Req r = ksched::req_load(rs, &bd, k);
-      if (!r.complement && r.values)
-        for (int b = 0; b < 64; ++b) if ((r.values >> b) & 1) universe[kv.first].insert(E.key_values[k][b]);
+    }
+    bool any_bound = false;  // only consulted for pods bound to nodes
+    for (auto& n : P.nodes) any_bound = any_bound || !n.pods.empty();
+    if (any_bound) {
+      excluded.reserve(B.E.pods.size() * 2);
+      for (auto* p : B.E.pods) excluded.insert(p->uid);
     }
   }
-  auto namespace_list = [](const std::string& ns, const std::vector<std::string>& nss) {
-    if (nss.empty()) return std::set<std::string>{ns};
-    return std::set<std::string>(nss.begin(), nss.end());
-  };
-  auto make_filter = [&](Group& g, const Pod& p) {  // MakeTopologyNodeFilter topologynodefilter.go:30-47
+  void make_filter(Group& g, const Pod& p) const {  // MakeTopologyNodeFilter topologynodefilter.go:30-47
     g.filter_nil = false;
     auto canon = [&](const ksched_reqset& rs, const ksched_bounds& bd) {
       std::string s;
-      for (int k = 0; k < NK; ++k) {
+      for (int k = 0; k < (int)B.E.key_names.size(); ++k) {
         Req r = ksched::req_load(rs, &bd, k);
         if (!r.present) continue;
         s += std::to_string(k) + ":" + std::to_string(r.complement) + ":" + std::to_string(r.values) + ":" +
@@ -1421,7 +1437,7 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
     auto add_term = [&](const std::vector<NodeSelectorRequirement>* term) {
       ksched_reqset rs{}; ksched_bounds bd{};
       Builder::Special sp;
-      B.add_selector_reqs(rs, bd, Builder::label_reqs(p.node_selector), &sp);
+      B.add_selector_reqs(rs, bd, label_reqs(p.node_selector), &sp);
       if (term) B.add_selector_reqs(rs, bd, *term, &sp);
       if (!sp.hostname.empty() || !sp.itype.empty()) unsupported("topology spread node filter on hostname / instance-type");
       g.filter.push_back({rs, bd});
@@ -1431,140 +1447,109 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
     else for (auto& t : p.required_node_terms) add_term(&t);
     std::sort(parts.begin(), parts.end());
     for (auto& s : parts) g.filter_key += "(" + s + ")";
-  };
-  auto filter_matches_labels = [&](const Group& g, const Labels& labels) {  // TopologyNodeFilter.Matches
+  }
+  bool filter_matches_labels(const Group& g, const Labels& labels) const {  // TopologyNodeFilter.Matches
     if (g.filter_nil || g.filter.empty()) return true;
     ksched_reqset rs{}; ksched_bounds bd{};
     Builder::Special sp;
-    B.add_selector_reqs(rs, bd, Builder::label_reqs(labels), &sp);
+    B.add_selector_reqs(rs, bd, label_reqs(labels), &sp);
     for (auto& f : g.filter)
       if (B.compatible(rs, bd, f.first, f.second)) return true;
     return false;
-  };
-  // pods of the batch are not counted as cluster pods (topology.go:66-70); only consulted for pods bound to nodes
-  std::unordered_set<std::string> excluded;
-  {
-    bool any_bound = false;
-    for (auto& n : P.nodes) any_bound = any_bound || !n.pods.empty();
-    if (any_bound) {
-      excluded.reserve(NP * 2);
-      for (auto* p : E.pods) excluded.insert(p->uid);
-    }
   }
-  auto new_group = [&](int type, const std::string& key, const Pod& p, std::set<std::string> nss, const LabelSelector& sel, int32_t skew) {
+  Group new_group(int type, const std::string& key, const Pod& p, const std::vector<std::string>& nss, const LabelSelector& sel, int32_t skew) const {
     Group g;
-    g.type = type; g.key = key; g.max_skew = skew; g.namespaces = std::move(nss); g.selector = sel;
+    g.type = type; g.key = key; g.max_skew = skew; g.selector = sel;
+    if (nss.empty()) g.namespaces = {p.ns};
+    else g.namespaces.insert(nss.begin(), nss.end());
     if (type == 0) make_filter(g, p);
     else g.filter_key = "<nil>";
     auto u = universe.find(key);
     if (u != universe.end()) for (auto& d : u->second) g.counts[d] = 0;
     return g;
-  };
-  auto count_domains = [&](Group& g) {  // topology.go:231-276
-    for (auto& n : P.nodes)
+  }
+  void count_domains(Group& g) const {  // topology.go:231-276
+    for (auto& n : B.P.nodes)
       for (auto& p : n.pods) {
         if (!g.namespaces.count(p.ns)) continue;
         if (!g.selector.is_nil && !selector_matches(g.selector, p.labels)) continue;  // TopologyListOptions: nil lists everything
         if (p.terminal || p.terminating) continue;
         if (excluded.count(p.uid)) continue;
-        std::string domain;
         auto it = n.labels.find(g.key);
-        bool ok = it != n.labels.end();
-        if (ok) domain = it->second;
-        if (!ok && g.key == kHostname) { domain = n.name; ok = true; }
-        if (!ok) continue;
+        if (it == n.labels.end() && g.key != kHostname) continue;  // a node without a hostname label is its own domain
         if (!filter_matches_labels(g, n.labels)) continue;
-        g.counts[domain]++;
+        g.counts[it != n.labels.end() ? it->second : n.name]++;
       }
-  };
-  auto spec_groups = [&](const Pod& p) {  // newForTopologies + newForAffinities topology.go:278-322
-    std::vector<Group> out;
-    for (auto& cs : p.topology_spread) out.push_back(new_group(0, cs.topology_key, p, {p.ns}, cs.selector, cs.max_skew));
-    for (auto& t : p.pod_affinity_required) out.push_back(new_group(1, t.topology_key, p, namespace_list(p.ns, t.namespaces), t.selector, INT32_MAX));
-    for (auto& t : p.pod_affinity_preferred) out.push_back(new_group(1, t.term.topology_key, p, namespace_list(p.ns, t.term.namespaces), t.term.selector, INT32_MAX));
-    for (auto& t : p.pod_anti_affinity_required) out.push_back(new_group(2, t.topology_key, p, namespace_list(p.ns, t.namespaces), t.selector, INT32_MAX));
-    for (auto& t : p.pod_anti_affinity_preferred) out.push_back(new_group(2, t.term.topology_key, p, namespace_list(p.ns, t.term.namespaces), t.term.selector, INT32_MAX));
-    return out;
-  };
-  auto inverse_groups = [&](const Pod& p, const Labels* node_labels, int owner_spec) {  // updateInverseAntiAffinity topology.go:202-227
-    for (auto& term : p.pod_anti_affinity_required) {
-      Group g = new_group(2, term.topology_key, p, namespace_list(p.ns, term.namespaces), term.selector, INT32_MAX);
-      g.inverse = true;
-      std::string h = g.hash();
-      auto it = inverse_group_of.find(h);
-      size_t gi;
-      if (it == inverse_group_of.end()) { gi = groups.size(); inverse_group_of[h] = gi; groups.push_back(std::move(g)); }
-      else gi = it->second;
-      if (node_labels) {
-        auto d = node_labels->find(groups[gi].key);
-        if (d != node_labels->end()) groups[gi].counts[d->second]++;
-      }
-      if (owner_spec >= 0) groups[gi].owner_specs.insert((size_t)owner_spec);
-    }
-  };
-  if (!P.empty_topology) {
-    for (auto& n : P.nodes)  // updateInverseAffinities topology.go:185-198
+  }
+  // The group of a topology term, made and counted (countDomains) when it is new; a relaxed variant's new group is dormant.
+  size_t add_group(Group g, bool dormant) {
+    const std::string h = g.hash();
+    auto it = group_of.find(h);
+    if (it != group_of.end()) return it->second;
+    group_of[h] = groups.size();
+    g.dormant = dormant;
+    count_domains(g);
+    groups.push_back(std::move(g));
+    return groups.size() - 1;
+  }
+  // The inverse anti-affinity group of a required anti-affinity term (updateInverseAntiAffinity topology.go:202-227), made
+  // when it is new and `create`; -1 when it does not exist.
+  int inverse_group(const Pod& p, const PodAffinityTerm& term, bool create) {
+    Group g = new_group(2, term.topology_key, p, term.namespaces, term.selector, INT32_MAX);
+    g.inverse = true;
+    const std::string h = g.hash();
+    auto it = inverse_group_of.find(h);
+    if (it != inverse_group_of.end()) return (int)it->second;
+    if (!create) return -1;
+    inverse_group_of[h] = groups.size();
+    groups.push_back(std::move(g));
+    return (int)groups.size() - 1;
+  }
+  void build() {
+    for (auto& n : B.P.nodes)  // updateInverseAffinities topology.go:185-198
       for (auto& p : n.pods) {
         if (p.pod_anti_affinity_required.empty() || excluded.count(p.uid)) continue;
-        inverse_groups(p, &n.labels, -1);
-      }
-    // Topology.Update for every pod of the batch, in Solve's pod order (topology.go:73-75); group creation order
-    // only matters for countDomains, which is order-independent.
-    std::vector<bool> seen(specs.size(), false);
-    for (size_t i = 0; i < NP; ++i) {
-      uint32_t s = E.pod_class[i];
-      if (seen[s]) continue;
-      seen[s] = true;
-      const Pod& p = specs[s].pod;
-      if (!p.pod_anti_affinity_required.empty() || !p.pod_anti_affinity_preferred.empty()) inverse_groups(p, nullptr, (int)s);
-      for (auto& g : spec_groups(p)) {
-        std::string h = g.hash();
-        auto it = group_of.find(h);
-        size_t gi;
-        if (it == group_of.end()) { gi = groups.size(); group_of[h] = gi; count_domains(g); groups.push_back(std::move(g)); }
-        else gi = it->second;
-        groups[gi].owner_specs.insert(s);
-      }
-    }
-    // relaxed variants: Topology.Update after Relax (scheduler.go:119-123). Their groups must already exist.
-    for (size_t s = 0; s < specs.size(); ++s) {
-      if (seen[s]) continue;
-      const Pod& p = specs[s].pod;
-      if (!p.pod_anti_affinity_required.empty() || !p.pod_anti_affinity_preferred.empty()) {
         for (auto& term : p.pod_anti_affinity_required) {
-          Group g = new_group(2, term.topology_key, p, namespace_list(p.ns, term.namespaces), term.selector, INT32_MAX);
-          g.inverse = true;
-          auto it = inverse_group_of.find(g.hash());
-          if (it == inverse_group_of.end()) unsupported("relaxation creates a new inverse topology group");
-          groups[it->second].owner_specs.insert(s);
+          Group& g = groups[(size_t)inverse_group(p, term, true)];
+          auto d = n.labels.find(g.key);
+          if (d != n.labels.end()) g.counts[d->second]++;
         }
       }
-      for (auto& g : spec_groups(p)) {
-        std::string h = g.hash();
-        auto it = group_of.find(h);
-        size_t gi;
-        if (it == group_of.end()) {
-          // Topology.Update creates this group when the pod is relaxed (e.g. the node filter of a spread constraint
-          // changes with the required node-affinity terms): counts come from the cluster at that moment, which is the
-          // same static state countDomains sees at the start of the solve.
-          gi = groups.size();
-          group_of[h] = gi;
-          g.dormant = true;
-          count_domains(g);
-          groups.push_back(std::move(g));
-        } else {
-          gi = it->second;
-        }
-        groups[gi].owner_specs.insert(s);
+    // Topology.Update of every class of the batch, in Solve's pod order (topology.go:73-75); group creation order only matters
+    // for countDomains, which is order-independent. Then of the relaxed variants (Topology.Update after Relax,
+    // scheduler.go:119-123): their inverse groups must already exist, and a new group (e.g. the node filter of a spread
+    // constraint changes with the required node-affinity terms) is dormant and counts the cluster at that moment, which is the
+    // same static state countDomains sees at the start of the solve.
+    std::vector<bool> seen(B.specs.size(), false);
+    std::vector<uint32_t> order;
+    for (uint32_t s : B.E.pod_class) if (!seen[s]) { seen[s] = true; order.push_back(s); }
+    const size_t n_batch = order.size();
+    for (uint32_t s = 0; s < (uint32_t)B.specs.size(); ++s) if (!seen[s]) order.push_back(s);
+    for (size_t i = 0; i < order.size(); ++i) {
+      const uint32_t s = order[i];
+      const bool relaxed = i >= n_batch;
+      const Pod& p = B.specs[s].pod;
+      for (auto& term : p.pod_anti_affinity_required) {
+        const int gi = inverse_group(p, term, !relaxed);
+        if (gi < 0) unsupported("relaxation creates a new inverse topology group");
+        groups[(size_t)gi].owner_specs.insert(s);
       }
+      pod_topology_terms(p, [&](int type, const std::string& key, const std::vector<std::string>& nss, const LabelSelector& sel, int32_t skew) {
+        groups[add_group(new_group(type, key, p, nss, sel, skew), relaxed)].owner_specs.insert(s);
+      });
     }
   }
-  const int NG = (int)groups.size();
+};
+
+// The groups' flat rows, their node filters and their counts per domain / per existing node.
+void group_tables(Builder& B, const std::vector<Group>& groups) {
+  Encoded& E = B.E;
+  const int NG = (int)groups.size(), NE = (int)E.existing.size();
   E.groups.resize(NG);
   E.group_domain_counts.assign((size_t)NG * 64, 0);
   E.group_existing_counts.assign((size_t)NG * std::max(NE, 1), 0);
   for (int g = 0; g < NG; ++g) {
-    Group& G = groups[g];
+    const Group& G = groups[g];
     ksched_topo_group& o = E.groups[g];
     std::memset(&o, 0, sizeof o);
     o.type = (uint8_t)G.type;
@@ -1581,8 +1566,8 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
     if (G.key == kHostname) {
       o.key = KSCHED_KEY_HOSTNAME;
       for (auto& kv : G.counts) {
-        auto s = hostname_slot.find(kv.first);
-        if (s != hostname_slot.end()) E.group_existing_counts[(size_t)g * std::max(NE, 1) + s->second] = kv.second;
+        auto s = B.hostname_slot.find(kv.first);
+        if (s != B.hostname_slot.end()) E.group_existing_counts[(size_t)g * std::max(NE, 1) + s->second] = kv.second;
         else if (kv.second > 0) o.extra_nonzero_domains++;
       }
     } else {
@@ -1602,64 +1587,73 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
       }
     }
   }
+}
 
-  if (cluster_superset && NG > 0) {
-    // What countDomains (topology.go:231-276) and updateInverseAffinities (:183-227) would add for a bound pod of each class,
-    // split into its class part (namespace, selector, owned inverse groups) and its node part (label value, node filter).
-    const int NCs = (int)specs.size();
-    E.class_count_begin.assign((size_t)NCs + 1, 0);
-    for (int c = 0; c < NCs; ++c) {
-      const Pod& p = specs[(size_t)c].pod;
-      E.class_count_begin[(size_t)c] = (uint32_t)E.class_count.size();
-      std::map<size_t, int> inverse_times;
-      for (auto& term : p.pod_anti_affinity_required) {
-        Group g = new_group(2, term.topology_key, p, namespace_list(p.ns, term.namespaces), term.selector, INT32_MAX);
-        g.inverse = true;
-        auto it = inverse_group_of.find(g.hash());
-        if (it != inverse_group_of.end()) inverse_times[it->second]++;
-      }
-      for (int g = 0; g < NG; ++g) {
-        const Group& G = groups[(size_t)g];
-        if (G.inverse) {
-          auto it = inverse_times.find((size_t)g);
-          if (it != inverse_times.end()) E.class_count.push_back({(uint32_t)g, KSCHED_COUNT_INVERSE, (uint8_t)std::min(it->second, 255), 0});
-        } else if (G.namespaces.count(p.ns) && (G.selector.is_nil || selector_matches(G.selector, p.labels))) {
-          E.class_count.push_back({(uint32_t)g, KSCHED_COUNT_DOMAINS, 1, 0});
-        }
-      }
+// What countDomains (topology.go:231-276) and updateInverseAffinities (:183-227) would add for a bound pod of each class,
+// split into its class part (namespace, selector, owned inverse groups) and its node part (label value, node filter).
+void superset_counts(Builder& B, Topology& T) {
+  Encoded& E = B.E;
+  const int NG = (int)T.groups.size(), NE = (int)E.existing.size(), NK = (int)E.key_names.size();
+  const int NCs = (int)B.specs.size();
+  E.class_count_begin.assign((size_t)NCs + 1, 0);
+  for (int c = 0; c < NCs; ++c) {
+    const Pod& p = B.specs[(size_t)c].pod;
+    E.class_count_begin[(size_t)c] = (uint32_t)E.class_count.size();
+    std::map<size_t, int> inverse_times;
+    for (auto& term : p.pod_anti_affinity_required) {
+      const int gi = T.inverse_group(p, term, false);
+      if (gi >= 0) inverse_times[(size_t)gi]++;
     }
-    E.class_count_begin[(size_t)NCs] = (uint32_t)E.class_count.size();
-    E.node_domain.assign((size_t)std::max(NK, 1) * std::max(NE, 1), -1);
-    E.node_has_hostname_label.assign((size_t)std::max(NE, 1), 0);
-    const int FW = (NE + 31) / 32;
-    E.group_filter_match.assign((size_t)NG * std::max(FW, 1), 0);
-    std::map<std::string, std::vector<char>> filter_memo;  // node labels without the hostname -> verdict per group
-    for (int e = 0; e < NE; ++e) {
-      const StateNode& n = P.nodes[(size_t)E.existing_state_index[(size_t)e]];
-      for (int k = 0; k < NK; ++k) {
-        auto l = n.labels.find(E.key_names[(size_t)k]);
-        if (l == n.labels.end()) continue;
-        auto v = B.value_id[(size_t)k].find(l->second);
-        if (v != B.value_id[(size_t)k].end()) E.node_domain[(size_t)k * NE + e] = (int8_t)v->second;
+    for (int g = 0; g < NG; ++g) {
+      const Group& G = T.groups[(size_t)g];
+      if (G.inverse) {
+        auto it = inverse_times.find((size_t)g);
+        if (it != inverse_times.end()) E.class_count.push_back({(uint32_t)g, KSCHED_COUNT_INVERSE, (uint8_t)std::min(it->second, 255), 0});
+      } else if (G.namespaces.count(p.ns) && (G.selector.is_nil || selector_matches(G.selector, p.labels))) {
+        E.class_count.push_back({(uint32_t)g, KSCHED_COUNT_DOMAINS, 1, 0});
       }
-      E.node_has_hostname_label[(size_t)e] = n.labels.count(kHostname) ? 1 : 0;
-      Labels sig = n.labels;
-      sig.erase(kHostname);
-      const std::string key = labels_key(sig);
-      auto memo = filter_memo.find(key);
-      if (memo == filter_memo.end()) {
-        std::vector<char> v((size_t)NG, 1);
-        for (int g = 0; g < NG; ++g) v[(size_t)g] = filter_matches_labels(groups[(size_t)g], n.labels) ? 1 : 0;
-        memo = filter_memo.emplace(key, std::move(v)).first;
-      }
-      for (int g = 0; g < NG; ++g)
-        if (memo->second[(size_t)g]) E.group_filter_match[(size_t)g * FW + (e >> 5)] |= 1u << (e & 31);
     }
   }
+  E.class_count_begin[(size_t)NCs] = (uint32_t)E.class_count.size();
+  E.node_domain.assign((size_t)std::max(NK, 1) * std::max(NE, 1), -1);
+  E.node_has_hostname_label.assign((size_t)std::max(NE, 1), 0);
+  const int FW = (NE + 31) / 32;
+  E.group_filter_match.assign((size_t)NG * std::max(FW, 1), 0);
+  std::map<std::string, std::vector<char>> filter_memo;  // node labels without the hostname -> verdict per group
+  for (int e = 0; e < NE; ++e) {
+    const StateNode& n = B.P.nodes[(size_t)E.existing_state_index[(size_t)e]];
+    for (int k = 0; k < NK; ++k) {
+      auto l = n.labels.find(E.key_names[(size_t)k]);
+      if (l == n.labels.end()) continue;
+      auto v = B.value_id[(size_t)k].find(l->second);
+      if (v != B.value_id[(size_t)k].end()) E.node_domain[(size_t)k * NE + e] = (int8_t)v->second;
+    }
+    E.node_has_hostname_label[(size_t)e] = n.labels.count(kHostname) ? 1 : 0;
+    Labels sig = n.labels;
+    sig.erase(kHostname);
+    const std::string key = labels_key(sig);
+    auto memo = filter_memo.find(key);
+    if (memo == filter_memo.end()) {
+      std::vector<char> v((size_t)NG, 1);
+      for (int g = 0; g < NG; ++g) v[(size_t)g] = T.filter_matches_labels(T.groups[(size_t)g], n.labels) ? 1 : 0;
+      memo = filter_memo.emplace(key, std::move(v)).first;
+    }
+    for (int g = 0; g < NG; ++g)
+      if (memo->second[(size_t)g]) E.group_filter_match[(size_t)g * FW + (e >> 5)] |= 1u << (e & 31);
+  }
+}
+std::vector<Group> topology_groups(Builder& B) {
+  Topology T(B);
+  if (!B.P.empty_topology) T.build();
+  group_tables(B, T.groups);
+  if (B.superset && !T.groups.empty()) superset_counts(B, T);
+  return std::move(T.groups);
+}
 
-  phase("topology groups");
-  // ------------------------------------------------------------------ class rows
-  const int NC = (int)specs.size();
+// ------------------------------------------------------------------ class rows
+void class_rows(Builder& B, const std::vector<Group>& groups) {
+  Encoded& E = B.E;
+  const int NC = (int)B.specs.size(), NG = (int)groups.size();
   E.classes.resize(NC);
   E.class_bounds.resize(NC);
   std::map<std::string, uint32_t> itype_req_id;
@@ -1670,7 +1664,7 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
       for (int g = 0; g < NG; ++g) {
         const Group& G = groups[g];
         const bool owns = G.owner_specs.count(c) > 0;
-        const bool sel = G.selects(specs[c].pod);
+        const bool sel = G.selects(B.specs[c].pod);
         uint32_t flags = 0;
         if (sel) flags |= KSCHED_TOPO_SELECTS;
         if (!G.inverse && owns) flags |= KSCHED_TOPO_CONSTRAINS;
@@ -1680,61 +1674,42 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
         rel[c * NG + g] = (uint8_t)flags;
       }
   });
-  phase("  class relations");
+  B.phase("  class relations");
+  // Sets from id 64 on are existing nodes' only; their bits go to a table of their own, so problems with at most 64 sets encode
+  // as before.
+  const size_t NS = B.taintsets.size();
+  E.n_taintsets = (int)NS;
+  E.tolerated_ext_words = NS > 64 ? (int)((NS - 64 + 63) / 64) : 0;
+  E.class_tolerated_ext.assign((size_t)NC * E.tolerated_ext_words, 0);
   E.class_requests_ext.assign((size_t)NC * E.n_res_ext, 0);
   E.class_res_ext_present.assign(E.n_res_ext ? NC : 0, 0);
   for (int c = 0; c < NC; ++c) {
-    const Pod& p = specs[c].pod;
+    const Spec& s = B.specs[c];
     ksched_pod_row& row = E.classes[c];
     std::memset(&row, 0, sizeof row);
     std::memset(&E.class_bounds[c], 0, sizeof(ksched_bounds));
-    row.res_present = B.fill_resources(specs[c].req, row.requests);
-    if (E.n_res_ext) E.class_res_ext_present[c] = B.fill_ext(specs[c].req, &E.class_requests_ext[(size_t)c * E.n_res_ext]);
+    row.res_present = B.fill_resources(s.req, row.requests);
+    if (E.n_res_ext) E.class_res_ext_present[c] = B.fill_ext(s.req, &E.class_requests_ext[(size_t)c * E.n_res_ext]);
     ksched_reqset rs{};
     Builder::Special sp;
-    B.pod_requirements(p, rs, E.class_bounds[c], &sp);
+    B.pod_requirements(s.pod, rs, E.class_bounds[c], &sp);
     std::memcpy(row.values, rs.values, sizeof row.values);
     row.meta = rs.meta;
     if (rs.meta >> KSCHED_META_HASGT_SHIFT) E.any_class_bounds = true;
-    row.relax_next = specs[c].next;
+    row.relax_next = s.next;
     row.reserved = (uint64_t)c;  // class index, so a row copied into the FFD-ordered pod matrix knows its class
     row.itype_req = KSCHED_NONE;
     row.hostname_req = KSCHED_NONE;
     if (!sp.itype.empty()) {
-      // intersection of all instance-type requirements of the pod as (complement, name set)
-      bool comp = true;
-      std::set<std::string> names;
-      bool first = true;
-      for (auto& r : sp.itype) {
-        if (r.op == Op::Gt || r.op == Op::Lt) unsupported("Gt/Lt on instance-type");
-        bool rc = !(r.op == Op::In || r.op == Op::DoesNotExist);
-        std::set<std::string> rv;
-        if (r.op == Op::In || r.op == Op::NotIn) rv.insert(r.values.begin(), r.values.end());
-        if (first) { comp = rc; names = rv; first = false; continue; }
-        std::set<std::string> nv;
-        if (comp && rc) { nv = names; nv.insert(rv.begin(), rv.end()); }
-        else if (comp && !rc) { for (auto& x : rv) if (!names.count(x)) nv.insert(x); }
-        else if (!comp && rc) { for (auto& x : names) if (!rv.count(x)) nv.insert(x); }
-        else { for (auto& x : names) if (rv.count(x)) nv.insert(x); }
-        comp = comp && rc;
-        names = nv;
-      }
-      std::string key = std::to_string(comp) + ":";
-      for (auto& n : names) key += n + ",";
-      auto it = itype_req_id.find(key);
-      if (it == itype_req_id.end()) {
-        uint32_t id = (uint32_t)E.itype_req_complement.size();
-        itype_req_id[key] = id;
-        E.itype_req_complement.push_back(comp ? 1 : 0);
-        size_t base = E.itype_req_sets.size();
-        E.itype_req_sets.resize(base + E.type_words, 0);
-        for (int col = 0; col < NT; ++col) {
-          bool in = names.count(P.instance_types[E.type_input_index[col]].name) > 0;
-          if (comp ? !in : in) E.itype_req_sets[base + col / 64] |= 1ull << (col % 64);
-        }
-        row.itype_req = id;
-      } else {
-        row.itype_req = it->second;
+      const auto set = itype_intersection(sp.itype);
+      std::string key = std::to_string(set.first) + ":";
+      for (auto& n : set.second) key += n + ",";
+      auto id = itype_req_id.emplace(key, (uint32_t)E.itype_req_complement.size());
+      row.itype_req = id.first->second;
+      if (id.second) {
+        E.itype_req_complement.push_back(set.first ? 1 : 0);
+        const std::vector<uint64_t> words = itype_columns(B, set);
+        E.itype_req_sets.insert(E.itype_req_sets.end(), words.begin(), words.end());
       }
     }
     if (!sp.hostname.empty()) {
@@ -1745,13 +1720,17 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
       else if (r.op == Op::NotIn && r.values.size() == 1) comp = 1;
       else if (r.op == Op::Exists) comp = 1;
       else unsupported("hostname requirement form");
-      if (!r.values.empty()) { auto s = hostname_slot.find(r.values[0]); if (s != hostname_slot.end()) slot = s->second; }
+      if (!r.values.empty()) { auto h = B.hostname_slot.find(r.values[0]); if (h != B.hostname_slot.end()) slot = h->second; }
       row.hostname_req = (uint32_t)(E.hostname_reqs.size() / 2);
       E.hostname_reqs.push_back(comp);
       E.hostname_reqs.push_back(slot);
     }
-    auto hps = host_ports(p);
-    for (auto& hp : hps) row.hostport_entries |= 1ull << B.hp_entry(hp);
+    for (auto& hp : host_ports(s.pod)) row.hostport_entries |= 1ull << B.hp_entry(hp);
+    for (size_t t = 0; t < NS; ++t) {  // the taint-set table is complete: templates and existing nodes are encoded
+      if (!tolerates_all(B.taintsets[t], s.pod.tolerations)) continue;
+      if (t < 64) row.tolerated_taintsets |= 1ull << t;
+      else E.class_tolerated_ext[(size_t)c * E.tolerated_ext_words + (t - 64) / 64] |= 1ull << ((t - 64) % 64);
+    }
     // topology relations
     row.topo_begin = (uint32_t)E.class_topo.size();
     for (int g = 0; g < NG; ++g) {
@@ -1760,71 +1739,56 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
     }
     row.topo_end = (uint32_t)E.class_topo.size();
   }
-  if (!vol_drivers.empty()) {
+  if (!B.vol_drivers.empty()) {
     E.class_volumes.resize(NC);
     bool any = false;
-    for (int c = 0; c < NC; ++c) any = !volume_signature(specs[c].pod, &E.class_volumes[c]).empty() || any;
+    for (int c = 0; c < NC; ++c) any = !B.volume_signature(B.specs[c].pod, &E.class_volumes[c]).empty() || any;
     if (!any) E.class_volumes.clear();  // no pod of the batch mounts a limited claim: the kernels never look
-    for (auto& kv : vol_tracked) {
-      const size_t d = (size_t)(std::find(vol_drivers.begin(), vol_drivers.end(), kv.first.first) - vol_drivers.begin());
-      E.volume_driver_mask[d] |= 1ull << kv.second;
-    }
+    for (auto& kv : B.vol_tracked) E.volume_driver_mask[B.driver_index(kv.first.first)] |= 1ull << kv.second;
   }
-  // host-port conflict masks and tolerated taint sets need the complete entry / taint-set tables. Sets from id 64 on are
-  // existing nodes' only; their bits go to a table of their own, so problems with at most 64 sets encode as before.
-  const size_t NS = B.taintsets.size();
-  E.n_taintsets = (int)NS;
-  E.tolerated_ext_words = NS > 64 ? (int)((NS - 64 + 63) / 64) : 0;
-  E.class_tolerated_ext.assign((size_t)NC * E.tolerated_ext_words, 0);
-  for (int c = 0; c < NC; ++c) {
-    const Pod& p = specs[c].pod;
-    for (auto& hp : host_ports(p))
+  // host-port conflict masks need the complete entry table
+  for (int c = 0; c < NC; ++c)
+    for (auto& hp : host_ports(B.specs[c].pod))
       for (size_t e = 0; e < B.hp_entries.size(); ++e)
         if (hp_matches(hp, B.hp_entries[e])) E.classes[c].hostport_conflicts |= 1ull << e;
-    for (size_t s = 0; s < NS; ++s) {
-      if (!tolerates_all(B.taintsets[s], p.tolerations)) continue;
-      if (s < 64) E.classes[c].tolerated_taintsets |= 1ull << s;
-      else E.class_tolerated_ext[(size_t)c * E.tolerated_ext_words + (s - 64) / 64] |= 1ull << ((s - 64) % 64);
-    }
-  }
+}
 
-  phase("class rows");
-  // ------------------------------------------------------------------ per-pod queue keys (queue.go:74-110)
+// ------------------------------------------------------------------ per-pod queue keys (queue.go:74-110)
+void queue_keys(Builder& B) {
+  Encoded& E = B.E;
+  const size_t NP = E.pods.size();
   E.pod_uid_rank.resize(NP);
-  {
-    if (uids_ascending) {
-      for (size_t i = 0; i < NP; ++i) E.pod_uid_rank[i] = (uint32_t)i;
-    } else {
-      std::vector<uint32_t> order(NP);
-      for (size_t i = 0; i < NP; ++i) order[i] = (uint32_t)i;
-      std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return E.pods[a]->uid < E.pods[b]->uid; });
-      for (size_t r = 0; r < NP; ++r) E.pod_uid_rank[order[r]] = (uint32_t)r;
-    }
+  if (B.uids_ascending) {
+    for (size_t i = 0; i < NP; ++i) E.pod_uid_rank[i] = (uint32_t)i;
+    return;
   }
+  std::vector<uint32_t> order(NP);
+  for (size_t i = 0; i < NP; ++i) order[i] = (uint32_t)i;
+  std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return E.pods[a]->uid < E.pods[b]->uid; });
+  for (size_t r = 0; r < NP; ++r) E.pod_uid_rank[order[r]] = (uint32_t)r;
+}
 
-  phase("queue keys");
-  // ------------------------------------------------------------------ wire up the flat structs
+// ------------------------------------------------------------------ wire up the flat structs
+void wire(Builder& B) {
+  Encoded& E = B.E;
+  const int NE = (int)E.existing.size(), NC = (int)E.classes.size(), NV = (int)E.templates.size();
   ksched_catalog& cat = E.catalog;
-  cat.n_keys = NK; cat.n_res = (int)E.res_names.size() - E.n_res_ext; cat.n_types = NT; cat.n_templates = NV;
+  cat.n_keys = (int)E.key_names.size(); cat.n_res = (int)E.res_names.size() - E.n_res_ext; cat.n_types = (int)E.types.size(); cat.n_templates = NV;
   cat.n_res_ext = E.n_res_ext;
   cat.type_alloc_ext = E.n_res_ext ? E.type_alloc_ext.data() : nullptr;
   cat.keys = E.keys.data();
   cat.key_int_values = E.key_int_values.data();
   cat.types = E.types.data();
-  cat.type_bounds = nullptr;
   cat.type_capacity = E.type_capacity.data();
   cat.templates = E.templates.data();
-  cat.template_bounds = nullptr;
   cat.offering_keys = E.offering_keys.data();
   ksched_problem& pr = E.problem;
-  pr.n_pods = (int)NP; pr.n_classes = NC; pr.n_existing = NE; pr.n_groups = NG;
+  pr.n_pods = (int)E.pods.size(); pr.n_classes = NC; pr.n_existing = NE; pr.n_groups = (int)E.groups.size();
   pr.classes = E.classes.data();
-  pr.class_bounds = nullptr;
   pr.pod_class = E.pod_class.data();
   pr.pod_timestamp = E.pod_timestamp.data();
   pr.pod_uid_rank = E.pod_uid_rank.data();
   pr.existing = E.existing.data();
-  pr.existing_bounds = nullptr;
   pr.groups = E.groups.data();
   pr.group_domain_counts = E.group_domain_counts.data();
   pr.group_existing_counts = E.group_existing_counts.data();
@@ -1837,8 +1801,7 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
   pr.n_itype_reqs = (int)E.itype_req_complement.size();
   pr.hostname_reqs = E.hostname_reqs.data();
   pr.n_hostname_reqs = (int)E.hostname_reqs.size() / 2;
-  pr.max_new_nodes = (int)NP;
-  pr.write_feasibility = 0;
+  pr.max_new_nodes = (int)E.pods.size();
   if (!E.class_volumes.empty() && NE > 0) {
     pr.class_volumes = E.class_volumes.data();
     pr.existing_volumes = E.existing_volumes.data();
@@ -1853,7 +1816,7 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
   }
   pr.count_nodes_visited = 0;  // the exact nodes_visited statistic is opt-in (kh_set_count_visited / tests): it turns the pack kernel's steady-state paths off
   // Gt/Lt leave the host algebra here: templates and pod classes in region form (types and filter terms already are)
-  for (int v = 0; v < NV; ++v) B.to_region_form(E.templates[v].reqs, tb[v]);
+  for (int v = 0; v < NV; ++v) B.to_region_form(E.templates[v].reqs, E.template_bounds[v]);
   for (int c = 0; c < NC; ++c) {
     ksched_reqset rs{};
     std::memcpy(rs.values, E.classes[c].values, sizeof rs.values);
@@ -1863,6 +1826,38 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
     E.classes[c].meta = rs.meta;
   }
   cat.key_regions = E.key_regions.empty() ? nullptr : E.key_regions.data();
+}
+
+}  // namespace
+
+std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candidates, bool cluster_superset) {
+  auto enc = std::make_unique<Encoded>();
+  enc->problem_ref = &P;
+  Builder B(P, *enc, cluster_superset);
+  participants(B, candidates);
+  B.phase("who takes part");
+  csi_volumes(B);
+  pod_classes(B);
+  B.phase("pod classes");
+  keys_and_dictionary(B);
+  B.phase("keys + dictionary");
+  resources(B);
+  B.phase("resources");
+  instance_types(B);
+  B.phase("instance types");
+  templates(B);
+  B.phase("templates");
+  daemonset_overhead(B);
+  B.phase("daemonset overhead");
+  existing_nodes(B);
+  B.phase("existing nodes");
+  const std::vector<Group> groups = topology_groups(B);
+  B.phase("topology groups");
+  class_rows(B, groups);
+  B.phase("class rows");
+  queue_keys(B);
+  B.phase("queue keys");
+  wire(B);
   return enc;
 }
 

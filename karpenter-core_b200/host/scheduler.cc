@@ -345,6 +345,16 @@ Encoded* kh_encode(const Problem* P, const int* candidates, int ncand) {
     return nullptr;
   }
 }
+// the cluster-superset encoding ksched_load_cluster takes (tests digest it like kh_encode's)
+Encoded* kh_encode_cluster(const Problem* P, const int* candidates, int ncand) {
+  try {
+    std::vector<int> c(candidates, candidates + ncand);
+    return khost::encode(*P, c, true).release();
+  } catch (const std::exception& e) {
+    fail(error_code(e), e.what());
+    return nullptr;
+  }
+}
 void kh_encoded_free(Encoded* E) {
   if (E == g_gpu_encoded) { g_gpu_encoded = nullptr; g_gpu_current = false; }
   delete E;
@@ -1306,6 +1316,17 @@ extern "C" unsigned long long kh_encoded_digest(const Encoded* E) {
     for (auto& k : E->folded_keys) str(k);
     for (auto& m : E->template_folded) { size_t n = m.size(); bytes(&n, sizeof n); for (auto& kv : m) { str(kv.first); str(kv.second); } }
   }
+  // absent when no key has value classes: those digests predate them
+  if (std::any_of(E->key_representatives.begin(), E->key_representatives.end(), [](int32_t n) { return n != 0; })) vec(E->key_representatives);
+  // cluster-superset fields, each absent when empty: plain encodings leave them empty and their digests predate them
+  if (!E->pod_node.empty()) vec(E->pod_node);
+  if (!E->existing_template.empty()) vec(E->existing_template);
+  if (!E->existing_capacity.empty()) vec(E->existing_capacity);
+  if (!E->class_count_begin.empty()) vec(E->class_count_begin);
+  if (!E->class_count.empty()) vec(E->class_count);
+  if (!E->node_domain.empty()) vec(E->node_domain);
+  if (!E->node_has_hostname_label.empty()) vec(E->node_has_hostname_label);
+  if (!E->group_filter_match.empty()) vec(E->group_filter_match);
   const ksched_catalog& c = E->catalog;
   int cat[4] = {c.n_keys, c.n_res, c.n_types, c.n_templates};
   bytes(cat, sizeof cat);

@@ -12,7 +12,7 @@ sys.path.insert(0, str(ROOT / "tests" / "golden"))
 def test_encoder_output_matches_committed_digests(pkg):
     import make_encoding_digests as m
     want = json.loads((ROOT / "tests" / "golden" / "encoding_digests.json").read_text())
-    got = {name: m.digest(pkg, problem, cands) for name, problem, cands in m.corpus(pkg)}
+    got = {name: m.digest(pkg, problem, cands, superset) for name, problem, cands, superset in m.corpus(pkg)}
     assert set(got) == set(want)
     wrong = [n for n in got if got[n] != want[n]]
     assert not wrong, wrong[:10]

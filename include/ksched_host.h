@@ -39,7 +39,14 @@ typedef struct kh_result kh_result;    /* ([]*Node, []*ExistingNode) of one Solv
 typedef struct kh_cluster kh_cluster;  /* one consolidation pass: candidates ranked, cluster resident on the device */
 
 /* ---- problems and results */
-kh_problem* kh_problem_from_json(const char* text); /* NULL on a parse error: kh_last_error() */
+/* NULL on a parse error: kh_last_error(). Pod (anti-)affinity terms, required and preferred, of pending, bound and daemonset
+ * pods: {labelSelector, namespaces[], namespaceSelector, topologyKey}. A namespaceSelector ({} selects every namespace) is
+ * resolved as buildNamespaceList does (topology.go:326-347) against the document's top-level namespaces[] {name, labels},
+ * the cluster's Namespace objects. Refused here: a namespaceSelector in a document without namespaces[], one that
+ * metav1.LabelSelectorAsSelector rejects (an operator other than In / NotIn / Exists / DoesNotExist, In / NotIn without
+ * values, Exists / DoesNotExist with values, an invalid label key or value), duplicate namespace names, and a pod or
+ * Namespace named "<no namespace>" (the loader's name for a selector that resolved to no namespace). */
+kh_problem* kh_problem_from_json(const char* text);
 void kh_problem_free(kh_problem* p);
 const char* kh_last_error(void);
 long long kh_parse_quantity(const char* s);         /* k8s resource.Quantity -> milli-units */

@@ -131,21 +131,7 @@ bool selector_valid(const LabelSelector& s) {
   return true;
 }
 bool selector_matches(const LabelSelector& s, const Labels& labels) {  // s non-nil
-  if (!selector_valid(s)) return false;
-  for (auto& kv : s.match_labels) {
-    auto it = labels.find(kv.first);
-    if (it == labels.end() || it->second != kv.second) return false;
-  }
-  for (auto& e : s.match_expressions) {
-    auto it = labels.find(e.key);
-    bool has = it != labels.end();
-    bool in = has && std::find(e.values.begin(), e.values.end(), it->second) != e.values.end();
-    if (e.op == Op::In && !in) return false;
-    if (e.op == Op::NotIn && has && in) return false;
-    if (e.op == Op::Exists && !has) return false;
-    if (e.op == Op::DoesNotExist && has) return false;
-  }
-  return true;
+  return selector_valid(s) && selector_matches_labels(s, labels);
 }
 std::string selector_key(const LabelSelector& s) {
   if (s.is_nil) return "<nil>";
@@ -182,6 +168,7 @@ std::string labels_key(const Labels& l) {
 std::string term_key(const PodAffinityTerm& t) {
   std::string s = t.topology_key + "|" + selector_key(t.selector) + "|";
   for (auto& n : t.namespaces) s += n + ",";
+  if (!t.namespace_selector.is_nil) s += "|ns=" + selector_key(t.namespace_selector);
   return s;
 }
 
@@ -197,7 +184,8 @@ bool same_selector(const LabelSelector& a, const LabelSelector& b) {
   return a.is_nil == b.is_nil && a.match_labels == b.match_labels && same_reqs(a.match_expressions, b.match_expressions);
 }
 bool same_term(const PodAffinityTerm& a, const PodAffinityTerm& b) {
-  return a.topology_key == b.topology_key && a.namespaces == b.namespaces && same_selector(a.selector, b.selector);
+  return a.topology_key == b.topology_key && a.namespaces == b.namespaces && same_selector(a.selector, b.selector) &&
+         same_selector(a.namespace_selector, b.namespace_selector);
 }
 template <class T, class F>
 bool same_vec(const std::vector<T>& a, const std::vector<T>& b, F eq) {
@@ -251,12 +239,18 @@ uint64_t spec_hash(const Pod& p) {
   for (auto& t : p.required_node_terms) { mix(t.size()); for (auto& r : t) { str(r.key); mix((uint64_t)r.op); mix(r.values.size()); } }
   mix(p.preferred_node_terms.size());
   for (auto& t : p.preferred_node_terms) mix((uint64_t)t.weight);
+  // a namespace selector is mixed in only where one is set: pods without one hash as they always did
+  auto ns_selector = [&](const PodAffinityTerm& t) {
+    if (!t.namespace_selector.is_nil) { labels(t.namespace_selector.match_labels); mix(t.namespace_selector.match_expressions.size() + 1); }
+  };
   mix(p.pod_affinity_required.size());
-  for (auto& t : p.pod_affinity_required) str(t.topology_key);
+  for (auto& t : p.pod_affinity_required) { str(t.topology_key); ns_selector(t); }
   mix(p.pod_affinity_preferred.size());
+  for (auto& t : p.pod_affinity_preferred) ns_selector(t.term);
   mix(p.pod_anti_affinity_required.size());
-  for (auto& t : p.pod_anti_affinity_required) str(t.topology_key);
+  for (auto& t : p.pod_anti_affinity_required) { str(t.topology_key); ns_selector(t); }
   mix(p.pod_anti_affinity_preferred.size());
+  for (auto& t : p.pod_anti_affinity_preferred) ns_selector(t.term);
   mix(p.topology_spread.size());
   for (auto& t : p.topology_spread) { mix((uint64_t)t.max_skew); str(t.topology_key); mix((uint64_t)t.schedule_anyway); }
   mix(p.tolerations.size());

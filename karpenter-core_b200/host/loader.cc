@@ -3,6 +3,8 @@
 // (pkg/test/pods.go:62-111, pkg/test/provisioner.go, pkg/cloudprovider/fake/instancetype.go).
 #include "loader.h"
 
+#include <cctype>
+#include <set>
 #include <stdexcept>
 
 #include "json.h"
@@ -106,13 +108,94 @@ LabelSelector selector(const Value* v) {
   s.match_expressions = reqs(v->get("matchExpressions"));
   return s;
 }
+// k8s.io/apimachinery validation: a label name part / value ([A-Za-z0-9]([-A-Za-z0-9_.]*[A-Za-z0-9])?, at most 63) and a
+// qualified name (an optional DNS-1123 subdomain prefix and '/' before the name part).
+bool label_name_part(const std::string& s) {
+  if (s.empty() || s.size() > 63 || !std::isalnum((unsigned char)s.front()) || !std::isalnum((unsigned char)s.back())) return false;
+  for (unsigned char c : s)
+    if (!std::isalnum(c) && c != '-' && c != '_' && c != '.') return false;
+  return true;
+}
+bool qualified_name(const std::string& s) {
+  const size_t slash = s.find('/');
+  if (slash == std::string::npos) return label_name_part(s);
+  const std::string prefix = s.substr(0, slash), name = s.substr(slash + 1);
+  if (prefix.empty() || prefix.size() > 253 || name.find('/') != std::string::npos) return false;
+  for (size_t i = 0; i < prefix.size(); ++i) {
+    const char c = prefix[i];
+    const bool alnum = (c >= 'a' && c <= 'z') || (c >= '0' && c <= '9');
+    const bool edge = i == 0 || i + 1 == prefix.size() || prefix[i - 1] == '.' || prefix[i + 1] == '.';
+    if (!alnum && (edge || (c != '-' && c != '.'))) return false;
+  }
+  return label_name_part(name);
+}
+// metav1.LabelSelectorAsSelector's checks (labels.NewRequirement): buildNamespaceList returns its error, so NewScheduler
+// fails on a namespaceSelector it rejects.
+void check_namespace_selector(const LabelSelector& s) {
+  auto fail = [](const std::string& why) { throw std::runtime_error("invalid namespaceSelector: " + why); };
+  for (auto& kv : s.match_labels) {
+    if (!qualified_name(kv.first)) fail("label key \"" + kv.first + "\"");
+    if (!kv.second.empty() && !label_name_part(kv.second)) fail("label value \"" + kv.second + "\"");
+  }
+  for (auto& r : s.match_expressions) {
+    if (r.op != Op::In && r.op != Op::NotIn && r.op != Op::Exists && r.op != Op::DoesNotExist)
+      fail("\"" + r.key + "\": operator is not one of In, NotIn, Exists, DoesNotExist");
+    if (!qualified_name(r.key)) fail("label key \"" + r.key + "\"");
+    const bool set_op = r.op == Op::In || r.op == Op::NotIn;
+    if (set_op && r.values.empty()) fail("\"" + r.key + "\": In and NotIn need values");
+    if (!set_op && !r.values.empty()) fail("\"" + r.key + "\": Exists and DoesNotExist take no values");
+    for (auto& v : r.values)
+      if (!v.empty() && !label_name_part(v)) fail("label value \"" + v + "\"");
+  }
+}
 PodAffinityTerm affinity_term(const Value& e) {
   PodAffinityTerm t;
   t.selector = selector(e.get("labelSelector"));
   if (const Value* ns = e.get("namespaces"))
     for (auto& x : ns->arr) t.namespaces.push_back(x.str);
+  t.namespace_selector = selector(e.get("namespaceSelector"));
+  if (!t.namespace_selector.is_nil) check_namespace_selector(t.namespace_selector);
   t.topology_key = e.s("topologyKey");
   return t;
+}
+// buildNamespaceList (topology.go:326-347) of every term with a namespaceSelector, done once here because the document
+// holds all it reads: the term's `namespaces` become the Namespace objects the selector matches plus the ones the term
+// named (the pod's own namespace is not added), {kNoNamespace} when that is empty (model.h). A batch repeats one term
+// thousands of times, so each distinct selector is matched against the Namespaces once.
+void resolve_namespace_selectors(Problem& P, bool listed) {
+  std::map<std::string, std::vector<std::string>> matched;  // selector -> the Namespaces it matches
+  auto resolve = [&](PodAffinityTerm& t) {
+    if (t.namespace_selector.is_nil) return;
+    if (!listed) throw std::runtime_error("a pod affinity term has a namespaceSelector but the document lists no namespaces");
+    std::string key;
+    for (auto& kv : t.namespace_selector.match_labels) key += kv.first + "=" + kv.second + ",";
+    for (auto& r : t.namespace_selector.match_expressions) {
+      key += "|" + r.key + ":" + std::to_string((int)r.op) + ":";
+      for (auto& v : r.values) key += v + ",";
+    }
+    auto it = matched.find(key);
+    if (it == matched.end()) {
+      std::vector<std::string> names;
+      for (auto& n : P.namespaces)
+        if (selector_matches_labels(t.namespace_selector, n.labels)) names.push_back(n.name);
+      it = matched.emplace(key, std::move(names)).first;
+    }
+    std::set<std::string> out(it->second.begin(), it->second.end());
+    out.insert(t.namespaces.begin(), t.namespaces.end());
+    if (out.empty()) out.insert(kNoNamespace);
+    t.namespaces.assign(out.begin(), out.end());
+  };
+  auto pod_terms = [&](Pod& p) {
+    if (p.ns == kNoNamespace) throw std::runtime_error("a pod may not be in namespace " + p.ns);
+    for (auto* terms : {&p.pod_affinity_required, &p.pod_anti_affinity_required})
+      for (auto& t : *terms) resolve(t);
+    for (auto* terms : {&p.pod_affinity_preferred, &p.pod_anti_affinity_preferred})
+      for (auto& t : *terms) resolve(t.term);
+  };
+  for (auto* ps : {&P.pods, &P.daemonset_pods})
+    for (auto& p : *ps) pod_terms(p);
+  for (auto& n : P.nodes)
+    for (auto& p : n.pods) pod_terms(p);
 }
 std::vector<Taint> taints(const Value* v) {
   std::vector<Taint> out;
@@ -295,6 +378,18 @@ Problem* problem_from_json(const char* text) {
       b.disruptions_allowed = (int32_t)e.i("disruptionsAllowed");
       P.pdbs.push_back(std::move(b));
     }
+  const Value* nss = root.get("namespaces");
+  const bool listed = nss && !nss->is_null();
+  if (listed) {
+    std::set<std::string> names;
+    for (auto& e : nss->arr) {
+      Namespace n{e.s("name"), labels(e.get("labels"))};
+      if (n.name == kNoNamespace) throw std::runtime_error("a Namespace may not be named " + n.name);
+      if (!names.insert(n.name).second) throw std::runtime_error("duplicate namespace " + n.name);
+      P.namespaces.push_back(std::move(n));
+    }
+  }
+  resolve_namespace_selectors(P, listed);
   P.now_ts = root.d("now");
   P.derive_candidates = root.boolean("deriveCandidates");
   P.simulation_mode = root.boolean("simulationMode");

@@ -48,9 +48,36 @@ struct LabelSelector {
   std::vector<NodeSelectorRequirement> match_expressions;  // In/NotIn/Exists/DoesNotExist
 };
 
+// Selector.Matches of a selector that LabelSelectorAsSelector accepts (matchLabels; In / NotIn / Exists / DoesNotExist,
+// where NotIn matches a missing key).
+inline bool selector_matches_labels(const LabelSelector& s, const Labels& labels) {
+  for (auto& kv : s.match_labels) {
+    auto it = labels.find(kv.first);
+    if (it == labels.end() || it->second != kv.second) return false;
+  }
+  for (auto& e : s.match_expressions) {
+    auto it = labels.find(e.key);
+    const bool has = it != labels.end();
+    bool in = false;
+    for (auto& v : e.values) in = in || (has && it->second == v);
+    if ((e.op == Op::In && !in) || (e.op == Op::NotIn && in) || (e.op == Op::Exists && !has) || (e.op == Op::DoesNotExist && has))
+      return false;
+  }
+  return true;
+}
+
+// The namespace list of a term whose namespaceSelector resolved to no namespace at all. It is not a DNS-1123 label, so no
+// Namespace can carry it, and the loader refuses pods and Namespaces named so: a group over it counts and selects nobody.
+inline const char* const kNoNamespace = "<no namespace>";
+
+// v1.PodAffinityTerm. namespace_selector: nil = not set, {} = every namespace. The loader resolves a set selector as
+// buildNamespaceList does (topology.go:326-347) against Problem::namespaces: `namespaces` then holds the resolved set
+// (the matched Namespaces plus the ones the term named, in string order, or {kNoNamespace} when that is empty), so every
+// reader of `namespaces` sees the namespaces the term's group counts. The selector itself stays for the term's identity.
 struct PodAffinityTerm {
   LabelSelector selector;
   std::vector<std::string> namespaces;
+  LabelSelector namespace_selector;
   std::string topology_key;
 };
 struct WeightedPodAffinityTerm {
@@ -177,6 +204,12 @@ struct PodDisruptionBudget {
   int32_t disruptions_allowed = 0;
 };
 
+// v1.Namespace as buildNamespaceList lists it (topology.go:338-345)
+struct Namespace {
+  std::string name;
+  Labels labels;
+};
+
 // Derived, dictionary-independent facts about the cluster state that every encoding of the same Problem needs again
 // (consolidation encodes one Problem once per probe): filled lazily by the encoder, owned by the Problem.
 struct ProblemDerived {
@@ -200,6 +233,7 @@ struct Problem {
   std::vector<Pod> pods;            // pending pods handed to Solve
   std::vector<Pod> daemonset_pods;  // daemonset template pods (getDaemonSetPods)
   std::vector<PodDisruptionBudget> pdbs;
+  std::vector<Namespace> namespaces;  // the cluster's Namespace objects; the loader requires them when a term has a namespaceSelector
   double now_ts = 0;                 // the clock candidateNodes reads (seconds)
   bool derive_candidates = false;    // candidate / disruption_cost of every node come from rank_candidates, not from the fields
   bool simulation_mode = false;

@@ -71,6 +71,11 @@ enum Counter : int {
   kCtrRoundCycles, kCtrRounds, kCtrRoundPods,
   kCtrStretchPinned, kCtrStretchFresh = kCtrStretchPinned + 16,  // round stretches by length 1..16
   kCtrMaskSteps = kCtrStretchFresh + 16, kCtrMaskMultiDomain, kCtrMaskRoundable,
+  // pinned rounds with equal counts whose bucket stretch stopped before a second round, by the first lane's reason: singleton
+  // bucket whose head accepts again, singleton bucket whose head is done, unpinned key, inexact room word, kM1Lv, staged end
+  kCtrBucketEnd,
+  kCtrFillLen = kCtrBucketEnd + 6,   // fill stretches by length 1..16 (rounds that keep every zone's head)
+  kCtrRoundsUnequal = kCtrFillLen + 16,  // single rounds whose counts are not all equal
   kNumCounters
 };
 constexpr uint64_t kNoBest = ~0ull;
@@ -1173,6 +1178,7 @@ static int run_pack(ksched_handle* h) {
   s.use_level_warp = std::getenv("KSCHED_NO_LEVELWARP") ? 0 : 1;
   s.use_varstore = std::getenv("KSCHED_NO_VARSTORE") ? 0 : 1;
   s.use_round_stretch = std::getenv("KSCHED_NO_ROUNDSTRETCH") ? 0 : 1;
+  s.use_fill_stretch = s.use_round_stretch && !std::getenv("KSCHED_NO_FILLSTRETCH") ? 1 : 0;
   s.vstore = h->d_vstore.ptr;
   // block size: the chain is latency-bound on ONE thread's commit; more warps only help when there are many candidate
   // nodes to examine per pod (existing nodes, large in-flight sets)
@@ -1294,6 +1300,13 @@ static void print_pack_profile(const long long* counters) {
     for (int r = 0; r < 16; ++r) fprintf(stderr, r ? ",%lld" : "%lld", c[k + r]);
     fprintf(stderr, "]");
   }
+  fprintf(stderr, "\n");
+  fprintf(stderr, "[pack profile] mask run rounds: bucket stretch below 2 rounds ended by [singleton bucket, head accepts again; "
+                  "singleton bucket, head done; unpinned key; inexact room; kM1Lv; staged end]=%lld,%lld,%lld,%lld,%lld,%lld | "
+                  "single rounds with unequal counts=%lld | fill stretch length (1..16):",
+          c[kCtrBucketEnd], c[kCtrBucketEnd + 1], c[kCtrBucketEnd + 2], c[kCtrBucketEnd + 3], c[kCtrBucketEnd + 4],
+          c[kCtrBucketEnd + 5], c[kCtrRoundsUnequal]);
+  for (int r = 0; r < 16; ++r) fprintf(stderr, r ? ",%lld" : " %lld", c[kCtrFillLen + r]);
   fprintf(stderr, "\n");
   fprintf(stderr, "[pack profile] class_run without mask-key spread: cycles=%lld pods=%lld level+fill iterations=%lld (fill %lld) fresh=%lld per-pod=%lld | with: cycles=%lld pods=%lld fresh=%lld per-pod=%lld\n",
           c[kCtrRunLvCycles], c[kCtrRunLvPods], c[kCtrRunLvSteps], c[kCtrRunLvFills], c[kCtrRunLvFresh], c[kCtrRunLvPerPod], c[kCtrRunCycles],

@@ -1764,6 +1764,39 @@ __device__ __forceinline__ void m1_fresh(const RunEnv& e, int buf, int vi, int a
   g_m1.fr[f] = (uint32_t)a | ((uint32_t)vi << 16);
 }
 
+// ---- fill stretch (DESIGN.md section 4): every domain of an all-equal round has a head that is alone in its bucket (pod
+// count c). The round sends it to the FRONT of block c + 1, where nothing of its list lies before it, so while it accepts,
+// stays below the unpinned head and does not pass the node behind it, the next rounds take the same node per domain. The
+// order inside a round is known: heads of lower count first, and keys of equal count break ties on the previous round's
+// ticks (later first), so inside a group of equal head count every round reverses the order of the one before. The pod of
+// round r on this lane's node is pod r * na + m1_fill_pos(r, fp) of the step, fp = its place in the even rounds | its place
+// in the odd rounds << 8.
+__device__ __forceinline__ int m1_fill_pos(int r, int fp) { return (r & 1) ? fp >> 8 : fp & 0xFF; }
+// warp-wide: this lane's bound on the rounds (32 outside the round) and its places fp
+__device__ __forceinline__ int m1_fill_len(const RunEnv& e, const M1Lane& l, bool act, unsigned okm, int na, int cap,
+                                           unsigned long long ukey, int ltick, int& fp) {
+  const int c = (int)(l.hk >> 32);
+  int rank0 = 0, lo = 0, gs = 0;  // the head's place in round 0; heads of the round with a lower / the same pod count
+  for (unsigned m = okm; m; m &= m - 1) {
+    const unsigned long long k2 = __shfl_sync(kFull, l.hk, __ffs(m) - 1);
+    rank0 += k2 < l.hk;
+    lo += (int)(k2 >> 32) < c;
+    gs += (int)(k2 >> 32) == c;
+  }
+  fp = rank0 | (2 * lo + gs - 1 - rank0) << 8;
+  if (!act) return 32;
+  const int c1 = l.n1 >= 0 ? (int)(l.nk >> 32) : 0x7fffffff;  // pod count of the node behind the head
+  if (c1 == c || (l.hr & 0xFFFF) == kRoomSlow || l.hk >= ukey) return 0;
+  int rd = run_fill_cap(e, l.h, (int)(l.hr & 0xFFFF));  // room and hostname limits
+  if (kM1Lv - 1 - c < rd) rd = kM1Lv - 1 - c;            // round r commits at count c + r + 1 < kM1Lv
+  if (c1 != 0x7fffffff && c1 - c + 1 < rd) rd = c1 - c + 1;  // at count c + r > c1 the node behind comes first
+  if (cap < rd) rd = cap;
+  if (ukey != ~0ull)  // round r's key: count c + r, tie-break from the tick of round r - 1
+    for (int r = 1; r < rd; ++r)
+      if (order_key(c + r, -(ltick + (r - 1) * na + m1_fill_pos(r - 1, fp) + 1)) >= ukey) rd = r;
+  return rd;
+}
+
 // ---- round / round stretch. Skew 1 with a self-matching selector: only the domains with the fewest pods admit a pod, so
 // once every one of them has a pinned node at hand and the unpinned nodes come later in the order, the next pods go one to
 // each of these domains, smallest head key first - a whole round is committed at once, every lane its own domain. Returns
@@ -1785,7 +1818,7 @@ __device__ __forceinline__ int m1_round(const RunEnv& e, int buf, M1Lane& l, M1W
   // one pod, so the counts stay equal and the round's shape repeats. R rounds are placed in one step while R single rounds
   // would take the same nodes (DESIGN.md section 4): pinned, the r-th members of each head's bucket; fresh, R fresh nodes
   // per domain that take no second pod.
-  int R = 0, vi_s = -1;
+  int R = 0, vi_s = -1, Rf = 0, fp = 0;  // Rf: rounds of a fill stretch, fp: its places (m1_fill_pos)
   const bool pinned = hv == okm;
   const int jd = __popc(okm & ((1u << L) - 1u));  // act: this domain's place among the round's domains
 #ifdef KSCHED_PROFILE_PACK
@@ -1812,6 +1845,25 @@ __device__ __forceinline__ int m1_round(const RunEnv& e, int buf, M1Lane& l, M1W
         }
       }
       R = __reduce_min_sync(kFull, act ? rd : 32);
+#ifdef KSCHED_PROFILE_PACK
+      if (R < 2) {  // why the bucket stretch stopped, on the first lane that stopped it
+        int why = 3;  // (a second member with an inexact room word)
+        if (act && rd < 2) {
+          const int c = (int)(l.hk >> 32);
+          if ((l.hr & 0xFFFF) == kRoomSlow) why = 3;
+          else if (c + 1 >= kM1Lv) why = 4;
+          else if (l.hk >= ukey) why = 2;
+          else if (l.n1 < 0 || (int)(l.nk >> 32) != c) why = run_fill_cap(e, l.h, (int)(l.hr & 0xFFFF)) >= 2 ? 0 : 1;
+          else if (l.nk >= ukey) why = 2;
+        }
+        why = __shfl_sync(kFull, why, __ffs(__ballot_sync(kFull, act && rd < 2)) - 1);
+        if (L == 0) s.counters[kCtrBucketEnd + why] += 1;
+      }
+      if (R < 2)
+#else
+      if (R < 2 && s.use_fill_stretch)
+#endif
+        Rf = __reduce_min_sync(kFull, m1_fill_len(e, l, act, okm, na, cap, ukey, w.ltick, fp));
     } else if (hv == 0 && ukey == ~0ull && (okm & ~rc.m_tallow[0]) == 0) {  // fresh nodes that never re-enter a list
       if (act) vi_s = run_ring_find(rc, 1, L, 0);
       const bool shut = vi_s >= 0 && ((rc.var[vi_s].rp & 0xFFFF) == 0 || (rc.var[vi_s].rp & kRpDead));
@@ -1824,12 +1876,33 @@ __device__ __forceinline__ int m1_round(const RunEnv& e, int buf, M1Lane& l, M1W
     }
 #ifdef KSCHED_PROFILE_PACK
     if (L == 0 && R > 0) s.counters[(pinned ? kCtrStretchPinned : kCtrStretchFresh) + (R > 16 ? 16 : R) - 1] += 1;
+    if (L == 0 && Rf > 0) s.counters[kCtrFillLen + (Rf > 16 ? 16 : Rf) - 1] += 1;
     if (!s.use_round_stretch) R = 0;
+    if (!s.use_fill_stretch) Rf = 0;
 #endif
+    if (Rf >= 2) R = Rf;
   }
+#ifdef KSCHED_PROFILE_PACK
+  else if (L == 0 && pinned && okm == e.m_reg0) s.counters[kCtrBucketEnd + 5] += 1;
+#endif
   if (R >= 2) {
     const int np = R * na;
-    if (pinned) {
+    if (Rf >= 2) {  // each domain's lane commits its head once for its R pods: no pop or insert per round
+      bool closed_l = false;
+      if (act) {
+        const int a = l.h, c = (int)(l.hk >> 32);
+        const uint32_t rp = l.hr;
+        l.pop_head(e, c);
+        for (int r = 0; r < R; ++r) rc.q_node[buf][w.li + r * na + m1_fill_pos(r, fp)] = -(a + 2);
+        const int tl = w.ltick + (R - 1) * na + m1_fill_pos(R - 1, fp);  // tick of its last pod
+        const uint32_t rp2 = run_record_host(rc, e.hc, e.n_host, a, rp, R);
+        closed_l = run_settle(e, a, rp2, c + R, -(tl + 1));
+        if ((rp2 & 0xFFFF) != 0 && !(rp2 & kRpDead)) l.insert_front(e, a, c + R, order_key(c + R, -(tl + 1)), rp2);
+        w.cnt_d += R;
+      }
+      const unsigned tb = __ballot_sync(kFull, closed_l);
+      if (L == 0 && tb) rc.tomb = rc.tomb + __popc(tb);
+    } else if (pinned) {
       const int c = (int)(l.hk >> 32);
       if (act) for (int r = 0; r < R; ++r) l.pop_head(e, c);  // (reads the keys of the bucket before they change)
       __syncwarp();
@@ -1911,6 +1984,9 @@ __device__ __forceinline__ int m1_round(const RunEnv& e, int buf, M1Lane& l, M1W
   if (nf && L < e.n_host && rc.h_times[L]) rc.h_inc[L] = rc.h_inc[L] + nf;
   const unsigned tb = __ballot_sync(kFull, closed_l);
   if (L == 0 && tb) rc.tomb = rc.tomb + __popc(tb);
+#ifdef KSCHED_PROFILE_PACK
+  if (L == 0 && okm != e.m_reg0) s.counters[kCtrRoundsUnequal] += 1;
+#endif
   w.lnew += nf;
   w.lact += nf;
   w.nfr += nf;

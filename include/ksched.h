@@ -114,8 +114,9 @@ typedef struct ksched_pod_row {
   uint64_t values[KSCHED_MAX_KEYS]; /* NewPodRequirements on the mask keys */
   uint64_t meta;
   uint64_t tolerated_taintsets; /* bit s: pod tolerates every taint of taint set s (s < 64; see problem.class_tolerated_ext) */
-  uint64_t hostport_conflicts;  /* host-port entries this pod's ports clash with (hostportusage.go:45-57) */
-  uint64_t hostport_entries;    /* host-port entries this pod reserves */
+  uint64_t hostport_conflicts;  /* host-port entries this pod's ports clash with (hostportusage.go:45-57); entries < 64 (see
+                                   problem.class_hostport_conflicts_ext) */
+  uint64_t hostport_entries;    /* host-port entries this pod reserves (entries < 64) */
   uint32_t res_present;         /* bit r: resource r is a key of the pod's request map */
   uint32_t relax_next;          /* class after one successful Relax, or KSCHED_NONE */
   uint32_t itype_req;           /* index into problem.itype_req_sets (instance-type key), or KSCHED_NONE */
@@ -188,7 +189,7 @@ typedef struct ksched_existing_node {
   uint32_t available_present, requests_present;
   uint32_t taintset;
   uint32_t itype;                     /* node's instance-type label as a type column, or KSCHED_NONE */
-  uint64_t hostport_entries;          /* entries already reserved by bound pods */
+  uint64_t hostport_entries;          /* entries already reserved by bound pods (entries < 64; see problem.existing_hostport_ext) */
   uint64_t label_keys_other;          /* reserved */
 } ksched_existing_node;
 
@@ -277,6 +278,15 @@ typedef struct ksched_problem {
   const int64_t* class_requests_ext;      /* [n_classes][n_res_ext] request (ceiling over init containers) */
   const uint32_t* class_res_ext_present;  /* [n_classes] bit x: ext resource x is a key of the class's request map */
   const int64_t* existing_available_ext;  /* [n_existing][n_res_ext] state.Node.Available() (0 where the node lacks it) */
+  /* Host-port entries beyond the 64 of ksched_pod_row.hostport_conflicts / hostport_entries and
+     ksched_existing_node.hostport_entries. Entry e >= 64 is bit (e - 64) % 64 of word (e - 64) / 64 of a row of these tables;
+     entries 0-63 stay in the row and node words. Relaxed classes are classes and have rows too. All three NULL and the count 0
+     when every entry is below 64; ksched_upload answers KSCHED_ERR_INVALID when the tables and the count disagree. */
+  const uint64_t* class_hostport_conflicts_ext; /* [n_classes][n_hostport_ext_words] */
+  const uint64_t* class_hostport_entries_ext;   /* [n_classes][n_hostport_ext_words] */
+  const uint64_t* existing_hostport_ext;        /* [n_existing][n_hostport_ext_words] (may be NULL when n_existing is 0) */
+  int32_t n_hostport_ext_words;
+  int32_t pad_hostport;
 } ksched_problem;
 
 typedef struct ksched_new_node {

@@ -126,6 +126,7 @@ def lib():
     L.kh_encoded_dims.argtypes = [C.c_void_p, C.POINTER(C.c_longlong)]
     L.kh_encoded_key_info.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(C.c_longlong)]
     L.kh_encoded_resource_id.argtypes = [C.c_void_p, C.c_char_p]
+    L.kh_encoded_hostport.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_int]
     L.kh_value_class_selftest.argtypes = [C.c_uint, C.c_int]
     L.kh_gpu_load.argtypes = [C.c_void_p]
     L.kh_encoded_set_count_visited.argtypes = [C.c_void_p, C.c_int]
@@ -573,10 +574,18 @@ class ResidentSolve:
         if not self.enc:
             msg = lib().kh_scheduler_error().decode()
             raise KschedError(KSCHED_ERR_UNSUPPORTED if msg.startswith("unsupported:") else KSCHED_ERR_INVALID, msg)
-        d = (C.c_longlong * 12)()
+        d = (C.c_longlong * 14)()
         lib().kh_encoded_dims(self.enc, d)
         self.dims = dict(zip(["pods", "classes", "existing", "groups", "types", "templates", "keys", "resources", "type_words", "class_topo",
-                              "taintsets", "resources_ext"], list(d)))
+                              "taintsets", "resources_ext", "hostports", "hostport_ext_words"], list(d)))
+
+    def hostports(self):
+        """the host-port entries of this encoding in id order, as (ip, port, protocol): the ones the encoder kept"""
+        out, buf = [], C.create_string_buffer(256)
+        while lib().kh_encoded_hostport(self.enc, len(out), buf, len(buf)) == 0:
+            ip, port, proto = buf.value.decode().split(" ")
+            out.append((ip, int(port), proto))
+        return out
 
     def key_info(self, key):
         """dictionary of one mask key: {values, representatives (of unnamed value classes, 0 = none), thresholds}, or None

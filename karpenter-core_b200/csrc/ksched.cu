@@ -190,6 +190,12 @@ struct ksched_handle {
   DevBuf<int32_t> d_cls_cursor;
   DevBuf<uint64_t> d_cls_tol_ext;  // [n_classes][tol_ext_words] taint sets from id 64 on (ksched_problem.class_tolerated_ext)
   int tol_ext_words = 0;
+  // host-port entries from id 64 on (ksched_problem.class_hostport_conflicts_ext); allocated only when the problem has some
+  DevBuf<uint64_t> d_cls_hpc_ext, d_cls_hpe_ext;  // [n_classes][hp_ext_words]
+  DevBuf<uint8_t> d_cls_hp_ext;                   // [n_classes] 1: the class has a conflict or an entry from id 64 on
+  DevBuf<uint64_t> d_ex_hp_ext, d_ex_hp_ext0;     // [hp_ext_words][n_existing] working copy / pristine copy
+  DevBuf<uint64_t> d_nn_hp_ext;                   // [hp_ext_words][max_new]
+  int hp_ext_words = 0;
   // ext resources (ksched.h: ksched_catalog.n_res_ext); allocated only when the catalog has some
   DevBuf<int64_t> d_alloc_ext, d_cls_req_ext, d_ex_avail_ext, d_ex_req_ext, d_nn_req_ext;
   DevBuf<uint32_t> d_cls_ext_present, d_nn_ext_present;
@@ -685,6 +691,16 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
       }
   }
   {
+    // host-port entries from id 64 on: the three tables exist exactly when the count is positive
+    const int hw = pb->n_hostport_ext_words;
+    const bool any = pb->class_hostport_conflicts_ext || pb->class_hostport_entries_ext || pb->existing_hostport_ext;
+    if (hw < 0 || (hw > 0 ? !(pb->class_hostport_conflicts_ext && pb->class_hostport_entries_ext && (pb->existing_hostport_ext || pb->n_existing == 0))
+                          : any)) {
+      h->err = "host-port entry tables must be set exactly when n_hostport_ext_words is positive";
+      return KSCHED_ERR_INVALID;
+    }
+  }
+  {
     // ext resources: the tables exist exactly when the catalog has ext resources, and name no resource beyond them
     const int X = h->cat.n_res_ext;
     const bool any = pb->class_requests_ext || pb->class_res_ext_present || pb->existing_available_ext;
@@ -803,6 +819,24 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
     CUDA_TRY(h, upload_vec(h, h->d_ex_vals0, vals));
     CUDA_TRY(h, upload_vec(h, h->d_ex_meta0, meta));
     CUDA_TRY(h, upload_vec(h, h->d_ex_hp0, hp));
+    // host-port entries from id 64 on: per-class tables as given, the existing nodes' words as [word][node] like ex_hp
+    const int HW = pb->n_hostport_ext_words;
+    h->hp_ext_words = HW;
+    std::vector<uint64_t> hp_ext(HW > 0 ? (size_t)HW * std::max(NE, 1) : 0, 0);
+    std::vector<uint8_t> cls_hp(HW > 0 ? (size_t)std::max(NC, 1) : 0, 0);
+    if (HW > 0) {
+      for (int e = 0; e < NE; ++e)
+        for (int w = 0; w < HW; ++w) hp_ext[(size_t)w * NE + e] = pb->existing_hostport_ext[(size_t)e * HW + w];
+      for (int c2 = 0; c2 < NC; ++c2)
+        for (int w = 0; w < HW; ++w)
+          if (pb->class_hostport_conflicts_ext[(size_t)c2 * HW + w] | pb->class_hostport_entries_ext[(size_t)c2 * HW + w]) cls_hp[c2] = 1;
+      CUDA_TRY(h, upload(h, h->d_cls_hpc_ext, pb->class_hostport_conflicts_ext, (size_t)NC * HW));
+      CUDA_TRY(h, upload(h, h->d_cls_hpe_ext, pb->class_hostport_entries_ext, (size_t)NC * HW));
+      CUDA_TRY(h, upload_vec(h, h->d_cls_hp_ext, cls_hp));
+      CUDA_TRY(h, upload_vec(h, h->d_ex_hp_ext0, hp_ext));
+      CUDA_TRY(h, h->d_ex_hp_ext.ensure(hp_ext.size()));
+      CUDA_TRY(h, h->d_nn_hp_ext.ensure((size_t)HW * MAXN));
+    }
     h->have_volumes = pb->class_volumes != nullptr && pb->existing_volumes != nullptr && NE > 0;
     if (h->have_volumes) {
       CUDA_TRY(h, upload(h, h->d_cls_vol, pb->class_volumes, (size_t)NC));
@@ -1085,6 +1119,7 @@ static int reset_state(ksched_handle* h, const int64_t* d_remaining_src = nullpt
   add(h->d_ex_vals.ptr, h->d_ex_vals0.ptr, (size_t)16 * NE * 8);
   add(h->d_ex_meta.ptr, h->d_ex_meta0.ptr, (size_t)NE * 8);
   add(h->d_ex_hp.ptr, h->d_ex_hp0.ptr, (size_t)NE * 8);
+  if (h->hp_ext_words) add(h->d_ex_hp_ext.ptr, h->d_ex_hp_ext0.ptr, (size_t)h->hp_ext_words * NE * 8);  // new nodes: set at creation
   add(h->d_ex_closed.ptr, nullptr, (size_t)NE);
   add(h->d_cls_cursor.ptr, nullptr, (size_t)std::max(h->n_classes, 1) * 4);
   if (h->have_volumes) add(h->d_ex_vol.ptr, h->d_ex_vol0.ptr, (size_t)h->n_existing * sizeof(ksched_node_volumes));
@@ -1142,6 +1177,10 @@ static int run_pack(ksched_handle* h) {
   s.ex_hp = h->d_ex_hp.ptr; s.ex_closed = h->d_ex_closed.ptr;
   s.cls_cursor = h->d_cls_cursor.ptr;
   s.cls_tol_ext = h->tol_ext_words > 0 ? h->d_cls_tol_ext.ptr : nullptr; s.tol_ext_words = h->tol_ext_words;
+  const bool hpx = h->hp_ext_words > 0;
+  s.cls_hpc_ext = hpx ? h->d_cls_hpc_ext.ptr : nullptr; s.cls_hpe_ext = hpx ? h->d_cls_hpe_ext.ptr : nullptr;
+  s.cls_hp_ext = hpx ? h->d_cls_hp_ext.ptr : nullptr; s.ex_hp_ext = hpx ? h->d_ex_hp_ext.ptr : nullptr;
+  s.nn_hp_ext = hpx ? h->d_nn_hp_ext.ptr : nullptr; s.hp_ext_words = h->hp_ext_words;
   const bool ext = h->cat.n_res_ext > 0;
   s.cls_req_ext = ext ? h->d_cls_req_ext.ptr : nullptr; s.cls_ext_present = ext ? h->d_cls_ext_present.ptr : nullptr;
   s.ex_avail_ext = ext ? h->d_ex_avail_ext.ptr : nullptr; s.ex_req_ext = ext ? h->d_ex_req_ext.ptr : nullptr;

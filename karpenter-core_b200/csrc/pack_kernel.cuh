@@ -435,6 +435,40 @@ __device__ __forceinline__ bool tolerates_node_set(const PackState& s, uint64_t 
   const uint64_t w = ts < 64 ? tol : s.cls_tol_ext[(size_t)cls * s.tol_ext_words + ((ts - 64) >> 6)];
   return (w >> (ts & 63)) & 1;
 }
+// Host ports (HostPortUsage, hostportusage.go:65-93). Entries 0-63 are bits of the row's and the nodes' words; entries from
+// 64 on are words of the per-class tables and of the nodes' [word][node] arrays (ksched.h: class_hostport_conflicts_ext).
+// A class whose entries all have ids from 64 on has zero row words, so every gate that means "no host port" asks
+// has_host_ports: such a class takes the generic step, the only one that checks and commits entries.
+__device__ __forceinline__ bool class_hp_ext(const PackState& s, unsigned cls) { return s.cls_hp_ext && s.cls_hp_ext[cls]; }
+__device__ __forceinline__ bool has_host_ports(const PackState& s, const PodRegs& p) {
+  return (p.hpc | p.hpe) != 0 || class_hp_ext(s, (unsigned)p.cls64);
+}
+// HostPortUsage.validate: node idx of `words` / `ext` (`stride` nodes per ext word) holds an entry the class conflicts with.
+// hpx: class_hp_ext of the class.
+__device__ __forceinline__ bool node_hp_conflict(const PackState& s, uint64_t hpc, bool hpx, unsigned cls, const uint64_t* words,
+                                                 const uint64_t* ext, int stride, int idx) {
+  if (hpc && (words[idx] & hpc)) return true;
+  if (!hpx) return false;
+  const uint64_t* cw = s.cls_hpc_ext + (size_t)cls * s.hp_ext_words;
+  for (int w = 0; w < s.hp_ext_words; ++w)
+    if (cw[w] & ext[(size_t)w * stride + idx]) return true;
+  return false;
+}
+// HostPortUsage.Add: the class's entries join those node idx holds
+__device__ __forceinline__ void node_hp_commit(const PackState& s, uint64_t hpe, bool hpx, unsigned cls, uint64_t* words, uint64_t* ext,
+                                               int stride, int idx) {
+  if (hpe) words[idx] |= hpe;
+  if (!hpx) return;
+  const uint64_t* ce = s.cls_hpe_ext + (size_t)cls * s.hp_ext_words;
+  for (int w = 0; w < s.hp_ext_words; ++w) ext[(size_t)w * stride + idx] |= ce[w];
+}
+// A new node holds its first pod's entries and nothing else. Every site that opens a node writes all its words (the class
+// runs' nodes with hpe = 0, hpx = false), so a later host-port pod's in-flight scan never reads a word of an earlier Solve.
+__device__ __forceinline__ void fresh_node_hp(const PackState& s, uint64_t hpe, bool hpx, unsigned cls, int n) {
+  s.nn_hp[n] = hpe;
+  for (int w = 0; w < s.hp_ext_words; ++w)
+    s.nn_hp_ext[(size_t)w * s.max_new + n] = hpx ? s.cls_hpe_ext[(size_t)cls * s.hp_ext_words + w] : 0;
+}
 struct ExRunIO { int qi, head, qlen, seq, parity, placed; long long add_calls; };
 __shared__ ExRunIO g_xio;
 // one partial sum per warp, double-buffered: every warp of the largest block the kernel is launched with needs a slot
@@ -599,7 +633,8 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
     const uint32_t p_ext = kExt ? class_ext(s, cls) : 0u;
     const int X = c.n_res_ext;
     const bool plain = p_keys == 0 && !pt_nonempty && p_itype == KSCHED_NONE && p_hostname == KSCHED_NONE && !p_ext;  // no requirement can change
-    const bool simple = !has_topo && p_hpc == 0 && p_hpe == 0 && !p_ext;  // the requirement verdict memo (HotSmem::absorbed/rejected) applies
+    const bool p_hpx = class_hp_ext(s, cls);  // host-port entries from id 64 on
+    const bool simple = !has_topo && p_hpc == 0 && p_hpe == 0 && !p_hpx && !p_ext;  // the requirement verdict memo (HotSmem::absorbed/rejected) applies
 
     bool placed = false;
     ksched_class_volumes p_vol{};
@@ -621,7 +656,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
       for (int e = start + tid; e < NE; e += blockDim.x) {
         if (s.ex_closed[e]) continue;
         if (!tolerates_node_set(s, p_tol, cls, s.ex_taintset[e])) continue;
-        if (p_hpc && (s.ex_hp[e] & p_hpc)) continue;
+        if (node_hp_conflict(s, p_hpc, p_hpx, cls, s.ex_hp, s.ex_hp_ext, NE, e)) continue;
         if (has_vol) {  // volumeUsage.Validate(pod).Exceeds(volumeLimits) existingnode.go:88-96
           const ksched_node_volumes nv = s.ex_vol[e];
           const uint64_t all = nv.mounted | p_vol.shared;
@@ -683,7 +718,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
           }
           s.ex_req_present[e] |= p_res;
           for (uint32_t m = p_ext; m; m &= m - 1) { const int x = __ffs(m) - 1; s.ex_req_ext[(size_t)x * NE + e] += s.cls_req_ext[(size_t)cls * X + x]; }
-          if (p_hpe) s.ex_hp[e] |= p_hpe;
+          node_hp_commit(s, p_hpe, p_hpx, cls, s.ex_hp, s.ex_hp_ext, NE, e);
           if (has_vol) {  // volumeUsage.Add existingnode.go:128
             ksched_node_volumes nv = s.ex_vol[e];
             nv.mounted |= p_vol.shared;
@@ -736,7 +771,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
           for (int r = 0; r < kHotRes; ++r) { q[r] = H.q(r, a) + preq[r]; b1[r] = H.bound(r, a); b2[r] = H.bound2(r, a); }
           const int qf = quick_fit(q, qp, RH, b1, b2, fl);
           if (qf == 0) continue;
-          if (p_hpc && (s.nn_hp[H.node(a)] & p_hpc)) continue;
+          if ((p_hpc || p_hpx) && node_hp_conflict(s, p_hpc, p_hpx, cls, s.nn_hp, s.nn_hp_ext, MAXN, H.node(a))) continue;
           if (simple && H.rejected(a) == cls) continue;  // memo: same class, node untouched since it was refused
           const bool fast = (plain || (simple && H.absorbed(a) == cls)) && qf == 1;  // nothing can change and an option holds the requests
           if (!fast) {
@@ -864,7 +899,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
             if ((p_res >> r) & 1) s.nn_req[(size_t)r * MAXN + n] += row.requests[r];
           if ((p_res >> kHotRes) || ((p_res & 0xF) & ~((fl >> 1) & 0xF))) s.nn_req_present[n] |= p_res;
           fl |= (unsigned short)((p_res & 0xF) << 1);
-          if (p_hpe) s.nn_hp[n] |= p_hpe;
+          node_hp_commit(s, p_hpe, p_hpx, cls, s.nn_hp, s.nn_hp_ext, MAXN, n);
           const int count = (int)(wkey >> 32) + 1;
           s.nn_count[n] = count;
           s.nn_tb[n] = -(tick + 1);  // front of the next pod-count block under a stable sort
@@ -1100,7 +1135,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
             for (int x = 0; x < X; ++x) s.nn_req_ext[(size_t)n * X + x] = ((p_ext >> x) & 1) ? s.cls_req_ext[(size_t)cls * X + x] : 0;
             s.nn_ext_present[n] = p_ext;
           }
-          s.nn_hp[n] = p_hpe;
+          fresh_node_hp(s, p_hpe, p_hpx, cls, n);
           s.nn_count[n] = 1;
           s.nn_tb[n] = tick + 1;  // appended: last of the one-pod block
           const bool closed = node_closed(sh.q, s.min_req, RH, sh.bound, sh.bound2, sh.front_bits);
@@ -2250,7 +2285,7 @@ __device__ __forceinline__ void m1_store_fresh(const RunEnv& e) {
       s.nn_meta[n] = v.meta;
       s.nn_tmpl[n] = (uint8_t)(v.fl >> 8);
       s.nn_req_present[n] = v.qp;
-      s.nn_hp[n] = 0;
+      fresh_node_hp(s, 0, false, 0, n);
       if (((e.rpv[a] >> 16) & 0x7FFF) == 0) {  // no further pod so far: (1, creation tick); otherwise the run's write-back stores them
         s.nn_count[n] = 1;
         s.nn_tb[n] = (int)((unsigned)e.hs->key[a] ^ 0x80000000u);
@@ -2560,7 +2595,7 @@ __device__ __forceinline__ bool run_fresh_step(const RunEnv& e, int buf, int i, 
     s.nn_meta[n] = v.meta;
     s.nn_tmpl[n] = (uint8_t)(v.fl >> 8);
     s.nn_req_present[n] = v.qp;
-    s.nn_hp[n] = 0;
+    fresh_node_hp(s, 0, false, 0, n);
     s.nn_count[n] = 1;
     s.nn_tb[n] = tk + 1;
     if (n_mask > 0) e.zv[a] = (1u << fd0) | (3u << 16);
@@ -3060,7 +3095,8 @@ __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
     bool skip_run = true;
     if (fast_allowed && s.use_class_run && qi < s.n_pods && n_active <= kActCap) {
       const bool topo_cls = nxt.topo_begin != nxt.topo_end;
-      const bool shape_ok = nxt.hpc == 0 && nxt.hpe == 0 && (nxt.res >> kHotRes) == 0 && !(kExt && class_ext(s, (unsigned)nxt.cls64)) &&
+      // (host-port classes never get here, so the variant store's signature, which reads the row words only, never meets one)
+      const bool shape_ok = !has_host_ports(s, nxt) && (nxt.res >> kHotRes) == 0 && !(kExt && class_ext(s, (unsigned)nxt.cls64)) &&
                             (!topo_cls || (((nxt.meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF) == 0 && nxt.itype == KSCHED_NONE && nxt.hostname == KSCHED_NONE));
       if (shape_ok && (unsigned)nxt.cls64 != run_block_cls) {
         if (fresh_valid && fresh_cls == (unsigned)nxt.cls64) skip_run = false;  // a fresh node of this class to capture
@@ -3113,7 +3149,7 @@ __global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
     // ---- existing-node run (see existing_run): identical plain pods take the existing nodes in one prefix-sum pass
     if (NE > 0 && !s.count_visited && qi < s.n_pods && (unsigned)nxt.cls64 != xrun_block_cls &&
         ((nxt.meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF) == 0 && nxt.topo_begin == nxt.topo_end && nxt.itype == KSCHED_NONE &&
-        nxt.hostname == KSCHED_NONE && nxt.hpc == 0 && nxt.hpe == 0 && (nxt.res >> kHotRes) == 0 && !class_has_volumes(s, (unsigned)nxt.cls64) &&
+        nxt.hostname == KSCHED_NONE && !has_host_ports(s, nxt) && (nxt.res >> kHotRes) == 0 && !class_has_volumes(s, (unsigned)nxt.cls64) &&
         !(kExt && class_ext(s, (unsigned)nxt.cls64))) {
       __syncthreads();
       if (tid == 0) { ExRunIO& io = g_xio; io.qi = qi; io.head = head; io.qlen = qlen; io.seq = seq; io.parity = parity; io.add_calls = add_calls; io.placed = 0; }

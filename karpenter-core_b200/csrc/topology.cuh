@@ -136,6 +136,13 @@ struct PackState {
   int64_t* ex_req_ext;               // [n_res_ext][n_existing] what the batch's pods placed there request
   int64_t* nn_req_ext;               // [max_new][n_res_ext]
   uint32_t* nn_ext_present;          // [max_new]
+  // host-port entries from id 64 on (ksched.h: class_hostport_conflicts_ext), all nullptr without them
+  const uint64_t* cls_hpc_ext;       // [n_classes][hp_ext_words] conflicts
+  const uint64_t* cls_hpe_ext;       // [n_classes][hp_ext_words] entries
+  const uint8_t* cls_hp_ext;         // [n_classes] 1: the class has a word of either table that is not 0
+  uint64_t* ex_hp_ext;               // [hp_ext_words][n_existing]
+  uint64_t* nn_hp_ext;               // [hp_ext_words][max_new]
+  int hp_ext_words;
 };
 
 struct K2Params {

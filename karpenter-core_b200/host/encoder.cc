@@ -463,8 +463,9 @@ struct Builder {
   std::vector<KeyMeta> key_meta;
   std::map<std::string, int> taintset_id;
   std::vector<std::vector<Taint>> taintsets;
-  std::vector<HostPortEntry> hp_entries;
-  std::map<std::string, int> type_col;                     // instance type name -> column
+  std::vector<HostPortEntry> hp_entries;                   // host-port entries in id order (host_port_table)
+  std::map<HostPortEntry, int> hp_id;                      // every entry of the problem -> id, -1 = left out
+  std::map<std::string, int> type_col;                    // instance type name -> column
   bool res_pruned = false;                                 // resource names no request reads were left out of res_id
   std::vector<Daemon> daemons;
   std::map<std::string, int> hostname_slot;                // hostname -> existing slot
@@ -538,12 +539,16 @@ struct Builder {
     taintsets.push_back(ts);
     return id;
   }
-  int hp_entry(const HostPortEntry& e) {
-    for (size_t i = 0; i < hp_entries.size(); ++i)
-      if (hp_entries[i].ip == e.ip && hp_entries[i].port == e.port && hp_entries[i].protocol == e.protocol) return (int)i;
-    if (hp_entries.size() >= 64) unsupported("more than 64 distinct host-port entries");
-    hp_entries.push_back(e);
-    return (int)hp_entries.size() - 1;
+  int hp_entry(const HostPortEntry& e) const {  // id of an entry (host_port_table), -1 when it was left out
+    auto it = hp_id.find(e);
+    if (it == hp_id.end()) throw std::runtime_error("internal: host-port entry missing from the table");
+    return it->second;
+  }
+  // entry `id`'s bit: of `word` below 64, of ext[(id - 64) / 64] (a table row of E.hostport_ext_words words) from 64 on
+  static void hp_bit(int id, uint64_t& word, uint64_t* ext) {
+    if (id < 0) return;  // left out: the entry can turn no pod away
+    if (id < 64) word |= 1ull << id;
+    else ext[(id - 64) / 64] |= 1ull << ((id - 64) % 64);
   }
   int resource(const std::string& name) const {
     auto it = res_id.find(name);
@@ -1288,6 +1293,69 @@ void daemonset_overhead(Builder& B) {
 }
 
 // ------------------------------------------------------------------ existing nodes (scheduler.go:221-248, existingnode.go:41-75)
+// ------------------------------------------------------------------ host-port entries (hostportusage.go)
+// Ids in order of first appearance: the bound pods of the owned state nodes that stay, then the pod classes. With more than
+// 64 entries, the ones that can never turn a pod away are left out (no id, no bit). HostPortUsage.validate
+// (hostportusage.go:80-93) refuses pod p on a node only for an entry e that a DIFFERENT pod q on that node holds and a port
+// of p matches. So e is kept iff some pod of the problem holds it (bound to a node that stays, or a pod of the batch, which
+// can be committed) and another pod of the batch has a port matching it. Two pods of one class are different pods; a pod
+// whose containers repeat a port is one. Matching is not transitive, so each entry is tested against ports.
+// Problems with at most 64 entries keep their ids and encode as before.
+void host_port_table(Builder& B) {
+  const Problem& P = B.P;
+  Encoded& E = B.E;
+  std::vector<HostPortEntry> seen;  // every entry, first appearance order
+  std::map<HostPortEntry, int> index;
+  auto note = [&](const HostPortEntry& e) { if (index.emplace(e, (int)seen.size()).second) seen.push_back(e); };
+  std::vector<int> owned;  // state nodes that become existing nodes (existing_nodes)
+  for (int si : B.state_nodes) {
+    auto own = P.nodes[si].labels.find(kProvisionerName);
+    if (own == P.nodes[si].labels.end() || own->second.empty()) continue;
+    owned.push_back(si);
+    for (auto& hp : B.facts.node[(size_t)si].hostports) note(hp);
+  }
+  const size_t NC = B.specs.size();
+  std::vector<std::vector<HostPortEntry>> ports(NC);
+  for (size_t c = 0; c < NC; ++c) {
+    ports[c] = host_ports(B.specs[c].pod);
+    for (auto& hp : ports[c]) note(hp);
+  }
+  std::vector<uint8_t> keep(seen.size(), 1);
+  if (seen.size() > 64) {
+    struct Pods {  // distinct pods seen, counted up to two, and the first one
+      int n = 0;
+      const Pod* first = nullptr;
+      void add(const Pod* p) { if (n == 0) { n = 1; first = p; } else if (n == 1 && p != first) n = 2; }
+    };
+    std::vector<Pods> holders(seen.size()), matchers(seen.size());
+    for (int si : owned)
+      for (auto& p : P.nodes[si].pods)
+        for (auto& hp : host_ports(p)) holders[(size_t)index.at(hp)].add(&p);
+    std::vector<std::vector<int>> matched(NC);  // entries some port of the class matches
+    for (size_t c = 0; c < NC; ++c)
+      for (size_t u = 0; u < seen.size() && !ports[c].empty(); ++u)
+        for (auto& hp : ports[c])
+          if (hp_matches(hp, seen[u])) { matched[c].push_back((int)u); break; }
+    for (size_t i = 0; i < E.pods.size(); ++i) {
+      const uint32_t c = E.pod_class[i];
+      for (auto& hp : ports[c]) holders[(size_t)index.at(hp)].add(E.pods[i]);
+      for (int u : matched[c]) matchers[(size_t)u].add(E.pods[i]);
+    }
+    for (size_t u = 0; u < seen.size(); ++u) {
+      const Pods &h = holders[u], &m = matchers[u];
+      keep[u] = h.n > 0 && m.n > 0 && !(h.n == 1 && m.n == 1 && h.first == m.first);
+    }
+  }
+  for (size_t u = 0; u < seen.size(); ++u) {
+    B.hp_id[seen[u]] = keep[u] ? (int)B.hp_entries.size() : -1;
+    if (!keep[u]) continue;
+    B.hp_entries.push_back(seen[u]);
+    E.hostports.push_back(seen[u].ip + " " + std::to_string(seen[u].port) + " " + seen[u].protocol);
+  }
+  const size_t n = B.hp_entries.size();
+  E.hostport_ext_words = n > 64 ? (int)((n - 64 + 63) / 64) : 0;
+}
+
 void existing_nodes(Builder& B) {
   const Problem& P = B.P;
   Encoded& E = B.E;
@@ -1317,7 +1385,12 @@ void existing_nodes(Builder& B) {
     e.itype = KSCHED_NONE;
     auto itl = n.labels.find(kInstanceType);
     if (itl != n.labels.end()) { auto c = B.type_col.find(itl->second); if (c != B.type_col.end()) e.itype = (uint32_t)c->second; }
-    for (auto& hp : nf.hostports) e.hostport_entries |= 1ull << B.hp_entry(hp);
+    if (const int W = E.hostport_ext_words) {
+      E.existing_hostport_ext.resize(E.existing_hostport_ext.size() + W, 0);
+      for (auto& hp : nf.hostports) B.hp_bit(B.hp_entry(hp), e.hostport_entries, &E.existing_hostport_ext[E.existing_hostport_ext.size() - W]);
+    } else {
+      for (auto& hp : nf.hostports) B.hp_bit(B.hp_entry(hp), e.hostport_entries, nullptr);
+    }
     std::string hostname;
     auto h = n.labels.find(kHostname);
     if (h != n.labels.end()) hostname = h->second;
@@ -1677,6 +1750,9 @@ void class_rows(Builder& B, const std::vector<Group>& groups) {
   E.class_tolerated_ext.assign((size_t)NC * E.tolerated_ext_words, 0);
   E.class_requests_ext.assign((size_t)NC * E.n_res_ext, 0);
   E.class_res_ext_present.assign(E.n_res_ext ? NC : 0, 0);
+  const int HW = E.hostport_ext_words;
+  E.class_hostport_conflicts_ext.assign((size_t)NC * HW, 0);
+  E.class_hostport_entries_ext.assign((size_t)NC * HW, 0);
   for (int c = 0; c < NC; ++c) {
     const Spec& s = B.specs[c];
     ksched_pod_row& row = E.classes[c];
@@ -1719,7 +1795,11 @@ void class_rows(Builder& B, const std::vector<Group>& groups) {
       E.hostname_reqs.push_back(comp);
       E.hostname_reqs.push_back(slot);
     }
-    for (auto& hp : host_ports(s.pod)) row.hostport_entries |= 1ull << B.hp_entry(hp);
+    for (auto& hp : host_ports(s.pod)) {  // the entry table is complete: host_port_table ran before the existing nodes
+      B.hp_bit(B.hp_entry(hp), row.hostport_entries, HW ? &E.class_hostport_entries_ext[(size_t)c * HW] : nullptr);
+      for (size_t e = 0; e < B.hp_entries.size(); ++e)
+        if (hp_matches(hp, B.hp_entries[e])) B.hp_bit((int)e, row.hostport_conflicts, HW ? &E.class_hostport_conflicts_ext[(size_t)c * HW] : nullptr);
+    }
     for (size_t t = 0; t < NS; ++t) {  // the taint-set table is complete: templates and existing nodes are encoded
       if (!tolerates_all(B.taintsets[t], s.pod.tolerations)) continue;
       if (t < 64) row.tolerated_taintsets |= 1ull << t;
@@ -1740,11 +1820,6 @@ void class_rows(Builder& B, const std::vector<Group>& groups) {
     if (!any) E.class_volumes.clear();  // no pod of the batch mounts a limited claim: the kernels never look
     for (auto& kv : B.vol_tracked) E.volume_driver_mask[B.driver_index(kv.first.first)] |= 1ull << kv.second;
   }
-  // host-port conflict masks need the complete entry table
-  for (int c = 0; c < NC; ++c)
-    for (auto& hp : host_ports(B.specs[c].pod))
-      for (size_t e = 0; e < B.hp_entries.size(); ++e)
-        if (hp_matches(hp, B.hp_entries[e])) E.classes[c].hostport_conflicts |= 1ull << e;
 }
 
 // ------------------------------------------------------------------ per-pod queue keys (queue.go:74-110)
@@ -1803,6 +1878,12 @@ void wire(Builder& B) {
   }
   pr.class_tolerated_ext = E.class_tolerated_ext.empty() ? nullptr : E.class_tolerated_ext.data();
   pr.n_tolerated_ext_words = E.tolerated_ext_words;
+  if (E.hostport_ext_words) {
+    pr.class_hostport_conflicts_ext = E.class_hostport_conflicts_ext.data();
+    pr.class_hostport_entries_ext = E.class_hostport_entries_ext.data();
+    pr.existing_hostport_ext = NE > 0 ? E.existing_hostport_ext.data() : nullptr;
+    pr.n_hostport_ext_words = E.hostport_ext_words;
+  }
   if (E.n_res_ext) {
     pr.class_requests_ext = E.class_requests_ext.data();
     pr.class_res_ext_present = E.class_res_ext_present.data();
@@ -1843,6 +1924,8 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
   B.phase("templates");
   daemonset_overhead(B);
   B.phase("daemonset overhead");
+  host_port_table(B);
+  B.phase("host-port entries");
   existing_nodes(B);
   B.phase("existing nodes");
   const std::vector<Group> groups = topology_groups(B);

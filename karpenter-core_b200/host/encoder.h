@@ -97,6 +97,11 @@ struct Encoded {
   std::vector<int64_t> class_requests_ext;            // [n_classes][n_res_ext]
   std::vector<uint32_t> class_res_ext_present;        // [n_classes]
   std::vector<int64_t> existing_available_ext;        // [n_existing][n_res_ext]
+  std::vector<std::string> hostports;                 // host-port entries in id order, "ip port protocol" (DESIGN.md §3)
+  int hostport_ext_words = 0;                         // entries from id 64 on (ksched.h); 0 with at most 64 entries kept
+  std::vector<uint64_t> class_hostport_conflicts_ext; // [n_classes][hostport_ext_words]; empty without such entries
+  std::vector<uint64_t> class_hostport_entries_ext;   // [n_classes][hostport_ext_words]
+  std::vector<uint64_t> existing_hostport_ext;        // [n_existing][hostport_ext_words]
 
   ksched_catalog catalog{};
   ksched_problem problem{};

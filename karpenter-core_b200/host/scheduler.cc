@@ -359,12 +359,21 @@ void kh_encoded_free(Encoded* E) {
   if (E == g_gpu_encoded) { g_gpu_encoded = nullptr; g_gpu_current = false; }
   delete E;
 }
-// dims: [pods, classes, existing, groups, types, templates, keys, resources, type_words, class_topo, taintsets, resources_ext]
+// dims: [pods, classes, existing, groups, types, templates, keys, resources, type_words, class_topo, taintsets, resources_ext,
+//        hostports, hostport_ext_words]
 void kh_encoded_dims(const Encoded* E, long long* out) {
   out[0] = (long long)E->pods.size(); out[1] = (long long)E->classes.size(); out[2] = (long long)E->existing.size();
   out[3] = (long long)E->groups.size(); out[4] = (long long)E->types.size(); out[5] = (long long)E->templates.size();
   out[6] = (long long)E->key_names.size(); out[7] = (long long)E->res_names.size() - E->n_res_ext; out[8] = E->type_words;
   out[9] = (long long)E->class_topo.size(); out[10] = E->n_taintsets; out[11] = E->n_res_ext;
+  out[12] = (long long)E->hostports.size(); out[13] = E->hostport_ext_words;
+}
+// Host-port entry `id` of an encoding as "ip port protocol" into out[cap] (tests): the entries the encoder kept, in id order.
+// Returns -1 when there is no such entry or it does not fit.
+int kh_encoded_hostport(const Encoded* E, int id, char* out, int cap) {
+  if (id < 0 || (size_t)id >= E->hostports.size() || (int)E->hostports[(size_t)id].size() >= cap) return -1;
+  std::memcpy(out, E->hostports[(size_t)id].c_str(), E->hostports[(size_t)id].size() + 1);
+  return 0;
 }
 void kh_encoded_set_count_visited(Encoded* E, int on) { E->problem.count_nodes_visited = on; }
 const ksched_catalog* kh_encoded_catalog(const Encoded* E) { return &E->catalog; }
@@ -1308,6 +1317,9 @@ extern "C" unsigned long long kh_encoded_digest(const Encoded* E) {
   vec(E->group_existing_counts); vec(E->class_topo); vec(E->filter_terms); vec(E->itype_req_sets); vec(E->itype_req_complement); vec(E->hostname_reqs);
   if (!E->class_volumes.empty()) { vec(E->class_volumes); vec(E->existing_volumes); bytes(E->volume_driver_mask, sizeof E->volume_driver_mask); }
   if (!E->class_tolerated_ext.empty()) vec(E->class_tolerated_ext);  // absent with at most 64 taint sets: those digests predate it
+  if (E->hostport_ext_words) {  // absent with at most 64 host-port entries: those digests predate the entry tables
+    vec(E->class_hostport_conflicts_ext); vec(E->class_hostport_entries_ext); vec(E->existing_hostport_ext);
+  }
   if (E->n_res_ext) {  // absent with at most 8 read resources: those digests predate ext resources
     bytes(&E->n_res_ext, sizeof E->n_res_ext);
     vec(E->type_alloc_ext); vec(E->class_requests_ext); vec(E->class_res_ext_present); vec(E->existing_available_ext);

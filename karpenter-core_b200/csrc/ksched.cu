@@ -48,6 +48,7 @@ namespace {
 constexpr int kMaxCG = 8;        // topology groups that may constrain one pod class
 constexpr int kMaxTouched = 8;   // requirement keys one Add may touch (pod keys + topology keys)
 constexpr int kPackThreads = 512;
+constexpr int kPackThreadsSmall = 256;  // blocks up to this size launch the pack_kernel instantiation with twice the registers
 constexpr int kFreshMemoSlots = 8192;  // PackState::fd_*
 // PackState::counters: the results of a Solve, then the KSCHED_PROFILE_PACK profile (print_pack_profile)
 enum Counter : int {
@@ -76,6 +77,9 @@ enum Counter : int {
   kCtrBucketEnd,
   kCtrFillLen = kCtrBucketEnd + 6,   // fill stretches by length 1..16 (rounds that keep every zone's head)
   kCtrRoundsUnequal = kCtrFillLen + 16,  // single rounds whose counts are not all equal
+  // class_run's fixed cost per call: open nodes at entry (summed), cycles from entry to the first loop iteration of the
+  // eligible calls (of which the per-node inputs), write-back cycles, and the compactions with the slots they scanned and their cycles
+  kCtrRunActiveSum, kCtrRunEntryCycles, kCtrRunInputCycles, kCtrRunWbCycles, kCtrRunCompacts, kCtrRunCompactSlots, kCtrRunCompactCycles,
   kNumCounters
 };
 constexpr uint64_t kNoBest = ~0ull;
@@ -326,8 +330,10 @@ int ksched_create(int device_ordinal, ksched_handle** out) {
   {
     // CUDA loads kernels lazily on first launch: pull ours in here, not inside the first Solve
     cudaFuncAttributes fa;
-    cudaFuncGetAttributes(&fa, pack_kernel<false>);
-    cudaFuncGetAttributes(&fa, pack_kernel<true>);
+    cudaFuncGetAttributes(&fa, pack_kernel<false, kPackThreadsSmall>);
+    cudaFuncGetAttributes(&fa, pack_kernel<true, kPackThreadsSmall>);
+    cudaFuncGetAttributes(&fa, pack_kernel<false, kPackThreads>);
+    cudaFuncGetAttributes(&fa, pack_kernel<true, kPackThreads>);
     cudaFuncGetAttributes(&fa, feasibility_kernel);
     cudaFuncGetAttributes(&fa, class_feasibility_kernel);
     cudaFuncGetAttributes(&fa, finalize_options_kernel);
@@ -1231,7 +1237,15 @@ static int run_pack(ksched_handle* h) {
     CUDA_TRY(h, cudaStreamWaitEvent(h->stream, done, 0));  // no-op for an event that was never recorded
     CUDA_TRY(h, cudaMemcpyToSymbolAsync(g_k2, &k2, sizeof(K2Params), 0, cudaMemcpyHostToDevice, h->stream));
     // the attribute belongs to the function, not to the handle: set it under the same lock as the launch
-    void (*kern)() = h->cat.n_res_ext > 0 ? pack_kernel<true> : pack_kernel<false>;
+    const bool ext = h->cat.n_res_ext > 0, small = threads <= kPackThreadsSmall;
+    void (*kern)() = small ? (ext ? pack_kernel<true, kPackThreadsSmall> : pack_kernel<false, kPackThreadsSmall>)
+                           : (ext ? pack_kernel<true, kPackThreads> : pack_kernel<false, kPackThreads>);
+    cudaFuncAttributes fa;
+    CUDA_TRY(h, cudaFuncGetAttributes(&fa, kern));
+    if (threads > fa.maxThreadsPerBlock) {  // the instantiation's register budget does not fit this block
+      h->err = "pack_kernel: " + std::to_string(threads) + " threads exceed the instantiation's limit of " + std::to_string(fa.maxThreadsPerBlock);
+      return KSCHED_ERR_INVALID;
+    }
     CUDA_TRY(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kern<<<1, threads, smem, h->stream>>>();
     CUDA_TRY(h, cudaGetLastError());
@@ -1321,6 +1335,9 @@ static void print_pack_profile(const long long* counters) {
           c[kCtrGenCommit]);
   fprintf(stderr, "[pack profile] class_run: calls=%lld pods=%lld bails=%lld ineligible=%lld cycles=%lld\n", c[kCtrRunCalls], c[kCtrRunPlaced],
           c[kCtrRunBails], c[kCtrRunIneligible], c[kCtrRunCallCycles]);
+  fprintf(stderr, "[pack profile] class_run fixed cost: open nodes at entry (sum)=%lld entry cycles=%lld (per-node inputs %lld) "
+                  "write-back cycles=%lld | compactions=%lld slots=%lld cycles=%lld\n", c[kCtrRunActiveSum], c[kCtrRunEntryCycles],
+          c[kCtrRunInputCycles], c[kCtrRunWbCycles], c[kCtrRunCompacts], c[kCtrRunCompactSlots], c[kCtrRunCompactCycles]);
   fprintf(stderr, "[pack profile] class_run round trips (status-1 stop -> entry of the next call that places pods): cycles=%lld | "
                   "stops for want of a variant=%lld, their round trips' cycles=%lld | variant store: hits=%lld entries=%lld\n",
           c[kCtrRoundTripCycles], c[kCtrNoVariantStops], c[kCtrNoVariantTripCycles], c[kCtrVarStoreHits], c[kCtrVarStoreEntries]);

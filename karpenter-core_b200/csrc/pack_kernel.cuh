@@ -2621,6 +2621,10 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
   KS_K2
   RunCtx& rc = g_rc;
   RunIO& io = g_rio;
+#ifdef KSCHED_PROFILE_PACK
+  const long long cr_e0 = clock64();
+  if (threadIdx.x == 0) s.counters[kCtrRunActiveSum] += io.n_active;
+#endif
   HotSmem* hs = reinterpret_cast<HotSmem*>(dyn_smem);
   uint32_t* zv = reinterpret_cast<uint32_t*>(dyn_smem + sizeof(HotSmem) + s.run_off);  // [kRunMask][kTopoCap] bits 0..15 admitted domains, 16 exact (In), 17 present
   uint32_t* rpv = zv + (size_t)kRunMask * kTopoCap;                                      // [kActCap] room | placed << 16 | dead
@@ -2729,6 +2733,9 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
       if (tid == 0) rc.m_registered[j] = (uint32_t)s.grp_registered[rc.m_group[j]];
     }
   }
+#ifdef KSCHED_PROFILE_PACK
+  const long long cr_in0 = clock64();
+#endif
   for (int a = tid; a < n_active; a += T) {
     const unsigned short fl = hs->flags[a];
     unsigned rm;
@@ -2754,6 +2761,9 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
     rpv[a] = rm;
   }
   __syncthreads();
+#ifdef KSCHED_PROFILE_PACK
+  if (tid == 0) s.counters[kCtrRunInputCycles] += clock64() - cr_in0;
+#endif
   // ---- capture the node generic_step has just created for this class as a fresh-node variant
   if (fresh_valid && !s.any_limits && W32 <= kRunW32 && fresh_a == n_active - 1 && fresh_a >= 0) {
     const int a = fresh_a, n = hs->node[a];
@@ -2918,6 +2928,9 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
     if (qlen == 0) break;
   }
   __syncthreads();
+#ifdef KSCHED_PROFILE_PACK
+  const long long cr_t1 = clock64();
+#endif
   // ---- the run is over: write back what the commits deferred
   const int placed_total = qi - qi0;
   run_store_chunk(e, buf, qi - cb < CH ? qi - cb : CH, seq0 + (cb - qi0));  // assignments of the partly consumed chunk
@@ -2955,24 +2968,43 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
     if (rc.m_rec[j] && warp == 0 && lane < kRunDom && ((rc.m_registered[j] >> lane) & 1)) s.grp_cnt[(size_t)rc.m_group[j] * 64 + lane] = rc.cnt[0][j][lane];
   __syncthreads();
   if (tid < n_host && rc.h_inc[tid]) s.grp_host_total[rc.h_group[tid]] += rc.h_inc[tid];
-  // ---- compact the active list (tombstones out); slot order is irrelevant, ownership ends with the run
+#ifdef KSCHED_PROFILE_PACK
+  const long long cr_t2 = clock64();
+  const int cr_slots = rc.tomb > 0 ? n_active : 0;  // slots the compaction scans
+#endif
+  // ---- compact the active list (tombstones out); ownership ends with the run. The k-th tombstone below n_live (ascending)
+  // takes the k-th live slot at or above n_live (descending), the order of the two-pointer scan the slots always had.
   if (rc.tomb > 0) {
-    if (tid == 0) {
-      int i = 0, j = n_active - 1;
-      while (true) {
-        while (j >= 0 && hs->key[j] == ~0ull) --j;
-        while (i < j && hs->key[i] != ~0ull) ++i;
-        if (i >= j) break;
-        hs->key[i] = hs->key[j];
-        for (int r = 0; r < kHotRes; ++r) { hs->q[r][i] = hs->q[r][j]; hs->bound[r][i] = hs->bound[r][j]; hs->bound2[r][i] = hs->bound2[r][j]; }
-        hs->node[i] = hs->node[j]; hs->flags[i] = hs->flags[j]; hs->absorbed[i] = hs->absorbed[j]; hs->rejected[i] = hs->rejected[j];
-        hs->key[j] = ~0ull;
-      }
+    const int n_live = n_active - rc.tomb;
+    const int per = (n_active + T - 1) / T, a0 = tid * per, a1 = min(a0 + per, n_active);  // each thread: one stretch of slots
+    int live = 0;
+    for (int a = a0; a < a1; ++a) live += hs->key[a] != ~0ull;
+    int total, xpar = 0;
+    int lb = block_scan_incl(live, &total, xpar) - live;  // live slots below a0, then below the slot at hand
+    uint32_t* hole = rpv;  // hole rank -> slot (rpv is dead after the write-back)
+    int a = a0;
+    for (; a < a1 && a < n_live; ++a) {
+      if (hs->key[a] == ~0ull) hole[a - lb] = a;  // rank: tombstones below a
+      else ++lb;
     }
-    n_active -= rc.tomb;
+    __syncthreads();
+    for (; a < a1; ++a) {  // slots at or above n_live: only their owner touches them
+      if (hs->key[a] == ~0ull) continue;
+      const int i = hole[n_live - 1 - lb];  // rank: live slots above a
+      hs->key[i] = hs->key[a];
+#pragma unroll
+      for (int r = 0; r < kHotRes; ++r) { hs->q[r][i] = hs->q[r][a]; hs->bound[r][i] = hs->bound[r][a]; hs->bound2[r][i] = hs->bound2[r][a]; }
+      hs->node[i] = hs->node[a]; hs->flags[i] = hs->flags[a]; hs->absorbed[i] = hs->absorbed[a]; hs->rejected[i] = hs->rejected[a];
+      hs->key[a] = ~0ull;
+      ++lb;
+    }
+    n_active = n_live;
   }
 #ifdef KSCHED_PROFILE_PACK
   if (tid == 0) {
+    const long long cr_t3 = clock64();
+    s.counters[kCtrRunEntryCycles] += cr_t0 - cr_e0; s.counters[kCtrRunWbCycles] += cr_t2 - cr_t1;
+    if (cr_slots) { s.counters[kCtrRunCompacts] += 1; s.counters[kCtrRunCompactSlots] += cr_slots; s.counters[kCtrRunCompactCycles] += cr_t3 - cr_t2; }
     if (lvl) {
       s.counters[kCtrRunLvCycles] += clock64() - cr_t0; s.counters[kCtrRunLvPods] += placed_total;
       s.counters[kCtrRunLvSteps] += cr_it[0] + cr_it[1]; s.counters[kCtrRunLvFresh] += cr_it[2]; s.counters[kCtrRunLvPerPod] += cr_it[3];
@@ -3000,8 +3032,11 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
 #endif
 
 // kExt: the problem has ext resources (DESIGN.md §3). Without them the kernel is compiled without any ext gate.
-template <bool kExt>
-__global__ void __launch_bounds__(kPackThreads, 1) pack_kernel() {
+// kMaxThreads: the largest block the instantiation is launched with. Its register budget is 64 K / kMaxThreads (capped at
+// 255): 128 registers at 512 threads spill in class_run and the generic step, 254 at 256 threads do not (run_pack picks the instantiation).
+template <bool kExt, int kMaxThreads>
+__global__ void __launch_bounds__(kMaxThreads, 1) pack_kernel() {
+  static_assert(kMaxThreads % 32 == 0 && kMaxThreads <= kPackThreads, "pack_kernel: whole warps, at most kPackThreads");
 #ifdef KSCHED_PROFILE_PACK
   long long pk_acc[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
   long long pk_last = clock64();

@@ -39,6 +39,7 @@ extern "C" {
 #define KSCHED_ROW_WORDS 32 /* canonical 256-byte rows (SURVEY.md 8d: B_pod = B_col = 256 B) */
 #define KSCHED_KEY_HOSTNAME 255
 #define KSCHED_NONE 0xFFFFFFFFu
+#define KSCHED_HOSTNAME_TABLE (-2) /* hostname_reqs[i][1]: the admitted existing slots are row i of problem.hostname_slots */
 
 /* error codes (negative) */
 #define KSCHED_OK 0
@@ -233,6 +234,9 @@ typedef struct ksched_topo_group {
 #define KSCHED_TOPO_SELECTS 2    /* TopologyGroup.selects(pod), topologygroup.go:246 */
 #define KSCHED_TOPO_RECORDS 4    /* group in Topology.topologies and selects the class (topology.go:122-135) */
 #define KSCHED_TOPO_RECORDS_INVERSE 8 /* inverse group owned by the class (topology.go:138-142) */
+#define KSCHED_TOPO_HOST_EXTRA 16 /* hostname affinity group the class constrains: its hostname requirement admits a domain with a
+                                     count that is no existing slot (ksched_topo_group.extra_nonzero_domains), so the group's
+                                     options for the class are never empty (topologygroup.go:202-231) */
 typedef struct ksched_class_topo {
   uint32_t group;
   uint32_t flags;
@@ -257,7 +261,8 @@ typedef struct ksched_problem {
   const uint64_t* itype_req_sets;     /* [n_itype_reqs][type_words]: allowed types per instance-type requirement */
   const uint8_t* itype_req_complement; /* [n_itype_reqs] 1 = NotIn/Exists form (allows types outside the catalog) */
   int32_t n_itype_reqs;
-  const int32_t* hostname_reqs;       /* [n_hostname_reqs][2]: {complement, existing node slot or -1 (= none of ours)} */
+  const int32_t* hostname_reqs;       /* [n_hostname_reqs][2]: {complement, existing node slot or -1 (= none of ours)}, or
+                                         {admits new nodes (0/1), KSCHED_HOSTNAME_TABLE}: see hostname_slots */
   int32_t n_hostname_reqs;
   int32_t max_new_nodes;              /* capacity for new nodes (<= n_pods) */
   int32_t write_feasibility;          /* also copy the dense feasibility bitmask back (result.feasibility) */
@@ -287,6 +292,17 @@ typedef struct ksched_problem {
   const uint64_t* existing_hostport_ext;        /* [n_existing][n_hostport_ext_words] (may be NULL when n_existing is 0) */
   int32_t n_hostport_ext_words;
   int32_t pad_hostport;
+  /* Hostname requirements beyond the {complement, slot} pair (In / NotIn one value, Exists): value lists, several
+     requirements on one pod, DoesNotExist, Gt / Lt. An entry i of hostname_reqs whose second word is KSCHED_HOSTNAME_TABLE
+     admits existing slot e iff bit e % 64 of hostname_slots[i][e / 64] is set, and a new node iff hostname_reqs[i][0] is 1 (a
+     new node's hostname is a placeholder). Rows of pair entries hold the slots the pair admits; the kernels read the pair.
+     filter_term_hostname[f] is the hostname part of filter term f, an entry of hostname_reqs, or KSCHED_NONE; it is NULL
+     when no term names the hostname. Both tables NULL and the count 0 when no entry needs them; ksched_upload answers
+     KSCHED_ERR_INVALID when the tables and the count disagree. */
+  const uint64_t* hostname_slots;        /* [n_hostname_reqs][n_hostname_words] */
+  const uint32_t* filter_term_hostname;  /* [n_filter_terms] (needs hostname_slots) */
+  int32_t n_hostname_words;
+  int32_t pad_hostname;
 } ksched_problem;
 
 typedef struct ksched_new_node {

@@ -127,6 +127,11 @@ def lib():
     L.kh_encoded_key_info.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(C.c_longlong)]
     L.kh_encoded_resource_id.argtypes = [C.c_void_p, C.c_char_p]
     L.kh_encoded_hostport.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_int]
+    L.kh_encoded_hostname_req.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_longlong), C.c_int]
+    L.kh_encoded_class_hostname.argtypes = [C.c_void_p, C.c_int]
+    L.kh_encoded_class_hostname.restype = C.c_longlong
+    L.kh_encoded_pod_class.argtypes = [C.c_void_p, C.c_int]
+    L.kh_encoded_pod_class.restype = C.c_longlong
     L.kh_value_class_selftest.argtypes = [C.c_uint, C.c_int]
     L.kh_gpu_load.argtypes = [C.c_void_p]
     L.kh_encoded_set_count_visited.argtypes = [C.c_void_p, C.c_int]
@@ -574,10 +579,28 @@ class ResidentSolve:
         if not self.enc:
             msg = lib().kh_scheduler_error().decode()
             raise KschedError(KSCHED_ERR_UNSUPPORTED if msg.startswith("unsupported:") else KSCHED_ERR_INVALID, msg)
-        d = (C.c_longlong * 14)()
+        d = (C.c_longlong * 16)()
         lib().kh_encoded_dims(self.enc, d)
         self.dims = dict(zip(["pods", "classes", "existing", "groups", "types", "templates", "keys", "resources", "type_words", "class_topo",
-                              "taintsets", "resources_ext", "hostports", "hostport_ext_words"], list(d)))
+                              "taintsets", "resources_ext", "hostports", "hostport_ext_words", "hostname_reqs", "hostname_words"], list(d)))
+
+    def hostname_reqs(self):
+        """every hostname requirement of this encoding in entry order, as (admits new nodes, [admitted existing slots])"""
+        out, buf = [], (C.c_longlong * (self.dims["existing"] + 1))()
+        for i in range(self.dims["hostname_reqs"]):
+            n = lib().kh_encoded_hostname_req(self.enc, i, buf, len(buf))
+            assert n >= 0, n
+            out.append((bool(buf[0]), list(buf[1:n + 1])))
+        return out
+
+    def pod_class(self, i):
+        """the initial class of pod i of Solve's pod list"""
+        return lib().kh_encoded_pod_class(self.enc, i)
+
+    def class_hostname_req(self, c):
+        """the hostname_reqs entry of class c, or None without a hostname requirement"""
+        i = lib().kh_encoded_class_hostname(self.enc, c)
+        return None if i < 0 else i
 
     def hostports(self):
         """the host-port entries of this encoding in id order, as (ip, port, protocol): the ones the encoder kept"""

@@ -200,6 +200,11 @@ struct ksched_handle {
   DevBuf<uint64_t> d_ex_hp_ext, d_ex_hp_ext0;     // [hp_ext_words][n_existing] working copy / pristine copy
   DevBuf<uint64_t> d_nn_hp_ext;                   // [hp_ext_words][max_new]
   int hp_ext_words = 0;
+  // hostname requirement table (ksched_problem.hostname_slots); allocated only when the problem has one
+  DevBuf<uint64_t> d_hostname_slots;  // [n_hostname_reqs][hostname_words]
+  DevBuf<uint32_t> d_filter_hostname; // [n_filter_terms]
+  int hostname_words = 0;
+  bool filter_hostname = false;
   // ext resources (ksched.h: ksched_catalog.n_res_ext); allocated only when the catalog has some
   DevBuf<int64_t> d_alloc_ext, d_cls_req_ext, d_ex_avail_ext, d_ex_req_ext, d_nn_req_ext;
   DevBuf<uint32_t> d_cls_ext_present, d_nn_ext_present;
@@ -707,6 +712,20 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
     }
   }
   {
+    // hostname requirement table: set exactly when the count is positive, wide enough for every existing slot, and present
+    // when an entry or a filter term reads it
+    const int hw = pb->n_hostname_words;
+    bool ok = hw >= 0 && (hw > 0) == (pb->hostname_slots != nullptr) && (hw > 0 || !pb->filter_term_hostname) &&
+              (hw == 0 || (int64_t)hw * 64 >= pb->n_existing);
+    for (int i = 0; ok && i < pb->n_hostname_reqs; ++i) ok = pb->hostname_reqs[2 * i + 1] != KSCHED_HOSTNAME_TABLE || hw > 0;
+    for (int f = 0; ok && pb->filter_term_hostname && f < pb->n_filter_terms; ++f)
+      ok = pb->filter_term_hostname[f] == KSCHED_NONE || pb->filter_term_hostname[f] < (uint32_t)pb->n_hostname_reqs;
+    if (!ok) {
+      h->err = "hostname_slots / filter_term_hostname must be set exactly when n_hostname_words is positive and cover the entries";
+      return KSCHED_ERR_INVALID;
+    }
+  }
+  {
     // ext resources: the tables exist exactly when the catalog has ext resources, and name no resource beyond them
     const int X = h->cat.n_res_ext;
     const bool any = pb->class_requests_ext || pb->class_res_ext_present || pb->existing_available_ext;
@@ -802,6 +821,10 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
   CUDA_TRY(h, upload(h, h->d_class_topo, pb->class_topo, (size_t)pb->n_class_topo));
   CUDA_TRY(h, upload(h, h->d_filter_terms, pb->filter_terms, (size_t)pb->n_filter_terms));
   CUDA_TRY(h, upload(h, h->d_hostname_reqs, pb->hostname_reqs, (size_t)pb->n_hostname_reqs * 2));
+  h->hostname_words = pb->n_hostname_words;
+  h->filter_hostname = pb->filter_term_hostname != nullptr;
+  if (h->hostname_words) CUDA_TRY(h, upload(h, h->d_hostname_slots, pb->hostname_slots, (size_t)pb->n_hostname_reqs * h->hostname_words));
+  if (h->filter_hostname) CUDA_TRY(h, upload(h, h->d_filter_hostname, pb->filter_term_hostname, (size_t)pb->n_filter_terms));
   CUDA_TRY(h, upload(h, h->d_itype_comp, pb->itype_req_complement, (size_t)pb->n_itype_reqs));
   CUDA_TRY(h, upload(h, h->d_itype_sets, reinterpret_cast<const uint32_t*>(pb->itype_req_sets), (size_t)pb->n_itype_reqs * W32));
   // existing nodes -> SoA
@@ -901,7 +924,9 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
         x.group = ct.group; x.flags = ct.flags; x.key = g.key; x.type = g.type; x.has_filter = g.filter_begin != g.filter_end;
         // a term without any requirement is Compatible with every node (topologynodefilter.go:57-70): such a filter always matches
         for (uint32_t f = g.filter_begin; f < g.filter_end && f < (uint32_t)pb->n_filter_terms; ++f)
-          if (((pb->filter_terms[f].meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF) == 0) x.has_filter = 0;
+          if (((pb->filter_terms[f].meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF) == 0 &&
+              (!pb->filter_term_hostname || pb->filter_term_hostname[f] == KSCHED_NONE))
+            x.has_filter = 0;
         x.max_skew = g.max_skew; x.host_row = host_row[ct.group];
         relx[e] = x;
       }
@@ -1172,6 +1197,8 @@ static int run_pack(ksched_handle* h) {
   s.relx = h->d_relx.ptr;
   s.classes = h->d_classes.ptr; s.groups = h->d_groups.ptr; s.class_topo = h->d_class_topo.ptr; s.filter_terms = h->d_filter_terms.ptr;
   s.itype_sets = h->d_itype_sets.ptr; s.itype_complement = h->d_itype_comp.ptr; s.hostname_reqs = h->d_hostname_reqs.ptr;
+  s.hostname_slots = h->hostname_words ? h->d_hostname_slots.ptr : nullptr; s.hostname_words = h->hostname_words;
+  s.filter_hostname = h->filter_hostname ? h->d_filter_hostname.ptr : nullptr;
   s.order = h->d_order.ptr; s.rows = h->d_rows.ptr; s.F = h->d_F.ptr; s.best = h->d_best.ptr;
   s.pod_pos = h->d_pod_pos.ptr; s.use_F = h->world == 1 ? 1 : 0;
   s.n_pods = h->n_pods; s.n_classes = h->n_classes; s.n_existing = h->n_existing; s.n_groups = h->n_groups; s.max_new = h->max_new;

@@ -418,7 +418,8 @@ struct LoopVars {
 
 // ---- existing-node run ("water-fill") --------------------------------------------------------------------------------
 // A run of consecutive first-pass pods of ONE plain class (no requirement key, no topology relation, no host port, no
-// volume, no instance-type / hostname requirement) is placed on the existing nodes in one pass. First fit over existing
+// volume, no instance-type requirement) is placed on the existing nodes in one pass. A hostname requirement only removes the
+// slots it does not admit (K_e = 0): that verdict never changes for the class, so the cursor stays exact. First fit over existing
 // nodes in slice order (scheduler.go:176-180) sends identical pods to the first node that still fits one, until it does not:
 // node e takes K_e = min over requested resources of floor((available - requests) / request) of them, so the run is an
 // exclusive prefix sum of K over the nodes from the class's cursor on. Every effect of the sequential commits is reproduced
@@ -509,7 +510,8 @@ __device__ __noinline__ void existing_run(const PodRegs& first) {
   while (placed < m && e0 < NE) {
     const int e = e0 + tid;
     int k = 0;
-    if (e < NE && !s.ex_closed[e] && tolerates_node_set(s, first.tol, cls, s.ex_taintset[e])) {
+    if (e < NE && !s.ex_closed[e] && tolerates_node_set(s, first.tol, cls, s.ex_taintset[e]) &&
+        (first.hostname == KSCHED_NONE || hostname_req_allows(s, first.hostname, e, true))) {
       long long K = m - placed;
       const uint32_t qp = s.ex_req_present[e] | first.res, ap = s.ex_avail_present[e];
       for (int r = 0; r < R && K > 0; ++r) {
@@ -3184,7 +3186,7 @@ __global__ void __launch_bounds__(kMaxThreads, 1) pack_kernel() {
     // ---- existing-node run (see existing_run): identical plain pods take the existing nodes in one prefix-sum pass
     if (NE > 0 && !s.count_visited && qi < s.n_pods && (unsigned)nxt.cls64 != xrun_block_cls &&
         ((nxt.meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF) == 0 && nxt.topo_begin == nxt.topo_end && nxt.itype == KSCHED_NONE &&
-        nxt.hostname == KSCHED_NONE && !has_host_ports(s, nxt) && (nxt.res >> kHotRes) == 0 && !class_has_volumes(s, (unsigned)nxt.cls64) &&
+        !has_host_ports(s, nxt) && (nxt.res >> kHotRes) == 0 && !class_has_volumes(s, (unsigned)nxt.cls64) &&
         !(kExt && class_ext(s, (unsigned)nxt.cls64))) {
       __syncthreads();
       if (tid == 0) { ExRunIO& io = g_xio; io.qi = qi; io.head = head; io.qlen = qlen; io.seq = seq; io.parity = parity; io.add_calls = add_calls; io.placed = 0; }

@@ -27,6 +27,9 @@ struct PackState {
   const uint32_t* itype_sets;        // [n][W32]
   const uint8_t* itype_complement;
   const int32_t* hostname_reqs;      // [n][2]
+  const uint64_t* hostname_slots;    // [n][hostname_words] admitted existing slots of table entries (ksched.h), or nullptr
+  const uint32_t* filter_hostname;   // [n_filter_terms] hostname part of a filter term (hostname_reqs entry), or nullptr
+  int hostname_words;
   const uint32_t* order;             // FFD order: queue position -> pod
   const uint64_t* rows;              // [n_pods][32] dense pod-row matrix in FFD order (K0)
   uint32_t* pod_pos;                 // pod -> FFD position (row of F / best)
@@ -269,12 +272,41 @@ __device__ __noinline__ bool topo_hostname_ok(int j, int slot, bool pod_allows_s
   return cnt == 0 && pod_allows_slot;  // anti-affinity
 }
 
-// Does the pod's hostname requirement admit this slot? (requirement on kubernetes.io/hostname, never well-known)
-__device__ __forceinline__ bool hostname_allows(const PackState& s, const ksched_pod_row& row, int slot, bool is_existing) {
-  if (row.hostname_req == KSCHED_NONE) return true;
-  const int32_t comp = s.hostname_reqs[row.hostname_req * 2], target = s.hostname_reqs[row.hostname_req * 2 + 1];
+// Does hostname requirement `req` (an entry of hostname_reqs) admit this slot? The {complement, slot} pair, or a table entry:
+// the existing slot's bit, and for a new node (a placeholder hostname) the entry's first word. The table read is out of line:
+// the pair test is inlined at every caller, and the kernels' code size decides their speed (DESIGN.md §3).
+__device__ __noinline__ bool hostname_table_allows(uint32_t req, int slot, bool is_existing) {
+  KS_K2
+  if (!is_existing) return s.hostname_reqs[req * 2] != 0;
+  return ((s.hostname_slots[(size_t)req * s.hostname_words + (slot >> 6)] >> (slot & 63)) & 1) != 0;
+}
+__device__ __forceinline__ bool hostname_req_allows(const PackState& s, uint32_t req, int slot, bool is_existing) {
+  const int32_t comp = s.hostname_reqs[req * 2], target = s.hostname_reqs[req * 2 + 1];
+  if (target == KSCHED_HOSTNAME_TABLE) return hostname_table_allows(req, slot, is_existing);
   const bool same = is_existing && target == slot;
   return comp ? !same : same;
+}
+// Does the pod's hostname requirement admit this slot? (requirement on kubernetes.io/hostname, never well-known)
+__device__ __forceinline__ bool hostname_allows(const PackState& s, const ksched_pod_row& row, int slot, bool is_existing) {
+  return row.hostname_req == KSCHED_NONE || hostname_req_allows(s, row.hostname_req, slot, is_existing);
+}
+
+// nextDomainAffinity (topologygroup.go:202-231) of hostname group gi for a pod with hostname requirement `req`: does some
+// hostname the requirement admits have a matching pod? Existing slots by their own counts; new nodes together, as the
+// slots with a count that are neither existing nor extra domains (grp_host_total); extra domains (hostnames that are no slot)
+// by the encoder's KSCHED_TOPO_HOST_EXTRA, since their counts never change.
+__device__ __noinline__ bool hostname_affinity_options(int gi, int host_row, uint32_t req, uint32_t flags) {
+  KS_K2
+  if (flags & KSCHED_TOPO_HOST_EXTRA) return true;
+  const int NE = s.n_existing;
+  const uint16_t* cnt = s.grp_host + (size_t)host_row * (NE + s.max_new);
+  int ex_nonzero = 0;
+  for (int e = 0; e < NE; ++e) {
+    if (!cnt[e]) continue;
+    if (hostname_req_allows(s, req, e, true)) return true;
+    ++ex_nonzero;
+  }
+  return s.grp_host_total[gi] - s.groups[gi].extra_nonzero_domains - ex_nonzero > 0 && hostname_req_allows(s, req, NE, false);
 }
 
 // Requirement phase of Node.Add / ExistingNode.Add: Compatible(pod) + merge, topology tighten + Compatible + merge.
@@ -445,10 +477,10 @@ __device__ __noinline__ void fill_pod_topo_dynamic(int j) {
   pt.n_sorted[j] = 0;
   pt.ok_mask[j] = 0;
   if (gkey == KSCHED_KEY_HOSTNAME) {
-    if (gtype == 1) {
-      // options.Len()==0 <=> no admissible hostname has a matching pod (hostname requirements on the pod are
-      // restricted to a single existing slot, handled in topo_hostname_ok)
-      pt.bootstrap[j] = (s.grp_host_total[gi] == 0) && (flags & KSCHED_TOPO_SELECTS);
+    if (gtype == 1) {  // options.Len()==0 <=> no hostname the pod's requirement admits has a matching pod
+      const bool any = row.hostname_req == KSCHED_NONE ? s.grp_host_total[gi] != 0
+                                                       : hostname_affinity_options(gi, pt.host_row[j], row.hostname_req, flags);
+      pt.bootstrap[j] = !any && (flags & KSCHED_TOPO_SELECTS);
     }
     return;
   }
@@ -566,14 +598,16 @@ __device__ __forceinline__ bool topo_prefilter(const uint64_t* vals, uint64_t me
   return true;
 }
 
-// TopologyNodeFilter.MatchesRequirements (topologynodefilter.go:57-70): any term Compatible with the node requirements
+// TopologyNodeFilter.MatchesRequirements (topologynodefilter.go:57-70): any term Compatible with the node requirements. A
+// term's hostname part reads the node's hostname: the slot's bit for an existing node, the placeholder flag for a new one.
 __device__ __noinline__ bool filter_matches(const ksched_topo_group& g, const uint64_t* vals, uint64_t meta,
-                               int stride, int idx) {
+                               int stride, int idx, int slot) {
   KS_K2
   if (g.filter_begin == g.filter_end) return true;
   for (uint32_t f = g.filter_begin; f < g.filter_end; ++f) {
     const ksched_reqset& term = s.filter_terms[f];
-    bool ok = true;
+    const uint32_t host = s.filter_hostname ? s.filter_hostname[f] : KSCHED_NONE;
+    bool ok = host == KSCHED_NONE || hostname_req_allows(s, host, slot, slot < s.n_existing);
     uint32_t keys = (uint32_t)(term.meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF;
     while (keys && ok) {
       int k = __ffs(keys) - 1;
@@ -603,7 +637,7 @@ __device__ __noinline__ void topo_record_entry(uint32_t e, const uint64_t* vals,
   if (!active) return;  // the group does not exist yet
   bool rec = false, all_values = false;
   if (x.flags & KSCHED_TOPO_RECORDS) {
-    if (!x.has_filter || filter_matches(s.groups[gi], vals, meta, stride, idx)) { rec = true; all_values = (x.type == 2); }
+    if (!x.has_filter || filter_matches(s.groups[gi], vals, meta, stride, idx, slot)) { rec = true; all_values = (x.type == 2); }
   }
   const bool rec_inv = (x.flags & KSCHED_TOPO_RECORDS_INVERSE) != 0;
   if (x.key == KSCHED_KEY_HOSTNAME) {  // the node's hostname requirement is always In [its own hostname]

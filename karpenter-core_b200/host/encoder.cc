@@ -14,6 +14,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <limits>
+#include <optional>
 #include <tuple>
 #include <unordered_map>
 #include <unordered_set>
@@ -73,6 +74,65 @@ Req new_requirement(Op op, const std::vector<std::string>& values, const std::ma
   if (op == Op::Gt) { r.has_gt = true; parse_int(values.at(0), &r.gt); }
   if (op == Op::Lt) { r.has_lt = true; parse_int(values.at(0), &r.lt); }
   return r;
+}
+
+// A requirement on kubernetes.io/hostname in the reference's string algebra: NewRequirement (requirement.go:44-68),
+// Intersection (:117-150), Has (:171-176), Operator (:186-197). Hostnames are not dictionary values, so the encoder
+// evaluates these on strings and hands the device the existing slots they admit (DESIGN.md §3, hostname requirements).
+constexpr const char* kPlaceholderPrefix = "hostname-placeholder-";  // a new node's hostname (node.go:46, a per-Solve counter)
+struct HostnameReq {
+  bool comp = true;  // (true, {}, no bounds): Exists
+  std::set<std::string> values;
+  bool has_gt = false, has_lt = false;
+  int64_t gt = 0, lt = 0;
+  static HostnameReq make(const NodeSelectorRequirement& r) {
+    for (auto& v : r.values)
+      if (v.rfind(kPlaceholderPrefix, 0) == 0) unsupported("hostname requirement naming a placeholder hostname: " + v);
+    HostnameReq h;
+    h.comp = !(r.op == Op::In || r.op == Op::DoesNotExist);
+    if (r.op == Op::In || r.op == Op::NotIn) h.values.insert(r.values.begin(), r.values.end());
+    if (r.op == Op::Gt) { h.has_gt = true; parse_int(r.values.at(0), &h.gt); }
+    if (r.op == Op::Lt) { h.has_lt = true; parse_int(r.values.at(0), &h.lt); }
+    return h;
+  }
+  bool within(const std::string& v) const {
+    if (!has_gt && !has_lt) return true;
+    int64_t x;
+    if (!parse_int(v, &x)) return false;
+    return !(has_gt && gt >= x) && !(has_lt && lt <= x);
+  }
+  bool has(const std::string& v) const { return (values.count(v) > 0) != comp && within(v); }
+  HostnameReq intersect(const HostnameReq& o) const {
+    HostnameReq r;
+    r.has_gt = has_gt || o.has_gt;
+    r.gt = has_gt && o.has_gt ? std::max(gt, o.gt) : (has_gt ? gt : o.gt);
+    r.has_lt = has_lt || o.has_lt;
+    r.lt = has_lt && o.has_lt ? std::min(lt, o.lt) : (has_lt ? lt : o.lt);
+    if (r.has_gt && r.has_lt && r.gt >= r.lt) return HostnameReq{false, {}, false, false, 0, 0};  // DoesNotExist
+    r.comp = comp && o.comp;
+    if (comp && o.comp) { r.values = values; r.values.insert(o.values.begin(), o.values.end()); }
+    else if (comp) { for (auto& v : o.values) if (!values.count(v)) r.values.insert(v); }
+    else if (o.comp) { for (auto& v : values) if (!o.values.count(v)) r.values.insert(v); }
+    else { for (auto& v : values) if (o.values.count(v)) r.values.insert(v); }
+    for (auto it = r.values.begin(); it != r.values.end();) it = r.within(*it) ? std::next(it) : r.values.erase(it);
+    if (!r.comp) r.has_gt = r.has_lt = false;
+    return r;
+  }
+  // Operator() is NotIn or DoesNotExist: Compatible with a node that has no hostname label (requirements.go:123-133)
+  bool admits_unlabelled() const { return comp ? !values.empty() : values.empty(); }
+  // A new node's hostname is a placeholder: not an integer, and never one of `values` (make refuses such values)
+  bool admits_new() const { return comp && !has_gt && !has_lt; }
+  std::string key() const {
+    std::string s = comp ? "!" : "=";
+    for (auto& v : values) s += v + ",";
+    return s + "|" + (has_gt ? std::to_string(gt) : "") + "|" + (has_lt ? std::to_string(lt) : "");
+  }
+};
+// Requirements.Add of a pod's hostname requirements, in order (requirements.go:87-94)
+HostnameReq hostname_intersection(const std::vector<NodeSelectorRequirement>& rs) {
+  HostnameReq h = HostnameReq::make(rs.at(0));
+  for (size_t i = 1; i < rs.size(); ++i) h = HostnameReq::make(rs[i]).intersect(h);
+  return h;
 }
 
 // ---- resources (utils/resources/resources.go)
@@ -469,6 +529,12 @@ struct Builder {
   bool res_pruned = false;                                 // resource names no request reads were left out of res_id
   std::vector<Daemon> daemons;
   std::map<std::string, int> hostname_slot;                // hostname -> existing slot
+  std::vector<std::string> slot_hostname;                  // existing slot -> hostname (label, or the node's name)
+  // hostname_reqs entries: the string form of a table entry (admitted slots read from E.hostname_slots), none for the
+  // {complement, slot} pair form
+  std::vector<std::optional<HostnameReq>> hostname_forms;
+  std::map<std::string, uint32_t> hostname_table_id;       // HostnameReq::key() -> entry
+  bool filter_names_hostname = false;                      // some topology node filter term has a hostname part
 
   Builder(const Problem& p, Encoded& e, bool cluster_superset) : P(p), E(e), facts(cluster_facts(p)), superset(cluster_superset) {}
 
@@ -538,6 +604,22 @@ struct Builder {
     taintset_id[k] = id;
     taintsets.push_back(ts);
     return id;
+  }
+  // hostname_reqs entries (ksched.h): the {complement, slot} pair of In / NotIn one value and Exists, as before tables
+  // existed, or an entry whose admitted existing slots are a row of the table (one per distinct requirement)
+  uint32_t hostname_pair(int32_t comp, int32_t slot) {
+    E.hostname_reqs.push_back(comp);
+    E.hostname_reqs.push_back(slot);
+    hostname_forms.emplace_back();
+    return (uint32_t)hostname_forms.size() - 1;
+  }
+  uint32_t hostname_table(const HostnameReq& h) {
+    auto id = hostname_table_id.emplace(h.key(), (uint32_t)hostname_forms.size());
+    if (!id.second) return id.first->second;
+    E.hostname_reqs.push_back(h.admits_new() ? 1 : 0);
+    E.hostname_reqs.push_back(KSCHED_HOSTNAME_TABLE);
+    hostname_forms.push_back(h);
+    return id.first->second;
   }
   int hp_entry(const HostPortEntry& e) const {  // id of an entry (host_port_table), -1 when it was left out
     auto it = hp_id.find(e);
@@ -659,6 +741,7 @@ struct Group {
   LabelSelector selector;
   bool filter_nil = true;
   std::vector<std::pair<ksched_reqset, ksched_bounds>> filter;  // TopologyNodeFilter terms
+  std::vector<std::optional<HostnameReq>> filter_host;          // per term: its hostname part, if it names the hostname
   std::string filter_key;
   bool inverse = false;
   bool dormant = false;
@@ -1396,6 +1479,7 @@ void existing_nodes(Builder& B) {
     if (h != n.labels.end()) hostname = h->second;
     if (hostname.empty()) hostname = n.name;
     B.hostname_slot[hostname] = (int)E.existing.size();
+    B.slot_hostname.push_back(hostname);
     E.existing_state_index.push_back(si);
     auto ini = n.labels.find(kInitialized);
     E.existing_initialized.push_back(ini != n.labels.end() && ini->second == "true");
@@ -1506,9 +1590,12 @@ struct Topology {
       Builder::Special sp;
       B.add_selector_reqs(rs, bd, label_reqs(p.node_selector), &sp);
       if (term) B.add_selector_reqs(rs, bd, *term, &sp);
-      if (!sp.hostname.empty() || !sp.itype.empty()) unsupported("topology spread node filter on hostname / instance-type");
+      if (!sp.itype.empty()) unsupported("topology spread node filter on instance-type");
+      std::optional<HostnameReq> host;
+      if (!sp.hostname.empty()) host = hostname_intersection(sp.hostname);
       g.filter.push_back({rs, bd});
-      parts.push_back(canon(rs, bd));
+      g.filter_host.push_back(host);
+      parts.push_back(canon(rs, bd) + (host ? "hostname:" + host->key() : ""));
     };
     if (!p.has_node_affinity || !p.has_required_node_affinity) add_term(nullptr);
     else for (auto& t : p.required_node_terms) add_term(&t);
@@ -1520,8 +1607,14 @@ struct Topology {
     ksched_reqset rs{}; ksched_bounds bd{};
     Builder::Special sp;
     B.add_selector_reqs(rs, bd, label_reqs(labels), &sp);
-    for (auto& f : g.filter)
-      if (B.compatible(rs, bd, f.first, f.second)) return true;
+    for (size_t t = 0; t < g.filter.size(); ++t) {
+      if (!B.compatible(rs, bd, g.filter[t].first, g.filter[t].second)) continue;
+      if (const auto& h = g.filter_host[t]) {  // the labels' hostname In [label], or no hostname key at all
+        auto l = labels.find(kHostname);
+        if (l == labels.end() ? !h->admits_unlabelled() : !h->has(l->second)) continue;
+      }
+      return true;
+    }
     return false;
   }
   Group new_group(int type, const std::string& key, const Pod& p, const std::vector<std::string>& nss, const LabelSelector& sel, int32_t skew) const {
@@ -1624,10 +1717,13 @@ void group_tables(Builder& B, const std::vector<Group>& groups) {
     o.dormant = G.dormant;
     o.max_skew = G.max_skew;
     o.filter_begin = (uint32_t)E.filter_terms.size();
-    for (auto& f : G.filter) {
-      ksched_reqset term = f.first;
-      B.to_region_form(term, f.second);
+    for (size_t t = 0; t < G.filter.size(); ++t) {
+      ksched_reqset term = G.filter[t].first;
+      B.to_region_form(term, G.filter[t].second);
       E.filter_terms.push_back(term);
+      const auto& h = G.filter_host[t];
+      E.filter_term_hostname.push_back(h ? B.hostname_table(*h) : KSCHED_NONE);
+      if (h) B.filter_names_hostname = true;
     }
     o.filter_end = (uint32_t)E.filter_terms.size();
     if (G.key == kHostname) {
@@ -1686,7 +1782,8 @@ void superset_counts(Builder& B, Topology& T) {
   E.node_has_hostname_label.assign((size_t)std::max(NE, 1), 0);
   const int FW = (NE + 31) / 32;
   E.group_filter_match.assign((size_t)NG * std::max(FW, 1), 0);
-  std::map<std::string, std::vector<char>> filter_memo;  // node labels without the hostname -> verdict per group
+  // node labels -> verdict per group; without the hostname unless some filter term names it
+  std::map<std::string, std::vector<char>> filter_memo;
   for (int e = 0; e < NE; ++e) {
     const StateNode& n = B.P.nodes[(size_t)E.existing_state_index[(size_t)e]];
     for (int k = 0; k < NK; ++k) {
@@ -1697,7 +1794,7 @@ void superset_counts(Builder& B, Topology& T) {
     }
     E.node_has_hostname_label[(size_t)e] = n.labels.count(kHostname) ? 1 : 0;
     Labels sig = n.labels;
-    sig.erase(kHostname);
+    if (!B.filter_names_hostname) sig.erase(kHostname);
     const std::string key = labels_key(sig);
     auto memo = filter_memo.find(key);
     if (memo == filter_memo.end()) {
@@ -1715,6 +1812,27 @@ std::vector<Group> topology_groups(Builder& B) {
   group_tables(B, T.groups);
   if (B.superset && !T.groups.empty()) superset_counts(B, T);
   return std::move(T.groups);
+}
+
+// ------------------------------------------------------------------ hostname requirement table
+// Row i holds the existing slots hostname_reqs entry i admits: ExistingNode's requirement hostname In [label or name]
+// (existingnode.go) is Compatible with the requirement exactly when the requirement Has that hostname. Pair-form entries get
+// the row their {complement, slot} means. Without a table entry there is no table, so older problems encode as before.
+void hostname_slot_table(Builder& B) {
+  Encoded& E = B.E;
+  if (!B.filter_names_hostname) E.filter_term_hostname.clear();
+  if (B.hostname_table_id.empty()) return;
+  const int NE = (int)E.existing.size(), W = std::max(1, (NE + 63) / 64);
+  if (B.slot_hostname.size() != (size_t)NE) throw std::runtime_error("internal: hostname of an existing slot missing");
+  E.hostname_words = W;
+  E.hostname_slots.assign(B.hostname_forms.size() * (size_t)W, 0);
+  for (size_t i = 0; i < B.hostname_forms.size(); ++i) {
+    uint64_t* row = &E.hostname_slots[i * (size_t)W];
+    const auto& f = B.hostname_forms[i];
+    const int32_t comp = E.hostname_reqs[2 * i], slot = E.hostname_reqs[2 * i + 1];
+    for (int e = 0; e < NE; ++e)
+      if (f ? f->has(B.slot_hostname[(size_t)e]) : ((e == slot) != (comp != 0))) row[e / 64] |= 1ull << (e % 64);
+  }
 }
 
 // ------------------------------------------------------------------ class rows
@@ -1782,18 +1900,21 @@ void class_rows(Builder& B, const std::vector<Group>& groups) {
         E.itype_req_sets.insert(E.itype_req_sets.end(), words.begin(), words.end());
       }
     }
+    std::optional<HostnameReq> host;
     if (!sp.hostname.empty()) {
-      if (sp.hostname.size() != 1) unsupported("more than one hostname requirement on a pod");
+      // every hostname requirement of the class at its relaxation level (node selector, required term, heaviest preferred
+      // term), intersected as Requirements.Add does; placeholder-named values are refused by HostnameReq::make
+      const HostnameReq h = hostname_intersection(sp.hostname);
+      host = h;
       auto& r = sp.hostname[0];
-      int32_t comp, slot = -1;
-      if (r.op == Op::In && r.values.size() == 1) comp = 0;
-      else if (r.op == Op::NotIn && r.values.size() == 1) comp = 1;
-      else if (r.op == Op::Exists) comp = 1;
-      else unsupported("hostname requirement form");
-      if (!r.values.empty()) { auto h = B.hostname_slot.find(r.values[0]); if (h != B.hostname_slot.end()) slot = h->second; }
-      row.hostname_req = (uint32_t)(E.hostname_reqs.size() / 2);
-      E.hostname_reqs.push_back(comp);
-      E.hostname_reqs.push_back(slot);
+      const bool pair = sp.hostname.size() == 1 && (((r.op == Op::In || r.op == Op::NotIn) && r.values.size() == 1) || r.op == Op::Exists);
+      if (pair) {  // the {complement, slot} form
+        int32_t slot = -1;
+        if (!r.values.empty()) { auto f = B.hostname_slot.find(r.values[0]); if (f != B.hostname_slot.end()) slot = f->second; }
+        row.hostname_req = B.hostname_pair(r.op == Op::In ? 0 : 1, slot);
+      } else {
+        row.hostname_req = B.hostname_table(h);
+      }
     }
     for (auto& hp : host_ports(s.pod)) {  // the entry table is complete: host_port_table ran before the existing nodes
       B.hp_bit(B.hp_entry(hp), row.hostport_entries, HW ? &E.class_hostport_entries_ext[(size_t)c * HW] : nullptr);
@@ -1808,11 +1929,16 @@ void class_rows(Builder& B, const std::vector<Group>& groups) {
     // topology relations
     row.topo_begin = (uint32_t)E.class_topo.size();
     for (int g = 0; g < NG; ++g) {
-      const uint32_t flags = rel[(size_t)c * NG + g];
+      uint32_t flags = rel[(size_t)c * NG + g];
+      const Group& G = groups[g];
+      if (host && G.key == kHostname && G.type == 1 && (flags & KSCHED_TOPO_CONSTRAINS))  // nextDomainAffinity's options
+        for (auto& kv : G.counts)  // a domain with a count that is no existing slot is never counted on the device
+          if (kv.second > 0 && !B.hostname_slot.count(kv.first) && host->has(kv.first)) { flags |= KSCHED_TOPO_HOST_EXTRA; break; }
       if (flags & ~KSCHED_TOPO_SELECTS) E.class_topo.push_back({(uint32_t)g, flags});
     }
     row.topo_end = (uint32_t)E.class_topo.size();
   }
+  hostname_slot_table(B);
   if (!B.vol_drivers.empty()) {
     E.class_volumes.resize(NC);
     bool any = false;
@@ -1870,6 +1996,11 @@ void wire(Builder& B) {
   pr.n_itype_reqs = (int)E.itype_req_complement.size();
   pr.hostname_reqs = E.hostname_reqs.data();
   pr.n_hostname_reqs = (int)E.hostname_reqs.size() / 2;
+  if (E.hostname_words) {
+    pr.hostname_slots = E.hostname_slots.data();
+    pr.n_hostname_words = E.hostname_words;
+    pr.filter_term_hostname = E.filter_term_hostname.empty() ? nullptr : E.filter_term_hostname.data();
+  }
   pr.max_new_nodes = (int)E.pods.size();
   if (!E.class_volumes.empty() && NE > 0) {
     pr.class_volumes = E.class_volumes.data();

@@ -86,6 +86,9 @@ struct Encoded {
   std::vector<uint64_t> itype_req_sets;
   std::vector<uint8_t> itype_req_complement;
   std::vector<int32_t> hostname_reqs;
+  int hostname_words = 0;                             // ksched.h: n_hostname_words; 0 when every entry is a {complement, slot} pair
+  std::vector<uint64_t> hostname_slots;               // [n_hostname_reqs][hostname_words] admitted existing slots; empty without
+  std::vector<uint32_t> filter_term_hostname;         // [n_filter_terms] hostname_reqs entry or KSCHED_NONE; empty when no term names it
   std::vector<ksched_class_volumes> class_volumes;    // CSI volume limits (ksched.h); empty when no pod mounts a limited claim
   std::vector<ksched_node_volumes> existing_volumes;
   uint64_t volume_driver_mask[KSCHED_MAX_VOLUME_DRIVERS] = {};

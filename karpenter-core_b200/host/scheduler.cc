@@ -360,8 +360,9 @@ void kh_encoded_free(Encoded* E) {
   delete E;
 }
 // dims: [pods, classes, existing, groups, types, templates, keys, resources, type_words, class_topo, taintsets, resources_ext,
-//        hostports, hostport_ext_words]
+//        hostports, hostport_ext_words, hostname_reqs, hostname_words]
 void kh_encoded_dims(const Encoded* E, long long* out) {
+  out[14] = (long long)E->hostname_reqs.size() / 2; out[15] = E->hostname_words;
   out[0] = (long long)E->pods.size(); out[1] = (long long)E->classes.size(); out[2] = (long long)E->existing.size();
   out[3] = (long long)E->groups.size(); out[4] = (long long)E->types.size(); out[5] = (long long)E->templates.size();
   out[6] = (long long)E->key_names.size(); out[7] = (long long)E->res_names.size() - E->n_res_ext; out[8] = E->type_words;
@@ -374,6 +375,32 @@ int kh_encoded_hostport(const Encoded* E, int id, char* out, int cap) {
   if (id < 0 || (size_t)id >= E->hostports.size() || (int)E->hostports[(size_t)id].size() >= cap) return -1;
   std::memcpy(out, E->hostports[(size_t)id].c_str(), E->hostports[(size_t)id].size() + 1);
   return 0;
+}
+// Hostname requirement `i` of an encoding (ksched.h: hostname_reqs) into out[cap] (tests): out[0] = 1 when it admits new
+// nodes, then the existing slots it admits in ascending order. Returns the number of slots, -1 when there is no such
+// requirement, -2 when out is too small.
+int kh_encoded_hostname_req(const Encoded* E, int i, long long* out, int cap) {
+  if (i < 0 || (size_t)i >= E->hostname_reqs.size() / 2 || cap < 1) return -1;
+  const int32_t a = E->hostname_reqs[2 * (size_t)i], b = E->hostname_reqs[2 * (size_t)i + 1];
+  const int NE = (int)E->existing.size(), W = E->hostname_words;
+  int k = 0;
+  out[k++] = a != 0;  // the pair's complement admits a new node exactly as the table entry's flag does
+  for (int e = 0; e < NE; ++e) {
+    const bool in = b == KSCHED_HOSTNAME_TABLE ? ((E->hostname_slots[(size_t)i * W + e / 64] >> (e % 64)) & 1) != 0 : (e == b) != (a != 0);
+    if (!in) continue;
+    if (k >= cap) return -2;
+    out[k++] = e;
+  }
+  return k - 1;
+}
+// initial class of pod i of Solve's pod list (tests), -1 out of range
+long long kh_encoded_pod_class(const Encoded* E, int i) {
+  return i < 0 || (size_t)i >= E->pod_class.size() ? -1 : (long long)E->pod_class[(size_t)i];
+}
+// hostname_reqs entry of class c's row, or -1 without a hostname requirement (tests)
+long long kh_encoded_class_hostname(const Encoded* E, int c) {
+  if (c < 0 || (size_t)c >= E->classes.size() || E->classes[(size_t)c].hostname_req == KSCHED_NONE) return -1;
+  return E->classes[(size_t)c].hostname_req;
 }
 void kh_encoded_set_count_visited(Encoded* E, int on) { E->problem.count_nodes_visited = on; }
 const ksched_catalog* kh_encoded_catalog(const Encoded* E) { return &E->catalog; }
@@ -1320,6 +1347,7 @@ extern "C" unsigned long long kh_encoded_digest(const Encoded* E) {
   if (E->hostport_ext_words) {  // absent with at most 64 host-port entries: those digests predate the entry tables
     vec(E->class_hostport_conflicts_ext); vec(E->class_hostport_entries_ext); vec(E->existing_hostport_ext);
   }
+  if (E->hostname_words) { vec(E->hostname_slots); vec(E->filter_term_hostname); }  // absent without the hostname table: those digests predate it
   if (E->n_res_ext) {  // absent with at most 8 read resources: those digests predate ext resources
     bytes(&E->n_res_ext, sizeof E->n_res_ext);
     vec(E->type_alloc_ext); vec(E->class_requests_ext); vec(E->class_res_ext_present); vec(E->existing_available_ext);

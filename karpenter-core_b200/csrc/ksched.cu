@@ -176,6 +176,12 @@ struct DevBuf {
 
 }  // namespace
 
+// Every array a Solve mutates goes back to its pristine copy (or to zero) in ONE launch: a table of (dst, src, bytes)
+// segments passed by value (reset_kernel). (Round 1 issued ~20 cudaMemcpyAsync / cudaMemsetAsync calls per Solve; a
+// consolidation simulation is so short that those launches were most of it.)
+struct ResetSeg { void* dst; const void* src; unsigned long long bytes; };
+struct ResetTable { int n; ResetSeg seg[30]; };
+
 struct ksched_handle {
   K1Params k1_host;  // staging copies of the kernels' constant-memory parameters (must outlive the async copies)
   K2Params k2_host;  // staging copy of the pack kernel's constant-memory parameters (must outlive the async copy)
@@ -183,34 +189,78 @@ struct ksched_handle {
   int n_sm = 132;  // streaming multiprocessors of `device` (grid sizes of the grid-stride kernels)
   cudaStream_t stream = nullptr;
   std::string err;
-  // catalog
+  // ---- catalog (ksched_load_catalog): `cat` points into the buffers of this group
   bool have_catalog = false;
   DevCatalog cat{};
-  int W64 = 0;
+  int n_valrows = 1, n_offrows = 1;  // rows of cat.valset / cat.offset
+  std::vector<ksched_template> h_templates;
+  std::vector<unsigned char> catalog_blob;  // host copy of the resident catalog's inputs (ksched_load_catalog early-out)
   DevBuf<ksched_keyinfo> d_keys;
-  DevBuf<int64_t> d_key_int, d_capacity, d_alloc_sorted;
   DevBuf<ksched_key_regions> d_key_regions;
+  DevBuf<ksched_template> d_templates;
+  DevBuf<ksched_type_row> d_types;
+  DevBuf<int64_t> d_key_int, d_capacity, d_alloc_sorted, d_alloc_rt, d_alloc_ext;
+  DevBuf<float> d_price32;
+  DevBuf<int16_t> d_valrow, d_offrow;
+  DevBuf<int32_t> d_perm_desc;
+  DevBuf<uint32_t> d_valset, d_absent, d_negempty, d_offset, d_anyoffer, d_member, d_fitset, d_domset, d_input_index;
+  DevBuf<uint64_t> d_offer_keys;
+  // ---- problem (ksched_upload): `st` points into the buffers of this group; reset_state restores the `resets` segments
+  bool uploaded = false;
+  bool sorted = false;  // the FFD-ordered pod-row matrix of the uploaded problem exists
+  PackState st{};
+  ResetTable resets{};
+  // one-pass queue order (feasibility_kernel.cuh: sort_key1_kernel): total key bits, 0 = the three-key path
+  int sort1_bits = 0, sort1_ts_bits = 0, sort1_uid_bits = 0;
+  long long sort1_ts_min = 0;
+  size_t cub_tmp_bytes = 0;
+  // inputs
+  DevBuf<ksched_pod_row> d_classes;
+  DevBuf<ksched_topo_group> d_groups;
+  DevBuf<ksched_class_topo> d_class_topo;
+  DevBuf<RelX> d_relx;
+  DevBuf<ksched_reqset> d_filter_terms;
   DevBuf<ksched_class_volumes> d_cls_vol;
-  DevBuf<int32_t> d_cls_cursor;
-  DevBuf<uint64_t> d_cls_tol_ext;  // [n_classes][tol_ext_words] taint sets from id 64 on (ksched_problem.class_tolerated_ext)
-  int tol_ext_words = 0;
-  // host-port entries from id 64 on (ksched_problem.class_hostport_conflicts_ext); allocated only when the problem has some
-  DevBuf<uint64_t> d_cls_hpc_ext, d_cls_hpe_ext;  // [n_classes][hp_ext_words]
-  DevBuf<uint8_t> d_cls_hp_ext;                   // [n_classes] 1: the class has a conflict or an entry from id 64 on
-  DevBuf<uint64_t> d_ex_hp_ext, d_ex_hp_ext0;     // [hp_ext_words][n_existing] working copy / pristine copy
-  DevBuf<uint64_t> d_nn_hp_ext;                   // [hp_ext_words][max_new]
-  int hp_ext_words = 0;
-  // hostname requirement table (ksched_problem.hostname_slots); allocated only when the problem has one
-  DevBuf<uint64_t> d_hostname_slots;  // [n_hostname_reqs][hostname_words]
-  DevBuf<uint32_t> d_filter_hostname; // [n_filter_terms]
-  int hostname_words = 0;
-  bool filter_hostname = false;
-  // ext resources (ksched.h: ksched_catalog.n_res_ext); allocated only when the catalog has some
-  DevBuf<int64_t> d_alloc_ext, d_cls_req_ext, d_ex_avail_ext, d_ex_req_ext, d_nn_req_ext;
-  DevBuf<uint32_t> d_cls_ext_present, d_nn_ext_present;
-  // device-resident cluster snapshot (ksched_load_cluster)
+  DevBuf<int32_t> d_hostname_reqs, d_grp_host_row;
+  DevBuf<int64_t> d_ts, d_ex_avail, d_cls_req_ext, d_ex_avail_ext;
+  DevBuf<uint8_t> d_itype_comp, d_cls_hp_ext;
+  DevBuf<uint32_t> d_pod_class0, d_uid_rank, d_itype_sets, d_filter_hostname, d_cls_rank, d_cls_ext_present, d_ex_avail_present, d_ex_taintset,
+      d_ex_itype;
+  DevBuf<uint64_t> d_hostname_slots, d_cls_tol_ext, d_cls_hpc_ext, d_cls_hpe_ext;
+  // pristine copies of what a Solve mutates
+  DevBuf<ksched_node_volumes> d_ex_vol0;
+  DevBuf<int32_t> d_grp_cnt0, d_grp_host_total0;
+  DevBuf<int64_t> d_ex_req0;
+  DevBuf<uint8_t> d_grp_active0;
+  DevBuf<uint16_t> d_grp_host0;
+  DevBuf<uint32_t> d_ex_req_present0;
+  DevBuf<uint64_t> d_ex_vals0, d_ex_meta0, d_ex_hp0, d_ex_hp_ext0, d_grp_registered0;
+  // working state
+  DevBuf<ksched_node_volumes> d_ex_vol;
+  DevBuf<int32_t> d_relax, d_assign, d_place_seq, d_last_len, d_cls_cursor, d_grp_cnt, d_grp_host_total, d_grp_min_slot;
+  DevBuf<int64_t> d_ex_req, d_ex_req_ext, d_remaining;
+  DevBuf<uint8_t> d_ex_closed, d_grp_active;
+  DevBuf<uint16_t> d_grp_host;
+  DevBuf<uint32_t> d_pod_class, d_queue, d_last_epoch, d_ex_req_present;
+  DevBuf<uint64_t> d_ex_vals, d_ex_meta, d_ex_hp, d_ex_hp_ext, d_grp_registered;
+  DevBuf<long long> d_counters;  // kNumCounters entries (Counter)
+  // K0 / K1
+  DevBuf<uint32_t> d_order, d_idx_tmp, d_pod_pos, d_F, d_Fclass;
+  DevBuf<uint64_t> d_k_cpu, d_k_mem, d_k_tie, d_k_tmp, d_rows;
+  DevBuf<unsigned long long> d_best, d_best_class;
+  DevBuf<uint8_t> d_cub_tmp;
+  // new nodes, open-node overflow and the fresh-node memos (PackState)
+  DevBuf<int32_t> d_nn_count, d_nn_tb, d_ov_node;
+  DevBuf<int64_t> d_nn_req, d_nn_req_ext;
+  DevBuf<uint8_t> d_nn_tmpl, d_fc_state, d_fc_dom, d_fc_front_state, d_fd_state, d_fd_dom;
+  DevBuf<uint32_t> d_nn_req_present, d_nn_opts, d_nn_ext_present, d_ov_absorbed, d_ov_rejected, d_fc_opts, d_fc_qp, d_fd_fc, d_fd_opts;
+  DevBuf<uint64_t> d_nn_vals, d_nn_meta, d_nn_hp, d_nn_hp_ext, d_fc_vals, d_fc_meta, d_fd_meta, d_fd_vals;
+  DevBuf<unsigned long long> d_ov_key;
+  DevBuf<unsigned short> d_ov_flags;
+  DevBuf<long long> d_ov_q, d_ov_bound, d_ov_bound2, d_fc_bound, d_fc_bound2, d_fc_q, d_fd_bound, d_fd_bound2;
+  DevBuf<VarStoreEntry> d_vstore;
+  // ---- device-resident cluster snapshot (ksched_load_cluster)
   bool have_cluster = false;
-  int stop_new_nodes = 0;
   int sup_pods = 0, sup_pending = 0;
   std::vector<int32_t> h_node_first, h_node_count;   // per existing slot: first superset pod bound to it, how many
   DevBuf<int32_t> d_sup_pod_node, d_node_first, d_node_dst, d_set_nodes, d_pod_src;
@@ -224,68 +274,15 @@ struct ksched_handle {
   DevBuf<ksched_count_rel> d_cc;
   DevBuf<int8_t> d_node_dom;
   DevBuf<uint8_t> d_node_hostlabel;
-  DevBuf<uint8_t> d_gather_send, d_gather_recv;
+  // ---- candidate ranking (ksched_rank_candidates)
   DevBuf<int32_t> d_rk_off, d_rk_prio, d_rk_order, d_rk_n;
   DevBuf<double> d_rk_dc, d_rk_age, d_rk_ttl, d_rk_cost_in, d_rk_cost, d_rk_cost_out;
   DevBuf<uint8_t> d_rk_flags, d_rk_elig_in, d_rk_elig;
-  DevBuf<ksched_node_volumes> d_ex_vol, d_ex_vol0;
-  bool have_volumes = false;
-  uint64_t vol_mask[KSCHED_MAX_VOLUME_DRIVERS] = {};
-  DevBuf<ksched_template> d_templates;
-  DevBuf<ksched_type_row> d_types;
-  DevBuf<float> d_price32;
-  DevBuf<int16_t> d_valrow, d_offrow;
-  DevBuf<uint32_t> d_valset, d_absent, d_negempty, d_offset, d_anyoffer, d_member, d_fitset, d_domset, d_input_index;
-  DevBuf<uint64_t> d_offer_keys;
+  // ---- launch choices, all-gather, L2 flush, K1 profile
   DevBuf<ksched_launch_choice> d_launch;
-  std::vector<ksched_template> h_templates;
-  std::vector<unsigned char> catalog_blob;  // host copy of the resident catalog's inputs (ksched_load_catalog early-out)
-  int n_valrows = 1, n_offrows = 1;
-  // problem
-  bool uploaded = false;
-  bool sorted = false;  // the FFD-ordered pod-row matrix of the uploaded problem exists
-  int n_pods = 0, n_classes = 0, n_existing = 0, n_groups = 0, max_new = 0, n_hostgroups = 0;
-  DevBuf<ksched_pod_row> d_classes;
-  DevBuf<uint32_t> d_pod_pos, d_pod_class0, d_pod_class, d_uid_rank, d_order, d_idx_tmp, d_itype_sets, d_queue, d_last_epoch;
-  DevBuf<int64_t> d_ts;
-  DevBuf<uint64_t> d_k_cpu, d_k_mem, d_k_tie, d_k_tmp, d_rows;
-  DevBuf<uint8_t> d_cub_tmp, d_itype_comp, d_ex_closed, d_nn_tmpl;
-  DevBuf<ksched_topo_group> d_groups;
-  DevBuf<ksched_class_topo> d_class_topo;
-  DevBuf<RelX> d_relx;
-  DevBuf<ksched_reqset> d_filter_terms;
-  DevBuf<int32_t> d_hostname_reqs, d_relax, d_assign, d_place_seq, d_last_len, d_nn_count, d_nn_tb, d_ov_node, d_perm_desc, d_grp_cnt,
-      d_grp_cnt0, d_grp_host_row, d_grp_host_total, d_grp_host_total0;
-  DevBuf<uint32_t> d_F, d_Fclass;
-  DevBuf<unsigned long long> d_best_class;
-  DevBuf<unsigned long long> d_best;
-  DevBuf<int64_t> d_ex_req, d_ex_req0, d_ex_avail, d_nn_req, d_remaining, d_alloc_rt;
-  DevBuf<long long> d_ov_q, d_ov_bound, d_ov_bound2, d_fc_bound, d_fc_bound2;
-  DevBuf<unsigned long long> d_ov_key;
-  DevBuf<unsigned short> d_ov_flags;
-  DevBuf<uint8_t> d_fc_state, d_fc_dom, d_fc_front_state, d_grp_active, d_grp_active0;
-  DevBuf<int32_t> d_grp_min_slot;
-  DevBuf<uint32_t> d_fc_opts, d_fc_qp, d_ov_absorbed, d_ov_rejected;
-  DevBuf<uint64_t> d_fc_vals, d_fc_meta;
-  DevBuf<long long> d_fc_q;
-  DevBuf<uint8_t> d_fd_state, d_fd_dom;
-  DevBuf<uint32_t> d_fd_fc, d_fd_opts;
-  DevBuf<uint64_t> d_fd_meta, d_fd_vals;
-  DevBuf<long long> d_fd_bound, d_fd_bound2;
-  DevBuf<VarStoreEntry> d_vstore;
-  int count_visited = 1;
-  DevBuf<uint32_t> d_ex_req_present, d_ex_req_present0, d_ex_avail_present, d_ex_taintset, d_ex_itype, d_nn_req_present, d_nn_opts;
-  DevBuf<uint64_t> d_ex_vals, d_ex_vals0, d_ex_meta, d_ex_meta0, d_ex_hp, d_ex_hp0, d_nn_vals, d_nn_meta, d_nn_hp, d_grp_registered,
-      d_grp_registered0;
-  DevBuf<uint16_t> d_grp_host, d_grp_host0;
-  DevBuf<long long> d_counters, d_k1dbg;  // d_counters: kNumCounters entries (Counter)
+  DevBuf<uint8_t> d_gather_send, d_gather_recv;
   DevBuf<uint32_t> d_flush;
-  size_t cub_tmp_bytes = 0;
-  // one-pass queue order (feasibility_kernel.cuh: sort_key1_kernel): total key bits, 0 = the three-key path
-  int sort1_bits = 0, sort1_ts_bits = 0, sort1_uid_bits = 0;
-  long long sort1_ts_min = 0;
-  DevBuf<uint32_t> d_cls_rank;
-  int64_t min_req[KSCHED_MAX_RES] = {0};
+  DevBuf<long long> d_k1dbg;
   // sharding / nccl
   int rank = 0, world = 1;
   ncclComm_t comm = nullptr;
@@ -304,6 +301,57 @@ static cudaError_t upload(ksched_handle* h, DevBuf<T>& buf, const T* src, size_t
 }
 template <class T>
 static cudaError_t upload_vec(ksched_handle* h, DevBuf<T>& buf, const std::vector<T>& v) { return upload(h, buf, v.data(), v.size()); }
+
+template <class T>
+static cudaError_t download(ksched_handle* h, T* dst, const T* src, size_t n) {
+  h->tm.d2h_bytes += (int64_t)(n * sizeof(T));
+  return cudaMemcpyAsync(dst, src, n * sizeof(T), cudaMemcpyDeviceToHost, h->stream);
+}
+// The first n columns of a device SoA array [rows][pitch] (new nodes), packed to [rows][n] on the host.
+template <class T>
+static cudaError_t download_soa(ksched_handle* h, std::vector<T>& dst, const T* src, int rows, size_t pitch, int n) {
+  dst.resize((size_t)rows * n);
+  h->tm.d2h_bytes += (int64_t)(dst.size() * sizeof(T));
+  return cudaMemcpy2DAsync(dst.data(), (size_t)n * sizeof(T), src, pitch * sizeof(T), (size_t)n * sizeof(T), rows, cudaMemcpyDeviceToHost, h->stream);
+}
+// Node i's entries of a host copy [rows][n] of a SoA array, to row_of(i)[0 .. rows).
+template <class T, class RowOf>
+static void soa_to_rows(const std::vector<T>& soa, int rows, int n, RowOf row_of) {
+  for (int i = 0; i < n; ++i) {
+    T* row = row_of(i);
+    for (int r = 0; r < rows; ++r) row[r] = soa[(size_t)r * n + i];
+  }
+}
+
+static cudaError_t record_reset(ResetTable& t, void* dst, const void* src, size_t bytes) {
+  if (!bytes) return cudaSuccess;
+  if (t.n == (int)(sizeof t.seg / sizeof t.seg[0])) return cudaErrorInvalidValue;  // ResetTable::seg is too small
+  t.seg[t.n++] = ResetSeg{dst, src, (unsigned long long)bytes};
+  return cudaSuccess;
+}
+
+// One device array of the catalog or the problem: sized for n elements, `src` uploaded when given, and `field` (a DevCatalog
+// or PackState pointer) bound to it.
+template <class T, class F>
+static cudaError_t bind(ksched_handle* h, DevBuf<T>& buf, F*& field, size_t n, const T* src = nullptr) {
+  const cudaError_t e = src ? upload(h, buf, src, n) : buf.ensure(n);
+  field = buf.ptr;
+  return e;
+}
+// An array the pack kernel mutates: bound like bind(), with its pristine copy in `init` (uploaded from `src` when given,
+// otherwise filled by the caller) and restored from it by reset_state before every run.
+template <class T, class F>
+static cudaError_t bind_restored(ksched_handle* h, DevBuf<T>& buf, F*& field, DevBuf<T>& init, size_t n, const T* src = nullptr) {
+  cudaError_t e = src ? upload(h, init, src, n) : init.ensure(n);
+  if (e == cudaSuccess) e = bind(h, buf, field, n);
+  return e == cudaSuccess ? record_reset(h->resets, buf.ptr, init.ptr, n * sizeof(T)) : e;
+}
+// An array the pack kernel mutates that reset_state clears before every run.
+template <class T, class F>
+static cudaError_t bind_zeroed(ksched_handle* h, DevBuf<T>& buf, F*& field, size_t n) {
+  const cudaError_t e = bind(h, buf, field, n);
+  return e == cudaSuccess ? record_reset(h->resets, buf.ptr, nullptr, n * sizeof(T)) : e;
+}
 
 static int type_words64(int n_types) { int w = (n_types + 63) / 64; return w ? w : 1; }
 
@@ -362,8 +410,8 @@ void ksched_destroy(ksched_handle* h) {
 const char* ksched_last_error(const ksched_handle* h) { return h ? h->err.c_str() : "null handle"; }
 
 
-int ksched_load_catalog(ksched_handle* h, const ksched_catalog* cat) {
-  if (!h || !cat) return KSCHED_ERR_INVALID;
+// Every refusal of ksched_load_catalog, before it touches the handle (h->err aside).
+static int check_catalog(ksched_handle* h, const ksched_catalog* cat) {
   if (cat->n_keys > KSCHED_MAX_KEYS || cat->n_res > KSCHED_MAX_RES || cat->n_templates > KSCHED_MAX_TEMPLATES || cat->n_templates < 1 ||
       cat->n_types < 0) { h->err = "catalog dimensions out of range"; return KSCHED_ERR_INVALID; }
   if (cat->n_res_ext < 0 || cat->n_res_ext > KSCHED_MAX_RES_EXT || (cat->n_res_ext > 0 && (cat->n_res != KSCHED_MAX_RES || !cat->type_alloc_ext))) {
@@ -386,107 +434,125 @@ int ksched_load_catalog(ksched_handle* h, const ksched_catalog* cat) {
       if (g.n_thresholds < 0 || g.n_thresholds > KSCHED_MAX_THRESHOLDS || g.region_shift < 0 || g.region_shift + g.n_thresholds + 1 > 63 ||
           g.region_mask != want || (g.region_mask & cat->keys[k].dict_mask)) { h->err = "inconsistent ksched_key_regions"; return KSCHED_ERR_INVALID; }
     }
-  CUDA_TRY(h, cudaSetDevice(h->device));
-  const int T = cat->n_types, NK = cat->n_keys, V = cat->n_templates, R = cat->n_res;
-  const int W64 = type_words64(T), W32 = W64 * 2;
-  {
-    // Instance types change rarely: when the byte-identical catalog is already resident there is nothing to do (exact
-    // comparison against a host copy; the O(T^2) dominance table alone is milliseconds of host time at T = 1000).
-    std::vector<unsigned char> blob;
-    auto put = [&](const void* p, size_t n) { const unsigned char* b = (const unsigned char*)p; blob.insert(blob.end(), b, b + n); };
-    int dims[4] = {NK, R, T, V};
-    put(dims, sizeof dims);
-    put(cat->keys, sizeof(ksched_keyinfo) * (size_t)NK);
-    unsigned char has_int = cat->key_int_values != nullptr, has_off = cat->offering_keys != nullptr, has_reg = cat->key_regions != nullptr;
-    put(&has_int, 1); put(&has_off, 1); put(&has_reg, 1);
-    if (has_reg) put(cat->key_regions, sizeof(ksched_key_regions) * (size_t)NK);
-    if (has_int) put(cat->key_int_values, sizeof(int64_t) * (size_t)NK * 64);
-    put(cat->types, sizeof(ksched_type_row) * (size_t)T);
-    put(cat->type_capacity, sizeof(int64_t) * (size_t)T * KSCHED_MAX_RES);
-    if (has_off) put(cat->offering_keys, sizeof(uint64_t) * (size_t)T * 64);
-    put(&cat->n_res_ext, sizeof cat->n_res_ext);
-    if (cat->n_res_ext) put(cat->type_alloc_ext, sizeof(int64_t) * (size_t)T * cat->n_res_ext);
-    if (h->have_catalog && blob == h->catalog_blob) {
-      // same instance types: only the templates can differ (remaining provisioner limits move between solves, daemonset
-      // overhead with the daemonsets) - they are small, re-upload them when they changed
-      if (h->h_templates.size() != (size_t)V || std::memcmp(h->h_templates.data(), cat->templates, sizeof(ksched_template) * (size_t)V) != 0) {
-        CUDA_TRY(h, upload(h, h->d_templates, cat->templates, (size_t)V));
-        CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-        h->cat.templates = h->d_templates.ptr;
-        h->h_templates.assign(cat->templates, cat->templates + V);
-      }
-      return KSCHED_OK;
-    }
-    h->catalog_blob.swap(blob);
-  }
-  h->W64 = W64;
-  // ---- bit-sliced tables, built on the host (amortised: instance types change rarely)
-  std::vector<int16_t> valrow((size_t)NK * 64, -1), offrow(64, -1);
-  std::vector<uint32_t> valset, absent((size_t)std::max(NK, 1) * W32, 0), negempty((size_t)std::max(NK, 1) * W32, 0), offset, anyoffer(W32, 0),
-      member((size_t)V * W32, 0);
-  uint32_t type_relevant = 0;
-  int zone_key = -1, ct_key = -1;
-  for (int k = 0; k < NK; ++k) {
-    if (cat->keys[k].is_zone) zone_key = k;
-    if (cat->keys[k].is_capacity_type) ct_key = k;
-  }
-  std::vector<float> price32(std::max(T, 1), 0.f);
-  for (int t = 0; t < T; ++t) {
+  for (int t = 0; t < cat->n_types; ++t) {
     const ksched_type_row& row = cat->types[t];
     if (t > 0 && row.min_price < cat->types[t - 1].min_price) { h->err = "instance types must be in ascending price order"; return KSCHED_ERR_INVALID; }
-    price32[t] = (float)row.min_price;
+    for (int k = 0; k < cat->n_keys; ++k) {
+      const bool complement = (row.meta >> (KSCHED_META_PRESENT_SHIFT + k)) & (row.meta >> (KSCHED_META_COMPLEMENT_SHIFT + k)) & 1;
+      if (complement && !(cat->key_regions && cat->key_regions[k].region_mask)) {
+        h->err = "instance type with a complement requirement on a key without region bits";
+        return KSCHED_ERR_INVALID;
+      }
+    }
+  }
+  return KSCHED_OK;
+}
+
+// The catalog's inputs byte for byte: a catalog equal to the resident one needs no rebuild (ksched_load_catalog).
+static std::vector<unsigned char> catalog_key(const ksched_catalog* cat) {
+  const int NK = cat->n_keys, T = cat->n_types;
+  std::vector<unsigned char> blob;
+  auto put = [&](const void* p, size_t n) { const unsigned char* b = (const unsigned char*)p; blob.insert(blob.end(), b, b + n); };
+  int dims[4] = {NK, cat->n_res, T, cat->n_templates};
+  put(dims, sizeof dims);
+  put(cat->keys, sizeof(ksched_keyinfo) * (size_t)NK);
+  unsigned char has_int = cat->key_int_values != nullptr, has_off = cat->offering_keys != nullptr, has_reg = cat->key_regions != nullptr;
+  put(&has_int, 1); put(&has_off, 1); put(&has_reg, 1);
+  if (has_reg) put(cat->key_regions, sizeof(ksched_key_regions) * (size_t)NK);
+  if (has_int) put(cat->key_int_values, sizeof(int64_t) * (size_t)NK * 64);
+  put(cat->types, sizeof(ksched_type_row) * (size_t)T);
+  put(cat->type_capacity, sizeof(int64_t) * (size_t)T * KSCHED_MAX_RES);
+  if (has_off) put(cat->offering_keys, sizeof(uint64_t) * (size_t)T * 64);
+  put(&cat->n_res_ext, sizeof cat->n_res_ext);
+  if (cat->n_res_ext) put(cat->type_alloc_ext, sizeof(int64_t) * (size_t)T * cat->n_res_ext);
+  return blob;
+}
+
+// DevCatalog's bit-sliced tables, built on the host (amortised: instance types change rarely).
+struct CatalogTables {
+  std::vector<ksched_keyinfo> keys;
+  std::vector<int16_t> valrow, offrow;
+  std::vector<uint32_t> valset, absent, negempty, offset, anyoffer, member, fitset, domset, input_index;
+  std::vector<int32_t> perm_desc;
+  std::vector<int64_t> alloc_rt, alloc_sorted;
+  std::vector<float> price32;
+  uint32_t type_relevant = 0;
+  int zone_key = -1, ct_key = -1;
+  uint64_t pin_neutral[KSCHED_MAX_KEYS] = {};
+};
+
+static void build_catalog(const ksched_catalog* cat, CatalogTables& b) {
+  const int T = cat->n_types, NK = cat->n_keys, V = cat->n_templates, R = cat->n_res;
+  const int W32 = type_words64(T) * 2;
+  // the device's dict_mask includes the region bits: "every admissible value" of a complement requirement then covers the
+  // regions a complement instance type shares with it (catalog.cuh: key_typeset_word walks the admitted bits)
+  b.keys.assign(cat->keys, cat->keys + NK);
+  if (cat->key_regions) for (int k = 0; k < NK; ++k) b.keys[k].dict_mask |= cat->key_regions[k].region_mask;
+  b.valrow.assign((size_t)NK * 64, -1);
+  b.offrow.assign(64, -1);
+  b.absent.assign((size_t)std::max(NK, 1) * W32, 0);
+  b.negempty.assign((size_t)std::max(NK, 1) * W32, 0);
+  b.anyoffer.assign(W32, 0);
+  b.member.assign((size_t)V * W32, 0);
+  for (int k = 0; k < NK; ++k) {
+    if (cat->keys[k].is_zone) b.zone_key = k;
+    if (cat->keys[k].is_capacity_type) b.ct_key = k;
+  }
+  b.price32.assign(std::max(T, 1), 0.f);
+  for (int t = 0; t < T; ++t) {
+    const ksched_type_row& row = cat->types[t];
+    b.price32[t] = (float)row.min_price;
     const int w = t >> 5;
     const uint32_t bit = 1u << (t & 31);
     for (int k = 0; k < NK; ++k) {
       bool present = (row.meta >> (KSCHED_META_PRESENT_SHIFT + k)) & 1;
-      if (!present) { absent[(size_t)k * W32 + w] |= bit; continue; }
-      type_relevant |= 1u << k;
+      if (!present) { b.absent[(size_t)k * W32 + w] |= bit; continue; }
+      b.type_relevant |= 1u << k;
       uint64_t v = row.values[k];
       if ((row.meta >> (KSCHED_META_COMPLEMENT_SHIFT + k)) & 1) {
         // complement requirement (NotIn / Exists / Gt / Lt, region form): the type admits every value and region it does not
         // exclude; its operator is negative (NotIn) when it really excludes a value (requirement.go:186-197)
-        const uint64_t region_mask = cat->key_regions ? cat->key_regions[k].region_mask : 0;
-        if (!region_mask) { h->err = "instance type with a complement requirement on a key without region bits"; return KSCHED_ERR_INVALID; }
+        const uint64_t region_mask = cat->key_regions[k].region_mask;  // check_catalog: set
         ksched::Req r{v, 0, 0, true, true, false, false};
-        if (ksched::req_excluded(r, KeyMeta{0, nullptr, cat->key_regions + k}) != 0) negempty[(size_t)k * W32 + w] |= bit;
+        if (ksched::req_excluded(r, KeyMeta{0, nullptr, cat->key_regions + k}) != 0) b.negempty[(size_t)k * W32 + w] |= bit;
         v = ~v & (cat->keys[k].dict_mask | region_mask);
-      } else if (!v) { negempty[(size_t)k * W32 + w] |= bit; continue; }
+      } else if (!v) { b.negempty[(size_t)k * W32 + w] |= bit; continue; }
       while (v) {
-        int b = __builtin_ctzll(v);
+        int vb = __builtin_ctzll(v);
         v &= v - 1;
-        int16_t& r = valrow[(size_t)k * 64 + b];
-        if (r < 0) { r = (int16_t)(valset.size() / W32); valset.resize(valset.size() + W32, 0); }
-        valset[(size_t)r * W32 + w] |= bit;
+        int16_t& r = b.valrow[(size_t)k * 64 + vb];
+        if (r < 0) { r = (int16_t)(b.valset.size() / W32); b.valset.resize(b.valset.size() + W32, 0); }
+        b.valset[(size_t)r * W32 + w] |= bit;
       }
     }
     uint64_t o = row.offerings;
-    if (o) anyoffer[w] |= bit;
+    if (o) b.anyoffer[w] |= bit;
     while (o) {
-      int b = __builtin_ctzll(o);
+      int ob = __builtin_ctzll(o);
       o &= o - 1;
-      int16_t& r = offrow[b];
-      if (r < 0) { r = (int16_t)(offset.size() / W32); offset.resize(offset.size() + W32, 0); }
-      offset[(size_t)r * W32 + w] |= bit;
+      int16_t& r = b.offrow[ob];
+      if (r < 0) { r = (int16_t)(b.offset.size() / W32); b.offset.resize(b.offset.size() + W32, 0); }
+      b.offset[(size_t)r * W32 + w] |= bit;
     }
-    for (int v = 0; v < V; ++v) if ((row.template_members >> v) & 1) member[(size_t)v * W32 + w] |= bit;
+    for (int v = 0; v < V; ++v) if ((row.template_members >> v) & 1) b.member[(size_t)v * W32 + w] |= bit;
   }
-  if (valset.empty()) valset.resize(W32, 0);
-  if (offset.empty()) offset.resize(W32, 0);
-  std::vector<int32_t> perm_desc((size_t)std::max(R, 1) * std::max(T, 1), 0);
-  std::vector<int64_t> alloc_rt((size_t)std::max(R, 1) * std::max(T, 1), 0);
-  std::vector<int64_t> alloc_sorted((size_t)std::max(R, 1) * std::max(T, 1), 0);
-  std::vector<uint32_t> fitset((size_t)std::max(R, 1) * (T + 1) * W32, 0);
+  if (b.valset.empty()) b.valset.resize(W32, 0);
+  if (b.offset.empty()) b.offset.resize(W32, 0);
+  b.perm_desc.assign((size_t)std::max(R, 1) * std::max(T, 1), 0);
+  b.alloc_rt.assign((size_t)std::max(R, 1) * std::max(T, 1), 0);
+  b.alloc_sorted.assign((size_t)std::max(R, 1) * std::max(T, 1), 0);
+  b.fitset.assign((size_t)std::max(R, 1) * (T + 1) * W32, 0);
   {
     std::vector<int> perm(T);
     for (int r = 0; r < R; ++r) {
       for (int t = 0; t < T; ++t) perm[t] = t;
-      std::stable_sort(perm.begin(), perm.end(), [&](int a, int b) { return cat->types[a].allocatable[r] < cat->types[b].allocatable[r]; });
+      std::stable_sort(perm.begin(), perm.end(), [&](int a, int c) { return cat->types[a].allocatable[r] < cat->types[c].allocatable[r]; });
       for (int i = 0; i < T; ++i) {
-        alloc_sorted[(size_t)r * T + i] = cat->types[perm[i]].allocatable[r];
-        perm_desc[(size_t)r * T + (T - 1 - i)] = perm[i];
-        alloc_rt[(size_t)r * T + i] = cat->types[i].allocatable[r];
+        b.alloc_sorted[(size_t)r * T + i] = cat->types[perm[i]].allocatable[r];
+        b.perm_desc[(size_t)r * T + (T - 1 - i)] = perm[i];
+        b.alloc_rt[(size_t)r * T + i] = cat->types[i].allocatable[r];
       }
-      uint32_t* base = &fitset[(size_t)r * (T + 1) * W32];
+      uint32_t* base = &b.fitset[(size_t)r * (T + 1) * W32];
       for (int i = T - 1; i >= 0; --i) {
         uint32_t* cur = base + (size_t)i * W32;
         std::memcpy(cur, base + (size_t)(i + 1) * W32, W32 * sizeof(uint32_t));
@@ -495,136 +561,151 @@ int ksched_load_catalog(ksched_handle* h, const ksched_catalog* cat) {
     }
   }
   {
-    // the device's dict_mask includes the region bits: "every admissible value" of a complement requirement then covers the
-    // regions a complement instance type shares with it (catalog.cuh: key_typeset_word walks the admitted bits)
-    std::vector<ksched_keyinfo> dev_keys(cat->keys, cat->keys + NK);
-    if (cat->key_regions) for (int k = 0; k < NK; ++k) dev_keys[k].dict_mask |= cat->key_regions[k].region_mask;
-    CUDA_TRY(h, upload_vec(h, h->d_keys, dev_keys));
-    if (cat->key_regions) CUDA_TRY(h, upload(h, h->d_key_regions, cat->key_regions, (size_t)NK));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // dev_keys is a stack vector
-  }
-  if (cat->key_int_values) CUDA_TRY(h, upload(h, h->d_key_int, cat->key_int_values, (size_t)NK * 64));
-  CUDA_TRY(h, upload(h, h->d_templates, cat->templates, (size_t)V));
-  CUDA_TRY(h, upload(h, h->d_types, cat->types, (size_t)T));
-  CUDA_TRY(h, upload(h, h->d_capacity, cat->type_capacity, (size_t)T * KSCHED_MAX_RES));
-  CUDA_TRY(h, upload_vec(h, h->d_price32, price32));
-  CUDA_TRY(h, upload_vec(h, h->d_valrow, valrow));
-  CUDA_TRY(h, upload_vec(h, h->d_offrow, offrow));
-  CUDA_TRY(h, upload_vec(h, h->d_valset, valset));
-  CUDA_TRY(h, upload_vec(h, h->d_absent, absent));
-  CUDA_TRY(h, upload_vec(h, h->d_negempty, negempty));
-  CUDA_TRY(h, upload_vec(h, h->d_offset, offset));
-  CUDA_TRY(h, upload_vec(h, h->d_anyoffer, anyoffer));
-  CUDA_TRY(h, upload_vec(h, h->d_member, member));
-  CUDA_TRY(h, upload_vec(h, h->d_alloc_sorted, alloc_sorted));
-  CUDA_TRY(h, upload_vec(h, h->d_perm_desc, perm_desc));
-  CUDA_TRY(h, upload_vec(h, h->d_alloc_rt, alloc_rt));
-  {
     // dominance bitsets over the first min(R,4) resources (pack kernel: Pareto front of a node's options)
     const int RH = std::min(R, 4);
-    std::vector<uint32_t> domset((size_t)std::max(T, 1) * W32, 0);
+    b.domset.assign((size_t)std::max(T, 1) * W32, 0);
     for (int a = 0; a < T; ++a)
-      for (int b = 0; b < T; ++b) {
+      for (int c = 0; c < T; ++c) {
         bool dom = true;
-        for (int r = 0; r < RH && dom; ++r) dom = cat->types[a].allocatable[r] >= cat->types[b].allocatable[r];
-        if (dom) domset[(size_t)a * W32 + (b >> 5)] |= 1u << (b & 31);
+        for (int r = 0; r < RH && dom; ++r) dom = cat->types[a].allocatable[r] >= cat->types[c].allocatable[r];
+        if (dom) b.domset[(size_t)a * W32 + (c >> 5)] |= 1u << (c & 31);
       }
-    CUDA_TRY(h, upload_vec(h, h->d_domset, domset));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   }
-  CUDA_TRY(h, upload_vec(h, h->d_fitset, fitset));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  h->h_templates.assign(cat->templates, cat->templates + V);
-  h->n_valrows = (int)(valset.size() / W32);
-  h->n_offrows = (int)(offset.size() / W32);
-  DevCatalog& c = h->cat;
-  c.n_keys = NK; c.n_res = R; c.n_types = T; c.n_templates = V; c.W32 = W32;
-  c.keys = h->d_keys.ptr;
-  c.key_int_values = cat->key_int_values ? h->d_key_int.ptr : nullptr;
-  c.key_regions = cat->key_regions ? h->d_key_regions.ptr : nullptr;
-  c.templates = h->d_templates.ptr;
-  c.types = h->d_types.ptr;
-  c.capacity = h->d_capacity.ptr;
-  c.price32 = h->d_price32.ptr;
-  c.valrow = h->d_valrow.ptr; c.valset = h->d_valset.ptr; c.absent = h->d_absent.ptr; c.negempty = h->d_negempty.ptr;
-  c.type_relevant = type_relevant;
-  c.offrow = h->d_offrow.ptr; c.offset = h->d_offset.ptr; c.anyoffer = h->d_anyoffer.ptr; c.member = h->d_member.ptr;
-  c.alloc_sorted = h->d_alloc_sorted.ptr; c.fitset = h->d_fitset.ptr;
-  c.perm_desc = h->d_perm_desc.ptr; c.alloc_rt = h->d_alloc_rt.ptr; c.domset = h->d_domset.ptr;
-  c.offer_keys = nullptr;
-  c.input_index = nullptr;
-  c.n_res_ext = cat->n_res_ext;
-  c.alloc_ext = nullptr;
-  if (cat->n_res_ext > 0 && T > 0) {
-    CUDA_TRY(h, upload(h, h->d_alloc_ext, cat->type_alloc_ext, (size_t)T * cat->n_res_ext));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    c.alloc_ext = h->d_alloc_ext.ptr;
-  }
-  if (cat->offering_keys && T > 0) {
-    std::vector<uint32_t> input_index(T);
-    for (int t = 0; t < T; ++t) input_index[t] = cat->types[t].input_index;
-    CUDA_TRY(h, upload(h, h->d_offer_keys, cat->offering_keys, (size_t)T * 64));
-    CUDA_TRY(h, upload_vec(h, h->d_input_index, input_index));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // input_index is a stack vector
-    c.offer_keys = h->d_offer_keys.ptr;
-    c.input_index = h->d_input_index.ptr;
-  }
-  c.zone_key = zone_key; c.ct_key = ct_key;
+  if (cat->offering_keys)
+    for (int t = 0; t < T; ++t) b.input_index.push_back(cat->types[t].input_index);
   {
     // pin_neutral (catalog.cuh): U = union of every template's member types
+    const int zone_key = b.zone_key, ct_key = b.ct_key;
     std::vector<uint32_t> U(W32, 0);
-    for (int v = 0; v < V; ++v) for (int w = 0; w < W32; ++w) U[w] |= member[(size_t)v * W32 + w];
+    for (int v = 0; v < V; ++v) for (int w = 0; w < W32; ++w) U[w] |= b.member[(size_t)v * W32 + w];
     auto covers = [&](const std::vector<uint32_t>& set) { for (int w = 0; w < W32; ++w) if (U[w] & ~set[w]) return false; return true; };
     auto offer_rows = [&](int ct, int z, std::vector<uint32_t>& acc) {
-      const int16_t r = offrow[ct * 16 + z];
-      if (r >= 0) for (int w = 0; w < W32; ++w) acc[w] |= offset[(size_t)r * W32 + w];
+      const int16_t r = b.offrow[ct * 16 + z];
+      if (r >= 0) for (int w = 0; w < W32; ++w) acc[w] |= b.offset[(size_t)r * W32 + w];
     };
-    for (int k = 0; k < KSCHED_MAX_KEYS; ++k) c.pin_neutral[k] = 0;
     for (int k = 0; k < NK; ++k) {
-      for (int b = 0; b < 64; ++b) {
-        if (!((cat->keys[k].dict_mask >> b) & 1)) continue;
+      for (int d = 0; d < 64; ++d) {
+        if (!((cat->keys[k].dict_mask >> d) & 1)) continue;
         std::vector<uint32_t> set(W32, 0);
-        for (int w = 0; w < W32; ++w) set[w] = absent[(size_t)k * W32 + w];
-        if (valrow[(size_t)k * 64 + b] >= 0) for (int w = 0; w < W32; ++w) set[w] |= valset[(size_t)valrow[(size_t)k * 64 + b] * W32 + w];
+        for (int w = 0; w < W32; ++w) set[w] = b.absent[(size_t)k * W32 + w];
+        if (b.valrow[(size_t)k * 64 + d] >= 0) for (int w = 0; w < W32; ++w) set[w] |= b.valset[(size_t)b.valrow[(size_t)k * 64 + d] * W32 + w];
         bool ok = covers(set);
         if (ok && k == zone_key) {
-          if (b >= 16) ok = false;
+          if (d >= 16) ok = false;
           else if (ct_key >= 0) {
             for (int ct = 0; ct < 4 && ok; ++ct) {
               if (!((cat->keys[ct_key].dict_mask >> ct) & 1)) continue;
               std::vector<uint32_t> acc(W32, 0);
-              offer_rows(ct, b, acc);
+              offer_rows(ct, d, acc);
               ok = covers(acc);
             }
             if (cat->keys[ct_key].dict_mask >> 4) ok = false;
           } else {
             std::vector<uint32_t> acc(W32, 0);
-            for (int ct = 0; ct < 4; ++ct) offer_rows(ct, b, acc);
+            for (int ct = 0; ct < 4; ++ct) offer_rows(ct, d, acc);
             ok = covers(acc);
           }
         }
         if (ok && k == ct_key) {
-          if (b >= 4) ok = false;
+          if (d >= 4) ok = false;
           else if (zone_key >= 0) {
             for (int z = 0; z < 16 && ok; ++z) {
               if (!((cat->keys[zone_key].dict_mask >> z) & 1)) continue;
               std::vector<uint32_t> acc(W32, 0);
-              offer_rows(b, z, acc);
+              offer_rows(d, z, acc);
               ok = covers(acc);
             }
             if (cat->keys[zone_key].dict_mask >> 16) ok = false;
           } else {
             std::vector<uint32_t> acc(W32, 0);
-            for (int z = 0; z < 16; ++z) offer_rows(b, z, acc);
+            for (int z = 0; z < 16; ++z) offer_rows(d, z, acc);
             ok = covers(acc);
           }
         }
-        if (ok) c.pin_neutral[k] |= 1ull << b;
+        if (ok) b.pin_neutral[k] |= 1ull << d;
       }
     }
   }
+}
+
+// Uploads the tables and binds every DevCatalog field to them (ksched_load_catalog's commit).
+static int bind_catalog(ksched_handle* h, const ksched_catalog* cat, const CatalogTables& b) {
+  const int T = cat->n_types, NK = cat->n_keys, V = cat->n_templates;
+  DevCatalog& c = h->cat;
+  c = DevCatalog{};
+  c.n_keys = NK; c.n_res = cat->n_res; c.n_types = T; c.n_templates = V; c.W32 = type_words64(T) * 2;
+  c.type_relevant = b.type_relevant;
+  c.zone_key = b.zone_key; c.ct_key = b.ct_key;
+  std::memcpy(c.pin_neutral, b.pin_neutral, sizeof c.pin_neutral);
+  c.n_res_ext = cat->n_res_ext;
+  CUDA_TRY(h, bind(h, h->d_keys, c.keys, b.keys.size(), b.keys.data()));
+  if (cat->key_regions) CUDA_TRY(h, bind(h, h->d_key_regions, c.key_regions, (size_t)NK, cat->key_regions));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  if (cat->key_int_values) CUDA_TRY(h, bind(h, h->d_key_int, c.key_int_values, (size_t)NK * 64, cat->key_int_values));
+  CUDA_TRY(h, bind(h, h->d_templates, c.templates, (size_t)V, cat->templates));
+  CUDA_TRY(h, bind(h, h->d_types, c.types, (size_t)T, cat->types));
+  CUDA_TRY(h, bind(h, h->d_capacity, c.capacity, (size_t)T * KSCHED_MAX_RES, cat->type_capacity));
+  CUDA_TRY(h, bind(h, h->d_price32, c.price32, b.price32.size(), b.price32.data()));
+  CUDA_TRY(h, bind(h, h->d_valrow, c.valrow, b.valrow.size(), b.valrow.data()));
+  CUDA_TRY(h, bind(h, h->d_offrow, c.offrow, b.offrow.size(), b.offrow.data()));
+  CUDA_TRY(h, bind(h, h->d_valset, c.valset, b.valset.size(), b.valset.data()));
+  CUDA_TRY(h, bind(h, h->d_absent, c.absent, b.absent.size(), b.absent.data()));
+  CUDA_TRY(h, bind(h, h->d_negempty, c.negempty, b.negempty.size(), b.negempty.data()));
+  CUDA_TRY(h, bind(h, h->d_offset, c.offset, b.offset.size(), b.offset.data()));
+  CUDA_TRY(h, bind(h, h->d_anyoffer, c.anyoffer, b.anyoffer.size(), b.anyoffer.data()));
+  CUDA_TRY(h, bind(h, h->d_member, c.member, b.member.size(), b.member.data()));
+  CUDA_TRY(h, bind(h, h->d_alloc_sorted, c.alloc_sorted, b.alloc_sorted.size(), b.alloc_sorted.data()));
+  CUDA_TRY(h, bind(h, h->d_perm_desc, c.perm_desc, b.perm_desc.size(), b.perm_desc.data()));
+  CUDA_TRY(h, bind(h, h->d_alloc_rt, c.alloc_rt, b.alloc_rt.size(), b.alloc_rt.data()));
+  CUDA_TRY(h, bind(h, h->d_domset, c.domset, b.domset.size(), b.domset.data()));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, bind(h, h->d_fitset, c.fitset, b.fitset.size(), b.fitset.data()));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  if (cat->n_res_ext > 0 && T > 0) {
+    CUDA_TRY(h, bind(h, h->d_alloc_ext, c.alloc_ext, (size_t)T * cat->n_res_ext, cat->type_alloc_ext));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  }
+  if (cat->offering_keys && T > 0) {
+    CUDA_TRY(h, bind(h, h->d_offer_keys, c.offer_keys, (size_t)T * 64, cat->offering_keys));
+    CUDA_TRY(h, bind(h, h->d_input_index, c.input_index, b.input_index.size(), b.input_index.data()));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  }
+  return KSCHED_OK;
+}
+
+int ksched_load_catalog(ksched_handle* h, const ksched_catalog* cat) {
+  if (!h || !cat) return KSCHED_ERR_INVALID;
+  int rc = check_catalog(h, cat);
+  if (rc != KSCHED_OK) return rc;
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  const int V = cat->n_templates;
+  // Instance types change rarely: when the byte-identical catalog is already resident there is nothing to do (exact
+  // comparison against a host copy; the O(T^2) dominance table alone is milliseconds of host time at T = 1000).
+  std::vector<unsigned char> blob = catalog_key(cat);
+  if (h->have_catalog && blob == h->catalog_blob) {
+    // same instance types: only the templates can differ (remaining provisioner limits move between solves, daemonset
+    // overhead with the daemonsets) - they are small, re-upload them when they changed
+    if (std::memcmp(h->h_templates.data(), cat->templates, sizeof(ksched_template) * (size_t)V) != 0) {
+      const bool uploaded = h->uploaded;
+      h->have_catalog = h->uploaded = false;  // until the new templates are on the device
+      CUDA_TRY(h, bind(h, h->d_templates, h->cat.templates, (size_t)V, cat->templates));
+      CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+      h->h_templates.assign(cat->templates, cat->templates + V);
+      h->have_catalog = true;
+      h->uploaded = uploaded;
+    }
+    return KSCHED_OK;
+  }
+  CatalogTables tables;
+  build_catalog(cat, tables);
+  // a new catalog drops the resident problem; a CUDA error part-way through leaves neither
+  h->have_catalog = h->uploaded = false;
+  if ((rc = bind_catalog(h, cat, tables)) != KSCHED_OK) return rc;
+  h->n_valrows = (int)(tables.valset.size() / h->cat.W32);
+  h->n_offrows = (int)(tables.offset.size() / h->cat.W32);
+  h->h_templates.assign(cat->templates, cat->templates + V);
+  h->catalog_blob.swap(blob);
   h->have_catalog = true;
-  h->uploaded = false;
   return KSCHED_OK;
 }
 
@@ -680,17 +761,23 @@ int ksched_allgather(ksched_handle* h, const void* send, size_t bytes, void* rec
   return KSCHED_OK;
 }
 
-// ---- upload one problem (pods / nodes / topology) and keep pristine copies of everything the pack kernel mutates
-int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
-  if (!h || !pb) return KSCHED_ERR_INVALID;
+// The tables of one optional input are set exactly when its count is positive. `omittable` may also stay NULL then: a
+// per-existing-node table without existing nodes, or a table that only some entries read.
+static bool present_iff(bool positive, std::initializer_list<const void*> tables, const void* omittable, bool may_omit) {
+  for (const void* t : tables)
+    if ((t != nullptr) != positive) return false;
+  return omittable ? positive : !positive || may_omit;
+}
+
+// Every refusal of ksched_upload, before it touches the handle (h->err aside).
+static int check_problem(ksched_handle* h, const ksched_problem* pb) {
   if (!h->have_catalog) { h->err = "ksched_load_catalog must be called first"; return KSCHED_ERR_INVALID; }
   if (pb->class_bounds || pb->existing_bounds) { h->err = "bounds arrays must be NULL: Gt/Lt requirements are passed in region form (ksched_key_regions)"; return KSCHED_ERR_INVALID; }
-  for (int i = 0; i < pb->n_classes; ++i)
-    if (pb->classes[i].meta >> KSCHED_META_HASGT_SHIFT) { h->err = "requirement with HASGT/HASLT set: pass Gt/Lt in region form"; return KSCHED_ERR_INVALID; }
-  for (int i = 0; i < pb->n_existing; ++i)
-    if (pb->existing[i].reqs.meta >> KSCHED_META_HASGT_SHIFT) { h->err = "requirement with HASGT/HASLT set: pass Gt/Lt in region form"; return KSCHED_ERR_INVALID; }
-  for (int i = 0; i < pb->n_filter_terms; ++i)
-    if (pb->filter_terms[i].meta >> KSCHED_META_HASGT_SHIFT) { h->err = "requirement with HASGT/HASLT set: pass Gt/Lt in region form"; return KSCHED_ERR_INVALID; }
+  bool hasgt = false;
+  for (int i = 0; i < pb->n_classes; ++i) hasgt = hasgt || pb->classes[i].meta >> KSCHED_META_HASGT_SHIFT;
+  for (int i = 0; i < pb->n_existing; ++i) hasgt = hasgt || pb->existing[i].reqs.meta >> KSCHED_META_HASGT_SHIFT;
+  for (int i = 0; i < pb->n_filter_terms; ++i) hasgt = hasgt || pb->filter_terms[i].meta >> KSCHED_META_HASGT_SHIFT;
+  if (hasgt) { h->err = "requirement with HASGT/HASLT set: pass Gt/Lt in region form"; return KSCHED_ERR_INVALID; }
   {
     // taint sets from id 64 on: existing nodes only, each covered by the per-class table
     const int tol_words = pb->class_tolerated_ext ? pb->n_tolerated_ext_words : 0;
@@ -701,23 +788,15 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
         return KSCHED_ERR_INVALID;
       }
   }
-  {
-    // host-port entries from id 64 on: the three tables exist exactly when the count is positive
-    const int hw = pb->n_hostport_ext_words;
-    const bool any = pb->class_hostport_conflicts_ext || pb->class_hostport_entries_ext || pb->existing_hostport_ext;
-    if (hw < 0 || (hw > 0 ? !(pb->class_hostport_conflicts_ext && pb->class_hostport_entries_ext && (pb->existing_hostport_ext || pb->n_existing == 0))
-                          : any)) {
-      h->err = "host-port entry tables must be set exactly when n_hostport_ext_words is positive";
-      return KSCHED_ERR_INVALID;
-    }
+  const int NE = pb->n_existing, HP = pb->n_hostport_ext_words, HW = pb->n_hostname_words, X = h->cat.n_res_ext;
+  if (HP < 0 || !present_iff(HP > 0, {pb->class_hostport_conflicts_ext, pb->class_hostport_entries_ext}, pb->existing_hostport_ext, NE == 0)) {
+    h->err = "host-port entry tables must be set exactly when n_hostport_ext_words is positive";
+    return KSCHED_ERR_INVALID;
   }
   {
-    // hostname requirement table: set exactly when the count is positive, wide enough for every existing slot, and present
-    // when an entry or a filter term reads it
-    const int hw = pb->n_hostname_words;
-    bool ok = hw >= 0 && (hw > 0) == (pb->hostname_slots != nullptr) && (hw > 0 || !pb->filter_term_hostname) &&
-              (hw == 0 || (int64_t)hw * 64 >= pb->n_existing);
-    for (int i = 0; ok && i < pb->n_hostname_reqs; ++i) ok = pb->hostname_reqs[2 * i + 1] != KSCHED_HOSTNAME_TABLE || hw > 0;
+    // hostname requirement table: wide enough for every existing slot, and present when an entry reads it
+    bool ok = HW >= 0 && present_iff(HW > 0, {pb->hostname_slots}, pb->filter_term_hostname, true) && (HW == 0 || (int64_t)HW * 64 >= NE);
+    for (int i = 0; ok && i < pb->n_hostname_reqs; ++i) ok = pb->hostname_reqs[2 * i + 1] != KSCHED_HOSTNAME_TABLE || HW > 0;
     for (int f = 0; ok && pb->filter_term_hostname && f < pb->n_filter_terms; ++f)
       ok = pb->filter_term_hostname[f] == KSCHED_NONE || pb->filter_term_hostname[f] < (uint32_t)pb->n_hostname_reqs;
     if (!ok) {
@@ -725,70 +804,73 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
       return KSCHED_ERR_INVALID;
     }
   }
-  {
-    // ext resources: the tables exist exactly when the catalog has ext resources, and name no resource beyond them
-    const int X = h->cat.n_res_ext;
-    const bool any = pb->class_requests_ext || pb->class_res_ext_present || pb->existing_available_ext;
-    if (X > 0 ? !(pb->class_requests_ext && pb->class_res_ext_present && (pb->existing_available_ext || pb->n_existing == 0)) : any) {
-      h->err = "ext resource tables must be set exactly when the catalog has ext resources";
-      return KSCHED_ERR_INVALID;
-    }
-    for (int c2 = 0; c2 < (X > 0 ? pb->n_classes : 0); ++c2)
-      if (pb->class_res_ext_present[c2] >> X) { h->err = "class_res_ext_present names an ext resource beyond n_res_ext"; return KSCHED_ERR_INVALID; }
+  // ext resources: the tables exist exactly when the catalog has ext resources, and name no resource beyond them
+  if (!present_iff(X > 0, {pb->class_requests_ext, pb->class_res_ext_present}, pb->existing_available_ext, NE == 0)) {
+    h->err = "ext resource tables must be set exactly when the catalog has ext resources";
+    return KSCHED_ERR_INVALID;
   }
-  CUDA_TRY(h, cudaSetDevice(h->device));
-  // the superset buffers ksched_load_cluster filled are about to be overwritten: simulations need a new ksched_load_cluster
-  h->have_cluster = false;
-  h->tm.h2d_bytes = 0;
-  const DevCatalog& c = h->cat;
-  const int P = pb->n_pods, NC = pb->n_classes, NE = pb->n_existing, NG = pb->n_groups, W32 = c.W32, V = c.n_templates;
-  const int MAXN = std::max(1, std::min(pb->max_new_nodes > 0 ? pb->max_new_nodes : P, std::max(P, 1)));
-  h->n_pods = P; h->n_classes = NC; h->n_existing = NE; h->n_groups = NG; h->max_new = MAXN;
-  h->count_visited = pb->count_nodes_visited;
-  for (int c2 = 0; c2 < NC; ++c2) {
-    const ksched_pod_row& row = pb->classes[c2];
+  for (int c = 0; c < (X > 0 ? pb->n_classes : 0); ++c)
+    if (pb->class_res_ext_present[c] >> X) { h->err = "class_res_ext_present names an ext resource beyond n_res_ext"; return KSCHED_ERR_INVALID; }
+  const int NC = pb->n_classes, NG = pb->n_groups;
+  for (int e = 0; e < pb->n_class_topo; ++e)
+    if (pb->class_topo[e].group >= (uint32_t)NG) { h->err = "class_topo group out of range"; return KSCHED_ERR_INVALID; }
+  for (int c = 0; c < NC; ++c) {
+    const ksched_pod_row& row = pb->classes[c];
     if (row.relax_next != KSCHED_NONE && row.relax_next >= (uint32_t)NC) { h->err = "relax_next out of range"; return KSCHED_ERR_INVALID; }
     if (row.topo_end < row.topo_begin || row.topo_end > (uint32_t)pb->n_class_topo) { h->err = "class_topo range out of bounds"; return KSCHED_ERR_INVALID; }
     int ncg = 0, touched = __builtin_popcountll((row.meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF);
-    for (uint32_t e = row.topo_begin; e < row.topo_end; ++e) {
-      if (pb->class_topo[e].group >= (uint32_t)NG) { h->err = "class_topo group out of range"; return KSCHED_ERR_INVALID; }
+    for (uint32_t e = row.topo_begin; e < row.topo_end; ++e)
       if (pb->class_topo[e].flags & KSCHED_TOPO_CONSTRAINS) { ++ncg; if (pb->groups[pb->class_topo[e].group].key != KSCHED_KEY_HOSTNAME) ++touched; }
-    }
     if (ncg > kMaxCG || touched > kMaxTouched) { h->err = "a pod class is constrained by more topology groups / label keys than the pack kernel carries"; return KSCHED_ERR_UNSUPPORTED; }
   }
+  for (int g = 0; g < NG; ++g)
+    if (pb->groups[g].key != KSCHED_KEY_HOSTNAME && pb->groups[g].key >= h->cat.n_keys) { h->err = "topology group key out of range"; return KSCHED_ERR_INVALID; }
+  return KSCHED_OK;
+}
+
+// Uploads one checked problem and binds every PackState field to it (ksched_upload's commit). Arrays the pack kernel mutates
+// get a pristine copy that reset_state restores before every run.
+static int bind_problem(ksched_handle* h, const ksched_problem* pb) {
+  h->tm.h2d_bytes = 0;
+  const DevCatalog& c = h->cat;
+  PackState& s = h->st;
+  s = PackState{};
+  h->resets.n = 0;
+  const int P = pb->n_pods, NC = pb->n_classes, NE = pb->n_existing, NG = pb->n_groups, W32 = c.W32, V = c.n_templates;
+  const int MAXN = std::max(1, std::min(pb->max_new_nodes > 0 ? pb->max_new_nodes : P, std::max(P, 1)));
+  const size_t p1 = (size_t)std::max(P, 1), ne = (size_t)std::max(NE, 1), nc = (size_t)std::max(NC, 1), ng = (size_t)std::max(NG, 1), mn = (size_t)MAXN;
+  s.n_pods = P; s.n_classes = NC; s.n_existing = NE; s.n_groups = NG; s.max_new = MAXN;
+  s.count_visited = pb->count_nodes_visited;
   // min request per resource over all classes (node closing rule)
   for (int r = 0; r < KSCHED_MAX_RES; ++r) {
-    int64_t mn = INT64_MAX;
-    for (int c2 = 0; c2 < NC; ++c2) {
-      const ksched_pod_row& row = pb->classes[c2];
-      int64_t v = ((row.res_present >> r) & 1) ? row.requests[r] : 0;
-      mn = std::min(mn, v);
-    }
-    h->min_req[r] = (NC == 0 || mn == INT64_MAX || mn < 0) ? 0 : mn;
+    int64_t m = INT64_MAX;
+    for (int i = 0; i < NC; ++i) m = std::min(m, ((pb->classes[i].res_present >> r) & 1) ? pb->classes[i].requests[r] : (int64_t)0);
+    s.min_req[r] = (NC == 0 || m == INT64_MAX || m < 0) ? 0 : m;
   }
-  CUDA_TRY(h, upload(h, h->d_classes, pb->classes, (size_t)NC));
-  h->tol_ext_words = pb->class_tolerated_ext ? pb->n_tolerated_ext_words : 0;
-  if (h->tol_ext_words > 0) CUDA_TRY(h, upload(h, h->d_cls_tol_ext, pb->class_tolerated_ext, (size_t)NC * h->tol_ext_words));
+  CUDA_TRY(h, bind(h, h->d_classes, s.classes, (size_t)NC, pb->classes));
+  s.tol_ext_words = pb->class_tolerated_ext ? pb->n_tolerated_ext_words : 0;
+  if (s.tol_ext_words > 0) CUDA_TRY(h, bind(h, h->d_cls_tol_ext, s.cls_tol_ext, (size_t)NC * s.tol_ext_words, pb->class_tolerated_ext));
   if (const int X = c.n_res_ext) {
-    CUDA_TRY(h, upload(h, h->d_cls_req_ext, pb->class_requests_ext, (size_t)NC * X));
-    CUDA_TRY(h, upload(h, h->d_cls_ext_present, pb->class_res_ext_present, (size_t)NC));
+    CUDA_TRY(h, bind(h, h->d_cls_req_ext, s.cls_req_ext, (size_t)NC * X, pb->class_requests_ext));
+    CUDA_TRY(h, bind(h, h->d_cls_ext_present, s.cls_ext_present, (size_t)NC, pb->class_res_ext_present));
     // existing nodes: [x][n_existing] (the scan reads one resource of consecutive nodes)
-    std::vector<int64_t> avail((size_t)X * std::max(NE, 1), 0);
+    std::vector<int64_t> avail((size_t)X * ne, 0);
     for (int e = 0; e < NE; ++e)
       for (int x = 0; x < X; ++x) avail[(size_t)x * NE + e] = pb->existing_available_ext[(size_t)e * X + x];
-    CUDA_TRY(h, upload_vec(h, h->d_ex_avail_ext, avail));
+    CUDA_TRY(h, bind(h, h->d_ex_avail_ext, s.ex_avail_ext, avail.size(), avail.data()));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    CUDA_TRY(h, h->d_ex_req_ext.ensure((size_t)X * std::max(NE, 1)));
-    CUDA_TRY(h, h->d_nn_req_ext.ensure((size_t)X * MAXN));
-    CUDA_TRY(h, h->d_nn_ext_present.ensure((size_t)MAXN));
+    // ext sums of existing and new nodes: every mode that opens a node relies on zeros here
+    CUDA_TRY(h, bind_zeroed(h, h->d_ex_req_ext, s.ex_req_ext, (size_t)X * ne));
+    CUDA_TRY(h, bind_zeroed(h, h->d_nn_req_ext, s.nn_req_ext, (size_t)X * mn));
+    CUDA_TRY(h, bind_zeroed(h, h->d_nn_ext_present, s.nn_ext_present, mn));
   }
   {
     // queue.go:82-108 orders by cpu desc, memory desc, timestamp asc, UID asc. (cpu, memory) is a property of the class: rank
     // the classes once here, and the whole order is one packed key when rank, timestamp span and UID rank fit 64 bits.
-    std::vector<uint32_t> by((size_t)NC), rank((size_t)std::max(NC, 1), 0);
+    std::vector<uint32_t> by((size_t)NC), rank(nc, 0);
     for (int i = 0; i < NC; ++i) by[(size_t)i] = (uint32_t)i;
-    auto cpu = [&](uint32_t c) { return pb->classes[c].requests[0]; };
-    auto mem = [&](uint32_t c) { return pb->classes[c].requests[1]; };
+    auto cpu = [&](uint32_t i) { return pb->classes[i].requests[0]; };
+    auto mem = [&](uint32_t i) { return pb->classes[i].requests[1]; };
     std::sort(by.begin(), by.end(), [&](uint32_t a, uint32_t b) { return cpu(a) != cpu(b) ? cpu(a) > cpu(b) : mem(a) > mem(b); });
     uint32_t r = 0;
     for (int i = 0; i < NC; ++i) {
@@ -813,25 +895,23 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
     CUDA_TRY(h, upload_vec(h, h->d_cls_rank, rank));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // rank is a stack vector
   }
-  CUDA_TRY(h, upload(h, h->d_pod_class0, pb->pod_class, (size_t)P));
-  CUDA_TRY(h, h->d_pod_class.ensure(P));
+  CUDA_TRY(h, bind_restored(h, h->d_pod_class, s.pod_class, h->d_pod_class0, (size_t)P, pb->pod_class));
   CUDA_TRY(h, upload(h, h->d_ts, pb->pod_timestamp, (size_t)P));
   CUDA_TRY(h, upload(h, h->d_uid_rank, pb->pod_uid_rank, (size_t)P));
-  CUDA_TRY(h, upload(h, h->d_groups, pb->groups, (size_t)NG));
-  CUDA_TRY(h, upload(h, h->d_class_topo, pb->class_topo, (size_t)pb->n_class_topo));
-  CUDA_TRY(h, upload(h, h->d_filter_terms, pb->filter_terms, (size_t)pb->n_filter_terms));
-  CUDA_TRY(h, upload(h, h->d_hostname_reqs, pb->hostname_reqs, (size_t)pb->n_hostname_reqs * 2));
-  h->hostname_words = pb->n_hostname_words;
-  h->filter_hostname = pb->filter_term_hostname != nullptr;
-  if (h->hostname_words) CUDA_TRY(h, upload(h, h->d_hostname_slots, pb->hostname_slots, (size_t)pb->n_hostname_reqs * h->hostname_words));
-  if (h->filter_hostname) CUDA_TRY(h, upload(h, h->d_filter_hostname, pb->filter_term_hostname, (size_t)pb->n_filter_terms));
-  CUDA_TRY(h, upload(h, h->d_itype_comp, pb->itype_req_complement, (size_t)pb->n_itype_reqs));
-  CUDA_TRY(h, upload(h, h->d_itype_sets, reinterpret_cast<const uint32_t*>(pb->itype_req_sets), (size_t)pb->n_itype_reqs * W32));
+  CUDA_TRY(h, bind(h, h->d_groups, s.groups, (size_t)NG, pb->groups));
+  CUDA_TRY(h, bind(h, h->d_class_topo, s.class_topo, (size_t)pb->n_class_topo, pb->class_topo));
+  CUDA_TRY(h, bind(h, h->d_filter_terms, s.filter_terms, (size_t)pb->n_filter_terms, pb->filter_terms));
+  CUDA_TRY(h, bind(h, h->d_hostname_reqs, s.hostname_reqs, (size_t)pb->n_hostname_reqs * 2, pb->hostname_reqs));
+  s.hostname_words = pb->n_hostname_words;
+  if (s.hostname_words) CUDA_TRY(h, bind(h, h->d_hostname_slots, s.hostname_slots, (size_t)pb->n_hostname_reqs * s.hostname_words, pb->hostname_slots));
+  if (pb->filter_term_hostname) CUDA_TRY(h, bind(h, h->d_filter_hostname, s.filter_hostname, (size_t)pb->n_filter_terms, pb->filter_term_hostname));
+  CUDA_TRY(h, bind(h, h->d_itype_comp, s.itype_complement, (size_t)pb->n_itype_reqs, pb->itype_req_complement));
+  CUDA_TRY(h, bind(h, h->d_itype_sets, s.itype_sets, (size_t)pb->n_itype_reqs * W32, reinterpret_cast<const uint32_t*>(pb->itype_req_sets)));
   // existing nodes -> SoA
   {
-    std::vector<int64_t> req((size_t)8 * std::max(NE, 1), 0), avail((size_t)8 * std::max(NE, 1), 0);
-    std::vector<uint32_t> reqp(std::max(NE, 1), 0), availp(std::max(NE, 1), 0), ts(std::max(NE, 1), 0), it(std::max(NE, 1), 0);
-    std::vector<uint64_t> vals((size_t)16 * std::max(NE, 1), 0), meta(std::max(NE, 1), 0), hp(std::max(NE, 1), 0);
+    std::vector<int64_t> req(8 * ne, 0), avail(8 * ne, 0);
+    std::vector<uint32_t> reqp(ne, 0), availp(ne, 0), ts(ne, 0), it(ne, 0);
+    std::vector<uint64_t> vals(16 * ne, 0), meta(ne, 0), hp(ne, 0);
     for (int e = 0; e < NE; ++e) {
       const ksched_existing_node& n = pb->existing[e];
       for (int r = 0; r < 8; ++r) { req[(size_t)r * NE + e] = n.requests[r]; avail[(size_t)r * NE + e] = n.available[r]; }
@@ -839,103 +919,88 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
       meta[e] = n.reqs.meta & 0xFFFFFFFFull;
       reqp[e] = n.requests_present; availp[e] = n.available_present; ts[e] = n.taintset; it[e] = n.itype; hp[e] = n.hostport_entries;
     }
-    CUDA_TRY(h, upload_vec(h, h->d_ex_req0, req));
-    CUDA_TRY(h, upload_vec(h, h->d_ex_avail, avail));
-    CUDA_TRY(h, upload_vec(h, h->d_ex_req_present0, reqp));
-    CUDA_TRY(h, upload_vec(h, h->d_ex_avail_present, availp));
-    CUDA_TRY(h, upload_vec(h, h->d_ex_taintset, ts));
-    CUDA_TRY(h, upload_vec(h, h->d_ex_itype, it));
-    CUDA_TRY(h, upload_vec(h, h->d_ex_vals0, vals));
-    CUDA_TRY(h, upload_vec(h, h->d_ex_meta0, meta));
-    CUDA_TRY(h, upload_vec(h, h->d_ex_hp0, hp));
+    CUDA_TRY(h, bind_restored(h, h->d_ex_req, s.ex_req, h->d_ex_req0, req.size(), req.data()));
+    CUDA_TRY(h, bind(h, h->d_ex_avail, s.ex_avail, avail.size(), avail.data()));
+    CUDA_TRY(h, bind_restored(h, h->d_ex_req_present, s.ex_req_present, h->d_ex_req_present0, reqp.size(), reqp.data()));
+    CUDA_TRY(h, bind(h, h->d_ex_avail_present, s.ex_avail_present, availp.size(), availp.data()));
+    CUDA_TRY(h, bind(h, h->d_ex_taintset, s.ex_taintset, ts.size(), ts.data()));
+    CUDA_TRY(h, bind(h, h->d_ex_itype, s.ex_itype, it.size(), it.data()));
+    CUDA_TRY(h, bind_restored(h, h->d_ex_vals, s.ex_vals, h->d_ex_vals0, vals.size(), vals.data()));
+    CUDA_TRY(h, bind_restored(h, h->d_ex_meta, s.ex_meta, h->d_ex_meta0, meta.size(), meta.data()));
+    CUDA_TRY(h, bind_restored(h, h->d_ex_hp, s.ex_hp, h->d_ex_hp0, hp.size(), hp.data()));
     // host-port entries from id 64 on: per-class tables as given, the existing nodes' words as [word][node] like ex_hp
     const int HW = pb->n_hostport_ext_words;
-    h->hp_ext_words = HW;
-    std::vector<uint64_t> hp_ext(HW > 0 ? (size_t)HW * std::max(NE, 1) : 0, 0);
-    std::vector<uint8_t> cls_hp(HW > 0 ? (size_t)std::max(NC, 1) : 0, 0);
+    s.hp_ext_words = HW;
+    std::vector<uint64_t> hp_ext(HW > 0 ? (size_t)HW * ne : 0, 0);
+    std::vector<uint8_t> cls_hp(HW > 0 ? nc : 0, 0);
     if (HW > 0) {
       for (int e = 0; e < NE; ++e)
         for (int w = 0; w < HW; ++w) hp_ext[(size_t)w * NE + e] = pb->existing_hostport_ext[(size_t)e * HW + w];
-      for (int c2 = 0; c2 < NC; ++c2)
+      for (int i = 0; i < NC; ++i)
         for (int w = 0; w < HW; ++w)
-          if (pb->class_hostport_conflicts_ext[(size_t)c2 * HW + w] | pb->class_hostport_entries_ext[(size_t)c2 * HW + w]) cls_hp[c2] = 1;
-      CUDA_TRY(h, upload(h, h->d_cls_hpc_ext, pb->class_hostport_conflicts_ext, (size_t)NC * HW));
-      CUDA_TRY(h, upload(h, h->d_cls_hpe_ext, pb->class_hostport_entries_ext, (size_t)NC * HW));
-      CUDA_TRY(h, upload_vec(h, h->d_cls_hp_ext, cls_hp));
-      CUDA_TRY(h, upload_vec(h, h->d_ex_hp_ext0, hp_ext));
-      CUDA_TRY(h, h->d_ex_hp_ext.ensure(hp_ext.size()));
-      CUDA_TRY(h, h->d_nn_hp_ext.ensure((size_t)HW * MAXN));
+          if (pb->class_hostport_conflicts_ext[(size_t)i * HW + w] | pb->class_hostport_entries_ext[(size_t)i * HW + w]) cls_hp[i] = 1;
+      CUDA_TRY(h, bind(h, h->d_cls_hpc_ext, s.cls_hpc_ext, (size_t)NC * HW, pb->class_hostport_conflicts_ext));
+      CUDA_TRY(h, bind(h, h->d_cls_hpe_ext, s.cls_hpe_ext, (size_t)NC * HW, pb->class_hostport_entries_ext));
+      CUDA_TRY(h, bind(h, h->d_cls_hp_ext, s.cls_hp_ext, cls_hp.size(), cls_hp.data()));
+      CUDA_TRY(h, bind_restored(h, h->d_ex_hp_ext, s.ex_hp_ext, h->d_ex_hp_ext0, hp_ext.size(), hp_ext.data()));  // new nodes: set at creation
+      CUDA_TRY(h, bind(h, h->d_nn_hp_ext, s.nn_hp_ext, (size_t)HW * mn));
     }
-    h->have_volumes = pb->class_volumes != nullptr && pb->existing_volumes != nullptr && NE > 0;
-    if (h->have_volumes) {
-      CUDA_TRY(h, upload(h, h->d_cls_vol, pb->class_volumes, (size_t)NC));
-      CUDA_TRY(h, upload(h, h->d_ex_vol0, pb->existing_volumes, (size_t)NE));
-      CUDA_TRY(h, h->d_ex_vol.ensure((size_t)NE));
-      for (int d = 0; d < KSCHED_MAX_VOLUME_DRIVERS; ++d) h->vol_mask[d] = pb->volume_driver_mask[d];
+    if (pb->class_volumes && pb->existing_volumes && NE > 0) {
+      CUDA_TRY(h, bind(h, h->d_cls_vol, s.cls_vol, (size_t)NC, pb->class_volumes));
+      CUDA_TRY(h, bind_restored(h, h->d_ex_vol, s.ex_vol, h->d_ex_vol0, (size_t)NE, pb->existing_volumes));
+      std::memcpy(s.vol_mask, pb->volume_driver_mask, sizeof s.vol_mask);
     }
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // host vectors go out of scope
-    size_t ne = (size_t)std::max(NE, 1);
-    CUDA_TRY(h, h->d_ex_req.ensure(8 * ne));
-    CUDA_TRY(h, h->d_ex_req_present.ensure(ne));
-    CUDA_TRY(h, h->d_ex_vals.ensure(16 * ne));
-    CUDA_TRY(h, h->d_ex_meta.ensure(ne));
-    CUDA_TRY(h, h->d_ex_hp.ensure(ne));
-    CUDA_TRY(h, h->d_ex_closed.ensure(ne));
+    CUDA_TRY(h, bind_zeroed(h, h->d_ex_closed, s.ex_closed, ne));
   }
   // topology counters
   {
-    std::vector<int32_t> host_row(std::max(NG, 1), -1), host_total(std::max(NG, 1), 0), cnt((size_t)std::max(NG, 1) * 64, 0);
-    std::vector<uint64_t> registered(std::max(NG, 1), 0);
+    std::vector<int32_t> host_row(ng, -1), host_total(ng, 0), cnt(ng * 64, 0);
+    std::vector<uint64_t> registered(ng, 0);
+    std::vector<uint8_t> active(ng, 1);
     int nh = 0;
     for (int g = 0; g < NG; ++g) {
       if (pb->groups[g].key == KSCHED_KEY_HOSTNAME) host_row[g] = nh++;
-      else if (pb->groups[g].key >= c.n_keys) { h->err = "topology group key out of range"; return KSCHED_ERR_INVALID; }
       registered[g] = pb->groups[g].registered;
+      active[g] = pb->groups[g].dormant ? 0 : 1;
       for (int d = 0; d < 64; ++d) cnt[(size_t)g * 64 + d] = pb->group_domain_counts[(size_t)g * 64 + d];
     }
-    h->n_hostgroups = nh;
     const size_t stride = (size_t)NE + MAXN;
     // [hostname group][existing node | new node slot] counters: only the existing-node columns carry initial values, the
     // rest of the (up to 40 MB) matrix is zeroed on the device instead of being built and shipped from the host
-    std::vector<uint16_t> host((size_t)std::max(nh, 1) * std::max(NE, 1), 0);
+    std::vector<uint16_t> host((size_t)std::max(nh, 1) * ne, 0);
     for (int g = 0; g < NG; ++g) {
       if (host_row[g] < 0) continue;
       int total = pb->groups[g].extra_nonzero_domains;
       for (int e = 0; e < NE; ++e) {
-        int32_t v = pb->group_existing_counts[(size_t)g * std::max(NE, 1) + e];
+        int32_t v = pb->group_existing_counts[(size_t)g * ne + e];
         host[(size_t)host_row[g] * NE + e] = (uint16_t)std::min(v, 0xFFFF);
         if (v > 0) ++total;
       }
       host_total[g] = total;
     }
-    std::vector<uint8_t> active(std::max(NG, 1), 1);
-    for (int g = 0; g < NG; ++g) active[g] = pb->groups[g].dormant ? 0 : 1;
-    CUDA_TRY(h, upload_vec(h, h->d_grp_active0, active));
-    CUDA_TRY(h, h->d_grp_active.ensure(std::max(NG, 1)));
-    CUDA_TRY(h, h->d_grp_min_slot.ensure(std::max(NG, 1)));
-    CUDA_TRY(h, upload_vec(h, h->d_grp_host_row, host_row));
-    {
-      std::vector<RelX> relx((size_t)std::max(pb->n_class_topo, 1));
-      for (int e = 0; e < pb->n_class_topo; ++e) {
-        const ksched_class_topo& ct = pb->class_topo[e];
-        if ((int)ct.group >= NG) { h->err = "class_topo names a group out of range"; return KSCHED_ERR_INVALID; }
-        const ksched_topo_group& g = pb->groups[ct.group];
-        RelX x{};
-        x.group = ct.group; x.flags = ct.flags; x.key = g.key; x.type = g.type; x.has_filter = g.filter_begin != g.filter_end;
-        // a term without any requirement is Compatible with every node (topologynodefilter.go:57-70): such a filter always matches
-        for (uint32_t f = g.filter_begin; f < g.filter_end && f < (uint32_t)pb->n_filter_terms; ++f)
-          if (((pb->filter_terms[f].meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF) == 0 &&
-              (!pb->filter_term_hostname || pb->filter_term_hostname[f] == KSCHED_NONE))
-            x.has_filter = 0;
-        x.max_skew = g.max_skew; x.host_row = host_row[ct.group];
-        relx[e] = x;
-      }
-      CUDA_TRY(h, upload_vec(h, h->d_relx, relx));
+    std::vector<RelX> relx((size_t)std::max(pb->n_class_topo, 1));
+    for (int e = 0; e < pb->n_class_topo; ++e) {
+      const ksched_class_topo& ct = pb->class_topo[e];
+      const ksched_topo_group& g = pb->groups[ct.group];
+      RelX x{};
+      x.group = ct.group; x.flags = ct.flags; x.key = g.key; x.type = g.type; x.has_filter = g.filter_begin != g.filter_end;
+      // a term without any requirement is Compatible with every node (topologynodefilter.go:57-70): such a filter always matches
+      for (uint32_t f = g.filter_begin; f < g.filter_end && f < (uint32_t)pb->n_filter_terms; ++f)
+        if (((pb->filter_terms[f].meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF) == 0 &&
+            (!pb->filter_term_hostname || pb->filter_term_hostname[f] == KSCHED_NONE))
+          x.has_filter = 0;
+      x.max_skew = g.max_skew; x.host_row = host_row[ct.group];
+      relx[e] = x;
     }
-    CUDA_TRY(h, upload_vec(h, h->d_grp_host_total0, host_total));
-    CUDA_TRY(h, upload_vec(h, h->d_grp_cnt0, cnt));
-    CUDA_TRY(h, upload_vec(h, h->d_grp_registered0, registered));
-    CUDA_TRY(h, h->d_grp_host0.ensure((size_t)std::max(nh, 1) * stride));
+    CUDA_TRY(h, bind_restored(h, h->d_grp_active, s.grp_active, h->d_grp_active0, active.size(), active.data()));
+    CUDA_TRY(h, bind_zeroed(h, h->d_grp_min_slot, s.grp_min_slot, ng));
+    CUDA_TRY(h, bind(h, h->d_grp_host_row, s.grp_host_row, host_row.size(), host_row.data()));
+    CUDA_TRY(h, bind(h, h->d_relx, s.relx, relx.size(), relx.data()));
+    CUDA_TRY(h, bind_restored(h, h->d_grp_host_total, s.grp_host_total, h->d_grp_host_total0, host_total.size(), host_total.data()));
+    CUDA_TRY(h, bind_restored(h, h->d_grp_cnt, s.grp_cnt, h->d_grp_cnt0, cnt.size(), cnt.data()));
+    CUDA_TRY(h, bind_restored(h, h->d_grp_registered, s.grp_registered, h->d_grp_registered0, registered.size(), registered.data()));
+    CUDA_TRY(h, bind_restored(h, h->d_grp_host, s.grp_host, h->d_grp_host0, (size_t)std::max(nh, 1) * stride));
     CUDA_TRY(h, cudaMemsetAsync(h->d_grp_host0.ptr, 0, (size_t)std::max(nh, 1) * stride * sizeof(uint16_t), h->stream));
     if (NE > 0 && nh > 0) {
       CUDA_TRY(h, cudaMemcpy2DAsync(h->d_grp_host0.ptr, stride * sizeof(uint16_t), host.data(), (size_t)NE * sizeof(uint16_t), (size_t)NE * sizeof(uint16_t),
@@ -943,59 +1008,95 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
       h->tm.h2d_bytes += (int64_t)nh * NE * 2;
     }
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    CUDA_TRY(h, h->d_grp_host_total.ensure(std::max(NG, 1)));
-    CUDA_TRY(h, h->d_grp_cnt.ensure((size_t)std::max(NG, 1) * 64));
-    CUDA_TRY(h, h->d_grp_registered.ensure(std::max(NG, 1)));
-    CUDA_TRY(h, h->d_grp_host.ensure((size_t)std::max(nh, 1) * stride));
   }
   // scratch / state
-  const size_t p1 = (size_t)std::max(P, 1);
-  CUDA_TRY(h, h->d_order.ensure(p1)); CUDA_TRY(h, h->d_idx_tmp.ensure(p1)); CUDA_TRY(h, h->d_pod_pos.ensure(p1));
-  CUDA_TRY(h, h->d_k_cpu.ensure(p1)); CUDA_TRY(h, h->d_k_mem.ensure(p1)); CUDA_TRY(h, h->d_k_tie.ensure(p1)); CUDA_TRY(h, h->d_k_tmp.ensure(p1));
-  CUDA_TRY(h, h->d_rows.ensure(p1 * KSCHED_ROW_WORDS));
-  CUDA_TRY(h, h->d_F.ensure(p1 * V * W32));
-  CUDA_TRY(h, h->d_best.ensure(p1));
-  CUDA_TRY(h, h->d_Fclass.ensure((size_t)std::max(NC, 1) * V * W32));
-  CUDA_TRY(h, h->d_best_class.ensure((size_t)std::max(NC, 1)));
-  CUDA_TRY(h, h->d_relax.ensure(p1)); CUDA_TRY(h, h->d_assign.ensure(p1)); CUDA_TRY(h, h->d_place_seq.ensure(p1));
-  CUDA_TRY(h, h->d_queue.ensure(p1 + 1)); CUDA_TRY(h, h->d_last_len.ensure(p1)); CUDA_TRY(h, h->d_last_epoch.ensure(p1));
-  const size_t mn = (size_t)MAXN;
-  CUDA_TRY(h, h->d_nn_tmpl.ensure(mn)); CUDA_TRY(h, h->d_nn_count.ensure(mn)); CUDA_TRY(h, h->d_nn_tb.ensure(mn));
-  CUDA_TRY(h, h->d_nn_req.ensure(8 * mn)); CUDA_TRY(h, h->d_nn_req_present.ensure(mn));
-  CUDA_TRY(h, h->d_nn_vals.ensure(16 * mn)); CUDA_TRY(h, h->d_nn_meta.ensure(mn));
-  CUDA_TRY(h, h->d_nn_opts.ensure((size_t)W32 * mn)); CUDA_TRY(h, h->d_nn_hp.ensure(mn));
-  CUDA_TRY(h, h->d_ov_key.ensure(mn)); CUDA_TRY(h, h->d_ov_q.ensure(4 * mn)); CUDA_TRY(h, h->d_ov_bound.ensure(4 * mn)); CUDA_TRY(h, h->d_ov_bound2.ensure(4 * mn));
-  CUDA_TRY(h, h->d_ov_node.ensure(mn)); CUDA_TRY(h, h->d_ov_flags.ensure(mn));
-  CUDA_TRY(h, h->d_ov_absorbed.ensure(mn)); CUDA_TRY(h, h->d_ov_rejected.ensure(mn));
+  CUDA_TRY(h, bind(h, h->d_order, s.order, p1));
+  CUDA_TRY(h, h->d_idx_tmp.ensure(p1));
+  CUDA_TRY(h, bind(h, h->d_pod_pos, s.pod_pos, p1));
+  CUDA_TRY(h, h->d_k_cpu.ensure(p1));
+  CUDA_TRY(h, h->d_k_mem.ensure(p1));
+  CUDA_TRY(h, h->d_k_tie.ensure(p1));
+  CUDA_TRY(h, h->d_k_tmp.ensure(p1));
+  CUDA_TRY(h, bind(h, h->d_rows, s.rows, p1 * KSCHED_ROW_WORDS));
+  CUDA_TRY(h, bind(h, h->d_F, s.F, p1 * V * W32));
+  CUDA_TRY(h, bind(h, h->d_best, s.best, p1));
+  CUDA_TRY(h, h->d_Fclass.ensure(nc * V * W32));
+  CUDA_TRY(h, h->d_best_class.ensure(nc));
+  CUDA_TRY(h, bind_zeroed(h, h->d_relax, s.relax_level, p1));
+  CUDA_TRY(h, bind(h, h->d_assign, s.assign, p1));
+  CUDA_TRY(h, bind(h, h->d_place_seq, s.place_seq, p1));
+  CUDA_TRY(h, bind(h, h->d_queue, s.queue, p1 + 1));
+  CUDA_TRY(h, bind(h, h->d_last_len, s.last_len, p1));
+  CUDA_TRY(h, bind(h, h->d_last_epoch, s.last_epoch, p1));
+  CUDA_TRY(h, bind_zeroed(h, h->d_cls_cursor, s.cls_cursor, nc));
+  CUDA_TRY(h, bind(h, h->d_nn_tmpl, s.nn_tmpl, mn));
+  CUDA_TRY(h, bind(h, h->d_nn_count, s.nn_count, mn));
+  CUDA_TRY(h, bind(h, h->d_nn_tb, s.nn_tb, mn));
+  CUDA_TRY(h, bind(h, h->d_nn_req, s.nn_req, 8 * mn));
+  CUDA_TRY(h, bind(h, h->d_nn_req_present, s.nn_req_present, mn));
+  CUDA_TRY(h, bind(h, h->d_nn_vals, s.nn_vals, 16 * mn));
+  CUDA_TRY(h, bind(h, h->d_nn_meta, s.nn_meta, mn));
+  CUDA_TRY(h, bind(h, h->d_nn_opts, s.nn_opts, (size_t)W32 * mn));
+  CUDA_TRY(h, bind(h, h->d_nn_hp, s.nn_hp, mn));
+  CUDA_TRY(h, bind(h, h->d_ov_key, s.ov_key, mn));
+  CUDA_TRY(h, bind(h, h->d_ov_q, s.ov_q, 4 * mn));
+  CUDA_TRY(h, bind(h, h->d_ov_bound, s.ov_bound, 4 * mn));
+  CUDA_TRY(h, bind(h, h->d_ov_bound2, s.ov_bound2, 4 * mn));
+  CUDA_TRY(h, bind(h, h->d_ov_node, s.ov_node, mn));
+  CUDA_TRY(h, bind(h, h->d_ov_flags, s.ov_flags, mn));
+  CUDA_TRY(h, bind(h, h->d_ov_absorbed, s.ov_absorbed, mn));
+  CUDA_TRY(h, bind(h, h->d_ov_rejected, s.ov_rejected, mn));
+  const size_t nfc = nc * V;
+  CUDA_TRY(h, bind_zeroed(h, h->d_fc_state, s.fc_state, nfc));
+  CUDA_TRY(h, bind(h, h->d_fc_dom, s.fc_dom, nfc));
+  CUDA_TRY(h, bind_zeroed(h, h->d_fc_front_state, s.fc_front_state, nfc));
+  CUDA_TRY(h, bind(h, h->d_fc_bound, s.fc_bound, nfc * 4));
+  CUDA_TRY(h, bind(h, h->d_fc_bound2, s.fc_bound2, nfc * 4));
+  CUDA_TRY(h, bind(h, h->d_fc_opts, s.fc_opts, nfc * W32));
+  CUDA_TRY(h, bind(h, h->d_fc_vals, s.fc_vals, nfc * KSCHED_MAX_KEYS));
+  CUDA_TRY(h, bind(h, h->d_fc_meta, s.fc_meta, nfc));
+  CUDA_TRY(h, bind(h, h->d_fc_q, s.fc_q, nfc * KSCHED_MAX_RES));
+  CUDA_TRY(h, bind(h, h->d_fc_qp, s.fc_qp, nfc));
+  s.fd_cap = kFreshMemoSlots;
+  CUDA_TRY(h, bind_zeroed(h, h->d_fd_state, s.fd_state, kFreshMemoSlots));
+  CUDA_TRY(h, bind(h, h->d_fd_dom, s.fd_dom, kFreshMemoSlots));
+  CUDA_TRY(h, bind(h, h->d_fd_fc, s.fd_fc, kFreshMemoSlots));
+  CUDA_TRY(h, bind(h, h->d_fd_meta, s.fd_meta, kFreshMemoSlots));
+  CUDA_TRY(h, bind(h, h->d_fd_vals, s.fd_vals, (size_t)kFreshMemoSlots * KSCHED_MAX_KEYS));
+  CUDA_TRY(h, bind(h, h->d_fd_opts, s.fd_opts, (size_t)kFreshMemoSlots * W32));
+  CUDA_TRY(h, bind(h, h->d_fd_bound, s.fd_bound, (size_t)kFreshMemoSlots * 4));
+  CUDA_TRY(h, bind(h, h->d_fd_bound2, s.fd_bound2, (size_t)kFreshMemoSlots * 4));
+  CUDA_TRY(h, bind(h, h->d_remaining, s.remaining, (size_t)V * KSCHED_MAX_RES));  // reset_state: limits per call
+  CUDA_TRY(h, bind_zeroed(h, h->d_counters, s.counters, kNumCounters));
+  CUDA_TRY(h, bind(h, h->d_vstore, s.vstore, kVarStore));
   {
-    const size_t nfc = (size_t)std::max(NC, 1) * V;
-    CUDA_TRY(h, h->d_fc_state.ensure(nfc)); CUDA_TRY(h, h->d_fc_dom.ensure(nfc)); CUDA_TRY(h, h->d_fc_front_state.ensure(nfc)); CUDA_TRY(h, h->d_fc_bound.ensure(nfc * 4)); CUDA_TRY(h, h->d_fc_bound2.ensure(nfc * 4));
-    CUDA_TRY(h, h->d_fc_opts.ensure(nfc * W32));
-    CUDA_TRY(h, h->d_fc_vals.ensure(nfc * KSCHED_MAX_KEYS)); CUDA_TRY(h, h->d_fc_meta.ensure(nfc)); CUDA_TRY(h, h->d_fc_q.ensure(nfc * KSCHED_MAX_RES));
-    CUDA_TRY(h, h->d_fc_qp.ensure(nfc));
-    const size_t nfd = kFreshMemoSlots;
-    CUDA_TRY(h, h->d_fd_state.ensure(nfd)); CUDA_TRY(h, h->d_fd_dom.ensure(nfd)); CUDA_TRY(h, h->d_fd_fc.ensure(nfd)); CUDA_TRY(h, h->d_fd_meta.ensure(nfd));
-    CUDA_TRY(h, h->d_fd_vals.ensure(nfd * KSCHED_MAX_KEYS)); CUDA_TRY(h, h->d_fd_opts.ensure(nfd * W32));
-    CUDA_TRY(h, h->d_fd_bound.ensure(nfd * 4)); CUDA_TRY(h, h->d_fd_bound2.ensure(nfd * 4));
-  }
-  CUDA_TRY(h, h->d_remaining.ensure((size_t)V * KSCHED_MAX_RES));
-  CUDA_TRY(h, h->d_counters.ensure(kNumCounters));
-  CUDA_TRY(h, h->d_vstore.ensure(kVarStore));
-  {
-    size_t need = 0, n2 = 0;
+    size_t need = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, need, (uint64_t*)nullptr, (uint64_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)p1, 0, 64, h->stream);
-    n2 = need;
-    CUDA_TRY(h, h->d_cub_tmp.ensure(n2 + 256));
-    h->cub_tmp_bytes = n2 + 256;
+    CUDA_TRY(h, h->d_cub_tmp.ensure(need + 256));
+    h->cub_tmp_bytes = need + 256;
   }
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  return KSCHED_OK;
+}
+
+// ---- upload one problem (pods / nodes / topology) and keep pristine copies of everything the pack kernel mutates
+int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
+  if (!h || !pb) return KSCHED_ERR_INVALID;
+  int rc = check_problem(h, pb);
+  if (rc != KSCHED_OK) return rc;
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  // the resident problem is replaced from here on: a CUDA error part-way through leaves none
+  h->uploaded = false;
+  // the superset buffers ksched_load_cluster filled are about to be overwritten: simulations need a new ksched_load_cluster
+  h->have_cluster = false;
+  if ((rc = bind_problem(h, pb)) != KSCHED_OK) return rc;
   h->uploaded = true;
   h->sorted = false;
   return KSCHED_OK;
 }
 
-static int run_sort(ksched_handle* h) {
-  const int P = h->n_pods;
+// K0 over the first P pods (a simulation's batch, otherwise the whole problem); so are run_class_feasibility and run_feasibility.
+static int run_sort(ksched_handle* h, int P) {
   if (P == 0) return KSCHED_OK;
   const int threads = 256, blocks = (P + threads - 1) / threads;
   if (h->sort1_bits > 0) {  // one packed key, only its significant bits sorted
@@ -1033,14 +1134,13 @@ static int run_sort(ksched_handle* h) {
 static void fill_k1(ksched_handle* h, K1Params& k1) {
   // the row evaluation runs over the class table (every class once); feasibility_kernel replicates the rows per pod
   k1.cat = h->cat;
-  k1.rows = reinterpret_cast<const uint64_t*>(h->d_classes.ptr);
-  k1.n_pods = h->n_classes;
-  k1.itype_sets = h->d_itype_sets.ptr;
+  k1.rows = reinterpret_cast<const uint64_t*>(h->st.classes);
+  k1.n_pods = h->st.n_classes;
+  k1.itype_sets = h->st.itype_sets;
   k1.F = h->d_Fclass.ptr;
   k1.best = h->d_best_class.ptr;
-  const bool ext = h->cat.n_res_ext > 0;
-  k1.cls_req_ext = ext ? h->d_cls_req_ext.ptr : nullptr;
-  k1.cls_ext_present = ext ? h->d_cls_ext_present.ptr : nullptr;
+  k1.cls_req_ext = h->st.cls_req_ext;  // nullptr without ext resources
+  k1.cls_ext_present = h->st.cls_ext_present;
   const int W32 = h->cat.W32;
   if (h->world > 1) {
     ksched_shard_range(W32, h->rank, h->world, &k1.word_begin, &k1.word_end);
@@ -1054,8 +1154,9 @@ static std::mutex g_k1_mu;
 static cudaEvent_t g_k1_done[64] = {};
 
 // K1, class pass: every distinct pod row evaluated once (class_feasibility_kernel over the class table).
-static int run_class_feasibility(ksched_handle* h) {
-  if (h->n_pods == 0 || h->n_classes == 0) return KSCHED_OK;
+static int run_class_feasibility(ksched_handle* h, int P) {
+  const int NC = h->st.n_classes;
+  if (P == 0 || NC == 0) return KSCHED_OK;
   K1Params k1;
   fill_k1(h, k1);
   const DevCatalog& c = h->cat;
@@ -1070,7 +1171,7 @@ static int run_class_feasibility(ksched_handle* h) {
   if (k1.tables_in_smem) smem += table_bytes;
   // one warp per class row (a row evaluation is thousands of cycles of dependent work: no chunking)
   const int warps_per_block = kK1Threads / 32;
-  const int blocks = std::max(1, std::min(h->n_sm * 2, (h->n_classes + warps_per_block - 1) / warps_per_block));
+  const int blocks = std::max(1, std::min(h->n_sm * 2, (NC + warps_per_block - 1) / warps_per_block));
   k1.dbg = nullptr;
 #ifdef KSCHED_PROFILE_K1
   CUDA_TRY(h, h->d_k1dbg.ensure(8));
@@ -1087,7 +1188,7 @@ static int run_class_feasibility(ksched_handle* h) {
     CUDA_TRY(h, cudaMemcpyToSymbolAsync(g_k1, &h->k1_host, sizeof(K1Params), 0, cudaMemcpyHostToDevice, h->stream));
     CUDA_TRY(h, cudaFuncSetAttribute(class_feasibility_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));  // per function: under the launch lock
     if (h->world > 1)  // column words of the other shards read as 0
-      CUDA_TRY(h, cudaMemsetAsync(h->d_Fclass.ptr, 0, (size_t)std::max(h->n_classes, 1) * c.n_templates * c.W32 * 4, h->stream));
+      CUDA_TRY(h, cudaMemsetAsync(h->d_Fclass.ptr, 0, (size_t)NC * c.n_templates * c.W32 * 4, h->stream));
     class_feasibility_kernel<<<blocks, kK1Threads, smem, h->stream>>>();
     CUDA_TRY(h, cudaGetLastError());
     CUDA_TRY(h, cudaEventRecord(done, h->stream));
@@ -1105,25 +1206,20 @@ static int run_class_feasibility(ksched_handle* h) {
 }
 
 // K1 proper: the dense pods x (template, instance type) matrix and the per-pod best column, streamed from the class rows.
-static int run_feasibility(ksched_handle* h) {
-  if (h->n_pods == 0) return KSCHED_OK;
+static int run_feasibility(ksched_handle* h, int P) {
+  if (P == 0) return KSCHED_OK;
   const int RW = h->cat.n_templates * h->cat.W32;
-  const int nblk = (h->n_pods + 31) / 32;
+  const int nblk = (P + 31) / 32;
   const int blocks = std::max(1, std::min(h->n_sm * 8, (nblk + 7) / 8));  // 8 warps per CTA, one 32-row block per warp and iteration
-  feasibility_kernel<<<blocks, 256, 0, h->stream>>>(h->d_rows.ptr, h->n_pods, h->n_classes, RW, h->d_Fclass.ptr, h->d_best_class.ptr, h->d_F.ptr,
+  feasibility_kernel<<<blocks, 256, 0, h->stream>>>(h->d_rows.ptr, P, h->st.n_classes, RW, h->d_Fclass.ptr, h->d_best_class.ptr, h->d_F.ptr,
                                                     h->d_best.ptr);
   CUDA_TRY(h, cudaGetLastError());
   h->tm.feasibility_launches = 2;
   const long long C = (long long)h->cat.n_templates * h->cat.n_types;
-  h->tm.feasibility_bytes = (long long)h->n_pods * 256 + C * 256 + (long long)h->n_pods * C / 8;
+  h->tm.feasibility_bytes = (long long)P * 256 + C * 256 + (long long)P * C / 8;
   return KSCHED_OK;
 }
 
-// Every array a Solve mutates goes back to its pristine copy (or to zero) in ONE launch: a table of (dst, src, bytes)
-// segments passed by value. (Round 1 issued ~20 cudaMemcpyAsync / cudaMemsetAsync calls per Solve; a consolidation
-// simulation is so short that those launches were most of it.)
-struct ResetSeg { void* dst; const void* src; unsigned long long bytes; };
-struct ResetTable { int n; ResetSeg seg[30]; };
 __global__ void reset_kernel(ResetTable t) {
   const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (size_t)gridDim.x * blockDim.x;
   for (int q = 0; q < t.n; ++q) {
@@ -1138,46 +1234,19 @@ __global__ void reset_kernel(ResetTable t) {
   }
 }
 
-static int reset_state(ksched_handle* h, const int64_t* d_remaining_src = nullptr, void* also_zero = nullptr, size_t also_zero_bytes = 0) {
-  const int P = h->n_pods, NE = std::max(h->n_existing, 1), NG = std::max(h->n_groups, 1);
-  CUDA_TRY(h, h->d_cls_cursor.ensure((size_t)std::max(h->n_classes, 1)));
-  ResetTable t{};
-  auto add = [&](void* dst, const void* src, size_t bytes) { if (bytes) t.seg[t.n++] = ResetSeg{dst, src, (unsigned long long)bytes}; };
-  add(h->d_pod_class.ptr, h->d_pod_class0.ptr, (size_t)P * 4);
-  add(h->d_relax.ptr, nullptr, (size_t)std::max(P, 1) * 4);
-  add(h->d_ex_req.ptr, h->d_ex_req0.ptr, (size_t)8 * NE * 8);
-  add(h->d_ex_req_present.ptr, h->d_ex_req_present0.ptr, (size_t)NE * 4);
-  add(h->d_ex_vals.ptr, h->d_ex_vals0.ptr, (size_t)16 * NE * 8);
-  add(h->d_ex_meta.ptr, h->d_ex_meta0.ptr, (size_t)NE * 8);
-  add(h->d_ex_hp.ptr, h->d_ex_hp0.ptr, (size_t)NE * 8);
-  if (h->hp_ext_words) add(h->d_ex_hp_ext.ptr, h->d_ex_hp_ext0.ptr, (size_t)h->hp_ext_words * NE * 8);  // new nodes: set at creation
-  add(h->d_ex_closed.ptr, nullptr, (size_t)NE);
-  add(h->d_cls_cursor.ptr, nullptr, (size_t)std::max(h->n_classes, 1) * 4);
-  if (h->have_volumes) add(h->d_ex_vol.ptr, h->d_ex_vol0.ptr, (size_t)h->n_existing * sizeof(ksched_node_volumes));
-  if (h->cat.n_res_ext) {  // ext sums of existing and new nodes: every mode that opens a node relies on zeros here
-    add(h->d_ex_req_ext.ptr, nullptr, (size_t)h->cat.n_res_ext * NE * 8);
-    add(h->d_nn_req_ext.ptr, nullptr, (size_t)h->cat.n_res_ext * h->max_new * 8);
-    add(h->d_nn_ext_present.ptr, nullptr, (size_t)h->max_new * 4);
-  }
-  add(h->d_grp_cnt.ptr, h->d_grp_cnt0.ptr, (size_t)NG * 64 * 4);
-  add(h->d_grp_registered.ptr, h->d_grp_registered0.ptr, (size_t)NG * 8);
-  add(h->d_grp_host_total.ptr, h->d_grp_host_total0.ptr, (size_t)NG * 4);
-  add(h->d_grp_active.ptr, h->d_grp_active0.ptr, (size_t)NG);
-  add(h->d_grp_min_slot.ptr, nullptr, (size_t)NG * 4);
-  const size_t hs = (size_t)std::max(h->n_hostgroups, 1) * ((size_t)h->n_existing + h->max_new);
-  add(h->d_grp_host.ptr, h->d_grp_host0.ptr, hs * 2);
-  if (d_remaining_src)  // simulation on the cluster snapshot: limits with the removed nodes' capacity given back, already on the device
-    add(h->d_remaining.ptr, d_remaining_src, (size_t)h->cat.n_templates * KSCHED_MAX_RES * 8);
-  add(h->d_counters.ptr, nullptr, kNumCounters * sizeof(long long));
-  add(h->d_fc_state.ptr, nullptr, (size_t)std::max(h->n_classes, 1) * h->cat.n_templates);
-  add(h->d_fc_front_state.ptr, nullptr, (size_t)std::max(h->n_classes, 1) * h->cat.n_templates);
-  add(h->d_fd_state.ptr, nullptr, (size_t)kFreshMemoSlots);
-  add(also_zero, nullptr, also_zero_bytes);
-  if (!d_remaining_src) {
+// The segments ksched_upload recorded, and the provisioner limits: a simulation's (already on the device, with the removed
+// nodes' capacity given back; its candidate marks are cleared too) or the templates'.
+static int reset_state(ksched_handle* h, const int64_t* sim_remaining = nullptr) {
+  ResetTable t = h->resets;
+  const size_t rem_bytes = (size_t)h->cat.n_templates * KSCHED_MAX_RES * 8;
+  if (sim_remaining) {
+    CUDA_TRY(h, record_reset(t, h->st.remaining, sim_remaining, rem_bytes));
+    CUDA_TRY(h, record_reset(t, h->d_in_set.ptr, nullptr, (size_t)std::max(h->st.n_existing, 1)));
+  } else {
     std::vector<int64_t> rem((size_t)h->cat.n_templates * KSCHED_MAX_RES);
     for (int v = 0; v < h->cat.n_templates; ++v)
       for (int r = 0; r < KSCHED_MAX_RES; ++r) rem[(size_t)v * KSCHED_MAX_RES + r] = h->h_templates[v].remaining[r];
-    CUDA_TRY(h, cudaMemcpyAsync(h->d_remaining.ptr, rem.data(), rem.size() * 8, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(h->st.remaining, rem.data(), rem_bytes, cudaMemcpyHostToDevice, h->stream));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // rem is a stack vector
   }
   reset_kernel<<<h->n_sm * 2, 256, 0, h->stream>>>(t);
@@ -1190,51 +1259,17 @@ static int reset_state(ksched_handle* h, const int64_t* d_remaining_src = nullpt
 static std::mutex g_k2_mu;
 static cudaEvent_t g_k2_done[64] = {};
 
-static int run_pack(ksched_handle* h) {
+// The pack kernel over the first n_pods pods of the queue (a simulation's batch, otherwise the whole problem).
+static int run_pack(ksched_handle* h, int n_pods, int stop_new_nodes) {
   K2Params& k2 = h->k2_host;
   k2.cat = h->cat;
+  k2.st = h->st;
+  // what may change between launches of one upload: the batch, the column sharding (ksched_set_shard / ksched_nccl_init
+  // may follow the upload), the templates (ksched_load_catalog's early-out), the mode switches and the smem layout
   PackState& s = k2.st;
-  s.relx = h->d_relx.ptr;
-  s.classes = h->d_classes.ptr; s.groups = h->d_groups.ptr; s.class_topo = h->d_class_topo.ptr; s.filter_terms = h->d_filter_terms.ptr;
-  s.itype_sets = h->d_itype_sets.ptr; s.itype_complement = h->d_itype_comp.ptr; s.hostname_reqs = h->d_hostname_reqs.ptr;
-  s.hostname_slots = h->hostname_words ? h->d_hostname_slots.ptr : nullptr; s.hostname_words = h->hostname_words;
-  s.filter_hostname = h->filter_hostname ? h->d_filter_hostname.ptr : nullptr;
-  s.order = h->d_order.ptr; s.rows = h->d_rows.ptr; s.F = h->d_F.ptr; s.best = h->d_best.ptr;
-  s.pod_pos = h->d_pod_pos.ptr; s.use_F = h->world == 1 ? 1 : 0;
-  s.n_pods = h->n_pods; s.n_classes = h->n_classes; s.n_existing = h->n_existing; s.n_groups = h->n_groups; s.max_new = h->max_new;
-  for (int r = 0; r < KSCHED_MAX_RES; ++r) s.min_req[r] = h->min_req[r];
-  s.pod_class = h->d_pod_class.ptr; s.relax_level = h->d_relax.ptr; s.assign = h->d_assign.ptr; s.place_seq = h->d_place_seq.ptr;
-  s.queue = h->d_queue.ptr; s.last_len = h->d_last_len.ptr; s.last_epoch = h->d_last_epoch.ptr;
-  s.ex_req = h->d_ex_req.ptr; s.ex_avail = h->d_ex_avail.ptr; s.ex_req_present = h->d_ex_req_present.ptr; s.ex_avail_present = h->d_ex_avail_present.ptr;
-  s.ex_vals = h->d_ex_vals.ptr; s.ex_meta = h->d_ex_meta.ptr; s.ex_taintset = h->d_ex_taintset.ptr; s.ex_itype = h->d_ex_itype.ptr;
-  s.ex_hp = h->d_ex_hp.ptr; s.ex_closed = h->d_ex_closed.ptr;
-  s.cls_cursor = h->d_cls_cursor.ptr;
-  s.cls_tol_ext = h->tol_ext_words > 0 ? h->d_cls_tol_ext.ptr : nullptr; s.tol_ext_words = h->tol_ext_words;
-  const bool hpx = h->hp_ext_words > 0;
-  s.cls_hpc_ext = hpx ? h->d_cls_hpc_ext.ptr : nullptr; s.cls_hpe_ext = hpx ? h->d_cls_hpe_ext.ptr : nullptr;
-  s.cls_hp_ext = hpx ? h->d_cls_hp_ext.ptr : nullptr; s.ex_hp_ext = hpx ? h->d_ex_hp_ext.ptr : nullptr;
-  s.nn_hp_ext = hpx ? h->d_nn_hp_ext.ptr : nullptr; s.hp_ext_words = h->hp_ext_words;
-  const bool ext = h->cat.n_res_ext > 0;
-  s.cls_req_ext = ext ? h->d_cls_req_ext.ptr : nullptr; s.cls_ext_present = ext ? h->d_cls_ext_present.ptr : nullptr;
-  s.ex_avail_ext = ext ? h->d_ex_avail_ext.ptr : nullptr; s.ex_req_ext = ext ? h->d_ex_req_ext.ptr : nullptr;
-  s.nn_req_ext = ext ? h->d_nn_req_ext.ptr : nullptr; s.nn_ext_present = ext ? h->d_nn_ext_present.ptr : nullptr;
-  s.cls_vol = h->have_volumes ? h->d_cls_vol.ptr : nullptr; s.ex_vol = h->have_volumes ? h->d_ex_vol.ptr : nullptr;
-  for (int d = 0; d < KSCHED_MAX_VOLUME_DRIVERS; ++d) s.vol_mask[d] = h->vol_mask[d];
-  s.nn_tmpl = h->d_nn_tmpl.ptr; s.nn_count = h->d_nn_count.ptr; s.nn_tb = h->d_nn_tb.ptr; s.nn_req = h->d_nn_req.ptr;
-  s.nn_req_present = h->d_nn_req_present.ptr;
-  s.nn_vals = h->d_nn_vals.ptr; s.nn_meta = h->d_nn_meta.ptr; s.nn_opts = h->d_nn_opts.ptr; s.nn_hp = h->d_nn_hp.ptr;
-  s.ov_key = h->d_ov_key.ptr; s.ov_q = h->d_ov_q.ptr; s.ov_bound = h->d_ov_bound.ptr; s.ov_bound2 = h->d_ov_bound2.ptr; s.ov_node = h->d_ov_node.ptr; s.ov_flags = h->d_ov_flags.ptr;
-  s.fc_state = h->d_fc_state.ptr; s.fc_opts = h->d_fc_opts.ptr; s.fc_bound = h->d_fc_bound.ptr; s.fc_bound2 = h->d_fc_bound2.ptr; s.fc_dom = h->d_fc_dom.ptr; s.fc_front_state = h->d_fc_front_state.ptr;
-  s.fc_vals = h->d_fc_vals.ptr; s.fc_meta = h->d_fc_meta.ptr; s.fc_q = h->d_fc_q.ptr; s.fc_qp = h->d_fc_qp.ptr;
-  s.ov_absorbed = h->d_ov_absorbed.ptr; s.ov_rejected = h->d_ov_rejected.ptr;
-  s.fd_cap = kFreshMemoSlots; s.fd_state = h->d_fd_state.ptr; s.fd_fc = h->d_fd_fc.ptr; s.fd_meta = h->d_fd_meta.ptr; s.fd_vals = h->d_fd_vals.ptr;
-  s.fd_opts = h->d_fd_opts.ptr; s.fd_bound = h->d_fd_bound.ptr; s.fd_bound2 = h->d_fd_bound2.ptr; s.fd_dom = h->d_fd_dom.ptr;
-  s.count_visited = h->count_visited;
-  s.stop_new_nodes = h->stop_new_nodes;
-  s.grp_cnt = h->d_grp_cnt.ptr; s.grp_registered = h->d_grp_registered.ptr; s.grp_host = h->d_grp_host.ptr;
-  s.grp_host_row = h->d_grp_host_row.ptr; s.grp_host_total = h->d_grp_host_total.ptr; s.remaining = h->d_remaining.ptr;
-  s.grp_active = h->d_grp_active.ptr; s.grp_min_slot = h->d_grp_min_slot.ptr;
-  s.counters = h->d_counters.ptr;
+  s.n_pods = n_pods;
+  s.stop_new_nodes = stop_new_nodes;
+  s.use_F = h->world == 1 ? 1 : 0;
   const size_t alloc_bytes = (size_t)h->cat.n_res * h->cat.n_types * sizeof(int64_t);
   // 227 KB per CTA on sm_90a: the hot node window + ~4 KB of static shared memory come first
   const size_t static_smem = (size_t)(14 << 10);  // file-scope __shared__ objects (pod row, PodTopo, RunCtx with its variants, scratch)
@@ -1251,10 +1286,9 @@ static int run_pack(ksched_handle* h) {
   s.use_varstore = std::getenv("KSCHED_NO_VARSTORE") ? 0 : 1;
   s.use_round_stretch = std::getenv("KSCHED_NO_ROUNDSTRETCH") ? 0 : 1;
   s.use_fill_stretch = s.use_round_stretch && !std::getenv("KSCHED_NO_FILLSTRETCH") ? 1 : 0;
-  s.vstore = h->d_vstore.ptr;
   // block size: the chain is latency-bound on ONE thread's commit; more warps only help when there are many candidate
   // nodes to examine per pod (existing nodes, large in-flight sets)
-  int threads = h->n_existing >= 2048 ? kPackThreads : (h->n_existing >= 256 ? 256 : 128);
+  int threads = s.n_existing >= 2048 ? kPackThreads : (s.n_existing >= 256 ? 256 : 128);
   if (const char* e = getenv("KSCHED_PACK_THREADS")) { int v = atoi(e); if (v >= 32 && v <= kPackThreads && v % 32 == 0) threads = v; }
   {
     std::lock_guard<std::mutex> lock(g_k2_mu);
@@ -1278,7 +1312,7 @@ static int run_pack(ksched_handle* h) {
     CUDA_TRY(h, cudaGetLastError());
     CUDA_TRY(h, cudaEventRecord(done, h->stream));
   }
-  finalize_options_kernel<<<h->n_sm, 256, 0, h->stream>>>(h->cat, h->d_counters.ptr, h->d_nn_req.ptr, h->d_nn_req_present.ptr, h->d_nn_opts.ptr, h->max_new);
+  finalize_options_kernel<<<h->n_sm, 256, 0, h->stream>>>(h->cat, s.counters, s.nn_req, s.nn_req_present, s.nn_opts, s.max_new);
   h->tm.pack_launches = 2;
   return KSCHED_OK;
 }
@@ -1299,22 +1333,23 @@ static float ev_us(cudaEvent_t a, cudaEvent_t b) {
 int ksched_run_resident(ksched_handle* h, int do_flush) {
   if (!h || !h->uploaded) return KSCHED_ERR_INVALID;
   CUDA_TRY(h, cudaSetDevice(h->device));
+  const int P = h->st.n_pods;
   int rc;
   if ((rc = reset_state(h)) != KSCHED_OK) return rc;
   if (do_flush && (rc = flush_l2(h)) != KSCHED_OK) return rc;
   CUDA_TRY(h, cudaEventRecord(h->ev[0], h->stream));
-  if ((rc = run_sort(h)) != KSCHED_OK) return rc;
+  if ((rc = run_sort(h, P)) != KSCHED_OK) return rc;
   CUDA_TRY(h, cudaEventRecord(h->ev[1], h->stream));
-  if ((rc = run_class_feasibility(h)) != KSCHED_OK) return rc;
-  if ((rc = run_feasibility(h)) != KSCHED_OK) return rc;
+  if ((rc = run_class_feasibility(h, P)) != KSCHED_OK) return rc;
+  if ((rc = run_feasibility(h, P)) != KSCHED_OK) return rc;
   CUDA_TRY(h, cudaEventRecord(h->ev[2], h->stream));
   h->tm.allreduce_us = 0;
   if (h->world > 1 && h->comm) {
-    ncclResult_t r = ncclAllReduce(h->d_best.ptr, h->d_best.ptr, (size_t)h->n_pods, ncclUint64, ncclMin, h->comm, h->stream);
+    ncclResult_t r = ncclAllReduce(h->d_best.ptr, h->d_best.ptr, (size_t)P, ncclUint64, ncclMin, h->comm, h->stream);
     if (r != ncclSuccess) { h->err = std::string("ncclAllReduce: ") + ncclGetErrorString(r); return KSCHED_ERR_NCCL; }
   }
   CUDA_TRY(h, cudaEventRecord(h->ev[3], h->stream));
-  if ((rc = run_pack(h)) != KSCHED_OK) return rc;
+  if ((rc = run_pack(h, P, 0)) != KSCHED_OK) return rc;
   CUDA_TRY(h, cudaEventRecord(h->ev[4], h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   CUDA_TRY(h, cudaGetLastError());
@@ -1329,16 +1364,17 @@ int ksched_run_resident(ksched_handle* h, int do_flush) {
 int ksched_run_feasibility_only(ksched_handle* h, int do_flush, float* elapsed_us) {
   if (!h || !h->uploaded) return KSCHED_ERR_INVALID;
   CUDA_TRY(h, cudaSetDevice(h->device));
+  const int P = h->st.n_pods;
   int rc;
   if (!h->sorted) {  // K0 first: the kernel streams the FFD-ordered pod-row matrix
-    CUDA_TRY(h, cudaMemcpyAsync(h->d_pod_class.ptr, h->d_pod_class0.ptr, (size_t)h->n_pods * 4, cudaMemcpyDeviceToDevice, h->stream));
-    if ((rc = run_sort(h)) != KSCHED_OK) return rc;
+    CUDA_TRY(h, cudaMemcpyAsync(h->d_pod_class.ptr, h->d_pod_class0.ptr, (size_t)P * 4, cudaMemcpyDeviceToDevice, h->stream));
+    if ((rc = run_sort(h, P)) != KSCHED_OK) return rc;
   }
   CUDA_TRY(h, cudaEventRecord(h->ev[7], h->stream));
-  if ((rc = run_class_feasibility(h)) != KSCHED_OK) return rc;  // n_classes row evaluations (timed on their own)
+  if ((rc = run_class_feasibility(h, P)) != KSCHED_OK) return rc;  // n_classes row evaluations (timed on their own)
   if (do_flush && (rc = flush_l2(h)) != KSCHED_OK) return rc;
   CUDA_TRY(h, cudaEventRecord(h->ev[5], h->stream));
-  if ((rc = run_feasibility(h)) != KSCHED_OK) return rc;
+  if ((rc = run_feasibility(h, P)) != KSCHED_OK) return rc;
   CUDA_TRY(h, cudaEventRecord(h->ev[6], h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   CUDA_TRY(h, cudaGetLastError());
@@ -1400,9 +1436,11 @@ static void print_pack_profile(const long long* counters) {
 int ksched_download(ksched_handle* h, const ksched_problem* pb, ksched_result* res) {
   if (!h || !pb || !res || !h->uploaded) return KSCHED_ERR_INVALID;
   CUDA_TRY(h, cudaSetDevice(h->device));
-  const int P = h->n_pods, NE = h->n_existing, MAXN = h->max_new, W32 = h->cat.W32, W64 = h->W64, V = h->cat.n_templates;
+  const PackState& s = h->st;
+  const int P = s.n_pods, NE = s.n_existing, W32 = h->cat.W32, W64 = W32 / 2, V = h->cat.n_templates;
   long long counters[kNumCounters];
-  CUDA_TRY(h, cudaMemcpyAsync(counters, h->d_counters.ptr, sizeof counters, cudaMemcpyDeviceToHost, h->stream));
+  h->tm.d2h_bytes = 0;
+  CUDA_TRY(h, download(h, counters, s.counters, kNumCounters));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
 #ifdef KSCHED_PROFILE_PACK
   print_pack_profile(counters);
@@ -1412,76 +1450,67 @@ int ksched_download(ksched_handle* h, const ksched_problem* pb, ksched_result* r
     return (int)counters[kCtrError];
   }
   const int n_new = (int)counters[kCtrNewNodes];
-  h->tm.d2h_bytes = (int64_t)sizeof counters + (int64_t)P * 4 * ((res->assign != nullptr) + (res->relax_level != nullptr) + (res->place_seq != nullptr)) +
-                    (int64_t)n_new * (1 + 4 + 4 + 8 + 64 + 128 + (int64_t)W32 * 4) + (res->existing_reqs ? (int64_t)NE * 136 : 0) +
-                    (res->launch ? (int64_t)n_new * (int64_t)sizeof(ksched_launch_choice) : 0) +
-                    (res->feasibility ? (int64_t)P * V * W32 * 4 + (int64_t)P * 4 : 0) + (res->best_column ? (int64_t)P * 12 : 0);
   res->n_new_nodes = n_new;
   res->n_unscheduled = (int)counters[kCtrUnscheduled];
   res->nodes_visited = counters[kCtrNodesVisited];
   res->add_calls = counters[kCtrAddCalls];
   h->tm.pack_steps = counters[kCtrSteps];
-  if (res->assign) CUDA_TRY(h, cudaMemcpyAsync(res->assign, h->d_assign.ptr, (size_t)P * 4, cudaMemcpyDeviceToHost, h->stream));
-  if (res->relax_level) CUDA_TRY(h, cudaMemcpyAsync(res->relax_level, h->d_relax.ptr, (size_t)P * 4, cudaMemcpyDeviceToHost, h->stream));
-  if (res->place_seq) CUDA_TRY(h, cudaMemcpyAsync(res->place_seq, h->d_place_seq.ptr, (size_t)P * 4, cudaMemcpyDeviceToHost, h->stream));
+  if (res->assign) CUDA_TRY(h, download(h, res->assign, s.assign, (size_t)P));
+  if (res->relax_level) CUDA_TRY(h, download(h, res->relax_level, s.relax_level, (size_t)P));
+  if (res->place_seq) CUDA_TRY(h, download(h, res->place_seq, s.place_seq, (size_t)P));
   if (n_new > 0 && res->new_nodes && res->new_node_types) {
     std::vector<uint8_t> tmpl(n_new);
     std::vector<int32_t> count(n_new);
-    std::vector<int64_t> req((size_t)8 * n_new);
-    std::vector<uint32_t> reqp(n_new), opts((size_t)W32 * n_new);
-    std::vector<uint64_t> vals((size_t)16 * n_new), meta(n_new);
-    CUDA_TRY(h, cudaMemcpyAsync(tmpl.data(), h->d_nn_tmpl.ptr, n_new, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(count.data(), h->d_nn_count.ptr, (size_t)n_new * 4, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(reqp.data(), h->d_nn_req_present.ptr, (size_t)n_new * 4, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(meta.data(), h->d_nn_meta.ptr, (size_t)n_new * 8, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpy2DAsync(req.data(), (size_t)n_new * 8, h->d_nn_req.ptr, (size_t)MAXN * 8, (size_t)n_new * 8, 8, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpy2DAsync(vals.data(), (size_t)n_new * 8, h->d_nn_vals.ptr, (size_t)MAXN * 8, (size_t)n_new * 8, 16, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpy2DAsync(opts.data(), (size_t)n_new * 4, h->d_nn_opts.ptr, (size_t)MAXN * 4, (size_t)n_new * 4, W32, cudaMemcpyDeviceToHost, h->stream));
+    std::vector<uint32_t> reqp(n_new), opts;
+    std::vector<uint64_t> meta(n_new), vals;
+    std::vector<int64_t> req;
+    CUDA_TRY(h, download(h, tmpl.data(), s.nn_tmpl, (size_t)n_new));
+    CUDA_TRY(h, download(h, count.data(), s.nn_count, (size_t)n_new));
+    CUDA_TRY(h, download(h, reqp.data(), s.nn_req_present, (size_t)n_new));
+    CUDA_TRY(h, download(h, meta.data(), s.nn_meta, (size_t)n_new));
+    CUDA_TRY(h, download_soa(h, req, s.nn_req, 8, (size_t)s.max_new, n_new));
+    CUDA_TRY(h, download_soa(h, vals, s.nn_vals, 16, (size_t)s.max_new, n_new));
+    CUDA_TRY(h, download_soa(h, opts, s.nn_opts, W32, (size_t)s.max_new, n_new));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    auto types_of = [&](int n) { return reinterpret_cast<uint32_t*>(res->new_node_types + (size_t)n * W64); };
     for (int n = 0; n < n_new; ++n) {
       ksched_new_node& o = res->new_nodes[n];
       std::memset(&o, 0, sizeof o);
       o.template_index = tmpl[n];
       o.pod_count = count[n];
       o.requests_present = reqp[n];
-      for (int r = 0; r < 8; ++r) o.requests[r] = req[(size_t)r * n_new + n];
-      for (int k = 0; k < 16; ++k) o.reqs.values[k] = vals[(size_t)k * n_new + n];
       o.reqs.meta = meta[n];
-      uint32_t* dst = reinterpret_cast<uint32_t*>(res->new_node_types + (size_t)n * W64);
-      for (int w = 0; w < W32; ++w) dst[w] = opts[(size_t)w * n_new + n];
-      if (W32 & 1) dst[W32] = 0;  // the row is W64 64-bit words: the caller's buffer need not be cleared
+      if (W32 & 1) types_of(n)[W32] = 0;  // the row is W64 64-bit words: the caller's buffer need not be cleared
     }
+    soa_to_rows(req, 8, n_new, [&](int n) { return res->new_nodes[n].requests; });
+    soa_to_rows(vals, 16, n_new, [&](int n) { return res->new_nodes[n].reqs.values; });
+    soa_to_rows(opts, W32, n_new, types_of);
     if (const int X = h->cat.n_res_ext) {
-      if (res->new_node_requests_ext)
-        CUDA_TRY(h, cudaMemcpyAsync(res->new_node_requests_ext, h->d_nn_req_ext.ptr, (size_t)n_new * X * 8, cudaMemcpyDeviceToHost, h->stream));
-      if (res->new_node_requests_ext_present)
-        CUDA_TRY(h, cudaMemcpyAsync(res->new_node_requests_ext_present, h->d_nn_ext_present.ptr, (size_t)n_new * 4, cudaMemcpyDeviceToHost, h->stream));
+      if (res->new_node_requests_ext) CUDA_TRY(h, download(h, res->new_node_requests_ext, s.nn_req_ext, (size_t)n_new * X));
+      if (res->new_node_requests_ext_present) CUDA_TRY(h, download(h, res->new_node_requests_ext_present, s.nn_ext_present, (size_t)n_new));
       CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     }
   }
   if (res->launch && n_new > 0) {
     if (!h->cat.offer_keys) { h->err = "ksched_result.launch needs ksched_catalog.offering_keys"; return KSCHED_ERR_INVALID; }
     CUDA_TRY(h, h->d_launch.ensure((size_t)n_new));
-    launch_choice_kernel<<<h->n_sm, 256, 0, h->stream>>>(h->cat, h->d_counters.ptr, h->d_nn_vals.ptr, h->d_nn_meta.ptr, h->d_nn_opts.ptr, MAXN,
-                                                     h->d_launch.ptr);
-    CUDA_TRY(h, cudaMemcpyAsync(res->launch, h->d_launch.ptr, (size_t)n_new * sizeof(ksched_launch_choice), cudaMemcpyDeviceToHost, h->stream));
+    launch_choice_kernel<<<h->n_sm, 256, 0, h->stream>>>(h->cat, s.counters, s.nn_vals, s.nn_meta, s.nn_opts, s.max_new, h->d_launch.ptr);
+    CUDA_TRY(h, download(h, res->launch, h->d_launch.ptr, (size_t)n_new));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   }
   if (res->existing_reqs && NE > 0) {
     std::vector<uint64_t> vals((size_t)16 * NE), meta(NE);
-    CUDA_TRY(h, cudaMemcpyAsync(vals.data(), h->d_ex_vals.ptr, vals.size() * 8, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(meta.data(), h->d_ex_meta.ptr, meta.size() * 8, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, download(h, vals.data(), s.ex_vals, vals.size()));
+    CUDA_TRY(h, download(h, meta.data(), s.ex_meta, meta.size()));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    for (int e = 0; e < NE; ++e) {
-      for (int k = 0; k < 16; ++k) res->existing_reqs[e].values[k] = vals[(size_t)k * NE + e];
-      res->existing_reqs[e].meta = meta[e];
-    }
+    soa_to_rows(vals, 16, NE, [&](int e) { return res->existing_reqs[e].values; });
+    for (int e = 0; e < NE; ++e) res->existing_reqs[e].meta = meta[e];
   }
   if (res->feasibility) {
     // device rows are in FFD (queue) order; the caller gets them in its own pod order
     std::vector<uint32_t> order(P), F((size_t)P * V * W32);
-    CUDA_TRY(h, cudaMemcpyAsync(order.data(), h->d_order.ptr, (size_t)P * 4, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(F.data(), h->d_F.ptr, F.size() * 4, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, download(h, order.data(), s.order, order.size()));
+    CUDA_TRY(h, download(h, F.data(), s.F, F.size()));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     const size_t rowb = (size_t)V * W32;
     for (int j = 0; j < P; ++j) std::memcpy(reinterpret_cast<uint32_t*>(res->feasibility) + (size_t)order[j] * rowb, &F[(size_t)j * rowb], rowb * 4);
@@ -1489,8 +1518,8 @@ int ksched_download(ksched_handle* h, const ksched_problem* pb, ksched_result* r
   if (res->best_column) {
     std::vector<uint32_t> order(P);
     std::vector<unsigned long long> best(P);
-    CUDA_TRY(h, cudaMemcpyAsync(order.data(), h->d_order.ptr, (size_t)P * 4, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaMemcpyAsync(best.data(), h->d_best.ptr, (size_t)P * 8, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, download(h, order.data(), s.order, order.size()));
+    CUDA_TRY(h, download(h, best.data(), s.best, best.size()));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     for (int j = 0; j < P; ++j) res->best_column[order[j]] = best[j];
   }
@@ -1573,11 +1602,10 @@ int ksched_simulate_batch(ksched_handle* h, const ksched_candidate_set* sets, in
   if (!h->have_cluster) { h->err = "ksched_load_cluster must be called first"; return KSCHED_ERR_INVALID; }
   if (n_sets == 0) return KSCHED_OK;
   CUDA_TRY(h, cudaSetDevice(h->device));
-  const int NE = h->n_existing, V = h->cat.n_templates, W32 = h->cat.W32, W64 = h->W64;
+  const int NE = h->st.n_existing, V = h->cat.n_templates, W32 = h->cat.W32, W64 = W32 / 2;
   // stage every set's node list, per-node batch offsets and limits in one upload each
   std::vector<int32_t> all_nodes, all_dst((size_t)n_sets * std::max(NE, 1), 0), batch((size_t)n_sets, 0), node_off((size_t)n_sets + 1, 0);
   std::vector<int64_t> all_rem((size_t)n_sets * V * KSCHED_MAX_RES, 0);
-  std::vector<uint8_t> seen((size_t)std::max(NE, 1), 0);
   for (int q = 0; q < n_sets; ++q) {
     const ksched_candidate_set& cs = sets[q];
     if (cs.n_nodes < 0 || (cs.n_nodes > 0 && !cs.nodes)) { h->err = "bad candidate set"; return KSCHED_ERR_INVALID; }
@@ -1597,7 +1625,6 @@ int ksched_simulate_batch(ksched_handle* h, const ksched_candidate_set* sets, in
       for (int r = 0; r < KSCHED_MAX_RES; ++r)
         all_rem[((size_t)q * V + v) * KSCHED_MAX_RES + r] = cs.remaining ? cs.remaining[(size_t)v * KSCHED_MAX_RES + r] : h->h_templates[(size_t)v].remaining[r];
   }
-  (void)seen;
   if (all_nodes.empty()) all_nodes.push_back(0);
   CUDA_TRY(h, upload_vec(h, h->d_set_nodes, all_nodes));
   CUDA_TRY(h, upload_vec(h, h->d_node_dst, all_dst));
@@ -1608,11 +1635,10 @@ int ksched_simulate_batch(ksched_handle* h, const ksched_candidate_set* sets, in
   int rc = KSCHED_OK;
   // nothing computeConsolidation can return depends on what happens after a second new node is opened
   // (consolidation.go:214-224: len(newNodes) != 1 -> do nothing): the simulation stops there
-  h->stop_new_nodes = 2;
+  const int stop_new_nodes = 2;
   for (int q = 0; q < n_sets && rc == KSCHED_OK; ++q) {
-    const int n_nodes = node_off[(size_t)q + 1] - node_off[(size_t)q];
-    h->n_pods = batch[(size_t)q];
-    rc = reset_state(h, h->d_sim_remaining.ptr + (size_t)q * V * KSCHED_MAX_RES, h->d_in_set.ptr, (size_t)std::max(NE, 1));
+    const int n_nodes = node_off[(size_t)q + 1] - node_off[(size_t)q], P = batch[(size_t)q];
+    rc = reset_state(h, h->d_sim_remaining.ptr + (size_t)q * V * KSCHED_MAX_RES);
     if (rc != KSCHED_OK) break;
     if (n_nodes > 0)
       cluster_mark_kernel<<<(n_nodes + 255) / 256, 256, 0, h->stream>>>(h->d_set_nodes.ptr + node_off[(size_t)q], n_nodes, h->d_in_set.ptr, h->d_ex_closed.ptr);
@@ -1623,21 +1649,19 @@ int ksched_simulate_batch(ksched_handle* h, const ksched_candidate_set* sets, in
     if (h->cluster_topology && h->sup_pods > 0)
       cluster_topology_kernel<<<(h->sup_pods + 255) / 256, 256, 0, h->stream>>>(
           h->sup_pods, h->d_sup_pod_node.ptr, h->d_in_set.ptr, h->d_sup_class.ptr, h->d_cc_begin.ptr, h->d_cc.ptr, h->d_groups.ptr, h->d_node_dom.ptr,
-          h->d_node_hostlabel.ptr, h->d_filt.ptr, h->filt_words, NE, NE + h->max_new, h->d_grp_host_row.ptr, h->d_grp_cnt.ptr,
+          h->d_node_hostlabel.ptr, h->d_filt.ptr, h->filt_words, NE, NE + h->st.max_new, h->d_grp_host_row.ptr, h->d_grp_cnt.ptr,
           reinterpret_cast<unsigned long long*>(h->d_grp_registered.ptr), h->d_grp_host.ptr, h->d_grp_host_total.ptr);
     // the working copy of the pod classes (reset_state copied the previous batch's): refresh it from the new batch
-    if (h->n_pods > 0) CUDA_TRY(h, cudaMemcpyAsync(h->d_pod_class.ptr, h->d_pod_class0.ptr, (size_t)h->n_pods * 4, cudaMemcpyDeviceToDevice, h->stream));
-    if ((rc = run_sort(h)) != KSCHED_OK) break;
+    if (P > 0) CUDA_TRY(h, cudaMemcpyAsync(h->d_pod_class.ptr, h->d_pod_class0.ptr, (size_t)P * 4, cudaMemcpyDeviceToDevice, h->stream));
+    if ((rc = run_sort(h, P)) != KSCHED_OK) break;
     // the class rows of the feasibility matrix depend on the classes and the catalog only: once per batch
-    if (q == 0 && (rc = run_class_feasibility(h)) != KSCHED_OK) break;
-    if ((rc = run_feasibility(h)) != KSCHED_OK) break;
-    if ((rc = run_pack(h)) != KSCHED_OK) break;
-    cluster_collect_kernel<<<1, 64, 0, h->stream>>>(h->d_counters.ptr, h->n_pods, h->d_nn_tmpl.ptr, h->d_nn_count.ptr, h->d_nn_req.ptr, h->d_nn_req_present.ptr,
-                                                    h->d_nn_vals.ptr, h->d_nn_meta.ptr, h->d_nn_opts.ptr, h->max_new, W32, h->d_sim_results.ptr + q,
+    if (q == 0 && (rc = run_class_feasibility(h, P)) != KSCHED_OK) break;
+    if ((rc = run_feasibility(h, P)) != KSCHED_OK) break;
+    if ((rc = run_pack(h, P, stop_new_nodes)) != KSCHED_OK) break;
+    cluster_collect_kernel<<<1, 64, 0, h->stream>>>(h->d_counters.ptr, P, h->d_nn_tmpl.ptr, h->d_nn_count.ptr, h->d_nn_req.ptr, h->d_nn_req_present.ptr,
+                                                    h->d_nn_vals.ptr, h->d_nn_meta.ptr, h->d_nn_opts.ptr, h->st.max_new, W32, h->d_sim_results.ptr + q,
                                                     h->d_sim_types.ptr + (size_t)q * W32);
   }
-  h->n_pods = h->sup_pods;
-  h->stop_new_nodes = 0;
   if (rc != KSCHED_OK) return rc;
   CUDA_TRY(h, cudaEventRecord(h->ev[4], h->stream));
 #ifdef KSCHED_PROFILE_PACK

@@ -40,6 +40,7 @@ extern "C" {
 #define KSCHED_KEY_HOSTNAME 255
 #define KSCHED_NONE 0xFFFFFFFFu
 #define KSCHED_HOSTNAME_TABLE (-2) /* hostname_reqs[i][1]: the admitted existing slots are row i of problem.hostname_slots */
+#define KSCHED_ITYPE_UNLISTED 0xFFFFFFFEu /* problem.existing_itype: an instance-type label that names no type of the catalog */
 
 /* error codes (negative) */
 #define KSCHED_OK 0
@@ -303,6 +304,16 @@ typedef struct ksched_problem {
   const uint32_t* filter_term_hostname;  /* [n_filter_terms] (needs hostname_slots) */
   int32_t n_hostname_words;
   int32_t pad_hostname;
+  /* Topology node filter terms that name node.kubernetes.io/instance-type. Every value is an entry of itype_req_sets /
+     itype_req_complement, or KSCHED_NONE for "no requirement on the key". filter_term_itype[f] is the instance-type part of
+     filter term f. template_itype[v] is the requirement a new node of template v starts from (its provisioner's, from
+     NewMachineTemplate). existing_itype[e] is existing node e's requirement In [its instance-type label]; a label that is no
+     type of the catalog is KSCHED_ITYPE_UNLISTED. Pods' instance-type requirements intersect into these as they are added,
+     and a filter term's part is tested against the result with Intersects. All three NULL when no filter term names the
+     key (existing_itype may also be NULL without existing nodes); ksched_upload answers KSCHED_ERR_INVALID otherwise. */
+  const uint32_t* filter_term_itype;     /* [n_filter_terms] */
+  const uint32_t* template_itype;        /* [catalog n_templates] */
+  const uint32_t* existing_itype;        /* [n_existing] */
 } ksched_problem;
 
 typedef struct ksched_new_node {

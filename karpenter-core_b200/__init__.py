@@ -132,6 +132,8 @@ def lib():
     L.kh_encoded_class_hostname.restype = C.c_longlong
     L.kh_encoded_pod_class.argtypes = [C.c_void_p, C.c_int]
     L.kh_encoded_pod_class.restype = C.c_longlong
+    L.kh_encoded_group_total.argtypes = [C.c_void_p, C.c_int]
+    L.kh_encoded_group_total.restype = C.c_longlong
     L.kh_value_class_selftest.argtypes = [C.c_uint, C.c_int]
     L.kh_gpu_load.argtypes = [C.c_void_p]
     L.kh_encoded_set_count_visited.argtypes = [C.c_void_p, C.c_int]
@@ -579,10 +581,11 @@ class ResidentSolve:
         if not self.enc:
             msg = lib().kh_scheduler_error().decode()
             raise KschedError(KSCHED_ERR_UNSUPPORTED if msg.startswith("unsupported:") else KSCHED_ERR_INVALID, msg)
-        d = (C.c_longlong * 16)()
+        d = (C.c_longlong * 18)()
         lib().kh_encoded_dims(self.enc, d)
         self.dims = dict(zip(["pods", "classes", "existing", "groups", "types", "templates", "keys", "resources", "type_words", "class_topo",
-                              "taintsets", "resources_ext", "hostports", "hostport_ext_words", "hostname_reqs", "hostname_words"], list(d)))
+                              "taintsets", "resources_ext", "hostports", "hostport_ext_words", "hostname_reqs", "hostname_words",
+                              "itype_reqs", "itype_filter_terms"], list(d)))
 
     def hostname_reqs(self):
         """every hostname requirement of this encoding in entry order, as (admits new nodes, [admitted existing slots])"""
@@ -601,6 +604,10 @@ class ResidentSolve:
         """the hostname_reqs entry of class c, or None without a hostname requirement"""
         i = lib().kh_encoded_class_hostname(self.enc, c)
         return None if i < 0 else i
+
+    def group_total(self, g):
+        """the initial count of topology group g summed over its domains (countDomains)"""
+        return lib().kh_encoded_group_total(self.enc, g)
 
     def hostports(self):
         """the host-port entries of this encoding in id order, as (ip, port, protocol): the ones the encoder kept"""

@@ -227,6 +227,7 @@ struct ksched_handle {
   DevBuf<uint32_t> d_pod_class0, d_uid_rank, d_itype_sets, d_filter_hostname, d_cls_rank, d_cls_ext_present, d_ex_avail_present, d_ex_taintset,
       d_ex_itype;
   DevBuf<uint64_t> d_hostname_slots, d_cls_tol_ext, d_cls_hpc_ext, d_cls_hpe_ext;
+  DevBuf<uint32_t> d_filter_itype, d_tmpl_itype, d_ex_it0, d_ex_it, d_nn_it;  // instance-type filter tables and slot state
   // pristine copies of what a Solve mutates
   DevBuf<ksched_node_volumes> d_ex_vol0;
   DevBuf<int32_t> d_grp_cnt0, d_grp_host_total0;
@@ -804,6 +805,19 @@ static int check_problem(ksched_handle* h, const ksched_problem* pb) {
       return KSCHED_ERR_INVALID;
     }
   }
+  {
+    // instance-type filter tables: all three or none, every value an itype_req entry or KSCHED_NONE
+    const bool on = pb->filter_term_itype != nullptr;
+    bool ok = present_iff(on, {pb->template_itype}, pb->existing_itype, NE == 0);
+    auto entry = [&](uint32_t v) { return v == KSCHED_NONE || v < (uint32_t)pb->n_itype_reqs; };
+    for (int f = 0; ok && on && f < pb->n_filter_terms; ++f) ok = entry(pb->filter_term_itype[f]);
+    for (int v = 0; ok && on && v < h->cat.n_templates; ++v) ok = entry(pb->template_itype[v]);
+    for (int e = 0; ok && pb->existing_itype && e < NE; ++e) ok = entry(pb->existing_itype[e]) || pb->existing_itype[e] == KSCHED_ITYPE_UNLISTED;
+    if (!ok) {
+      h->err = "filter_term_itype / template_itype / existing_itype must be set together and name itype_req entries";
+      return KSCHED_ERR_INVALID;
+    }
+  }
   // ext resources: the tables exist exactly when the catalog has ext resources, and name no resource beyond them
   if (!present_iff(X > 0, {pb->class_requests_ext, pb->class_res_ext_present}, pb->existing_available_ext, NE == 0)) {
     h->err = "ext resource tables must be set exactly when the catalog has ext resources";
@@ -950,6 +964,25 @@ static int bind_problem(ksched_handle* h, const ksched_problem* pb) {
       CUDA_TRY(h, bind_restored(h, h->d_ex_vol, s.ex_vol, h->d_ex_vol0, (size_t)NE, pb->existing_volumes));
       std::memcpy(s.vol_mask, pb->volume_driver_mask, sizeof s.vol_mask);
     }
+    // instance-type requirement of every slot (topology.cuh: itype_state_add), only when a filter term names the key
+    std::vector<uint32_t> ex_it;
+    if (pb->filter_term_itype) {
+      const size_t IW = 1 + (size_t)W32;
+      const uint32_t* sets = reinterpret_cast<const uint32_t*>(pb->itype_req_sets);
+      ex_it.assign(ne * IW, 0);
+      for (int e = 0; e < NE; ++e) {
+        const uint32_t v = pb->existing_itype[e];
+        uint32_t* row = &ex_it[(size_t)e * IW];
+        if (v == KSCHED_ITYPE_UNLISTED) row[0] = kItPresent | kItOwn;
+        if (v == KSCHED_NONE || v == KSCHED_ITYPE_UNLISTED) continue;
+        row[0] = kItPresent | (pb->itype_req_complement[v] ? kItComp : 0u);
+        std::memcpy(row + 1, sets + (size_t)v * W32, (size_t)W32 * sizeof(uint32_t));
+      }
+      CUDA_TRY(h, bind(h, h->d_filter_itype, s.filter_itype, (size_t)pb->n_filter_terms, pb->filter_term_itype));
+      CUDA_TRY(h, bind(h, h->d_tmpl_itype, s.tmpl_itype, (size_t)V, pb->template_itype));
+      CUDA_TRY(h, bind_restored(h, h->d_ex_it, s.ex_it, h->d_ex_it0, ex_it.size(), ex_it.data()));
+      CUDA_TRY(h, bind(h, h->d_nn_it, s.nn_it, mn * IW));  // new nodes: set when they open
+    }
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // host vectors go out of scope
     CUDA_TRY(h, bind_zeroed(h, h->d_ex_closed, s.ex_closed, ne));
   }
@@ -988,7 +1021,8 @@ static int bind_problem(ksched_handle* h, const ksched_problem* pb) {
       // a term without any requirement is Compatible with every node (topologynodefilter.go:57-70): such a filter always matches
       for (uint32_t f = g.filter_begin; f < g.filter_end && f < (uint32_t)pb->n_filter_terms; ++f)
         if (((pb->filter_terms[f].meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF) == 0 &&
-            (!pb->filter_term_hostname || pb->filter_term_hostname[f] == KSCHED_NONE))
+            (!pb->filter_term_hostname || pb->filter_term_hostname[f] == KSCHED_NONE) &&
+            (!pb->filter_term_itype || pb->filter_term_itype[f] == KSCHED_NONE))
           x.has_filter = 0;
       x.max_skew = g.max_skew; x.host_row = host_row[ct.group];
       relx[e] = x;

@@ -721,6 +721,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
           s.ex_req_present[e] |= p_res;
           for (uint32_t m = p_ext; m; m &= m - 1) { const int x = __ffs(m) - 1; s.ex_req_ext[(size_t)x * NE + e] += s.cls_req_ext[(size_t)cls * X + x]; }
           node_hp_commit(s, p_hpe, p_hpx, cls, s.ex_hp, s.ex_hp_ext, NE, e);
+          if (s.ex_it && p_itype != KSCHED_NONE) itype_state_add(e, p_itype);
           if (has_vol) {  // volumeUsage.Add existingnode.go:128
             ksched_node_volumes nv = s.ex_vol[e];
             nv.mounted |= p_vol.shared;
@@ -902,6 +903,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
           if ((p_res >> kHotRes) || ((p_res & 0xF) & ~((fl >> 1) & 0xF))) s.nn_req_present[n] |= p_res;
           fl |= (unsigned short)((p_res & 0xF) << 1);
           node_hp_commit(s, p_hpe, p_hpx, cls, s.nn_hp, s.nn_hp_ext, MAXN, n);
+          if (s.nn_it && p_itype != KSCHED_NONE) itype_state_add(NE + n, p_itype);  // idempotent on a node that absorbed the class
           const int count = (int)(wkey >> 32) + 1;
           s.nn_count[n] = count;
           s.nn_tb[n] = -(tick + 1);  // front of the next pod-count block under a stable sort
@@ -1138,6 +1140,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
             s.nn_ext_present[n] = p_ext;
           }
           fresh_node_hp(s, p_hpe, p_hpx, cls, n);
+          if (s.nn_it) itype_state_open(n, v, p_itype);
           s.nn_count[n] = 1;
           s.nn_tb[n] = tick + 1;  // appended: last of the one-pod block
           const bool closed = node_closed(sh.q, s.min_req, RH, sh.bound, sh.bound2, sh.front_bits);
@@ -2288,6 +2291,7 @@ __device__ __forceinline__ void m1_store_fresh(const RunEnv& e) {
       s.nn_tmpl[n] = (uint8_t)(v.fl >> 8);
       s.nn_req_present[n] = v.qp;
       fresh_node_hp(s, 0, false, 0, n);
+      if (s.nn_it) itype_state_open(n, v.fl >> 8, KSCHED_NONE);  // the class run takes no instance-type class while the state is kept
       if (((e.rpv[a] >> 16) & 0x7FFF) == 0) {  // no further pod so far: (1, creation tick); otherwise the run's write-back stores them
         s.nn_count[n] = 1;
         s.nn_tb[n] = (int)((unsigned)e.hs->key[a] ^ 0x80000000u);
@@ -2598,6 +2602,7 @@ __device__ __forceinline__ bool run_fresh_step(const RunEnv& e, int buf, int i, 
     s.nn_tmpl[n] = (uint8_t)(v.fl >> 8);
     s.nn_req_present[n] = v.qp;
     fresh_node_hp(s, 0, false, 0, n);
+    if (s.nn_it) itype_state_open(n, v.fl >> 8, KSCHED_NONE);
     s.nn_count[n] = 1;
     s.nn_tb[n] = tk + 1;
     if (n_mask > 0) e.zv[a] = (1u << fd0) | (3u << 16);
@@ -3133,7 +3138,9 @@ __global__ void __launch_bounds__(kMaxThreads, 1) pack_kernel() {
     if (fast_allowed && s.use_class_run && qi < s.n_pods && n_active <= kActCap) {
       const bool topo_cls = nxt.topo_begin != nxt.topo_end;
       // (host-port classes never get here, so the variant store's signature, which reads the row words only, never meets one)
+      // (with the instance-type slot state, PackState::nn_it, only the generic step writes it: instance-type classes stay there)
       const bool shape_ok = !has_host_ports(s, nxt) && (nxt.res >> kHotRes) == 0 && !(kExt && class_ext(s, (unsigned)nxt.cls64)) &&
+                            (nxt.itype == KSCHED_NONE || !s.nn_it) &&
                             (!topo_cls || (((nxt.meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF) == 0 && nxt.itype == KSCHED_NONE && nxt.hostname == KSCHED_NONE));
       if (shape_ok && (unsigned)nxt.cls64 != run_block_cls) {
         if (fresh_valid && fresh_cls == (unsigned)nxt.cls64) skip_run = false;  // a fresh node of this class to capture

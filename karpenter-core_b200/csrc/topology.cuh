@@ -146,7 +146,16 @@ struct PackState {
   uint64_t* ex_hp_ext;               // [hp_ext_words][n_existing]
   uint64_t* nn_hp_ext;               // [hp_ext_words][max_new]
   int hp_ext_words;
+  // instance-type filter tables (ksched.h: filter_term_itype), all nullptr when no filter term names the key. Each slot's
+  // requirement on the key is a row [1 + W32]: word 0 the kIt* flags, then the admitted catalog types (itype_state_add).
+  const uint32_t* filter_itype;      // [n_filter_terms] itype_req entry or KSCHED_NONE
+  const uint32_t* tmpl_itype;        // [n_templates] itype_req entry a new node starts from, or KSCHED_NONE
+  uint32_t* ex_it;                   // [n_existing][1 + W32]
+  uint32_t* nn_it;                   // [max_new][1 + W32]
 };
+// flags of a slot's instance-type row: the node has the key; its complement bit (it admits every name outside the catalog,
+// which no requirement names); it admits its own label, a name outside the catalog (an existing node's, KSCHED_ITYPE_UNLISTED)
+constexpr uint32_t kItPresent = 1, kItComp = 2, kItOwn = 4;
 
 struct K2Params {
   DevCatalog cat;
@@ -598,8 +607,60 @@ __device__ __forceinline__ bool topo_prefilter(const uint64_t* vals, uint64_t me
   return true;
 }
 
+// ---- instance-type requirement of a slot (PackState::ex_it / nn_it), kept only when a filter term names the key
+__device__ __forceinline__ uint32_t* itype_row(const PackState& s, int W32, int slot) {
+  const size_t IW = 1 + (size_t)W32;
+  return slot < s.n_existing ? s.ex_it + (size_t)slot * IW : s.nn_it + (size_t)(slot - s.n_existing) * IW;
+}
+// Requirements.Add of itype_req entry `req` into the slot's requirement (ExistingNode.Add / Node.Add): the first one is
+// taken as it is, later ones intersect. A name outside the catalog survives only a complement entry.
+__device__ __noinline__ void itype_state_add(int slot, uint32_t req) {
+  KS_K2
+  uint32_t* r = itype_row(s, c.W32, slot);
+  const bool comp = s.itype_complement[req] != 0;
+  const uint32_t* set = s.itype_sets + (size_t)req * c.W32;
+  const uint32_t f = r[0];
+  r[0] = !(f & kItPresent) ? (kItPresent | (comp ? kItComp : 0u)) : (kItPresent | (comp ? (f & (kItComp | kItOwn)) : 0u));
+  for (int w = 0; w < c.W32; ++w) r[1 + w] = (f & kItPresent) ? (r[1 + w] & set[w]) : set[w];
+}
+// New node n of template v starts from its template's requirement (NewMachineTemplate), or without the key; then its first
+// pod's entry `req` (or KSCHED_NONE) is added
+__device__ __noinline__ void itype_state_open(int n, int v, uint32_t req) {
+  KS_K2
+  uint32_t* r = s.nn_it + (size_t)n * (1 + c.W32);
+  const uint32_t t = s.tmpl_itype[v];
+  r[0] = t == KSCHED_NONE ? 0u : (kItPresent | (s.itype_complement[t] ? kItComp : 0u));
+  if (t != KSCHED_NONE)
+    for (int w = 0; w < c.W32; ++w) r[1 + w] = s.itype_sets[(size_t)t * c.W32 + w];
+  if (req != KSCHED_NONE) itype_state_add(s.n_existing + n, req);
+}
+// Requirements.Intersects on the instance-type key (requirements.go:189-206) of the slot's requirement and filter term part
+// `req`: a node without the key passes; otherwise the intersection is not empty, or both operators are NotIn / DoesNotExist.
+// Out of line, like hostname_table_allows: problems without the tables do not carry its code in filter_matches.
+__device__ __noinline__ bool itype_filter_allows(int slot, uint32_t req) {
+  KS_K2
+  const uint32_t* r = itype_row(s, c.W32, slot);
+  const uint32_t f = r[0];
+  if (!(f & kItPresent)) return true;
+  const bool tcomp = s.itype_complement[req] != 0;
+  if (tcomp && (f & (kItComp | kItOwn))) return true;  // a name outside the catalog that both admit
+  const uint32_t* set = s.itype_sets + (size_t)req * c.W32;
+  int nn = 0, nt = 0;
+  for (int w = 0; w < c.W32; ++w) {
+    if (r[1 + w] & set[w]) return true;
+    nn += __popc(r[1 + w]);
+    nt += __popc(set[w]);
+  }
+  // Operator(): a complement is NotIn while it excludes a type, Exists otherwise; else In while it admits a name,
+  // DoesNotExist otherwise
+  const bool node_neg = (f & kItComp) ? nn < c.n_types : (nn == 0 && !(f & kItOwn));
+  const bool term_neg = tcomp ? nt < c.n_types : nt == 0;
+  return node_neg && term_neg;
+}
+
 // TopologyNodeFilter.MatchesRequirements (topologynodefilter.go:57-70): any term Compatible with the node requirements. A
-// term's hostname part reads the node's hostname: the slot's bit for an existing node, the placeholder flag for a new one.
+// term's hostname part reads the node's hostname: the slot's bit for an existing node, the placeholder flag for a new one;
+// its instance-type part the slot's instance-type requirement.
 __device__ __noinline__ bool filter_matches(const ksched_topo_group& g, const uint64_t* vals, uint64_t meta,
                                int stride, int idx, int slot) {
   KS_K2
@@ -608,6 +669,8 @@ __device__ __noinline__ bool filter_matches(const ksched_topo_group& g, const ui
     const ksched_reqset& term = s.filter_terms[f];
     const uint32_t host = s.filter_hostname ? s.filter_hostname[f] : KSCHED_NONE;
     bool ok = host == KSCHED_NONE || hostname_req_allows(s, host, slot, slot < s.n_existing);
+    const uint32_t it = s.filter_itype ? s.filter_itype[f] : KSCHED_NONE;
+    if (ok && it != KSCHED_NONE) ok = itype_filter_allows(slot, it);
     uint32_t keys = (uint32_t)(term.meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF;
     while (keys && ok) {
       int k = __ffs(keys) - 1;

@@ -128,6 +128,10 @@ struct HostnameReq {
     return s + "|" + (has_gt ? std::to_string(gt) : "") + "|" + (has_lt ? std::to_string(lt) : "");
   }
 };
+// A requirement on node.kubernetes.io/instance-type as (complement, names): the names it admits, or for a complement the
+// names it excludes (itype_intersection).
+using ItypeSet = std::pair<bool, std::set<std::string>>;
+
 // Requirements.Add of a pod's hostname requirements, in order (requirements.go:87-94)
 HostnameReq hostname_intersection(const std::vector<NodeSelectorRequirement>& rs) {
   HostnameReq h = HostnameReq::make(rs.at(0));
@@ -535,6 +539,10 @@ struct Builder {
   std::vector<std::optional<HostnameReq>> hostname_forms;
   std::map<std::string, uint32_t> hostname_table_id;       // HostnameReq::key() -> entry
   bool filter_names_hostname = false;                      // some topology node filter term has a hostname part
+  std::map<std::string, uint32_t> itype_req_id;            // (complement, names) -> itype_req entry (itype_entry)
+  // instance-type parts of topology node filter terms, in filter_terms order, and the templates' requirements on the key
+  std::vector<std::optional<ItypeSet>> filter_itype, template_itype;
+  std::string itype_unlisted;                              // a type name outside the catalog that a requirement keeps, or ""
 
   Builder(const Problem& p, Encoded& e, bool cluster_superset) : P(p), E(e), facts(cluster_facts(p)), superset(cluster_superset) {}
 
@@ -742,6 +750,7 @@ struct Group {
   bool filter_nil = true;
   std::vector<std::pair<ksched_reqset, ksched_bounds>> filter;  // TopologyNodeFilter terms
   std::vector<std::optional<HostnameReq>> filter_host;          // per term: its hostname part, if it names the hostname
+  std::vector<std::optional<ItypeSet>> filter_itype;            // per term: its instance-type part, if it names the key
   std::string filter_key;
   bool inverse = false;
   bool dormant = false;
@@ -1269,6 +1278,16 @@ std::pair<bool, std::set<std::string>> itype_intersection(const std::vector<Node
   }
   return {comp, names};
 }
+// Requirements.Intersects on the instance-type key of two requirements that both name it (requirements.go:189-206): the
+// intersection is not empty, or both operators are NotIn / DoesNotExist.
+bool itype_intersects(const ItypeSet& a, const ItypeSet& b) {
+  bool any = a.first && b.first;
+  for (auto& n : a.second) any = any || (a.first ? false : (b.first ? !b.second.count(n) : b.second.count(n) > 0));
+  for (auto& n : b.second) any = any || (!b.first && a.first && !a.second.count(n));
+  if (any) return true;
+  auto negative = [](const ItypeSet& s) { return s.first ? !s.second.empty() : s.second.empty(); };  // NotIn / DoesNotExist
+  return negative(a) && negative(b);
+}
 // Its instance-type columns: bit col % 64 of word col / 64 is set when the type of column col is admitted.
 std::vector<uint64_t> itype_columns(const Builder& B, const std::pair<bool, std::set<std::string>>& set) {
   std::vector<uint64_t> words((size_t)B.E.type_words, 0);
@@ -1277,6 +1296,23 @@ std::vector<uint64_t> itype_columns(const Builder& B, const std::pair<bool, std:
     if (set.first ? !in : in) words[col / 64] |= 1ull << (col % 64);
   }
   return words;
+}
+// The itype_req entry of a requirement, added when it is new. The columns keep only names of the catalog; the first other
+// name a requirement keeps is remembered, since a node filter that names the key needs such names told apart
+// (itype_filter_tables).
+uint32_t itype_entry(Builder& B, const ItypeSet& set) {
+  std::string key = std::to_string(set.first) + ":";
+  for (auto& n : set.second) {
+    key += n + ",";
+    if (B.itype_unlisted.empty() && !B.type_col.count(n)) B.itype_unlisted = n;
+  }
+  auto id = B.itype_req_id.emplace(key, (uint32_t)B.E.itype_req_complement.size());
+  if (id.second) {
+    B.E.itype_req_complement.push_back(set.first ? 1 : 0);
+    const std::vector<uint64_t> words = itype_columns(B, set);
+    B.E.itype_req_sets.insert(B.E.itype_req_sets.end(), words.begin(), words.end());
+  }
+  return id.first->second;
 }
 
 // ------------------------------------------------------------------ templates
@@ -1298,6 +1334,7 @@ void templates(Builder& B) {
     // instance-type requirement of the provisioner: fold into membership (types are singletons on that key); without instance
     // types nothing is folded (nor refused)
     const std::vector<uint64_t> allowed = NT ? itype_columns(B, itype_intersection(sp.itype)) : std::vector<uint64_t>((size_t)E.type_words, 0);
+    B.template_itype.push_back(sp.itype.empty() ? std::nullopt : std::optional<ItypeSet>(itype_intersection(sp.itype)));
     for (int idx : pr.instance_types) {
       int c = B.type_col.at(P.instance_types.at(idx).name);
       if ((allowed[c / 64] >> (c % 64)) & 1) E.types[c].template_members |= 1ull << v;
@@ -1590,12 +1627,19 @@ struct Topology {
       Builder::Special sp;
       B.add_selector_reqs(rs, bd, label_reqs(p.node_selector), &sp);
       if (term) B.add_selector_reqs(rs, bd, *term, &sp);
-      if (!sp.itype.empty()) unsupported("topology spread node filter on instance-type");
       std::optional<HostnameReq> host;
       if (!sp.hostname.empty()) host = hostname_intersection(sp.hostname);
+      std::optional<ItypeSet> itype;  // Gt/Lt refused by itype_intersection
+      std::string itype_key;
+      if (!sp.itype.empty()) {
+        itype = itype_intersection(sp.itype);
+        itype_key = "itype:" + std::to_string(itype->first) + ":";
+        for (auto& n : itype->second) itype_key += n + ",";
+      }
       g.filter.push_back({rs, bd});
       g.filter_host.push_back(host);
-      parts.push_back(canon(rs, bd) + (host ? "hostname:" + host->key() : ""));
+      g.filter_itype.push_back(itype);
+      parts.push_back(canon(rs, bd) + (host ? "hostname:" + host->key() : "") + itype_key);
     };
     if (!p.has_node_affinity || !p.has_required_node_affinity) add_term(nullptr);
     else for (auto& t : p.required_node_terms) add_term(&t);
@@ -1613,6 +1657,8 @@ struct Topology {
         auto l = labels.find(kHostname);
         if (l == labels.end() ? !h->admits_unlabelled() : !h->has(l->second)) continue;
       }
+      // the labels' instance type In [label], on strings; a node without the label does not have the key
+      if (g.filter_itype[t] && !sp.itype.empty() && !itype_intersects(itype_intersection(sp.itype), *g.filter_itype[t])) continue;
       return true;
     }
     return false;
@@ -1724,6 +1770,7 @@ void group_tables(Builder& B, const std::vector<Group>& groups) {
       const auto& h = G.filter_host[t];
       E.filter_term_hostname.push_back(h ? B.hostname_table(*h) : KSCHED_NONE);
       if (h) B.filter_names_hostname = true;
+      B.filter_itype.push_back(G.filter_itype[t]);  // entries after the classes' (itype_filter_tables)
     }
     o.filter_end = (uint32_t)E.filter_terms.size();
     if (G.key == kHostname) {
@@ -1841,7 +1888,6 @@ void class_rows(Builder& B, const std::vector<Group>& groups) {
   const int NC = (int)B.specs.size(), NG = (int)groups.size();
   E.classes.resize(NC);
   E.class_bounds.resize(NC);
-  std::map<std::string, uint32_t> itype_req_id;
   // (class, group) relations: selector matches of every class against every group, on all cores (pure reads)
   std::vector<uint8_t> rel((size_t)NC * std::max(NG, 1), 0);
   parallel_ranges((size_t)NC, 16, [&](size_t cb, size_t ce) {
@@ -1888,18 +1934,7 @@ void class_rows(Builder& B, const std::vector<Group>& groups) {
     row.reserved = (uint64_t)c;  // class index, so a row copied into the FFD-ordered pod matrix knows its class
     row.itype_req = KSCHED_NONE;
     row.hostname_req = KSCHED_NONE;
-    if (!sp.itype.empty()) {
-      const auto set = itype_intersection(sp.itype);
-      std::string key = std::to_string(set.first) + ":";
-      for (auto& n : set.second) key += n + ",";
-      auto id = itype_req_id.emplace(key, (uint32_t)E.itype_req_complement.size());
-      row.itype_req = id.first->second;
-      if (id.second) {
-        E.itype_req_complement.push_back(set.first ? 1 : 0);
-        const std::vector<uint64_t> words = itype_columns(B, set);
-        E.itype_req_sets.insert(E.itype_req_sets.end(), words.begin(), words.end());
-      }
-    }
+    if (!sp.itype.empty()) row.itype_req = itype_entry(B, itype_intersection(sp.itype));
     std::optional<HostnameReq> host;
     if (!sp.hostname.empty()) {
       // every hostname requirement of the class at its relaxation level (node selector, required term, heaviest preferred
@@ -1946,6 +1981,39 @@ void class_rows(Builder& B, const std::vector<Group>& groups) {
     if (!any) E.class_volumes.clear();  // no pod of the batch mounts a limited claim: the kernels never look
     for (auto& kv : B.vol_tracked) E.volume_driver_mask[B.driver_index(kv.first.first)] |= 1ull << kv.second;
   }
+}
+
+// ------------------------------------------------------------------ instance-type filter tables
+// When some topology node filter term names the instance type, Topology.Record and countDomains ask whether the node's
+// requirement on the key Intersects the term's. A new node's requirement is its template's (NewMachineTemplate) ∩ its pods',
+// an existing node's In [its label] ∩ its pods' (ExistingNode.Add). The device carries them as itype_req entries, which
+// keep only names of the catalog: every name outside it is then one that no requirement names, and the entry's complement
+// bit stands for all of them at once. An existing node's label outside the catalog is such a name of its own
+// (KSCHED_ITYPE_UNLISTED). A requirement that keeps a name outside the catalog would need that name told apart: refused.
+// Entries are added after the classes', so problems without such terms encode as before.
+void itype_filter_tables(Builder& B) {
+  Encoded& E = B.E;
+  bool any = false;
+  for (auto& f : B.filter_itype) any = any || f.has_value();
+  if (!any) return;
+  for (auto& f : B.filter_itype) E.filter_term_itype.push_back(f ? itype_entry(B, *f) : KSCHED_NONE);
+  for (auto& t : B.template_itype) E.template_itype.push_back(t ? itype_entry(B, *t) : KSCHED_NONE);
+  for (size_t e = 0; e < E.existing.size(); ++e) {
+    const StateNode& n = B.P.nodes[(size_t)E.existing_state_index[e]];
+    Builder::Special sp;
+    ksched_reqset rs{}; ksched_bounds bd{};
+    B.add_selector_reqs(rs, bd, label_reqs(n.labels), &sp);
+    uint32_t v = KSCHED_NONE;
+    if (!sp.itype.empty()) {
+      const ItypeSet own = itype_intersection(sp.itype);  // In [label] (both label keys when a node carries both)
+      bool listed = true;  // at most one name: In [a] ∩ In [b] is DoesNotExist
+      for (auto& name : own.second) listed = listed && B.type_col.count(name) > 0;
+      v = listed ? itype_entry(B, own) : KSCHED_ITYPE_UNLISTED;
+    }
+    E.existing_itype.push_back(v);
+  }
+  if (!B.itype_unlisted.empty())
+    unsupported("instance-type requirement naming " + B.itype_unlisted + ", a type outside the catalog, with an instance-type node filter");
 }
 
 // ------------------------------------------------------------------ per-pod queue keys (queue.go:74-110)
@@ -2000,6 +2068,11 @@ void wire(Builder& B) {
     pr.hostname_slots = E.hostname_slots.data();
     pr.n_hostname_words = E.hostname_words;
     pr.filter_term_hostname = E.filter_term_hostname.empty() ? nullptr : E.filter_term_hostname.data();
+  }
+  if (!E.filter_term_itype.empty()) {
+    pr.filter_term_itype = E.filter_term_itype.data();
+    pr.template_itype = E.template_itype.data();
+    pr.existing_itype = NE > 0 ? E.existing_itype.data() : nullptr;
   }
   pr.max_new_nodes = (int)E.pods.size();
   if (!E.class_volumes.empty() && NE > 0) {
@@ -2063,6 +2136,7 @@ std::unique_ptr<Encoded> encode(const Problem& P, const std::vector<int>& candid
   B.phase("topology groups");
   class_rows(B, groups);
   B.phase("class rows");
+  itype_filter_tables(B);
   queue_keys(B);
   B.phase("queue keys");
   wire(B);

@@ -89,6 +89,10 @@ struct Encoded {
   int hostname_words = 0;                             // ksched.h: n_hostname_words; 0 when every entry is a {complement, slot} pair
   std::vector<uint64_t> hostname_slots;               // [n_hostname_reqs][hostname_words] admitted existing slots; empty without
   std::vector<uint32_t> filter_term_hostname;         // [n_filter_terms] hostname_reqs entry or KSCHED_NONE; empty when no term names it
+  // instance-type filter tables (ksched.h: filter_term_itype): itype_req entries or KSCHED_NONE; all empty when no term names it
+  std::vector<uint32_t> filter_term_itype;            // [n_filter_terms]
+  std::vector<uint32_t> template_itype;               // [n_templates]
+  std::vector<uint32_t> existing_itype;               // [n_existing] (KSCHED_ITYPE_UNLISTED: a label outside the catalog)
   std::vector<ksched_class_volumes> class_volumes;    // CSI volume limits (ksched.h); empty when no pod mounts a limited claim
   std::vector<ksched_node_volumes> existing_volumes;
   uint64_t volume_driver_mask[KSCHED_MAX_VOLUME_DRIVERS] = {};

@@ -360,9 +360,12 @@ void kh_encoded_free(Encoded* E) {
   delete E;
 }
 // dims: [pods, classes, existing, groups, types, templates, keys, resources, type_words, class_topo, taintsets, resources_ext,
-//        hostports, hostport_ext_words, hostname_reqs, hostname_words]
+//        hostports, hostport_ext_words, hostname_reqs, hostname_words, itype_reqs, itype_filter_terms]
+// (itype_filter_terms: filter terms with an instance-type part; 0 exactly when the problem has no instance-type filter tables)
 void kh_encoded_dims(const Encoded* E, long long* out) {
   out[14] = (long long)E->hostname_reqs.size() / 2; out[15] = E->hostname_words;
+  out[16] = (long long)E->itype_req_complement.size();
+  out[17] = (long long)std::count_if(E->filter_term_itype.begin(), E->filter_term_itype.end(), [](uint32_t v) { return v != KSCHED_NONE; });
   out[0] = (long long)E->pods.size(); out[1] = (long long)E->classes.size(); out[2] = (long long)E->existing.size();
   out[3] = (long long)E->groups.size(); out[4] = (long long)E->types.size(); out[5] = (long long)E->templates.size();
   out[6] = (long long)E->key_names.size(); out[7] = (long long)E->res_names.size() - E->n_res_ext; out[8] = E->type_words;
@@ -392,6 +395,16 @@ int kh_encoded_hostname_req(const Encoded* E, int i, long long* out, int cap) {
     out[k++] = e;
   }
   return k - 1;
+}
+// total initial count of group g over its domains (countDomains, tests): mask-key domains, or existing slots for a hostname
+// group; -1 out of range
+long long kh_encoded_group_total(const Encoded* E, int g) {
+  if (g < 0 || (size_t)g >= E->groups.size()) return -1;
+  const size_t NE = std::max<size_t>(E->existing.size(), 1);
+  long long t = 0;
+  for (int d = 0; d < 64; ++d) t += E->group_domain_counts[(size_t)g * 64 + d];
+  for (size_t e = 0; e < E->existing.size(); ++e) t += E->group_existing_counts[(size_t)g * NE + e];
+  return t;
 }
 // initial class of pod i of Solve's pod list (tests), -1 out of range
 long long kh_encoded_pod_class(const Encoded* E, int i) {
@@ -1348,6 +1361,7 @@ extern "C" unsigned long long kh_encoded_digest(const Encoded* E) {
     vec(E->class_hostport_conflicts_ext); vec(E->class_hostport_entries_ext); vec(E->existing_hostport_ext);
   }
   if (E->hostname_words) { vec(E->hostname_slots); vec(E->filter_term_hostname); }  // absent without the hostname table: those digests predate it
+  if (!E->filter_term_itype.empty()) { vec(E->filter_term_itype); vec(E->template_itype); vec(E->existing_itype); }  // likewise
   if (E->n_res_ext) {  // absent with at most 8 read resources: those digests predate ext resources
     bytes(&E->n_res_ext, sizeof E->n_res_ext);
     vec(E->type_alloc_ext); vec(E->class_requests_ext); vec(E->class_res_ext_present); vec(E->existing_available_ext);

@@ -200,8 +200,11 @@ typedef struct ksched_existing_node {
  * The API Gets of VolumeUsage.validate (:133-190: claim -> storage class / bound volume -> CSI driver) are the caller's; what
  * crosses the ABI is counting. Only drivers that some existing node limits matter (<= KSCHED_MAX_VOLUME_DRIVERS). A claim that
  * exactly one pod of (batch + bound pods) mounts is counted (priv / used); a claim several pods share is a TRACKED id, one bit
- * of a 64-bit mask, so that mounting it twice on a node counts once (volumes.union, :55-70). Pod p fits node e iff for every
- * limited driver d:  used[d] + popcount((mounted | shared) & volume_driver_mask[d]) + priv[d] <= limit[d].
+ * of a mask, so that mounting it twice on a node counts once (volumes.union, :55-70). When that rule would track more than 64
+ * claims, a claim is tracked only when two different pods mount it and one of them is a pod of the batch; a claim only bound
+ * pods mount stays in each node's used[]. Ids 0-63 are bits of shared / mounted / volume_driver_mask[d], ids from 64 on bits
+ * of the problem's *_volumes_*_ext tables (see class_volumes_shared_ext). Pod p fits node e iff for every limited driver d:
+ *   used[d] + popcount over all words of ((mounted | shared) & volume_driver_mask[d]) + priv[d] <= limit[d].
  * A node that already exceeds a limit accepts nobody (Exceeds walks the node's own drivers too, :101-112): the caller marks it
  * by an `available` vector no pod fits.
  */
@@ -314,6 +317,15 @@ typedef struct ksched_problem {
   const uint32_t* filter_term_itype;     /* [n_filter_terms] */
   const uint32_t* template_itype;        /* [catalog n_templates] */
   const uint32_t* existing_itype;        /* [n_existing] */
+  /* Tracked volume claims beyond the 64 of ksched_class_volumes.shared, ksched_node_volumes.mounted and volume_driver_mask.
+     Claim t >= 64 is bit (t - 64) % 64 of word (t - 64) / 64 of a row of these tables; claims 0-63 stay in the words. Relaxed
+     classes are classes and have rows too. All three NULL and the count 0 when at most 64 claims are tracked, and they need
+     class_volumes / existing_volumes; ksched_upload answers KSCHED_ERR_INVALID when the tables and the count disagree. */
+  const uint64_t* class_volumes_shared_ext;     /* [n_classes][n_volume_ext_words] */
+  const uint64_t* existing_volumes_mounted_ext; /* [n_existing][n_volume_ext_words] */
+  const uint64_t* volume_driver_mask_ext;       /* [KSCHED_MAX_VOLUME_DRIVERS][n_volume_ext_words] */
+  int32_t n_volume_ext_words;
+  int32_t pad_volume;
 } ksched_problem;
 
 typedef struct ksched_new_node {

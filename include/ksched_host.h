@@ -117,6 +117,11 @@ int kh_consolidate_validated(const kh_problem* before, const kh_problem* after, 
 int kh_consolidate_single_validated(const kh_problem* before, const kh_problem* after, int first, int last, int batch, int* out4, int* node,
                                     int* options, int options_cap, int* trace, int* trace_valid, int trace_cap, int* n_trace, int* failed_validation);
 
+/* ---- an encoding's volume claims (tests): `enc` is an encoding of kh_encode / kh_encode_cluster. Tracked claim `id` as
+ * "driver claim" into out[cap], in id order (ksched.h: ksched_class_volumes); -1 when there is no such claim or it does not
+ * fit. */
+int kh_encoded_volume_claim(const void* enc, int id, char* out, int cap);
+
 /* ---- self-test of the encoder's value classes (CPU, no device): random wide keys and requirement pairs, the exact string
  * algebra against the collapsed masks (host form and region form). Returns the number of mismatches. */
 int kh_value_class_selftest(unsigned seed, int iters);

@@ -127,6 +127,7 @@ def lib():
     L.kh_encoded_key_info.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(C.c_longlong)]
     L.kh_encoded_resource_id.argtypes = [C.c_void_p, C.c_char_p]
     L.kh_encoded_hostport.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_int]
+    L.kh_encoded_volume_claim.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_int]
     L.kh_encoded_hostname_req.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_longlong), C.c_int]
     L.kh_encoded_class_hostname.argtypes = [C.c_void_p, C.c_int]
     L.kh_encoded_class_hostname.restype = C.c_longlong
@@ -581,11 +582,11 @@ class ResidentSolve:
         if not self.enc:
             msg = lib().kh_scheduler_error().decode()
             raise KschedError(KSCHED_ERR_UNSUPPORTED if msg.startswith("unsupported:") else KSCHED_ERR_INVALID, msg)
-        d = (C.c_longlong * 18)()
+        d = (C.c_longlong * 20)()
         lib().kh_encoded_dims(self.enc, d)
         self.dims = dict(zip(["pods", "classes", "existing", "groups", "types", "templates", "keys", "resources", "type_words", "class_topo",
                               "taintsets", "resources_ext", "hostports", "hostport_ext_words", "hostname_reqs", "hostname_words",
-                              "itype_reqs", "itype_filter_terms"], list(d)))
+                              "itype_reqs", "itype_filter_terms", "volume_claims", "volume_ext_words"], list(d)))
 
     def hostname_reqs(self):
         """every hostname requirement of this encoding in entry order, as (admits new nodes, [admitted existing slots])"""
@@ -615,6 +616,14 @@ class ResidentSolve:
         while lib().kh_encoded_hostport(self.enc, len(out), buf, len(buf)) == 0:
             ip, port, proto = buf.value.decode().split(" ")
             out.append((ip, int(port), proto))
+        return out
+
+    def volume_claims(self):
+        """the tracked volume claims of this encoding in id order, as (driver, claim)"""
+        out, buf = [], C.create_string_buffer(1024)
+        while lib().kh_encoded_volume_claim(self.enc, len(out), buf, len(buf)) == 0:
+            driver, claim = buf.value.decode().split(" ", 1)
+            out.append((driver, claim))
         return out
 
     def key_info(self, key):

@@ -223,10 +223,10 @@ struct ksched_handle {
   DevBuf<ksched_class_volumes> d_cls_vol;
   DevBuf<int32_t> d_hostname_reqs, d_grp_host_row;
   DevBuf<int64_t> d_ts, d_ex_avail, d_cls_req_ext, d_ex_avail_ext;
-  DevBuf<uint8_t> d_itype_comp, d_cls_hp_ext;
+  DevBuf<uint8_t> d_itype_comp, d_cls_hp_ext, d_cls_has_vol;
   DevBuf<uint32_t> d_pod_class0, d_uid_rank, d_itype_sets, d_filter_hostname, d_cls_rank, d_cls_ext_present, d_ex_avail_present, d_ex_taintset,
       d_ex_itype;
-  DevBuf<uint64_t> d_hostname_slots, d_cls_tol_ext, d_cls_hpc_ext, d_cls_hpe_ext;
+  DevBuf<uint64_t> d_hostname_slots, d_cls_tol_ext, d_cls_hpc_ext, d_cls_hpe_ext, d_cls_vol_ext, d_vol_mask_ext;
   DevBuf<uint32_t> d_filter_itype, d_tmpl_itype, d_ex_it0, d_ex_it, d_nn_it;  // instance-type filter tables and slot state
   // pristine copies of what a Solve mutates
   DevBuf<ksched_node_volumes> d_ex_vol0;
@@ -235,7 +235,7 @@ struct ksched_handle {
   DevBuf<uint8_t> d_grp_active0;
   DevBuf<uint16_t> d_grp_host0;
   DevBuf<uint32_t> d_ex_req_present0;
-  DevBuf<uint64_t> d_ex_vals0, d_ex_meta0, d_ex_hp0, d_ex_hp_ext0, d_grp_registered0;
+  DevBuf<uint64_t> d_ex_vals0, d_ex_meta0, d_ex_hp0, d_ex_hp_ext0, d_ex_vol_ext0, d_grp_registered0;
   // working state
   DevBuf<ksched_node_volumes> d_ex_vol;
   DevBuf<int32_t> d_relax, d_assign, d_place_seq, d_last_len, d_cls_cursor, d_grp_cnt, d_grp_host_total, d_grp_min_slot;
@@ -243,7 +243,7 @@ struct ksched_handle {
   DevBuf<uint8_t> d_ex_closed, d_grp_active;
   DevBuf<uint16_t> d_grp_host;
   DevBuf<uint32_t> d_pod_class, d_queue, d_last_epoch, d_ex_req_present;
-  DevBuf<uint64_t> d_ex_vals, d_ex_meta, d_ex_hp, d_ex_hp_ext, d_grp_registered;
+  DevBuf<uint64_t> d_ex_vals, d_ex_meta, d_ex_hp, d_ex_hp_ext, d_ex_vol_ext, d_grp_registered;
   DevBuf<long long> d_counters;  // kNumCounters entries (Counter)
   // K0 / K1
   DevBuf<uint32_t> d_order, d_idx_tmp, d_pod_pos, d_F, d_Fclass;
@@ -795,6 +795,17 @@ static int check_problem(ksched_handle* h, const ksched_problem* pb) {
     return KSCHED_ERR_INVALID;
   }
   {
+    // tracked volume claims from id 64 on: the three tables exist exactly when the count is positive, and only beside the
+    // volume tables they extend
+    const int VW = pb->n_volume_ext_words;
+    const bool vol = pb->class_volumes && pb->existing_volumes && NE > 0;
+    if (VW < 0 || !present_iff(VW > 0, {pb->class_volumes_shared_ext, pb->existing_volumes_mounted_ext, pb->volume_driver_mask_ext}, nullptr, true) ||
+        (VW > 0 && !vol)) {
+      h->err = "volume claim tables must be set exactly when n_volume_ext_words is positive, with class_volumes and existing_volumes";
+      return KSCHED_ERR_INVALID;
+    }
+  }
+  {
     // hostname requirement table: wide enough for every existing slot, and present when an entry reads it
     bool ok = HW >= 0 && present_iff(HW > 0, {pb->hostname_slots}, pb->filter_term_hostname, true) && (HW == 0 || (int64_t)HW * 64 >= NE);
     for (int i = 0; ok && i < pb->n_hostname_reqs; ++i) ok = pb->hostname_reqs[2 * i + 1] != KSCHED_HOSTNAME_TABLE || HW > 0;
@@ -963,6 +974,26 @@ static int bind_problem(ksched_handle* h, const ksched_problem* pb) {
       CUDA_TRY(h, bind(h, h->d_cls_vol, s.cls_vol, (size_t)NC, pb->class_volumes));
       CUDA_TRY(h, bind_restored(h, h->d_ex_vol, s.ex_vol, h->d_ex_vol0, (size_t)NE, pb->existing_volumes));
       std::memcpy(s.vol_mask, pb->volume_driver_mask, sizeof s.vol_mask);
+      // tracked claims from id 64 on: per-class table and driver masks as given, the existing nodes' words as [word][node];
+      // and per class whether it mounts a claim at all (its row or its table words)
+      const int VW = pb->n_volume_ext_words;
+      s.vol_ext_words = VW;
+      std::vector<uint8_t> has_vol(nc, 0);
+      for (int i = 0; i < NC; ++i) {
+        const ksched_class_volumes& v = pb->class_volumes[i];
+        has_vol[i] = (v.shared | v.priv[0] | v.priv[1] | v.priv[2] | v.priv[3]) != 0;
+        for (int w = 0; w < VW; ++w) has_vol[i] |= pb->class_volumes_shared_ext[(size_t)i * VW + w] != 0;
+      }
+      CUDA_TRY(h, bind(h, h->d_cls_has_vol, s.cls_has_vol, has_vol.size(), has_vol.data()));
+      std::vector<uint64_t> vol_ext(VW > 0 ? (size_t)VW * ne : 0, 0);
+      if (VW > 0) {
+        for (int e = 0; e < NE; ++e)
+          for (int w = 0; w < VW; ++w) vol_ext[(size_t)w * NE + e] = pb->existing_volumes_mounted_ext[(size_t)e * VW + w];
+        CUDA_TRY(h, bind(h, h->d_cls_vol_ext, s.cls_vol_ext, (size_t)NC * VW, pb->class_volumes_shared_ext));
+        CUDA_TRY(h, bind(h, h->d_vol_mask_ext, s.vol_mask_ext, (size_t)KSCHED_MAX_VOLUME_DRIVERS * VW, pb->volume_driver_mask_ext));
+        CUDA_TRY(h, bind_restored(h, h->d_ex_vol_ext, s.ex_vol_ext, h->d_ex_vol_ext0, vol_ext.size(), vol_ext.data()));
+      }
+      CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // host vectors go out of scope
     }
     // instance-type requirement of every slot (topology.cuh: itype_state_add), only when a filter term names the key
     std::vector<uint32_t> ex_it;

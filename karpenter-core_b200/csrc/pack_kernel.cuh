@@ -425,10 +425,41 @@ struct LoopVars {
 // exclusive prefix sum of K over the nodes from the class's cursor on. Every effect of the sequential commits is reproduced
 // (requests, closed flag, assign, place_seq); what the existing nodes cannot take is left to the generic step.
 constexpr int kExRunMax = 1 << 20;
-__device__ __forceinline__ bool class_has_volumes(const PackState& s, unsigned cls) {
-  if (!s.cls_vol) return false;
-  const ksched_class_volumes v = s.cls_vol[cls];
-  return (v.shared | v.priv[0] | v.priv[1] | v.priv[2] | v.priv[3]) != 0;
+// CSI volume limits (ksched.h: ksched_class_volumes). Tracked claims 0-63 are bits of the row's and the nodes' words; from 64
+// on they are words of the per-class table and of the nodes' [word][node] array (ksched.h: class_volumes_shared_ext). A class
+// whose tracked claims all have ids from 64 on and that has no private claim has a zero row, so the gates read the per-class
+// "mounts a claim" byte the upload derives from the row and the table (one byte load where the row test took 16 bytes).
+__device__ __forceinline__ bool class_has_volumes(const PackState& s, unsigned cls) { return s.cls_has_vol && s.cls_has_vol[cls]; }
+// Both volume helpers are out of line, like hostname_table_allows: the generic step carries a call, not the driver loop and
+// the table loops (DESIGN.md §3).
+// volumeUsage.Validate(pod).Exceeds(volumeLimits) of existing node e for a class with volumes (existingnode.go:88-96)
+__device__ __noinline__ bool node_vol_over(unsigned cls, int e) {
+  KS_K2
+  const ksched_node_volumes nv = s.ex_vol[e];
+  const ksched_class_volumes pv = s.cls_vol[cls];
+  const uint64_t all = nv.mounted | pv.shared;
+  const int W = s.vol_ext_words, NE = s.n_existing;
+  const uint64_t* cw = s.cls_vol_ext + (size_t)cls * W;
+  for (int d = 0; d < KSCHED_MAX_VOLUME_DRIVERS; ++d) {
+    if (nv.limit[d] < 0) continue;
+    const uint64_t* mw = s.vol_mask_ext + (size_t)d * W;
+    int n = nv.used[d] + __popcll(all & s.vol_mask[d]) + (int)pv.priv[d];
+    for (int w = 0; w < W; ++w) n += __popcll((s.ex_vol_ext[(size_t)w * NE + e] | cw[w]) & mw[w]);
+    if (n > nv.limit[d]) return true;
+  }
+  return false;
+}
+// volumeUsage.Add (existingnode.go:128): the class's claims join those existing node e mounts
+__device__ __noinline__ void node_vol_commit(unsigned cls, int e) {
+  KS_K2
+  ksched_node_volumes nv = s.ex_vol[e];
+  const ksched_class_volumes pv = s.cls_vol[cls];
+  nv.mounted |= pv.shared;
+#pragma unroll
+  for (int d = 0; d < KSCHED_MAX_VOLUME_DRIVERS; ++d) nv.used[d] += (int)pv.priv[d];
+  s.ex_vol[e] = nv;
+  const int W = s.vol_ext_words, NE = s.n_existing;
+  for (int w = 0; w < W; ++w) s.ex_vol_ext[(size_t)w * NE + e] |= s.cls_vol_ext[(size_t)cls * W + w];
 }
 // Taints.Tolerates (taints.go:28-40) of an existing node's taint set. Ids below 64 are bits of the row's word; ids from 64 on
 // only existing nodes carry (ksched.h: class_tolerated_ext), and they live in the per-class table.
@@ -639,12 +670,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
     const bool simple = !has_topo && p_hpc == 0 && p_hpe == 0 && !p_hpx && !p_ext;  // the requirement verdict memo (HotSmem::absorbed/rejected) applies
 
     bool placed = false;
-    ksched_class_volumes p_vol{};
-    bool has_vol = false;
-    if (s.cls_vol) {
-      p_vol = s.cls_vol[cls];
-      has_vol = (p_vol.shared | p_vol.priv[0] | p_vol.priv[1] | p_vol.priv[2] | p_vol.priv[3]) != 0;
-    }
+    const bool has_vol = class_has_volumes(s, cls);
     GK_T(kCtrGenTopo)
     // ------------------------------------------------------------ 1) existing nodes in caller order (scheduler.go:176-180)
     if (NE > 0) {
@@ -659,15 +685,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
         if (s.ex_closed[e]) continue;
         if (!tolerates_node_set(s, p_tol, cls, s.ex_taintset[e])) continue;
         if (node_hp_conflict(s, p_hpc, p_hpx, cls, s.ex_hp, s.ex_hp_ext, NE, e)) continue;
-        if (has_vol) {  // volumeUsage.Validate(pod).Exceeds(volumeLimits) existingnode.go:88-96
-          const ksched_node_volumes nv = s.ex_vol[e];
-          const uint64_t all = nv.mounted | p_vol.shared;
-          bool over = false;
-#pragma unroll
-          for (int d = 0; d < KSCHED_MAX_VOLUME_DRIVERS; ++d)
-            over = over || (nv.limit[d] >= 0 && nv.used[d] + __popcll(all & s.vol_mask[d]) + (int)p_vol.priv[d] > nv.limit[d]);
-          if (over) continue;
-        }
+        if (has_vol && node_vol_over(cls, e)) continue;
         bool ok = true;  // Fits(requests, available) comes first (existingnode.go:98-102)
         const uint32_t qp = s.ex_req_present[e] | p_res;
         for (int r = 0; r < R && ok; ++r) {
@@ -722,13 +740,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
           for (uint32_t m = p_ext; m; m &= m - 1) { const int x = __ffs(m) - 1; s.ex_req_ext[(size_t)x * NE + e] += s.cls_req_ext[(size_t)cls * X + x]; }
           node_hp_commit(s, p_hpe, p_hpx, cls, s.ex_hp, s.ex_hp_ext, NE, e);
           if (s.ex_it && p_itype != KSCHED_NONE) itype_state_add(e, p_itype);
-          if (has_vol) {  // volumeUsage.Add existingnode.go:128
-            ksched_node_volumes nv = s.ex_vol[e];
-            nv.mounted |= p_vol.shared;
-#pragma unroll
-            for (int d = 0; d < KSCHED_MAX_VOLUME_DRIVERS; ++d) nv.used[d] += (int)p_vol.priv[d];
-            s.ex_vol[e] = nv;
-          }
+          if (has_vol) node_vol_commit(cls, e);
           s.ex_closed[e] = closed;
           s.assign[pod] = e;
           s.place_seq[pod] = seq;

@@ -59,6 +59,7 @@ struct PackState {
   uint8_t* ex_closed;
   int32_t* cls_cursor;                  // [n_classes] existing nodes below it refuse the class for good (pack_kernel.cuh, generic step 1)
   const ksched_class_volumes* cls_vol;  // [n_classes] or nullptr: CSI volume limits (ksched.h)
+  const uint8_t* cls_has_vol;           // [n_classes] 1: the class mounts a claim (row or claim table), nullptr with cls_vol
   ksched_node_volumes* ex_vol;          // [n_existing]
   uint64_t vol_mask[KSCHED_MAX_VOLUME_DRIVERS];
   // new nodes (SoA, capacity max_new)
@@ -146,6 +147,11 @@ struct PackState {
   uint64_t* ex_hp_ext;               // [hp_ext_words][n_existing]
   uint64_t* nn_hp_ext;               // [hp_ext_words][max_new]
   int hp_ext_words;
+  // tracked volume claims from id 64 on (ksched.h: class_volumes_shared_ext), all nullptr without them
+  const uint64_t* cls_vol_ext;       // [n_classes][vol_ext_words]
+  const uint64_t* vol_mask_ext;      // [KSCHED_MAX_VOLUME_DRIVERS][vol_ext_words]
+  uint64_t* ex_vol_ext;              // [vol_ext_words][n_existing]
+  int vol_ext_words;
   // instance-type filter tables (ksched.h: filter_term_itype), all nullptr when no filter term names the key. Each slot's
   // requirement on the key is a row [1 + W32]: word 0 the kIt* flags, then the admitted catalog types (itype_state_add).
   const uint32_t* filter_itype;      // [n_filter_terms] itype_req entry or KSCHED_NONE

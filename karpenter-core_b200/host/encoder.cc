@@ -634,9 +634,10 @@ struct Builder {
     if (it == hp_id.end()) throw std::runtime_error("internal: host-port entry missing from the table");
     return it->second;
   }
-  // entry `id`'s bit: of `word` below 64, of ext[(id - 64) / 64] (a table row of E.hostport_ext_words words) from 64 on
-  static void hp_bit(int id, uint64_t& word, uint64_t* ext) {
-    if (id < 0) return;  // left out: the entry can turn no pod away
+  // host-port entry or tracked volume claim `id`'s bit: of `word` below 64, of ext[(id - 64) / 64] (a table row of
+  // E.hostport_ext_words / E.volume_ext_words words) from 64 on
+  static void id_bit(int id, uint64_t& word, uint64_t* ext) {
+    if (id < 0) return;  // a host-port entry left out: it can turn no pod away
     if (id < 64) word |= 1ull << id;
     else ext[(id - 64) / 64] |= 1ull << ((id - 64) % 64);
   }
@@ -680,22 +681,33 @@ struct Builder {
       if (!v.driver.empty() && driver_index(v.driver) < vol_drivers.size()) m[v.driver].insert(v.pvc_id);
     return m;
   }
-  std::string volume_signature(const Pod& p, ksched_class_volumes* out) const {
+  // The class's claims (out, and its tracked claims from id 64 on into ext[E.volume_ext_words] when given) and their part of
+  // the class key: "" without a claim. The key carries every word, so pods that differ in a claim beyond 64 stay apart.
+  std::string volume_signature(const Pod& p, ksched_class_volumes* out, uint64_t* ext = nullptr) const {
     ksched_class_volumes cv{};
+    std::vector<uint64_t> words((size_t)E.volume_ext_words, 0);
     if (!vol_drivers.empty())
       for (auto& kv : pod_claims(p)) {
         const size_t d = driver_index(kv.first);
         for (auto& c : kv.second) {
           auto t = vol_tracked.find({kv.first, c});
-          if (t != vol_tracked.end()) cv.shared |= 1ull << t->second;
+          if (t != vol_tracked.end()) id_bit(t->second, cv.shared, words.data());
           else if (cv.priv[d] == 0xFFFF) unsupported("more than 65535 volume claims on one pod");
           else cv.priv[d]++;
         }
       }
     if (out) *out = cv;
+    if (ext) std::copy(words.begin(), words.end(), ext);
     char b[96];
     std::snprintf(b, sizeof b, "|V=%llx:%u:%u:%u:%u", (unsigned long long)cv.shared, cv.priv[0], cv.priv[1], cv.priv[2], cv.priv[3]);
-    return (cv.shared | cv.priv[0] | cv.priv[1] | cv.priv[2] | cv.priv[3]) ? std::string(b) : std::string();
+    std::string key(b);
+    bool any = (cv.shared | cv.priv[0] | cv.priv[1] | cv.priv[2] | cv.priv[3]) != 0;
+    for (uint64_t w : words) {
+      std::snprintf(b, sizeof b, ":%llx", (unsigned long long)w);
+      key += b;
+      any = any || w != 0;
+    }
+    return any ? key : std::string();
   }
 
   // ------------------------------------------------------------ pod classes and relaxation chains
@@ -877,22 +889,38 @@ void participants(Builder& B, const std::vector<int>& candidates) {
 
 // ------------------------------------------------------------------ CSI volume limits (ksched.h: ksched_class_volumes)
 // Drivers some owned state node limits; claims by how many pods (batch + bound) mount them: one -> counted, several -> tracked id.
+// When that would track more than 64 claims, a claim is tracked only when two different pods mount it and one of them is a pod
+// of the batch (DESIGN.md §3, volume claims beyond the word). A claim only bound pods mount stays in their nodes' used[], which
+// count it once per node already; a claim exactly one pod mounts is private to it. Problems that fit keep their encoding.
 void csi_volumes(Builder& B) {
   std::set<std::string> drivers;
   for (int si : B.state_nodes) for (auto& kv : B.P.nodes[si].volume_limits) drivers.insert(kv.first);
   B.vol_drivers.assign(drivers.begin(), drivers.end());
   if (B.vol_drivers.size() > KSCHED_MAX_VOLUME_DRIVERS) unsupported("more than 4 CSI drivers with node volume limits");
   if (B.vol_drivers.empty()) return;
-  std::map<std::pair<std::string, std::string>, int> refs;
-  auto count = [&](const Pod& p) { for (auto& kv : B.pod_claims(p)) for (auto& c : kv.second) refs[{kv.first, c}]++; };
-  for (auto* p : B.E.pods) count(*p);
-  for (int si : B.state_nodes) for (auto& p : B.P.nodes[si].pods) count(p);
-  for (auto& kv : refs)
-    if (kv.second > 1) {
-      if (B.vol_tracked.size() >= 64) unsupported("more than 64 volume claims shared between pods");
-      const int bit = (int)B.vol_tracked.size();
-      B.vol_tracked[kv.first] = bit;
+  struct Mounts { int refs = 0; const Pod* first = nullptr; bool two_pods = false, batch = false; };
+  std::map<std::pair<std::string, std::string>, Mounts> claims;
+  // (a candidate's pod is reached through E.pods and through its node's pod list: one Pod object, one pod)
+  auto count = [&](const Pod& p, bool batch) {
+    for (auto& kv : B.pod_claims(p))
+      for (auto& c : kv.second) {
+        Mounts& m = claims[{kv.first, c}];
+        m.refs++;
+        if (!m.first) m.first = &p; else m.two_pods = m.two_pods || m.first != &p;
+        m.batch = m.batch || batch;
+      }
+  };
+  for (auto* p : B.E.pods) count(*p, true);
+  for (int si : B.state_nodes) for (auto& p : B.P.nodes[si].pods) count(p, false);
+  size_t shared = 0;
+  for (auto& kv : claims) shared += kv.second.refs > 1;
+  for (auto& kv : claims)
+    if (shared <= 64 ? kv.second.refs > 1 : kv.second.two_pods && kv.second.batch) {
+      B.vol_tracked[kv.first] = (int)B.E.volume_claims.size();
+      B.E.volume_claims.push_back(kv.first);
     }
+  const size_t n = B.E.volume_claims.size();
+  B.E.volume_ext_words = n > 64 ? (int)((n - 64 + 63) / 64) : 0;
 }
 
 // ------------------------------------------------------------------ pod specs: classes and relaxation chains
@@ -1507,9 +1535,9 @@ void existing_nodes(Builder& B) {
     if (itl != n.labels.end()) { auto c = B.type_col.find(itl->second); if (c != B.type_col.end()) e.itype = (uint32_t)c->second; }
     if (const int W = E.hostport_ext_words) {
       E.existing_hostport_ext.resize(E.existing_hostport_ext.size() + W, 0);
-      for (auto& hp : nf.hostports) B.hp_bit(B.hp_entry(hp), e.hostport_entries, &E.existing_hostport_ext[E.existing_hostport_ext.size() - W]);
+      for (auto& hp : nf.hostports) B.id_bit(B.hp_entry(hp), e.hostport_entries, &E.existing_hostport_ext[E.existing_hostport_ext.size() - W]);
     } else {
-      for (auto& hp : nf.hostports) B.hp_bit(B.hp_entry(hp), e.hostport_entries, nullptr);
+      for (auto& hp : nf.hostports) B.id_bit(B.hp_entry(hp), e.hostport_entries, nullptr);
     }
     std::string hostname;
     auto h = n.labels.find(kHostname);
@@ -1522,6 +1550,9 @@ void existing_nodes(Builder& B) {
     E.existing_initialized.push_back(ini != n.labels.end() && ini->second == "true");
     if (!B.vol_drivers.empty()) {  // state.Node.VolumeUsage() / VolumeLimits() (state/cluster.go:292-303,340-347)
       ksched_node_volumes nv{};
+      const int VW = E.volume_ext_words;
+      E.existing_volumes_mounted_ext.resize(E.existing_volumes_mounted_ext.size() + VW, 0);
+      uint64_t* ext = VW ? &E.existing_volumes_mounted_ext[E.existing_volumes_mounted_ext.size() - VW] : nullptr;
       std::map<std::string, std::set<std::string>> mounted;
       for (auto& p : n.pods) for (auto& kv : B.pod_claims(p)) mounted[kv.first].insert(kv.second.begin(), kv.second.end());
       bool over = false;
@@ -1534,7 +1565,7 @@ void existing_nodes(Builder& B) {
         for (auto& c : mounted[B.vol_drivers[d]]) {
           ++total;
           auto t = B.vol_tracked.find({B.vol_drivers[d], c});
-          if (t != B.vol_tracked.end()) nv.mounted |= 1ull << t->second; else nv.used[d]++;
+          if (t != B.vol_tracked.end()) B.id_bit(t->second, nv.mounted, ext); else nv.used[d]++;
         }
         if (nv.limit[d] >= 0 && total > nv.limit[d]) over = true;
       }
@@ -1952,9 +1983,9 @@ void class_rows(Builder& B, const std::vector<Group>& groups) {
       }
     }
     for (auto& hp : host_ports(s.pod)) {  // the entry table is complete: host_port_table ran before the existing nodes
-      B.hp_bit(B.hp_entry(hp), row.hostport_entries, HW ? &E.class_hostport_entries_ext[(size_t)c * HW] : nullptr);
+      B.id_bit(B.hp_entry(hp), row.hostport_entries, HW ? &E.class_hostport_entries_ext[(size_t)c * HW] : nullptr);
       for (size_t e = 0; e < B.hp_entries.size(); ++e)
-        if (hp_matches(hp, B.hp_entries[e])) B.hp_bit((int)e, row.hostport_conflicts, HW ? &E.class_hostport_conflicts_ext[(size_t)c * HW] : nullptr);
+        if (hp_matches(hp, B.hp_entries[e])) B.id_bit((int)e, row.hostport_conflicts, HW ? &E.class_hostport_conflicts_ext[(size_t)c * HW] : nullptr);
     }
     for (size_t t = 0; t < NS; ++t) {  // the taint-set table is complete: templates and existing nodes are encoded
       if (!tolerates_all(B.taintsets[t], s.pod.tolerations)) continue;
@@ -1975,11 +2006,17 @@ void class_rows(Builder& B, const std::vector<Group>& groups) {
   }
   hostname_slot_table(B);
   if (!B.vol_drivers.empty()) {
+    const int VW = E.volume_ext_words;
     E.class_volumes.resize(NC);
+    E.class_volumes_shared_ext.assign((size_t)NC * VW, 0);
+    E.volume_driver_mask_ext.assign((size_t)KSCHED_MAX_VOLUME_DRIVERS * VW, 0);
     bool any = false;
-    for (int c = 0; c < NC; ++c) any = !B.volume_signature(B.specs[c].pod, &E.class_volumes[c]).empty() || any;
+    for (int c = 0; c < NC; ++c)
+      any = !B.volume_signature(B.specs[c].pod, &E.class_volumes[c], VW ? &E.class_volumes_shared_ext[(size_t)c * VW] : nullptr).empty() || any;
     if (!any) E.class_volumes.clear();  // no pod of the batch mounts a limited claim: the kernels never look
-    for (auto& kv : B.vol_tracked) E.volume_driver_mask[B.driver_index(kv.first.first)] |= 1ull << kv.second;
+    for (auto& kv : B.vol_tracked)
+      B.id_bit(kv.second, E.volume_driver_mask[B.driver_index(kv.first.first)],
+               VW ? &E.volume_driver_mask_ext[B.driver_index(kv.first.first) * VW] : nullptr);
   }
 }
 
@@ -2079,6 +2116,12 @@ void wire(Builder& B) {
     pr.class_volumes = E.class_volumes.data();
     pr.existing_volumes = E.existing_volumes.data();
     for (int d = 0; d < KSCHED_MAX_VOLUME_DRIVERS; ++d) pr.volume_driver_mask[d] = E.volume_driver_mask[d];
+    if (E.volume_ext_words) {
+      pr.class_volumes_shared_ext = E.class_volumes_shared_ext.data();
+      pr.existing_volumes_mounted_ext = E.existing_volumes_mounted_ext.data();
+      pr.volume_driver_mask_ext = E.volume_driver_mask_ext.data();
+      pr.n_volume_ext_words = E.volume_ext_words;
+    }
   }
   pr.class_tolerated_ext = E.class_tolerated_ext.empty() ? nullptr : E.class_tolerated_ext.data();
   pr.n_tolerated_ext_words = E.tolerated_ext_words;

@@ -96,6 +96,11 @@ struct Encoded {
   std::vector<ksched_class_volumes> class_volumes;    // CSI volume limits (ksched.h); empty when no pod mounts a limited claim
   std::vector<ksched_node_volumes> existing_volumes;
   uint64_t volume_driver_mask[KSCHED_MAX_VOLUME_DRIVERS] = {};
+  std::vector<std::pair<std::string, std::string>> volume_claims;  // tracked (driver, claim) in id order (DESIGN.md §3)
+  int volume_ext_words = 0;                           // tracked claims from id 64 on (ksched.h); 0 with at most 64 tracked
+  std::vector<uint64_t> class_volumes_shared_ext;     // [n_classes][volume_ext_words]; empty without such claims
+  std::vector<uint64_t> existing_volumes_mounted_ext; // [n_existing][volume_ext_words]
+  std::vector<uint64_t> volume_driver_mask_ext;       // [KSCHED_MAX_VOLUME_DRIVERS][volume_ext_words]
   int n_taintsets = 0;                                // distinct taint sets of templates and existing nodes
   std::vector<uint64_t> class_tolerated_ext;          // [n_classes][tolerated_ext_words] sets from id 64 on (ksched.h); empty with <= 64 sets
   int tolerated_ext_words = 0;

@@ -360,7 +360,8 @@ void kh_encoded_free(Encoded* E) {
   delete E;
 }
 // dims: [pods, classes, existing, groups, types, templates, keys, resources, type_words, class_topo, taintsets, resources_ext,
-//        hostports, hostport_ext_words, hostname_reqs, hostname_words, itype_reqs, itype_filter_terms]
+//        hostports, hostport_ext_words, hostname_reqs, hostname_words, itype_reqs, itype_filter_terms, volume_claims,
+//        volume_ext_words]
 // (itype_filter_terms: filter terms with an instance-type part; 0 exactly when the problem has no instance-type filter tables)
 void kh_encoded_dims(const Encoded* E, long long* out) {
   out[14] = (long long)E->hostname_reqs.size() / 2; out[15] = E->hostname_words;
@@ -371,12 +372,22 @@ void kh_encoded_dims(const Encoded* E, long long* out) {
   out[6] = (long long)E->key_names.size(); out[7] = (long long)E->res_names.size() - E->n_res_ext; out[8] = E->type_words;
   out[9] = (long long)E->class_topo.size(); out[10] = E->n_taintsets; out[11] = E->n_res_ext;
   out[12] = (long long)E->hostports.size(); out[13] = E->hostport_ext_words;
+  out[18] = (long long)E->volume_claims.size(); out[19] = E->volume_ext_words;
 }
 // Host-port entry `id` of an encoding as "ip port protocol" into out[cap] (tests): the entries the encoder kept, in id order.
 // Returns -1 when there is no such entry or it does not fit.
 int kh_encoded_hostport(const Encoded* E, int id, char* out, int cap) {
   if (id < 0 || (size_t)id >= E->hostports.size() || (int)E->hostports[(size_t)id].size() >= cap) return -1;
   std::memcpy(out, E->hostports[(size_t)id].c_str(), E->hostports[(size_t)id].size() + 1);
+  return 0;
+}
+// Tracked volume claim `id` of an encoding as "driver claim" into out[cap] (tests): the claims the encoder tracks, in id
+// order. Returns -1 when there is no such claim or it does not fit.
+int kh_encoded_volume_claim(const Encoded* E, int id, char* out, int cap) {
+  if (id < 0 || (size_t)id >= E->volume_claims.size()) return -1;
+  const std::string s = E->volume_claims[(size_t)id].first + " " + E->volume_claims[(size_t)id].second;
+  if ((int)s.size() >= cap) return -1;
+  std::memcpy(out, s.c_str(), s.size() + 1);
   return 0;
 }
 // Hostname requirement `i` of an encoding (ksched.h: hostname_reqs) into out[cap] (tests): out[0] = 1 when it admits new
@@ -1356,6 +1367,9 @@ extern "C" unsigned long long kh_encoded_digest(const Encoded* E) {
   vec(E->pod_class); vec(E->pod_timestamp); vec(E->pod_uid_rank); vec(E->existing); vec(E->groups); vec(E->group_domain_counts);
   vec(E->group_existing_counts); vec(E->class_topo); vec(E->filter_terms); vec(E->itype_req_sets); vec(E->itype_req_complement); vec(E->hostname_reqs);
   if (!E->class_volumes.empty()) { vec(E->class_volumes); vec(E->existing_volumes); bytes(E->volume_driver_mask, sizeof E->volume_driver_mask); }
+  if (E->volume_ext_words) {  // absent with at most 64 tracked claims: those digests predate the claim tables
+    vec(E->class_volumes_shared_ext); vec(E->existing_volumes_mounted_ext); vec(E->volume_driver_mask_ext);
+  }
   if (!E->class_tolerated_ext.empty()) vec(E->class_tolerated_ext);  // absent with at most 64 taint sets: those digests predate it
   if (E->hostport_ext_words) {  // absent with at most 64 host-port entries: those digests predate the entry tables
     vec(E->class_hostport_conflicts_ext); vec(E->class_hostport_entries_ext); vec(E->existing_hostport_ext);

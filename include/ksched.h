@@ -132,7 +132,7 @@ typedef struct ksched_type_row {
   int64_t allocatable[KSCHED_MAX_RES]; /* Capacity - Overhead.Total(), types.go:87-89; 0 where absent */
   uint64_t values[KSCHED_MAX_KEYS];
   uint64_t meta;
-  uint64_t offerings;        /* bit (ct*16 + zone): an AVAILABLE offering exists (node.go:151-159) */
+  uint64_t offerings;        /* bit s: an AVAILABLE offering exists in offering slot s (node.go:151-159; ksched_catalog.zone_slots) */
   uint64_t template_members; /* bit v: type is in template v's GetInstanceTypes list (and meets its template-only keys) */
   double min_price;          /* cheapest available offering */
   uint32_t res_present;      /* resources present in Capacity */
@@ -171,9 +171,10 @@ typedef struct ksched_catalog {
   const ksched_template* templates; /* [n_templates], weight order (v1alpha5/provisioner.go:132) */
   const ksched_bounds* template_bounds; /* must be NULL (region form) */
   /* Launch choice (the step after the path: fake/cloudprovider.go:74-84 orders the surviving options by their cheapest
-     compatible offering, cloudprovider/types.go:128-145 picks that offering). [n_types][64], slot = ct*16 + zone:
-     (rank of the offering's price among all distinct prices of the catalog) << 16 | position in the type's Offerings
-     list << 8 | slot, for AVAILABLE offerings; ~0 elsewhere. NULL: ksched_result.launch is not filled. */
+     compatible offering, cloudprovider/types.go:128-145 picks that offering). [n_types][64], one entry per offering slot s
+     (see zone_slots): (rank of the offering's price among all distinct prices of the catalog) << 16 | position in the type's
+     Offerings list << 8 | s, for AVAILABLE offerings (the smallest such key when several offerings share a slot); ~0
+     elsewhere. NULL: ksched_result.launch is not filled. */
   const uint64_t* offering_keys;
   /* Ext resources: resources from the 9th on (at most KSCHED_MAX_RES_EXT). n_res keeps its meaning (the <= 8 row slots), so
      no reader of the rows indexes past them. Only pod classes request ext resources: no daemonset, provisioner limit or
@@ -181,6 +182,15 @@ typedef struct ksched_catalog {
   int32_t n_res_ext;
   int32_t pad_ext;
   const int64_t* type_alloc_ext;   /* [n_types][n_res_ext] allocatable of ext resource x (0 where the type lacks it) */
+  /* Offering slots: bit s of ksched_type_row.offerings and entry s of offering_keys stand for one (capacity type, zone) pair
+     of dictionary ids (without a zone or capacity-type mask key every offering counts as value 0 of that key). Both NULL: slot
+     = ct*16 + zone, which holds zone ids below 16 and capacity-type ids below 4. Otherwise zone_slots[z] is the set of slots
+     whose zone is value z and ct_slots[c] the set whose capacity type is value c, so the slot of pair (c, z) is
+     zone_slots[z] & ct_slots[c]. Every slot belongs to exactly one zone and one capacity type, and every offerings bit of
+     every type is a slot of the tables; ksched_load_catalog answers KSCHED_ERR_INVALID otherwise. The host encoder numbers
+     the distinct pairs of available offerings in ascending (capacity-type id, zone id) order (DESIGN.md §3). */
+  const uint64_t* zone_slots; /* [64] or NULL */
+  const uint64_t* ct_slots;   /* [64] or NULL */
 } ksched_catalog;
 
 /* Existing (real / in-flight) node: NewExistingNode, existingnode.go:41-75. */
@@ -341,7 +351,7 @@ typedef struct ksched_new_node {
    cheapest (ties: provider input order), and that offering (ties: Offerings list order). */
 typedef struct ksched_launch_choice {
   int32_t type_column;    /* column (price order) of the chosen instance type, -1 if the node has no option */
-  int32_t offering_slot;  /* ct*16 + zone */
+  int32_t offering_slot;  /* the offering's slot (ksched_catalog.zone_slots) */
   uint32_t price_rank;    /* rank of the offering's price (see ksched_catalog.offering_keys) */
   uint32_t offering_index; /* position of that offering in the instance type's Offerings list */
 } ksched_launch_choice;

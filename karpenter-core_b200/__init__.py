@@ -128,6 +128,9 @@ def lib():
     L.kh_encoded_resource_id.argtypes = [C.c_void_p, C.c_char_p]
     L.kh_encoded_hostport.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_int]
     L.kh_encoded_volume_claim.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_int]
+    L.kh_encoded_offering_slot.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_int]
+    L.kh_encoded_offering_slots.argtypes = [C.c_void_p]
+    L.kh_encoded_offering_slots.restype = C.c_longlong
     L.kh_encoded_hostname_req.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_longlong), C.c_int]
     L.kh_encoded_class_hostname.argtypes = [C.c_void_p, C.c_int]
     L.kh_encoded_class_hostname.restype = C.c_longlong
@@ -587,6 +590,7 @@ class ResidentSolve:
         self.dims = dict(zip(["pods", "classes", "existing", "groups", "types", "templates", "keys", "resources", "type_words", "class_topo",
                               "taintsets", "resources_ext", "hostports", "hostport_ext_words", "hostname_reqs", "hostname_words",
                               "itype_reqs", "itype_filter_terms", "volume_claims", "volume_ext_words"], list(d)))
+        self.dims["offering_slots"] = lib().kh_encoded_offering_slots(self.enc)
 
     def hostname_reqs(self):
         """every hostname requirement of this encoding in entry order, as (admits new nodes, [admitted existing slots])"""
@@ -624,6 +628,14 @@ class ResidentSolve:
         while lib().kh_encoded_volume_claim(self.enc, len(out), buf, len(buf)) == 0:
             driver, claim = buf.value.decode().split(" ", 1)
             out.append((driver, claim))
+        return out
+
+    def offering_slots(self):
+        """the dense offering slots of this encoding in slot order, as (capacity type, zone); [] for the ct*16 + zone layout"""
+        out, buf = [], C.create_string_buffer(1024)
+        while lib().kh_encoded_offering_slot(self.enc, len(out), buf, len(buf)) == 0:
+            ct, zone = buf.value.decode().split(" ", 1)
+            out.append((ct, zone))
         return out
 
     def key_info(self, key):

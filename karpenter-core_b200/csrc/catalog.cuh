@@ -21,8 +21,12 @@ struct DevCatalog {
   const uint32_t* negempty;          // [n_keys][W32] type requirement on key is DoesNotExist
   uint32_t type_relevant;            // bit k: some type defines key k
   const int16_t* offrow;             // [64] row in offset table or -1
-  const uint32_t* offset;            // [rows][W32] type has an available offering (ct*16+zone)
+  const uint32_t* offset;            // [rows][W32] type has an available offering in the row's slot
   const uint32_t* anyoffer;          // [W32]
+  const uint64_t* slots;             // [128] zone value -> its offering slots, then capacity-type value -> its slots (ksched.h)
+  uint64_t zone_used, ct_used;       // zone / capacity-type values that own a slot
+  uint64_t all_slots;                // every slot of the tables
+  uint64_t offer_used;               // slots with an offset row
   const uint32_t* member;            // [n_templates][W32]
   const int64_t* alloc_sorted;       // [n_res][n_types] ascending
   const uint32_t* fitset;            // [n_res][n_types+1][W32]  rank -> types with alloc >= alloc_sorted[rank]
@@ -88,22 +92,16 @@ __device__ __forceinline__ uint32_t key_typeset_word(const DevCatalog& c, int k,
   }
   return s;
 }
-// hasOffering (node.go:151-159) for one word: zmask / cmask = admitted zone / capacity-type value bits
-__device__ __forceinline__ uint32_t offer_word(const DevCatalog& c, uint32_t zmask, uint32_t cmask, bool unconstrained, int w) {
+// hasOffering (node.go:151-159) for one word: slots = the offering slots the node's zone / capacity-type requirements admit
+// (ksched::admitted_slots)
+__device__ __forceinline__ uint32_t offer_word(const DevCatalog& c, uint64_t slots, bool unconstrained, int w) {
   if (unconstrained) return c.anyoffer[w];
   uint32_t s = 0;
-  uint32_t cm = cmask & 0xF;
-  while (cm) {
-    int ct = __ffs(cm) - 1;
-    cm &= cm - 1;
-    uint32_t zm = zmask & 0xFFFF;
-    while (zm) {
-      int z = __ffs(zm) - 1;
-      zm &= zm - 1;
-      int row = c.offrow[ct * 16 + z];
-      if (row >= 0) s |= c.offset[(size_t)row * c.W32 + w];
-    }
-  }
+  for (uint64_t m = slots & c.offer_used; m; m &= m - 1) s |= c.offset[(size_t)c.offrow[__ffsll((long long)m) - 1] * c.W32 + w];
   return s;
+}
+// admitted offering slots of a node from its zone / capacity-type allowed value bits
+__device__ __forceinline__ uint64_t node_slots(const DevCatalog& c, uint64_t zallowed, uint64_t callowed) {
+  return ksched::admitted_slots(c.slots, c.zone_used, c.ct_used, c.all_slots, zallowed, callowed);
 }
 

@@ -116,7 +116,7 @@ __device__ __noinline__ unsigned long long k1_compute_row(int j, uint64_t word, 
         if (res_used) rank = fit_rank(c.alloc_sorted, T, lane, (int64_t)word + tm.daemon_requests[lane]);
       }
       const uint32_t res_mask = __ballot_sync(0xffffffffu, res_used);
-      uint64_t zallowed = 0xFFFF, callowed = 0xF;
+      uint64_t zallowed = ~0ull, callowed = ~0ull;
       bool zc_unconstrained = true;
       if (c.zone_key >= 0) {
         bool zp = __shfl_sync(0xffffffffu, (int)present, 8 + c.zone_key);
@@ -128,6 +128,7 @@ __device__ __noinline__ unsigned long long k1_compute_row(int j, uint64_t word, 
         uint64_t ca = __shfl_sync(0xffffffffu, allowed, 8 + c.ct_key);
         if (cp) { callowed = ca; zc_unconstrained = false; }
       }
+      const uint64_t slots = zc_unconstrained ? ~0ull : node_slots(c, zallowed, callowed);
       bool any = false;
       int first_word = -1;
       uint32_t first_bits = 0;
@@ -144,7 +145,7 @@ __device__ __noinline__ unsigned long long k1_compute_row(int j, uint64_t word, 
           bool ng = __shfl_sync(0xffffffffu, (int)neg, 8 + kk);
           if (s) s &= key_typeset_word(c, kk, a, ng, w);
         }
-        if (s) s &= offer_word(c, (uint32_t)zallowed, (uint32_t)callowed, zc_unconstrained, w);
+        if (s) s &= offer_word(c, slots, zc_unconstrained, w);
         uint32_t rm = res_mask, fit = 0xFFFFFFFFu;
         while (rm) {  // the loads do not depend on each other (nor on s): one memory round trip for all resources
           int r = __ffs(rm) - 1;
@@ -205,7 +206,8 @@ __global__ void __launch_bounds__(kK1Threads, 1) class_feasibility_kernel() {
     ksched_keyinfo* s_keys = reinterpret_cast<ksched_keyinfo*>(ptr); ptr += sizeof(ksched_keyinfo) * KSCHED_MAX_KEYS;
     int64_t* s_alloc = reinterpret_cast<int64_t*>(ptr); ptr += p.alloc_in_smem ? sizeof(int64_t) * R * T : 0;
     int16_t* s_valrow = reinterpret_cast<int16_t*>(ptr); ptr += sizeof(int16_t) * KSCHED_MAX_KEYS * 64;
-    int16_t* s_offrow = reinterpret_cast<int16_t*>(ptr);
+    int16_t* s_offrow = reinterpret_cast<int16_t*>(ptr); ptr += sizeof(int16_t) * 64;
+    uint64_t* s_slots = reinterpret_cast<uint64_t*>(ptr);
     // cp.async (LDGSTS): every 4-byte element of every table is requested before anything is waited on, so the whole
     // staging costs about one memory round trip instead of one per table.
     auto stage4 = [&](void* dst, const void* src, int n_words) {
@@ -229,9 +231,10 @@ __global__ void __launch_bounds__(kK1Threads, 1) class_feasibility_kernel() {
     if (p.alloc_in_smem) stage4(s_alloc, c.alloc_sorted, R * T * 2);
     stage4(s_valrow, c.valrow, NK * 64 / 2);
     stage4(s_offrow, c.offrow, 32);
+    stage4(s_slots, c.slots, 128 * 2);
     if (p.tables_in_smem) {
       // the narrow column bitsets: one 4*W32-byte row per (key,value) / key / offering / template
-      uint32_t* sp = reinterpret_cast<uint32_t*>(reinterpret_cast<unsigned char*>(s_offrow) + sizeof(int16_t) * 64);
+      uint32_t* sp = reinterpret_cast<uint32_t*>(s_slots + 128);
       auto stage = [&](const uint32_t*& tbl, int rows) {
         stage4(sp, tbl, rows * W32);
         tbl = sp;
@@ -250,6 +253,7 @@ __global__ void __launch_bounds__(kK1Threads, 1) class_feasibility_kernel() {
     if (p.alloc_in_smem) c.alloc_sorted = s_alloc;
     c.valrow = s_valrow;
     c.offrow = s_offrow;
+    c.slots = s_slots;
     if (threadIdx.x == 0) g_k1cat = c;
   }
   __syncthreads();

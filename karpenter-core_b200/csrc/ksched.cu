@@ -102,17 +102,18 @@ __global__ void launch_choice_kernel(DevCatalog c, const long long* counters, co
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
   for (int n = warp; n < n_new; n += nwarps) {
-    // zones / capacity types the node's requirements admit (Offerings.Requirements, types.go:120-126)
-    uint32_t zmask = 0xFFFF, cmask = 0xF;
+    // offering slots the node's requirements admit (Offerings.Requirements, types.go:120-126)
+    uint64_t zallowed = ~0ull, callowed = ~0ull;
     const uint64_t meta = nn_meta[n];
     if (c.zone_key >= 0) {
       const Req z = load_soa(nn_vals, meta, max_new, n, c.zone_key);
-      if (z.present) zmask = (uint32_t)ksched::req_allowed(z, c.keys[c.zone_key].dict_mask, key_meta(c, c.zone_key));
+      if (z.present) zallowed = ksched::req_allowed(z, c.keys[c.zone_key].dict_mask, key_meta(c, c.zone_key));
     }
     if (c.ct_key >= 0) {
       const Req ct = load_soa(nn_vals, meta, max_new, n, c.ct_key);
-      if (ct.present) cmask = (uint32_t)ksched::req_allowed(ct, c.keys[c.ct_key].dict_mask, key_meta(c, c.ct_key));
+      if (ct.present) callowed = ksched::req_allowed(ct, c.keys[c.ct_key].dict_mask, key_meta(c, c.ct_key));
     }
+    const uint64_t slots = node_slots(c, zallowed, callowed) & c.offer_used;
     unsigned long long best = ~0ull, best_off = ksched::kNoOffering;
     int best_col = -1;
     for (int w = lane; w < c.W32; w += 32) {
@@ -120,7 +121,7 @@ __global__ void launch_choice_kernel(DevCatalog c, const long long* counters, co
       while (m) {
         const int t = w * 32 + __ffs(m) - 1;
         m &= m - 1;
-        const uint64_t ok = ksched::offering_min_key(c.offer_keys + (size_t)t * 64, zmask, cmask);
+        const uint64_t ok = ksched::offering_min_key(c.offer_keys + (size_t)t * 64, slots);
         if (ok == ksched::kNoOffering) continue;
         const unsigned long long key = ksched::option_key(ok, c.input_index[t]);
         if (key < best) { best = key; best_off = ok; best_col = t; }
@@ -204,7 +205,7 @@ struct ksched_handle {
   DevBuf<int16_t> d_valrow, d_offrow;
   DevBuf<int32_t> d_perm_desc;
   DevBuf<uint32_t> d_valset, d_absent, d_negempty, d_offset, d_anyoffer, d_member, d_fitset, d_domset, d_input_index;
-  DevBuf<uint64_t> d_offer_keys;
+  DevBuf<uint64_t> d_offer_keys, d_slots;
   // ---- problem (ksched_upload): `st` points into the buffers of this group; reset_state restores the `resets` segments
   bool uploaded = false;
   bool sorted = false;  // the FFD-ordered pod-row matrix of the uploaded problem exists
@@ -446,6 +447,23 @@ static int check_catalog(ksched_handle* h, const ksched_catalog* cat) {
       }
     }
   }
+  // offering slot tables (read only here, after every check of the fields that precede them)
+  if (!cat->zone_slots != !cat->ct_slots) { h->err = "zone_slots and ct_slots must both be set or both be NULL"; return KSCHED_ERR_INVALID; }
+  if (cat->zone_slots) {
+    uint64_t zones = 0, cts = 0;
+    bool overlap = false;
+    for (int v = 0; v < 64; ++v) {
+      overlap = overlap || (zones & cat->zone_slots[v]) || (cts & cat->ct_slots[v]);
+      zones |= cat->zone_slots[v];
+      cts |= cat->ct_slots[v];
+    }
+    uint64_t offered = 0;
+    for (int t = 0; t < cat->n_types; ++t) offered |= cat->types[t].offerings;
+    if (overlap || zones != cts || (offered & ~zones)) {
+      h->err = "inconsistent offering slot tables: every slot belongs to exactly one zone and one capacity type, and every offering is a slot";
+      return KSCHED_ERR_INVALID;
+    }
+  }
   return KSCHED_OK;
 }
 
@@ -466,6 +484,9 @@ static std::vector<unsigned char> catalog_key(const ksched_catalog* cat) {
   if (has_off) put(cat->offering_keys, sizeof(uint64_t) * (size_t)T * 64);
   put(&cat->n_res_ext, sizeof cat->n_res_ext);
   if (cat->n_res_ext) put(cat->type_alloc_ext, sizeof(int64_t) * (size_t)T * cat->n_res_ext);
+  const unsigned char has_slots = cat->zone_slots != nullptr;
+  put(&has_slots, 1);
+  if (has_slots) { put(cat->zone_slots, sizeof(uint64_t) * 64); put(cat->ct_slots, sizeof(uint64_t) * 64); }
   return blob;
 }
 
@@ -480,6 +501,8 @@ struct CatalogTables {
   uint32_t type_relevant = 0;
   int zone_key = -1, ct_key = -1;
   uint64_t pin_neutral[KSCHED_MAX_KEYS] = {};
+  std::vector<uint64_t> slots;  // [128] zone value -> its slots, capacity-type value -> its slots (the tables or the formula)
+  uint64_t zone_used = 0, ct_used = 0, all_slots = 0, offer_used = 0;
 };
 
 static void build_catalog(const ksched_catalog* cat, CatalogTables& b) {
@@ -491,6 +514,18 @@ static void build_catalog(const ksched_catalog* cat, CatalogTables& b) {
   if (cat->key_regions) for (int k = 0; k < NK; ++k) b.keys[k].dict_mask |= cat->key_regions[k].region_mask;
   b.valrow.assign((size_t)NK * 64, -1);
   b.offrow.assign(64, -1);
+  b.slots.assign(128, 0);
+  if (cat->zone_slots) {
+    std::copy(cat->zone_slots, cat->zone_slots + 64, b.slots.begin());
+    std::copy(cat->ct_slots, cat->ct_slots + 64, b.slots.begin() + 64);
+  } else {
+    ksched::formula_slot_tables(b.slots.data(), b.slots.data() + 64);
+  }
+  for (int v = 0; v < 64; ++v) {
+    if (b.slots[v]) b.zone_used |= 1ull << v;
+    if (b.slots[64 + v]) b.ct_used |= 1ull << v;
+    b.all_slots |= b.slots[v];
+  }
   b.absent.assign((size_t)std::max(NK, 1) * W32, 0);
   b.negempty.assign((size_t)std::max(NK, 1) * W32, 0);
   b.anyoffer.assign(W32, 0);
@@ -532,7 +567,7 @@ static void build_catalog(const ksched_catalog* cat, CatalogTables& b) {
       int ob = __builtin_ctzll(o);
       o &= o - 1;
       int16_t& r = b.offrow[ob];
-      if (r < 0) { r = (int16_t)(b.offset.size() / W32); b.offset.resize(b.offset.size() + W32, 0); }
+      if (r < 0) { r = (int16_t)(b.offset.size() / W32); b.offset.resize(b.offset.size() + W32, 0); b.offer_used |= 1ull << ob; }
       b.offset[(size_t)r * W32 + w] |= bit;
     }
     for (int v = 0; v < V; ++v) if ((row.template_members >> v) & 1) b.member[(size_t)v * W32 + w] |= bit;
@@ -580,9 +615,25 @@ static void build_catalog(const ksched_catalog* cat, CatalogTables& b) {
     std::vector<uint32_t> U(W32, 0);
     for (int v = 0; v < V; ++v) for (int w = 0; w < W32; ++w) U[w] |= b.member[(size_t)v * W32 + w];
     auto covers = [&](const std::vector<uint32_t>& set) { for (int w = 0; w < W32; ++w) if (U[w] & ~set[w]) return false; return true; };
-    auto offer_rows = [&](int ct, int z, std::vector<uint32_t>& acc) {
-      const int16_t r = b.offrow[ct * 16 + z];
-      if (r >= 0) for (int w = 0; w < W32; ++w) acc[w] |= b.offset[(size_t)r * W32 + w];
+    // types with an available offering in one of `slots`
+    auto offers = [&](uint64_t slots) {
+      std::vector<uint32_t> acc(W32, 0);
+      for (uint64_t m = slots & b.offer_used; m; m &= m - 1) {
+        const int16_t r = b.offrow[__builtin_ctzll(m)];
+        for (int w = 0; w < W32; ++w) acc[w] |= b.offset[(size_t)r * W32 + w];
+      }
+      return acc;
+    };
+    // pinning value d of one of the two offering keys (own = its value -> slots table) is neutral when d owns a slot and,
+    // for every value of the other key (other, other_key), the types offered in the pair's slots cover U
+    auto offering_neutral = [&](const uint64_t* own, const uint64_t* other, int other_key, int d) {
+      if (!own[d]) return false;
+      if (other_key < 0) return covers(offers(own[d]));
+      for (uint64_t m = cat->keys[other_key].dict_mask; m; m &= m - 1) {
+        const int v = __builtin_ctzll(m);
+        if (!other[v] || !covers(offers(own[d] & other[v]))) return false;
+      }
+      return true;
     };
     for (int k = 0; k < NK; ++k) {
       for (int d = 0; d < 64; ++d) {
@@ -591,38 +642,8 @@ static void build_catalog(const ksched_catalog* cat, CatalogTables& b) {
         for (int w = 0; w < W32; ++w) set[w] = b.absent[(size_t)k * W32 + w];
         if (b.valrow[(size_t)k * 64 + d] >= 0) for (int w = 0; w < W32; ++w) set[w] |= b.valset[(size_t)b.valrow[(size_t)k * 64 + d] * W32 + w];
         bool ok = covers(set);
-        if (ok && k == zone_key) {
-          if (d >= 16) ok = false;
-          else if (ct_key >= 0) {
-            for (int ct = 0; ct < 4 && ok; ++ct) {
-              if (!((cat->keys[ct_key].dict_mask >> ct) & 1)) continue;
-              std::vector<uint32_t> acc(W32, 0);
-              offer_rows(ct, d, acc);
-              ok = covers(acc);
-            }
-            if (cat->keys[ct_key].dict_mask >> 4) ok = false;
-          } else {
-            std::vector<uint32_t> acc(W32, 0);
-            for (int ct = 0; ct < 4; ++ct) offer_rows(ct, d, acc);
-            ok = covers(acc);
-          }
-        }
-        if (ok && k == ct_key) {
-          if (d >= 4) ok = false;
-          else if (zone_key >= 0) {
-            for (int z = 0; z < 16 && ok; ++z) {
-              if (!((cat->keys[zone_key].dict_mask >> z) & 1)) continue;
-              std::vector<uint32_t> acc(W32, 0);
-              offer_rows(d, z, acc);
-              ok = covers(acc);
-            }
-            if (cat->keys[zone_key].dict_mask >> 16) ok = false;
-          } else {
-            std::vector<uint32_t> acc(W32, 0);
-            for (int z = 0; z < 16; ++z) offer_rows(d, z, acc);
-            ok = covers(acc);
-          }
-        }
+        if (ok && k == zone_key) ok = offering_neutral(b.slots.data(), b.slots.data() + 64, ct_key, d);
+        if (ok && k == ct_key) ok = offering_neutral(b.slots.data() + 64, b.slots.data(), zone_key, d);
         if (ok) b.pin_neutral[k] |= 1ull << d;
       }
     }
@@ -638,6 +659,7 @@ static int bind_catalog(ksched_handle* h, const ksched_catalog* cat, const Catal
   c.type_relevant = b.type_relevant;
   c.zone_key = b.zone_key; c.ct_key = b.ct_key;
   std::memcpy(c.pin_neutral, b.pin_neutral, sizeof c.pin_neutral);
+  c.zone_used = b.zone_used; c.ct_used = b.ct_used; c.all_slots = b.all_slots; c.offer_used = b.offer_used;
   c.n_res_ext = cat->n_res_ext;
   CUDA_TRY(h, bind(h, h->d_keys, c.keys, b.keys.size(), b.keys.data()));
   if (cat->key_regions) CUDA_TRY(h, bind(h, h->d_key_regions, c.key_regions, (size_t)NK, cat->key_regions));
@@ -654,6 +676,7 @@ static int bind_catalog(ksched_handle* h, const ksched_catalog* cat, const Catal
   CUDA_TRY(h, bind(h, h->d_negempty, c.negempty, b.negempty.size(), b.negempty.data()));
   CUDA_TRY(h, bind(h, h->d_offset, c.offset, b.offset.size(), b.offset.data()));
   CUDA_TRY(h, bind(h, h->d_anyoffer, c.anyoffer, b.anyoffer.size(), b.anyoffer.data()));
+  CUDA_TRY(h, bind(h, h->d_slots, c.slots, b.slots.size(), b.slots.data()));
   CUDA_TRY(h, bind(h, h->d_member, c.member, b.member.size(), b.member.data()));
   CUDA_TRY(h, bind(h, h->d_alloc_sorted, c.alloc_sorted, b.alloc_sorted.size(), b.alloc_sorted.data()));
   CUDA_TRY(h, bind(h, h->d_perm_desc, c.perm_desc, b.perm_desc.size(), b.perm_desc.data()));
@@ -1228,7 +1251,7 @@ static int run_class_feasibility(ksched_handle* h, int P) {
   const size_t alloc_bytes = (size_t)c.n_res * c.n_types * sizeof(int64_t);
   k1.alloc_in_smem = alloc_bytes <= (size_t)(128 << 10) ? 1 : 0;
   size_t smem = sizeof(ksched_template) * c.n_templates + sizeof(ksched_keyinfo) * KSCHED_MAX_KEYS + (k1.alloc_in_smem ? alloc_bytes : 0) +
-                sizeof(int16_t) * KSCHED_MAX_KEYS * 64 + sizeof(int16_t) * 64;
+                sizeof(int16_t) * KSCHED_MAX_KEYS * 64 + sizeof(int16_t) * 64 + sizeof(uint64_t) * 128;
   k1.n_valrows = h->n_valrows;
   k1.n_offrows = h->n_offrows;
   const size_t table_bytes = (size_t)(h->n_valrows + 2 * c.n_keys + h->n_offrows + 1 + c.n_templates) * c.W32 * sizeof(uint32_t);

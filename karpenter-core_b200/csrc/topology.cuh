@@ -389,9 +389,9 @@ struct TypeCtx {
   int nkeys;
   int8_t key[KSCHED_MAX_KEYS];
   uint64_t allowed[KSCHED_MAX_KEYS];
+  uint64_t slots;  // admitted offering slots (offer_word), when offer_needed and not offer_unconstrained
   bool neg[KSCHED_MAX_KEYS];
   bool offer_needed, offer_unconstrained;
-  uint32_t zmask, cmask;
   uint32_t itype_req;
 };
 __device__ __noinline__ void build_type_ctx(const Touched& t, const long long* q,
@@ -429,20 +429,22 @@ __device__ __noinline__ void build_type_ctx(const Touched& t, const long long* q
       if (t.key[i] == c.zone_key || t.key[i] == c.ct_key) x.offer_needed = true;
     }
   }
-  x.zmask = 0xFFFF; x.cmask = 0xF; x.offer_unconstrained = true;
+  x.slots = ~0ull; x.offer_unconstrained = true;
   if (x.offer_needed) {
+    uint64_t zallowed = ~0ull, callowed = ~0ull;
     auto final_req = [&](int k) -> Req {
       for (int i = 0; i < t.n; ++i) if (t.key[i] == k) return t.fin[i];
       return load_soa(vals, meta, stride, idx, k);
     };
     if (c.zone_key >= 0) {
       Req z = final_req(c.zone_key);
-      if (z.present) { x.zmask = (uint32_t)ksched::req_allowed(z, c.keys[c.zone_key].dict_mask, key_meta(c, c.zone_key)); x.offer_unconstrained = false; }
+      if (z.present) { zallowed = ksched::req_allowed(z, c.keys[c.zone_key].dict_mask, key_meta(c, c.zone_key)); x.offer_unconstrained = false; }
     }
     if (c.ct_key >= 0) {
       Req ct = final_req(c.ct_key);
-      if (ct.present) { x.cmask = (uint32_t)ksched::req_allowed(ct, c.keys[c.ct_key].dict_mask, key_meta(c, c.ct_key)); x.offer_unconstrained = false; }
+      if (ct.present) { callowed = ksched::req_allowed(ct, c.keys[c.ct_key].dict_mask, key_meta(c, c.ct_key)); x.offer_unconstrained = false; }
     }
+    if (!x.offer_unconstrained) x.slots = node_slots(c, zallowed, callowed);
   }
   x.itype_req = row.itype_req;
 }
@@ -458,7 +460,7 @@ __device__ __forceinline__ uint32_t type_word_res(const DevCatalog& c, const Typ
 }
 __device__ __forceinline__ uint32_t type_word_keys(const DevCatalog& c, const PackState& s, const TypeCtx& x, uint32_t sw, int w) {
   for (int i = 0; i < x.nkeys && sw; ++i) sw &= key_typeset_word(c, x.key[i], x.allowed[i], x.neg[i], w);
-  if (sw && x.offer_needed) sw &= offer_word(c, x.zmask, x.cmask, x.offer_unconstrained, w);
+  if (sw && x.offer_needed) sw &= offer_word(c, x.slots, x.offer_unconstrained, w);
   if (sw && x.itype_req != KSCHED_NONE) sw &= s.itype_sets[(size_t)x.itype_req * c.W32 + w];
   return sw;
 }

@@ -1237,6 +1237,38 @@ void instance_types(Builder& B) {
     for (auto& o : it.offerings) if (o.available) prices.insert(o.price);
   E.price_by_rank.assign(prices.begin(), prices.end());
   E.offering_keys.assign((size_t)NT * 64, ~0ull);
+  // Offering slots. An available offering whose zone / capacity type is not a dictionary value can never satisfy a *present*
+  // requirement and gets no slot; when a key is inactive every offering counts as its value 0, which is exactly "key not
+  // constrained". The pair (ct, z) is slot ct*16 + z while every pair fits that; otherwise the distinct pairs are numbered
+  // densely in ascending (ct, z) order, and the slot tables of ksched_catalog say which pairs the slots are.
+  auto offering_pair = [&](const Offering& o, int& z, int& ct) {
+    z = 0; ct = 0;
+    if (zone_key >= 0) { auto f = B.value_id[zone_key].find(o.zone); if (f == B.value_id[zone_key].end()) return false; z = f->second; }
+    if (ct_key >= 0) { auto f = B.value_id[ct_key].find(o.capacity_type); if (f == B.value_id[ct_key].end()) return false; ct = f->second; }
+    return true;
+  };
+  std::set<std::pair<int, int>> pairs;  // (ct, z)
+  for (auto& it : P.instance_types)
+    for (auto& o : it.offerings) {
+      int z, ct;
+      if (o.available && offering_pair(o, z, ct)) pairs.insert({ct, z});
+    }
+  const bool formula = std::all_of(pairs.begin(), pairs.end(), [](const std::pair<int, int>& p) { return p.first < 4 && p.second < 16; });
+  std::map<std::pair<int, int>, int> slot_of;
+  if (formula) {
+    for (auto& p : pairs) slot_of[p] = p.first * 16 + p.second;
+  } else {
+    if (pairs.size() > 64)
+      unsupported("more than 64 (capacity type, zone) pairs with an available offering (" + std::to_string(pairs.size()) + " pairs)");
+    E.offering_slots = (int)pairs.size();
+    E.offering_slot_tables.assign(128, 0);
+    for (auto& p : pairs) {
+      const int s = (int)slot_of.size();
+      slot_of[p] = s;
+      E.offering_slot_tables[(size_t)p.second] |= 1ull << s;
+      E.offering_slot_tables[64 + (size_t)p.first] |= 1ull << s;
+    }
+  }
   for (int c = 0; c < NT; ++c) {
     const InstanceType& it = P.instance_types[E.type_input_index[c]];
     if (B.type_col.count(it.name)) unsupported("duplicate instance type name " + it.name);
@@ -1265,21 +1297,17 @@ void instance_types(Builder& B) {
     row.res_present = B.fill_resources(alloc, row.allocatable);
     B.fill_resources(it.capacity, &E.type_capacity[(size_t)c * KSCHED_MAX_RES]);
     if (E.n_res_ext) B.fill_ext(alloc, &E.type_alloc_ext[(size_t)c * E.n_res_ext]);
-    // offerings whose zone / capacity-type is not a dictionary value can never satisfy a *present* requirement; when the key
-    // is inactive every offering maps to z=0 / ct=0, which is exactly "key not constrained"
     for (size_t oi = 0; oi < it.offerings.size(); ++oi) {
       const Offering& o = it.offerings[oi];
-      if (!o.available) continue;
-      int z = 0, ct = 0;
-      if (zone_key >= 0) { auto f = B.value_id[zone_key].find(o.zone); if (f == B.value_id[zone_key].end()) continue; z = f->second; }
-      if (ct_key >= 0) { auto f = B.value_id[ct_key].find(o.capacity_type); if (f == B.value_id[ct_key].end()) continue; ct = f->second; }
-      if (z >= 16 || ct >= 4) unsupported("more than 16 zones or 4 capacity types");
-      row.offerings |= 1ull << (ct * 16 + z);
+      int z, ct;
+      if (!o.available || !offering_pair(o, z, ct)) continue;
+      const int slot = slot_of.at({ct, z});
+      row.offerings |= 1ull << slot;
       // (price rank, Offerings list position, slot): the smallest key of a slot wins when several offerings share it
       if (oi > 255) unsupported("instance type " + it.name + " has more than 256 offerings");
       const uint64_t rank = (uint64_t)(std::lower_bound(E.price_by_rank.begin(), E.price_by_rank.end(), o.price) - E.price_by_rank.begin());
-      const uint64_t key = (rank << 16) | ((uint64_t)oi << 8) | (uint64_t)(ct * 16 + z);
-      uint64_t& cell = E.offering_keys[(size_t)c * 64 + ct * 16 + z];
+      const uint64_t key = (rank << 16) | ((uint64_t)oi << 8) | (uint64_t)slot;
+      uint64_t& cell = E.offering_keys[(size_t)c * 64 + slot];
       if (key < cell) cell = key;
     }
     row.min_price = min_price[E.type_input_index[c]];
@@ -2082,6 +2110,8 @@ void wire(Builder& B) {
   cat.type_capacity = E.type_capacity.data();
   cat.templates = E.templates.data();
   cat.offering_keys = E.offering_keys.data();
+  cat.zone_slots = E.offering_slots ? E.offering_slot_tables.data() : nullptr;
+  cat.ct_slots = E.offering_slots ? E.offering_slot_tables.data() + 64 : nullptr;
   ksched_problem& pr = E.problem;
   pr.n_pods = (int)E.pods.size(); pr.n_classes = NC; pr.n_existing = NE; pr.n_groups = (int)E.groups.size();
   pr.classes = E.classes.data();

@@ -69,6 +69,8 @@ struct Encoded {
   std::vector<int64_t> type_capacity;
   std::vector<uint64_t> offering_keys;                // [n_types][64] launch-choice table (ksched_catalog.offering_keys)
   std::vector<double> price_by_rank;                  // distinct available offering prices, ascending (rank -> price)
+  int offering_slots = 0;                             // dense offering slots (ksched.h: zone_slots); 0 = the ct*16 + zone layout
+  std::vector<uint64_t> offering_slot_tables;         // [128] zone_slots then ct_slots; empty for the ct*16 + zone layout
   std::vector<ksched_template> templates;
   std::vector<ksched_bounds> template_bounds;
   std::vector<ksched_pod_row> classes;

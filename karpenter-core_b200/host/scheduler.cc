@@ -362,6 +362,7 @@ void kh_encoded_free(Encoded* E) {
 // dims: [pods, classes, existing, groups, types, templates, keys, resources, type_words, class_topo, taintsets, resources_ext,
 //        hostports, hostport_ext_words, hostname_reqs, hostname_words, itype_reqs, itype_filter_terms, volume_claims,
 //        volume_ext_words]
+// (fixed at 20 entries: callers size their buffers by it; later counts have accessors of their own, kh_encoded_offering_slots)
 // (itype_filter_terms: filter terms with an instance-type part; 0 exactly when the problem has no instance-type filter tables)
 void kh_encoded_dims(const Encoded* E, long long* out) {
   out[14] = (long long)E->hostname_reqs.size() / 2; out[15] = E->hostname_words;
@@ -373,6 +374,26 @@ void kh_encoded_dims(const Encoded* E, long long* out) {
   out[9] = (long long)E->class_topo.size(); out[10] = E->n_taintsets; out[11] = E->n_res_ext;
   out[12] = (long long)E->hostports.size(); out[13] = E->hostport_ext_words;
   out[18] = (long long)E->volume_claims.size(); out[19] = E->volume_ext_words;
+}
+// dense offering slots of an encoding (ksched.h: zone_slots), 0 for the ct*16 + zone layout
+long long kh_encoded_offering_slots(const Encoded* E) { return E->offering_slots; }
+// Offering slot `slot` of an encoding with slot tables as "capacity-type zone" into out[cap] (tests): the pair the slot stands
+// for, each part the dictionary value (empty when the problem has no such mask key). Returns -1 when there is no such slot or
+// it does not fit.
+int kh_encoded_offering_slot(const Encoded* E, int slot, char* out, int cap) {
+  if (slot < 0 || slot >= E->offering_slots) return -1;
+  std::string names[2];
+  const char* keys[2] = {"karpenter.sh/capacity-type", "topology.kubernetes.io/zone"};
+  const int table[2] = {64, 0};
+  for (int part = 0; part < 2; ++part)
+    for (size_t k = 0; k < E->key_names.size(); ++k)
+      if (E->key_names[k] == keys[part])
+        for (int v = 0; v < 64; ++v)
+          if ((E->offering_slot_tables[(size_t)(table[part] + v)] >> slot) & 1) names[part] = E->key_values[k][(size_t)v];
+  const std::string pair = names[0] + " " + names[1];
+  if ((int)pair.size() >= cap) return -1;
+  std::memcpy(out, pair.c_str(), pair.size() + 1);
+  return 0;
 }
 // Host-port entry `id` of an encoding as "ip port protocol" into out[cap] (tests): the entries the encoder kept, in id order.
 // Returns -1 when there is no such entry or it does not fit.
@@ -1289,7 +1310,8 @@ extern "C" int kh_launch_table_selfcheck(const Problem* P, const Result* ref) {
       if (E->key_names[k] == "karpenter.sh/capacity-type") ct_key = (int)k;
     }
     // admissible dictionary ids of a rendered requirement ("In [a b]", "NotIn [a]", "Exists", "DoesNotExist")
-    auto allowed = [&](int key, const std::map<std::string, std::string>& reqs, uint32_t all) -> uint32_t {
+    auto allowed = [&](int key, const std::map<std::string, std::string>& reqs) -> uint64_t {
+      const uint64_t all = ~0ull;
       if (key < 0) return all;
       auto it = reqs.find(E->key_names[(size_t)key]);
       if (it == reqs.end()) return all;
@@ -1302,23 +1324,34 @@ extern "C" int kh_launch_table_selfcheck(const Problem* P, const Result* ref) {
         if (!cur.empty()) vals.insert(cur);
       }
       const bool is_in = r.rfind("In", 0) == 0, is_notin = r.rfind("NotIn", 0) == 0, exists = r.rfind("Exists", 0) == 0;
-      uint32_t m = 0;
+      uint64_t m = 0;
       for (size_t b = 0; b < E->key_values[(size_t)key].size(); ++b) {
         const bool has = vals.count(E->key_values[(size_t)key][b]) > 0;
-        if (exists || (is_in && has) || (is_notin && !has)) m |= 1u << b;
+        if (exists || (is_in && has) || (is_notin && !has)) m |= 1ull << b;
       }
       return m;
     };
     std::vector<int> col_of(P->instance_types.size(), -1);
     for (size_t c = 0; c < E->type_input_index.size(); ++c) col_of[(size_t)E->type_input_index[c]] = (int)c;
+    // the offering slot tables the catalog carries, or those of the ct*16 + zone layout (ksched.h: zone_slots)
+    std::vector<uint64_t> tables(128, 0);
+    if (E->offering_slots) tables = E->offering_slot_tables;
+    else ksched::formula_slot_tables(tables.data(), tables.data() + 64);
+    uint64_t zone_used = 0, ct_used = 0, all_slots = 0;
+    for (int v = 0; v < 64; ++v) {
+      if (tables[(size_t)v]) zone_used |= 1ull << v;
+      if (tables[64 + (size_t)v]) ct_used |= 1ull << v;
+      all_slots |= tables[(size_t)v];
+    }
     int bad = 0;
     for (auto& nn : ref->new_nodes) {
-      const uint32_t zmask = allowed(zone_key, nn.requirements, 0xFFFF), cmask = allowed(ct_key, nn.requirements, 0xF);
+      const uint64_t slots = ksched::admitted_slots(tables.data(), zone_used, ct_used, all_slots, allowed(zone_key, nn.requirements),
+                                                    allowed(ct_key, nn.requirements));
       uint64_t best = ~0ull, best_off = ksched::kNoOffering;
       int best_col = -1;
       for (int ti : kmodel::node_options(*ref, nn)) {
         const int c = col_of[(size_t)ti];
-        const uint64_t ok = ksched::offering_min_key(&E->offering_keys[(size_t)c * 64], zmask, cmask);
+        const uint64_t ok = ksched::offering_min_key(&E->offering_keys[(size_t)c * 64], slots);
         if (ok == ksched::kNoOffering) continue;
         const uint64_t key = ksched::option_key(ok, E->types[(size_t)c].input_index);
         if (key < best) { best = key; best_off = ok; best_col = c; }
@@ -1374,6 +1407,7 @@ extern "C" unsigned long long kh_encoded_digest(const Encoded* E) {
   if (E->hostport_ext_words) {  // absent with at most 64 host-port entries: those digests predate the entry tables
     vec(E->class_hostport_conflicts_ext); vec(E->class_hostport_entries_ext); vec(E->existing_hostport_ext);
   }
+  if (E->offering_slots) vec(E->offering_slot_tables);  // absent for the ct*16 + zone layout: those digests predate the slot tables
   if (E->hostname_words) { vec(E->hostname_slots); vec(E->filter_term_hostname); }  // absent without the hostname table: those digests predate it
   if (!E->filter_term_itype.empty()) { vec(E->filter_term_itype); vec(E->template_itype); vec(E->existing_itype); }  // likewise
   if (E->n_res_ext) {  // absent with at most 8 read resources: those digests predate ext resources

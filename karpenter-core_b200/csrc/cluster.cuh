@@ -137,9 +137,11 @@ __global__ void rank_cost_kernel(int n_nodes, const int32_t* __restrict__ pod_of
   cost[n] = c;
   eligible[n] = ok ? 1 : 0;
 }
+// The disruption order's strict weak order (R8): a NaN cost sorts after every number and ties with another NaN.
+__device__ __forceinline__ bool cost_before(double a, double b) { return !isnan(a) && (isnan(b) || a < b); }
 // sort.Slice(nodes, disruptionCost <) as a rank computation: position of an eligible node = the number of eligible nodes with
-// a smaller cost, or the same cost and a smaller index (R4: stable). O(n^2) compares over shared-memory tiles - thousands of
-// nodes, microseconds.
+// a smaller cost, or an equal cost and a smaller index (R4: stable, R8: NaN last). O(n^2) compares over shared-memory tiles -
+// thousands of nodes, microseconds.
 __global__ void rank_position_kernel(int n_nodes, const double* __restrict__ cost, const uint8_t* __restrict__ eligible, int32_t* __restrict__ order,
                                      double* __restrict__ cost_out, int32_t* __restrict__ n_out) {
   __shared__ double t_cost[256];
@@ -158,7 +160,7 @@ __global__ void rank_position_kernel(int n_nodes, const double* __restrict__ cos
       if (!t_ok[q]) continue;
       ++total;
       const double cj = t_cost[q];
-      if (cj < ci || (!(ci < cj) && base + q < i)) ++rank;
+      if (cost_before(cj, ci) || (!cost_before(ci, cj) && base + q < i)) ++rank;
     }
     __syncthreads();
   }

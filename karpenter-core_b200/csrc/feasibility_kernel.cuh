@@ -6,30 +6,15 @@
 // ------------------------------------------------------------------------------------------------
 // K0: queue order
 // ------------------------------------------------------------------------------------------------
-__global__ void sort_keys_kernel(int n, const ksched_pod_row* __restrict__ classes, const uint32_t* __restrict__ pod_class,
-                                 const int64_t* __restrict__ ts, const uint32_t* __restrict__ uid_rank,
-                                 uint64_t* k_cpu, uint64_t* k_mem, uint64_t* k_tie, uint32_t* idx) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const ksched_pod_row& row = classes[pod_class[i]];
-  // descending cpu / memory -> ascending on the complemented value (milli-units are < 2^62)
-  k_cpu[i] = ~(uint64_t)(row.requests[0] + (1ll << 62));
-  k_mem[i] = ~(uint64_t)(row.requests[1] + (1ll << 62));
-  k_tie[i] = ((uint64_t)(ts[i] + (1ll << 32)) << 30) | (uint64_t)uid_rank[i];
-  idx[i] = (uint32_t)i;
-}
-// The same order from ONE packed key when it fits 64 bits: (rank of the class's (cpu, memory) pair among all classes,
-// timestamp - min timestamp, UID rank). cls_rank is built on the host at upload (classes are few).
+// queue.go:82-108 (cpu desc, memory desc, timestamp asc, UID asc) as ONE packed key: (rank of the class's (cpu, memory)
+// pair among all classes, timestamp - ts_min or the timestamp's dense rank, UID rank). cls_rank and the timestamp field are
+// chosen on the host at upload (bind_problem).
 __global__ void sort_key1_kernel(int n, const uint32_t* __restrict__ cls_rank, const uint32_t* __restrict__ pod_class, const int64_t* __restrict__ ts,
                                  const uint32_t* __restrict__ uid_rank, long long ts_min, int ts_bits, int uid_bits, uint64_t* key, uint32_t* idx) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   key[i] = ((uint64_t)cls_rank[pod_class[i]] << (ts_bits + uid_bits)) | ((uint64_t)(ts[i] - ts_min) << uid_bits) | (uint64_t)uid_rank[i];
   idx[i] = (uint32_t)i;
-}
-__global__ void gather_u64_kernel(int n, const uint64_t* __restrict__ src, const uint32_t* __restrict__ idx, uint64_t* dst) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) dst[i] = src[idx[i]];
 }
 // FFD-ordered dense pod-row matrix: row j = class row of the j-th pod of the queue. One warp per row,
 // 256-byte coalesced loads and stores.

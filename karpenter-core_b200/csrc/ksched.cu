@@ -211,9 +211,10 @@ struct ksched_handle {
   bool sorted = false;  // the FFD-ordered pod-row matrix of the uploaded problem exists
   PackState st{};
   ResetTable resets{};
-  // one-pass queue order (feasibility_kernel.cuh: sort_key1_kernel): total key bits, 0 = the three-key path
+  // queue order (feasibility_kernel.cuh: sort_key1_kernel): total key bits and the timestamp field's width and origin
   int sort1_bits = 0, sort1_ts_bits = 0, sort1_uid_bits = 0;
   long long sort1_ts_min = 0;
+  std::vector<int64_t> ts_dense;  // each pod's rank among the distinct timestamps when the offset is too wide, else empty
   size_t cub_tmp_bytes = 0;
   // inputs
   DevBuf<ksched_pod_row> d_classes;
@@ -248,7 +249,7 @@ struct ksched_handle {
   DevBuf<long long> d_counters;  // kNumCounters entries (Counter)
   // K0 / K1
   DevBuf<uint32_t> d_order, d_idx_tmp, d_pod_pos, d_F, d_Fclass;
-  DevBuf<uint64_t> d_k_cpu, d_k_mem, d_k_tie, d_k_tmp, d_rows;
+  DevBuf<uint64_t> d_k_tie, d_k_tmp, d_rows;
   DevBuf<unsigned long long> d_best, d_best_class;
   DevBuf<uint8_t> d_cub_tmp;
   // new nodes, open-node overflow and the fresh-node memos (PackState)
@@ -393,8 +394,7 @@ int ksched_create(int device_ordinal, ksched_handle** out) {
     cudaFuncGetAttributes(&fa, class_feasibility_kernel);
     cudaFuncGetAttributes(&fa, finalize_options_kernel);
     cudaFuncGetAttributes(&fa, gather_rows_kernel);
-    cudaFuncGetAttributes(&fa, sort_keys_kernel);
-    cudaFuncGetAttributes(&fa, gather_u64_kernel);
+    cudaFuncGetAttributes(&fa, sort_key1_kernel);
   }
   *out = h;
   return KSCHED_OK;
@@ -876,6 +876,11 @@ static int check_problem(ksched_handle* h, const ksched_problem* pb) {
   return KSCHED_OK;
 }
 
+// the timestamps sort_key1_kernel reads for pb, once bind_problem has chosen the timestamp field
+static const int64_t* queue_timestamps(const ksched_handle* h, const ksched_problem* pb) {
+  return h->ts_dense.empty() ? pb->pod_timestamp : h->ts_dense.data();
+}
+
 // Uploads one checked problem and binds every PackState field to it (ksched_upload's commit). Arrays the pack kernel mutates
 // get a pristine copy that reset_state restores before every run.
 static int bind_problem(ksched_handle* h, const ksched_problem* pb) {
@@ -914,7 +919,7 @@ static int bind_problem(ksched_handle* h, const ksched_problem* pb) {
   }
   {
     // queue.go:82-108 orders by cpu desc, memory desc, timestamp asc, UID asc. (cpu, memory) is a property of the class: rank
-    // the classes once here, and the whole order is one packed key when rank, timestamp span and UID rank fit 64 bits.
+    // the classes once here, and the whole order is one packed key of class rank, timestamp field and UID rank.
     std::vector<uint32_t> by((size_t)NC), rank(nc, 0);
     for (int i = 0; i < NC; ++i) by[(size_t)i] = (uint32_t)i;
     auto cpu = [&](uint32_t i) { return pb->classes[i].requests[0]; };
@@ -934,17 +939,35 @@ static int bind_problem(ksched_handle* h, const ksched_problem* pb) {
       if (i == 0 || t > ts_max) ts_max = t;
       uid_max = std::max(uid_max, pb->pod_uid_rank[i]);
     }
-    const unsigned long long span = (unsigned long long)(ts_max - ts_min);
+    // the timestamp field: the offset from the earliest timestamp, or, when that is too wide, the timestamp's rank among
+    // the batch's distinct timestamps (the same order). Every field is then at most bits(P - 1) wide, so the key always
+    // fits for batches of up to 2^21 pods.
+    const unsigned long long span = (unsigned long long)ts_max - (unsigned long long)ts_min;
+    h->ts_dense.clear();
     h->sort1_ts_bits = bits(span);
     h->sort1_uid_bits = bits(uid_max);
     h->sort1_ts_min = ts_min;
-    const int total = bits(r) + h->sort1_ts_bits + h->sort1_uid_bits;
-    h->sort1_bits = (span < (1ull << 62) && total <= 64 && !std::getenv("KSCHED_SORT3")) ? total : 0;
+    if (span >= (1ull << 62) || bits(r) + h->sort1_ts_bits + h->sort1_uid_bits > 64) {
+      std::vector<int64_t> distinct(pb->pod_timestamp, pb->pod_timestamp + P);
+      std::sort(distinct.begin(), distinct.end());
+      distinct.erase(std::unique(distinct.begin(), distinct.end()), distinct.end());
+      h->ts_dense.resize((size_t)P);
+      for (int i = 0; i < P; ++i)
+        h->ts_dense[(size_t)i] = std::lower_bound(distinct.begin(), distinct.end(), pb->pod_timestamp[i]) - distinct.begin();
+      h->sort1_ts_bits = bits(distinct.size() - 1);
+      h->sort1_ts_min = 0;
+    }
+    h->sort1_bits = bits(r) + h->sort1_ts_bits + h->sort1_uid_bits;
+    if (h->sort1_bits > 64) {
+      h->err = "unsupported: the queue order key of " + std::to_string(P) + " pods needs " + std::to_string(h->sort1_bits) +
+               " bits (class, timestamp and UID ranks; at most 64)";
+      return KSCHED_ERR_UNSUPPORTED;
+    }
     CUDA_TRY(h, upload_vec(h, h->d_cls_rank, rank));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));  // rank is a stack vector
   }
   CUDA_TRY(h, bind_restored(h, h->d_pod_class, s.pod_class, h->d_pod_class0, (size_t)P, pb->pod_class));
-  CUDA_TRY(h, upload(h, h->d_ts, pb->pod_timestamp, (size_t)P));
+  CUDA_TRY(h, upload(h, h->d_ts, queue_timestamps(h, pb), (size_t)P));
   CUDA_TRY(h, upload(h, h->d_uid_rank, pb->pod_uid_rank, (size_t)P));
   CUDA_TRY(h, bind(h, h->d_groups, s.groups, (size_t)NG, pb->groups));
   CUDA_TRY(h, bind(h, h->d_class_topo, s.class_topo, (size_t)pb->n_class_topo, pb->class_topo));
@@ -1101,8 +1124,6 @@ static int bind_problem(ksched_handle* h, const ksched_problem* pb) {
   CUDA_TRY(h, bind(h, h->d_order, s.order, p1));
   CUDA_TRY(h, h->d_idx_tmp.ensure(p1));
   CUDA_TRY(h, bind(h, h->d_pod_pos, s.pod_pos, p1));
-  CUDA_TRY(h, h->d_k_cpu.ensure(p1));
-  CUDA_TRY(h, h->d_k_mem.ensure(p1));
   CUDA_TRY(h, h->d_k_tie.ensure(p1));
   CUDA_TRY(h, h->d_k_tmp.ensure(p1));
   CUDA_TRY(h, bind(h, h->d_rows, s.rows, p1 * KSCHED_ROW_WORDS));
@@ -1187,34 +1208,15 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
 static int run_sort(ksched_handle* h, int P) {
   if (P == 0) return KSCHED_OK;
   const int threads = 256, blocks = (P + threads - 1) / threads;
-  if (h->sort1_bits > 0) {  // one packed key, only its significant bits sorted
-    sort_key1_kernel<<<blocks, threads, 0, h->stream>>>(P, h->d_cls_rank.ptr, h->d_pod_class.ptr, h->d_ts.ptr, h->d_uid_rank.ptr, h->sort1_ts_min,
-                                                        h->sort1_ts_bits, h->sort1_uid_bits, h->d_k_tie.ptr, h->d_idx_tmp.ptr);
-    size_t tmp1 = h->cub_tmp_bytes;
-    CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(h->d_cub_tmp.ptr, tmp1, h->d_k_tie.ptr, h->d_k_tmp.ptr, h->d_idx_tmp.ptr, h->d_order.ptr, P, 0, h->sort1_bits,
-                                                h->stream));
-    const int gblocks1 = std::min((P + 7) / 8, h->n_sm * 8);
-    gather_rows_kernel<<<gblocks1, 256, 0, h->stream>>>(P, h->d_classes.ptr, h->d_pod_class.ptr, h->d_order.ptr, h->d_rows.ptr);
-    h->tm.sort_launches = 3;
-    h->sorted = true;
-    return KSCHED_OK;
-  }
-  sort_keys_kernel<<<blocks, threads, 0, h->stream>>>(P, h->d_classes.ptr, h->d_pod_class.ptr, h->d_ts.ptr, h->d_uid_rank.ptr, h->d_k_cpu.ptr,
-                                                      h->d_k_mem.ptr, h->d_k_tie.ptr, h->d_order.ptr);
-  // LSD over three 64-bit keys with a stable radix sort: tie-break key first, cpu last
+  // one packed key (bind_problem), only its significant bits sorted
+  sort_key1_kernel<<<blocks, threads, 0, h->stream>>>(P, h->d_cls_rank.ptr, h->d_pod_class.ptr, h->d_ts.ptr, h->d_uid_rank.ptr, h->sort1_ts_min,
+                                                      h->sort1_ts_bits, h->sort1_uid_bits, h->d_k_tie.ptr, h->d_idx_tmp.ptr);
   size_t tmp = h->cub_tmp_bytes;
-  uint32_t *ia = h->d_order.ptr, *ib = h->d_idx_tmp.ptr;
-  CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(h->d_cub_tmp.ptr, tmp, h->d_k_tie.ptr, h->d_k_tmp.ptr, ia, ib, P, 0, 64, h->stream));
-  gather_u64_kernel<<<blocks, threads, 0, h->stream>>>(P, h->d_k_mem.ptr, ib, h->d_k_tie.ptr);
-  tmp = h->cub_tmp_bytes;
-  CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(h->d_cub_tmp.ptr, tmp, h->d_k_tie.ptr, h->d_k_tmp.ptr, ib, ia, P, 0, 64, h->stream));
-  gather_u64_kernel<<<blocks, threads, 0, h->stream>>>(P, h->d_k_cpu.ptr, ia, h->d_k_tie.ptr);
-  tmp = h->cub_tmp_bytes;
-  CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(h->d_cub_tmp.ptr, tmp, h->d_k_tie.ptr, h->d_k_tmp.ptr, ia, ib, P, 0, 64, h->stream));
-  CUDA_TRY(h, cudaMemcpyAsync(h->d_order.ptr, ib, (size_t)P * sizeof(uint32_t), cudaMemcpyDeviceToDevice, h->stream));
+  CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(h->d_cub_tmp.ptr, tmp, h->d_k_tie.ptr, h->d_k_tmp.ptr, h->d_idx_tmp.ptr, h->d_order.ptr, P, 0, h->sort1_bits,
+                                              h->stream));
   const int gblocks = std::min((P + 7) / 8, h->n_sm * 8);
   gather_rows_kernel<<<gblocks, 256, 0, h->stream>>>(P, h->d_classes.ptr, h->d_pod_class.ptr, h->d_order.ptr, h->d_rows.ptr);
-  h->tm.sort_launches = 7;
+  h->tm.sort_launches = 3;
   h->sorted = true;
   return KSCHED_OK;
 }
@@ -1657,7 +1659,7 @@ int ksched_load_cluster(ksched_handle* h, const ksched_cluster* cl) {
   if (rc != KSCHED_OK) return rc;
   CUDA_TRY(h, upload(h, h->d_sup_pod_node, cl->pod_node, (size_t)P));
   CUDA_TRY(h, upload(h, h->d_sup_class, pb->pod_class, (size_t)P));
-  CUDA_TRY(h, upload(h, h->d_sup_ts, pb->pod_timestamp, (size_t)P));
+  CUDA_TRY(h, upload(h, h->d_sup_ts, queue_timestamps(h, pb), (size_t)P));
   CUDA_TRY(h, upload(h, h->d_sup_uid, pb->pod_uid_rank, (size_t)P));
   CUDA_TRY(h, upload_vec(h, h->d_node_first, first));
   CUDA_TRY(h, h->d_node_dst.ensure((size_t)std::max(NE, 1)));

@@ -140,10 +140,17 @@ HostnameReq hostname_intersection(const std::vector<NodeSelectorRequirement>& rs
 }
 
 // ---- resources (utils/resources/resources.go)
-ResourceList merge(const ResourceList& a, const ResourceList& b) {
+ResourceList merge(const ResourceList& a, const ResourceList& b) {  // checked: sums stay inside kQuantityBound
   ResourceList r = a;
-  for (auto& kv : b) r[kv.first] += kv.second;
+  for (auto& kv : b) r[kv.first] = checked_quantity((__int128)r[kv.first] + kv.second, kv.first);
   return r;
+}
+// lhs[k] -= rhs[k] for the keys of lhs that rhs has (resources.Subtract), checked like merge
+void subtract_in_place(ResourceList& lhs, const ResourceList& rhs) {
+  for (auto& kv : lhs) {
+    auto f = rhs.find(kv.first);
+    if (f != rhs.end()) kv.second = checked_quantity((__int128)kv.second - f->second, kv.first);
+  }
 }
 ResourceList pod_requests(const Pod& p) {  // RequestsForPods(pod): Ceiling + pods:1
   ResourceList r;
@@ -1293,7 +1300,7 @@ void instance_types(Builder& B) {
     row.meta = rs.meta;
     ResourceList overhead = merge(merge(it.kube_reserved, it.system_reserved), it.eviction_threshold);
     ResourceList alloc = it.capacity;  // resources.Subtract only over keys of capacity
-    for (auto& kv : alloc) { auto o = overhead.find(kv.first); if (o != overhead.end()) kv.second -= o->second; }
+    subtract_in_place(alloc, overhead);
     row.res_present = B.fill_resources(alloc, row.allocatable);
     B.fill_resources(it.capacity, &E.type_capacity[(size_t)c * KSCHED_MAX_RES]);
     if (E.n_res_ext) B.fill_ext(alloc, &E.type_alloc_ext[(size_t)c * E.n_res_ext]);
@@ -1536,6 +1543,9 @@ void existing_nodes(Builder& B) {
   const Problem& P = B.P;
   Encoded& E = B.E;
   const int NV = (int)E.templates.size();
+  E.remaining_exact.resize((size_t)NV * KSCHED_MAX_RES);
+  for (int v = 0; v < NV; ++v)
+    for (int r = 0; r < KSCHED_MAX_RES; ++r) E.remaining_exact[(size_t)v * KSCHED_MAX_RES + r] = E.templates[v].remaining[r];
   for (int si : B.state_nodes) {
     const StateNode& n = P.nodes[si];
     auto own = n.labels.find(kProvisionerName);
@@ -1548,9 +1558,10 @@ void existing_nodes(Builder& B) {
     B.add_selector_reqs(e.reqs, nb, nf.label_reqs, &sp);
     // the daemonsets' requests not yet bound: resources.Subtract over keys of lhs, clamped at 0
     ResourceList rem = daemon_overhead(B, n.taints, e.reqs, nb, false);  // raw Spec.Taints (scheduler.go:231)
-    for (auto& kv : rem) { auto f = nf.ds_req.find(kv.first); if (f != nf.ds_req.end()) kv.second -= f->second; if (kv.second < 0) kv.second = 0; }
+    subtract_in_place(rem, nf.ds_req);
+    for (auto& kv : rem) if (kv.second < 0) kv.second = 0;
     ResourceList avail = n.allocatable;
-    for (auto& kv : avail) { auto f = nf.pod_req.find(kv.first); if (f != nf.pod_req.end()) kv.second -= f->second; }
+    subtract_in_place(avail, nf.pod_req);
     e.available_present = B.fill_resources(avail, e.available);
     e.requests_present = B.fill_resources(rem, e.requests);
     if (E.n_res_ext) {
@@ -1609,7 +1620,11 @@ void existing_nodes(Builder& B) {
         int64_t cap[KSCHED_MAX_RES];
         uint32_t present = B.fill_resources(n.capacity, cap);
         for (int r = 0; r < KSCHED_MAX_RES; ++r)
-          if ((E.templates[v].limit_present >> r) & 1 && (present >> r) & 1) { E.templates[v].remaining[r] -= cap[r]; charged_cap[r] = cap[r]; }
+          if ((E.templates[v].limit_present >> r) & 1 && (present >> r) & 1) {
+            E.templates[v].remaining[r] = remaining_minus(E.templates[v].remaining[r], cap[r]);
+            E.remaining_exact[(size_t)v * KSCHED_MAX_RES + r] -= cap[r];
+            charged_cap[r] = cap[r];
+          }
         charged = v;
       }
     if (B.superset) {

@@ -48,6 +48,8 @@ struct Encoded {
   std::vector<int> existing_state_index;              // existing slot -> Problem.nodes index
   std::vector<int32_t> pod_node;                      // cluster_superset: existing slot a batch pod is bound to, -1 = pending
   std::vector<int64_t> existing_capacity;             // cluster_superset: [n_existing][KSCHED_MAX_RES] node capacity (limits bookkeeping)
+  std::vector<__int128> remaining_exact;              // [n_templates][KSCHED_MAX_RES] limits minus every charged node's capacity,
+                                                      // exact; templates[v].remaining holds it at remaining_minus's floor
   std::vector<int32_t> existing_template;
   // cluster_superset with topology groups: what a bound pod that stays contributes to the counters (ksched.h: ksched_cluster)
   std::vector<uint32_t> class_count_begin;

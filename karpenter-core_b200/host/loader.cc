@@ -13,7 +13,8 @@ namespace kmodel {
 
 // resource.MustParse restated for the suffixes the reference uses. Exact: the result
 // must be a whole number of milli-units, otherwise the quantity is rejected
-// (SURVEY.md 7-H6).
+// (SURVEY.md 7-H6). |milli| must stay below kQuantityBound = 2^62 (DESIGN §2): sums of two
+// admitted values then never wrap int64, and the device's sort key adds 2^62.
 int64_t parse_quantity_milli(const std::string& s) {
   if (s.empty()) throw std::runtime_error("empty quantity");
   size_t i = 0;
@@ -27,6 +28,11 @@ int64_t parse_quantity_milli(const std::string& s) {
     if (c >= '0' && c <= '9') {
       mant = mant * 10 + (c - '0');
       if (seen_dot) ++frac_digits;
+      // mant * (suffix multiplier < 2^61) and 10^frac_digits must stay exact in __int128, so mantissas of 21 or more
+      // digits (leading zeros aside) and more than 30 fractional digits are refused; an admitted value has at most 19
+      // digits of milli-units
+      if (mant >= (__int128)100000000000LL * 1000000000LL || frac_digits > 30)
+        throw std::runtime_error("quantity has too many digits: " + s);
       any = true;
     } else if (c == '.' && !seen_dot) {
       seen_dot = true;
@@ -55,7 +61,7 @@ int64_t parse_quantity_milli(const std::string& s) {
   __int128 num = mant * mul;
   if (num % div != 0) throw std::runtime_error("sub-milli quantity rejected: " + s);
   __int128 v = num / div;
-  if (v > (__int128)INT64_MAX) throw std::runtime_error("quantity overflow: " + s);
+  if (v >= (__int128)kQuantityBound) throw std::runtime_error("quantity out of range (|milli| >= 2^62): " + s);
   int64_t r = (int64_t)v;
   return neg ? -r : r;
 }
@@ -67,9 +73,19 @@ ResourceList resources(const Value* v) {
   ResourceList r;
   if (!v || v->is_null()) return r;
   for (auto& kv : v->obj) {
-    if (kv.second.kind == Value::Str) r[kv.first] = parse_quantity_milli(kv.second.str);
-    else r[kv.first] = parse_quantity_milli(kv.second.str);  // raw number text
+    try {
+      r[kv.first] = parse_quantity_milli(kv.second.str);  // a string, or the raw text of a number
+    } catch (const std::runtime_error& e) {
+      throw std::runtime_error("resource " + kv.first + ": " + e.what());
+    }
   }
+  return r;
+}
+// Capacities charged against provisioner limits must not be negative: remaining_minus (model.h) relies on it
+ResourceList capacity(const Value* v, const std::string& owner) {
+  ResourceList r = resources(v);
+  for (auto& kv : r)
+    if (kv.second < 0) throw std::runtime_error(owner + ": negative capacity of resource " + kv.first);
   return r;
 }
 Labels labels(const Value* v) {
@@ -207,6 +223,10 @@ Container container(const Value& e) {
   Container c;
   c.requests = resources(e.get("requests"));
   c.limits = resources(e.get("limits"));
+  // the API server refuses negative requests and limits (ValidateResourceRequirements); node sums rely on it (oracle.cc)
+  for (auto* l : {&c.requests, &c.limits})
+    for (auto& kv : *l)
+      if (kv.second < 0) throw std::runtime_error("resource " + kv.first + ": negative request or limit");
   if (const Value* ports = e.get("ports"))
     for (auto& p : ports->arr) {
       HostPort hp;
@@ -301,7 +321,7 @@ Problem* problem_from_json(const char* text) {
       if (const Value* ofs = e.get("offerings"))
         for (auto& o : ofs->arr)
           it.offerings.push_back({o.s("capacityType"), o.s("zone"), o.d("price"), o.boolean("available", true)});
-      it.capacity = resources(e.get("capacity"));
+      it.capacity = capacity(e.get("capacity"), "instance type " + it.name);
       if (const Value* ov = e.get("overhead"); ov && !ov->is_null()) {
         it.kube_reserved = resources(ov->get("kubeReserved"));
         it.system_reserved = resources(ov->get("systemReserved"));
@@ -339,8 +359,8 @@ Problem* problem_from_json(const char* text) {
       n.taints = taints(e.get("taints"));
       n.startup_taints = taints(e.get("startupTaints"));
       n.allocatable = resources(e.get("allocatable"));
-      n.capacity = resources(e.get("capacity"));
-      if (n.capacity.empty()) n.capacity = n.allocatable;
+      n.capacity = capacity(e.get("capacity"), "node " + n.name);
+      if (n.capacity.empty()) n.capacity = capacity(e.get("allocatable"), "node " + n.name);
       if (const Value* ps = e.get("pods")) {
         size_t k = 0;
         for (auto& p : ps->arr) {

@@ -17,6 +17,7 @@
 #include <map>
 #include <memory>
 #include <mutex>
+#include <stdexcept>
 #include <string>
 #include <vector>
 
@@ -24,6 +25,23 @@ namespace kmodel {
 
 using ResourceList = std::map<std::string, int64_t>;  // name -> milli-units
 using Labels = std::map<std::string, std::string>;
+
+// Every quantity the loader admits, and every sum or difference of quantities the scheduler keeps, lies strictly inside
+// (-kQuantityBound, kQuantityBound) (DESIGN §2): two such values add or subtract without wrapping int64, where the
+// reference's resource.Quantity is exact at any size. A sum that leaves the range is refused, never wrapped.
+inline constexpr int64_t kQuantityBound = int64_t(1) << 62;
+inline int64_t checked_quantity(__int128 v, const std::string& name) {
+  if (v >= kQuantityBound || v <= -kQuantityBound)
+    throw std::runtime_error("resource " + name + ": a sum of quantities is out of range (|milli| >= 2^62)");
+  return (int64_t)v;
+}
+// A provisioner's remaining limit minus a node's capacity (capacities are >= 0, the loader refuses others). Within one
+// Solve a remaining limit only goes down, and once it is at or below -kQuantityBound no instance type fits it
+// (capacities are > -kQuantityBound), so holding it at that floor gives the same filterByRemainingResources answers.
+inline int64_t remaining_minus(int64_t remaining, int64_t capacity) {
+  const int64_t r = remaining - capacity;  // remaining >= -2^62, 0 <= capacity < 2^62: no wrap
+  return r < -kQuantityBound ? -kQuantityBound : r;
+}
 
 enum class Op : uint8_t { In, NotIn, Exists, DoesNotExist, Gt, Lt };
 

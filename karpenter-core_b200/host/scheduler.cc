@@ -766,15 +766,19 @@ SimBatch simulate_on(ksched_handle* h, const Encoded& E, const std::vector<std::
   std::vector<std::vector<int64_t>> rem(n);
   std::vector<ksched_candidate_set> cs(n);
   std::vector<char> removed(NE);
+  std::vector<__int128> exact;
   for (size_t q = 0; q < n; ++q) {
     std::fill(removed.begin(), removed.end(), 0);
-    rem[q].resize(V * KSCHED_MAX_RES);
-    for (size_t v = 0; v < V; ++v) for (int r = 0; r < KSCHED_MAX_RES; ++r) rem[q][v * KSCHED_MAX_RES + r] = E.templates[v].remaining[r];
+    // scheduler.go:221-248 only charges the nodes that stay: the exact remaining with the removed nodes' capacity given
+    // back, then held at remaining_minus's floor like a Solve's
+    exact = E.remaining_exact;
     for (int32_t e : slot_sets[q]) {
       removed[(size_t)e] = 1;
-      const int v = E.existing_template[(size_t)e];  // scheduler.go:221-248 only charges the nodes that stay
-      if (v >= 0) for (int r = 0; r < KSCHED_MAX_RES; ++r) rem[q][(size_t)v * KSCHED_MAX_RES + r] += E.existing_capacity[(size_t)e * KSCHED_MAX_RES + r];
+      const int v = E.existing_template[(size_t)e];
+      if (v >= 0) for (int r = 0; r < KSCHED_MAX_RES; ++r) exact[(size_t)v * KSCHED_MAX_RES + r] += E.existing_capacity[(size_t)e * KSCHED_MAX_RES + r];
     }
+    rem[q].resize(V * KSCHED_MAX_RES);
+    for (size_t i = 0; i < V * KSCHED_MAX_RES; ++i) rem[q][i] = exact[i] < -kQuantityBound ? -kQuantityBound : (int64_t)exact[i];
     for (size_t e = 0; e < NE; ++e) if (!removed[e] && !E.existing_initialized[e]) out.skip[q] = 1;
     cs[q] = ksched_candidate_set{slot_sets[q].data(), (int32_t)slot_sets[q].size(), 0, rem[q].data()};
   }

@@ -57,17 +57,25 @@ bool g_fast = false;
 void set_fast(bool on) { g_fast = on; }
 
 // ---------------------------------------------------------------- resources (utils/resources/resources.go)
+// Sums and differences are checked against kQuantityBound (model.h): out of range is refused, like the product does.
 static ResourceList merge(const ResourceList& a, const ResourceList& b) {  // :47-60
   ResourceList r = a;
-  for (auto& kv : b) r[kv.first] += kv.second;
+  for (auto& kv : b) r[kv.first] = checked_quantity((__int128)r[kv.first] + kv.second, kv.first);
   return r;
 }
 static ResourceList subtract(const ResourceList& lhs, const ResourceList& rhs) {  // :62-75
   ResourceList r = lhs;
   for (auto& kv : lhs) {
     auto it = rhs.find(kv.first);
-    if (it != rhs.end()) r[kv.first] = kv.second - it->second;
+    if (it != rhs.end()) r[kv.first] = checked_quantity((__int128)kv.second - it->second, kv.first);
   }
+  return r;
+}
+// A node's requests plus one pod's, unchecked: requests are >= 0 (the loader refuses others) and a node's requests never
+// pass an allocatable inside kQuantityBound, so the sum is below 2^63 and exact; Fits then answers as the reference does.
+static ResourceList add_requests(const ResourceList& a, const ResourceList& b) {
+  ResourceList r = a;
+  for (auto& kv : b) r[kv.first] += kv.second;
   return r;
 }
 static ResourceList max_resources(const ResourceList& a, const ResourceList& b) {  // :92-102
@@ -817,7 +825,7 @@ struct Scheduler {
           for (auto& kv : n.max_alloc) kv.second = std::max(kv.second, getq(t->allocatable, kv.first));
         n.max_alloc_valid = true;
       }
-      if (!fits(merge(n.requests, pod_requests(pi)), n.max_alloc)) return false;
+      if (!fits(add_requests(n.requests, pod_requests(pi)), n.max_alloc)) return false;
     }
     if (!tolerates(templates[n.tmpl].taints, pod)) return false;
     if (!n.ports.validate(pod)) return false;
@@ -830,7 +838,7 @@ struct Scheduler {
     if (!topology.AddRequirements(pod_req, node_req, pod, &topo_req)) return false;
     if (!node_req.Compatible(topo_req, wk)) return false;
     node_req.AddAll(topo_req);
-    ResourceList requests = merge(n.requests, pod_requests(pi));
+    ResourceList requests = add_requests(n.requests, pod_requests(pi));
     auto types = filter_types(n.options, node_req, requests);
     if (types.empty()) return false;
     n.pods.push_back(pi);
@@ -847,7 +855,7 @@ struct Scheduler {
     if (!tolerates(n.taints, pod)) return false;
     if (!n.ports.validate(pod)) return false;
     if (n.volumes.exceeds(pod, n.volume_limits)) return false;  // :88-96
-    ResourceList requests = merge(n.requests, requests_for_pod(pod));
+    ResourceList requests = add_requests(n.requests, requests_for_pod(pod));
     if (!fits(requests, n.available)) return false;
     Requirements node_req;
     node_req.AddAll(n.req);
@@ -1049,7 +1057,10 @@ struct Scheduler {
       auto pit = std::find_if(templates.begin(), templates.end(), [&](const MachineTemplate& m) { return m.name == own->second; });
       if (pit != templates.end() && has_remaining[pit - templates.begin()]) {
         size_t v = pit - templates.begin();
-        remaining[v] = subtract(remaining[v], n.capacity);
+        for (auto& kv : remaining[v]) {  // resources.Subtract over the limits' keys, held at remaining_minus's floor
+          auto c = n.capacity.find(kv.first);
+          if (c != n.capacity.end()) kv.second = remaining_minus(kv.second, c->second);
+        }
       }
     }
   }
@@ -1243,7 +1254,8 @@ void rank_candidates(const Problem& P, std::vector<int>* order, std::vector<doub
     if (blocked) continue;
     cands.push_back({(int)i, cost});
   }
-  std::stable_sort(cands.begin(), cands.end(), [](const C& a, const C& b) { return a.cost < b.cost; });
+  // R8: a NaN cost (a "NaN" deletion-cost annotation, a TTL of 0 at age 0) sorts after every number, stable among NaNs
+  std::stable_sort(cands.begin(), cands.end(), [](const C& a, const C& b) { return !std::isnan(a.cost) && (std::isnan(b.cost) || a.cost < b.cost); });
   order->clear();
   if (cost_out) cost_out->clear();
   for (auto& c : cands) { order->push_back(c.node); if (cost_out) cost_out->push_back(c.cost); }

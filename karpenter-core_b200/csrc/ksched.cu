@@ -46,7 +46,6 @@ using ksched::Req;
 namespace {
 
 constexpr int kMaxCG = 8;        // topology groups that may constrain one pod class
-constexpr int kMaxTouched = 8;   // requirement keys one Add may touch (pod keys + topology keys)
 constexpr int kPackThreads = 512;
 constexpr int kPackThreadsSmall = 256;  // blocks up to this size launch the pack_kernel instantiation with twice the registers
 constexpr int kFreshMemoSlots = 8192;  // PackState::fd_*
@@ -866,10 +865,10 @@ static int check_problem(ksched_handle* h, const ksched_problem* pb) {
     const ksched_pod_row& row = pb->classes[c];
     if (row.relax_next != KSCHED_NONE && row.relax_next >= (uint32_t)NC) { h->err = "relax_next out of range"; return KSCHED_ERR_INVALID; }
     if (row.topo_end < row.topo_begin || row.topo_end > (uint32_t)pb->n_class_topo) { h->err = "class_topo range out of bounds"; return KSCHED_ERR_INVALID; }
-    int ncg = 0, touched = __builtin_popcountll((row.meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF);
+    int ncg = 0;
     for (uint32_t e = row.topo_begin; e < row.topo_end; ++e)
-      if (pb->class_topo[e].flags & KSCHED_TOPO_CONSTRAINS) { ++ncg; if (pb->groups[pb->class_topo[e].group].key != KSCHED_KEY_HOSTNAME) ++touched; }
-    if (ncg > kMaxCG || touched > kMaxTouched) { h->err = "a pod class is constrained by more topology groups / label keys than the pack kernel carries"; return KSCHED_ERR_UNSUPPORTED; }
+      if (pb->class_topo[e].flags & KSCHED_TOPO_CONSTRAINS) ++ncg;
+    if (ncg > kMaxCG) { h->err = "a pod class is constrained by more topology groups than the pack kernel carries"; return KSCHED_ERR_UNSUPPORTED; }
   }
   for (int g = 0; g < NG; ++g)
     if (pb->groups[g].key != KSCHED_KEY_HOSTNAME && pb->groups[g].key >= h->cat.n_keys) { h->err = "topology group key out of range"; return KSCHED_ERR_INVALID; }

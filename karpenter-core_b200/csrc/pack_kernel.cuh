@@ -327,12 +327,12 @@ __device__ __noinline__ bool evaluate_slow(bool plain,
   KS_ROW
   const int MAXN = s.max_new, NE = s.n_existing, R = c.n_res, W32 = c.W32;
   const uint32_t p_res = row.res_present, p_ext = kExt ? class_ext(s, (unsigned)row.reserved) : 0u;
-  t.n = 0;
+  t.clear();
   e.changed = false;
   bool need_types = !(fl & 1) || row.itype_req != KSCHED_NONE || p_ext;
   if (!plain) {
     if (!requirements_phase(s.nn_vals, s.nn_meta[n], MAXN, n, NE + n, false, t)) return false;
-    for (int i = 0; i < t.n; ++i) e.changed = e.changed || t.changed[i];
+    e.changed = t.changed != 0;
     need_types = need_types || e.changed;
   }
   for (int r = 0; r < kHotRes; ++r) e.q[r] = q_hot[r];
@@ -350,22 +350,19 @@ __device__ __noinline__ bool evaluate_slow(bool plain,
   }
   return false;
 }
-// Requirement part of a commit: the node's new masks.
+// Requirement part of a commit into a node's requirement set (SoA vals / meta, column idx): its new masks.
+__device__ __forceinline__ uint64_t commit_touched(const Touched& t, uint64_t* vals, uint64_t* metas, int stride, int idx) {
+  for (uint32_t m = t.keys; m; m &= m - 1) {
+    const int k = __ffs(m) - 1;
+    vals[(size_t)k * stride + idx] = t.fin[k];
+  }
+  const uint64_t meta = t.overlay_meta(metas[idx]);
+  metas[idx] = meta;
+  return meta;
+}
 __device__ __forceinline__ uint64_t commit_reqs(int n, const Touched& t) {
   KS_K2
-  const int MAXN = s.max_new;
-  uint64_t meta = s.nn_meta[n];
-  for (int i = 0; i < t.n; ++i) {
-    const int k = t.key[i];
-    const Req& f = t.fin[i];
-    const uint64_t bit = 1ull << k;
-    meta &= ~((bit << KSCHED_META_PRESENT_SHIFT) | (bit << KSCHED_META_COMPLEMENT_SHIFT));
-    if (f.present) meta |= bit << KSCHED_META_PRESENT_SHIFT;
-    if (f.present && f.complement) meta |= bit << KSCHED_META_COMPLEMENT_SHIFT;
-    s.nn_vals[(size_t)k * MAXN + n] = f.values;
-  }
-  s.nn_meta[n] = meta;
-  return meta;
+  return commit_touched(t, s.nn_vals, s.nn_meta, s.max_new, n);
 }
 // Requirement-changing commit done by ONE thread (fallback mode): new masks, requirement-driven narrowing of the stored
 // options, new bounds.
@@ -680,7 +677,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
       const int start = s.cls_cursor[cls];
       unsigned mine = ~0u, soft = ~0u;  // first node this thread accepts / first node it did not refuse for good
       Touched t;
-      t.n = 0;
+      t.clear();
       for (int e = start + tid; e < NE; e += blockDim.x) {
         if (s.ex_closed[e]) continue;
         if (!tolerates_node_set(s, p_tol, cls, s.ex_taintset[e])) continue;
@@ -717,19 +714,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
         const int e = (int)w;
         nodes_visited += e + 1;
         if (mine == w32) {  // the winning thread commits its own candidate
-          uint64_t meta = s.ex_meta[e];
-          if (!plain) {
-            for (int i = 0; i < t.n; ++i) {
-              const int k = t.key[i];
-              const Req& f = t.fin[i];
-              const uint64_t bit = 1ull << k;
-              meta &= ~((bit << KSCHED_META_PRESENT_SHIFT) | (bit << KSCHED_META_COMPLEMENT_SHIFT));
-              if (f.present) meta |= bit << KSCHED_META_PRESENT_SHIFT;
-              if (f.present && f.complement) meta |= bit << KSCHED_META_COMPLEMENT_SHIFT;
-              s.ex_vals[(size_t)k * NE + e] = f.values;
-            }
-            s.ex_meta[e] = meta;
-          }
+          if (!plain) commit_touched(t, s.ex_vals, s.ex_meta, NE, e);
           bool closed = false;
           for (int r = 0; r < R; ++r) {
             if ((p_res >> r) & 1) s.ex_req[(size_t)r * NE + e] += row.requests[r];
@@ -995,23 +980,14 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
           else if (st == 2) path = kPathCachedEmpty;
           else {
             bool ok = (p_tol >> tm.taintset) & 1;
-            fresh_t.n = 0;
+            fresh_t.clear();
             if (ok && !plain) ok = requirements_phase(tm.reqs.values, tm.reqs.meta & 0xFFFFFFFFull, 1, 0, NE + n, false, fresh_t);
             if (ok) {
               sh.qp = tm.daemon_res_present | p_res;
               for (int r = 0; r < KSCHED_MAX_RES; ++r) sh.q[r] = r < R ? tm.daemon_requests[r] + (((p_res >> r) & 1) ? row.requests[r] : 0) : 0;
-              bool same = f_valid;  // topology left every requirement exactly as K1 saw it
-              for (int i = 0; i < fresh_t.n && same; ++i) same = req_equal(fresh_t.fin[i], fresh_t.merged[i]);
+              const bool same = f_valid && fresh_t.fin_is_merged();  // topology left every requirement exactly as K1 saw it
               // the new node's requirement set: the template's, overlaid by what this Add touched
-              uint64_t meta = tm.reqs.meta & 0xFFFFFFFFull;
-              for (int i = 0; i < fresh_t.n; ++i) {
-                const int k = fresh_t.key[i];
-                const Req& f = fresh_t.fin[i];
-                const uint64_t bit = 1ull << k;
-                meta &= ~((bit << KSCHED_META_PRESENT_SHIFT) | (bit << KSCHED_META_COMPLEMENT_SHIFT));
-                if (f.present) meta |= bit << KSCHED_META_PRESENT_SHIFT;
-                if (f.present && f.complement) meta |= bit << KSCHED_META_COMPLEMENT_SHIFT;
-              }
+              const uint64_t meta = fresh_t.overlay_meta(tm.reqs.meta & 0xFFFFFFFFull);
               sh.meta = meta;
               sh.fd_slot = -1;
               if (same) path = kPathRow;
@@ -1021,8 +997,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
                   uint64_t vals[KSCHED_MAX_KEYS];
                   uint64_t hsh = ((uint64_t)fc + 1) * 0x9E3779B97F4A7C15ull ^ meta;
                   for (int k = 0; k < c.n_keys; ++k) {
-                    uint64_t val = tm.reqs.values[k];
-                    for (int i = 0; i < fresh_t.n; ++i) if (fresh_t.key[i] == k) val = fresh_t.fin[i].values;
+                    const uint64_t val = ((fresh_t.keys >> k) & 1) ? fresh_t.fin[k] : tm.reqs.values[k];
                     vals[k] = val;
                     hsh = (hsh ^ val) * 0xBF58476D1CE4E5B9ull;
                     hsh ^= hsh >> 29;
@@ -1085,8 +1060,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
           }
           if (local_any) atomicOr(&sh.any, 1u);
           if (tid < c.n_keys) {
-            uint64_t val = tm.reqs.values[tid];
-            for (int i = 0; i < fresh_t.n; ++i) if (fresh_t.key[i] == tid) val = fresh_t.fin[i].values;
+            const uint64_t val = ((fresh_t.keys >> tid) & 1) ? fresh_t.fin[tid] : tm.reqs.values[tid];
             s.nn_vals[(size_t)tid * MAXN + n] = val;
             if (memo) s.fc_vals[fc * KSCHED_MAX_KEYS + tid] = val;
           }

@@ -174,13 +174,47 @@ struct K2Params {
 __constant__ K2Params g_k2;
 #define KS_K2 const DevCatalog& c = g_k2.cat; const PackState& s = g_k2.st; (void)c; (void)s;
 
+// The requirement keys one Add touched: the pod's keys and the keys of its constraining topology groups, at most the 16 mask
+// keys, with one slot per key. Device requirements never carry gt / lt (region form), so a slot is its value word and the
+// present / complement / changed bits are masks over keys.
 struct Touched {
-  int n;
-  int8_t key[kMaxTouched];
-  Req merged[kMaxTouched];  // node ∩ pod          (node.go:81)
-  Req fin[kMaxTouched];     // ... ∩ topology      (node.go:90)
-  bool changed[kMaxTouched];
+  uint16_t keys;               // touched keys
+  uint16_t changed;            // touched keys whose final requirement differs from the node's
+  uint16_t m_present, m_comp;  // merged: node ∩ pod          (node.go:81)
+  uint16_t f_present, f_comp;  // fin:    ... ∩ topology      (node.go:90)
+  uint64_t merged[KSCHED_MAX_KEYS];
+  uint64_t fin[KSCHED_MAX_KEYS];
+
+  __device__ __forceinline__ void clear() { keys = changed = m_present = m_comp = f_present = f_comp = 0; }
+  __device__ __forceinline__ static Req req_of(uint64_t v, uint16_t present, uint16_t comp, int k) {
+    Req r;
+    r.present = (present >> k) & 1;
+    r.complement = (comp >> k) & 1;
+    r.has_gt = r.has_lt = false;
+    r.gt = r.lt = 0;
+    r.values = v;
+    return r;
+  }
+  __device__ __forceinline__ static void set_bit(uint16_t& m, int k, bool on) {
+    m = on ? (uint16_t)(m | (1u << k)) : (uint16_t)(m & ~(1u << k));
+  }
+  __device__ __forceinline__ Req merged_req(int k) const { return req_of(merged[k], m_present, m_comp, k); }
+  __device__ __forceinline__ Req fin_req(int k) const { return req_of(fin[k], f_present, f_comp, k); }
+  __device__ __forceinline__ void set_merged(int k, const Req& r) { merged[k] = r.values; set_bit(m_present, k, r.present); set_bit(m_comp, k, r.complement); }
+  __device__ __forceinline__ void set_fin(int k, const Req& r) { fin[k] = r.values; set_bit(f_present, k, r.present); set_bit(f_comp, k, r.complement); }
+  // every touched key's final requirement equals its merged one: topology narrowed nothing
+  __device__ __forceinline__ bool fin_is_merged() const {
+    if ((f_present ^ m_present) | (f_comp ^ m_comp)) return false;
+    for (uint32_t m = keys; m; m &= m - 1) if (fin[__ffs(m) - 1] != merged[__ffs(m) - 1]) return false;
+    return true;
+  }
+  // a requirement set's meta word with the touched keys' final present / complement bits
+  __device__ __forceinline__ uint64_t overlay_meta(uint64_t meta) const {
+    meta &= ~(((uint64_t)keys << KSCHED_META_PRESENT_SHIFT) | ((uint64_t)keys << KSCHED_META_COMPLEMENT_SHIFT));
+    return meta | ((uint64_t)f_present << KSCHED_META_PRESENT_SHIFT) | ((uint64_t)(f_present & f_comp) << KSCHED_META_COMPLEMENT_SHIFT);
+  }
 };
+static_assert(KSCHED_MAX_KEYS <= 16, "Touched keeps its key masks in 16 bits");
 
 struct PodTopo {  // per (pod step, constraining group): node-independent part of TopologyGroup.Get
   int n;
@@ -329,54 +363,47 @@ __device__ __noinline__ bool hostname_affinity_options(int gi, int host_row, uin
 __device__ __noinline__ bool requirements_phase(const uint64_t* vals, uint64_t meta, int stride, int idx, int slot, bool is_existing, Touched& t) {
   KS_K2
   KS_ROW KS_PT
-  t.n = 0;
+  t.clear();
   if (!hostname_allows(s, row, slot, is_existing)) return false;
-  uint32_t podkeys = (uint32_t)(row.meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF;
-  while (podkeys) {
-    int k = __ffs(podkeys) - 1;
-    podkeys &= podkeys - 1;
+  const uint32_t podkeys = (uint32_t)(row.meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF;
+  for (uint32_t m = podkeys; m; m &= m - 1) {
+    const int k = __ffs(m) - 1;
     Req node = load_soa(vals, meta, stride, idx, k);
     Req pod = pod_req(row, k);
     KeyMeta km = key_meta(c, k);
     if (!ksched::key_compatible(node, pod, c.keys[k].well_known != 0, km)) return false;
-    if (t.n >= kMaxTouched) return false;
     Req merged = ksched::key_add(node, pod, km);
-    t.key[t.n] = (int8_t)k;
-    t.merged[t.n] = merged;
-    t.fin[t.n] = merged;
-    t.changed[t.n] = !req_equal(merged, node);
-    ++t.n;
+    t.set_merged(k, merged);
+    t.set_fin(k, merged);
+    if (!req_equal(merged, node)) t.changed |= (uint16_t)(1u << k);
   }
+  t.keys = (uint16_t)podkeys;
   for (int j = 0; j < pt.n; ++j) {
     if (pt.gkey[j] == KSCHED_KEY_HOSTNAME) {
       if (!topo_hostname_ok(j, slot, hostname_allows(s, row, slot, is_existing))) return false;
       continue;
     }
     const int k = pt.gkey[j];
-    int ti = -1;
-    for (int i = 0; i < t.n; ++i) if (t.key[i] == k) ti = i;
-    if (ti < 0) {
-      if (t.n >= kMaxTouched) return false;
-      ti = t.n++;
+    if (!((t.keys >> k) & 1)) {
+      t.keys |= (uint16_t)(1u << k);
       Req node = load_soa(vals, meta, stride, idx, k);
-      t.key[ti] = (int8_t)k;
-      t.merged[ti] = node;
-      t.fin[ti] = node;
-      t.changed[ti] = false;
+      t.set_merged(k, node);
+      t.set_fin(k, node);
     }
     uint64_t dom;
-    if (!topo_domains_mask(j, t.merged[ti], &dom)) return false;
+    if (!topo_domains_mask(j, t.merged_req(k), &dom)) return false;
     Req d{dom, 0, 0, true, false, false, false};
     KeyMeta km = key_meta(c, k);
-    t.fin[ti] = ksched::key_add(t.fin[ti], d, km);  // requirements.Add(domains) topology.go:164
+    t.set_fin(k, ksched::key_add(t.fin_req(k), d, km));  // requirements.Add(domains) topology.go:164
   }
   // nodeRequirements.Compatible(topologyRequirements) node.go:87 — only topology keys can differ
-  for (int i = 0; i < t.n; ++i) {
-    if (req_equal(t.fin[i], t.merged[i])) continue;
-    const int k = t.key[i];
-    if (!ksched::key_compatible(t.merged[i], t.fin[i], c.keys[k].well_known != 0, key_meta(c, k))) return false;
-    t.fin[i] = ksched::key_add(t.merged[i], t.fin[i], key_meta(c, k));
-    t.changed[i] = true;
+  for (uint32_t m = t.keys; m; m &= m - 1) {
+    const int k = __ffs(m) - 1;
+    const Req merged = t.merged_req(k), fin = t.fin_req(k);
+    if (req_equal(fin, merged)) continue;
+    if (!ksched::key_compatible(merged, fin, c.keys[k].well_known != 0, key_meta(c, k))) return false;
+    t.set_fin(k, ksched::key_add(merged, fin, key_meta(c, k)));
+    t.changed |= (uint16_t)(1u << k);
   }
   return true;
 }
@@ -414,27 +441,22 @@ __device__ __noinline__ void build_type_ctx(const Touched& t, const long long* q
   };
   if (fresh) {
     // every key of the new node's requirement set is evaluated from scratch
-    uint32_t done = 0;
-    for (int i = 0; i < t.n; ++i) { add_key(t.key[i], t.fin[i]); done |= 1u << t.key[i]; }
-    uint32_t rest = ((uint32_t)(meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF) & ~done;
-    while (rest) {
-      int k = __ffs(rest) - 1;
-      rest &= rest - 1;
-      add_key(k, load_soa(vals, meta, stride, idx, k));
+    for (uint32_t m = t.keys | ((uint32_t)(meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF); m; m &= m - 1) {
+      const int k = __ffs(m) - 1;
+      add_key(k, ((t.keys >> k) & 1) ? t.fin_req(k) : load_soa(vals, meta, stride, idx, k));
     }
   } else {
-    for (int i = 0; i < t.n; ++i) {
-      if (!t.changed[i]) continue;
-      add_key(t.key[i], t.fin[i]);
-      if (t.key[i] == c.zone_key || t.key[i] == c.ct_key) x.offer_needed = true;
+    for (uint32_t m = t.changed; m; m &= m - 1) {
+      const int k = __ffs(m) - 1;
+      add_key(k, t.fin_req(k));
+      if (k == c.zone_key || k == c.ct_key) x.offer_needed = true;
     }
   }
   x.slots = ~0ull; x.offer_unconstrained = true;
   if (x.offer_needed) {
     uint64_t zallowed = ~0ull, callowed = ~0ull;
     auto final_req = [&](int k) -> Req {
-      for (int i = 0; i < t.n; ++i) if (t.key[i] == k) return t.fin[i];
-      return load_soa(vals, meta, stride, idx, k);
+      return ((t.keys >> k) & 1) ? t.fin_req(k) : load_soa(vals, meta, stride, idx, k);
     };
     if (c.zone_key >= 0) {
       Req z = final_req(c.zone_key);

@@ -122,6 +122,14 @@ int kh_consolidate_single_validated(const kh_problem* before, const kh_problem* 
  * fit. */
 int kh_encoded_volume_claim(const void* enc, int id, char* out, int cap);
 
+/* ---- K1's paths (tests). kh_encoded_class_row: the 32 u64 words of class c's ksched_pod_row in out[32]; -1 out of range.
+ * kh_gpu_k1_plan: the process handle's last K1 class pass as out[5] = {blocks, class rows per warp, consecutive-row cache
+ * on, sorted allocatable arrays staged in shared memory, column tables staged in shared memory}. kh_gpu_set_shard: the
+ * column shard of the process handle (ksched_set_shard); (0, 1) computes every column. */
+int kh_encoded_class_row(const void* enc, int c, uint64_t* out);
+int kh_gpu_k1_plan(int* out);
+int kh_gpu_set_shard(int rank, int world);
+
 /* ---- self-test of the encoder's value classes (CPU, no device): random wide keys and requirement pairs, the exact string
  * algebra against the collapsed masks (host form and region form). Returns the number of mismatches. */
 int kh_value_class_selftest(unsigned seed, int iters);

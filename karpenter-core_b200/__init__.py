@@ -147,6 +147,9 @@ def lib():
     L.kh_gpu_timings.argtypes = [C.POINTER(Timings)]
     L.kh_gpu_solve_e2e.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_double)]
     L.kh_gpu_load_catalog.argtypes = [C.c_void_p]
+    L.kh_encoded_class_row.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+    L.kh_gpu_k1_plan.argtypes = [C.POINTER(C.c_int)]
+    L.kh_gpu_set_shard.argtypes = [C.c_int, C.c_int]
     L.kh_consolidate.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int,
                                  C.POINTER(C.c_int)]
     L.kh_consolidate_candidates.argtypes = [C.c_void_p]
@@ -194,6 +197,12 @@ def shard_range(n_words32, rank, world):
     if rc != KSCHED_OK:
         raise KschedError(rc, "ksched_shard_range")
     return b.value, e.value
+
+
+def set_shard(rank, world):
+    """column shard of the process handle (ksched_set_shard): K1 computes only `rank`'s words of F and the pack kernel
+    evaluates fresh nodes without F. (0, 1) computes every column."""
+    _check(lib().kh_gpu_set_shard(rank, world))
 
 
 def _check(rc):
@@ -645,6 +654,21 @@ class ResidentSolve:
         if lib().kh_encoded_key_info(self.enc, key.encode(), out) != 0:
             return None
         return dict(zip(["values", "representatives", "thresholds"], list(out)))
+
+    def class_row(self, c):
+        """the 32 u64 words of class c's pod row as the device receives it (include/ksched.h: ksched_pod_row)"""
+        out = np.zeros(32, dtype=np.uint64)
+        if lib().kh_encoded_class_row(self.enc, c, out.ctypes.data) != 0:
+            raise IndexError(c)
+        return out
+
+    @staticmethod
+    def k1_plan():
+        """the process handle's last K1 class pass: {blocks, chunk (class rows per warp), cacheable, alloc_in_smem,
+        tables_in_smem}"""
+        out = (C.c_int * 5)()
+        _check(lib().kh_gpu_k1_plan(out))
+        return dict(zip(["blocks", "chunk", "cacheable", "alloc_in_smem", "tables_in_smem"], list(out)))
 
     def resource_id(self, name):
         """id of a resource in this encoding: a row slot below 8, an ext resource from 8 on; -1 when it is not carried"""

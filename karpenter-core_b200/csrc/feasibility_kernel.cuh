@@ -167,6 +167,11 @@ __device__ __noinline__ unsigned long long k1_compute_row(int j, uint64_t word, 
 constexpr int kK1Threads = 512;
 constexpr int kK1Cache = 16;  // per-lane words of the previous row's result kept for identical consecutive rows
 
+// The class pass's work split and cache rule, shared by the kernel and the host's record of its launch (ksched_k1_plan):
+// each warp owns a contiguous chunk of rows, and the consecutive-row cache holds V * wpl words per lane.
+__host__ __device__ constexpr int k1_chunk(int n_rows, int n_warps) { return (n_rows + n_warps - 1) / n_warps; }
+__host__ __device__ constexpr bool k1_cacheable(int n_templates, int W32) { return n_templates * ((W32 + 31) >> 5) <= kK1Cache; }
+
 struct K1Params;
 
 // class_feasibility_kernel: the row evaluation, run over the n_classes DISTINCT pod rows (K1Params::rows = the class table):
@@ -249,10 +254,10 @@ __global__ void __launch_bounds__(kK1Threads, 1) class_feasibility_kernel() {
   const int lane = threadIdx.x & 31;
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  const int chunk = (p.n_pods + nwarps - 1) / nwarps;
+  const int chunk = k1_chunk(p.n_pods, nwarps);
   const int j0 = warp * chunk, j1 = min(p.n_pods, j0 + chunk);
   const int wpl = (W32 + 31) >> 5;  // column words per lane
-  const bool cacheable = V * wpl <= kK1Cache;
+  const bool cacheable = k1_cacheable(V, W32);
   // fields of the row that feasibility depends on (requests, requirement masks, meta, tolerations, res_present, itype_req)
   // With ext resources the class index (word 31) as well: two classes may differ in an ext request only.
   const uint64_t cmp_mask = lane <= 25 ? ~0ull : ((lane == 28 || lane == 29) ? 0xFFFFFFFFull : ((lane == 31 && p.cls_ext_present) ? ~0ull : 0ull));

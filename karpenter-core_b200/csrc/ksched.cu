@@ -185,6 +185,7 @@ struct ResetTable { int n; ResetSeg seg[30]; };
 struct ksched_handle {
   K1Params k1_host;  // staging copies of the kernels' constant-memory parameters (must outlive the async copies)
   K2Params k2_host;  // staging copy of the pack kernel's constant-memory parameters (must outlive the async copy)
+  int k1_plan[5] = {};  // last class pass: blocks, rows per warp, cacheable, alloc_in_smem, tables_in_smem (tests)
   int device = 0;
   int n_sm = 132;  // streaming multiprocessors of `device` (grid sizes of the grid-stride kernels)
   cudaStream_t stream = nullptr;
@@ -1261,6 +1262,11 @@ static int run_class_feasibility(ksched_handle* h, int P) {
   // one warp per class row (a row evaluation is thousands of cycles of dependent work: no chunking)
   const int warps_per_block = kK1Threads / 32;
   const int blocks = std::max(1, std::min(h->n_sm * 2, (NC + warps_per_block - 1) / warps_per_block));
+  {  // the launch as class_feasibility_kernel sees it (the same k1_chunk / k1_cacheable it calls), kept for ksched_k1_plan
+    const int plan[5] = {blocks, k1_chunk(NC, blocks * warps_per_block), k1_cacheable(c.n_templates, c.W32) ? 1 : 0, k1.alloc_in_smem,
+                         k1.tables_in_smem};
+    std::copy(plan, plan + 5, h->k1_plan);
+  }
   k1.dbg = nullptr;
 #ifdef KSCHED_PROFILE_K1
   CUDA_TRY(h, h->d_k1dbg.ensure(8));
@@ -1837,3 +1843,10 @@ int ksched_get_timings(const ksched_handle* h, ksched_timings* out) {
 }
 
 }  // extern "C"
+
+// The launch plan of the handle's last K1 class pass (host layer: kh_gpu_k1_plan). Not part of the C-ABI.
+int ksched_k1_plan(const ksched_handle* h, int out[5]) {
+  if (!h || !out) return KSCHED_ERR_INVALID;
+  std::copy(h->k1_plan, h->k1_plan + 5, out);
+  return KSCHED_OK;
+}

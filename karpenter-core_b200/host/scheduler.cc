@@ -45,6 +45,11 @@ void handle_taken() {
   g_resident_session = 0;
   g_gpu_current = false;
 }
+}  // namespace
+
+int ksched_k1_plan(const ksched_handle* h, int out[5]);  // csrc/ksched.cu, outside the C-ABI
+
+namespace {
 int g_count_visited = 0;  // exact nodes_visited statistic (opt-in: tests); switches the pack kernel's steady-state paths off
 
 int fail(int code, const std::string& msg) {
@@ -447,6 +452,12 @@ long long kh_encoded_class_hostname(const Encoded* E, int c) {
   if (c < 0 || (size_t)c >= E->classes.size() || E->classes[(size_t)c].hostname_req == KSCHED_NONE) return -1;
   return E->classes[(size_t)c].hostname_req;
 }
+// the 32 words of class c's row as the device receives it (tests); -1 out of range
+int kh_encoded_class_row(const Encoded* E, int c, uint64_t* out) {
+  if (c < 0 || (size_t)c >= E->classes.size()) return -1;
+  std::memcpy(out, &E->classes[(size_t)c], sizeof(ksched_pod_row));
+  return 0;
+}
 void kh_encoded_set_count_visited(Encoded* E, int on) { E->problem.count_nodes_visited = on; }
 const ksched_catalog* kh_encoded_catalog(const Encoded* E) { return &E->catalog; }
 const ksched_problem* kh_encoded_problem(const Encoded* E) { return &E->problem; }
@@ -538,6 +549,13 @@ int kh_gpu_load_catalog(Encoded* E) {
   return KSCHED_OK;
 }
 int kh_gpu_timings(ksched_timings* t) { return g_handle ? ksched_get_timings(g_handle, t) : KSCHED_ERR_INVALID; }
+int kh_gpu_k1_plan(int* out) { return g_handle ? ksched_k1_plan(g_handle, out) : fail(KSCHED_ERR_INVALID, "no handle"); }
+int kh_gpu_set_shard(int rank, int world) {
+  int rc = ensure_handle();
+  if (rc != KSCHED_OK) return rc;
+  rc = ksched_set_shard(g_handle, rank, world);
+  return rc == KSCHED_OK ? rc : fail(rc, "ksched_set_shard: invalid rank / world");
+}
 
 }  // extern "C"
 

@@ -5,6 +5,7 @@ the cluster after the TTL."""
 import pytest
 
 import extended_resource_problems as xp
+import k1_problems as kp
 import validation_oracle as vo
 from oracle_compare import MODE_SWITCHES, compare, set_modes
 
@@ -83,7 +84,8 @@ def test_gpu_cluster_validation_equals_oracle(pkg, oracle):
 
 def test_neighbouring_classes_that_differ_in_an_ext_amount(pkg, oracle):
     """more classes than K1 has warps: one warp evaluates both classes of a pair back to back (extended_resource_problems.pairs)"""
+    k1_warps = kp.max_warps(kp.device_sm_count())
     prob = xp.pairs()
     rs = pkg.ResidentSolve(pkg.Problem.from_dict(prob))
-    assert rs.dims["classes"] == len(prob["pods"]) > 132 * 2 * 16 and rs.resource_id("aws.amazon.com/neuron") >= 8
+    assert rs.dims["classes"] == len(prob["pods"]) > k1_warps and rs.resource_id("aws.amazon.com/neuron") >= 8
     compare(pkg, oracle, pkg.Problem.from_dict(prob), refusal_skips=False)

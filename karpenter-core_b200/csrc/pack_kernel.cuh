@@ -4,8 +4,8 @@
 //  * one CTA (128..512 threads), four modes: the failure memo (pods of the class that has just failed are requeued in
 //    one step), the class run over the shared-memory window of open nodes (consecutive pods of one class whose accept
 //    test is exact there; class_run), the existing-node run (identical plain pods fill the existing nodes in one
-//    prefix-sum pass; existing_run), and the out-of-line generic step (existing nodes, requirement / topology
-//    evaluation, fresh nodes, relaxation);
+//    prefix-sum pass; existing_run), and the out-of-line generic step (staging: gen_stage, existing nodes,
+//    requirement / topology evaluation, fresh nodes, relaxation: gen_requeue);
 //  * candidate nodes are examined one per thread and the reference's scan order is recovered by an argmin over
 //    (pod count, stable tie-break) = the position under sort.Slice(newNodes, len(Pods)<) treated as a stable sort;
 //  * the state every candidate check needs (order key, request vector, Pareto front of the allocatable vectors of the
@@ -498,6 +498,46 @@ __device__ __forceinline__ void fresh_node_hp(const PackState& s, uint64_t hpe, 
   for (int w = 0; w < s.hp_ext_words; ++w)
     s.nn_hp_ext[(size_t)w * s.max_new + n] = hpx ? s.cls_hpe_ext[(size_t)cls * s.hp_ext_words + w] : 0;
 }
+// The scalar global state of new node n, opened from template v: requirement meta, template, request keys, host-port
+// entries, instance-type slot state and, when `count` is set, the pod count and tie-break of its first pod. The class runs
+// open nodes with hpe = 0, hpx = false and itype = KSCHED_NONE.
+__device__ __forceinline__ void open_node(const PackState& s, int n, int v, uint64_t meta, uint32_t qp, uint64_t hpe, bool hpx, unsigned cls,
+                                          uint32_t itype, bool count, int tb) {
+  s.nn_meta[n] = meta;
+  s.nn_tmpl[n] = (uint8_t)v;
+  s.nn_req_present[n] = qp;
+  fresh_node_hp(s, hpe, hpx, cls, n);
+  if (s.nn_it) itype_state_open(n, v, itype);
+  if (count) {
+    s.nn_count[n] = 1;
+    s.nn_tb[n] = tb;
+  }
+}
+// Ext sums of one node, resource x at sums[x * stride], against / plus the class's ext requests creq (ext bits p_ext)
+__device__ __forceinline__ bool ext_fits(const int64_t* sums, const int64_t* avail, size_t stride, const int64_t* creq, uint32_t p_ext) {
+  for (uint32_t m = p_ext; m; m &= m - 1) {
+    const int x = __ffs(m) - 1;
+    if (sums[x * stride] + creq[x] > avail[x * stride]) return false;
+  }
+  return true;
+}
+__device__ __forceinline__ void ext_add(int64_t* sums, size_t stride, const int64_t* creq, uint32_t p_ext) {
+  for (uint32_t m = p_ext; m; m &= m - 1) { const int x = __ffs(m) - 1; sums[x * stride] += creq[x]; }
+}
+// k pods requesting req (resources res) join existing node e. Returns its closed flag: no pod of the batch fits it any more
+// (min_req: per-resource minimum request over all pod classes).
+template <class Req>
+__device__ __forceinline__ bool existing_add(const PackState& s, int R, int e, uint32_t res, const Req* req, long long k) {
+  const int NE = s.n_existing;
+  bool closed = false;
+  for (int r = 0; r < R; ++r) {
+    if ((res >> r) & 1) s.ex_req[(size_t)r * NE + e] += k * req[r];
+    const long long a = ((s.ex_avail_present[e] >> r) & 1) ? s.ex_avail[(size_t)r * NE + e] : 0;
+    if (s.min_req[r] > 0 && s.ex_req[(size_t)r * NE + e] + s.min_req[r] > a) closed = true;
+  }
+  s.ex_req_present[e] |= res;
+  return closed;
+}
 struct ExRunIO { int qi, head, qlen, seq, parity, placed; long long add_calls; };
 __shared__ ExRunIO g_xio;
 // one partial sum per warp, double-buffered: every warp of the largest block the kernel is launched with needs a slot
@@ -557,14 +597,8 @@ __device__ __noinline__ void existing_run(const PodRegs& first) {
     const int excl = incl - k, want = m - placed;
     const int take = excl < want ? min(k, want - excl) : 0;
     if (take > 0) {
-      bool closed = false;
-      for (int r = 0; r < R; ++r) {
-        if (r < kHotRes && ((first.res >> r) & 1)) s.ex_req[(size_t)r * NE + e] += (long long)take * first.req[r];
-        const long long a = ((s.ex_avail_present[e] >> r) & 1) ? s.ex_avail[(size_t)r * NE + e] : 0;
-        if (s.min_req[r] > 0 && s.ex_req[(size_t)r * NE + e] + s.min_req[r] > a) closed = true;
-      }
-      s.ex_req_present[e] |= first.res;
-      s.ex_closed[e] = closed;
+      // (the run's pods request hot resources only: its gate admits no class with res >> kHotRes)
+      s.ex_closed[e] = existing_add(s, R, e, first.res & ((1u << kHotRes) - 1), first.req, take);
       for (int j = 0; j < take; ++j) {
         const uint32_t pod = s.order[qi + placed + excl + j];
         s.assign[pod] = e;
@@ -591,6 +625,112 @@ __device__ __noinline__ void existing_run(const PodRegs& first) {
   __syncthreads();
 }
 
+// Cycle and event counters of the profiling build (KSCHED_PROFILE_PACK): PK_T in pack_kernel (pk_acc / pk_last), GK_T / GK_C
+// in the generic step (gk_last, the PackState s)
+#ifdef KSCHED_PROFILE_PACK
+#define PK_T(i) { long long _now = clock64(); pk_acc[i] += _now - pk_last; pk_last = _now; }
+#define GK_T(i) { if (threadIdx.x == 0) { long long _n = clock64(); s.counters[i] += _n - gk_last; gk_last = _n; } }
+#define GK_C(i) { if (threadIdx.x == 0) s.counters[i] += 1; }
+#else
+#define PK_T(i)
+#define GK_T(i)
+#define GK_C(i)
+#endif
+
+// generic step, staging: the pod's row into g_row and its topology constraints into g_pt. false: PodTopo overflowed
+// (L.fatal is set).
+__device__ __forceinline__ bool gen_stage(const ksched_pod_row* src, uint32_t cls, bool has_topo, LoopVars& L) {
+  const int tid = threadIdx.x;
+  PodTopo& pt = g_pt;
+  // The pod's 256-byte row lives in shared memory (everything below reads it with immediate addresses); rows of one
+  // class are identical, so it is copied on a class change only.
+  const bool new_row = L.row_class != cls;
+  const bool topo_step = has_topo || L.pt_nonempty;
+  if (new_row || topo_step) {
+    __syncthreads();  // previous step's readers of g_row / g_pt are done
+    if (tid < 32) {
+      if (new_row) {
+        reinterpret_cast<uint64_t*>(&g_row)[tid] = reinterpret_cast<const uint64_t*>(src)[tid];
+        __syncwarp();
+      }
+      if (topo_step) {
+        if (L.pt_class == cls && !pt.overflow) refresh_pod_topo();  // same relations as the previous step, new counters
+        else build_pod_topo();
+      }
+    }
+    L.row_class = cls;
+    if (topo_step) L.pt_class = cls;
+    __syncthreads();
+    if (topo_step) {
+      L.pt_nonempty = pt.n != 0;
+      if (pt.overflow) { L.fatal = KSCHED_ERR_UNSUPPORTED; return false; }
+    }
+  }
+  return true;
+}
+// generic step, failure: relax + requeue (scheduler.go:117-123, queue.go:61-68)
+__device__ __forceinline__ void gen_requeue(uint32_t pod, bool has_topo, LoopVars& L) {
+  KS_K2
+  KS_ROW
+  const int qcap = s.n_pods + 1;
+  GK_C(kCtrGenFailures)
+  const uint32_t nx = row.relax_next;
+  int tail = L.head + L.qlen;
+  if (tail >= qcap) tail -= qcap;
+  if (threadIdx.x == 0) {
+    s.queue[tail] = pod;
+    if (nx != KSCHED_NONE) {
+      s.pod_class[pod] = nx;
+      s.relax_level[pod] += 1;
+      // Topology.Update(pod): groups that only the relaxed spec owns come into existence now
+      const ksched_pod_row& nrow = s.classes[nx];
+      for (uint32_t e = nrow.topo_begin; e < nrow.topo_end; ++e) {
+        const ksched_class_topo ct = s.class_topo[e];
+        if ((ct.flags & KSCHED_TOPO_CONSTRAINS) && !s.grp_active[ct.group]) {
+          s.grp_active[ct.group] = 1;
+          s.grp_min_slot[ct.group] = s.n_existing + L.n_new;
+        }
+      }
+    } else {
+      s.last_len[pod] = L.qlen + 1;
+      s.last_epoch[pod] = L.epoch;
+    }
+  }
+  ++L.qlen;
+  if (nx != KSCHED_NONE) ++L.epoch;  // a successful relaxation resets the lastLen map
+  L.fail_memo = nx == KSCHED_NONE && !has_topo && !L.pt_nonempty;
+  __syncthreads();
+}
+
+// generic step, in-flight winner that failed its full check: no later argmin of this step picks it again
+__device__ __forceinline__ void exclude_winner(const Hot& H, int wa, bool simple, unsigned cls, int& n_excl, bool& full_eval) {
+  if (threadIdx.x == 0) {
+    if (n_excl < kMaxExcl) g_sh.excl[n_excl] = wa;
+    if (simple) H.rejected(wa) = cls;
+  }
+  ++n_excl;
+  if (n_excl >= kMaxExcl) full_eval = true;
+  __syncthreads();
+}
+// generic step, option word w of in-flight node: narrowed by the winner's requirements and, for an ext class, its ext sums
+__device__ __forceinline__ uint32_t narrow_word(const DevCatalog& c, const PackState& s, const TypeCtx& x, uint32_t base, int w,
+                                                const int64_t* node_ext, const int64_t* cls_ext, uint32_t p_ext) {
+  uint32_t sw = type_word_keys(c, s, x, base, w);
+  if (sw && p_ext) sw = ext_fit_word(c, node_ext, cls_ext, p_ext, sw, w);
+  return sw;
+}
+// generic step, Pareto front of a memoised option set: entry i of (bound, bound2, dom) in the fc_* or fd_* tables, to / from g_sh
+__device__ __forceinline__ void front_load(const long long* b1, const long long* b2, const uint8_t* dom, size_t i) {
+  StepShared& sh = g_sh;
+  for (int r = 0; r < kHotRes; ++r) { sh.bound[r] = b1[i * kHotRes + r]; sh.bound2[r] = b2[i * kHotRes + r]; }
+  sh.front_bits = dom[i];
+}
+__device__ __forceinline__ void front_store(long long* b1, long long* b2, uint8_t* dom, size_t i) {
+  const StepShared& sh = g_sh;
+  for (int r = 0; r < kHotRes; ++r) { b1[i * kHotRes + r] = sh.bound[r]; b2[i * kHotRes + r] = sh.bound2[r]; }
+  dom[i] = (uint8_t)sh.front_bits;
+}
+
 // One full Scheduler.add for one pod (existing nodes -> in-flight nodes -> new node -> relax/requeue). Every thread of
 // the CTA calls it together. Kept out of line: the steady-state path in pack_kernel must stay a few KB of code, because a
 // single resident CTA runs straight out of the instruction cache hierarchy (L0 ~6 KB, L1.5 32 KB).
@@ -601,8 +741,6 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
   const int tid = threadIdx.x, lane = tid & 31;
   const int W32 = c.W32, V = c.n_templates, NE = s.n_existing, MAXN = s.max_new;
   const int R = c.n_res, RH = R < kHotRes ? R : kHotRes;
-  const int qcap = s.n_pods + 1;
-  PodTopo& pt = g_pt;
   Touched& fresh_t = g_fresh_t;
   TypeCtx& fresh_x = g_fresh_x;
   unsigned long long (*red)[32] = g_red;
@@ -610,18 +748,11 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
   const uint32_t* tmpl_taintset = g_tmpl_taintset;
   const Hot H = make_hot(s);
   const int64_t* alloc_sorted = alloc_table(c, s);
-  int &head = L.head, &qlen = L.qlen, &n_new = L.n_new, &n_active = L.n_active, &tick = L.tick, &seq = L.seq, &parity = L.parity, &fatal = L.fatal;
-  uint32_t& epoch = L.epoch;
+  int &n_new = L.n_new, &n_active = L.n_active, &tick = L.tick, &seq = L.seq, &parity = L.parity, &fatal = L.fatal;
   bool& pt_nonempty = L.pt_nonempty;
   long long& nodes_visited = L.nodes_visited;
-  uint32_t& pt_class = L.pt_class;
 #ifdef KSCHED_PROFILE_PACK
   long long gk_last = clock64();
-#define GK_T(i) { if (tid == 0) { long long _n = clock64(); s.counters[i] += _n - gk_last; gk_last = _n; } }
-#define GK_C(i) { if (tid == 0) s.counters[i] += 1; }
-#else
-#define GK_T(i)
-#define GK_C(i)
 #endif
     const uint32_t pod = cur.pod, cls = (uint32_t)cur.cls64;
     L.fresh_valid = 0;
@@ -634,30 +765,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
     const uint64_t p_tol = cur.tol, p_hpc = cur.hpc, p_hpe = cur.hpe;
     const uint32_t p_keys = (uint32_t)(cur.meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF, p_itype = cur.itype, p_hostname = cur.hostname;
     const bool has_topo = cur.topo_begin != cur.topo_end;
-    // The pod's 256-byte row lives in shared memory (everything below reads it with immediate addresses); rows of one
-    // class are identical, so it is copied on a class change only.
-    const bool new_row = L.row_class != cls;
-    const bool topo_step = has_topo || pt_nonempty;
-    if (new_row || topo_step) {
-      __syncthreads();  // previous step's readers of g_row / g_pt are done
-      if (tid < 32) {
-        if (new_row) {
-          reinterpret_cast<uint64_t*>(&g_row)[tid] = reinterpret_cast<const uint64_t*>(cur.row)[tid];
-          __syncwarp();
-        }
-        if (topo_step) {
-          if (pt_class == cls && !pt.overflow) refresh_pod_topo();  // same relations as the previous step, new counters
-          else build_pod_topo();
-        }
-      }
-      L.row_class = cls;
-      if (topo_step) pt_class = cls;
-      __syncthreads();
-      if (topo_step) {
-        pt_nonempty = pt.n != 0;
-        if (pt.overflow) { fatal = KSCHED_ERR_UNSUPPORTED; return; }
-      }
-    }
+    if (!gen_stage(cur.row, cls, has_topo, L)) return;
     // ext resources (DESIGN.md §3): checked on every node this class is placed on, narrowed eagerly into new nodes' options.
     // A class that requests one is neither plain nor simple: no in-flight node accepts it without the full check.
     const uint32_t p_ext = kExt ? class_ext(s, cls) : 0u;
@@ -691,11 +799,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
           long long a = ((s.ex_avail_present[e] >> r) & 1) ? s.ex_avail[(size_t)r * NE + e] : 0;
           ok = q <= a;
         }
-        for (uint32_t m = p_ext; m && ok; m &= m - 1) {
-          const int x = __ffs(m) - 1;
-          ok = s.ex_req_ext[(size_t)x * NE + e] + s.cls_req_ext[(size_t)cls * X + x] <= s.ex_avail_ext[(size_t)x * NE + e];
-        }
-        if (!ok) continue;
+        if (!ok || !ext_fits(s.ex_req_ext + e, s.ex_avail_ext + e, NE, s.cls_req_ext + (size_t)cls * X, p_ext)) continue;
         if (soft == ~0u) soft = (unsigned)e;
         if (p_itype != KSCHED_NONE) {
           const uint32_t it = s.ex_itype[e];
@@ -715,14 +819,8 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
         nodes_visited += e + 1;
         if (mine == w32) {  // the winning thread commits its own candidate
           if (!plain) commit_touched(t, s.ex_vals, s.ex_meta, NE, e);
-          bool closed = false;
-          for (int r = 0; r < R; ++r) {
-            if ((p_res >> r) & 1) s.ex_req[(size_t)r * NE + e] += row.requests[r];
-            long long a = ((s.ex_avail_present[e] >> r) & 1) ? s.ex_avail[(size_t)r * NE + e] : 0;
-            if (s.min_req[r] > 0 && s.ex_req[(size_t)r * NE + e] + s.min_req[r] > a) closed = true;
-          }
-          s.ex_req_present[e] |= p_res;
-          for (uint32_t m = p_ext; m; m &= m - 1) { const int x = __ffs(m) - 1; s.ex_req_ext[(size_t)x * NE + e] += s.cls_req_ext[(size_t)cls * X + x]; }
+          const bool closed = existing_add(s, R, e, p_res, row.requests, 1);
+          ext_add(s.ex_req_ext + e, NE, s.cls_req_ext + (size_t)cls * X, p_ext);
           node_hp_commit(s, p_hpe, p_hpx, cls, s.ex_hp, s.ex_hp_ext, NE, e);
           if (s.ex_it && p_itype != KSCHED_NONE) itype_state_add(e, p_itype);
           if (has_vol) node_vol_commit(cls, e);
@@ -821,13 +919,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
         __syncthreads();
         const int wa = sh.win_a, wn = sh.win_n;
         if (sh.win_fail) {  // the prefilter let through a node the full requirement check refuses
-          if (tid == 0) {
-            if (n_excl < kMaxExcl) sh.excl[n_excl] = wa;
-            if (simple) H.rejected(wa) = cls;
-          }
-          ++n_excl;
-          if (n_excl >= kMaxExcl) full_eval = true;
-          __syncthreads();
+          exclude_winner(H, wa, simple, cls, n_excl, full_eval);
           continue;
         }
         const bool coop = sh.win_need != 0;
@@ -848,19 +940,12 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
           for (int w = tid; w < W32; w += blockDim.x) {
             const uint32_t base = s.nn_opts[(size_t)w * MAXN + wn];
             if (!base) continue;
-            uint32_t sw = type_word_keys(c, s, fresh_x, base, w);
-            if (sw && p_ext) sw = ext_fit_word(c, wn_ext, s.cls_req_ext + (size_t)cls * X, p_ext, sw, w);
+            const uint32_t sw = narrow_word(c, s, fresh_x, base, w, wn_ext, s.cls_req_ext + (size_t)cls * X, p_ext);
             if (w == tid) { keep_base = base; keep = sw; }
             if (sw && type_word_res(c, fresh_x, sw, w)) local_any = 1;
           }
           if (!__syncthreads_or(local_any)) {  // no option survives: Node.Add fails on this node (node.go:92-95)
-            if (tid == 0) {
-              if (n_excl < kMaxExcl) sh.excl[n_excl] = wa;
-              if (simple) H.rejected(wa) = cls;
-            }
-            ++n_excl;
-            if (n_excl >= kMaxExcl) full_eval = true;
-            __syncthreads();
+            exclude_winner(H, wa, simple, cls, n_excl, full_eval);
             continue;
           }
           if (sh.win_commit) {  // requirement-driven narrowing of the stored options; resources stay lazy
@@ -869,8 +954,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
             for (int w = tid + blockDim.x; w < W32; w += blockDim.x) {
               const uint32_t base = s.nn_opts[(size_t)w * MAXN + wn];
               if (!base) continue;
-              uint32_t sw = type_word_keys(c, s, fresh_x, base, w);
-              if (sw && p_ext) sw = ext_fit_word(c, wn_ext, s.cls_req_ext + (size_t)cls * X, p_ext, sw, w);
+              const uint32_t sw = narrow_word(c, s, fresh_x, base, w, wn_ext, s.cls_req_ext + (size_t)cls * X, p_ext);
               if (sw != base) { s.nn_opts[(size_t)w * MAXN + wn] = sw; local_changed = 1; }
             }
             opts_changed = __syncthreads_or(local_changed) != 0;
@@ -924,7 +1008,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
             }
           }
           if (p_ext) {  // after the narrowing above, which read the node's sums before this pod
-            for (uint32_t m = p_ext; m; m &= m - 1) { const int x = __ffs(m) - 1; s.nn_req_ext[(size_t)n * X + x] += s.cls_req_ext[(size_t)cls * X + x]; }
+            ext_add(s.nn_req_ext + (size_t)n * X, 1, s.cls_req_ext + (size_t)cls * X, p_ext);
             s.nn_ext_present[n] |= p_ext;
           }
           H.flags(a) = fl;
@@ -1082,8 +1166,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
           uint64_t meta;
           if (path == kPathCached) {
             meta = s.fc_meta[fc];
-            for (int r = 0; r < kHotRes; ++r) { sh.bound[r] = s.fc_bound[fc * kHotRes + r]; sh.bound2[r] = s.fc_bound2[fc * kHotRes + r]; }
-            sh.front_bits = s.fc_dom[fc];
+            front_load(s.fc_bound, s.fc_bound2, s.fc_dom, fc);
             sh.qp = s.fc_qp[fc];
             for (int r = 0; r < KSCHED_MAX_RES; ++r) sh.q[r] = s.fc_q[fc * KSCHED_MAX_RES + r];
           } else {
@@ -1091,44 +1174,34 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
             // K1-row path without limits: the option set, hence its Pareto front, depends on (class, template) only
             const bool front_memo = path == kPathRow && !limits_active;
             if (front_memo && s.fc_front_state[fc]) {
-              for (int r = 0; r < kHotRes; ++r) { sh.bound[r] = s.fc_bound[fc * kHotRes + r]; sh.bound2[r] = s.fc_bound2[fc * kHotRes + r]; }
-              sh.front_bits = s.fc_dom[fc];
+              front_load(s.fc_bound, s.fc_bound2, s.fc_dom, fc);
             } else if (path == kPathDynCached) {
-              for (int r = 0; r < kHotRes; ++r) { sh.bound[r] = s.fd_bound[(size_t)fd_slot * kHotRes + r]; sh.bound2[r] = s.fd_bound2[(size_t)fd_slot * kHotRes + r]; }
-              sh.front_bits = s.fd_dom[fd_slot];
+              front_load(s.fd_bound, s.fd_bound2, s.fd_dom, fd_slot);
             } else {  // (front_fresh: computed by the CTA above)
               if (front_memo) {
-                for (int r = 0; r < kHotRes; ++r) { s.fc_bound[fc * kHotRes + r] = sh.bound[r]; s.fc_bound2[fc * kHotRes + r] = sh.bound2[r]; }
-                s.fc_dom[fc] = (uint8_t)sh.front_bits;
+                front_store(s.fc_bound, s.fc_bound2, s.fc_dom, fc);
                 s.fc_front_state[fc] = 1;
               }
               if (path == kPathDynamic && fd_slot >= 0) {
-                for (int r = 0; r < kHotRes; ++r) { s.fd_bound[(size_t)fd_slot * kHotRes + r] = sh.bound[r]; s.fd_bound2[(size_t)fd_slot * kHotRes + r] = sh.bound2[r]; }
-                s.fd_dom[fd_slot] = (uint8_t)sh.front_bits;
+                front_store(s.fd_bound, s.fd_bound2, s.fd_dom, fd_slot);
                 s.fd_state[fd_slot] = 1;
               }
             }
             if (memo) {
               s.fc_meta[fc] = meta;
-              for (int r = 0; r < kHotRes; ++r) { s.fc_bound[fc * kHotRes + r] = sh.bound[r]; s.fc_bound2[fc * kHotRes + r] = sh.bound2[r]; }
-              s.fc_dom[fc] = (uint8_t)sh.front_bits;
+              front_store(s.fc_bound, s.fc_bound2, s.fc_dom, fc);
               s.fc_qp[fc] = sh.qp;
               for (int r = 0; r < KSCHED_MAX_RES; ++r) s.fc_q[fc * KSCHED_MAX_RES + r] = sh.q[r];
               s.fc_state[fc] = 1;
             }
           }
-          s.nn_meta[n] = meta;
-          s.nn_tmpl[n] = (uint8_t)v;
+          // requests and ext sums first, as the class runs write them (the same thread, no barrier before open_node)
           for (int r = 0; r < KSCHED_MAX_RES; ++r) s.nn_req[(size_t)r * MAXN + n] = sh.q[r];
-          s.nn_req_present[n] = sh.qp;
           if (kExt) {  // a fresh node's ext sums are the pod's: no daemonset requests an ext resource
             for (int x = 0; x < X; ++x) s.nn_req_ext[(size_t)n * X + x] = ((p_ext >> x) & 1) ? s.cls_req_ext[(size_t)cls * X + x] : 0;
             s.nn_ext_present[n] = p_ext;
           }
-          fresh_node_hp(s, p_hpe, p_hpx, cls, n);
-          if (s.nn_it) itype_state_open(n, v, p_itype);
-          s.nn_count[n] = 1;
-          s.nn_tb[n] = tick + 1;  // appended: last of the one-pod block
+          open_node(s, n, v, meta, sh.qp, p_hpe, p_hpx, cls, p_itype, true, tick + 1);  // appended: last of the one-pod block
           const bool closed = node_closed(sh.q, s.min_req, RH, sh.bound, sh.bound2, sh.front_bits);
           if (!closed) {
             H.key(a) = order_key(1, tick + 1);
@@ -1170,36 +1243,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
       if (fatal) return;
     }
     GK_T(kCtrGenFresh)
-    // ------------------------------------------------------------ failure: relax + requeue (scheduler.go:117-123, queue.go:61-68)
-    if (!placed) {
-      GK_C(kCtrGenFailures)
-      const uint32_t nx = row.relax_next;
-      int tail = head + qlen;
-      if (tail >= qcap) tail -= qcap;
-      if (tid == 0) {
-        s.queue[tail] = pod;
-        if (nx != KSCHED_NONE) {
-          s.pod_class[pod] = nx;
-          s.relax_level[pod] += 1;
-          // Topology.Update(pod): groups that only the relaxed spec owns come into existence now
-          const ksched_pod_row& nrow = s.classes[nx];
-          for (uint32_t e = nrow.topo_begin; e < nrow.topo_end; ++e) {
-            const ksched_class_topo ct = s.class_topo[e];
-            if ((ct.flags & KSCHED_TOPO_CONSTRAINS) && !s.grp_active[ct.group]) {
-              s.grp_active[ct.group] = 1;
-              s.grp_min_slot[ct.group] = NE + n_new;
-            }
-          }
-        } else {
-          s.last_len[pod] = qlen + 1;
-          s.last_epoch[pod] = epoch;
-        }
-      }
-      ++qlen;
-      if (nx != KSCHED_NONE) ++epoch;  // a successful relaxation resets the lastLen map
-      L.fail_memo = nx == KSCHED_NONE && !has_topo && !pt_nonempty;
-      __syncthreads();
-    }
+    if (!placed) gen_requeue(pod, has_topo, L);
   }
 
 // no requirement of the pod can change a node's requirements
@@ -2272,17 +2316,11 @@ __device__ __forceinline__ void m1_store_fresh(const RunEnv& e) {
     if (w < e.W32) s.nn_opts[(size_t)w * e.MAXN + n] = v.opts[w];
     if (w < c.n_keys) s.nn_vals[(size_t)w * e.MAXN + n] = v.vals[w];
     if (w < KSCHED_MAX_RES) s.nn_req[(size_t)w * e.MAXN + n] = v.q[w];
-    if (w == 0) {
-      s.nn_meta[n] = v.meta;
-      s.nn_tmpl[n] = (uint8_t)(v.fl >> 8);
-      s.nn_req_present[n] = v.qp;
-      fresh_node_hp(s, 0, false, 0, n);
-      if (s.nn_it) itype_state_open(n, v.fl >> 8, KSCHED_NONE);  // the class run takes no instance-type class while the state is kept
-      if (((e.rpv[a] >> 16) & 0x7FFF) == 0) {  // no further pod so far: (1, creation tick); otherwise the run's write-back stores them
-        s.nn_count[n] = 1;
-        s.nn_tb[n] = (int)((unsigned)e.hs->key[a] ^ 0x80000000u);
-      }
-    }
+    // the class run takes no instance-type class while the slot state is kept; the pod count and tie-break are (1, creation
+    // tick) while the node has no further pod, otherwise the run's write-back stores them
+    if (w == 0)
+      open_node(s, n, v.fl >> 8, v.meta, v.qp, 0, false, 0, KSCHED_NONE, ((e.rpv[a] >> 16) & 0x7FFF) == 0,
+                (int)((unsigned)e.hs->key[a] ^ 0x80000000u));
   }
 }
 
@@ -2584,13 +2622,7 @@ __device__ __forceinline__ bool run_fresh_step(const RunEnv& e, int buf, int i, 
     const int t = (K - j * m < m ? K - j * m : m) - 1;  // further pods on this node (the last one may get fewer)
     const int tk = tick + j * m;                          // tick of its first pod
     run_fresh(e, v, a, n, tk + 1);
-    s.nn_meta[n] = v.meta;
-    s.nn_tmpl[n] = (uint8_t)(v.fl >> 8);
-    s.nn_req_present[n] = v.qp;
-    fresh_node_hp(s, 0, false, 0, n);
-    if (s.nn_it) itype_state_open(n, v.fl >> 8, KSCHED_NONE);
-    s.nn_count[n] = 1;
-    s.nn_tb[n] = tk + 1;
+    open_node(s, n, v.fl >> 8, v.meta, v.qp, 0, false, 0, KSCHED_NONE, true, tk + 1);
     if (n_mask > 0) e.zv[a] = (1u << fd0) | (3u << 16);
     if (n_mask > 1) e.zv[kTopoCap + a] = (1u << fd1) | (3u << 16);
     // the fill's t further pods (the slot holds the variant's requests and front, and v.rp carries no placed pod)
@@ -3018,15 +3050,9 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
 }
 
 
-#ifdef KSCHED_PROFILE_PACK
-#define PK_T(i) { long long _now = clock64(); pk_acc[i] += _now - pk_last; pk_last = _now; }
-#else
-#define PK_T(i)
-#endif
-
 // kExt: the problem has ext resources (DESIGN.md §3). Without them the kernel is compiled without any ext gate.
 // kMaxThreads: the largest block the instantiation is launched with. Its register budget is 64 K / kMaxThreads (capped at
-// 255): 128 registers at 512 threads spill in class_run and the generic step, 254 at 256 threads do not (run_pack picks the instantiation).
+// 255): 128 registers at 512 threads spill in class_run and the generic step, 222 at 256 threads do not (run_pack picks the instantiation).
 template <bool kExt, int kMaxThreads>
 __global__ void __launch_bounds__(kMaxThreads, 1) pack_kernel() {
   static_assert(kMaxThreads % 32 == 0 && kMaxThreads <= kPackThreads, "pack_kernel: whole warps, at most kPackThreads");

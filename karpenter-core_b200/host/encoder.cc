@@ -79,6 +79,7 @@ Req new_requirement(Op op, const std::vector<std::string>& values, const std::ma
 // A requirement on kubernetes.io/hostname in the reference's string algebra: NewRequirement (requirement.go:44-68),
 // Intersection (:117-150), Has (:171-176), Operator (:186-197). Hostnames are not dictionary values, so the encoder
 // evaluates these on strings and hands the device the existing slots they admit (DESIGN.md §3, hostname requirements).
+// The daemonset overhead uses the same algebra on node.kubernetes.io/instance-type (string_compatible).
 constexpr const char* kPlaceholderPrefix = "hostname-placeholder-";  // a new node's hostname (node.go:46, a per-Solve counter)
 struct HostnameReq {
   bool comp = true;  // (true, {}, no bounds): Exists
@@ -88,6 +89,9 @@ struct HostnameReq {
   static HostnameReq make(const NodeSelectorRequirement& r) {
     for (auto& v : r.values)
       if (v.rfind(kPlaceholderPrefix, 0) == 0) unsupported("hostname requirement naming a placeholder hostname: " + v);
+    return of(r);
+  }
+  static HostnameReq of(const NodeSelectorRequirement& r) {  // NewRequirement on any key
     HostnameReq h;
     h.comp = !(r.op == Op::In || r.op == Op::DoesNotExist);
     if (r.op == Op::In || r.op == Op::NotIn) h.values.insert(r.values.begin(), r.values.end());
@@ -137,6 +141,23 @@ HostnameReq hostname_intersection(const std::vector<NodeSelectorRequirement>& rs
   HostnameReq h = HostnameReq::make(rs.at(0));
   for (size_t i = 1; i < rs.size(); ++i) h = HostnameReq::make(rs[i]).intersect(h);
   return h;
+}
+// Requirements.Add of a list of requirements on one key, on strings; nullopt for an empty list (the key is not defined)
+std::optional<HostnameReq> string_requirement(const std::vector<NodeSelectorRequirement>& rs) {
+  if (rs.empty()) return std::nullopt;
+  HostnameReq h = HostnameReq::of(rs[0]);
+  for (size_t i = 1; i < rs.size(); ++i) h = HostnameReq::of(rs[i]).intersect(h);
+  return h;
+}
+// One key of Requirements.Compatible (requirements.go:123-133) on strings, `node` the receiver and nullopt where a side does
+// not define the key: an undefined node key admits anything on a well-known key and only NotIn / DoesNotExist on another;
+// a defined one must Intersect (:189-206): a non-empty intersection, or NotIn / DoesNotExist on both sides.
+bool string_compatible(const std::optional<HostnameReq>& node, const std::optional<HostnameReq>& inc, bool well_known) {
+  if (!inc) return true;
+  if (!node) return well_known || inc->admits_unlabelled();
+  const HostnameReq i = node->intersect(*inc);
+  if (i.comp || !i.values.empty()) return true;  // Len() of a complement is never 0
+  return node->admits_unlabelled() && inc->admits_unlabelled();
 }
 
 // ---- resources (utils/resources/resources.go)
@@ -510,8 +531,8 @@ struct Profile {  // KSCHED_ENCODE_PROFILE: one line per phase of encode() on st
 };
 
 struct Spec { Pod pod; ResourceList req; uint32_t next = KSCHED_NONE; };  // a pod class and the class its relaxation leads to
-// a daemonset pod's requirements (`special`: it has hostname / instance-type ones) and requests
-struct Daemon { const Pod* pod; ksched_reqset rs; ksched_bounds bd; bool special; ResourceList req; };
+// a daemonset pod's requirements (on the mask keys, and on the hostname / instance-type keys when it names them) and requests
+struct Daemon { const Pod* pod; ksched_reqset rs; ksched_bounds bd; std::optional<HostnameReq> hostname, itype; ResourceList req; };
 
 // The encoder's state: what one phase of encode() hands to the next.
 struct Builder {
@@ -1445,15 +1466,19 @@ void templates(Builder& B) {
 }
 
 // ------------------------------------------------------------------ daemonset overhead (scheduler.go:250-267)
-// The daemonset pods a node with these taints and requirements runs: their requests, and one pod each. A template refuses a
-// daemon that tolerates its taints and names a hostname or an instance type.
-ResourceList daemon_overhead(const Builder& B, const std::vector<Taint>& taints, const ksched_reqset& rs, const ksched_bounds& bd, bool is_template) {
+// The daemonset pods a node with these taints and requirements runs (Taints.Tolerates, then Requirements.Compatible with
+// the daemon's NewPodRequirements): their requests, and one pod each. `itype` / `hostname` are the node's requirements on
+// those keys, nullopt where it defines none. Instance-type is well-known, so a node that does not define it is compatible
+// with any instance-type requirement. A template refuses a daemon that tolerates its taints and names a hostname.
+ResourceList daemon_overhead(const Builder& B, const std::vector<Taint>& taints, const ksched_reqset& rs, const ksched_bounds& bd,
+                             const std::optional<HostnameReq>& itype, const std::optional<HostnameReq>& hostname, bool is_template) {
   ResourceList total;
   int count = 0;
   for (auto& d : B.daemons) {
     if (!tolerates_all(taints, d.pod->tolerations)) continue;
-    if (is_template && d.special) unsupported("daemonset pod with hostname / instance-type requirement");
+    if (is_template && d.hostname) unsupported("daemonset pod with a hostname requirement");
     if (!B.compatible(rs, bd, d.rs, d.bd)) continue;
+    if (!string_compatible(itype, d.itype, true) || !string_compatible(hostname, d.hostname, false)) continue;
     total = merge(total, d.req);
     ++count;
   }
@@ -1462,15 +1487,21 @@ ResourceList daemon_overhead(const Builder& B, const std::vector<Taint>& taints,
 }
 void daemonset_overhead(Builder& B) {
   for (auto& d : B.P.daemonset_pods) {
-    Daemon x{&d, {}, {}, false, pod_requests(d)};
+    Daemon x{&d, {}, {}, std::nullopt, std::nullopt, pod_requests(d)};
     Builder::Special sp;
     B.pod_requirements(d, x.rs, x.bd, &sp);
-    x.special = !sp.hostname.empty() || !sp.itype.empty();
+    x.hostname = string_requirement(sp.hostname);
+    x.itype = string_requirement(sp.itype);
     B.daemons.push_back(x);
   }
+  // per template, as getDaemonOverhead does: a template that does not define the instance-type key charges a daemon with an
+  // instance-type requirement on every type it offers (DESIGN.md §3, daemonset overhead)
   for (size_t v = 0; v < B.E.templates.size(); ++v) {
     ksched_template& t = B.E.templates[v];
-    const ResourceList total = daemon_overhead(B, B.P.provisioners[B.E.template_provisioner[v]].taints, t.reqs, B.E.template_bounds[v], true);
+    std::optional<HostnameReq> itype;  // the template's own requirement on the key: provisioner requirements and labels
+    if (const auto& own = B.template_itype[v]) itype = HostnameReq{own->first, own->second};
+    const ResourceList total = daemon_overhead(B, B.P.provisioners[B.E.template_provisioner[v]].taints, t.reqs, B.E.template_bounds[v],
+                                               itype, std::nullopt, true);
     t.daemon_res_present = B.fill_resources(total, t.daemon_requests);
   }
 }
@@ -1546,6 +1577,8 @@ void existing_nodes(Builder& B) {
   E.remaining_exact.resize((size_t)NV * KSCHED_MAX_RES);
   for (int v = 0; v < NV; ++v)
     for (int r = 0; r < KSCHED_MAX_RES; ++r) E.remaining_exact[(size_t)v * KSCHED_MAX_RES + r] = E.templates[v].remaining[r];
+  bool daemon_itype = false, daemon_hostname = false;
+  for (auto& d : B.daemons) { daemon_itype = daemon_itype || d.itype; daemon_hostname = daemon_hostname || d.hostname; }
   for (int si : B.state_nodes) {
     const StateNode& n = P.nodes[si];
     auto own = n.labels.find(kProvisionerName);
@@ -1556,8 +1589,11 @@ void existing_nodes(Builder& B) {
     Builder::Special sp;
     const NodeFacts& nf = B.facts.node[(size_t)si];
     B.add_selector_reqs(e.reqs, nb, nf.label_reqs, &sp);
-    // the daemonsets' requests not yet bound: resources.Subtract over keys of lhs, clamped at 0
-    ResourceList rem = daemon_overhead(B, n.taints, e.reqs, nb, false);  // raw Spec.Taints (scheduler.go:231)
+    // the daemonsets' requests not yet bound: resources.Subtract over keys of lhs, clamped at 0. The node's labels define its
+    // instance type and hostname (In [label], both instance-type label keys when a node carries both); a key no daemon names
+    // cannot turn one away, so it is only read when some daemon does.
+    ResourceList rem = daemon_overhead(B, n.taints, e.reqs, nb, daemon_itype ? string_requirement(sp.itype) : std::nullopt,
+                                       daemon_hostname ? string_requirement(sp.hostname) : std::nullopt, false);  // raw Spec.Taints (scheduler.go:231)
     subtract_in_place(rem, nf.ds_req);
     for (auto& kv : rem) if (kv.second < 0) kv.second = 0;
     ResourceList avail = n.allocatable;

@@ -14,21 +14,13 @@ Prints one JSON line per workload with the card name and power limit read in the
 """
 import argparse
 import copy
-import json
 import random
 import statistics
-import subprocess
-import sys
 import time
-from pathlib import Path
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
-
-import daemonset_itype_problems as dp  # noqa: E402
-import fixtures as fx  # noqa: E402
-from conftest import load_pkg  # noqa: E402
+import daemonset_itype_problems as dp
+import fixtures as fx
+from timing_lib import card, emit, load_pkg, need_device
 
 GENERAL = ["m5.large", "m5.xlarge", "m5.2xlarge", "c5.xlarge", "c5.4xlarge"]
 
@@ -87,9 +79,8 @@ def main():
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     pkg = load_pkg()
-    if pkg.device_count() < 1:
-        raise SystemExit("needs a CUDA device")
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    need_device(pkg)
+    gpu = card()
     lines = []
 
     c4 = c4_dict()
@@ -109,11 +100,10 @@ def main():
             enc.append(ph["encode_us"] / 1000)
             solve.append(ph["total_us"] / 1000)
             placed = sum(1 for x in res.to_dict(brief=True)["assign"] if x >= 0)
-    lines.append({"card": card, "workload": "c4-daemonsets", "pods": len(c4["pods"]), "existing": rs.dims["existing"],
+    lines.append({"card": gpu, "workload": "c4-daemonsets", "pods": len(c4["pods"]), "existing": rs.dims["existing"],
                   "templates": rs.dims["templates"], "reps": a.reps, "encode_ms_median": statistics.median(enc),
                   "k1_ms_median": statistics.median(k1), "k2_ms_median": statistics.median(k2),
                   "solve_ms_median": statistics.median(solve), "placed": placed})
-    print(json.dumps(lines[-1]), flush=True)
 
     c5 = pkg.Problem.from_dict(c5_dict())
     load, search, sweep = [], [], []
@@ -131,14 +121,11 @@ def main():
             load.append((t1 - t0) * 1000)
             search.append((t2 - t1) * 1000)
             sweep.append((t3 - t2) * 1000)
-    lines.append({"card": card, "workload": "c5-daemonsets", "nodes": 2000, "candidates": cs.n_candidates, "reps": a.reps,
+    lines.append({"card": gpu, "workload": "c5-daemonsets", "nodes": 2000, "candidates": cs.n_candidates, "reps": a.reps,
                   "cluster_load_ms_median": statistics.median(load), "multi_node_search_ms_median": statistics.median(search),
                   "single_node_sweep_512_ms_median": statistics.median(sweep), "action": full["action"],
                   "nodes_removed": full["nodes_removed"], "probes": len(full["probes"]), "sweep_hits": sum(1 for x, _ in sw if x)})
-    print(json.dumps(lines[-1]), flush=True)
-    if a.out:
-        Path(a.out).parent.mkdir(parents=True, exist_ok=True)
-        Path(a.out).write_text("\n".join(json.dumps(x) for x in lines) + "\n")
+    emit(lines, a.out)
 
 
 if __name__ == "__main__":

@@ -14,19 +14,10 @@ Prints one JSON line per run with the card name, power limit and clock read in t
     python tests/gpu_extres_timing.py [--reps R] [--pods N] [--out FILE]
 """
 import argparse
-import json
 import statistics
-import subprocess
-import sys
-import time
-from pathlib import Path
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
-
-import fixtures as fx  # noqa: E402
-from conftest import load_pkg  # noqa: E402
+import fixtures as fx
+from timing_lib import card, emit, load_pkg, need_device, sweep_singles, timed
 
 EXT = [f"example.com/accel-{i}" for i in range(6)]
 QUOTA = {f"example.com/quota-{i}": "100000000" for i in range(5)}  # with cpu, memory, pods: the 8 row slots
@@ -80,16 +71,6 @@ def cluster_dict(ext, nodes=5000, pods_per_node=10, types=1000):
                       deriveCandidates=True)
 
 
-def timed(fn, reps):
-    fn()
-    ts, out = [], None
-    for _ in range(reps):
-        t0 = time.perf_counter()
-        out = fn()
-        ts.append(time.perf_counter() - t0)
-    return 1000 * statistics.median(ts), out
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
@@ -97,9 +78,8 @@ def main():
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     pkg = load_pkg()
-    if pkg.device_count() < 1:
-        raise SystemExit("needs a CUDA device")
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    need_device(pkg)
+    gpu = card()
     lines = []
     for share in (0.0, 0.05, 0.30):
         d, ext_pods = batch_dict(a.pods, share)
@@ -113,32 +93,22 @@ def main():
             if i:
                 k1.append(t["feasibility_us"]); k2.append(t["pack_us"]); tot.append(t["total_us"])
         e2e = statistics.median(rs.solve_e2e()[0] for _ in range(a.reps))
-        line = {"card": card, "workload": "batch", "pods": a.pods, "ext_share": share, "ext_pods_generic_step": ext_pods,
+        line = {"card": gpu, "workload": "batch", "pods": a.pods, "ext_share": share, "ext_pods_generic_step": ext_pods,
                 "resources": rs.dims["resources"], "resources_ext": rs.dims["resources_ext"], "classes": rs.dims["classes"],
                 "k1_ms": statistics.median(k1) / 1000, "k2_ms": statistics.median(k2) / 1000, "resident_ms": statistics.median(tot) / 1000,
                 "e2e_ms": e2e / 1000}
-        print(json.dumps(line), flush=True)
         lines.append(line)
     for ext in (True, False):
         problem = pkg.Problem.from_dict(cluster_dict(ext))
-        line = {"card": card, "workload": "cluster", "nodes": 5000, "bound_pods": 50000, "ext_requests": ext}
+        line = {"card": gpu, "workload": "cluster", "nodes": 5000, "bound_pods": 50000, "ext_requests": ext}
         multi = pkg.MultiNodeConsolidation(problem)
         line["multi_node_search_ms"], r = timed(multi.first_n_node_consolidation_option, a.reps)
         line["multi_node_action"], line["multi_node_removed"] = r["action"], r["nodes_removed"]
 
-        def sweep_all():
-            s = pkg.ClusterSession(problem)
-            acts = []
-            for lo in range(0, s.n_candidates, 64):
-                acts += [x[0] for x in s.probe_sets([[i] for i in range(lo, min(s.n_candidates, lo + 64))], False)]
-            s.close()
-            return acts
-        line["single_node_sweep_ms"], acts = timed(sweep_all, a.reps)
+        line["single_node_sweep_ms"], acts = timed(lambda: sweep_singles(pkg, problem), a.reps)
         line["single_node_candidates"] = len(acts)
-        print(json.dumps(line), flush=True)
         lines.append(line)
-    if a.out:
-        Path(a.out).write_text("\n".join(json.dumps(x) for x in lines) + "\n")
+    emit(lines, a.out)
 
 
 if __name__ == "__main__":

@@ -8,19 +8,11 @@ counted), and the card name and power limit read in the same run.
     python tests/gpu_hostname_timing.py [--reps R] [--out FILE]
 """
 import argparse
-import json
 import random
 import statistics
-import subprocess
-import sys
-from pathlib import Path
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
-
-import fixtures as fx  # noqa: E402
-from conftest import load_pkg  # noqa: E402
+import fixtures as fx
+from timing_lib import card, emit, load_pkg, need_device
 
 
 def c4_dict(excluded, nodes=2000, deployments=20, types=400, seed=4):
@@ -48,9 +40,8 @@ def main():
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     pkg = load_pkg()
-    if pkg.device_count() < 1:
-        raise SystemExit("needs a CUDA device")
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    need_device(pkg)
+    gpu = card()
     variants = {"plain": c4_dict(()), "notin5": c4_dict((0, 1, 2, 3, 4))}
     problems = {k: pkg.Problem.from_dict(v) for k, v in variants.items()}
     pack = {k: [] for k in variants}
@@ -71,15 +62,12 @@ def main():
                 d = res.to_dict()
                 n_ex = len(d["existing"])
                 big = [i for i, p in enumerate(variants[k]["pods"]) if p["labels"]["app"] == "d0"]
-                lines.append({"card": card, "variant": k, "pods": len(variants[k]["pods"]), "existing_nodes": n_ex,
+                lines.append({"card": gpu, "variant": k, "pods": len(variants[k]["pods"]), "existing_nodes": n_ex,
                               "pack_ms_median": statistics.median(pack[k]), "solve_ms_median": statistics.median(solve[k]),
                               "largest_deployment_on_existing": sum(1 for i in big if 0 <= d["assign"][i] < n_ex),
                               "largest_deployment_on_excluded": sum(1 for i in big if 0 <= d["assign"][i] < 5),
                               "hostname_words": rs.dims["hostname_words"]})
-    for x in lines:
-        print(json.dumps(x), flush=True)
-    if a.out:
-        Path(a.out).write_text("\n".join(json.dumps(x) for x in lines) + "\n")
+    emit(lines, a.out)
 
 
 if __name__ == "__main__":

@@ -8,20 +8,10 @@ prints one JSON line per run with the card name and power limit read in the same
     python tests/gpu_hostport_timing.py [--reps R] [--ports N] [--out FILE]
 """
 import argparse
-import json
-import statistics
-import subprocess
-import sys
-import time
-from pathlib import Path
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
-
-import fixtures as fx  # noqa: E402
-import hostport_problems as hp  # noqa: E402
-from conftest import load_pkg  # noqa: E402
+import fixtures as fx
+import hostport_problems as hp
+from timing_lib import card, emit, load_pkg, need_device, sweep_singles, timed
 
 
 def c5_dict(ports, nodes=5000, pods_per_node=10, types=1000):
@@ -41,16 +31,6 @@ def c5_dict(ports, nodes=5000, pods_per_node=10, types=1000):
     return fx.problem([], instance_types=its, provisioners=provs, nodes=ns, deriveCandidates=True)
 
 
-def timed(fn, reps):
-    fn()
-    ts, out = [], None
-    for _ in range(reps):
-        t0 = time.perf_counter()
-        out = fn()
-        ts.append(time.perf_counter() - t0)
-    return 1000 * statistics.median(ts), out
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
@@ -58,33 +38,23 @@ def main():
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     pkg = load_pkg()
-    if pkg.device_count() < 1:
-        raise SystemExit("needs a CUDA device")
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    need_device(pkg)
+    gpu = card()
     lines = []
     for ports in (a.ports, 0):
         d = c5_dict(ports)
         problem = pkg.Problem.from_dict(d)
-        line = {"card": card, "nodes": len(d["nodes"]), "bound_pods": sum(len(n["pods"]) for n in d["nodes"]),
+        line = {"card": gpu, "nodes": len(d["nodes"]), "bound_pods": sum(len(n["pods"]) for n in d["nodes"]),
                 "host_port_entries": len({e for n in d["nodes"] for p in n["pods"] for e in hp.pod_ports(p)})}
         multi = pkg.MultiNodeConsolidation(problem)
         line["multi_node_search_ms"], r = timed(multi.first_n_node_consolidation_option, a.reps)
         line["multi_node_action"], line["multi_node_removed"] = r["action"], r["nodes_removed"]
 
-        def sweep_all():
-            s = pkg.ClusterSession(problem)
-            acts = []
-            for lo in range(0, s.n_candidates, 64):
-                acts += [x[0] for x in s.probe_sets([[i] for i in range(lo, min(s.n_candidates, lo + 64))], False)]
-            s.close()
-            return acts
-        line["single_node_sweep_ms"], acts = timed(sweep_all, a.reps)
+        line["single_node_sweep_ms"], acts = timed(lambda: sweep_singles(pkg, problem), a.reps)
         line["single_node_candidates"] = len(acts)
         line["single_node_actionable"] = sum(1 for x in acts if x in (1, 2))
-        print(json.dumps(line), flush=True)
         lines.append(line)
-    if a.out:
-        Path(a.out).write_text("\n".join(json.dumps(x) for x in lines) + "\n")
+    emit(lines, a.out)
 
 
 if __name__ == "__main__":

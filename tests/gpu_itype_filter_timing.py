@@ -8,19 +8,11 @@ pods placed, and the card name and power limit read in the same run.
     python tests/gpu_itype_filter_timing.py [--reps R] [--out FILE]
 """
 import argparse
-import json
 import random
 import statistics
-import subprocess
-import sys
-from pathlib import Path
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
-
-import fixtures as fx  # noqa: E402
-from conftest import load_pkg  # noqa: E402
+import fixtures as fx
+from timing_lib import card, emit, load_pkg, need_device
 
 
 def c4_dict(via_itype, nodes=2000, deployments=20, pinned=6, types=400, seed=4):
@@ -55,9 +47,8 @@ def main():
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     pkg = load_pkg()
-    if pkg.device_count() < 1:
-        raise SystemExit("needs a CUDA device")
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    need_device(pkg)
+    gpu = card()
     variants = {"label": c4_dict(False), "itype": c4_dict(True)}
     problems = {k: pkg.Problem.from_dict(v) for k, v in variants.items()}
     pack = {k: [] for k in variants}
@@ -76,13 +67,10 @@ def main():
                 solve[k].append(ph["total_us"] / 1000)
             if rep == a.reps:
                 d = res.to_dict()
-                lines.append({"card": card, "variant": k, "pods": len(variants[k]["pods"]),
+                lines.append({"card": gpu, "variant": k, "pods": len(variants[k]["pods"]),
                               "pack_ms_median": statistics.median(pack[k]), "solve_ms_median": statistics.median(solve[k]),
                               "placed": sum(1 for x in d["assign"] if x >= 0), "itype_filter_terms": rs.dims["itype_filter_terms"]})
-    for x in lines:
-        print(json.dumps(x), flush=True)
-    if a.out:
-        Path(a.out).write_text("\n".join(json.dumps(x) for x in lines) + "\n")
+    emit(lines, a.out)
 
 
 if __name__ == "__main__":

@@ -8,20 +8,12 @@ end-to-end Solves, the pods placed, and the card name and power limit read in th
     python tests/gpu_many_key_timing.py [--reps R] [--out FILE]
 """
 import argparse
-import json
 import random
 import statistics
-import subprocess
-import sys
-from pathlib import Path
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
-
-import fixtures as fx  # noqa: E402
-import many_key_problems as mk  # noqa: E402
-from conftest import load_pkg  # noqa: E402
+import fixtures as fx
+import many_key_problems as mk
+from timing_lib import card, emit, load_pkg, need_device
 
 
 def c4_dict(n_keys, pods=100_000, deployments=20, seed=4):
@@ -51,9 +43,8 @@ def main():
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     pkg = load_pkg()
-    if pkg.device_count() < 1:
-        raise SystemExit("needs a CUDA device")
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    need_device(pkg)
+    gpu = card()
     variants = {"12keys": 12, "6keys": 6}
     problems = {k: pkg.Problem.from_dict(c4_dict(n)) for k, n in variants.items()}
     k1 = {k: [] for k in variants}
@@ -74,14 +65,11 @@ def main():
                 solve[k].append(ph["total_us"] / 1000)
             if rep == a.reps:
                 d = res.to_dict()
-                lines.append({"card": card, "variant": k, "pods": rs.dims["pods"], "types": rs.dims["types"], "keys": rs.dims["keys"],
+                lines.append({"card": gpu, "variant": k, "pods": rs.dims["pods"], "types": rs.dims["types"], "keys": rs.dims["keys"],
                               "k1_ms_median": statistics.median(k1[k]), "k2_ms_median": statistics.median(k2[k]),
                               "solve_ms_median": statistics.median(solve[k]),
                               "placed": sum(1 for x in d["assign"] if x >= 0), "new_nodes": len(d["newNodes"])})
-    for x in lines:
-        print(json.dumps(x), flush=True)
-    if a.out:
-        Path(a.out).write_text("\n".join(json.dumps(x) for x in lines) + "\n")
+    emit(lines, a.out)
 
 
 if __name__ == "__main__":

@@ -6,20 +6,13 @@ pods x (template, type) feasibility matrix, P x V x W32 words of 4 bytes.
     python tests/gpu_provisioner_timing.py [--pods N] [--reps R] [--out FILE]
 """
 import argparse
-import json
 import random
 import statistics
-import sys
 import time
-from pathlib import Path
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT / "tests"))
-sys.path.insert(0, str(ROOT))
-
-import fixtures as fx  # noqa: E402
-import provisioner_problems as pp  # noqa: E402
-from __graft_entry__ import load_pkg  # noqa: E402
+import fixtures as fx
+import provisioner_problems as pp
+from timing_lib import emit, load_pkg, need_device
 
 CPU = ["100m", "250m", "500m", "1", "1500m"]
 MEM = ["100Mi", "256Mi", "512Mi", "1Gi", "2Gi", "4Gi"]
@@ -61,8 +54,7 @@ def main():
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     pkg = load_pkg()
-    if pkg.device_count() < 1:
-        raise SystemExit("needs a CUDA device")
+    need_device(pkg)
     lines = []
     for v in (16, 32, 64):
         d = problem(a.pods, v)
@@ -90,11 +82,9 @@ def main():
                 "folded": rs.key_info(pp.PROVISIONER_NAME) is None, "new_nodes": res.num_new_nodes,
                 "k1_class_ms": statistics.median(k1c) / 1e3, "k1_ms": statistics.median(k1) / 1e3, "k2_ms": statistics.median(k2) / 1e3,
                 "e2e_solve_ms": statistics.median(e2e) / 1e3, "encode_ms": encode_ms, "F_MB": f_bytes / 1e6}
-        print(json.dumps(line), flush=True)
         lines.append(line)
         del rs
-    if a.out:
-        Path(a.out).write_text("\n".join(json.dumps(x) for x in lines) + "\n")
+    emit(lines, a.out)
 
 
 if __name__ == "__main__":

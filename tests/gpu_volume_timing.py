@@ -10,20 +10,11 @@ limit read in the same run.
     python tests/gpu_volume_timing.py [--reps R] [--deploy N] [--claims N] [--out FILE]
 """
 import argparse
-import json
 import statistics
-import subprocess
-import sys
-import time
-from pathlib import Path
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
-
-import fixtures as fx  # noqa: E402
-import volume_problems as vp  # noqa: E402
-from conftest import load_pkg  # noqa: E402
+import fixtures as fx
+from timing_lib import card, emit, load_pkg, need_device, sweep_singles, timed
+import volume_problems as vp
 
 
 def c5_dict(claims, deploy, nodes=5000, pods_per_node=10, types=1000):
@@ -62,16 +53,6 @@ def solve_dict(claims, nodes=2000, types=1000):
     return fx.problem(pods, instance_types=its, nodes=ns)
 
 
-def timed(fn, reps):
-    fn()
-    ts, out = [], None
-    for _ in range(reps):
-        t0 = time.perf_counter()
-        out = fn()
-        ts.append(time.perf_counter() - t0)
-    return 1000 * statistics.median(ts), out
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=3)
@@ -80,30 +61,21 @@ def main():
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     pkg = load_pkg()
-    if pkg.device_count() < 1:
-        raise SystemExit("needs a CUDA device")
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    need_device(pkg)
+    gpu = card()
     lines = []
     for claims in (True, False):
         d = c5_dict(claims, a.deploy)
         problem = pkg.Problem.from_dict(d)
-        line = {"card": card, "workload": "cluster", "nodes": len(d["nodes"]), "bound_pods": sum(len(n["pods"]) for n in d["nodes"]),
+        line = {"card": gpu, "workload": "cluster", "nodes": len(d["nodes"]), "bound_pods": sum(len(n["pods"]) for n in d["nodes"]),
                 "claims": sum(len(p.get("volumes", [])) for n in d["nodes"] for p in n["pods"])}
         multi = pkg.MultiNodeConsolidation(problem)
         line["multi_node_search_ms"], r = timed(multi.first_n_node_consolidation_option, a.reps)
         line["multi_node_action"], line["multi_node_removed"] = r["action"], r["nodes_removed"]
 
-        def sweep_all():
-            s = pkg.ClusterSession(problem)
-            acts = []
-            for lo in range(0, s.n_candidates, 64):
-                acts += [x[0] for x in s.probe_sets([[i] for i in range(lo, min(s.n_candidates, lo + 64))], False)]
-            s.close()
-            return acts
-        line["single_node_sweep_ms"], acts = timed(sweep_all, a.reps)
+        line["single_node_sweep_ms"], acts = timed(lambda: sweep_singles(pkg, problem), a.reps)
         line["single_node_candidates"] = len(acts)
         line["single_node_actionable"] = sum(1 for x in acts if x in (1, 2))
-        print(json.dumps(line), flush=True)
         lines.append(line)
     rs = pkg.ResidentSolve(pkg.Problem.from_dict(solve_dict(a.claims)))
     rs.set_count_visited(False)
@@ -115,13 +87,11 @@ def main():
         if i:
             k2.append(t["pack_us"]); tot.append(t["total_us"])
     e2e = statistics.median(rs.solve_e2e()[0] for _ in range(a.reps))
-    line = {"card": card, "workload": "solve", "existing": rs.dims["existing"], "pods": rs.dims["pods"], "classes": rs.dims["classes"],
+    line = {"card": gpu, "workload": "solve", "existing": rs.dims["existing"], "pods": rs.dims["pods"], "classes": rs.dims["classes"],
             "volume_claims": rs.dims["volume_claims"], "volume_ext_words": rs.dims["volume_ext_words"],
             "k2_ms": statistics.median(k2) / 1000, "resident_ms": statistics.median(tot) / 1000, "e2e_ms": e2e / 1000}
-    print(json.dumps(line), flush=True)
     lines.append(line)
-    if a.out:
-        Path(a.out).write_text("\n".join(json.dumps(x) for x in lines) + "\n")
+    emit(lines, a.out)
 
 
 if __name__ == "__main__":

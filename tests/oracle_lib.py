@@ -80,6 +80,23 @@ class Oracle:
         rc = self.lib.oracle_solve(problem.ptr, arr, len(candidates), result.ptr)
         return rc
 
+    def solve_dict(self, pkg, prob, candidates=(), fast=False):
+        """Solve a problem dict, in fast mode if asked (the literal path again afterwards) -> (problem, result)"""
+        problem = pkg.Problem.from_dict(prob)
+        res = pkg.Result()
+        self.lib.oracle_set_fast(int(fast))
+        try:
+            assert self.solve(problem, res, candidates) == 0, res.error
+        finally:
+            self.lib.oracle_set_fast(0)
+        return problem, res
+
+    def assert_fast_equals_literal(self, pkg, prob):
+        """Fast mode's shortcuts are result-neutral on this problem: digest and whole result -> (literal, fast) results"""
+        literal, fast = (self.solve_dict(pkg, prob, fast=f)[1] for f in (False, True))
+        assert fast.digest() == literal.digest() and fast.to_dict() == literal.to_dict()
+        return literal, fast
+
     def consolidate_probe(self, problem, count):
         """computeConsolidation over the `count` cheapest candidates -> (action, options)"""
         nopt = C.c_int()

@@ -144,17 +144,6 @@ def test_near_misses_are_refused(pkg, name, prob):
 
 
 # ---------------------------------------------------------------- the oracle's results
-def _solve(pkg, oracle, prob, fast=False):
-    problem = pkg.Problem.from_dict(prob)
-    res = pkg.Result()
-    oracle.lib.oracle_set_fast(1 if fast else 0)
-    try:
-        assert oracle.solve(problem, res) == 0, res.error
-    finally:
-        oracle.lib.oracle_set_fast(0)
-    return problem, res
-
-
 BATCHES = [(n, p) for n, p in CORPUS if p["pods"]]
 BIDS = [n for n, _ in BATCHES]
 
@@ -163,7 +152,7 @@ BIDS = [n for n, _ in BATCHES]
 def test_oracle_holds_every_node_to_its_overhead(pkg, oracle, name, prob):
     """every option of every new node holds the node's pods plus its template's overhead; every existing node holds its new
     pods plus the remaining overhead within what its bound pods leave"""
-    _, res = _solve(pkg, oracle, prob)
+    _, res = oracle.solve_dict(pkg, prob)
     d = res.to_dict()
     pods, its = prob["pods"], prob["instanceTypes"]
     overhead = dp.template_overhead(prob)
@@ -183,13 +172,13 @@ def test_oracle_holds_every_node_to_its_overhead(pkg, oracle, name, prob):
 
 
 def test_miscount_scenario_places_the_pod_on_n0(pkg, oracle):
-    _, res = _solve(pkg, oracle, dict(CORPUS)["miscount"])
+    _, res = oracle.solve_dict(pkg, dict(CORPUS)["miscount"])
     assert res.to_dict()["assign"] == [0]
 
 
 @pytest.mark.parametrize("name,prob", [b for b in BATCHES if not b[1].get("nodes")], ids=[n for n, p in BATCHES if not p.get("nodes")])
 def test_oracle_results_keep_the_invariants(pkg, oracle, name, prob):
-    problem, res = _solve(pkg, oracle, prob)
+    problem, res = oracle.solve_dict(pkg, prob)
     d = res.to_dict(brief=True)
     overhead = dp.template_overhead(prob)
     for nn in d["newNodes"]:  # the invariants sum the pods only: take the template's overhead off first
@@ -210,9 +199,7 @@ class _Brief:
 
 @pytest.mark.parametrize("name,prob", BATCHES, ids=BIDS)
 def test_oracle_fast_mode_equals_literal(pkg, oracle, name, prob):
-    _, literal = _solve(pkg, oracle, prob)
-    _, fast = _solve(pkg, oracle, prob, fast=True)
-    assert fast.to_dict() == literal.to_dict()
+    oracle.assert_fast_equals_literal(pkg, prob)
 
 
 KNOWN = dp.known_answers()
@@ -220,7 +207,7 @@ KNOWN = dp.known_answers()
 
 @pytest.mark.parametrize("name,prob,want", KNOWN, ids=[k[0] for k in KNOWN])
 def test_known_answers(pkg, oracle, name, prob, want):
-    _, res = _solve(pkg, oracle, prob)
+    _, res = oracle.solve_dict(pkg, prob)
     d = res.to_dict()
     assert d["assign"] == [0]
     it = next(i for i in prob["instanceTypes"] if i["name"] == launched_type(prob, d, 0))

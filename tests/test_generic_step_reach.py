@@ -23,17 +23,11 @@ def queue_order(prob):
     return sorted(range(len(prob["pods"])), key=key)
 
 
-def _solve(pkg, oracle, prob):
-    res = pkg.Result()
-    assert oracle.solve(pkg.Problem.from_dict(prob), res) == 0, res.error
-    return res.to_dict()
-
-
 def _prefix(pkg, oracle, prob, full, pos):
     """(prefix problem, its result): the pods before queue position pos; their placements equal the full run's"""
     order = queue_order(prob)[:pos]
     sub = dict(prob, pods=[prob["pods"][i] for i in order])
-    res = _solve(pkg, oracle, sub)
+    res = oracle.solve_dict(pkg, sub)[1].to_dict()
     assert res["assign"] == [full["assign"][i] for i in order]
     return sub, res
 
@@ -399,7 +393,7 @@ REACH = {
 @pytest.mark.parametrize("name", IDS)
 def test_scenario_reaches_its_mechanism(pkg, oracle, name):
     prob, facts = gp.build(name)
-    full = _solve(pkg, oracle, prob)
+    full = oracle.solve_dict(pkg, prob)[1].to_dict()
     REACH[name](pkg, oracle, prob, facts, full, name)
 
 
@@ -407,7 +401,7 @@ def test_scenario_reaches_its_mechanism(pkg, oracle, name):
 def test_every_option_holds_its_node(pkg, oracle, name):
     """independently of the oracle's Fits: every option of every new node holds the node's final requests"""
     prob, _ = gp.build(name)
-    full = _solve(pkg, oracle, prob)
+    full = oracle.solve_dict(pkg, prob)[1].to_dict()
     ds = ea.daemon_overhead(prob)
     for k, nn in enumerate(full["newNodes"]):
         pods = [prob["pods"][i] for i in nn["pods"]]
@@ -418,15 +412,4 @@ def test_every_option_holds_its_node(pkg, oracle, name):
 
 @pytest.mark.parametrize("name", IDS)
 def test_fast_mode_equals_literal(pkg, oracle, name):
-    problem = pkg.Problem.from_dict(gp.build(name)[0])
-    out = []
-    for fast in (0, 1):
-        oracle.lib.oracle_set_fast(fast)
-        try:
-            res = pkg.Result()
-            assert oracle.solve(problem, res) == 0, res.error
-        finally:
-            oracle.lib.oracle_set_fast(0)
-        out.append(res)
-    assert out[0].to_dict() == out[1].to_dict()
-    assert out[0].digest() == out[1].digest()
+    oracle.assert_fast_equals_literal(pkg, gp.build(name)[0])

@@ -7,6 +7,7 @@ import pytest
 import consolidation_answers as ca
 import fixtures as fx
 import run_problems
+from oracle_compare import compare_probes, compare_searches
 from ranking_answers import CASES as RANK_CASES, SINGLE
 
 pytestmark = pytest.mark.gpu
@@ -68,25 +69,12 @@ def test_batched_simulations_equal_the_oracle_probe_for_probe(pkg, oracle):
     prefixes = [list(range(c)) for c in range(1, n, max(1, n // 40))]
     singles = [[i] for i in range(0, n, 2)]
     assert len(prefixes) + len(singles) >= 64
-    got_multi = cs.probe_sets(prefixes, True)
-    got_single = cs.probe_sets(singles, False)
-    for s_, g in zip(prefixes, got_multi):
-        assert g == oracle.consolidate_probe(problem, len(s_)), len(s_)
-    for s_, g in zip(singles, got_single):
-        w = oracle.consolidate_single(problem, s_[0])
-        assert g == (w["action"], w["options"]), s_
+    compare_probes(pkg, oracle, problem, cs, prefixes, singles)
 
 
 @pytest.mark.parametrize("seed", [1, 2, 3])
 def test_searches_on_the_snapshot_equal_the_oracle(pkg, oracle, seed):
-    problem = pkg.Problem.synth(*pkg_synth_args(seed, 150, 8))
-    got = pkg.MultiNodeConsolidation(problem).first_n_node_consolidation_option()
-    want = oracle.consolidate(problem)
-    assert (got["action"], got["nodes_removed"], got["options"], got["probes"], got["probe_actions"]) == \
-           (want["action"], want["nodes_removed"], want["options"], want["probes"], want["probe_actions"])
-    got1 = pkg.SingleNodeConsolidation(problem).compute_command()
-    want1 = oracle.consolidate_single(problem)
-    assert (got1["action"], got1["node"], got1["options"]) == (want1["action"], want1["node"], want1["options"])
+    compare_searches(pkg, oracle, pkg.Problem.synth(*pkg_synth_args(seed, 150, 8)))
 
 
 def test_snapshot_with_provisioner_limits_and_uninitialised_nodes(pkg, oracle):
@@ -151,13 +139,7 @@ def test_snapshot_equals_oracle_on_wide_zone_clusters(pkg, oracle, seed, zones, 
     assert cs.resident
     n = cs.n_candidates
     assert n == 3 * zones
-    prefixes = [list(range(c)) for c in range(1, n + 1)]
-    for s_, g in zip(prefixes, cs.probe_sets(prefixes, True)):
-        assert g == oracle.consolidate_probe(problem, len(s_)), ("prefix", len(s_))
-    singles = [[i] for i in range(n)]
-    for s_, g in zip(singles, cs.probe_sets(singles, False)):
-        w = oracle.consolidate_single(problem, s_[0])
-        assert g == (w["action"], w["options"]), ("single", s_)
+    compare_probes(pkg, oracle, problem, cs, [list(range(c)) for c in range(1, n + 1)], [[i] for i in range(n)])
 
 
 @pytest.mark.parametrize("seed", [s for s in range(400) if _candidate_cluster(s)[1] >= 2][:60])
@@ -171,11 +153,5 @@ def test_snapshot_equals_oracle_on_random_clusters_with_topology(pkg, oracle, se
             pytest.skip(f"refused loudly: {e}")
         raise
     assert cs.resident
-    order = cs.candidate_nodes()
-    prefixes = [list(range(c)) for c in range(1, len(order) + 1)]
-    singles = [[i] for i in range(len(order))]
-    for s_, g in zip(prefixes, cs.probe_sets(prefixes, True)):
-        assert g == oracle.consolidate_probe(problem, len(s_)), ("prefix", len(s_))
-    for s_, g in zip(singles, cs.probe_sets(singles, False)):
-        w = oracle.consolidate_single(problem, s_[0])
-        assert g == (w["action"], w["options"]), ("single", s_)
+    n = cs.n_candidates
+    compare_probes(pkg, oracle, problem, cs, [list(range(c)) for c in range(1, n + 1)], [[i] for i in range(n)])

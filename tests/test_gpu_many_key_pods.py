@@ -6,8 +6,7 @@ groups is still refused at upload."""
 import pytest
 
 import many_key_problems as mk
-import validation_oracle as vo
-from oracle_compare import MODE_SWITCHES, compare, set_modes
+from oracle_compare import MODE_SWITCHES, compare, compare_cluster, compare_validation, set_modes
 
 pytestmark = pytest.mark.gpu
 
@@ -52,36 +51,8 @@ def test_nine_groups_are_refused_at_upload(pkg):
 
 
 def test_many_key_cluster_equals_oracle_probe_for_probe(pkg, oracle):
-    problem = pkg.Problem.from_dict(mk.cluster(0))
-    cs = pkg.ClusterSession(problem)
-    assert cs.resident
-    order = cs.candidate_nodes()
-    assert len(order) >= 2
-    prefixes = [list(range(c)) for c in range(1, len(order) + 1)]
-    for s_, g in zip(prefixes, cs.probe_sets(prefixes, True)):
-        assert g == oracle.consolidate_probe(problem, len(s_)), ("prefix", len(s_))
-    singles = [[i] for i in range(len(order))]
-    for s_, g in zip(singles, cs.probe_sets(singles, False)):
-        w = oracle.consolidate_single(problem, s_[0])
-        assert g == (w["action"], w["options"]), ("single", s_)
-    got = pkg.MultiNodeConsolidation(problem).first_n_node_consolidation_option()
-    want = oracle.consolidate(problem)
-    assert (got["action"], got["nodes_removed"], got["options"], got["probes"]) == \
-           (want["action"], want["nodes_removed"], want["options"], want["probes"])
-    one = pkg.SingleNodeConsolidation(problem).compute_command()
-    want1 = oracle.consolidate_single(problem)
-    assert (one["action"], one["node"], one["options"]) == (want1["action"], want1["node"], want1["options"])
+    compare_cluster(pkg, oracle, pkg.Problem.from_dict(mk.cluster(0)))
 
 
 def test_many_key_validation_equals_oracle(pkg, oracle):
-    b, a = mk.cluster(0), mk.after(0)
-    before, after = (b, pkg.Problem.from_dict(b)), (a, pkg.Problem.from_dict(a))
-    keys = ("action", "position", "node", "options", "validations", "failed_validation")
-    want = vo.single_compute_command(before, after)
-    for batch in (1, 64):
-        got = pkg.SingleNodeConsolidation(before[1]).compute_command(batch=batch, after=after[1])
-        assert {k: got[k] for k in keys} == {k: want[k] for k in keys}, batch
-    mkeys = ("action", "nodes_removed", "options", "probes", "probe_actions", "validations")
-    got_m = pkg.MultiNodeConsolidation(before[1]).compute_command(after[1])
-    want_m = vo.multi_compute_command(before, after)
-    assert {k: got_m[k] for k in mkeys} == {k: want_m[k] for k in mkeys}
+    compare_validation(pkg, mk.cluster(0), mk.after(0))

@@ -7,7 +7,7 @@ import pytest
 
 import exact_arith as ea
 import numeric_problems as nprob
-from oracle_compare import MODE_SWITCHES, compare, set_modes
+from oracle_compare import MODE_SWITCHES, compare, compare_cluster, set_modes
 from test_numeric_edges import same_costs
 
 pytestmark = pytest.mark.gpu
@@ -49,25 +49,7 @@ def test_sums_past_the_bound_are_refused(pkg, name, prob, answer):
 
 @pytest.mark.parametrize("kept", [0, 2])
 def test_limit_cluster_equals_oracle_probe_for_probe(pkg, oracle, kept):
-    problem = pkg.Problem.from_dict(nprob.limit_cluster(kept))
-    cs = pkg.ClusterSession(problem)
-    assert cs.resident
-    order = cs.candidate_nodes()
-    assert len(order) == 3
-    prefixes = [list(range(c)) for c in range(1, len(order) + 1)]
-    for s_, g in zip(prefixes, cs.probe_sets(prefixes, True)):
-        assert g == oracle.consolidate_probe(problem, len(s_)), ("prefix", len(s_))
-    singles = [[i] for i in range(len(order))]
-    for s_, g in zip(singles, cs.probe_sets(singles, False)):
-        w = oracle.consolidate_single(problem, s_[0])
-        assert g == (w["action"], w["options"]), ("single", s_)
-    got = pkg.MultiNodeConsolidation(problem).first_n_node_consolidation_option()
-    want = oracle.consolidate(problem)
-    assert (got["action"], got["nodes_removed"], got["options"], got["probes"]) == \
-           (want["action"], want["nodes_removed"], want["options"], want["probes"])
-    one = pkg.SingleNodeConsolidation(problem).compute_command()
-    want1 = oracle.consolidate_single(problem)
-    assert (one["action"], one["node"], one["options"]) == (want1["action"], want1["node"], want1["options"])
+    assert compare_cluster(pkg, oracle, pkg.Problem.from_dict(nprob.limit_cluster(kept)), 3).n_candidates == 3
 
 
 @pytest.mark.parametrize("name,prob", RANKING, ids=[r[0] for r in RANKING])

@@ -10,33 +10,19 @@ import validation_oracle as vo
 import validation_problems as vp
 import fixtures as fx
 import consolidation_answers as ca
+from oracle_compare import VALIDATION_KEYS, compare_validation
 
 pytestmark = pytest.mark.gpu
-
-KEYS = ("action", "position", "node", "options", "validations", "failed_validation")
-MKEYS = ("action", "nodes_removed", "options", "probes", "probe_actions", "validations")
 
 
 def _pp(pkg, d):
     return d, pkg.Problem.from_dict(d)
 
 
-def _compare(pkg, oracle, b, a, label):
-    before, after = _pp(pkg, b), _pp(pkg, a)
-    want = vo.single_compute_command(before, after)
-    for batch in (1, 64):
-        got = pkg.SingleNodeConsolidation(before[1]).compute_command(batch=batch, after=after[1])
-        assert {k: got[k] for k in KEYS} == {k: want[k] for k in KEYS}, (label, batch)
-    got_m = pkg.MultiNodeConsolidation(before[1]).compute_command(after[1])
-    want_m = vo.multi_compute_command(before, after)
-    assert {k: got_m[k] for k in MKEYS} == {k: want_m[k] for k in MKEYS}, label
-    return got, got_m
-
-
 @pytest.mark.parametrize("name,ref,build", va.CASES, ids=[c[0] for c in va.CASES])
 def test_known_answer_on_device(pkg, oracle, name, ref, build):
     (b, a), check = build()
-    check(*_compare(pkg, oracle, b, a, name))
+    check(*compare_validation(pkg, b, a, name))
 
 
 PAIRS = vp.pairs()
@@ -46,7 +32,7 @@ PAIRS = vp.pairs()
 def test_corpus_pair_on_device(pkg, oracle, i):
     name, b, a = PAIRS[i]
     try:
-        _compare(pkg, oracle, b, a, name)
+        compare_validation(pkg, b, a, name)
     except pkg.KschedError as e:
         if e.code == pkg.KSCHED_ERR_UNSUPPORTED:
             pytest.skip(f"refused loudly: {e}")
@@ -60,7 +46,7 @@ def test_single_node_shares_merge_on_device(pkg, oracle):
         sn = pkg.SingleNodeConsolidation(before[1])
         merged = pkg.merge_single_node_shares([sn.compute_command(0, n // 2, 64, after=after[1]), sn.compute_command(n // 2, -1, 64, after=after[1])])
         whole = sn.compute_command(batch=64, after=after[1])
-        assert {k: merged[k] for k in KEYS} == {k: whole[k] for k in KEYS}, name
+        assert {k: merged[k] for k in VALIDATION_KEYS} == {k: whole[k] for k in VALIDATION_KEYS}, name
 
 
 def test_cluster_validate_batches_of_64(pkg, oracle):
@@ -110,7 +96,7 @@ def test_refused_snapshot_validates_through_fresh_solves(pkg, oracle):
                    topologySpreadConstraints=[fx.spread(fx.HOSTNAME, {f"k{j}": "v"}) for j in range(10)])
     a["nodes"].append(ca.node_of_type("crowd", big, [crowd], 1.0))
     assert not pkg.ClusterSession(pkg.Problem.from_dict(a)).resident
-    got, got_m = _compare(pkg, oracle, b, a, "refused")
+    got, got_m = compare_validation(pkg, b, a, "refused")
     assert got["validations"] == [(0, True)]
 
 

@@ -5,7 +5,7 @@ import pytest
 
 import wide_problems as wp
 from fuzz_problems import random_problem_with_bounds
-from oracle_compare import compare
+from oracle_compare import compare, compare_cluster
 
 pytestmark = pytest.mark.gpu
 
@@ -18,25 +18,7 @@ def test_wide_problem_equals_oracle(pkg, oracle, name, prob):
 
 
 def test_wide_cluster_equals_oracle_probe_for_probe(pkg, oracle):
-    problem = pkg.Problem.from_dict(wp.cluster(0))
-    cs = pkg.ClusterSession(problem)
-    assert cs.resident
-    order = cs.candidate_nodes()
-    assert len(order) >= 2
-    prefixes = [list(range(c)) for c in range(1, len(order) + 1)]
-    for s_, g in zip(prefixes, cs.probe_sets(prefixes, True)):
-        assert g == oracle.consolidate_probe(problem, len(s_)), ("prefix", len(s_))
-    singles = [[i] for i in range(len(order))]
-    for s_, g in zip(singles, cs.probe_sets(singles, False)):
-        w = oracle.consolidate_single(problem, s_[0])
-        assert g == (w["action"], w["options"]), ("single", s_)
-    got = pkg.MultiNodeConsolidation(problem).first_n_node_consolidation_option()
-    want = oracle.consolidate(problem)
-    assert (got["action"], got["nodes_removed"], got["options"], got["probes"]) == \
-           (want["action"], want["nodes_removed"], want["options"], want["probes"])
-    one = pkg.SingleNodeConsolidation(problem).compute_command()
-    want1 = oracle.consolidate_single(problem)
-    assert (one["action"], one["node"], one["options"]) == (want1["action"], want1["node"], want1["options"])
+    compare_cluster(pkg, oracle, pkg.Problem.from_dict(wp.cluster(0)))
 
 
 def _wide_bound_seeds():

@@ -62,15 +62,9 @@ def test_cluster_candidates_keep_more_than_64_entries(pkg):
         assert rs.hostports() == kept and rs.dims["hostport_ext_words"] == _words(len(kept))
 
 
-def _solve(pkg, oracle, prob):
-    res = pkg.Result()
-    assert oracle.solve(pkg.Problem.from_dict(prob), res) == 0, res.error
-    return res.to_dict()
-
-
 @pytest.mark.parametrize("name,prob,table", CORPUS, ids=IDS)
 def test_oracle_never_puts_matching_ports_together(pkg, oracle, name, prob, table):
-    d = _solve(pkg, oracle, prob)
+    d = oracle.solve_dict(pkg, prob)[1].to_dict()
     assert hp.node_conflicts(prob, d) == []
     with_ports = [i for i, p in enumerate(prob["pods"]) if hp.pod_ports(p)]
     assert with_ports == [] or any(d["assign"][i] >= 0 for i in with_ports)
@@ -95,7 +89,7 @@ def test_entries_beyond_64_turn_pods_away(pkg, oracle, name, prob, table):
     """some pod that the oracle puts on an existing node once the entries from id 64 on are gone is turned away from that
     node, which holds such an entry matching one of its ports, and placed elsewhere or left unscheduled"""
     high = set(pkg.ResidentSolve(pkg.Problem.from_dict(prob)).hostports()[64:])
-    real, stripped = _solve(pkg, oracle, prob), _solve(pkg, oracle, _strip(prob, high))
+    real, stripped = oracle.solve_dict(pkg, prob)[1].to_dict(), oracle.solve_dict(pkg, _strip(prob, high))[1].to_dict()
     on, on_s = _on_existing(real), _on_existing(stripped)
     turned = 0
     for i, node in on_s.items():

@@ -12,12 +12,6 @@ IDS = [c[0] for c in CORPUS]
 TABLE = [c for c in CORPUS if c[2]]
 
 
-def _solve(pkg, oracle, prob):
-    res = pkg.Result()
-    assert oracle.solve(pkg.Problem.from_dict(prob), res) == 0, res.error
-    return res.to_dict()
-
-
 def _admitted(prob, reqs):
     """(admits a new node, existing slots admitted) of a list of requirements intersected (requirements.go:87-94); every
     provisioner-owned node is an existing slot in this corpus"""
@@ -93,24 +87,18 @@ def _check_placements(prob, res):
 
 @pytest.mark.parametrize("name,prob,table", CORPUS, ids=IDS)
 def test_oracle_places_pods_only_where_admitted(pkg, oracle, name, prob, table):
-    _check_placements(prob, _solve(pkg, oracle, prob))
+    _check_placements(prob, oracle.solve_dict(pkg, prob)[1].to_dict())
 
 
 @pytest.mark.parametrize("name,prob,table", CORPUS, ids=IDS)
 def test_oracle_fast_mode_equals_literal(pkg, oracle, name, prob, table):
-    literal = _solve(pkg, oracle, prob)
-    oracle.lib.oracle_set_fast(1)
-    try:
-        fast = _solve(pkg, oracle, prob)
-    finally:
-        oracle.lib.oracle_set_fast(0)
-    assert fast == literal
+    oracle.assert_fast_equals_literal(pkg, prob)
 
 
 def test_scenarios_cross_what_they_were_built_for(pkg, oracle):
     # In lists: the listed nodes fill (slots >= 64 used), the rest stay unscheduled and no new node opens for them
     prob = hn.in_list(5, 1)
-    d = _solve(pkg, oracle, prob)
+    d = oracle.solve_dict(pkg, prob)[1].to_dict()
     pinned = [i for i, p in enumerate(prob["pods"]) if p["labels"]["app"] == "pinned"]
     on = {d["existing"][d["assign"][i]]["node"] for i in pinned if 0 <= d["assign"][i] < len(d["existing"])}
     assert any(s >= 64 for s in on)
@@ -118,7 +106,7 @@ def test_scenarios_cross_what_they_were_built_for(pkg, oracle):
     assert all(d["assign"][i] < len(d["existing"]) for i in pinned)
     # NotIn: pods go to new nodes while the excluded nodes still have room
     prob = hn.not_in(2000, 3, 0)
-    d = _solve(pkg, oracle, prob)
+    d = oracle.solve_dict(pkg, prob)[1].to_dict()
     web = [i for i, p in enumerate(prob["pods"]) if p["labels"]["app"] == "web"]
     assert any(d["assign"][i] >= len(d["existing"]) for i in web)
     excluded = set(prob["pods"][web[0]]["nodeAffinity"]["required"][0][0]["values"])
@@ -126,13 +114,13 @@ def test_scenarios_cross_what_they_were_built_for(pkg, oracle):
                    prob["nodes"][d["existing"][d["assign"][i]]["node"]]["name"] in excluded for i in web)
     # selector a plus NotIn [a] admits nothing
     prob = hn.selector_and_affinity(0)
-    d = _solve(pkg, oracle, prob)
+    d = oracle.solve_dict(pkg, prob)[1].to_dict()
     assert all(d["assign"][i] < 0 for i, p in enumerate(prob["pods"]) if p["labels"]["app"] == "none")
     assert any(d["assign"][i] >= 0 for i, p in enumerate(prob["pods"]) if p["labels"]["app"] == "one")
     # hostname affinity: matching pods only on excluded nodes still bootstrap onto an admitted node (lists and the pair
     # form); a matching pod on an admitted node draws the pods there; the extra-domain flag is set for the unowned node
     prob = hn.affinity_lists(0)
-    d = _solve(pkg, oracle, prob)
+    d = oracle.solve_dict(pkg, prob)[1].to_dict()
     host = {i: prob["nodes"][d["existing"][a]["node"]]["name"] for i, a in enumerate(d["assign"]) if 0 <= a < len(d["existing"])}
     app = {i: p["labels"]["app"] for i, p in enumerate(prob["pods"])}
     assert {host[i] for i in host if app[i] == "a1"} and {host[i] for i in host if app[i] == "a1"} <= {"n-004", "n-005", "n-012"}
@@ -140,7 +128,7 @@ def test_scenarios_cross_what_they_were_built_for(pkg, oracle):
     assert {host[i] for i in host if app[i] == "a3"} == {"n-010"}
     # two terms: some pods land on the second list after the first is full
     prob = hn.two_terms(0)
-    d = _solve(pkg, oracle, prob)
+    d = oracle.solve_dict(pkg, prob)[1].to_dict()
     second = {n["name"] for n in prob["nodes"][5:8]}
     assert any(0 <= a < len(d["existing"]) and prob["nodes"][d["existing"][a]["node"]]["name"] in second for a in d["assign"])
 

@@ -12,12 +12,6 @@ CORPUS = itf.corpus()
 IDS = [c[0] for c in CORPUS]
 
 
-def _solve(pkg, oracle, prob):
-    res = pkg.Result()
-    assert oracle.solve(pkg.Problem.from_dict(prob), res) == 0, res.error
-    return res.to_dict()
-
-
 @pytest.mark.parametrize("name,prob,table", CORPUS, ids=IDS)
 def test_encoder_takes_the_scenario(pkg, name, prob, table):
     rs = pkg.ResidentSolve(pkg.Problem.from_dict(prob))
@@ -104,25 +98,19 @@ def _check_placements(prob, res):
 
 @pytest.mark.parametrize("name,prob,table", CORPUS, ids=IDS)
 def test_oracle_places_pods_only_where_admitted(pkg, oracle, name, prob, table):
-    _check_placements(prob, _solve(pkg, oracle, prob))
+    _check_placements(prob, oracle.solve_dict(pkg, prob)[1].to_dict())
 
 
 @pytest.mark.parametrize("name,prob,table", CORPUS, ids=IDS)
 def test_oracle_fast_mode_equals_literal(pkg, oracle, name, prob, table):
-    literal = _solve(pkg, oracle, prob)
-    oracle.lib.oracle_set_fast(1)
-    try:
-        fast = _solve(pkg, oracle, prob)
-    finally:
-        oracle.lib.oracle_set_fast(0)
-    assert fast == literal
+    oracle.assert_fast_equals_literal(pkg, prob)
 
 
 def test_narrowed_nodes_are_not_recorded(pkg, oracle):
     """the scenario reaches what it was built for: some small selector pods share a node with a pod that excluded the listed
     types, and some spread pods land on new nodes"""
     prob = itf.narrowed(0)
-    d = _solve(pkg, oracle, prob)
+    d = oracle.solve_dict(pkg, prob)[1].to_dict()
     n_ex = len(d["existing"])
     by_node = {}
     for i, a in enumerate(d["assign"]):

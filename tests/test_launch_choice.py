@@ -12,17 +12,10 @@ from fuzz_problems import random_problem
 ZONE, CT, ARCH = "topology.kubernetes.io/zone", "karpenter.sh/capacity-type", "kubernetes.io/arch"
 
 
-def _solve(pkg, oracle, prob):
-    problem = pkg.Problem.from_dict(prob)
-    res = pkg.Result()
-    assert oracle.solve(problem, res) == 0, res.error
-    return problem, res
-
-
 @pytest.mark.parametrize("seed", range(40))
 def test_oracle_launch_equals_python_restatement_and_encoded_table(pkg, oracle, seed):
     prob = random_problem(seed)
-    problem, res = _solve(pkg, oracle, prob)
+    problem, res = oracle.solve_dict(pkg, prob)
     d = res.to_dict()
     for node in d["newNodes"]:
         want = fx.launch(prob, node)
@@ -86,7 +79,7 @@ CASES = [
 def test_launches_on_one_of_the_cheapest_valid_instances(pkg, oracle, name, pod_kw, prov_kw, pred):
     its = _assorted()
     prob = fx.problem([fx.pod(**pod_kw)], instance_types=its, provisioners=[fx.provisioner(**prov_kw)])
-    problem, res = _solve(pkg, oracle, prob)
+    problem, res = oracle.solve_dict(pkg, prob)
     d = res.to_dict()
     assert d["assign"] == [0] and len(d["newNodes"]) == 1
     node = d["newNodes"][0]

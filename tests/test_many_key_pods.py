@@ -74,17 +74,6 @@ def resident(pkg, prob):
     return pkg.ResidentSolve(pkg.Problem.from_dict(prob), candidates=cands if not prob["pods"] else ())
 
 
-def _solve(pkg, oracle, prob, fast=False):
-    problem = pkg.Problem.from_dict(prob)
-    res = pkg.Result()
-    oracle.lib.oracle_set_fast(1 if fast else 0)
-    try:
-        assert oracle.solve(problem, res) == 0, res.error
-    finally:
-        oracle.lib.oracle_set_fast(0)
-    return problem, res
-
-
 def _many_key_pods(pkg, prob, d):
     """pods whose class at their final relaxation level was refused by the former count"""
     rs = pkg.ResidentSolve(pkg.Problem.from_dict(prob))
@@ -134,7 +123,7 @@ def test_seventeen_keys_are_refused(pkg):
 def test_oracle_places_many_key_classes_on_existing_in_flight_and_fresh_nodes(pkg, oracle):
     kinds = set()
     for name, prob in CORPUS:
-        _, res = _solve(pkg, oracle, prob)
+        _, res = oracle.solve_dict(pkg, prob)
         d = res.to_dict()
         many = _many_key_pods(pkg, prob, d)
         n_ex = len(d["existing"])
@@ -155,7 +144,7 @@ def test_grown_requirements_keep_in_pods_off_bare_nodes(pkg, oracle):
     pods never take a node without that custom key"""
     for seed in range(2):
         prob = mk.existing(seed)
-        _, res = _solve(pkg, oracle, prob)
+        _, res = oracle.solve_dict(pkg, prob)
         d = res.to_dict()
         n_ex = len(d["existing"])
         app = lambda i: prob["pods"][i]["labels"]["app"]
@@ -175,12 +164,10 @@ BATCHES = [(n, p) for n, p in CORPUS if not p.get("nodes")]
 
 @pytest.mark.parametrize("name,prob", BATCHES, ids=[n for n, _ in BATCHES])
 def test_oracle_results_keep_the_invariants(pkg, oracle, name, prob):
-    problem, res = _solve(pkg, oracle, prob)
+    problem, res = oracle.solve_dict(pkg, prob)
     pi.check(problem, res, n_zones=2 if name.startswith("inflight") else 3)
 
 
 @pytest.mark.parametrize("name,prob", CORPUS, ids=IDS)
 def test_oracle_fast_mode_equals_literal(pkg, oracle, name, prob):
-    _, literal = _solve(pkg, oracle, prob)
-    _, fast = _solve(pkg, oracle, prob, fast=True)
-    assert fast.to_dict() == literal.to_dict()
+    oracle.assert_fast_equals_literal(pkg, prob)

@@ -16,13 +16,6 @@ IDS = [c[0] for c in CORPUS]
 GOLDEN = Path(__file__).parent / "golden" / "zone_layout_digests.json"
 
 
-def _solve(pkg, oracle, prob):
-    problem = pkg.Problem.from_dict(prob)
-    res = pkg.Result()
-    assert oracle.solve(problem, res) == 0, res.error
-    return problem, res
-
-
 @pytest.mark.parametrize("name,prob,table", CORPUS, ids=IDS)
 def test_encoder_takes_the_scenario(pkg, name, prob, table):
     rs = pkg.ResidentSolve(pkg.Problem.from_dict(prob))
@@ -59,7 +52,7 @@ def test_more_than_64_pairs_is_refused(pkg):
 
 @pytest.mark.parametrize("name,prob,table", CORPUS, ids=IDS)
 def test_launch_choice_three_ways(pkg, oracle, name, prob, table):
-    problem, res = _solve(pkg, oracle, prob)
+    problem, res = oracle.solve_dict(pkg, prob)
     d = res.to_dict()
     for node in d["newNodes"]:
         got = node["launch"]
@@ -69,7 +62,7 @@ def test_launch_choice_three_ways(pkg, oracle, name, prob, table):
 
 @pytest.mark.parametrize("name,prob,table", CORPUS, ids=IDS)
 def test_every_option_has_an_admitted_offering(pkg, oracle, name, prob, table):
-    _, res = _solve(pkg, oracle, prob)
+    _, res = oracle.solve_dict(pkg, prob)
     for node in res.to_dict()["newNodes"]:
         assert node["options"]
         assert all(zp.has_offering(prob, node, i) for i in node["options"])
@@ -77,18 +70,12 @@ def test_every_option_has_an_admitted_offering(pkg, oracle, name, prob, table):
 
 @pytest.mark.parametrize("name,prob,table", CORPUS, ids=IDS)
 def test_oracle_fast_mode_equals_literal(pkg, oracle, name, prob, table):
-    literal = _solve(pkg, oracle, prob)[1].to_dict()
-    oracle.lib.oracle_set_fast(1)
-    try:
-        fast = _solve(pkg, oracle, prob)[1].to_dict()
-    finally:
-        oracle.lib.oracle_set_fast(0)
-    assert fast == literal
+    oracle.assert_fast_equals_literal(pkg, prob)
 
 
 def test_scenarios_cross_what_they_were_built_for(pkg, oracle):
     # the capacity-type typo: the plain pods schedule on one new node, the two typo pods do not
-    _, res = _solve(pkg, oracle, zp.ct_typo())
+    _, res = oracle.solve_dict(pkg, zp.ct_typo())
     d = res.to_dict()
     assert d["assign"][:5] == [d["assign"][0]] * 5 and d["assign"][0] >= 0 and d["assign"][5:] == [-1, -1]
     # a zone only a pod names pushes the last offered zone to id 16
@@ -96,7 +83,7 @@ def test_scenarios_cross_what_they_were_built_for(pkg, oracle):
     assert rs.dims["offering_slots"] == 16 and rs.key_info(fx.ZONE)["values"] == 17
     # Local-Zone pods land in their Local Zone
     prob = zp.local_pinned(0)
-    d = _solve(pkg, oracle, prob)[1].to_dict()
+    d = oracle.solve_dict(pkg, prob)[1].to_dict()
     lz = prob["pods"][33]["nodeSelector"][fx.ZONE]
     n_ex = len(d["existing"])
     nodes = {d["assign"][i] for i in range(33, 45)}

@@ -103,15 +103,9 @@ def test_more_than_four_limited_drivers_stay_refused(pkg):
     assert "more than 4 CSI drivers" in str(e.value)
 
 
-def _solve(pkg, oracle, prob):
-    res = pkg.Result()
-    assert oracle.solve(pkg.Problem.from_dict(prob), res) == 0, res.error
-    return res
-
-
 @pytest.mark.parametrize("name,prob,table", CORPUS, ids=IDS)
 def test_oracle_keeps_volume_limits(pkg, oracle, name, prob, table):
-    d = _solve(pkg, oracle, prob).to_dict()
+    d = oracle.solve_dict(pkg, prob)[1].to_dict()
     assert vp.volume_violations(prob, d) == []
     with_claims = [i for i, p in enumerate(prob["pods"]) if p.get("volumes")]
     assert any(d["assign"][i] >= 0 for i in with_claims)
@@ -119,11 +113,4 @@ def test_oracle_keeps_volume_limits(pkg, oracle, name, prob, table):
 
 @pytest.mark.parametrize("name,prob,table", CORPUS, ids=IDS)
 def test_oracle_fast_mode_equals_literal(pkg, oracle, name, prob, table):
-    out = []
-    for fast in (0, 1):
-        oracle.lib.oracle_set_fast(fast)
-        try:
-            out.append(_solve(pkg, oracle, prob))
-        finally:
-            oracle.lib.oracle_set_fast(0)
-    assert out[0].digest() == out[1].digest() and out[0].to_dict() == out[1].to_dict()
+    oracle.assert_fast_equals_literal(pkg, prob)

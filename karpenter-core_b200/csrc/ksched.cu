@@ -67,7 +67,10 @@ enum Counter : int {
   kCtrRunFresh, kCtrRunCalls, kCtrRunPlaced, kCtrRunBails, kCtrRunIneligible, kCtrRunLvPerPod, kCtrRunPerPod, kCtrRunLvFills,
   kCtrMaskBuildRefused, kCtrMaskUnpinnedSingle,
   kCtrPinSteps, kCtrPinPods, kCtrPinEndStaged, kCtrPinEndCount, kCtrPinEndKey, kCtrPinEndRefused, kCtrPinEndList,
-  kCtrRoundTripCycles, kCtrNoVariantStops, kCtrNoVariantTripCycles, kCtrVarStoreHits, kCtrVarStoreEntries,
+  kCtrRoundTripCycles,
+  kCtrNoVariantStops, kCtrStopRoomSlow, kCtrStopCapacity, kCtrStopOther,  // status-1 stops by StopCause (in that order)
+  kCtrNoVariantTripCycles, kCtrVarStoreHits, kCtrVarStoreEntries, kCtrRunCaptures,
+  kCtrRunDerives, kCtrRunDeriveCycles, kCtrRunDeriveRefused,  // variants derived inside a class run (run_derive)
   kCtrRoundCycles, kCtrRounds, kCtrRoundPods,
   kCtrStretchPinned, kCtrStretchFresh = kCtrStretchPinned + 16,  // round stretches by length 1..16
   kCtrMaskSteps = kCtrStretchFresh + 16, kCtrMaskMultiDomain, kCtrMaskRoundable,
@@ -1379,6 +1382,7 @@ static int run_pack(ksched_handle* h, int n_pods, int stop_new_nodes) {
   s.use_mask_run = std::getenv("KSCHED_NO_MASKRUN") ? 0 : 1;
   s.use_level_warp = std::getenv("KSCHED_NO_LEVELWARP") ? 0 : 1;
   s.use_varstore = std::getenv("KSCHED_NO_VARSTORE") ? 0 : 1;
+  s.use_run_derive = std::getenv("KSCHED_NO_RUNDERIVE") ? 0 : 1;
   s.use_round_stretch = std::getenv("KSCHED_NO_ROUNDSTRETCH") ? 0 : 1;
   s.use_fill_stretch = s.use_round_stretch && !std::getenv("KSCHED_NO_FILLSTRETCH") ? 1 : 0;
   // block size: the chain is latency-bound on ONE thread's commit; more warps only help when there are many candidate
@@ -1497,8 +1501,14 @@ static void print_pack_profile(const long long* counters) {
                   "write-back cycles=%lld | compactions=%lld slots=%lld cycles=%lld\n", c[kCtrRunActiveSum], c[kCtrRunEntryCycles],
           c[kCtrRunInputCycles], c[kCtrRunWbCycles], c[kCtrRunCompacts], c[kCtrRunCompactSlots], c[kCtrRunCompactCycles]);
   fprintf(stderr, "[pack profile] class_run round trips (status-1 stop -> entry of the next call that places pods): cycles=%lld | "
-                  "stops for want of a variant=%lld, their round trips' cycles=%lld | variant store: hits=%lld entries=%lld\n",
-          c[kCtrRoundTripCycles], c[kCtrNoVariantStops], c[kCtrNoVariantTripCycles], c[kCtrVarStoreHits], c[kCtrVarStoreEntries]);
+                  "stops for want of a variant=%lld, their round trips' cycles=%lld | variant store: hits=%lld entries=%lld | "
+                  "entry captures=%lld\n",
+          c[kCtrRoundTripCycles], c[kCtrNoVariantStops], c[kCtrNoVariantTripCycles], c[kCtrVarStoreHits], c[kCtrVarStoreEntries],
+          c[kCtrRunCaptures]);
+  fprintf(stderr, "[pack profile] class_run derivations of a missing variant=%lld cycles=%lld refused=%lld\n", c[kCtrRunDerives],
+          c[kCtrRunDeriveCycles], c[kCtrRunDeriveRefused]);
+  fprintf(stderr, "[pack profile] class_run status-1 stops by cause [no variant, kRoomSlow winner, capacity guard, other]=%lld,%lld,%lld,%lld\n",
+          c[kCtrNoVariantStops], c[kCtrStopRoomSlow], c[kCtrStopCapacity], c[kCtrStopOther]);
   fprintf(stderr, "[pack profile] mask run steps=%lld with >1 admissible domain=%lld round-able=%lld\n", c[kCtrMaskSteps], c[kCtrMaskMultiDomain],
           c[kCtrMaskRoundable]);
   fprintf(stderr, "[pack profile] mask run: build cycles=%lld (refused %lld) loop cycles=%lld pods=%lld entries=%lld\n", c[kCtrMaskBuildCycles],

@@ -411,6 +411,10 @@ struct LoopVars {
   // the step failed and depends on nothing but (class, placements so far, relaxations so far): no topology relation of
   // any kind, no relaxation left. pack_kernel requeues the following pods of the class without evaluating them again.
   int fail_memo;
+  // in: class_run asks for a fresh node only (run_derive): no in-flight node is tried, the pod is neither assigned nor
+  // recorded in the topology counters nor requeued, and the caller keeps its tick / seq. Out: n_new / n_active as the
+  // step would have left them.
+  int derive;
 };
 
 // ---- existing-node run ("water-fill") --------------------------------------------------------------------------------
@@ -843,7 +847,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
     // verifies the winner's instance-type options word-parallel and, if they survive, narrows them in place. A winner
     // whose options do not survive is excluded and the argmin is repeated (after kMaxExcl such failures every candidate is
     // checked in full by its own thread, which needs no verification).
-    if (!placed && n_active > 0) {
+    if (!placed && n_active > 0 && !L.derive) {
       int n_excl = 0;
       bool full_eval = false;
       const bool two_stage = pt_nonempty;  // topology-constrained pod
@@ -1042,7 +1046,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
     GK_T(kCtrGenCommit)
     // ------------------------------------------------------------ 3) open a new node, templates in weight order (scheduler.go:194-217)
     if (!placed) {
-      GK_C(kCtrGenFreshSteps)
+      if (!L.derive) { GK_C(kCtrGenFreshSteps) }
       const bool f_valid = s.use_F && (first_pass || s.relax_level[pod] == 0);  // K1's row is valid while the pod has its original class
       const uint32_t fpos = first_pass ? (uint32_t)fpos_first : s.pod_pos[pod];
       const bool no_column = f_valid && s.best[fpos] == kNoBest;  // no feasible (template, type) column at all
@@ -1212,8 +1216,10 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
             H.rejected(a) = KSCHED_NONE;
           }
           sh.placed_closed = closed ? 1 : 0;
-          s.assign[pod] = NE + n;
-          s.place_seq[pod] = seq;
+          if (!L.derive) {
+            s.assign[pod] = NE + n;
+            s.place_seq[pod] = seq;
+          }
           if (limits_active) {  // subtractMax (scheduler.go:273-290): largest capacity among the surviving options
             for (int r = 0; r < R; ++r) {
               if (!((tm.limit_present >> r) & 1)) continue;
@@ -1234,7 +1240,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
         ++tick;
         ++seq;
         __syncthreads();
-        if (has_topo) topo_record_block(s.nn_vals, s.nn_meta[n], MAXN, n, NE + n);  // Topology.Record, one relation per thread
+        if (has_topo && !L.derive) topo_record_block(s.nn_vals, s.nn_meta[n], MAXN, n, NE + n);  // Topology.Record, one relation per thread
         ++n_new;
         if (!sh.placed_closed) { L.fresh_valid = 1; L.fresh_a = n_active; L.fresh_cls = cls; ++n_active; }
         placed = true;
@@ -1243,7 +1249,7 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
       if (fatal) return;
     }
     GK_T(kCtrGenFresh)
-    if (!placed) gen_requeue(pod, has_topo, L);
+    if (!placed && !L.derive) gen_requeue(pod, has_topo, L);
   }
 
 // no requirement of the pod can change a node's requirements
@@ -1269,14 +1275,14 @@ __device__ __forceinline__ bool plain_pod_regs(const PodRegs& r) {
 //    plus, per spread key of the class, the node's admissible domains (`zv`);
 //  * a candidate is accepted here only when the verdict is EXACT and nothing but counters changes: requirements untouched
 //    (plain / absorbed classes) or a spread domain that is already pinned on the node - or that can be pinned without
-//    touching the option set (DevCatalog::pin_neutral). Any other winner, a pod that fails, or a fresh node of a shape not
-//    seen before in the run hands the pod to generic_step (status 1);
+//    touching the option set (DevCatalog::pin_neutral). Any other winner or a pod that fails hands the pod to generic_step
+//    (status 1); a fresh node of a shape not seen before in the run has its variant derived first (run_derive, status 3);
 //  * a node that becomes full is tombstoned (key = ~0) and the active list is compacted when the run ends; assignments
 //    are staged per queue chunk and stored coalesced;
 //  * fresh nodes replay a VARIANT: NewNode+Add for (class, template, resulting requirement masks) is a pure function
-//    when no provisioner limit is active (same argument as PackState::fd_*), so the node generic_step created last for
-//    this class is captured (options, masks, requests, Pareto front) and replayed for every later pod of the run whose
-//    spread domains come out the same.
+//    when no provisioner limit is active (same argument as PackState::fd_*), so a node generic_step created for this
+//    class (last before the run, or in derive mode for the run) is captured (options, masks, requests, Pareto front) and
+//    replayed for every later pod of the run whose spread domains come out the same.
 constexpr int kRunHost = 4;      // hostname-keyed relations of a run-eligible class
 constexpr int kRunMask = 2;      // spread relations over a mask key
 constexpr int kRunDom = 16;      // domains of such a key
@@ -1287,6 +1293,10 @@ constexpr int kRunW32 = 64;      // option words a variant holds (T <= 2048)
 constexpr int kRunWarps = kPackThreads / 32;
 constexpr int kRunChunk = 128;   // queue entries staged in shared memory at a time
 constexpr unsigned kRoomSlow = 0xFFFFu, kRoomMax = 0x7FFEu, kRpDead = 0x80000000u;
+// why a class run stopped with status 1 (profile: kCtrNoVariantStops + cause - 1): no variant for the fresh node's domain, a
+// winner whose verdict is not exact (kRoomSlow), a capacity guard (MAXN, kActCap, kTopoCap), anything else (a pin that is not
+// neutral, no admissible domain or hostname for a fresh node)
+enum StopCause : int { kStopNone, kStopNoVariant, kStopRoomSlow, kStopCapacity, kStopOther };
 constexpr size_t kRunArrayBytes = (size_t)kTopoCap * (kRunMask * 4 + kRunHost * 2) + (size_t)kActCap * 4;
 
 struct RunVariant {
@@ -1442,7 +1452,7 @@ struct M1Ctx {
                                       // leaves it when a pod pins it, fresh nodes are pinned), so it is the rest of the
                                       // segment the build sorted, and the pin step reads its next members without the links
   uint16_t ps[32];                    // pin step: the node of each pod; round stretch: the node of each (round, domain)
-  int out_adv, out_reason, out_tick, out_n_new, out_n_active;
+  int out_adv, out_reason, out_tick, out_n_new, out_n_active, out_why;  // out_why: StopCause of out_reason 1
   int n_fresh;                        // nodes created by this entry of the mask run: slot | variant << 16; their global
   uint32_t fr[kRunChunk];             // state (option words, requirement values, requests, ...) is stored by the CTA afterwards
 };
@@ -1452,9 +1462,16 @@ struct RunIO {
   int qi, head, qlen, tick, seq, n_active, n_new, parity;
   long long add_calls;
   int placed;        // pods this call consumed
-  int status;        // 0 the run ended (class change / end of the first pass); 1 the pod at qi needs generic_step; 2 class not eligible
+  int status;        // 0 the run ended (class change / end of the first pass); 1 the pod at qi needs generic_step; 2 class not
+                     // eligible; 3 the pod at qi needs a variant derived (see resume)
   int fresh_valid, fresh_a;  // in: generic_step has just created node slot fresh_a for fresh_cls (nothing happened since)
   uint32_t fresh_cls;
+  int staged;        // out: a variant was derived in the run (run_derive), so g_row and g_pt hold this class's row and topology
+  // status 3: the pod at qi needs a variant the run does not have. Nothing is written back: the pack loop derives the variant
+  // (run_derive) and re-enters with `resume`, and the run goes on from the state it left in shared memory and in these fields
+  // (its first queue position and seq, the staged chunk, the level parity, the mask-run flags, the pod derived for)
+  int resume;
+  int r_qi0, r_seq0, r_cb, r_buf, r_lvp, r_m1, r_derived;
 };
 __shared__ RunIO g_rio;
 
@@ -2149,19 +2166,21 @@ __device__ __forceinline__ int m1_pin_step(const RunEnv& e, int buf, M1Lane& l, 
 }
 
 // ---- single step: the pod goes to the head of list wl (key wkey); the per-pod loop's commit, relation by relation on the
-// first lanes. Returns 0, or the reason the walk ends: 1 the pod needs generic_step, 2 per-pod loop from the next pod on.
-__device__ __forceinline__ int m1_single(const RunEnv& e, int buf, M1Lane& l, M1Walk& w, unsigned long long wkey, int wl, bool allowed) {
+// first lanes. Returns 0, or the reason the walk ends: 1 the pod needs generic_step (why: StopCause), 2 per-pod loop from the
+// next pod on.
+__device__ __forceinline__ int m1_single(const RunEnv& e, int buf, M1Lane& l, M1Walk& w, unsigned long long wkey, int wl, bool allowed,
+                                         int& why) {
   const PackState& s = g_k2.st; (void)s;  // (c: the pod count below)
   RunCtx& rc = g_rc;
   const int L = l.L;
   const int a = __shfl_sync(kFull, l.h, wl);
   const uint32_t rp = __shfl_sync(kFull, l.hr, wl);
-  if ((rp & 0xFFFF) == kRoomSlow) return 1;  // the winner needs the full evaluation
+  if ((rp & 0xFFFF) == kRoomSlow) { why = kStopRoomSlow; return 1; }  // the winner needs the full evaluation
   int d = wl;
   const bool pin = wl == kM1Dom;
   if (pin) {  // the placement pins the node's domain: fewest pods, lowest id among the admissible ones (run_pick)
     d = warp_pick(allowed, w.cnt_d);
-    if (!((rc.m_neutral[0] >> d) & 1) || !((e.zv[a] & (1u << 17)) || rc.m_wk[0])) return 1;
+    if (!((rc.m_neutral[0] >> d) & 1) || !((e.zv[a] & (1u << 17)) || rc.m_wk[0])) { why = kStopOther; return 1; }
 #ifdef KSCHED_PROFILE_PACK
     if (L == 0) s.counters[kCtrMaskUnpinnedSingle] += 1;
 #endif
@@ -2197,20 +2216,20 @@ __device__ __forceinline__ int m1_single(const RunEnv& e, int buf, M1Lane& l, M1
 }
 
 // ---- single step when nobody accepts: NewNode + Add replayed from the variant of the domain a fresh node gets. Returns 0,
-// or 1 when the pod needs generic_step (novar: for want of a variant).
-__device__ __forceinline__ int m1_single_fresh(const RunEnv& e, int buf, M1Lane& l, M1Walk& w, unsigned okm, int& novar) {
+// or 1 when the pod needs generic_step (why: StopCause).
+__device__ __forceinline__ int m1_single_fresh(const RunEnv& e, int buf, M1Lane& l, M1Walk& w, unsigned okm, int& why) {
   RunCtx& rc = g_rc;
   const int L = l.L;
-  if (w.lnew >= e.MAXN || w.lact >= kActCap || w.lact >= kTopoCap) return 1;
+  if (w.lnew >= e.MAXN || w.lact >= kActCap || w.lact >= kTopoCap) { why = kStopCapacity; return 1; }
   bool ok = true;
   for (int j = 0; j < e.n_host; ++j) ok = ok && rc.h_lim[j] >= 0;
   const unsigned cand = rc.m_tallow[0] & okm;
-  if (!ok || !cand) return 1;
+  if (!ok || !cand) { why = kStopOther; return 1; }
   const int fd = warp_pick((cand >> L) & 1, w.cnt_d);  // (cand is a subset of okm: lanes below kM1Dom)
   int vi = run_ring_find(rc, 1, fd, 0);
   if (vi < 0 && rc.vs_ok && !((w.fr_used >> rc.var_next) & 1))
     vi = vs_fetch(rc, e.cls, vs_pattern(1, rc.m_key, fd, 0), L);
-  if (vi < 0) { novar = 1; return 1; }
+  if (vi < 0) { why = kStopNoVariant; return 1; }
   const RunVariant& v = rc.var[vi];
   w.fr_used |= 1u << vi;
   if (L < e.n_host && rc.h_times[L]) rc.h_inc[L] = rc.h_inc[L] + 1;
@@ -2227,7 +2246,7 @@ __device__ __forceinline__ int m1_single_fresh(const RunEnv& e, int buf, M1Lane&
 
 // ---- mask run, warp 0's steps from staged entry i on: each pod's node is the smallest head key over the lists of the
 // admissible domains. The outcome goes to g_m1.out_*.
-__device__ __forceinline__ void m1_walk(const RunEnv& e, int buf, int i, int qlen, int tick, int n_new, int n_active, int& novar) {
+__device__ __forceinline__ void m1_walk(const RunEnv& e, int buf, int i, int qlen, int tick, int n_new, int n_active, int& why) {
   KS_K2
   RunCtx& rc = g_rc;
   M1Ctx& m1 = g_m1;
@@ -2292,15 +2311,15 @@ __device__ __forceinline__ void m1_walk(const RunEnv& e, int buf, int i, int qle
           continue;
         }
       }
-      reason = m1_single(e, buf, l, w, wkey, wl, allowed);
-    } else reason = m1_single_fresh(e, buf, l, w, okm, novar);
+      reason = m1_single(e, buf, l, w, wkey, wl, allowed, why);
+    } else reason = m1_single_fresh(e, buf, l, w, okm, why);
     if (reason) break;
   }
   __syncwarp();
   // every warp's copy of the spread counters follows (the per-pod loop and the write-back read them)
   if (L < kM1Dom) for (int wi = 0; wi < nwarps; ++wi) rc.cnt[wi][0][L] = w.cnt_d;
   if (L < kM1Lists) m1.head[L] = l.h >= 0 ? (uint16_t)l.h : kM1None;
-  if (L == 0) { m1.out_adv = w.li - i; m1.out_reason = reason; m1.out_tick = w.ltick; m1.out_n_new = w.lnew; m1.out_n_active = w.lact; m1.n_fresh = w.nfr; }
+  if (L == 0) { m1.out_adv = w.li - i; m1.out_reason = reason; m1.out_tick = w.ltick; m1.out_n_new = w.lnew; m1.out_n_active = w.lact; m1.n_fresh = w.nfr; m1.out_why = why; }
 }
 
 // ---- mask run, fresh-node store (block): the global state of the nodes the walk created, 64 words per node across the CTA
@@ -2472,8 +2491,9 @@ __device__ __forceinline__ int run_level_block(const RunEnv& e, int buf, int i, 
 
 // ---- per-pod argmin step: the node the reference's scan takes, by a block argmin on the order key over the accepting
 // nodes (their admissible domains included), committed by its owner. Returns 0 when the pod is placed, 1 when the winner
-// needs the full evaluation, 2 when nobody accepts; okm0 / okm1: the admissible domains of each spread relation.
-__device__ __forceinline__ int run_argmin_step(const RunEnv& e, int buf, int i, int n_active, int& tick, int& parity, uint32_t& okm0, uint32_t& okm1) {
+// needs the full evaluation (why: StopCause), 2 when nobody accepts; okm0 / okm1: the admissible domains of each spread relation.
+__device__ __forceinline__ int run_argmin_step(const RunEnv& e, int buf, int i, int n_active, int& tick, int& parity, uint32_t& okm0, uint32_t& okm1,
+                                               int& why) {
   RunCtx& rc = g_rc;
   HotSmem* hs = e.hs;
   const int tid = threadIdx.x, T = blockDim.x, lane = tid & 31, warp = tid >> 5, nwarps = T >> 5;
@@ -2501,10 +2521,10 @@ __device__ __forceinline__ int run_argmin_step(const RunEnv& e, int buf, int i, 
     if (n_mask > 1) { z1 = e.zv[kTopoCap + a]; ok = ok && (z1 & okm1) != 0; }
     if (ok) { mine = key; best_a = a; best_rp = rp; best_z0 = z0; best_z1 = z1; }
   }
-  // payload of this thread's candidate: slot | slow << 11 | pin bits << 13 | domains << 15 / 19
+  // payload of this thread's candidate: slot | slow << 11 | inexact room << 12 | pin bits << 13 | domains << 15 / 19
   unsigned pay = (unsigned)best_a;
   if (mine != ~0ull) {
-    if ((best_rp & 0xFFFF) == kRoomSlow) pay |= 1u << 11;
+    if ((best_rp & 0xFFFF) == kRoomSlow) pay |= 3u << 11;
 #pragma unroll
     for (int j = 0; j < kRunMask; ++j) {
       if (j >= n_mask) break;
@@ -2531,7 +2551,7 @@ __device__ __forceinline__ int run_argmin_step(const RunEnv& e, int buf, int i, 
   if (wkey == ~0ull) return 2;
   const unsigned src = __ballot_sync(0xffffffffu, rk == wkey);
   const unsigned wp = __shfl_sync(0xffffffffu, rp_l, __ffs(src) - 1);
-  if (wp & (1u << 11)) return 1;  // the winner needs the full evaluation
+  if (wp & (1u << 11)) { why = (wp >> 12) & 1 ? kStopRoomSlow : kStopOther; return 1; }  // the winner needs the full evaluation
   const int fd0 = (wp >> 15) & 0xF, fd1 = (wp >> 19) & 0xF;
   if (mine == wkey) {  // the owner commits its node: a handful of shared-memory stores
     const int a = best_a;
@@ -2556,14 +2576,14 @@ __device__ __forceinline__ int run_argmin_step(const RunEnv& e, int buf, int i, 
 // created from). Fill step on the fresh node: it takes `cap` further pods of the class while it is the only accepting node
 // and then refuses (room 0 or a hostname limit reached). With an exact cap the run needs F such nodes in a row, m = 1 + cap
 // pods each: all of them are created in this step, one per thread (slot a belongs to thread a % T as everywhere). Returns
-// false when the pod needs generic_step (novar: for want of a variant); else `adv` pods are placed.
+// false when the pod needs generic_step (why: StopCause); else `adv` pods are placed.
 __device__ __forceinline__ bool run_fresh_step(const RunEnv& e, int buf, int i, int k_avail, bool lvl, uint32_t okm0, uint32_t okm1,
-                                               int& tick, int& n_new, int& n_active, int& adv, int& novar) {
+                                               int& tick, int& n_new, int& n_active, int& adv, int& why) {
   KS_K2
   RunCtx& rc = g_rc;
   const int tid = threadIdx.x, T = blockDim.x, lane = tid & 31, warp = tid >> 5;
   const int n_mask = e.n_mask, MAXN = e.MAXN;
-  if (n_new >= MAXN || n_active >= kActCap || (e.topo && n_active >= kTopoCap)) return false;
+  if (n_new >= MAXN || n_active >= kActCap || (e.topo && n_active >= kTopoCap)) { why = kStopCapacity; return false; }
   bool ok = true;
 #pragma unroll
   for (int j = 0; j < kRunHost; ++j) ok = ok && (j >= e.n_host || rc.h_lim[j] >= 0);  // a fresh hostname has count 0
@@ -2587,7 +2607,7 @@ __device__ __forceinline__ bool run_fresh_step(const RunEnv& e, int buf, int i, 
     __syncthreads();
     vi = rc.vs_got;
   }
-  if (vi < 0) { novar = ok; return false; }
+  if (vi < 0) { why = ok ? kStopNoVariant : kStopOther; return false; }
   const RunVariant& v = rc.var[vi];
   int cap = 0, F = 1;
   bool cap_exact = false;
@@ -2642,6 +2662,129 @@ __device__ __forceinline__ bool run_fresh_step(const RunEnv& e, int buf, int i, 
   return true;
 }
 
+// ---- capture node slot a (node hs->node[a]), which the generic step opened for the run's class with one pod, as a
+// fresh-node variant: into the ring and, when the class shares, into the store. zv / rpv hold the slot's per-run inputs.
+// Returns the ring slot, or -1 when the node does not pin one exact domain per mask relation or the ring already holds a
+// variant of its template and domains. Block-wide.
+__device__ __forceinline__ int run_capture(const HotSmem* hs, const uint32_t* zv, const uint32_t* rpv, int a, int n_mask, unsigned cls) {
+  KS_K2
+  RunCtx& rc = g_rc;
+  const int tid = threadIdx.x, T = blockDim.x, lane = tid & 31, warp = tid >> 5;
+  const int MAXN = s.max_new, W32 = c.W32, n = hs->node[a];
+  int dom[kRunMask] = {0, 0};
+  bool ok = true;
+#pragma unroll
+  for (int j = 0; j < kRunMask; ++j) {
+    if (j >= n_mask) continue;
+    const uint32_t z = zv[j * kTopoCap + a], v = z & 0xFFFF;
+    if (!v || (v & (v - 1)) || !(z & (1u << 16))) ok = false;
+    else dom[j] = __ffs(v) - 1;
+  }
+  for (int i = 0; i < rc.n_var && ok; ++i) {
+    bool same = (rc.var[i].fl >> 8) == (hs->flags[a] >> 8);
+#pragma unroll
+    for (int j = 0; j < kRunMask; ++j) same = same && (j >= n_mask || rc.var[i].dom[j] == dom[j]);
+    if (same) ok = false;  // already known
+  }
+  const int slot = rc.var_next;  // read BEFORE the barrier: thread 0 moves it while the others still copy (racecheck warning, round 2)
+  __syncthreads();  // rc.n_var / var_next read by everybody before thread 0 moves them
+  if (!ok) return -1;
+  RunVariant& v = rc.var[slot];
+  for (int w = tid; w < W32; w += T) v.opts[w] = s.nn_opts[(size_t)w * MAXN + n];
+  if (tid < KSCHED_MAX_KEYS) v.vals[tid] = tid < c.n_keys ? s.nn_vals[(size_t)tid * MAXN + n] : 0;
+  if (tid == 0) {
+    v.meta = s.nn_meta[n];
+    for (int r = 0; r < KSCHED_MAX_RES; ++r) v.q[r] = r < kHotRes ? hs->q[r][a] : s.nn_req[(size_t)r * MAXN + n];
+    for (int r = 0; r < kHotRes; ++r) { v.b1[r] = hs->bound[r][a]; v.b2[r] = hs->bound2[r][a]; }
+    v.qp = s.nn_req_present[n];
+    v.fl = hs->flags[a];
+    v.rp = rpv[a] & (kRpDead | 0xFFFF);
+    for (int j = 0; j < kRunMask; ++j) v.dom[j] = (uint8_t)dom[j];
+    rc.var_next = (slot + 1) % kRunVariants;
+    if (rc.n_var < kRunVariants) rc.n_var++;
+  }
+  __syncthreads();
+  // into the store (not looked up first: a class captures a variant only after a miss, so duplicates are rare and
+  // harmless, and the capture stays free of dependent loads)
+  if (warp == 0 && rc.vs_ok && rc.vs_n < kVarStore) {
+    const uint32_t pat = vs_pattern(n_mask, rc.m_key, dom[0], dom[1]);
+    const int e = rc.vs_n;
+    VarStoreEntry& d = s.vstore[e];
+    const uint32_t* src = reinterpret_cast<const uint32_t*>(&rc.var[slot]);
+    uint32_t* dst = reinterpret_cast<uint32_t*>(&d.v);
+    for (int w = lane; w < (int)(sizeof(RunVariant) / 4); w += 32) dst[w] = src[w];
+    __syncwarp();
+    if (lane == 0) {
+      d.sig = rc.sig; d.pat = pat; d.cls = cls;
+      d.v.rp = rc.var[slot].rp & 0xFFFF;
+      rc.vs_tag[e] = vs_tag(rc.sig, pat);
+      rc.vs_n = e + 1;
+#ifdef KSCHED_PROFILE_PACK
+      s.counters[kCtrVarStoreEntries] += 1;
+#endif
+    }
+    __syncwarp();
+  }
+  __syncthreads();  // the ring slot and the store entry are complete
+  return slot;
+}
+
+// ---- derive the variant a run is missing for the fresh node of the pod at FFD position fpos: the generic step's
+// NewNode + Add (generic_step, derive mode) opens node n_new at slot n_active as the step would open it for this pod, from
+// the topology counts as they stand (the run's counts of its mask relations are stored first, as its write-back stores
+// them), and the node is captured (run_capture). Its slot and node stay unused: the run replays the variant into them.
+// Returns the ring slot, or -1 (the pod fails, or the node closes at once, pins no single domain or is known already).
+// Block-wide; the guards of a capture (no provisioner limit, W32 <= kRunW32) and the run's capacity guards hold.
+__device__ __noinline__ int run_derive(const PodRegs& first_in, int fpos, int n_new, int n_active, int tick, int seq, int parity) {
+  KS_K2
+  RunCtx& rc = g_rc;
+  HotSmem* hs = reinterpret_cast<HotSmem*>(dyn_smem);
+  uint32_t* zv = reinterpret_cast<uint32_t*>(dyn_smem + sizeof(HotSmem) + s.run_off);
+  uint32_t* rpv = zv + (size_t)kRunMask * kTopoCap;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int n_mask = rc.n_mask, n_host = rc.n_host, MAXN = s.max_new;
+  for (int j = 0; j < n_mask; ++j)
+    if (rc.m_rec[j] && warp == 0 && lane < kRunDom && ((rc.m_registered[j] >> lane) & 1)) s.grp_cnt[(size_t)rc.m_group[j] * 64 + lane] = rc.cnt[0][j][lane];
+  if (tid == 0) g_rio.staged = 1;
+  int fatal = 0;
+  uint32_t epoch = 0;
+  bool pt_nonempty = true;  // g_pt is built for the class whatever it holds now
+  long long nodes_visited = 0;
+  LoopVars L{0, 0, n_new, n_active, tick, seq, parity, fatal, epoch, pt_nonempty, nodes_visited, KSCHED_NONE, KSCHED_NONE, 0, 0, KSCHED_NONE, 0, 1};
+  generic_step<false>(first_in, true, fpos, L);  // (run classes request no ext resource)
+  if (L.n_new != n_new + 1 || L.n_active != n_active + 1) return -1;  // no node, or one that closed at once
+  const int a = n_active, n = n_new;
+  if (tid == 0) {  // the slot's per-run inputs as class_run's entry computes them (its hostname counts: the relations' times)
+    long long p_req[kHotRes];
+    for (int r = 0; r < kHotRes; ++r) p_req[r] = first_in.req[r];
+    unsigned rm = run_room(hs, a, p_req, first_in.res, c.n_res < kHotRes ? c.n_res : kHotRes);
+    for (int j = 0; j < n_host; ++j) if ((int)rc.h_times[j] > rc.h_lim[j]) rm |= kRpDead;
+    rpv[a] = rm;
+    const uint64_t meta = s.nn_meta[n];
+    for (int j = 0; j < n_mask; ++j) {
+      const int k = rc.m_key[j];
+      const Req r = load_soa(s.nn_vals, meta, MAXN, n, k);
+      const uint32_t allowed = (uint32_t)(r.present ? ksched::req_allowed(r, c.keys[k].dict_mask, key_meta(c, k)) : c.keys[k].dict_mask);
+      zv[j * kTopoCap + a] = allowed | ((r.present && !r.complement) ? 1u << 16 : 0) | (r.present ? 1u << 17 : 0);
+    }
+  }
+  __syncthreads();
+  return run_capture(hs, zv, rpv, a, n_mask, rc.cls);
+}
+
+// run_derive for class_run's loop: true when the variant is in the ring (profile: derivations, their cycles, refusals)
+__device__ __forceinline__ bool run_derive_at(const PodRegs& first_in, int fpos, int n_new, int n_active, int tick, int seq, int parity) {
+#ifdef KSCHED_PROFILE_PACK
+  const long long t0 = clock64();
+#endif
+  const int vi = run_derive(first_in, fpos, n_new, n_active, tick, seq, parity);
+#ifdef KSCHED_PROFILE_PACK
+  KS_K2
+  if (threadIdx.x == 0) { s.counters[kCtrRunDerives] += 1; s.counters[kCtrRunDeriveCycles] += clock64() - t0; s.counters[kCtrRunDeriveRefused] += vi < 0; }
+#endif
+  return vi >= 0;
+}
+
 __device__ __noinline__ void class_run(const PodRegs& first_in) {
   KS_K2
   RunCtx& rc = g_rc;
@@ -2670,11 +2813,12 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
   const bool plain = plain_pod_regs(first_in);
   const bool simple = !topo;
   const uint32_t topo_begin = first_in.topo_begin, topo_end = first_in.topo_end;
-  const int qi0 = io.qi, seq0 = io.seq;
-  int qi = qi0, qlen = io.qlen, tick = io.tick, n_active = io.n_active, n_new = io.n_new, parity = io.parity;
+  const bool resume = io.resume;
+  const int qi0 = resume ? io.r_qi0 : io.qi, seq0 = resume ? io.r_seq0 : io.seq;
+  int qi = io.qi, qlen = io.qlen, tick = io.tick, n_active = io.n_active, n_new = io.n_new, parity = io.parity;
   const int fresh_valid = io.fresh_valid && io.fresh_cls == cls, fresh_a = io.fresh_a;
   const int CH = T < kRunChunk ? T : kRunChunk;  // queue entries staged at a time: one per thread
-  if (tid == 0) { rc.q_end[0] = CH; rc.q_end[1] = CH; rc.lv_cnt[0] = 0; rc.lv_cnt[1] = 0; }  // (nobody reads these outside class_run)
+  if (tid == 0 && !resume) { rc.q_end[0] = CH; rc.q_end[1] = CH; rc.lv_cnt[0] = 0; rc.lv_cnt[1] = 0; }  // (nobody reads these outside class_run)
   const bool new_cls = rc.cls != cls;  // read BEFORE the barrier: thread 0 rewrites rc.cls right after it (racecheck, round 2)
   __syncthreads();  // everybody has read g_rio; earlier readers of g_rc are done
 
@@ -2727,6 +2871,9 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
   }
   if (!rc.eligible || (topo && n_active > kTopoCap)) {
     if (tid == 0) { io.status = rc.eligible ? 1 : 2; io.placed = 0; io.parity = parity; }
+#ifdef KSCHED_PROFILE_PACK
+    if (tid == 0 && rc.eligible) s.counters[kCtrStopCapacity] += 1;
+#endif
     __syncthreads();
     return;
   }
@@ -2734,7 +2881,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
 
   // ---- queue staging: the next CH (pod, class) entries; the chunk after them is fetched into registers meanwhile
   const ksched_pod_row* ffd_rows = reinterpret_cast<const ksched_pod_row*>(s.rows);
-  int cb = qi, buf = 0;
+  int cb = resume ? io.r_cb : qi, buf = resume ? io.r_buf : 0;
   uint32_t nx_pod = 0, nx_cls = KSCHED_NONE;
   auto stage = [&](int b, uint32_t pd, uint32_t pc) {  // thread tid < CH: entry cb + tid into buffer b, entry cb + CH + tid into registers
     rc.q_pod[b][tid] = pd; rc.q_cls[b][tid] = pc;
@@ -2744,15 +2891,19 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
     nx_cls = KSCHED_NONE;
     if (idx2 < s.n_pods) { nx_pod = s.order[idx2]; nx_cls = (uint32_t)ffd_rows[idx2].reserved; }
   };
-  if (tid < CH) {
+  if (tid < CH && resume) {  // the staged chunk is in place: the one after it into registers
+    const int idx2 = cb + CH + tid;
+    if (idx2 < s.n_pods) { nx_pod = s.order[idx2]; nx_cls = (uint32_t)ffd_rows[idx2].reserved; }
+  } else if (tid < CH) {
     const int idx = cb + tid;
     const bool in = idx < s.n_pods;
     stage(0, in ? s.order[idx] : 0, in ? (uint32_t)ffd_rows[idx].reserved : KSCHED_NONE);
   }
-  // ---- per-run state: spread counters (one copy per warp), per-node inputs (each thread fills the slots it owns)
-  if (tid == 0) rc.tomb = 0;
-  if (tid < kRunHost) rc.h_inc[tid] = 0;
-  if (topo) {
+  // ---- per-run state: spread counters (one copy per warp), per-node inputs (each thread fills the slots it owns). A run
+  // that resumes has them in shared memory as it left them.
+  if (tid == 0 && !resume) rc.tomb = 0;
+  if (tid < kRunHost && !resume) rc.h_inc[tid] = 0;
+  if (topo && !resume) {
     for (int j = 0; j < n_mask; ++j) {
       if (lane < kRunDom) rc.cnt[warp][j][lane] = s.grp_cnt[(size_t)rc.m_group[j] * 64 + lane];
       if (tid == 0) rc.m_registered[j] = (uint32_t)s.grp_registered[rc.m_group[j]];
@@ -2761,7 +2912,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
 #ifdef KSCHED_PROFILE_PACK
   const long long cr_in0 = clock64();
 #endif
-  for (int a = tid; a < n_active; a += T) {
+  for (int a = tid; a < (resume ? 0 : n_active); a += T) {
     const unsigned short fl = hs->flags[a];
     unsigned rm;
     if (!((p_tol >> tmpl_taintset[fl >> 8]) & 1)) rm = 0;                        // Taints.Tolerates
@@ -2791,62 +2942,11 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
 #endif
   // ---- capture the node generic_step has just created for this class as a fresh-node variant
   if (fresh_valid && !s.any_limits && W32 <= kRunW32 && fresh_a == n_active - 1 && fresh_a >= 0) {
-    const int a = fresh_a, n = hs->node[a];
-    int dom[kRunMask] = {0, 0};
-    bool ok = true;
-#pragma unroll
-    for (int j = 0; j < kRunMask; ++j) {
-      if (j >= n_mask) continue;
-      const uint32_t z = zv[j * kTopoCap + a], v = z & 0xFFFF;
-      if (!v || (v & (v - 1)) || !(z & (1u << 16))) ok = false;
-      else dom[j] = __ffs(v) - 1;
-    }
-    for (int i = 0; i < rc.n_var && ok; ++i) {
-      bool same = (rc.var[i].fl >> 8) == (hs->flags[a] >> 8);
-#pragma unroll
-      for (int j = 0; j < kRunMask; ++j) same = same && (j >= n_mask || rc.var[i].dom[j] == dom[j]);
-      if (same) ok = false;  // already known
-    }
-    const int slot = rc.var_next;  // read BEFORE the barrier: thread 0 moves it while the others still copy (racecheck warning, round 2)
-    __syncthreads();  // rc.n_var / var_next read by everybody before thread 0 moves them
-    if (ok) {
-      RunVariant& v = rc.var[slot];
-      for (int w = tid; w < W32; w += T) v.opts[w] = s.nn_opts[(size_t)w * MAXN + n];
-      if (tid < KSCHED_MAX_KEYS) v.vals[tid] = tid < c.n_keys ? s.nn_vals[(size_t)tid * MAXN + n] : 0;
-      if (tid == 0) {
-        v.meta = s.nn_meta[n];
-        for (int r = 0; r < KSCHED_MAX_RES; ++r) v.q[r] = r < kHotRes ? hs->q[r][a] : s.nn_req[(size_t)r * MAXN + n];
-        for (int r = 0; r < kHotRes; ++r) { v.b1[r] = hs->bound[r][a]; v.b2[r] = hs->bound2[r][a]; }
-        v.qp = s.nn_req_present[n];
-        v.fl = hs->flags[a];
-        v.rp = rpv[a] & (kRpDead | 0xFFFF);
-        for (int j = 0; j < kRunMask; ++j) v.dom[j] = (uint8_t)dom[j];
-        rc.var_next = (slot + 1) % kRunVariants;
-        if (rc.n_var < kRunVariants) rc.n_var++;
-      }
-      __syncthreads();
-      // into the store (not looked up first: a class captures a variant only after a miss, so duplicates are rare and
-      // harmless, and the capture stays free of dependent loads)
-      if (warp == 0 && rc.vs_ok && rc.vs_n < kVarStore) {
-        const uint32_t pat = vs_pattern(n_mask, rc.m_key, dom[0], dom[1]);
-        const int e = rc.vs_n;
-        VarStoreEntry& d = s.vstore[e];
-        const uint32_t* src = reinterpret_cast<const uint32_t*>(&rc.var[slot]);
-        uint32_t* dst = reinterpret_cast<uint32_t*>(&d.v);
-        for (int w = lane; w < (int)(sizeof(RunVariant) / 4); w += 32) dst[w] = src[w];
-        __syncwarp();
-        if (lane == 0) {
-          d.sig = rc.sig; d.pat = pat; d.cls = cls;
-          d.v.rp = rc.var[slot].rp & 0xFFFF;
-          rc.vs_tag[e] = vs_tag(rc.sig, pat);
-          rc.vs_n = e + 1;
+    const int slot = run_capture(hs, zv, rpv, fresh_a, n_mask, cls);
 #ifdef KSCHED_PROFILE_PACK
-          s.counters[kCtrVarStoreEntries] += 1;
+    if (tid == 0 && slot >= 0) s.counters[kCtrRunCaptures] += 1;
 #endif
-        }
-        __syncwarp();
-      }
-    }
+    (void)slot;
   }
 
   RunEnv e{hs, zv, rpv, hc, NE, MAXN, W32, RH, hstride, n_host, n_mask, cls, topo, simple};
@@ -2856,12 +2956,16 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
   e.m_bias0 = n_mask > 0 ? (int)rc.m_self[0] - rc.m_skew[0] : 0; e.m_bias1 = n_mask > 1 ? (int)rc.m_self[1] - rc.m_skew[1] : 0;
   e.m_rec0 = n_mask > 0 && rc.m_rec[0]; e.m_rec1 = n_mask > 1 && rc.m_rec[1];
   int status = 0;
-  int novar = 0;  // the run stopped because no variant was known for the fresh node's domain (profile)
+  int why = kStopNone;  // StopCause of a status-1 stop
+  // a stop for want of a variant ends the call with status 3 (the variant is derived and the run resumes, see RunIO::resume),
+  // once per pod: a pod whose step still finds no variant (the derived node pinned another domain) stops the run
+  const bool derive_ok = s.use_run_derive && !s.any_limits && W32 <= kRunW32;
+  int derived_at = resume ? io.r_derived : -1;
   const bool lvl = s.use_level_run && n_mask == 0;
   // mask run (see M1Ctx): one mask-key spread relation, domains and counts small enough for the lists
-  bool m1_ok = s.use_mask_run && n_mask == 1 && (e.m_reg0 >> kM1Dom) == 0;
-  bool m1_built = false;
-  int lvp = 0;
+  bool m1_ok = resume ? (io.r_m1 & 1) != 0 : s.use_mask_run && n_mask == 1 && (e.m_reg0 >> kM1Dom) == 0;
+  bool m1_built = resume && (io.r_m1 & 2);
+  int lvp = resume ? io.r_lvp : 0;
 #ifdef KSCHED_PROFILE_PACK
   const long long cr_t0 = clock64();
   int cr_it[4] = {0, 0, 0, 0};  // iterations: level, fill, fresh, per-pod argmin
@@ -2897,18 +3001,19 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
 #ifdef KSCHED_PROFILE_PACK
       const long long m1_t1 = clock64();
 #endif
-      if (warp == 0) m1_walk(e, buf, i, qlen, tick, n_new, n_active, novar);
+      if (warp == 0) m1_walk(e, buf, i, qlen, tick, n_new, n_active, why);
       __syncthreads();
       m1_store_fresh(e);
       const int m_adv = g_m1.out_adv, m_reason = g_m1.out_reason;
       tick = g_m1.out_tick; n_new = g_m1.out_n_new; n_active = g_m1.out_n_active;
+      why = g_m1.out_why;  // (warp 0's: the status below is the same in every warp)
       qi += m_adv;
       qlen -= m_adv;
       __syncthreads();  // out_* are rewritten by the next entry
 #ifdef KSCHED_PROFILE_PACK
       if (tid == 0) { s.counters[kCtrMaskCycles] += clock64() - m1_t1; s.counters[kCtrMaskPods] += m_adv; s.counters[kCtrMaskEntries] += 1; }
 #endif
-      if (m_reason == 1) { status = 1; break; }
+      if (m_reason == 1) { status = why == kStopNoVariant && derive_ok && qi != derived_at ? 3 : 1; break; }
       if (qlen == 0) break;
       if (m_reason == 2) m1_ok = false;
       continue;
@@ -2939,12 +3044,15 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
     uint32_t okm0 = 0, okm1 = 0;
     if (mode == 0) {
       CR_IT(3)
-      const int r = run_argmin_step(e, buf, i, n_active, tick, parity, okm0, okm1);
+      const int r = run_argmin_step(e, buf, i, n_active, tick, parity, okm0, okm1, why);
       if (r == 1) { status = 1; break; }
       if (r == 2) mode = 2;
     }
     if (mode == 2) {
-      if (!run_fresh_step(e, buf, i, k_avail, lvl, okm0, okm1, tick, n_new, n_active, adv, novar)) { status = 1; break; }
+      if (!run_fresh_step(e, buf, i, k_avail, lvl, okm0, okm1, tick, n_new, n_active, adv, why)) {
+        status = why == kStopNoVariant && derive_ok && qi != derived_at ? 3 : 1;
+        break;
+      }
       CR_IT(2)
     }
     // ---- the pods are placed: pop them
@@ -2953,6 +3061,14 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
     if (qlen == 0) break;
   }
   __syncthreads();
+  if (status == 3) {  // (see RunIO::resume)
+    if (tid == 0) {
+      io.qi = qi; io.qlen = qlen; io.tick = tick; io.n_active = n_active; io.n_new = n_new; io.parity = parity; io.placed = 0; io.status = 3;
+      io.r_qi0 = qi0; io.r_seq0 = seq0; io.r_cb = cb; io.r_buf = buf; io.r_lvp = lvp; io.r_m1 = (m1_ok ? 1 : 0) | (m1_built ? 2 : 0); io.r_derived = qi;
+    }
+    __syncthreads();
+    return;
+  }
 #ifdef KSCHED_PROFILE_PACK
   const long long cr_t1 = clock64();
 #endif
@@ -3038,7 +3154,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
       s.counters[kCtrRunFresh] += cr_it[2]; s.counters[kCtrRunPerPod] += cr_it[3];
     }
     s.counters[kCtrRunLvFills] += cr_it[1];
-    if (status == 1 && novar) s.counters[kCtrNoVariantStops] += 1;
+    if (status == 1 && why != kStopNone) s.counters[kCtrNoVariantStops + why - 1] += 1;
   }
 #endif
   if (tid == 0) {
@@ -3166,7 +3282,7 @@ __global__ void __launch_bounds__(kMaxThreads, 1) pack_kernel() {
         RunIO& io = g_rio;
         io.qi = qi; io.head = head; io.qlen = qlen; io.tick = tick; io.seq = seq; io.n_active = n_active; io.n_new = n_new; io.parity = parity;
         io.add_calls = add_calls; io.placed = 0; io.status = 0;
-        io.fresh_valid = fresh_valid; io.fresh_a = fresh_a; io.fresh_cls = fresh_cls;
+        io.fresh_valid = fresh_valid; io.fresh_a = fresh_a; io.fresh_cls = fresh_cls; io.staged = 0; io.resume = 0;
       }
       __syncthreads();
 #ifdef KSCHED_PROFILE_PACK
@@ -3174,11 +3290,18 @@ __global__ void __launch_bounds__(kMaxThreads, 1) pack_kernel() {
       const long long pk_novar0 = tid == 0 ? s.counters[kCtrNoVariantStops] : 0;
 #endif
       class_run(nxt);
+      while (g_rio.status == 3) {  // derive the variant the run needs, then resume it
+        run_derive_at(nxt, g_rio.qi, g_rio.n_new, g_rio.n_active, g_rio.tick, g_rio.seq, g_rio.parity);
+        if (tid == 0) { g_rio.resume = 1; g_rio.fresh_valid = 0; }
+        __syncthreads();
+        class_run(nxt);
+      }
       const RunIO& io = g_rio;
       const int placed = io.placed, status = io.status;
       qi = io.qi; head = io.head; qlen = io.qlen; tick = io.tick; seq = io.seq; n_active = io.n_active; n_new = io.n_new; parity = io.parity;
       add_calls = io.add_calls;
       fresh_valid = 0;
+      if (io.staged) { row_class = KSCHED_NONE; pt_class = KSCHED_NONE; pt_nonempty = true; }  // (rebuilt by the next generic step)
 #ifdef KSCHED_PROFILE_PACK
       if (tid == 0) {
         s.counters[kCtrRunCalls] += 1; s.counters[kCtrRunPlaced] += placed; s.counters[kCtrRunBails] += status == 1; s.counters[kCtrRunIneligible] += status == 2;

@@ -115,6 +115,7 @@ struct PackState {
   int use_level_warp;                // class_run: the level / fill steps on one warp while at most 32 nodes are open (KSCHED_NO_LEVELWARP=1: off)
   int use_mask_run;                  // class_run: list-driven loop on warp 0 for one mask-key spread relation (KSCHED_NO_MASKRUN=1: off)
   int use_varstore;                  // class_run: fresh-node variants shared by classes of one shape (KSCHED_NO_VARSTORE=1: off)
+  int use_run_derive;                // class_run: a fresh node's missing variant derived inside the run (KSCHED_NO_RUNDERIVE=1: off)
   int use_round_stretch;             // mask run: several rounds of a zone spread in one step (KSCHED_NO_ROUNDSTRETCH=1: off)
   int use_fill_stretch;              // mask run: rounds that keep the same head per zone in one step (KSCHED_NO_FILLSTRETCH=1 or
                                      // KSCHED_NO_ROUNDSTRETCH=1: off)

@@ -374,6 +374,11 @@ typedef struct ksched_result {
      [max_new_nodes] presence masks (bit x: ext resource x is a key of the node's request map). */
   int64_t* new_node_requests_ext;
   uint32_t* new_node_requests_ext_present;
+  /* Written by ksched_simulate_full only (simulateScheduling's verdicts, deprovisioning/helpers.go:96-114): every pod of the
+     batch was placed, and an existing node of the simulation (one that stays) is not initialised, in which case the
+     reference returns nil, false whatever the placements. */
+  int32_t all_pods_scheduled;
+  int32_t uninitialized_existing;
 } ksched_result;
 
 /*
@@ -408,12 +413,23 @@ typedef struct ksched_cluster {
   const int8_t* node_domain;              /* [n_keys][n_existing] dictionary id of the node's label value, -1 = no such label */
   const uint8_t* node_has_hostname_label; /* [n_existing] */
   const uint32_t* group_filter_match;     /* [n_groups][(n_existing + 31) / 32] bit e: TopologyNodeFilter.Matches(node e) */
+  /* What ksched_simulate_full needs besides (ksched_simulate_batch ignores them; NULL / 0 as noted):
+     node_removable[e] = 1 when every reschedulable pod of slot e is a pod of the superset (the slot is a candidate), so that
+     removing it loses no pod; NULL = every slot. node_initialized[e] = the node carries karpenter.sh/initialized=true; NULL =
+     every node. n_pending_lead = how many of the pending pods come before the removed nodes' pods in a full simulation's pod
+     order (simulateScheduling: the provisioner's pending pods, then the candidates' pods, then the pods of nodes marked for
+     deletion, helpers.go:74-88); the other pending pods follow them. 0 <= n_pending_lead <= the number of pending pods. */
+  const uint8_t* node_removable;   /* [n_existing] or NULL */
+  const uint8_t* node_initialized; /* [n_existing] or NULL */
+  int32_t n_pending_lead;
+  int32_t pad;
 } ksched_cluster;
 
 typedef struct ksched_candidate_set {
   const int32_t* nodes;     /* existing slots removed by this simulation (the candidates, helpers.go:52-68), distinct */
   int32_t n_nodes;
-  int32_t pad;
+  int32_t capacity;         /* ksched_simulate_full: pods the set's ksched_result holds (per-pod arrays) and new nodes it holds
+                               (per-node arrays); ksched_simulate_batch ignores it */
   const int64_t* remaining; /* [n_templates][KSCHED_MAX_RES] provisioner limits left with the removed nodes' capacity given back
                                (scheduler.go:221-248 only subtracts the nodes that stay), or NULL = as in the catalog */
 } ksched_candidate_set;
@@ -504,6 +520,16 @@ int ksched_load_cluster(ksched_handle* h, const ksched_cluster* cluster);
 /* results[n_sets]; node0_types[n_sets][type_words] = surviving InstanceTypeOptions of each simulation's first new node.
    The simulations run back to back on the handle's stream with one synchronisation at the end. */
 int ksched_simulate_batch(ksched_handle* h, const ksched_candidate_set* sets, int n_sets, ksched_sim_result* results, uint64_t* node0_types);
+/* simulateScheduling's whole answer for each set (deprovisioning/helpers.go:42-115): every pod of the batch placed, with no
+   stop after a second new node. results[q] is written as ksched_solve would write it for the problem encoded fresh with set q's
+   nodes as the candidates, in that problem's numbering: pods are the first n_pending_lead pending pods, then the removed
+   nodes' pods node by node in the order set q lists the nodes, then the other pending pods; existing slot e becomes its
+   index among the slots that stay; new node i is n_existing - n_nodes + i. Filled: assign, relax_level, place_seq,
+   new_nodes, new_node_types, launch (when not NULL; needs ksched_catalog.offering_keys), the ext arrays (when not NULL),
+   the counts and the two flags; existing_reqs, feasibility and best_column are not written. nodes_visited counts the
+   removed slots the pack kernel skips as well. A slot out of range, repeated or not removable, or a capacity below the
+   set's batch, is KSCHED_ERR_INVALID. The snapshot is left as it was; one stream synchronisation per call. */
+int ksched_simulate_full(ksched_handle* h, const ksched_candidate_set* sets, int n_sets, ksched_result* results);
 
 /* order[0..*n_candidates) = node indices by ascending disruption cost (ties: input order), cost[i] = cost of order[i]. */
 int ksched_rank_candidates(ksched_handle* h, const ksched_rank_input* in, int32_t* order, double* cost, int32_t* n_candidates);

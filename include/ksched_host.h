@@ -60,6 +60,10 @@ void kh_result_assign(const kh_result* r, int* out);  /* [pods] -1 | existing no
 void kh_result_relax(const kh_result* r, int* out);   /* [pods] successful Preferences.Relax calls */
 long long kh_result_new_node_options(const kh_result* r, long long node, int* out, long long cap); /* InstanceTypeOptions, input order */
 long long kh_result_to_json(const kh_result* r, char* buf, long long cap); /* everything, incl. requirements, requests, launch choice */
+/* simulateScheduling's verdicts (deprovisioning/helpers.go:96-114) of a Solve or a simulation of the GPU path: every pod was
+ * placed; an existing node of the result is not initialised (the reference then returns nil, false). Not part of the JSON. */
+int kh_result_all_pods_scheduled(const kh_result* r);
+int kh_result_uninitialized_existing(const kh_result* r);
 
 /* ---- the device */
 int kh_set_device(int ordinal);   /* CUDA device of this process's scheduler handle (default 0) */
@@ -87,6 +91,15 @@ int kh_cluster_candidates(const kh_cluster* c, int* nodes, int cap); /* disrupti
  * options[q * options_stride ...], n_options[q] of them. */
 int kh_cluster_probe_sets(kh_cluster* c, const int* sets, const int* set_off, int n_sets, int multi, int* actions, int* options, int options_stride,
                           int* n_options);
+
+/* simulateScheduling's whole result (deprovisioning/helpers.go:42-115), as Expiration, Drift and computeConsolidation read it,
+ * for n_sets candidate sets in one device call on the session's resident cluster. Set q = sets[set_off[q] .. set_off[q+1]) as
+ * node indices of the problem, in the order the caller picked them (they must be candidates of the session). out[q] (caller
+ * allocated, kh_result_new) is what kh_scheduler_solve(p, set q) returns, pod for pod and node for node, nodes_visited aside
+ * (a simulation also counts the removed nodes the kernel skips), with both verdicts set. A node marked for deletion is
+ * errCandidateNodeDeleting (KSCHED_ERR_INVALID). On a session whose snapshot was refused (resident = 0) each set is a freshly
+ * encoded Solve: the same results, slower. */
+int kh_cluster_simulate(kh_cluster* c, const int* sets, const int* set_off, int n_sets, kh_result** out);
 
 /* MultiNodeConsolidation.firstNNodeConsolidationOption. out4 = [action, nodes removed (a prefix of the disruption order),
  * simulations, n_options]; probes / probe_actions = the binary search's trace. */

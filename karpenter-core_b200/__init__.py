@@ -30,7 +30,7 @@ ABI_SYMBOLS = [
     "ksched_abi_version", "ksched_device_count", "ksched_create", "ksched_destroy", "ksched_last_error",
     "ksched_type_words", "ksched_load_catalog", "ksched_set_shard", "ksched_shard_range", "ksched_nccl_unique_id", "ksched_nccl_init",
     "ksched_solve", "ksched_upload", "ksched_run_resident", "ksched_download", "ksched_run_feasibility_only",
-    "ksched_get_timings", "ksched_load_cluster", "ksched_simulate_batch", "ksched_allgather", "ksched_rank_candidates",
+    "ksched_get_timings", "ksched_load_cluster", "ksched_simulate_batch", "ksched_simulate_full", "ksched_allgather", "ksched_rank_candidates",
 ]
 
 
@@ -80,6 +80,7 @@ def model_lib():
     for name in ("kh_result_num_pods", "kh_result_num_new_nodes", "kh_result_num_existing", "kh_result_nodes_visited", "kh_result_add_calls"):
         getattr(L, name).restype = C.c_longlong
         getattr(L, name).argtypes = [C.c_void_p]
+    L.kh_result_all_pods_scheduled.argtypes = L.kh_result_uninitialized_existing.argtypes = [C.c_void_p]
     L.kh_result_assign.argtypes = [C.c_void_p, C.c_void_p]
     L.kh_result_relax.argtypes = [C.c_void_p, C.c_void_p]
     L.kh_result_new_node_info.argtypes = [C.c_void_p, C.c_void_p]
@@ -159,6 +160,7 @@ def lib():
     L.kh_cluster_probe_sets.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int,
                                         C.POINTER(C.c_int)]
     L.kh_cluster_candidates.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.c_int]
+    L.kh_cluster_simulate.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_void_p)]
     L.kh_consolidate_single.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int]
     L.kh_consolidate_validated.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
                                            C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
@@ -275,6 +277,16 @@ class Result:
         return out
 
     @property
+    def all_pods_scheduled(self):
+        """simulateScheduling's allPodsScheduled (helpers.go:96-114): every pod was placed (GPU Solves and simulations)"""
+        return bool(model_lib().kh_result_all_pods_scheduled(self.ptr))
+
+    @property
+    def uninitialized_existing(self):
+        """an existing node of the result is not initialised: simulateScheduling then returns nil, false (helpers.go:104-110)"""
+        return bool(model_lib().kh_result_uninitialized_existing(self.ptr))
+
+    @property
     def num_new_nodes(self):
         return model_lib().kh_result_num_new_nodes(self.ptr)
 
@@ -388,6 +400,22 @@ class ClusterSession:
         _check(lib().kh_cluster_probe_sets(self.ptr, (C.c_int * max(1, len(flat)))(*flat), (C.c_int * len(off))(*off), len(sets), int(multi), actions, opts, stride,
                                            nopt))
         return [(int(actions[q]), list(opts[q * stride:q * stride + min(nopt[q], stride)])) for q in range(len(sets))]
+
+    def simulate(self, sets):
+        """simulateScheduling's whole result (helpers.go:42-115) for every set of node indices of the problem, in the order
+        Expiration, Drift or computeConsolidation picked them, in one device call -> [Result], each what
+        Scheduler(problem).solve(candidates=set) returns (nodes_visited aside: a simulation also counts the removed nodes it
+        skips), with all_pods_scheduled and uninitialized_existing set. The nodes must be candidates of the session."""
+        if not sets:
+            return []
+        flat = [int(i) for s_ in sets for i in s_]
+        off = [0]
+        for s_ in sets:
+            off.append(off[-1] + len(s_))
+        out = [Result() for _ in sets]
+        ptrs = (C.c_void_p * len(sets))(*[r.ptr for r in out])
+        _check(lib().kh_cluster_simulate(self.ptr, (C.c_int * max(1, len(flat)))(*flat), (C.c_int * len(off))(*off), len(sets), ptrs))
+        return out
 
     def validate(self, after: Problem, commands):
         """Validation.IsValid (validation.go:63-172) of commands against `after`, the cluster when the TTL ends, in one device

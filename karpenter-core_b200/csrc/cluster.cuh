@@ -102,6 +102,81 @@ __global__ void cluster_collect_kernel(const long long* __restrict__ counters, i
   for (int w = tid; w < W32; w += blockDim.x) out_types[w] = nn_opts[(size_t)w * max_new];
 }
 
+// The scalars of one full simulation (ksched_simulate_full), copied out with its arrays.
+struct SimFullDev {
+  long long nodes_visited, add_calls;
+  int32_t n_new_nodes, n_unscheduled, error, all_pods_scheduled, uninitialized_existing, pad;
+};
+// Where cluster_full_collect_kernel writes one simulation: arrays laid out as the caller's ksched_result, so that each copies
+// out in one piece.
+struct SimFullOut {
+  int32_t *assign, *relax, *seq;
+  ksched_new_node* nodes;
+  uint64_t* types;                 // [capacity][W64]
+  int64_t* ext;                    // [capacity][X]
+  uint32_t* ext_present;           // [capacity]
+  SimFullDev* scalars;
+};
+// simulateScheduling's whole answer in the numbering of the problem encoded fresh for this set. The batch holds the
+// pending pods (the first n_lead of them lead), then the removed nodes' pods in the set's order (cluster_select_kernel with
+// the set's offsets): batch position b goes to pod b, b + n_removed_pods or b - n_pending + n_lead. slot_map[e] = the slot's
+// index among the slots that stay, -1 for a removed one. The new nodes are gathered from the pack kernel's columns
+// (PackState nn_*) into rows. One block per simulation, a few thousand pods and nodes: microseconds.
+__global__ void cluster_full_collect_kernel(const long long* __restrict__ counters, int n_pods, int n_pending, int n_lead, int n_removed_pods,
+                                            const int32_t* __restrict__ assign, const int32_t* __restrict__ relax, const int32_t* __restrict__ seq,
+                                            const int32_t* __restrict__ slot_map, const uint8_t* __restrict__ initialized, int n_existing,
+                                            int n_stay, const uint8_t* __restrict__ nn_tmpl, const int32_t* __restrict__ nn_count,
+                                            const int64_t* __restrict__ nn_req, const uint32_t* __restrict__ nn_req_present,
+                                            const uint64_t* __restrict__ nn_vals, const uint64_t* __restrict__ nn_meta,
+                                            const uint32_t* __restrict__ nn_opts, const int64_t* __restrict__ nn_req_ext,
+                                            const uint32_t* __restrict__ nn_ext_present, int max_new, int W32, int X, SimFullOut out) {
+  __shared__ int uninit;
+  const int tid = threadIdx.x;
+  const int n_new = (int)counters[kCtrNewNodes];
+  if (tid == 0) uninit = 0;
+  __syncthreads();
+  for (int b = tid; b < n_pods; b += blockDim.x) {
+    const int p = b < n_lead ? b : (b < n_pending ? b + n_removed_pods : b - n_pending + n_lead);
+    const int a = assign[b];
+    out.assign[p] = a < 0 ? -1 : (a < n_existing ? slot_map[a] : n_stay + (a - n_existing));
+    out.relax[p] = relax[b];
+    out.seq[p] = seq[b];
+  }
+  for (int e = tid; e < n_existing; e += blockDim.x)
+    if (slot_map[e] >= 0 && initialized && !initialized[e]) uninit = 1;  // helpers.go:104-110 walks every node that stays
+  const int W64 = W32 / 2;  // DevCatalog::W32 is even
+  for (int n = tid; n < n_new; n += blockDim.x) {
+    ksched_new_node o;
+    o.template_index = nn_tmpl[n];
+    o.pod_count = nn_count[n];
+    o.requests_present = nn_req_present[n];
+    o.pad = 0;
+    for (int r = 0; r < KSCHED_MAX_RES; ++r) o.requests[r] = nn_req[(size_t)r * max_new + n];
+    for (int k = 0; k < KSCHED_MAX_KEYS; ++k) o.reqs.values[k] = nn_vals[(size_t)k * max_new + n];
+    o.reqs.meta = nn_meta[n];
+    out.nodes[n] = o;
+    uint32_t* row = reinterpret_cast<uint32_t*>(out.types + (size_t)n * W64);
+    for (int w = 0; w < W32; ++w) row[w] = nn_opts[(size_t)w * max_new + n];
+    if (out.ext) {
+      for (int x = 0; x < X; ++x) out.ext[(size_t)n * X + x] = nn_req_ext[(size_t)n * X + x];
+      out.ext_present[n] = nn_ext_present[n];
+    }
+  }
+  __syncthreads();
+  if (tid == 0) {
+    SimFullDev d;
+    d.nodes_visited = counters[kCtrNodesVisited];
+    d.add_calls = counters[kCtrAddCalls];
+    d.n_new_nodes = n_new;
+    d.n_unscheduled = (int32_t)counters[kCtrUnscheduled];
+    d.error = (int32_t)counters[kCtrError];
+    d.all_pods_scheduled = d.n_unscheduled == 0 ? 1 : 0;
+    d.uninitialized_existing = uninit;
+    d.pad = 0;
+    *out.scalars = d;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // Candidate ranking for deprovisioning (deprovisioning/helpers.go:125-165,275-287, consolidation.go:85-103)
 // ------------------------------------------------------------------------------------------------

@@ -274,6 +274,18 @@ struct ksched_handle {
   DevBuf<int64_t> d_sup_ts, d_sim_remaining;
   DevBuf<uint8_t> d_in_set;
   DevBuf<SimResultDev> d_sim_results;
+  // full simulations (ksched_simulate_full): which slots a set may remove, the initialised flags, the leading pending pods,
+  // and the staging arrays every set's results are gathered into before they are copied out
+  std::vector<uint8_t> h_node_removable;
+  int sup_lead = 0;
+  DevBuf<uint8_t> d_node_init;
+  DevBuf<int32_t> d_slot_map, d_full_i32;
+  DevBuf<ksched_new_node> d_full_nodes;
+  DevBuf<uint64_t> d_full_types;
+  DevBuf<int64_t> d_full_ext;
+  DevBuf<uint32_t> d_full_ext_present;
+  DevBuf<ksched_launch_choice> d_full_launch;
+  DevBuf<SimFullDev> d_full_scalars;
   bool cluster_topology = false;
   int filt_words = 0;
   DevBuf<uint32_t> d_cc_begin, d_filt;
@@ -1670,6 +1682,10 @@ int ksched_load_cluster(ksched_handle* h, const ksched_cluster* cl) {
     else if (cl->pod_node[i - 1] != nd) { h->err = "the pods of one node must be contiguous"; return KSCHED_ERR_INVALID; }
     ++count[nd];
   }
+  if (cl->n_pending_lead < 0 || cl->n_pending_lead > pending) { h->err = "n_pending_lead out of range"; return KSCHED_ERR_INVALID; }
+  std::vector<uint8_t> removable((size_t)std::max(NE, 1), 1), init((size_t)std::max(NE, 1), 1);
+  if (cl->node_removable) std::copy(cl->node_removable, cl->node_removable + NE, removable.begin());
+  if (cl->node_initialized) std::copy(cl->node_initialized, cl->node_initialized + NE, init.begin());
   int rc = ksched_upload(h, pb);  // the superset problem: buffers sized for the largest batch, existing-node state, class tables
   if (rc != KSCHED_OK) return rc;
   CUDA_TRY(h, upload(h, h->d_sup_pod_node, cl->pod_node, (size_t)P));
@@ -1680,6 +1696,7 @@ int ksched_load_cluster(ksched_handle* h, const ksched_cluster* cl) {
   CUDA_TRY(h, h->d_node_dst.ensure((size_t)std::max(NE, 1)));
   CUDA_TRY(h, h->d_in_set.ensure((size_t)std::max(NE, 1)));
   CUDA_TRY(h, h->d_pod_src.ensure((size_t)std::max(P, 1)));
+  CUDA_TRY(h, upload_vec(h, h->d_node_init, init));
   h->cluster_topology = topo;
   if (topo) {
     const int NC = pb->n_classes, NK = h->cat.n_keys;
@@ -1696,33 +1713,42 @@ int ksched_load_cluster(ksched_handle* h, const ksched_cluster* cl) {
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   h->h_node_first.swap(first);
   h->h_node_count.swap(count);
+  h->h_node_removable.swap(removable);
   h->sup_pods = P;
   h->sup_pending = pending;
+  h->sup_lead = cl->n_pending_lead;
   h->have_cluster = true;
   return KSCHED_OK;
 }
 
-int ksched_simulate_batch(ksched_handle* h, const ksched_candidate_set* sets, int n_sets, ksched_sim_result* results, uint64_t* node0_types) {
-  if (!h || !sets || n_sets < 0 || (n_sets > 0 && !results)) return KSCHED_ERR_INVALID;
-  if (!h->have_cluster) { h->err = "ksched_load_cluster must be called first"; return KSCHED_ERR_INVALID; }
-  if (n_sets == 0) return KSCHED_OK;
-  CUDA_TRY(h, cudaSetDevice(h->device));
-  const int NE = h->st.n_existing, V = h->cat.n_templates, W32 = h->cat.W32, W64 = W32 / 2;
-  // stage every set's node list, per-node batch offsets and limits in one upload each
-  std::vector<int32_t> all_nodes, all_dst((size_t)n_sets * std::max(NE, 1), 0), batch((size_t)n_sets, 0), node_off((size_t)n_sets + 1, 0);
+// Every set's node list, per-node batch offsets and limits, staged in one upload each. A set's batch lists the removed
+// nodes' pods after the pending ones, node by node: in slot order for the consolidation simulator (the queue sorts them
+// anyway, queue.go:35-110), in the set's own order for a full simulation, whose results keep that order. A full simulation
+// also refuses slots whose pods the superset does not hold.
+static int stage_sets(ksched_handle* h, const ksched_candidate_set* sets, int n_sets, bool full, std::vector<int32_t>& node_off, std::vector<int32_t>& batch) {
+  const int NE = h->st.n_existing, V = h->cat.n_templates;
+  std::vector<int32_t> all_nodes, all_dst((size_t)n_sets * std::max(NE, 1), 0);
   std::vector<int64_t> all_rem((size_t)n_sets * V * KSCHED_MAX_RES, 0);
+  node_off.assign((size_t)n_sets + 1, 0);
+  batch.assign((size_t)n_sets, 0);
+  std::vector<uint8_t> seen((size_t)std::max(NE, 1), 0);
   for (int q = 0; q < n_sets; ++q) {
     const ksched_candidate_set& cs = sets[q];
     if (cs.n_nodes < 0 || (cs.n_nodes > 0 && !cs.nodes)) { h->err = "bad candidate set"; return KSCHED_ERR_INVALID; }
     std::vector<int32_t> nodes(cs.nodes, cs.nodes + cs.n_nodes);
-    std::sort(nodes.begin(), nodes.end());  // the batch lists the removed nodes' pods in slot order (the queue sorts them anyway, queue.go:35-110)
+    if (!full) std::sort(nodes.begin(), nodes.end());
     int pos = h->sup_pending;
-    for (size_t i = 0; i < nodes.size(); ++i) {
-      const int nd = nodes[i];
-      if (nd < 0 || nd >= NE || (i > 0 && nodes[i - 1] == nd)) { h->err = "candidate set: existing slot out of range or repeated"; return KSCHED_ERR_INVALID; }
+    for (const int nd : nodes) {
+      if (nd < 0 || nd >= NE || seen[(size_t)nd]) { h->err = "candidate set: existing slot out of range or repeated"; return KSCHED_ERR_INVALID; }
+      if (full && !h->h_node_removable[(size_t)nd]) {
+        h->err = "candidate set: existing slot " + std::to_string(nd) + " is not removable (its pods are not in the snapshot)";
+        return KSCHED_ERR_INVALID;
+      }
+      seen[(size_t)nd] = 1;
       all_dst[(size_t)q * NE + nd] = pos;
       pos += h->h_node_count[(size_t)nd];
     }
+    for (const int nd : nodes) seen[(size_t)nd] = 0;
     batch[(size_t)q] = pos;
     all_nodes.insert(all_nodes.end(), nodes.begin(), nodes.end());
     node_off[(size_t)q + 1] = (int32_t)all_nodes.size();
@@ -1734,35 +1760,54 @@ int ksched_simulate_batch(ksched_handle* h, const ksched_candidate_set* sets, in
   CUDA_TRY(h, upload_vec(h, h->d_set_nodes, all_nodes));
   CUDA_TRY(h, upload_vec(h, h->d_node_dst, all_dst));
   CUDA_TRY(h, upload_vec(h, h->d_sim_remaining, all_rem));
+  return KSCHED_OK;
+}
+
+// One simulation of set q (stage_sets) on the handle's stream, up to and including the pack kernel: the snapshot's state
+// restored with the set's limits, its slots closed, its batch gathered, the counters of the pods that stay, K0, K1 (the
+// class pass only when `class_pass`: it depends on the classes and the catalog alone) and K2.
+static int run_simulation(ksched_handle* h, int q, const std::vector<int32_t>& node_off, int P, bool class_pass, int stop_new_nodes) {
+  const int NE = h->st.n_existing, V = h->cat.n_templates;
+  const int n_nodes = node_off[(size_t)q + 1] - node_off[(size_t)q];
+  int rc = reset_state(h, h->d_sim_remaining.ptr + (size_t)q * V * KSCHED_MAX_RES);
+  if (rc != KSCHED_OK) return rc;
+  if (n_nodes > 0)
+    cluster_mark_kernel<<<(n_nodes + 255) / 256, 256, 0, h->stream>>>(h->d_set_nodes.ptr + node_off[(size_t)q], n_nodes, h->d_in_set.ptr, h->d_ex_closed.ptr);
+  if (h->sup_pods > 0)
+    cluster_select_kernel<<<(h->sup_pods + 255) / 256, 256, 0, h->stream>>>(h->sup_pods, h->d_sup_pod_node.ptr, h->d_in_set.ptr, h->d_node_dst.ptr + (size_t)q * NE,
+                                                                            h->d_node_first.ptr, h->sup_pending, h->d_sup_class.ptr, h->d_sup_ts.ptr, h->d_sup_uid.ptr,
+                                                                            h->d_pod_class0.ptr, h->d_ts.ptr, h->d_uid_rank.ptr, h->d_pod_src.ptr);
+  if (h->cluster_topology && h->sup_pods > 0)
+    cluster_topology_kernel<<<(h->sup_pods + 255) / 256, 256, 0, h->stream>>>(
+        h->sup_pods, h->d_sup_pod_node.ptr, h->d_in_set.ptr, h->d_sup_class.ptr, h->d_cc_begin.ptr, h->d_cc.ptr, h->d_groups.ptr, h->d_node_dom.ptr,
+        h->d_node_hostlabel.ptr, h->d_filt.ptr, h->filt_words, NE, NE + h->st.max_new, h->d_grp_host_row.ptr, h->d_grp_cnt.ptr,
+        reinterpret_cast<unsigned long long*>(h->d_grp_registered.ptr), h->d_grp_host.ptr, h->d_grp_host_total.ptr);
+  // the working copy of the pod classes (reset_state copied the previous batch's): refresh it from the new batch
+  if (P > 0) CUDA_TRY(h, cudaMemcpyAsync(h->d_pod_class.ptr, h->d_pod_class0.ptr, (size_t)P * 4, cudaMemcpyDeviceToDevice, h->stream));
+  if ((rc = run_sort(h, P)) != KSCHED_OK) return rc;
+  if (class_pass && (rc = run_class_feasibility(h, P)) != KSCHED_OK) return rc;
+  if ((rc = run_feasibility(h, P)) != KSCHED_OK) return rc;
+  return run_pack(h, P, stop_new_nodes);
+}
+
+int ksched_simulate_batch(ksched_handle* h, const ksched_candidate_set* sets, int n_sets, ksched_sim_result* results, uint64_t* node0_types) {
+  if (!h || !sets || n_sets < 0 || (n_sets > 0 && !results)) return KSCHED_ERR_INVALID;
+  if (!h->have_cluster) { h->err = "ksched_load_cluster must be called first"; return KSCHED_ERR_INVALID; }
+  if (n_sets == 0) return KSCHED_OK;
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  const int W32 = h->cat.W32, W64 = W32 / 2;
+  std::vector<int32_t> node_off, batch;
+  int rc = stage_sets(h, sets, n_sets, false, node_off, batch);
+  if (rc != KSCHED_OK) return rc;
   CUDA_TRY(h, h->d_sim_results.ensure((size_t)n_sets));
   CUDA_TRY(h, h->d_sim_types.ensure((size_t)n_sets * W32));
   CUDA_TRY(h, cudaEventRecord(h->ev[0], h->stream));
-  int rc = KSCHED_OK;
   // nothing computeConsolidation can return depends on what happens after a second new node is opened
   // (consolidation.go:214-224: len(newNodes) != 1 -> do nothing): the simulation stops there
   const int stop_new_nodes = 2;
   for (int q = 0; q < n_sets && rc == KSCHED_OK; ++q) {
-    const int n_nodes = node_off[(size_t)q + 1] - node_off[(size_t)q], P = batch[(size_t)q];
-    rc = reset_state(h, h->d_sim_remaining.ptr + (size_t)q * V * KSCHED_MAX_RES);
-    if (rc != KSCHED_OK) break;
-    if (n_nodes > 0)
-      cluster_mark_kernel<<<(n_nodes + 255) / 256, 256, 0, h->stream>>>(h->d_set_nodes.ptr + node_off[(size_t)q], n_nodes, h->d_in_set.ptr, h->d_ex_closed.ptr);
-    if (h->sup_pods > 0)
-      cluster_select_kernel<<<(h->sup_pods + 255) / 256, 256, 0, h->stream>>>(h->sup_pods, h->d_sup_pod_node.ptr, h->d_in_set.ptr, h->d_node_dst.ptr + (size_t)q * NE,
-                                                                              h->d_node_first.ptr, h->sup_pending, h->d_sup_class.ptr, h->d_sup_ts.ptr, h->d_sup_uid.ptr,
-                                                                              h->d_pod_class0.ptr, h->d_ts.ptr, h->d_uid_rank.ptr, h->d_pod_src.ptr);
-    if (h->cluster_topology && h->sup_pods > 0)
-      cluster_topology_kernel<<<(h->sup_pods + 255) / 256, 256, 0, h->stream>>>(
-          h->sup_pods, h->d_sup_pod_node.ptr, h->d_in_set.ptr, h->d_sup_class.ptr, h->d_cc_begin.ptr, h->d_cc.ptr, h->d_groups.ptr, h->d_node_dom.ptr,
-          h->d_node_hostlabel.ptr, h->d_filt.ptr, h->filt_words, NE, NE + h->st.max_new, h->d_grp_host_row.ptr, h->d_grp_cnt.ptr,
-          reinterpret_cast<unsigned long long*>(h->d_grp_registered.ptr), h->d_grp_host.ptr, h->d_grp_host_total.ptr);
-    // the working copy of the pod classes (reset_state copied the previous batch's): refresh it from the new batch
-    if (P > 0) CUDA_TRY(h, cudaMemcpyAsync(h->d_pod_class.ptr, h->d_pod_class0.ptr, (size_t)P * 4, cudaMemcpyDeviceToDevice, h->stream));
-    if ((rc = run_sort(h, P)) != KSCHED_OK) break;
-    // the class rows of the feasibility matrix depend on the classes and the catalog only: once per batch
-    if (q == 0 && (rc = run_class_feasibility(h, P)) != KSCHED_OK) break;
-    if ((rc = run_feasibility(h, P)) != KSCHED_OK) break;
-    if ((rc = run_pack(h, P, stop_new_nodes)) != KSCHED_OK) break;
+    const int P = batch[(size_t)q];
+    if ((rc = run_simulation(h, q, node_off, P, q == 0, stop_new_nodes)) != KSCHED_OK) break;
     cluster_collect_kernel<<<1, 64, 0, h->stream>>>(h->d_counters.ptr, P, h->d_nn_tmpl.ptr, h->d_nn_count.ptr, h->d_nn_req.ptr, h->d_nn_req_present.ptr,
                                                     h->d_nn_vals.ptr, h->d_nn_meta.ptr, h->d_nn_opts.ptr, h->st.max_new, W32, h->d_sim_results.ptr + q,
                                                     h->d_sim_types.ptr + (size_t)q * W32);
@@ -1799,6 +1844,101 @@ int ksched_simulate_batch(ksched_handle* h, const ksched_candidate_set* sets, in
       std::memset(node0_types + (size_t)q * W64, 0, (size_t)W64 * 8);
       if (d.n_new_nodes >= 1) std::memcpy(node0_types + (size_t)q * W64, &types[(size_t)q * W32], (size_t)W32 * 4);
     }
+  }
+  return KSCHED_OK;
+}
+
+int ksched_simulate_full(ksched_handle* h, const ksched_candidate_set* sets, int n_sets, ksched_result* results) {
+  if (!h || !sets || n_sets < 0 || (n_sets > 0 && !results)) return KSCHED_ERR_INVALID;
+  if (!h->have_cluster) { h->err = "ksched_load_cluster must be called first"; return KSCHED_ERR_INVALID; }
+  if (n_sets == 0) return KSCHED_OK;
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  const int NE = h->st.n_existing, W32 = h->cat.W32, W64 = W32 / 2, X = h->cat.n_res_ext;
+  std::vector<int32_t> node_off, batch;
+  int rc = stage_sets(h, sets, n_sets, true, node_off, batch);
+  if (rc != KSCHED_OK) return rc;
+  // the sets' staging regions (one per set, `batch` pods and as many new nodes) and their slot maps
+  std::vector<size_t> off((size_t)n_sets + 1, 0);
+  std::vector<int32_t> slot_map((size_t)n_sets * std::max(NE, 1), 0);
+  for (int q = 0; q < n_sets; ++q) {
+    const ksched_result& r = results[q];
+    if (sets[q].capacity < batch[(size_t)q]) {
+      h->err = "result of set " + std::to_string(q) + " holds " + std::to_string(sets[q].capacity) + " pods, its batch has " + std::to_string(batch[(size_t)q]);
+      return KSCHED_ERR_INVALID;
+    }
+    if (!r.assign || !r.relax_level || !r.place_seq || !r.new_nodes || !r.new_node_types) { h->err = "a result array is missing"; return KSCHED_ERR_INVALID; }
+    if (r.launch && !h->cat.offer_keys) { h->err = "ksched_result.launch needs ksched_catalog.offering_keys"; return KSCHED_ERR_INVALID; }
+    off[(size_t)q + 1] = off[(size_t)q] + (size_t)std::max(batch[(size_t)q], 1);
+    int32_t* map = &slot_map[(size_t)q * NE];
+    for (int i = node_off[(size_t)q]; i < node_off[(size_t)q + 1]; ++i) map[sets[q].nodes[i - node_off[(size_t)q]]] = -1;
+    for (int e = 0, stay = 0; e < NE; ++e) if (map[e] == 0) map[e] = stay++; else map[e] = -1;
+  }
+  const size_t total = off[(size_t)n_sets];
+  if (!slot_map.empty()) CUDA_TRY(h, upload_vec(h, h->d_slot_map, slot_map));
+  CUDA_TRY(h, h->d_full_i32.ensure(3 * total));
+  CUDA_TRY(h, h->d_full_nodes.ensure(total));
+  CUDA_TRY(h, h->d_full_types.ensure(total * W64));
+  CUDA_TRY(h, h->d_full_ext.ensure(total * std::max(X, 1)));
+  CUDA_TRY(h, h->d_full_ext_present.ensure(total));
+  CUDA_TRY(h, h->d_full_launch.ensure(total));
+  CUDA_TRY(h, h->d_full_scalars.ensure((size_t)n_sets));
+  CUDA_TRY(h, cudaEventRecord(h->ev[0], h->stream));
+  bool class_pass = true;
+  for (int q = 0; q < n_sets && rc == KSCHED_OK; ++q) {
+    const int P = batch[(size_t)q], n_nodes = node_off[(size_t)q + 1] - node_off[(size_t)q];
+    // simulateScheduling places every pod: no stop after a second new node
+    if ((rc = run_simulation(h, q, node_off, P, class_pass, 0)) != KSCHED_OK) break;
+    class_pass = class_pass && P == 0;  // K1's class pass returns early on an empty batch
+    const size_t o = off[(size_t)q];
+    if (results[q].launch)
+      launch_choice_kernel<<<h->n_sm, 256, 0, h->stream>>>(h->cat, h->d_counters.ptr, h->d_nn_vals.ptr, h->d_nn_meta.ptr, h->d_nn_opts.ptr, h->st.max_new,
+                                                           h->d_full_launch.ptr + o);
+    SimFullOut out{h->d_full_i32.ptr + o, h->d_full_i32.ptr + total + o, h->d_full_i32.ptr + 2 * total + o, h->d_full_nodes.ptr + o,
+                   h->d_full_types.ptr + o * W64, X ? h->d_full_ext.ptr + o * X : nullptr, h->d_full_ext_present.ptr + o, h->d_full_scalars.ptr + q};
+    int removed_pods = 0;
+    for (int i = 0; i < n_nodes; ++i) removed_pods += h->h_node_count[(size_t)sets[q].nodes[i]];
+    cluster_full_collect_kernel<<<1, 256, 0, h->stream>>>(h->d_counters.ptr, P, h->sup_pending, h->sup_lead, removed_pods, h->d_assign.ptr, h->d_relax.ptr,
+                                                          h->d_place_seq.ptr, h->d_slot_map.ptr + (size_t)q * NE, h->d_node_init.ptr, NE, NE - n_nodes,
+                                                          h->d_nn_tmpl.ptr, h->d_nn_count.ptr, h->d_nn_req.ptr, h->d_nn_req_present.ptr, h->d_nn_vals.ptr,
+                                                          h->d_nn_meta.ptr, h->d_nn_opts.ptr, h->d_nn_req_ext.ptr, h->d_nn_ext_present.ptr, h->st.max_new, W32,
+                                                          X, out);
+    CUDA_TRY(h, cudaGetLastError());
+  }
+  if (rc != KSCHED_OK) return rc;
+  CUDA_TRY(h, cudaEventRecord(h->ev[4], h->stream));
+  // every set's arrays straight into the caller's buffers (capacity-sized: the counts are not known before the one
+  // synchronisation), then the scalars
+  std::vector<SimFullDev> sc((size_t)n_sets);
+  for (int q = 0; q < n_sets; ++q) {
+    ksched_result& r = results[q];
+    const size_t o = off[(size_t)q], P = (size_t)batch[(size_t)q];
+    if (P == 0) continue;
+    CUDA_TRY(h, download(h, r.assign, h->d_full_i32.ptr + o, P));
+    CUDA_TRY(h, download(h, r.relax_level, h->d_full_i32.ptr + total + o, P));
+    CUDA_TRY(h, download(h, r.place_seq, h->d_full_i32.ptr + 2 * total + o, P));
+    CUDA_TRY(h, download(h, r.new_nodes, h->d_full_nodes.ptr + o, P));
+    CUDA_TRY(h, download(h, r.new_node_types, h->d_full_types.ptr + o * W64, P * W64));
+    if (r.launch) CUDA_TRY(h, download(h, r.launch, h->d_full_launch.ptr + o, P));
+    if (X && r.new_node_requests_ext) CUDA_TRY(h, download(h, r.new_node_requests_ext, h->d_full_ext.ptr + o * X, P * X));
+    if (X && r.new_node_requests_ext_present) CUDA_TRY(h, download(h, r.new_node_requests_ext_present, h->d_full_ext_present.ptr + o, P));
+  }
+  CUDA_TRY(h, download(h, sc.data(), h->d_full_scalars.ptr, sc.size()));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaGetLastError());
+  h->tm.total_us = ev_us(h->ev[0], h->ev[4]);
+  for (int q = 0; q < n_sets; ++q) {
+    const SimFullDev& d = sc[(size_t)q];
+    if (d.error != 0) {
+      h->err = "set " + std::to_string(q) + ": " + (d.error == KSCHED_ERR_OVERFLOW ? "new-node capacity exceeded" : "a pod is constrained by more topology groups than the kernel supports");
+      return d.error;
+    }
+    ksched_result& r = results[q];
+    r.n_new_nodes = d.n_new_nodes;
+    r.n_unscheduled = d.n_unscheduled;
+    r.nodes_visited = d.nodes_visited;
+    r.add_calls = d.add_calls;
+    r.all_pods_scheduled = d.all_pods_scheduled;
+    r.uninitialized_existing = d.uninitialized_existing;
   }
   return KSCHED_OK;
 }

@@ -283,6 +283,10 @@ struct Result {
   int64_t nodes_visited = 0;  // sum over Add attempts of candidate nodes examined (SURVEY 8d K2 bytes)
   int64_t add_calls = 0;      // number of Scheduler.add calls (queue pops)
   std::string error;
+  // simulateScheduling's verdicts (deprovisioning/helpers.go:96-114), set by the GPU path's Solve and simulations: every pod
+  // was placed, and an existing node of the result is not initialised (the reference then returns nil, false)
+  bool all_pods_scheduled = false;
+  bool uninitialized_existing = false;
 };
 
 // InstanceTypeOptions of a new node: its own list, or the shared one it names

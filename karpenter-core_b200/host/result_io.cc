@@ -56,6 +56,8 @@ long long kh_result_num_new_nodes(const Result* r) { return (long long)r->new_no
 long long kh_result_num_existing(const Result* r) { return (long long)r->existing_node_index.size(); }
 long long kh_result_nodes_visited(const Result* r) { return r->nodes_visited; }
 long long kh_result_add_calls(const Result* r) { return r->add_calls; }
+int kh_result_all_pods_scheduled(const Result* r) { return r->all_pods_scheduled ? 1 : 0; }
+int kh_result_uninitialized_existing(const Result* r) { return r->uninitialized_existing ? 1 : 0; }
 void kh_result_assign(const Result* r, int* out) { std::memcpy(out, r->assign.data(), r->assign.size() * sizeof(int32_t)); }
 void kh_result_relax(const Result* r, int* out) { std::memcpy(out, r->relax_level.data(), r->relax_level.size() * sizeof(int32_t)); }
 // per new node: [provisioner, n_pods, n_options]

@@ -77,8 +77,10 @@ struct ResultBuffers {
   // ksched_solve overwrites every per-pod entry and the rows of the nodes it reports (ksched_download), decode reads nothing
   // else: the buffers are sized, not cleared - kh_scheduler_solve keeps one set per thread, so a 100 000-pod Solve does not
   // fault in and zero ~35 MB per call.
-  void prepare(const Encoded& E, bool want_feasibility) {
-    const size_t P = E.pods.size(), N = (size_t)std::max(1, E.problem.max_new_nodes);
+  // pods: the batch the buffers hold, E's own unless a simulation's on a superset encoding (which can open as many nodes)
+  void prepare(const Encoded& E, bool want_feasibility, size_t pods = SIZE_MAX) {
+    const size_t P = pods == SIZE_MAX ? E.pods.size() : pods;
+    const size_t N = (size_t)std::max(1, pods == SIZE_MAX ? E.problem.max_new_nodes : (int)pods);
     assign.resize(P);
     relax.resize(P);
     seq.resize(P);
@@ -113,13 +115,14 @@ struct ResultBuffers {
 
 // ksched_result -> the reference's ([]*Node, []*ExistingNode) shape (node.go:34-40, existingnode.go:28-39). The per-node part
 // (pods in Add order, requests, rendered requirements, launch choice) is independent node by node and runs on all host cores.
-void decode(const Encoded& E, const ResultBuffers& B, Result& out) {
-  const size_t P = E.pods.size(), NE = E.existing.size(), NN = (size_t)B.r.n_new_nodes, NA = NE + NN;
+// P pods and the existing nodes `existing_index` (Problem.nodes indices): E's own, or a simulation's on a superset encoding.
+void decode(const Encoded& E, const ResultBuffers& B, size_t P, const std::vector<int>& existing_index, Result& out) {
+  const size_t NE = existing_index.size(), NN = (size_t)B.r.n_new_nodes, NA = NE + NN;
   out.assign.assign(B.assign.begin(), B.assign.begin() + (ptrdiff_t)P);
   out.relax_level.assign(B.relax.begin(), B.relax.begin() + (ptrdiff_t)P);
   out.nodes_visited = B.r.nodes_visited;
   out.add_calls = B.r.add_calls;
-  out.existing_node_index = E.existing_state_index;
+  out.existing_node_index = existing_index;
   out.existing_pods.assign(NE, {});
   out.new_nodes.assign(NN, {});
   // pods per node in Add order: place_seq is a permutation of 0..placed-1 over the placed pods. Counting sort by node, then
@@ -215,6 +218,13 @@ void decode(const Encoded& E, const ResultBuffers& B, Result& out) {
     }
   });
 }
+void decode(const Encoded& E, const ResultBuffers& B, Result& out) { decode(E, B, E.pods.size(), E.existing_state_index, out); }
+
+// simulateScheduling's verdicts on a Solve of E (helpers.go:96-114): every pod placed; an existing node not initialised
+void set_verdicts(const Encoded& E, const ResultBuffers& B, Result& out) {
+  out.all_pods_scheduled = B.r.n_unscheduled == 0;
+  out.uninitialized_existing = std::find(E.existing_initialized.begin(), E.existing_initialized.end(), false) != E.existing_initialized.end();
+}
 
 int error_code(const std::exception& e) {
   std::string m = e.what();
@@ -298,6 +308,7 @@ int kh_scheduler_solve(const Problem* P, const int* candidates, int ncand, Resul
     int rc = solve_encoded(*E, B, false);
     if (rc != KSCHED_OK) { out->error = g_err; return rc; }
     decode(*E, B, *out);
+    set_verdicts(*E, B, *out);
     return KSCHED_OK;
   } catch (const std::exception& e) {
     out->error = e.what();
@@ -753,13 +764,25 @@ Cmd compute_consolidation_encoded(const Problem* P, const std::vector<Cand>& sel
   return finish_command(P, *E, sel, scheduled == E->pods.size(), B.r.n_new_nodes, B.nodes[0].reqs, &B.types[0], multi);
 }
 
-// ksched_load_catalog + ksched_load_cluster of a superset encoding (khost::encode(..., true)) on h
-int load_snapshot(ksched_handle* h, Encoded& E) {
+// ksched_load_catalog + ksched_load_cluster of a superset encoding (khost::encode(..., true)) of the candidates `cands`
+// (Problem.nodes indices) on h
+int load_snapshot(ksched_handle* h, Encoded& E, const std::vector<int>& cands) {
   int rc = ksched_load_catalog(h, &E.catalog);
   if (rc != KSCHED_OK) return rc;
   ksched_cluster cl{};
   cl.problem = &E.problem;
   cl.pod_node = E.pod_node.data();
+  // what a full simulation needs: the candidates' slots, the initialised nodes, and Solve's pod order (helpers.go:74-88:
+  // the pending pods, the candidates' pods, the pods of nodes marked for deletion)
+  const std::set<int> cand(cands.begin(), cands.end());
+  std::vector<uint8_t> removable, initialized;
+  for (size_t e = 0; e < E.existing.size(); ++e) {
+    removable.push_back(cand.count(E.existing_state_index[e]) ? 1 : 0);
+    initialized.push_back(E.existing_initialized[e] ? 1 : 0);
+  }
+  cl.node_removable = removable.data();
+  cl.node_initialized = initialized.data();
+  cl.n_pending_lead = (int32_t)E.problem_ref->pods.size();
   if (E.problem.n_groups > 0) {
     cl.class_count_begin = E.class_count_begin.data();
     cl.class_count = E.class_count.data();
@@ -777,26 +800,31 @@ struct SimBatch {
   std::vector<uint64_t> types;  // [simulation][type_words]: the first new node's InstanceTypeOptions
   std::vector<char> skip;
 };
+// scheduler.go:221-248 only charges the nodes that stay: the provisioner limits left when the existing slots `slots` of E's
+// snapshot are removed - the exact remaining with their capacity given back, then held at remaining_minus's floor like a
+// Solve's
+std::vector<int64_t> remaining_without(const Encoded& E, const std::vector<int32_t>& slots) {
+  std::vector<__int128> exact = E.remaining_exact;
+  for (int32_t e : slots) {
+    const int v = E.existing_template[(size_t)e];
+    if (v >= 0) for (int r = 0; r < KSCHED_MAX_RES; ++r) exact[(size_t)v * KSCHED_MAX_RES + r] += E.existing_capacity[(size_t)e * KSCHED_MAX_RES + r];
+  }
+  std::vector<int64_t> rem(exact.size());
+  for (size_t i = 0; i < exact.size(); ++i) rem[i] = exact[i] < -kQuantityBound ? -kQuantityBound : (int64_t)exact[i];
+  return rem;
+}
+
 SimBatch simulate_on(ksched_handle* h, const Encoded& E, const std::vector<std::vector<int32_t>>& slot_sets) {
-  const size_t n = slot_sets.size(), NE = E.existing.size(), V = E.templates.size();
+  const size_t n = slot_sets.size(), NE = E.existing.size();
   SimBatch out;
   out.skip.assign(n, 0);
   std::vector<std::vector<int64_t>> rem(n);
   std::vector<ksched_candidate_set> cs(n);
   std::vector<char> removed(NE);
-  std::vector<__int128> exact;
   for (size_t q = 0; q < n; ++q) {
     std::fill(removed.begin(), removed.end(), 0);
-    // scheduler.go:221-248 only charges the nodes that stay: the exact remaining with the removed nodes' capacity given
-    // back, then held at remaining_minus's floor like a Solve's
-    exact = E.remaining_exact;
-    for (int32_t e : slot_sets[q]) {
-      removed[(size_t)e] = 1;
-      const int v = E.existing_template[(size_t)e];
-      if (v >= 0) for (int r = 0; r < KSCHED_MAX_RES; ++r) exact[(size_t)v * KSCHED_MAX_RES + r] += E.existing_capacity[(size_t)e * KSCHED_MAX_RES + r];
-    }
-    rem[q].resize(V * KSCHED_MAX_RES);
-    for (size_t i = 0; i < V * KSCHED_MAX_RES; ++i) rem[q][i] = exact[i] < -kQuantityBound ? -kQuantityBound : (int64_t)exact[i];
+    for (int32_t e : slot_sets[q]) removed[(size_t)e] = 1;
+    rem[q] = remaining_without(E, slot_sets[q]);
     for (size_t e = 0; e < NE; ++e) if (!removed[e] && !E.existing_initialized[e]) out.skip[q] = 1;
     cs[q] = ksched_candidate_set{slot_sets[q].data(), (int32_t)slot_sets[q].size(), 0, rem[q].data()};
   }
@@ -860,7 +888,7 @@ struct ValidationSnapshot {
     h.reset(raw);
     auto sup = khost::encode(*A, cands, true);
     sup->problem.count_nodes_visited = 0;
-    int rc = load_snapshot(h.get(), *sup);
+    int rc = load_snapshot(h.get(), *sup, cands);
     if (rc == KSCHED_ERR_UNSUPPORTED) return;  // resident stays false
     if (rc != KSCHED_OK) throw std::runtime_error(ksched_last_error(h.get()));
     E = std::move(sup);
@@ -932,7 +960,7 @@ struct ClusterSession {
     auto sup = khost::encode(*P, nodes, true);
     sup->problem.count_nodes_visited = 0;
     handle_taken();
-    int rc = load_snapshot(g_handle, *sup);
+    int rc = load_snapshot(g_handle, *sup, nodes);
     if (rc == KSCHED_ERR_UNSUPPORTED) return;  // resident stays false
     if (rc != KSCHED_OK) throw std::runtime_error(ksched_last_error(g_handle));
     E = std::move(sup);
@@ -962,12 +990,7 @@ struct ClusterSession {
         if (e < 0) throw std::runtime_error("candidate is not an existing node of the snapshot");
         slots[q].push_back(e);
       }
-    if (g_resident_session != id) {  // displaced: the time of one reload, the same answers
-      if (ensure_handle() != KSCHED_OK) throw std::runtime_error(g_err);
-      handle_taken();
-      if (load_snapshot(g_handle, *E) != KSCHED_OK) throw std::runtime_error(ksched_last_error(g_handle));
-      g_resident_session = id;
-    }
+    make_current();
     SimBatch sb = simulate_on(g_handle, *E, slots);
     for (size_t q = 0; q < sets.size(); ++q) {
       if (sb.skip[q]) continue;
@@ -977,6 +1000,79 @@ struct ClusterSession {
     }
     return out;
   }
+  // the session's snapshot on g_handle again when something else displaced it: the time of one reload, the same answers
+  void make_current() {
+    if (g_resident_session == id) return;
+    if (ensure_handle() != KSCHED_OK) throw std::runtime_error(g_err);
+    handle_taken();
+    std::vector<int> nodes;
+    for (auto& c : cands) nodes.push_back(c.node);
+    if (load_snapshot(g_handle, *E, nodes) != KSCHED_OK) throw std::runtime_error(ksched_last_error(g_handle));
+    g_resident_session = id;
+  }
+
+  // simulateScheduling's whole result for every set (Problem.nodes indices, candidates of the session, in the caller's
+  // order): one ksched_simulate_full call, each result decoded as kh_scheduler_solve decodes a Solve of that set
+  std::vector<Result> simulate(const std::vector<std::vector<int>>& sets) {
+    std::vector<int> position(P->nodes.size(), -1);
+    for (size_t i = 0; i < cands.size(); ++i) position[(size_t)cands[i].node] = (int)i;
+    for (auto& set : sets)
+      for (int n : set) {
+        if (n < 0 || (size_t)n >= P->nodes.size()) throw std::runtime_error("node index out of range");
+        if (P->nodes[(size_t)n].marked_for_deletion) throw std::runtime_error("a candidate node is marked for deletion");  // errCandidateNodeDeleting
+        if (position[(size_t)n] < 0) throw std::runtime_error("node " + std::to_string(n) + " is not a candidate of the session");
+        if (std::count(set.begin(), set.end(), n) > 1) throw std::runtime_error("node " + std::to_string(n) + " is repeated in a set");
+      }
+    simulations += (int)sets.size();
+    std::vector<Result> out(sets.size());
+    if (!resident) {
+      for (size_t q = 0; q < sets.size(); ++q) {
+        auto F = khost::encode(*P, sets[q]);
+        F->problem.count_nodes_visited = g_count_visited;
+        ResultBuffers B;
+        if (solve_encoded(*F, B, false) != KSCHED_OK) throw std::runtime_error(g_err);
+        decode(*F, B, out[q]);
+        set_verdicts(*F, B, out[q]);
+      }
+      return out;
+    }
+    const size_t n = sets.size(), NE = E->existing.size();
+    std::vector<std::vector<int32_t>> slots(n);
+    std::vector<std::vector<int64_t>> rem(n);
+    std::vector<ksched_candidate_set> cs(n);
+    std::vector<ResultBuffers> B(n);
+    std::vector<size_t> pods_in_batch(n);
+    size_t pending = 0;
+    std::vector<size_t> node_pods(NE, 0);  // the snapshot's pods per slot
+    for (int32_t e : E->pod_node) if (e >= 0) ++node_pods[(size_t)e]; else ++pending;
+    for (size_t q = 0; q < n; ++q) {
+      pods_in_batch[q] = pending;
+      for (int i : sets[q]) {
+        slots[q].push_back(slot_of_node[(size_t)i]);
+        pods_in_batch[q] += node_pods[(size_t)slots[q].back()];
+      }
+      rem[q] = remaining_without(*E, slots[q]);
+      B[q].prepare(*E, false, pods_in_batch[q]);
+      cs[q] = ksched_candidate_set{slots[q].data(), (int32_t)slots[q].size(), (int32_t)pods_in_batch[q], rem[q].data()};
+    }
+    make_current();
+    std::vector<ksched_result> res(n);
+    for (size_t q = 0; q < n; ++q) res[q] = B[q].r;
+    if (ksched_simulate_full(g_handle, cs.data(), (int)n, res.data()) != KSCHED_OK) throw std::runtime_error(ksched_last_error(g_handle));
+    std::vector<char> removed(P->nodes.size(), 0);
+    for (size_t q = 0; q < n; ++q) {
+      B[q].r = res[q];
+      for (int i : sets[q]) removed[(size_t)i] = 1;
+      std::vector<int> existing_index;
+      for (int si : E->existing_state_index) if (!removed[(size_t)si]) existing_index.push_back(si);
+      for (int i : sets[q]) removed[(size_t)i] = 0;
+      decode(*E, B[q], pods_in_batch[q], existing_index, out[q]);
+      out[q].all_pods_scheduled = res[q].all_pods_scheduled != 0;
+      out[q].uninitialized_existing = res[q].uninitialized_existing != 0;
+    }
+    return out;
+  }
+
   Cmd compute_prefix(int count) {
     std::vector<int> set;
     for (int i = 0; i < count; ++i) set.push_back(i);
@@ -1109,6 +1205,24 @@ int kh_cluster_probe_sets(ClusterSession* cs, const int* sets, const int* set_of
       n_options[q] = (int)cmds[(size_t)q].options.size();
       for (size_t i = 0; i < cmds[(size_t)q].options.size() && (int)i < options_stride; ++i) options[(size_t)q * options_stride + i] = cmds[(size_t)q].options[i];
     }
+    return KSCHED_OK;
+  } catch (const std::exception& e) {
+    return fail(error_code(e), e.what());
+  }
+}
+// simulateScheduling's whole result for n_sets candidate sets in ONE ksched_simulate_full call (ClusterSession::simulate).
+// set q = sets[set_off[q] .. set_off[q+1]) as Problem.nodes indices; out[q] = what kh_scheduler_solve returns for that set.
+int kh_cluster_simulate(ClusterSession* cs, const int* sets, const int* set_off, int n_sets, Result** out) {
+  try {
+    if (!cs || n_sets < 0 || (n_sets > 0 && (!set_off || !out || set_off[0] < 0))) return fail(KSCHED_ERR_INVALID, "n_sets / set_off out of range");
+    std::vector<std::vector<int>> v((size_t)n_sets);
+    for (int q = 0; q < n_sets; ++q) {
+      if (set_off[q + 1] < set_off[q]) return fail(KSCHED_ERR_INVALID, "set_off must be non-decreasing");
+      if (!out[q]) return fail(KSCHED_ERR_INVALID, "a result is missing");
+      v[(size_t)q].assign(sets + set_off[q], sets + set_off[q + 1]);
+    }
+    auto res = cs->simulate(v);
+    for (int q = 0; q < n_sets; ++q) *out[q] = std::move(res[(size_t)q]);
     return KSCHED_OK;
   } catch (const std::exception& e) {
     return fail(error_code(e), e.what());

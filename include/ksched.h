@@ -475,6 +475,10 @@ typedef struct ksched_timings {
   int32_t pad;
   int64_t h2d_bytes, d2h_bytes; /* host<->device bytes moved by the last ksched_solve (upload + download) */
   double class_feasibility_us;  /* ksched_run_feasibility_only: the per-class row evaluations that precede the dense-matrix kernel */
+  /* the last downloaded Solve: the pack kernel's variant table (first block's start to last block's end of its build, in the
+     row gather's launch), the class runs' variants fetched from it and those derived inside the pack kernel */
+  double vt_build_us;
+  int64_t vt_fetches, run_derives;
 } ksched_timings;
 
 typedef struct ksched_handle ksched_handle;

@@ -45,7 +45,8 @@ class Timings(C.Structure):
                 ("download_us", C.c_double), ("total_us", C.c_double), ("allreduce_us", C.c_double),
                 ("feasibility_bytes", C.c_int64), ("pack_steps", C.c_int64),
                 ("feasibility_launches", C.c_int32), ("pack_launches", C.c_int32), ("sort_launches", C.c_int32), ("pad", C.c_int32),
-                ("h2d_bytes", C.c_int64), ("d2h_bytes", C.c_int64), ("class_feasibility_us", C.c_double)]
+                ("h2d_bytes", C.c_int64), ("d2h_bytes", C.c_int64), ("class_feasibility_us", C.c_double),
+                ("vt_build_us", C.c_double), ("vt_fetches", C.c_int64), ("run_derives", C.c_int64)]
 
     def as_dict(self):
         return {k: getattr(self, k) for k, _ in self._fields_ if k != "pad"}

@@ -16,12 +16,20 @@ __global__ void sort_key1_kernel(int n, const uint32_t* __restrict__ cls_rank, c
   key[i] = ((uint64_t)cls_rank[pod_class[i]] << (ts_bits + uid_bits)) | ((uint64_t)(ts[i] - ts_min) << uid_bits) | (uint64_t)uid_rank[i];
   idx[i] = (uint32_t)i;
 }
+__device__ void vt_build_block(int b);  // pack_kernel.cuh
 // FFD-ordered dense pod-row matrix: row j = class row of the j-th pod of the queue. One warp per row,
-// 256-byte coalesced loads and stores.
+// 256-byte coalesced loads and stores. kTable: the blocks from `blocks` on build the pack kernel's variant table
+// (vt_build_block), which depends on nothing this launch writes; the launches without a table keep the gather's small
+// register and shared-memory footprint.
+template <bool kTable>
 __global__ void gather_rows_kernel(int n, const ksched_pod_row* __restrict__ classes, const uint32_t* __restrict__ pod_class,
-                                   const uint32_t* __restrict__ order, uint64_t* __restrict__ rows) {
+                                   const uint32_t* __restrict__ order, uint64_t* __restrict__ rows, int blocks) {
+  if (kTable && (int)blockIdx.x >= blocks) {
+    vt_build_block((int)blockIdx.x - blocks);
+    return;
+  }
   int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  int nwarps = (gridDim.x * blockDim.x) >> 5;
+  int nwarps = (blocks * blockDim.x) >> 5;
   for (int j = warp; j < n; j += nwarps) {
     const uint64_t* src = reinterpret_cast<const uint64_t*>(&classes[pod_class[order[j]]]);
     rows[(size_t)j * KSCHED_ROW_WORDS + lane] = src[lane];

@@ -69,8 +69,9 @@ enum Counter : int {
   kCtrPinSteps, kCtrPinPods, kCtrPinEndStaged, kCtrPinEndCount, kCtrPinEndKey, kCtrPinEndRefused, kCtrPinEndList,
   kCtrRoundTripCycles,
   kCtrNoVariantStops, kCtrStopRoomSlow, kCtrStopCapacity, kCtrStopOther,  // status-1 stops by StopCause (in that order)
-  kCtrNoVariantTripCycles, kCtrVarStoreHits, kCtrVarStoreEntries, kCtrRunCaptures,
-  kCtrRunDerives, kCtrRunDeriveCycles, kCtrRunDeriveRefused,  // variants derived inside a class run (run_derive)
+  kCtrNoVariantTripCycles, kCtrVtFetches, kCtrVtEntries, kCtrRunCaptures,  // variant table: fetches (always), entries built (profile)
+  kCtrVtStart, kCtrVtEnd,  // variant table build: ~first start, last end (globaltimer ns)
+  kCtrRunDerives, kCtrRunDeriveCycles, kCtrRunDeriveRefused,  // variants derived inside a class run (run_derive; the count always)
   kCtrRoundCycles, kCtrRounds, kCtrRoundPods,
   kCtrStretchPinned, kCtrStretchFresh = kCtrStretchPinned + 16,  // round stretches by length 1..16
   kCtrMaskSteps = kCtrStretchFresh + 16, kCtrMaskMultiDomain, kCtrMaskRoundable,
@@ -211,6 +212,7 @@ struct ksched_handle {
   DevBuf<uint64_t> d_offer_keys, d_slots;
   // ---- problem (ksched_upload): `st` points into the buffers of this group; reset_state restores the `resets` segments
   bool uploaded = false;
+  int vt_ndom = 1;  // variant table: domain ids below it have entries (1 + the largest registered id below kM1Dom at upload)
   bool sorted = false;  // the FFD-ordered pod-row matrix of the uploaded problem exists
   PackState st{};
   ResetTable resets{};
@@ -264,7 +266,8 @@ struct ksched_handle {
   DevBuf<unsigned long long> d_ov_key;
   DevBuf<unsigned short> d_ov_flags;
   DevBuf<long long> d_ov_q, d_ov_bound, d_ov_bound2, d_fc_bound, d_fc_bound2, d_fc_q, d_fd_bound, d_fd_bound2;
-  DevBuf<VarStoreEntry> d_vstore;
+  DevBuf<RunVariant> d_vtable;
+  DevBuf<uint32_t> d_vt_ok;
   // ---- device-resident cluster snapshot (ksched_load_cluster)
   bool have_cluster = false;
   int sup_pods = 0, sup_pending = 0;
@@ -408,7 +411,8 @@ int ksched_create(int device_ordinal, ksched_handle** out) {
     cudaFuncGetAttributes(&fa, feasibility_kernel);
     cudaFuncGetAttributes(&fa, class_feasibility_kernel);
     cudaFuncGetAttributes(&fa, finalize_options_kernel);
-    cudaFuncGetAttributes(&fa, gather_rows_kernel);
+    cudaFuncGetAttributes(&fa, gather_rows_kernel<false>);
+    cudaFuncGetAttributes(&fa, gather_rows_kernel<true>);
     cudaFuncGetAttributes(&fa, sort_key1_kernel);
   }
   *out = h;
@@ -1082,11 +1086,13 @@ static int bind_problem(ksched_handle* h, const ksched_problem* pb) {
   {
     std::vector<int32_t> host_row(ng, -1), host_total(ng, 0), cnt(ng * 64, 0);
     std::vector<uint64_t> registered(ng, 0);
+    h->vt_ndom = 1;
     std::vector<uint8_t> active(ng, 1);
     int nh = 0;
     for (int g = 0; g < NG; ++g) {
       if (pb->groups[g].key == KSCHED_KEY_HOSTNAME) host_row[g] = nh++;
       registered[g] = pb->groups[g].registered;
+      for (int d = 1; d < kM1Dom; ++d) if ((registered[g] >> d) & 1) h->vt_ndom = std::max(h->vt_ndom, d + 1);
       active[g] = pb->groups[g].dormant ? 0 : 1;
       for (int d = 0; d < 64; ++d) cnt[(size_t)g * 64 + d] = pb->group_domain_counts[(size_t)g * 64 + d];
     }
@@ -1192,7 +1198,11 @@ static int bind_problem(ksched_handle* h, const ksched_problem* pb) {
   CUDA_TRY(h, bind(h, h->d_fd_bound2, s.fd_bound2, (size_t)kFreshMemoSlots * 4));
   CUDA_TRY(h, bind(h, h->d_remaining, s.remaining, (size_t)V * KSCHED_MAX_RES));  // reset_state: limits per call
   CUDA_TRY(h, bind_zeroed(h, h->d_counters, s.counters, kNumCounters));
-  CUDA_TRY(h, bind(h, h->d_vstore, s.vstore, kVarStore));
+  {  // the variant table's capacity is fixed here: the first kVtClasses classes
+    const size_t n = (size_t)std::max(1, std::min(s.n_classes, kVtClasses)) * kM1Dom;
+    CUDA_TRY(h, bind(h, h->d_vtable, s.vtable, n));
+    CUDA_TRY(h, bind_zeroed(h, h->d_vt_ok, s.vt_ok, n));
+  }
   {
     size_t need = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, need, (uint64_t*)nullptr, (uint64_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)p1, 0, 64, h->stream);
@@ -1220,7 +1230,14 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
 }
 
 // K0 over the first P pods (a simulation's batch, otherwise the whole problem); so are run_class_feasibility and run_feasibility.
-static int run_sort(ksched_handle* h, int P) {
+// g_k2 is one __constant__ object per device: a launch may only overwrite it after the previous launch that reads it (the pack kernel, the variant table build) on that
+// device (possibly of another handle, on another stream) has finished. Ordered on the device, never on the host.
+static std::mutex g_k2_mu;
+static cudaEvent_t g_k2_done[64] = {};
+static int set_k2(ksched_handle* h, int n_pods, int stop_new_nodes, bool with_table);
+// with_table: the row gather's launch also builds the pack kernel's variant table (vt_build_block), for the pack launch
+// that follows with the same flag
+static int run_sort(ksched_handle* h, int P, bool with_table = false) {
   if (P == 0) return KSCHED_OK;
   const int threads = 256, blocks = (P + threads - 1) / threads;
   // one packed key (bind_problem), only its significant bits sorted
@@ -1230,7 +1247,17 @@ static int run_sort(ksched_handle* h, int P) {
   CUDA_TRY(h, cub::DeviceRadixSort::SortPairs(h->d_cub_tmp.ptr, tmp, h->d_k_tie.ptr, h->d_k_tmp.ptr, h->d_idx_tmp.ptr, h->d_order.ptr, P, 0, h->sort1_bits,
                                               h->stream));
   const int gblocks = std::min((P + 7) / 8, h->n_sm * 8);
-  gather_rows_kernel<<<gblocks, 256, 0, h->stream>>>(P, h->d_classes.ptr, h->d_pod_class.ptr, h->d_order.ptr, h->d_rows.ptr);
+  if (with_table) {  // g_k2 is read by the table blocks: the same lock and ordering as run_pack
+    std::lock_guard<std::mutex> lock(g_k2_mu);
+    int rc = set_k2(h, P, 0, true);
+    if (rc != KSCHED_OK) return rc;
+    const int vt_blocks = h->k2_host.st.vt_classes * h->vt_ndom;
+    gather_rows_kernel<true><<<gblocks + vt_blocks, 256, 0, h->stream>>>(P, h->d_classes.ptr, h->d_pod_class.ptr, h->d_order.ptr, h->d_rows.ptr, gblocks);
+    CUDA_TRY(h, cudaGetLastError());
+    CUDA_TRY(h, cudaEventRecord(g_k2_done[h->device], h->stream));
+  } else {
+    gather_rows_kernel<false><<<gblocks, 256, 0, h->stream>>>(P, h->d_classes.ptr, h->d_pod_class.ptr, h->d_order.ptr, h->d_rows.ptr, gblocks);
+  }
   h->tm.sort_launches = 3;
   h->sorted = true;
   return KSCHED_OK;
@@ -1364,13 +1391,10 @@ static int reset_state(ksched_handle* h, const int64_t* sim_remaining = nullptr)
   return KSCHED_OK;
 }
 
-// g_k2 is one __constant__ object per device: a launch may only overwrite it after the previous pack kernel on that
-// device (possibly of another handle, on another stream) has finished. Ordered on the device, never on the host.
-static std::mutex g_k2_mu;
-static cudaEvent_t g_k2_done[64] = {};
 
-// The pack kernel over the first n_pods pods of the queue (a simulation's batch, otherwise the whole problem).
-static int run_pack(ksched_handle* h, int n_pods, int stop_new_nodes) {
+// The pack kernel's parameters into g_k2 (caller holds g_k2_mu), once the previous reader of g_k2 on the device is done.
+// with_table: the launch replays the variant table a run_sort(with_table) of this Solve built.
+static int set_k2(ksched_handle* h, int n_pods, int stop_new_nodes, bool with_table) {
   K2Params& k2 = h->k2_host;
   k2.cat = h->cat;
   k2.st = h->st;
@@ -1386,28 +1410,38 @@ static int run_pack(ksched_handle* h, int n_pods, int stop_new_nodes) {
   const size_t smem_left = (size_t)(227 << 10) - sizeof(HotSmem) - kRunArrayBytes - static_smem;
   s.alloc_in_smem = alloc_bytes <= smem_left ? 1 : 0;
   s.run_off = s.alloc_in_smem ? (int)((alloc_bytes + 15) & ~(size_t)15) : 0;
-  const size_t smem = sizeof(HotSmem) + (size_t)s.run_off + kRunArrayBytes;
   s.any_limits = 0;
   for (const ksched_template& tm : h->h_templates) if (tm.has_limits && tm.limit_present) s.any_limits = 1;
   s.use_class_run = getenv("KSCHED_NO_CLASSRUN") ? 0 : 1;
   s.use_level_run = std::getenv("KSCHED_NO_LEVELRUN") ? 0 : 1;
   s.use_mask_run = std::getenv("KSCHED_NO_MASKRUN") ? 0 : 1;
   s.use_level_warp = std::getenv("KSCHED_NO_LEVELWARP") ? 0 : 1;
-  s.use_varstore = std::getenv("KSCHED_NO_VARSTORE") ? 0 : 1;
   s.use_run_derive = std::getenv("KSCHED_NO_RUNDERIVE") ? 0 : 1;
+  s.vt_classes = with_table && !std::getenv("KSCHED_NO_VARSTORE") ? std::min(s.n_classes, kVtClasses) : 0;
+  s.vt_ndom = h->vt_ndom;
   s.use_round_stretch = std::getenv("KSCHED_NO_ROUNDSTRETCH") ? 0 : 1;
   s.use_fill_stretch = s.use_round_stretch && !std::getenv("KSCHED_NO_FILLSTRETCH") ? 1 : 0;
+  if (h->device < 0 || h->device >= 64) { h->err = "device ordinal out of range"; return KSCHED_ERR_INVALID; }
+  cudaEvent_t& done = g_k2_done[h->device];
+  if (!done) CUDA_TRY(h, cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
+  CUDA_TRY(h, cudaStreamWaitEvent(h->stream, done, 0));  // no-op for an event that was never recorded
+  CUDA_TRY(h, cudaMemcpyToSymbolAsync(g_k2, &k2, sizeof(K2Params), 0, cudaMemcpyHostToDevice, h->stream));
+  return KSCHED_OK;
+}
+
+// The pack kernel over the first n_pods pods of the queue (a simulation's batch, otherwise the whole problem).
+static int run_pack(ksched_handle* h, int n_pods, int stop_new_nodes, bool with_table = false) {
+  const PackState& s = h->k2_host.st;
   // block size: the chain is latency-bound on ONE thread's commit; more warps only help when there are many candidate
   // nodes to examine per pod (existing nodes, large in-flight sets)
-  int threads = s.n_existing >= 2048 ? kPackThreads : (s.n_existing >= 256 ? 256 : 128);
+  int threads = h->st.n_existing >= 2048 ? kPackThreads : (h->st.n_existing >= 256 ? 256 : 128);
   if (const char* e = getenv("KSCHED_PACK_THREADS")) { int v = atoi(e); if (v >= 32 && v <= kPackThreads && v % 32 == 0) threads = v; }
   {
     std::lock_guard<std::mutex> lock(g_k2_mu);
-    if (h->device < 0 || h->device >= 64) { h->err = "device ordinal out of range"; return KSCHED_ERR_INVALID; }
+    int rc = set_k2(h, n_pods, stop_new_nodes, with_table);
+    if (rc != KSCHED_OK) return rc;
     cudaEvent_t& done = g_k2_done[h->device];
-    if (!done) CUDA_TRY(h, cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
-    CUDA_TRY(h, cudaStreamWaitEvent(h->stream, done, 0));  // no-op for an event that was never recorded
-    CUDA_TRY(h, cudaMemcpyToSymbolAsync(g_k2, &k2, sizeof(K2Params), 0, cudaMemcpyHostToDevice, h->stream));
+    const size_t smem = sizeof(HotSmem) + (size_t)s.run_off + kRunArrayBytes;
     // the attribute belongs to the function, not to the handle: set it under the same lock as the launch
     const bool ext = h->cat.n_res_ext > 0, small = threads <= kPackThreadsSmall;
     void (*kern)() = small ? (ext ? pack_kernel<true, kPackThreadsSmall> : pack_kernel<false, kPackThreadsSmall>)
@@ -1449,7 +1483,7 @@ int ksched_run_resident(ksched_handle* h, int do_flush) {
   if ((rc = reset_state(h)) != KSCHED_OK) return rc;
   if (do_flush && (rc = flush_l2(h)) != KSCHED_OK) return rc;
   CUDA_TRY(h, cudaEventRecord(h->ev[0], h->stream));
-  if ((rc = run_sort(h, P)) != KSCHED_OK) return rc;
+  if ((rc = run_sort(h, P, true)) != KSCHED_OK) return rc;
   CUDA_TRY(h, cudaEventRecord(h->ev[1], h->stream));
   if ((rc = run_class_feasibility(h, P)) != KSCHED_OK) return rc;
   if ((rc = run_feasibility(h, P)) != KSCHED_OK) return rc;
@@ -1460,7 +1494,7 @@ int ksched_run_resident(ksched_handle* h, int do_flush) {
     if (r != ncclSuccess) { h->err = std::string("ncclAllReduce: ") + ncclGetErrorString(r); return KSCHED_ERR_NCCL; }
   }
   CUDA_TRY(h, cudaEventRecord(h->ev[3], h->stream));
-  if ((rc = run_pack(h, P, 0)) != KSCHED_OK) return rc;
+  if ((rc = run_pack(h, P, 0, true)) != KSCHED_OK) return rc;
   CUDA_TRY(h, cudaEventRecord(h->ev[4], h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   CUDA_TRY(h, cudaGetLastError());
@@ -1513,9 +1547,9 @@ static void print_pack_profile(const long long* counters) {
                   "write-back cycles=%lld | compactions=%lld slots=%lld cycles=%lld\n", c[kCtrRunActiveSum], c[kCtrRunEntryCycles],
           c[kCtrRunInputCycles], c[kCtrRunWbCycles], c[kCtrRunCompacts], c[kCtrRunCompactSlots], c[kCtrRunCompactCycles]);
   fprintf(stderr, "[pack profile] class_run round trips (status-1 stop -> entry of the next call that places pods): cycles=%lld | "
-                  "stops for want of a variant=%lld, their round trips' cycles=%lld | variant store: hits=%lld entries=%lld | "
+                  "stops for want of a variant=%lld, their round trips' cycles=%lld | variant table: fetches=%lld entries=%lld | "
                   "entry captures=%lld\n",
-          c[kCtrRoundTripCycles], c[kCtrNoVariantStops], c[kCtrNoVariantTripCycles], c[kCtrVarStoreHits], c[kCtrVarStoreEntries],
+          c[kCtrRoundTripCycles], c[kCtrNoVariantStops], c[kCtrNoVariantTripCycles], c[kCtrVtFetches], c[kCtrVtEntries],
           c[kCtrRunCaptures]);
   fprintf(stderr, "[pack profile] class_run derivations of a missing variant=%lld cycles=%lld refused=%lld\n", c[kCtrRunDerives],
           c[kCtrRunDeriveCycles], c[kCtrRunDeriveRefused]);
@@ -1572,6 +1606,9 @@ int ksched_download(ksched_handle* h, const ksched_problem* pb, ksched_result* r
   res->nodes_visited = counters[kCtrNodesVisited];
   res->add_calls = counters[kCtrAddCalls];
   h->tm.pack_steps = counters[kCtrSteps];
+  h->tm.vt_fetches = counters[kCtrVtFetches];
+  h->tm.run_derives = counters[kCtrRunDerives];
+  h->tm.vt_build_us = counters[kCtrVtEnd] ? (double)(counters[kCtrVtEnd] - (long long)~(unsigned long long)counters[kCtrVtStart]) / 1000.0 : 0.0;
   if (res->assign) CUDA_TRY(h, download(h, res->assign, s.assign, (size_t)P));
   if (res->relax_level) CUDA_TRY(h, download(h, res->relax_level, s.relax_level, (size_t)P));
   if (res->place_seq) CUDA_TRY(h, download(h, res->place_seq, s.place_seq, (size_t)P));

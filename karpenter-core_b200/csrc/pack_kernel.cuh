@@ -303,7 +303,7 @@ __device__ __forceinline__ PodRegs load_pod_regs(const ksched_pod_row* row, uint
 }
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 // Ext resources the class requests (DESIGN.md §3). Such classes take the generic step only: every closed-form mode below
-// reads the 8 row slots alone, and the variant store's key and row compare cannot see an ext amount.
+// reads the 8 row slots alone (the variant table builds no entry for them).
 __device__ __forceinline__ uint32_t class_ext(const PackState& s, unsigned cls) {
   return s.cls_ext_present ? s.cls_ext_present[cls] : 0u;
 }
@@ -735,6 +735,24 @@ __device__ __forceinline__ void front_store(long long* b1, long long* b2, uint8_
   dom[i] = (uint8_t)sh.front_bits;
 }
 
+// NewNode + Add of template tm for the pod in g_row / g_pt, requirement part (thread 0): Tolerates, then Compatible + merge
+// and the topology pin (t), on node slot `slot`. On success g_sh holds the node's requests (q, qp) and its requirement set's
+// meta word: the template's, overlaid by what this Add touched. Shared by the generic step and the variant table.
+__device__ __forceinline__ bool fresh_node_reqs(const ksched_template& tm, uint64_t p_tol, bool plain, uint32_t p_res, int slot, Touched& t) {
+  KS_K2
+  KS_ROW
+  StepShared& sh = g_sh;
+  const int R = c.n_res;
+  bool ok = (p_tol >> tm.taintset) & 1;
+  t.clear();
+  if (ok && !plain) ok = requirements_phase(tm.reqs.values, tm.reqs.meta & 0xFFFFFFFFull, 1, 0, slot, false, t);
+  if (!ok) return false;
+  sh.qp = tm.daemon_res_present | p_res;
+  for (int r = 0; r < KSCHED_MAX_RES; ++r) sh.q[r] = r < R ? tm.daemon_requests[r] + (((p_res >> r) & 1) ? row.requests[r] : 0) : 0;
+  sh.meta = t.overlay_meta(tm.reqs.meta & 0xFFFFFFFFull);
+  return true;
+}
+
 // One full Scheduler.add for one pod (existing nodes -> in-flight nodes -> new node -> relax/requeue). Every thread of
 // the CTA calls it together. Kept out of line: the steady-state path in pack_kernel must stay a few KB of code, because a
 // single resident CTA runs straight out of the instruction cache hierarchy (L0 ~6 KB, L1.5 32 KB).
@@ -1067,16 +1085,9 @@ __device__ __noinline__ void generic_step(const PodRegs& cur, bool first_pass, i
           if (st == 1) path = kPathCached;
           else if (st == 2) path = kPathCachedEmpty;
           else {
-            bool ok = (p_tol >> tm.taintset) & 1;
-            fresh_t.clear();
-            if (ok && !plain) ok = requirements_phase(tm.reqs.values, tm.reqs.meta & 0xFFFFFFFFull, 1, 0, NE + n, false, fresh_t);
-            if (ok) {
-              sh.qp = tm.daemon_res_present | p_res;
-              for (int r = 0; r < KSCHED_MAX_RES; ++r) sh.q[r] = r < R ? tm.daemon_requests[r] + (((p_res >> r) & 1) ? row.requests[r] : 0) : 0;
+            if (fresh_node_reqs(tm, p_tol, plain, p_res, NE + n, fresh_t)) {
               const bool same = f_valid && fresh_t.fin_is_merged();  // topology left every requirement exactly as K1 saw it
-              // the new node's requirement set: the template's, overlaid by what this Add touched
-              const uint64_t meta = fresh_t.overlay_meta(tm.reqs.meta & 0xFFFFFFFFull);
-              sh.meta = meta;
+              const uint64_t meta = sh.meta;
               sh.fd_slot = -1;
               if (same) path = kPathRow;
               else {
@@ -1288,7 +1299,6 @@ constexpr int kRunMask = 2;      // spread relations over a mask key
 constexpr int kRunDom = 16;      // domains of such a key
 constexpr int kTopoCap = 768;    // open nodes whose per-class topology inputs fit in shared memory
 constexpr int kRunVariants = 4;
-constexpr int kVarStore = 256;   // fresh-node variants one Solve shares between classes (VarStoreEntry)
 constexpr int kRunW32 = 64;      // option words a variant holds (T <= 2048)
 constexpr int kRunWarps = kPackThreads / 32;
 constexpr int kRunChunk = 128;   // queue entries staged in shared memory at a time
@@ -1330,100 +1340,9 @@ struct RunCtx {
   int lv_cnt[2];          // level step: members appended to the tie list (double-buffered)
   int lv_fill[2];         // fill step: pods the only eligible node takes
   RunVariant var[kRunVariants];
-  unsigned long long sig; // vs_signature of the class
-  int vs_ok;              // the class may share variants through the store
-  int vs_n;               // entries of PackState::vstore filled in this Solve
-  int vs_got;             // block-wide fetch: ring slot the store filled, or -1
-  uint32_t vs_tag[kVarStore];  // vs_tag of every store entry: a miss is found without a global load
+  int vt_got;             // block-wide fetch: ring slot the variant table filled, or -1
 };
 __shared__ RunCtx g_rc;
-
-// ---- variant store: fresh-node variants shared by the classes of one shape across the Solve ------------------------------
-// NewNode + Add on a fresh node reads nothing of the pod but the class row's requests, requirements, tolerations, host
-// ports and instance-type / hostname requirements, plus the domain every spread relation pins; with no provisioner limit
-// the outcome is a pure function of those (same argument as PackState::fd_*). FFD order puts many deployments of one
-// shape next to each other, so a variant captured for one class is replayed for the next classes of the same signature
-// instead of handing each one's first fresh node per domain back to generic_step. Entries are appended, never evicted;
-// a hit needs the signature hash, the relation pattern and a word-by-word compare of the two class rows to agree.
-struct VarStoreEntry {
-  unsigned long long sig;
-  uint32_t pat;           // vs_pattern
-  uint32_t cls;           // class the variant was captured for (its row is compared on a hit)
-  RunVariant v;           // v.rp: the room only (kRpDead depends on the class's hostname relations)
-};
-// words of ksched_pod_row NewNode + Add read: requests .. res_present (low half of word 28), itype_req, hostname_req
-__device__ __forceinline__ uint64_t vs_word(const ksched_pod_row* row, int w) {
-  const uint64_t x = w < 30 ? reinterpret_cast<const uint64_t*>(row)[w] : 0;
-  return w == 28 ? (x & 0xFFFFFFFFull) : x;
-}
-// hash of the signature fields the pod's registers hold (the requirement words are left to the full compare of a hit)
-__device__ __forceinline__ unsigned long long vs_signature(const PodRegs& p) {
-  unsigned long long x = 0;
-  auto mix = [&](uint64_t v) { x = (x ^ v) * 0x9E3779B97F4A7C15ull; x ^= x >> 29; };
-#pragma unroll
-  for (int r = 0; r < kHotRes; ++r) mix((uint64_t)p.req[r]);
-  mix(p.res); mix(p.tol); mix(p.meta); mix(p.hpc); mix(p.hpe); mix(p.itype | (uint64_t)p.hostname << 32);
-  return x;
-}
-__device__ __forceinline__ uint32_t vs_tag(unsigned long long sig, uint32_t pat) {
-  const unsigned long long x = (sig ^ pat) * 0x9E3779B97F4A7C15ull;
-  return (uint32_t)(x >> 32);
-}
-// warp-wide: some store entry carries the tag of (sig, pat)
-__device__ __forceinline__ bool vs_maybe(const RunCtx& rc, uint32_t tag, int lane) {
-  bool any = false;
-  for (int b = 0; b < rc.vs_n && !any; b += 32) any = __any_sync(0xffffffffu, b + lane < rc.vs_n && rc.vs_tag[b + lane] == tag);
-  return any;
-}
-// relation pattern of a variant: the mask keys of the spread relations and the domain each pinned
-__device__ __forceinline__ uint32_t vs_pattern(int n_mask, const uint8_t* keys, int d0, int d1) {
-  uint32_t p = (uint32_t)n_mask;
-  if (n_mask > 0) p |= (uint32_t)keys[0] << 2 | (uint32_t)d0 << 10;
-  if (n_mask > 1) p |= (uint32_t)keys[1] << 6 | (uint32_t)d1 << 14;
-  return p;
-}
-// warp-wide: the store entry of (class cls, pattern), or -1
-__device__ int vs_find(const RunCtx& rc, unsigned cls, uint32_t pat, int lane) {
-  KS_K2
-  const int n = rc.vs_n;
-  const unsigned long long sig = rc.sig;
-  const uint32_t tag = vs_tag(sig, pat);
-  for (int b = 0; b < n; b += 32) {
-    unsigned m = __ballot_sync(0xffffffffu, b + lane < n && rc.vs_tag[b + lane] == tag);
-    while (m) {
-      const int f = b + __ffs(m) - 1;
-      m &= m - 1;
-      if (s.vstore[f].sig != sig || s.vstore[f].pat != pat) continue;
-      const unsigned other = s.vstore[f].cls;
-      if (__all_sync(0xffffffffu, vs_word(s.classes + cls, lane) == vs_word(s.classes + other, lane))) return f;
-    }
-  }
-  return -1;
-}
-// warp-wide: replays the store's variant for (cls, pat) into ring slot rc.var_next, with the class's own kRpDead (a
-// fresh node holds one pod: its hostname counts are h_times); returns the slot, or -1 on a miss
-__device__ int vs_fetch(RunCtx& rc, unsigned cls, uint32_t pat, int lane) {
-  KS_K2
-  const int e = vs_find(rc, cls, pat, lane);
-  if (e < 0) return -1;
-  const int slot = rc.var_next;
-  const uint32_t* src = reinterpret_cast<const uint32_t*>(&s.vstore[e].v);
-  uint32_t* dst = reinterpret_cast<uint32_t*>(&rc.var[slot]);
-  for (int w = lane; w < (int)(sizeof(RunVariant) / 4); w += 32) dst[w] = src[w];
-  __syncwarp();
-  if (lane == 0) {
-    bool dead = false;
-    for (int j = 0; j < rc.n_host; ++j) dead = dead || rc.h_times[j] > rc.h_lim[j];
-    rc.var[slot].rp = s.vstore[e].v.rp | (dead ? kRpDead : 0u);
-    rc.var_next = (slot + 1) % kRunVariants;
-    if (rc.n_var < kRunVariants) rc.n_var++;
-#ifdef KSCHED_PROFILE_PACK
-    s.counters[kCtrVarStoreHits] += 1;
-#endif
-  }
-  __syncwarp();
-  return slot;
-}
 
 // ---- mask run: the class-run loop for ONE spread relation over a mask key (zone spread), driven by warp 0 alone ----------
 // The accepting nodes are kept in singly linked lists in the reference's order (pod count, then tie-break), one per
@@ -1457,6 +1376,34 @@ struct M1Ctx {
   uint32_t fr[kRunChunk];             // state (option words, requirement values, requests, ...) is stored by the CTA afterwards
 };
 __shared__ M1Ctx g_m1;
+
+// ---- variant table: every fresh-node variant a class run can replay, built before the pack kernel (vt_build_block) ------
+// With no provisioner limit NewNode + Add of a run class's fresh node depends on the class row, the template and the domain
+// its mask relation pins (the fresh hostname's counts are the relations' times), so entry (cls, d) is the variant that
+// run_derive + run_capture would store for the class and domain d (d = 0 without a mask relation), or none (vt_ok 0).
+constexpr int kVtClasses = 1024;  // classes the table covers (ids below; the others derive their variants)
+__device__ __forceinline__ size_t vt_index(unsigned cls, int d) { return (size_t)cls * kM1Dom + d; }
+// the table holds the variant of (cls, d) (uniform: every thread reads the same flag)
+__device__ __forceinline__ bool vt_has(const PackState& s, unsigned cls, int n_mask, int d) {
+  return n_mask < 2 && cls < (unsigned)s.vt_classes && d < s.vt_ndom && s.vt_ok[vt_index(cls, d)] != 0;
+}
+// warp-wide: copies the table's variant of (cls, d) into ring slot rc.var_next; returns the slot, or -1 when vt_has is false
+__device__ int vt_fetch(RunCtx& rc, unsigned cls, int n_mask, int d, int lane) {
+  KS_K2
+  if (!vt_has(s, cls, n_mask, d)) return -1;
+  const int slot = rc.var_next;
+  const uint32_t* src = reinterpret_cast<const uint32_t*>(&s.vtable[vt_index(cls, d)]);
+  uint32_t* dst = reinterpret_cast<uint32_t*>(&rc.var[slot]);
+  for (int w = lane; w < (int)(sizeof(RunVariant) / 4); w += 32) dst[w] = src[w];
+  __syncwarp();
+  if (lane == 0) {
+    rc.var_next = (slot + 1) % kRunVariants;
+    if (rc.n_var < kRunVariants) rc.n_var++;
+    s.counters[kCtrVtFetches] += 1;
+  }
+  __syncwarp();
+  return slot;
+}
 
 struct RunIO {
   int qi, head, qlen, tick, seq, n_active, n_new, parity;
@@ -1495,8 +1442,9 @@ __device__ __forceinline__ int warp_pick(bool in, int cnt) {
 }
 // How many more pods with request vector `req` (keys `res`) the node at slot a can take: exact by the Pareto front of its
 // options (quick_fit for the k-th pod <=> k <= room); kRoomSlow when the front is not exact.
-__device__ __noinline__ unsigned run_room(const HotSmem* hs, int a, const long long* req, uint32_t res, int RH) {
-  const unsigned short fl = hs->flags[a];
+// Room of a node with flags fl, hot requests q and front (b1, b2).
+__device__ __forceinline__ unsigned room_of(unsigned short fl, const long long* q, const long long* b1, const long long* b2, const long long* req,
+                                            uint32_t res, int RH) {
   const uint32_t qp = ((fl >> 1) & 0xF) | res;
   long long best = 0;
   bool inexact_ok = true;
@@ -1505,7 +1453,7 @@ __device__ __noinline__ unsigned run_room(const HotSmem* hs, int a, const long l
     long long rf = kRoomMax;
     for (int r = 0; r < RH; ++r) {
       if (!((qp >> r) & 1)) continue;
-      const long long slack = (f ? hs->bound2[r][a] : hs->bound[r][a]) - hs->q[r][a];
+      const long long slack = (f ? b2[r] : b1[r]) - q[r];
       if (req[r] > 0) {
         const long long k = slack < req[r] ? 0 : slack / req[r];
         rf = k < rf ? k : rf;
@@ -1516,6 +1464,18 @@ __device__ __noinline__ unsigned run_room(const HotSmem* hs, int a, const long l
   }
   if (!(fl & kFlExact)) return inexact_ok ? kRoomSlow : 0;  // per-resource maxima only: a necessary test
   return (unsigned)best;
+}
+__device__ __noinline__ unsigned run_room(const HotSmem* hs, int a, const long long* req, uint32_t res, int RH) {
+  long long q[kHotRes], b1[kHotRes], b2[kHotRes];
+#pragma unroll
+  for (int r = 0; r < kHotRes; ++r) { q[r] = hs->q[r][a]; b1[r] = hs->bound[r][a]; b2[r] = hs->bound2[r][a]; }
+  return room_of(hs->flags[a], q, b1, b2, req, res, RH);
+}
+// A fresh node's room word for the class: its room, dead when one of its hostname relations refuses the node's count
+// after its first pod (the relation's times)
+__device__ __forceinline__ uint32_t fresh_room_word(unsigned room, int n_host, const uint8_t* times, const int* lim) {
+  for (int j = 0; j < n_host; ++j) if ((int)times[j] > lim[j]) room |= kRpDead;
+  return room;
 }
 // A commit's Topology.Record for the class's hostname groups: t more pods on the node at slot a (counters saturate at
 // 0xFFFF). Returns the room word rp with t pods moved from room to placed, dead once a group no longer admits the node.
@@ -2227,8 +2187,7 @@ __device__ __forceinline__ int m1_single_fresh(const RunEnv& e, int buf, M1Lane&
   if (!ok || !cand) { why = kStopOther; return 1; }
   const int fd = warp_pick((cand >> L) & 1, w.cnt_d);  // (cand is a subset of okm: lanes below kM1Dom)
   int vi = run_ring_find(rc, 1, fd, 0);
-  if (vi < 0 && rc.vs_ok && !((w.fr_used >> rc.var_next) & 1))
-    vi = vs_fetch(rc, e.cls, vs_pattern(1, rc.m_key, fd, 0), L);
+  if (vi < 0 && !((w.fr_used >> rc.var_next) & 1)) vi = vt_fetch(rc, e.cls, 1, fd, L);
   if (vi < 0) { why = kStopNoVariant; return 1; }
   const RunVariant& v = rc.var[vi];
   w.fr_used |= 1u << vi;
@@ -2597,15 +2556,14 @@ __device__ __forceinline__ bool run_fresh_step(const RunEnv& e, int buf, int i, 
     if (!cand) ok = false; else fd1 = run_pick(cand, rc.cnt[warp][1]);
   }
   int vi = ok ? run_ring_find(rc, n_mask, fd0, fd1) : -1;
-  const uint32_t pat = vs_pattern(n_mask, rc.m_key, fd0, fd1);
-  if (vi < 0 && ok && rc.vs_ok && vs_maybe(rc, vs_tag(rc.sig, pat), lane)) {  // (every warp finds the same answer)
+  if (vi < 0 && ok && vt_has(s, e.cls, n_mask, fd0)) {  // (every warp finds the same answer)
     __syncthreads();  // every warp has scanned the ring
     if (warp == 0) {
-      const int got = vs_fetch(rc, e.cls, pat, lane);
-      if (lane == 0) rc.vs_got = got;
+      const int got = vt_fetch(rc, e.cls, n_mask, fd0, lane);
+      if (lane == 0) rc.vt_got = got;
     }
     __syncthreads();
-    vi = rc.vs_got;
+    vi = rc.vt_got;
   }
   if (vi < 0) { why = ok ? kStopNoVariant : kStopOther; return false; }
   const RunVariant& v = rc.var[vi];
@@ -2663,13 +2621,13 @@ __device__ __forceinline__ bool run_fresh_step(const RunEnv& e, int buf, int i, 
 }
 
 // ---- capture node slot a (node hs->node[a]), which the generic step opened for the run's class with one pod, as a
-// fresh-node variant: into the ring and, when the class shares, into the store. zv / rpv hold the slot's per-run inputs.
+// fresh-node variant into the ring. zv / rpv hold the slot's per-run inputs.
 // Returns the ring slot, or -1 when the node does not pin one exact domain per mask relation or the ring already holds a
 // variant of its template and domains. Block-wide.
-__device__ __forceinline__ int run_capture(const HotSmem* hs, const uint32_t* zv, const uint32_t* rpv, int a, int n_mask, unsigned cls) {
+__device__ __forceinline__ int run_capture(const HotSmem* hs, const uint32_t* zv, const uint32_t* rpv, int a, int n_mask) {
   KS_K2
   RunCtx& rc = g_rc;
-  const int tid = threadIdx.x, T = blockDim.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x, T = blockDim.x;
   const int MAXN = s.max_new, W32 = c.W32, n = hs->node[a];
   int dom[kRunMask] = {0, 0};
   bool ok = true;
@@ -2703,29 +2661,7 @@ __device__ __forceinline__ int run_capture(const HotSmem* hs, const uint32_t* zv
     rc.var_next = (slot + 1) % kRunVariants;
     if (rc.n_var < kRunVariants) rc.n_var++;
   }
-  __syncthreads();
-  // into the store (not looked up first: a class captures a variant only after a miss, so duplicates are rare and
-  // harmless, and the capture stays free of dependent loads)
-  if (warp == 0 && rc.vs_ok && rc.vs_n < kVarStore) {
-    const uint32_t pat = vs_pattern(n_mask, rc.m_key, dom[0], dom[1]);
-    const int e = rc.vs_n;
-    VarStoreEntry& d = s.vstore[e];
-    const uint32_t* src = reinterpret_cast<const uint32_t*>(&rc.var[slot]);
-    uint32_t* dst = reinterpret_cast<uint32_t*>(&d.v);
-    for (int w = lane; w < (int)(sizeof(RunVariant) / 4); w += 32) dst[w] = src[w];
-    __syncwarp();
-    if (lane == 0) {
-      d.sig = rc.sig; d.pat = pat; d.cls = cls;
-      d.v.rp = rc.var[slot].rp & 0xFFFF;
-      rc.vs_tag[e] = vs_tag(rc.sig, pat);
-      rc.vs_n = e + 1;
-#ifdef KSCHED_PROFILE_PACK
-      s.counters[kCtrVarStoreEntries] += 1;
-#endif
-    }
-    __syncwarp();
-  }
-  __syncthreads();  // the ring slot and the store entry are complete
+  __syncthreads();  // the ring slot is complete
   return slot;
 }
 
@@ -2757,9 +2693,7 @@ __device__ __noinline__ int run_derive(const PodRegs& first_in, int fpos, int n_
   if (tid == 0) {  // the slot's per-run inputs as class_run's entry computes them (its hostname counts: the relations' times)
     long long p_req[kHotRes];
     for (int r = 0; r < kHotRes; ++r) p_req[r] = first_in.req[r];
-    unsigned rm = run_room(hs, a, p_req, first_in.res, c.n_res < kHotRes ? c.n_res : kHotRes);
-    for (int j = 0; j < n_host; ++j) if ((int)rc.h_times[j] > rc.h_lim[j]) rm |= kRpDead;
-    rpv[a] = rm;
+    rpv[a] = fresh_room_word(run_room(hs, a, p_req, first_in.res, c.n_res < kHotRes ? c.n_res : kHotRes), n_host, rc.h_times, rc.h_lim);
     const uint64_t meta = s.nn_meta[n];
     for (int j = 0; j < n_mask; ++j) {
       const int k = rc.m_key[j];
@@ -2769,20 +2703,160 @@ __device__ __noinline__ int run_derive(const PodRegs& first_in, int fpos, int n_
     }
   }
   __syncthreads();
-  return run_capture(hs, zv, rpv, a, n_mask, rc.cls);
+  return run_capture(hs, zv, rpv, a, n_mask);
 }
 
-// run_derive for class_run's loop: true when the variant is in the ring (profile: derivations, their cycles, refusals)
+// run_derive for class_run's loop: true when the variant is in the ring (counts derivations; profile: their cycles, refusals)
 __device__ __forceinline__ bool run_derive_at(const PodRegs& first_in, int fpos, int n_new, int n_active, int tick, int seq, int parity) {
 #ifdef KSCHED_PROFILE_PACK
   const long long t0 = clock64();
 #endif
   const int vi = run_derive(first_in, fpos, n_new, n_active, tick, seq, parity);
-#ifdef KSCHED_PROFILE_PACK
   KS_K2
-  if (threadIdx.x == 0) { s.counters[kCtrRunDerives] += 1; s.counters[kCtrRunDeriveCycles] += clock64() - t0; s.counters[kCtrRunDeriveRefused] += vi < 0; }
+  if (threadIdx.x == 0) s.counters[kCtrRunDerives] += 1;
+#ifdef KSCHED_PROFILE_PACK
+  if (threadIdx.x == 0) { s.counters[kCtrRunDeriveCycles] += clock64() - t0; s.counters[kCtrRunDeriveRefused] += vi < 0; }
 #endif
   return vi >= 0;
+}
+
+// ---- variant table, entry (cls, d): the generic step's NewNode + Add for the class's fresh node with its mask relation
+// pinned to domain d (templates in weight order, the first that opens a node), captured as run_capture captures it.
+// Block-wide, in a launch before the pack kernel; reads only what is fixed for the Solve. The guards are the derivation's
+// (no provisioner limit, W32 <= kRunW32) and the classes a shared variant used to need (no instance-type or hostname
+// requirement, no volumes, no ext resource), with at most one mask relation and the relation checks of class_run's table
+// that depend on the class alone. The entry is none when no template opens a node, the node closes at once or it is not
+// pinned to exactly d (the pod's own requirement excludes d).
+__device__ void vt_build_entry(unsigned cls, int d) {
+  KS_K2
+  KS_PT
+  StepShared& sh = g_sh;
+  Touched& fresh_t = g_fresh_t;
+  TypeCtx& fresh_x = g_fresh_x;
+  const int tid = threadIdx.x, W32 = c.W32, V = c.n_templates, NE = s.n_existing;
+  const int RH = c.n_res < kHotRes ? c.n_res : kHotRes;
+  const ksched_pod_row* src = s.classes + cls;
+  __shared__ int vt_go, vt_key, vt_nhost;
+  __shared__ uint8_t vt_times[kRunHost];
+  __shared__ int vt_lim[kRunHost];
+  if (tid < 32) reinterpret_cast<uint64_t*>(&g_row)[tid] = reinterpret_cast<const uint64_t*>(src)[tid];
+  if (tid == 0) {
+    const ksched_pod_row& r = *src;
+    bool ok = !s.any_limits && W32 <= kRunW32 && r.itype_req == KSCHED_NONE && r.hostname_req == KSCHED_NONE &&
+              !class_has_volumes(s, cls) && !class_ext(s, cls) && !(r.topo_begin != r.topo_end && V != 1);
+    int n_mask = 0, n_host = 0, key = -1;
+    for (uint32_t e = r.topo_begin; e < r.topo_end && ok; ++e) {
+      const RelX x = s.relx[e];
+      if (!(x.flags & KSCHED_TOPO_CONSTRAINS) || ((x.flags & KSCHED_TOPO_RECORDS) && x.has_filter)) { ok = false; break; }
+      const int times = ((x.flags & KSCHED_TOPO_RECORDS) ? 1 : 0) + ((x.flags & KSCHED_TOPO_RECORDS_INVERSE) ? 1 : 0);
+      const int self = (x.flags & KSCHED_TOPO_SELECTS) ? 1 : 0;
+      if (x.key == KSCHED_KEY_HOSTNAME) {
+        if (x.type == 1 || n_host == kRunHost) { ok = false; break; }
+        const long long lim = x.type == 0 ? (long long)x.max_skew - self : 0;
+        if (lim < 0) { ok = false; break; }  // the run places no pod on a fresh node then
+        vt_times[n_host] = (uint8_t)times;
+        vt_lim[n_host++] = lim > 0x10000 ? 0x10000 : (int)lim;
+      } else {
+        const int k = x.key;
+        if (x.type != 0 || n_mask == 1 || (x.flags & KSCHED_TOPO_RECORDS_INVERSE) || (c.keys[k].dict_mask >> kRunDom) ||
+            !((s.grp_registered[x.group] >> d) & 1)) { ok = false; break; }
+        // the pin: d is the one admissible domain in (count, id) order, so the node gets d exactly when it admits d
+        fill_pod_topo_static(x, pt, 0);
+        pt.registered[0] = s.grp_registered[x.group];
+        pt.n_sorted[0] = 1;
+        pt.sorted[0][0] = (uint8_t)d;
+        pt.min_slot[0] = 0;
+        n_mask = 1;
+        key = k;
+      }
+    }
+    // (a fresh node's hostname count is 0 on every hostname relation, which admits it by lim >= 0: only the mask relation pins)
+    pt.n = n_mask;
+    pt.overflow = 0;
+    vt_go = ok && (n_mask == 1 || d == 0);
+    vt_key = key;
+    vt_nhost = n_host;
+  }
+  __syncthreads();
+  const size_t idx = vt_index(cls, d);
+  if (!vt_go) {
+    if (tid == 0) s.vt_ok[idx] = 0;
+    return;
+  }
+  RunVariant& out = s.vtable[idx];
+  const ksched_pod_row& row = g_row;
+  const uint64_t p_tol = row.tolerated_taintsets;
+  const uint32_t p_res = row.res_present;
+  const bool plain = ((row.meta >> KSCHED_META_PRESENT_SHIFT) & 0xFFFF) == 0 && row.topo_begin == row.topo_end;
+  int parity = 0;
+  bool built = false;
+  for (int v = 0; v < V && !built; ++v) {
+    const ksched_template& tm = c.templates[v];
+    __syncthreads();  // every reader of the previous template's g_sh / fresh_t / fresh_x is done
+    if (tid == 0) {
+      const bool ok = fresh_node_reqs(tm, p_tol, plain, p_res, NE, fresh_t);
+      if (ok) build_type_ctx(fresh_t, sh.q, sh.qp, tm.reqs.values, tm.reqs.meta & 0xFFFFFFFFull, 1, 0, true, c.alloc_sorted, fresh_x);
+      sh.path = ok ? 1 : 0;
+    }
+    __syncthreads();
+    if (!sh.path) continue;
+    bool any = false;
+    for (int w = tid; w < W32; w += blockDim.x) {
+      const uint32_t base = c.member[(size_t)v * W32 + w];
+      const uint32_t sw = base ? type_word(c, s, fresh_x, base, w) : 0u;
+      out.opts[w] = sw;
+      any = any || sw;
+    }
+    if (tid < KSCHED_MAX_KEYS) out.vals[tid] = tid < c.n_keys ? (((fresh_t.keys >> tid) & 1) ? fresh_t.fin[tid] : tm.reqs.values[tid]) : 0;
+    if (!__syncthreads_or(any)) continue;  // Node.Add fails on this template: the next one
+    built = true;
+    compute_front_block(out.opts, 1, 0, sh.bound, sh.bound2, &sh.front_bits, g_red, parity);
+    __syncthreads();
+    if (tid == 0) {
+      bool ok = !node_closed(sh.q, s.min_req, RH, sh.bound, sh.bound2, sh.front_bits);
+      const uint64_t meta = sh.meta;
+      if (ok && vt_key >= 0) {  // pinned to exactly d (an In requirement of the one value)
+        const int k = vt_key;
+        const Req r = load_soa(out.vals, meta, 1, 0, k);
+        const uint64_t allowed = r.present ? ksched::req_allowed(r, c.keys[k].dict_mask, key_meta(c, k)) : c.keys[k].dict_mask;
+        ok = r.present && !r.complement && allowed == (1ull << d);
+      }
+      if (ok) {
+        const unsigned short fl = (unsigned short)(sh.front_bits | ((sh.qp & 0xF) << 1) | (v << 8));
+        long long p_req[kHotRes];
+        for (int r = 0; r < kHotRes; ++r) p_req[r] = row.requests[r];
+        out.meta = meta;
+        for (int r = 0; r < KSCHED_MAX_RES; ++r) out.q[r] = sh.q[r];
+        for (int r = 0; r < kHotRes; ++r) { out.b1[r] = sh.bound[r]; out.b2[r] = sh.bound2[r]; }
+        out.qp = sh.qp;
+        out.fl = fl;
+        out.rp = fresh_room_word(room_of(fl, sh.q, sh.bound, sh.bound2, p_req, p_res, RH), vt_nhost, vt_times, vt_lim);
+        out.dom[0] = (uint8_t)(vt_key >= 0 ? d : 0);
+        out.dom[1] = 0;
+      }
+      s.vt_ok[idx] = ok ? 1 : 0;
+#ifdef KSCHED_PROFILE_PACK
+      if (ok) atomicAdd(reinterpret_cast<unsigned long long*>(&s.counters[kCtrVtEntries]), 1ull);
+#endif
+    }
+  }
+  if (!built && tid == 0) s.vt_ok[idx] = 0;
+}
+// block b of the table build: entry (b / vt_ndom, b % vt_ndom); the build's first start and last end (globaltimer, ns) go
+// to the Solve's counters
+__device__ void vt_build_block(int b) {
+  KS_K2
+  unsigned long long t;
+  if (threadIdx.x == 0) {
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    atomicMax(reinterpret_cast<unsigned long long*>(&s.counters[kCtrVtStart]), ~t);
+  }
+  vt_build_entry((unsigned)(b / s.vt_ndom), b % s.vt_ndom);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    atomicMax(reinterpret_cast<unsigned long long*>(&s.counters[kCtrVtEnd]), t);
+  }
 }
 
 __device__ __noinline__ void class_run(const PodRegs& first_in) {
@@ -2861,12 +2935,6 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
       }
       rc.eligible = ok;
     }
-    if (tid == 0) {
-      // instance-type / hostname requirements and volumes: not shared (a volume limit reads more than the row)
-      rc.vs_ok = s.use_varstore && !s.any_limits && W32 <= kRunW32 && first_in.itype == KSCHED_NONE &&
-                 first_in.hostname == KSCHED_NONE && !class_has_volumes(s, cls);
-      rc.sig = vs_signature(first_in);
-    }
     __syncthreads();
   }
   if (!rc.eligible || (topo && n_active > kTopoCap)) {
@@ -2942,7 +3010,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
 #endif
   // ---- capture the node generic_step has just created for this class as a fresh-node variant
   if (fresh_valid && !s.any_limits && W32 <= kRunW32 && fresh_a == n_active - 1 && fresh_a >= 0) {
-    const int slot = run_capture(hs, zv, rpv, fresh_a, n_mask, cls);
+    const int slot = run_capture(hs, zv, rpv, fresh_a, n_mask);
 #ifdef KSCHED_PROFILE_PACK
     if (tid == 0 && slot >= 0) s.counters[kCtrRunCaptures] += 1;
 #endif
@@ -3191,7 +3259,7 @@ __global__ void __launch_bounds__(kMaxThreads, 1) pack_kernel() {
   PodTopo& pt = g_pt;
   uint32_t* tmpl_taintset = g_tmpl_taintset;
   for (int v = tid; v < c.n_templates; v += blockDim.x) tmpl_taintset[v] = c.templates[v].taintset;
-  if (tid == 0) { pt.n = 0; g_rc.cls = KSCHED_NONE; g_rc.eligible = 0; g_rc.vs_n = 0; }
+  if (tid == 0) { pt.n = 0; g_rc.cls = KSCHED_NONE; g_rc.eligible = 0; }
 
   int head = 0, qlen = s.n_pods;
   const int qcap = s.n_pods + 1;
@@ -3265,7 +3333,7 @@ __global__ void __launch_bounds__(kMaxThreads, 1) pack_kernel() {
     bool skip_run = true;
     if (fast_allowed && s.use_class_run && qi < s.n_pods && n_active <= kActCap) {
       const bool topo_cls = nxt.topo_begin != nxt.topo_end;
-      // (host-port classes never get here, so the variant store's signature, which reads the row words only, never meets one)
+      // (host-port classes never get here)
       // (with the instance-type slot state, PackState::nn_it, only the generic step writes it: instance-type classes stay there)
       const bool shape_ok = !has_host_ports(s, nxt) && (nxt.res >> kHotRes) == 0 && !(kExt && class_ext(s, (unsigned)nxt.cls64)) &&
                             (nxt.itype == KSCHED_NONE || !s.nn_it) &&

@@ -114,12 +114,14 @@ struct PackState {
   int use_level_run;                 // class_run: level / fill steps for classes without mask-key spread (KSCHED_NO_LEVELRUN=1: off)
   int use_level_warp;                // class_run: the level / fill steps on one warp while at most 32 nodes are open (KSCHED_NO_LEVELWARP=1: off)
   int use_mask_run;                  // class_run: list-driven loop on warp 0 for one mask-key spread relation (KSCHED_NO_MASKRUN=1: off)
-  int use_varstore;                  // class_run: fresh-node variants shared by classes of one shape (KSCHED_NO_VARSTORE=1: off)
   int use_run_derive;                // class_run: a fresh node's missing variant derived inside the run (KSCHED_NO_RUNDERIVE=1: off)
   int use_round_stretch;             // mask run: several rounds of a zone spread in one step (KSCHED_NO_ROUNDSTRETCH=1: off)
   int use_fill_stretch;              // mask run: rounds that keep the same head per zone in one step (KSCHED_NO_FILLSTRETCH=1 or
                                      // KSCHED_NO_ROUNDSTRETCH=1: off)
-  struct VarStoreEntry* vstore;      // [kVarStore] (pack_kernel.cuh); valid entries: RunCtx::vs_n, reset per Solve
+  struct RunVariant* vtable;         // [classes][kM1Dom] fresh-node variants of the class runs (pack_kernel.cuh: vt_build_entry)
+  uint32_t* vt_ok;                   // [vt_classes][kM1Dom] 1: the entry holds a variant
+  int vt_classes;                    // classes the table covers in this launch (0: no table; KSCHED_NO_VARSTORE=1 turns it off)
+  int vt_ndom;                       // domain ids the table covers (below kM1Dom; the build has vt_classes * vt_ndom blocks)
   // topology counters
   int32_t* grp_cnt;                  // [n_groups][64]
   uint64_t* grp_registered;          // [n_groups]

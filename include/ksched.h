@@ -32,6 +32,7 @@ extern "C" {
 #endif
 
 #define KSCHED_ABI_VERSION 4
+#define KSCHED_PARAM_SLOTS 2 /* constant-parameter slots per device: handles on different slots do not wait for each other */
 #define KSCHED_MAX_RES_EXT 24 /* resources beyond the KSCHED_MAX_RES row slots (ksched_catalog.n_res_ext) */
 #define KSCHED_MAX_KEYS 16
 #define KSCHED_MAX_RES 8
@@ -479,6 +480,9 @@ typedef struct ksched_timings {
      row gather's launch), the class runs' variants fetched from it and those derived inside the pack kernel */
   double vt_build_us;
   int64_t vt_fetches, run_derives;
+  /* the last downloaded Solve's pack kernel launch, or the last simulation's of the last ksched_simulate_batch /
+     ksched_simulate_full call: its start and end on the device's %globaltimer, in ns (comparable between handles on one device) */
+  int64_t pack_interval_ns[2];
 } ksched_timings;
 
 typedef struct ksched_handle ksched_handle;
@@ -486,7 +490,11 @@ typedef struct ksched_handle ksched_handle;
 int ksched_abi_version(void);
 /* number of CUDA devices visible, or a negative error */
 int ksched_device_count(void);
-/* Bind a handle to one CUDA device. One handle = one stream, single-threaded; handles are independent. */
+/* Bind a handle to one CUDA device. One handle = one stream, used by one thread at a time; different handles may be used
+   from different threads at once. The kernels' constant parameters live in KSCHED_PARAM_SLOTS slots per device, and a
+   handle takes the slot of its device with the fewest live handles (the lowest on ties) until ksched_destroy: handles on
+   different slots run their kernels concurrently, handles that share a slot launch their parameter-reading kernels in
+   the order they were issued. */
 int ksched_create(int device_ordinal, ksched_handle** out);
 void ksched_destroy(ksched_handle* h);
 const char* ksched_last_error(const ksched_handle* h);

@@ -67,6 +67,22 @@ int kh_result_uninitialized_existing(const kh_result* r);
 
 /* ---- the device */
 int kh_set_device(int ordinal);   /* CUDA device of this process's scheduler handle (default 0) */
+/* ---- scheduler contexts. Every kh_* function without a context argument uses one process-wide context (one device
+ * handle) and takes a process-wide lock, so concurrent callers are serialized. A context made here owns a handle of its
+ * own: two contexts may be used from two threads at once, without a lock between them, and their kernels run
+ * concurrently on one device when their handles hold different parameter slots (ksched_create). One context is used by
+ * one thread at a time. A session opened on a context lives on the context's handle (its validation snapshot on a
+ * handle of its own, as always), and displaces only that context's snapshot. NULL from kh_context_create without a
+ * CUDA device (KSCHED_ERR_NO_DEVICE, kh_scheduler_error()): there is no CPU path. Destroy a context after its sessions. */
+typedef struct kh_context kh_context;
+kh_context* kh_context_create(int device);
+void kh_context_destroy(kh_context* ctx);
+/* kh_scheduler_solve on the context's handle */
+int kh_context_solve(kh_context* ctx, const kh_problem* p, const int* candidates, int n_candidates, kh_result* out);
+/* kh_cluster_open on the context's handle; every kh_cluster_* call on the session then runs there */
+kh_cluster* kh_context_cluster_open(kh_context* ctx, const kh_problem* p, int* resident, int* n_candidates);
+/* ksched_get_timings of the context's handle: pack_interval_ns is its last pack launch, a Solve's or a session's */
+int kh_context_timings(kh_context* ctx, ksched_timings* out);
 const char* kh_scheduler_error(void);
 int kh_nccl_init(const void* id128, int rank, int world); /* communicator for kh_allgather_i32 (id: ksched_nccl_unique_id) */
 int kh_allgather_i32(const int* send, int n, int* recv);  /* one ncclAllGather, recv holds world * n */

@@ -10,6 +10,7 @@ Names mirror the reference: `Scheduler.solve` <-> scheduling.Scheduler.Solve (sc
 """
 import ctypes as C
 import json
+import weakref
 from pathlib import Path
 
 import numpy as np
@@ -46,10 +47,13 @@ class Timings(C.Structure):
                 ("feasibility_bytes", C.c_int64), ("pack_steps", C.c_int64),
                 ("feasibility_launches", C.c_int32), ("pack_launches", C.c_int32), ("sort_launches", C.c_int32), ("pad", C.c_int32),
                 ("h2d_bytes", C.c_int64), ("d2h_bytes", C.c_int64), ("class_feasibility_us", C.c_double),
-                ("vt_build_us", C.c_double), ("vt_fetches", C.c_int64), ("run_derives", C.c_int64)]
+                ("vt_build_us", C.c_double), ("vt_fetches", C.c_int64), ("run_derives", C.c_int64),
+                ("pack_interval_ns", C.c_int64 * 2)]
 
     def as_dict(self):
-        return {k: getattr(self, k) for k, _ in self._fields_ if k != "pad"}
+        d = {k: getattr(self, k) for k, _ in self._fields_ if k != "pad"}
+        d["pack_interval_ns"] = tuple(self.pack_interval_ns)
+        return d
 
 
 _model = None
@@ -157,6 +161,13 @@ def lib():
     L.kh_consolidate_candidates.argtypes = [C.c_void_p]
     L.kh_cluster_open.restype = C.c_void_p
     L.kh_cluster_open.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    L.kh_context_create.restype = C.c_void_p
+    L.kh_context_create.argtypes = [C.c_int]
+    L.kh_context_destroy.argtypes = [C.c_void_p]
+    L.kh_context_solve.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.c_int, C.c_void_p]
+    L.kh_context_timings.argtypes = [C.c_void_p, C.POINTER(Timings)]
+    L.kh_context_cluster_open.restype = C.c_void_p
+    L.kh_context_cluster_open.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     L.kh_cluster_close.argtypes = [C.c_void_p]
     L.kh_cluster_probe_sets.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int,
                                         C.POINTER(C.c_int)]
@@ -333,11 +344,52 @@ def _cand_array(candidates):
     return arr, len(candidates)
 
 
-class Scheduler:
-    """scheduling.Scheduler: NewScheduler(...) then Solve(pods). GPU only."""
+class Context:
+    """A scheduler context: a device handle of its own (kh_context_create). Schedulers and sessions made with context=ctx
+    run on it; two contexts can be used from two threads at once, and their kernels overlap on one device. One context is
+    used by one thread at a time. Without a context, everything shares the process-wide handle, one call at a time."""
 
-    def __init__(self, problem: Problem):
+    def __init__(self, device=0):
+        self.ptr = lib().kh_context_create(int(device))
+        if not self.ptr:
+            msg = lib().kh_scheduler_error().decode()
+            raise KschedError(KSCHED_ERR_NO_DEVICE if "no usable CUDA device" in msg else KSCHED_ERR_INVALID, msg)
+        self.device = int(device)
+        self._sessions = weakref.WeakSet()  # open ClusterSessions on this context: destroy() refuses while there are any
+
+    def handle(self):
+        """the context's pointer for the C calls; refuses a destroyed context"""
+        if not self.ptr:
+            raise KschedError(KSCHED_ERR_INVALID, "the context has been destroyed")
+        return self.ptr
+
+    def timings(self):
+        """ksched_get_timings of the context's handle, as a dict (pack_interval_ns: its last pack launch in device ns)"""
+        t = Timings()
+        _check(lib().kh_context_timings(self.handle(), C.byref(t)))
+        return t.as_dict()
+
+    def destroy(self):
+        """frees the context's handle; refused while a session opened on it is still open (close it first)"""
+        if getattr(self, "ptr", None) and any(s.ptr for s in self._sessions):
+            raise KschedError(KSCHED_ERR_INVALID, "the context still has open sessions")
+        if getattr(self, "ptr", None) and _lib is not None:
+            _lib.kh_context_destroy(self.ptr)
+        self.ptr = None
+
+    def __del__(self):  # an open session keeps its context alive, so none is open here
+        if getattr(self, "ptr", None) and _lib is not None:
+            _lib.kh_context_destroy(self.ptr)
+        self.ptr = None
+
+
+class Scheduler:
+    """scheduling.Scheduler: NewScheduler(...) then Solve(pods). GPU only. context: a Context to solve on (default: the
+    process-wide handle)."""
+
+    def __init__(self, problem: Problem, context: "Context | None" = None):
         self.problem = problem
+        self.context = context
 
     def solve(self, candidates=(), count_visited=True):
         """count_visited=False is the production setting: the exact nodes_visited statistic is dropped and the pack
@@ -345,7 +397,10 @@ class Scheduler:
         lib().kh_set_count_visited(int(count_visited))
         res = Result()
         arr, n = _cand_array(list(candidates))
-        rc = lib().kh_scheduler_solve(self.problem.ptr, arr, n, res.ptr)
+        if self.context is None:
+            rc = lib().kh_scheduler_solve(self.problem.ptr, arr, n, res.ptr)
+        else:
+            rc = lib().kh_context_solve(self.context.handle(), self.problem.ptr, arr, n, res.ptr)
         _check(rc)
         return res
 
@@ -370,10 +425,16 @@ class ClusterSession:
     (ksched_load_cluster), every computeConsolidation one entry of a ksched_simulate_batch call."""
     OPTIONS_STRIDE = 2048
 
-    def __init__(self, problem: Problem):
+    def __init__(self, problem: Problem, context: "Context | None" = None):
         self.problem = problem
+        self.context = context  # kept alive as long as the session
         res, n = C.c_int(), C.c_int()
-        self.ptr = lib().kh_cluster_open(problem.ptr, C.byref(res), C.byref(n))
+        if context is None:
+            self.ptr = lib().kh_cluster_open(problem.ptr, C.byref(res), C.byref(n))
+        else:
+            self.ptr = lib().kh_context_cluster_open(context.handle(), problem.ptr, C.byref(res), C.byref(n))
+            if self.ptr:
+                context._sessions.add(self)
         if not self.ptr:
             msg = lib().kh_scheduler_error().decode()
             raise KschedError(KSCHED_ERR_NO_DEVICE if "no usable CUDA device" in msg else KSCHED_ERR_INVALID, msg)
@@ -467,13 +528,17 @@ def nccl_allgather_i32(values, world):
 
 
 class MultiNodeConsolidation:
-    def __init__(self, problem: Problem):
+    """context: the Context its session() opens on (default: the process-wide handle); the one-call searches below run on
+    the process-wide handle."""
+
+    def __init__(self, problem: Problem, context: "Context | None" = None):
         self.problem = problem
+        self.context = context
         self._session = None
 
     def session(self):
         if self._session is None:
-            self._session = ClusterSession(self.problem)
+            self._session = ClusterSession(self.problem, context=self.context)
         return self._session
 
     def first_n_node_consolidation_option(self):

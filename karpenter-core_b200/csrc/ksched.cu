@@ -83,20 +83,79 @@ enum Counter : int {
   // class_run's fixed cost per call: open nodes at entry (summed), cycles from entry to the first loop iteration of the
   // eligible calls (of which the per-node inputs), write-back cycles, and the compactions with the slots they scanned and their cycles
   kCtrRunActiveSum, kCtrRunEntryCycles, kCtrRunInputCycles, kCtrRunWbCycles, kCtrRunCompacts, kCtrRunCompactSlots, kCtrRunCompactCycles,
+  kCtrPackStart, kCtrPackEnd,  // the pack launch's start and end (globaltimer ns): ksched_timings::pack_interval_ns
   kNumCounters
 };
 constexpr uint64_t kNoBest = ~0ull;
 
 #include "catalog.cuh"
 #include "feasibility_kernel.cuh"
+#include "pack_state.cuh"
+
+// Every kernel that reads a __constant__ parameter block (g_k1, g_k2), with the device functions it calls, compiled once
+// per parameter slot: each slot's copy reads its own blocks with the same immediate constant-bank offsets, so handles on
+// different slots of one device launch without waiting for each other (ksched_create assigns the slot).
+static_assert(KSCHED_PARAM_SLOTS == 2, "one namespace per parameter slot below");
+namespace slot0 {
+#include "class_feasibility.cuh"
 #include "topology.cuh"
+#include "pack_kernel.cuh"
+}  // namespace slot0
+namespace slot1 {
+#include "class_feasibility.cuh"
+#include "topology.cuh"
+#include "pack_kernel.cuh"
+}  // namespace slot1
+// Host-side sizes come from slot 0's declarations: every slot compiles the same source.
+using slot0::HotSmem;
+using slot0::kRunArrayBytes;
+using slot0::kVtClasses;
+using slot0::kM1Dom;
+
+// One slot's copies of the parameter-reading kernels and its two constant blocks.
+struct SlotKernels {
+  void (*pack[2][2])();  // [ext resources][block of at most kPackThreadsSmall threads]
+  void (*gather_table)(int, const ksched_pod_row*, const uint32_t*, const uint32_t*, uint64_t*, int);
+  void (*class_feasibility)();
+  const void* k1;  // &g_k1
+  const void* k2;  // &g_k2
+};
+#define KS_SLOT_KERNELS(ns)                                                                                                \
+  {{{ns::pack_kernel<false, kPackThreads>, ns::pack_kernel<false, kPackThreadsSmall>},                                     \
+    {ns::pack_kernel<true, kPackThreads>, ns::pack_kernel<true, kPackThreadsSmall>}},                                      \
+   ns::gather_rows_kernel<true>, ns::class_feasibility_kernel, &ns::g_k1, &ns::g_k2}
+const SlotKernels g_slot_kernels[KSCHED_PARAM_SLOTS] = {KS_SLOT_KERNELS(slot0), KS_SLOT_KERNELS(slot1)};
+#undef KS_SLOT_KERNELS
 
 }  // namespace
 
-#include "pack_kernel.cuh"
 #include "cluster.cuh"
 
 namespace {
+
+// options_true = options_stored AND Fits(requests): one warp per new node (resources.Fits, utils/resources/resources.go:138).
+__global__ void finalize_options_kernel(DevCatalog c, const long long* counters, const int64_t* nn_req, const uint32_t* nn_req_present,
+                                        uint32_t* nn_opts, int max_new) {
+  const int n_new = (int)counters[kCtrNewNodes];
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  for (int n = warp; n < n_new; n += nwarps) {
+    const uint32_t qp = nn_req_present[n];
+    int rank = 0;
+    if (lane < c.n_res && ((qp >> lane) & 1)) rank = fit_rank(c.alloc_sorted, c.n_types, lane, nn_req[(size_t)lane * max_new + n]);
+    int ranks[KSCHED_MAX_RES];
+#pragma unroll
+    for (int r = 0; r < KSCHED_MAX_RES; ++r) ranks[r] = __shfl_sync(0xffffffffu, rank, r);  // every lane takes part
+    for (int w = lane; w < c.W32; w += 32) {
+      uint32_t sw = nn_opts[(size_t)w * max_new + n];
+#pragma unroll
+      for (int r = 0; r < KSCHED_MAX_RES; ++r)
+        if (r < c.n_res && ((qp >> r) & 1)) sw &= c.fitset[((size_t)r * (c.n_types + 1) + ranks[r]) * c.W32 + w];
+      nn_opts[(size_t)w * max_new + n] = sw;
+    }
+  }
+}
+
 
 // Launch choice per finished new node (launch.cuh): one warp per node, lanes over the words of its final option set.
 __global__ void launch_choice_kernel(DevCatalog c, const long long* counters, const uint64_t* nn_vals, const uint64_t* nn_meta,
@@ -191,6 +250,7 @@ struct ksched_handle {
   K2Params k2_host;  // staging copy of the pack kernel's constant-memory parameters (must outlive the async copy)
   int k1_plan[5] = {};  // last class pass: blocks, rows per warp, cacheable, alloc_in_smem, tables_in_smem (tests)
   int device = 0;
+  int slot = 0;  // parameter slot on `device` (ksched_create): which g_k1 / g_k2 and kernel copies this handle's launches use
   int n_sm = 132;  // streaming multiprocessors of `device` (grid sizes of the grid-stride kernels)
   cudaStream_t stream = nullptr;
   std::string err;
@@ -388,6 +448,10 @@ int ksched_device_count(void) {
   return n;
 }
 
+// Live handles per (device, parameter slot): ksched_create takes the least used slot of its device, ksched_destroy gives it back.
+static std::mutex g_slot_mu;
+static int g_slot_users[64][KSCHED_PARAM_SLOTS] = {};
+
 int ksched_create(int device_ordinal, ksched_handle** out) {
   if (!out) return KSCHED_ERR_INVALID;
   int n = 0;
@@ -401,18 +465,22 @@ int ksched_create(int device_ordinal, ksched_handle** out) {
     return KSCHED_ERR_CUDA;
   }
   for (auto& e : h->ev) cudaEventCreate(&e);
+  if (device_ordinal < 64) {
+    std::lock_guard<std::mutex> lock(g_slot_mu);
+    const int* users = g_slot_users[device_ordinal];
+    for (int q = 1; q < KSCHED_PARAM_SLOTS; ++q) if (users[q] < users[h->slot]) h->slot = q;
+    ++g_slot_users[device_ordinal][h->slot];
+  }
   {
     // CUDA loads kernels lazily on first launch: pull ours in here, not inside the first Solve
+    const SlotKernels& sk = g_slot_kernels[h->slot];
     cudaFuncAttributes fa;
-    cudaFuncGetAttributes(&fa, pack_kernel<false, kPackThreadsSmall>);
-    cudaFuncGetAttributes(&fa, pack_kernel<true, kPackThreadsSmall>);
-    cudaFuncGetAttributes(&fa, pack_kernel<false, kPackThreads>);
-    cudaFuncGetAttributes(&fa, pack_kernel<true, kPackThreads>);
+    for (auto& by_ext : sk.pack) for (auto kern : by_ext) cudaFuncGetAttributes(&fa, kern);
     cudaFuncGetAttributes(&fa, feasibility_kernel);
-    cudaFuncGetAttributes(&fa, class_feasibility_kernel);
+    cudaFuncGetAttributes(&fa, sk.class_feasibility);
     cudaFuncGetAttributes(&fa, finalize_options_kernel);
-    cudaFuncGetAttributes(&fa, gather_rows_kernel<false>);
-    cudaFuncGetAttributes(&fa, gather_rows_kernel<true>);
+    cudaFuncGetAttributes(&fa, slot0::gather_rows_kernel<false>);
+    cudaFuncGetAttributes(&fa, sk.gather_table);
     cudaFuncGetAttributes(&fa, sort_key1_kernel);
   }
   *out = h;
@@ -425,6 +493,10 @@ void ksched_destroy(ksched_handle* h) {
   if (h->comm) ncclCommDestroy(h->comm);
   for (auto& e : h->ev) if (e) cudaEventDestroy(e);
   if (h->stream) cudaStreamDestroy(h->stream);
+  if (h->device < 64) {
+    std::lock_guard<std::mutex> lock(g_slot_mu);
+    --g_slot_users[h->device][h->slot];
+  }
   delete h;  // every DevBuf frees its allocation
 }
 
@@ -1230,10 +1302,11 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
 }
 
 // K0 over the first P pods (a simulation's batch, otherwise the whole problem); so are run_class_feasibility and run_feasibility.
-// g_k2 is one __constant__ object per device: a launch may only overwrite it after the previous launch that reads it (the pack kernel, the variant table build) on that
-// device (possibly of another handle, on another stream) has finished. Ordered on the device, never on the host.
-static std::mutex g_k2_mu;
-static cudaEvent_t g_k2_done[64] = {};
+// g_k2 is one __constant__ object per (device, parameter slot): a launch may only overwrite it after the previous launch that reads
+// it (the pack kernel, the variant table build) on that device and slot (possibly of another handle, on another stream) has
+// finished. Ordered on the device, never on the host; handles on different slots do not wait for each other.
+static std::mutex g_k2_mu[64][KSCHED_PARAM_SLOTS];
+static cudaEvent_t g_k2_done[64][KSCHED_PARAM_SLOTS] = {};
 static int set_k2(ksched_handle* h, int n_pods, int stop_new_nodes, bool with_table);
 // with_table: the row gather's launch also builds the pack kernel's variant table (vt_build_block), for the pack launch
 // that follows with the same flag
@@ -1248,15 +1321,17 @@ static int run_sort(ksched_handle* h, int P, bool with_table = false) {
                                               h->stream));
   const int gblocks = std::min((P + 7) / 8, h->n_sm * 8);
   if (with_table) {  // g_k2 is read by the table blocks: the same lock and ordering as run_pack
-    std::lock_guard<std::mutex> lock(g_k2_mu);
+    if (h->device < 0 || h->device >= 64) { h->err = "device ordinal out of range"; return KSCHED_ERR_INVALID; }
+    std::lock_guard<std::mutex> lock(g_k2_mu[h->device][h->slot]);
     int rc = set_k2(h, P, 0, true);
     if (rc != KSCHED_OK) return rc;
     const int vt_blocks = h->k2_host.st.vt_classes * h->vt_ndom;
-    gather_rows_kernel<true><<<gblocks + vt_blocks, 256, 0, h->stream>>>(P, h->d_classes.ptr, h->d_pod_class.ptr, h->d_order.ptr, h->d_rows.ptr, gblocks);
+    g_slot_kernels[h->slot].gather_table<<<gblocks + vt_blocks, 256, 0, h->stream>>>(P, h->d_classes.ptr, h->d_pod_class.ptr, h->d_order.ptr,
+                                                                                     h->d_rows.ptr, gblocks);
     CUDA_TRY(h, cudaGetLastError());
-    CUDA_TRY(h, cudaEventRecord(g_k2_done[h->device], h->stream));
+    CUDA_TRY(h, cudaEventRecord(g_k2_done[h->device][h->slot], h->stream));
   } else {
-    gather_rows_kernel<false><<<gblocks, 256, 0, h->stream>>>(P, h->d_classes.ptr, h->d_pod_class.ptr, h->d_order.ptr, h->d_rows.ptr, gblocks);
+    slot0::gather_rows_kernel<false><<<gblocks, 256, 0, h->stream>>>(P, h->d_classes.ptr, h->d_pod_class.ptr, h->d_order.ptr, h->d_rows.ptr, gblocks);
   }
   h->tm.sort_launches = 3;
   h->sorted = true;
@@ -1282,8 +1357,8 @@ static void fill_k1(ksched_handle* h, K1Params& k1) {
   }
 }
 
-static std::mutex g_k1_mu;
-static cudaEvent_t g_k1_done[64] = {};
+static std::mutex g_k1_mu[64][KSCHED_PARAM_SLOTS];
+static cudaEvent_t g_k1_done[64][KSCHED_PARAM_SLOTS] = {};
 
 // K1, class pass: every distinct pod row evaluated once (class_feasibility_kernel over the class table).
 static int run_class_feasibility(ksched_handle* h, int P) {
@@ -1316,17 +1391,18 @@ static int run_class_feasibility(ksched_handle* h, int P) {
   k1.dbg = h->d_k1dbg.ptr;
 #endif
   {
-    std::lock_guard<std::mutex> lock(g_k1_mu);  // one __constant__ parameter block per device: see run_pack
     if (h->device < 0 || h->device >= 64) { h->err = "device ordinal out of range"; return KSCHED_ERR_INVALID; }
-    cudaEvent_t& done = g_k1_done[h->device];
+    std::lock_guard<std::mutex> lock(g_k1_mu[h->device][h->slot]);  // one __constant__ parameter block per device and slot: see run_pack
+    const SlotKernels& sk = g_slot_kernels[h->slot];
+    cudaEvent_t& done = g_k1_done[h->device][h->slot];
     if (!done) CUDA_TRY(h, cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
     CUDA_TRY(h, cudaStreamWaitEvent(h->stream, done, 0));
     h->k1_host = k1;
-    CUDA_TRY(h, cudaMemcpyToSymbolAsync(g_k1, &h->k1_host, sizeof(K1Params), 0, cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(h, cudaFuncSetAttribute(class_feasibility_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));  // per function: under the launch lock
+    CUDA_TRY(h, cudaMemcpyToSymbolAsync(sk.k1, &h->k1_host, sizeof(K1Params), 0, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(h, cudaFuncSetAttribute(sk.class_feasibility, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));  // per function: under the launch lock
     if (h->world > 1)  // column words of the other shards read as 0
       CUDA_TRY(h, cudaMemsetAsync(h->d_Fclass.ptr, 0, (size_t)NC * c.n_templates * c.W32 * 4, h->stream));
-    class_feasibility_kernel<<<blocks, kK1Threads, smem, h->stream>>>();
+    sk.class_feasibility<<<blocks, kK1Threads, smem, h->stream>>>();
     CUDA_TRY(h, cudaGetLastError());
     CUDA_TRY(h, cudaEventRecord(done, h->stream));
   }
@@ -1392,7 +1468,8 @@ static int reset_state(ksched_handle* h, const int64_t* sim_remaining = nullptr)
 }
 
 
-// The pack kernel's parameters into g_k2 (caller holds g_k2_mu), once the previous reader of g_k2 on the device is done.
+// The pack kernel's parameters into the handle's slot of g_k2 (caller holds its g_k2_mu), once the previous reader of that
+// block on the device is done.
 // with_table: the launch replays the variant table a run_sort(with_table) of this Solve built.
 static int set_k2(ksched_handle* h, int n_pods, int stop_new_nodes, bool with_table) {
   K2Params& k2 = h->k2_host;
@@ -1421,11 +1498,10 @@ static int set_k2(ksched_handle* h, int n_pods, int stop_new_nodes, bool with_ta
   s.vt_ndom = h->vt_ndom;
   s.use_round_stretch = std::getenv("KSCHED_NO_ROUNDSTRETCH") ? 0 : 1;
   s.use_fill_stretch = s.use_round_stretch && !std::getenv("KSCHED_NO_FILLSTRETCH") ? 1 : 0;
-  if (h->device < 0 || h->device >= 64) { h->err = "device ordinal out of range"; return KSCHED_ERR_INVALID; }
-  cudaEvent_t& done = g_k2_done[h->device];
+  cudaEvent_t& done = g_k2_done[h->device][h->slot];
   if (!done) CUDA_TRY(h, cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
   CUDA_TRY(h, cudaStreamWaitEvent(h->stream, done, 0));  // no-op for an event that was never recorded
-  CUDA_TRY(h, cudaMemcpyToSymbolAsync(g_k2, &k2, sizeof(K2Params), 0, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(h, cudaMemcpyToSymbolAsync(g_slot_kernels[h->slot].k2, &k2, sizeof(K2Params), 0, cudaMemcpyHostToDevice, h->stream));
   return KSCHED_OK;
 }
 
@@ -1437,15 +1513,15 @@ static int run_pack(ksched_handle* h, int n_pods, int stop_new_nodes, bool with_
   int threads = h->st.n_existing >= 2048 ? kPackThreads : (h->st.n_existing >= 256 ? 256 : 128);
   if (const char* e = getenv("KSCHED_PACK_THREADS")) { int v = atoi(e); if (v >= 32 && v <= kPackThreads && v % 32 == 0) threads = v; }
   {
-    std::lock_guard<std::mutex> lock(g_k2_mu);
+    if (h->device < 0 || h->device >= 64) { h->err = "device ordinal out of range"; return KSCHED_ERR_INVALID; }
+    std::lock_guard<std::mutex> lock(g_k2_mu[h->device][h->slot]);
     int rc = set_k2(h, n_pods, stop_new_nodes, with_table);
     if (rc != KSCHED_OK) return rc;
-    cudaEvent_t& done = g_k2_done[h->device];
+    cudaEvent_t& done = g_k2_done[h->device][h->slot];
     const size_t smem = sizeof(HotSmem) + (size_t)s.run_off + kRunArrayBytes;
     // the attribute belongs to the function, not to the handle: set it under the same lock as the launch
     const bool ext = h->cat.n_res_ext > 0, small = threads <= kPackThreadsSmall;
-    void (*kern)() = small ? (ext ? pack_kernel<true, kPackThreadsSmall> : pack_kernel<false, kPackThreadsSmall>)
-                           : (ext ? pack_kernel<true, kPackThreads> : pack_kernel<false, kPackThreads>);
+    void (*kern)() = g_slot_kernels[h->slot].pack[ext][small];
     cudaFuncAttributes fa;
     CUDA_TRY(h, cudaFuncGetAttributes(&fa, kern));
     if (threads > fa.maxThreadsPerBlock) {  // the instantiation's register budget does not fit this block
@@ -1609,6 +1685,8 @@ int ksched_download(ksched_handle* h, const ksched_problem* pb, ksched_result* r
   h->tm.vt_fetches = counters[kCtrVtFetches];
   h->tm.run_derives = counters[kCtrRunDerives];
   h->tm.vt_build_us = counters[kCtrVtEnd] ? (double)(counters[kCtrVtEnd] - (long long)~(unsigned long long)counters[kCtrVtStart]) / 1000.0 : 0.0;
+  h->tm.pack_interval_ns[0] = counters[kCtrPackStart];
+  h->tm.pack_interval_ns[1] = counters[kCtrPackEnd];
   if (res->assign) CUDA_TRY(h, download(h, res->assign, s.assign, (size_t)P));
   if (res->relax_level) CUDA_TRY(h, download(h, res->relax_level, s.relax_level, (size_t)P));
   if (res->place_seq) CUDA_TRY(h, download(h, res->place_seq, s.place_seq, (size_t)P));
@@ -1863,6 +1941,8 @@ int ksched_simulate_batch(ksched_handle* h, const ksched_candidate_set* sets, in
   std::vector<uint32_t> types((size_t)n_sets * W32);
   CUDA_TRY(h, cudaMemcpyAsync(dev.data(), h->d_sim_results.ptr, dev.size() * sizeof(SimResultDev), cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaMemcpyAsync(types.data(), h->d_sim_types.ptr, types.size() * 4, cudaMemcpyDeviceToHost, h->stream));
+  // the last simulation's pack launch (its counters stay until the next reset)
+  CUDA_TRY(h, cudaMemcpyAsync(h->tm.pack_interval_ns, h->d_counters.ptr + kCtrPackStart, 2 * sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   CUDA_TRY(h, cudaGetLastError());
   h->tm.total_us = ev_us(h->ev[0], h->ev[4]);
@@ -1960,6 +2040,8 @@ int ksched_simulate_full(ksched_handle* h, const ksched_candidate_set* sets, int
     if (X && r.new_node_requests_ext_present) CUDA_TRY(h, download(h, r.new_node_requests_ext_present, h->d_full_ext_present.ptr + o, P));
   }
   CUDA_TRY(h, download(h, sc.data(), h->d_full_scalars.ptr, sc.size()));
+  // the last simulation's pack launch (its counters stay until the next reset)
+  CUDA_TRY(h, cudaMemcpyAsync(h->tm.pack_interval_ns, h->d_counters.ptr + kCtrPackStart, 2 * sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   CUDA_TRY(h, cudaGetLastError());
   h->tm.total_us = ev_us(h->ev[0], h->ev[4]);

@@ -17,9 +17,7 @@
 //    checks / narrows the winner's instance-type words (exclude + retry when it fails);
 //  * parameters come from __constant__ memory (g_k2), the per-CTA working set is file-scope __shared__: out-of-line
 //    functions reach both with immediate addresses.
-#pragma once
-
-namespace {
+// Part of the single translation unit ksched.cu, which includes it once per parameter slot (after topology.cuh).
 
 constexpr int kActCap = 1280;  // open in-flight nodes whose hot state is held in shared memory
 constexpr int kHotRes = 4;     // resources covered by the hot request / bound vectors (cpu, memory, pods, +1)
@@ -145,13 +143,6 @@ __device__ __forceinline__ bool node_closed(const long long* q, const long long*
   return (fl & kFlTwo) ? (o1 && o2) : o1;
 }
 
-// 64-bit min over a warp with two 32-bit REDUX operations (hi word first, then lo word among the hi-minimal lanes)
-__device__ __forceinline__ unsigned long long warp_min_u64(unsigned long long v) {
-  const unsigned hi = (unsigned)(v >> 32), lo = (unsigned)v;
-  const unsigned mhi = __reduce_min_sync(0xffffffffu, hi);
-  const unsigned mlo = __reduce_min_sync(0xffffffffu, hi == mhi ? lo : 0xffffffffu);
-  return ((unsigned long long)mhi << 32) | mlo;
-}
 // single-sync block argmin (double-buffered scratch)
 __device__ __forceinline__ unsigned long long block_min_u64_db(unsigned long long v, unsigned long long (*red)[32], int& parity) {
   v = warp_min_u64(v);
@@ -1309,17 +1300,9 @@ constexpr unsigned kRoomSlow = 0xFFFFu, kRoomMax = 0x7FFEu, kRpDead = 0x80000000
 enum StopCause : int { kStopNone, kStopNoVariant, kStopRoomSlow, kStopCapacity, kStopOther };
 constexpr size_t kRunArrayBytes = (size_t)kTopoCap * (kRunMask * 4 + kRunHost * 2) + (size_t)kActCap * 4;
 
-struct RunVariant {
-  uint32_t opts[kRunW32];
-  uint64_t vals[KSCHED_MAX_KEYS];
-  uint64_t meta;
-  long long q[KSCHED_MAX_RES];
-  long long b1[kHotRes], b2[kHotRes];
-  uint32_t qp;
-  uint32_t rp;            // room of the fresh node for further pods of the class (+ dead flag)
-  unsigned short fl;      // HotSmem::flags of the fresh node (front bits, request keys, template)
-  uint8_t dom[kRunMask];  // domain each spread relation pinned
-};
+// RunVariant lives in pack_state.cuh (PackState points at the variant table) with the same three sizes
+static_assert(sizeof(RunVariant::b1) == kHotRes * sizeof(long long) && sizeof(RunVariant::dom) == kRunMask && sizeof(RunVariant::opts) == kRunW32 * 4,
+              "RunVariant is sized by kHotRes, kRunMask and kRunW32");
 struct RunCtx {
   uint32_t cls;           // class the relation tables and variants belong to (KSCHED_NONE: none)
   int eligible;
@@ -3248,6 +3231,11 @@ __global__ void __launch_bounds__(kMaxThreads, 1) pack_kernel() {
 #endif
   KS_K2
   const int tid = threadIdx.x;
+  if (tid == 0) {  // the launch's start (ksched_timings::pack_interval_ns)
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    s.counters[kCtrPackStart] = (long long)t;
+  }
   const int NE = s.n_existing, MAXN = s.max_new;
   const int R = c.n_res, RH = R < kHotRes ? R : kHotRes;
 
@@ -3457,34 +3445,12 @@ __global__ void __launch_bounds__(kMaxThreads, 1) pack_kernel() {
     s.counters[kCtrAddCalls] = add_calls;
     s.counters[kCtrError] = fatal;
     s.counters[kCtrSteps] = add_calls;
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    s.counters[kCtrPackEnd] = (long long)t;
 #ifdef KSCHED_PROFILE_PACK
     s.counters[kCtrRunCallCycles] = pk_acc[1];
     s.counters[kCtrGenCallCycles] = pk_acc[5];  // (incl. the call)
 #endif
   }
 }
-
-// options_true = options_stored AND Fits(requests): one warp per new node (resources.Fits, utils/resources/resources.go:138).
-__global__ void finalize_options_kernel(DevCatalog c, const long long* counters, const int64_t* nn_req, const uint32_t* nn_req_present,
-                                        uint32_t* nn_opts, int max_new) {
-  const int n_new = (int)counters[kCtrNewNodes];
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  for (int n = warp; n < n_new; n += nwarps) {
-    const uint32_t qp = nn_req_present[n];
-    int rank = 0;
-    if (lane < c.n_res && ((qp >> lane) & 1)) rank = fit_rank(c.alloc_sorted, c.n_types, lane, nn_req[(size_t)lane * max_new + n]);
-    int ranks[KSCHED_MAX_RES];
-#pragma unroll
-    for (int r = 0; r < KSCHED_MAX_RES; ++r) ranks[r] = __shfl_sync(0xffffffffu, rank, r);  // every lane takes part
-    for (int w = lane; w < c.W32; w += 32) {
-      uint32_t sw = nn_opts[(size_t)w * max_new + n];
-#pragma unroll
-      for (int r = 0; r < KSCHED_MAX_RES; ++r)
-        if (r < c.n_res && ((qp >> r) & 1)) sw &= c.fitset[((size_t)r * (c.n_types + 1) + ranks[r]) * c.W32 + w];
-      nn_opts[(size_t)w * max_new + n] = sw;
-    }
-  }
-}
-
-}  // namespace

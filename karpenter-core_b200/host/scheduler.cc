@@ -5,12 +5,14 @@
 // Everything that decides a placement runs on the GPU through ksched_* (include/ksched.h). There is NO CPU
 // fallback: without a CUDA device every call here fails with KSCHED_ERR_NO_DEVICE.
 #include <algorithm>
+#include <atomic>
 #include <chrono>
 #include <cstring>
 #include <limits>
 #include <map>
 #include <stdexcept>
 #include <memory>
+#include <mutex>
 #include <set>
 #include <string>
 #include <thread>
@@ -26,15 +28,32 @@
 using namespace kmodel;
 using khost::Encoded;
 
+// A scheduler context: one device handle and the session-displacement bookkeeping of the snapshot it holds. The kh_*
+// functions without a context argument share one process-wide context (g_default); kh_context_create makes others.
+struct kh_context {
+  ksched_handle* h = nullptr;
+  int device = 0;
+  // h holds one cluster snapshot at a time: the id of the ClusterSession whose snapshot it holds, 0 when anything else
+  // (a Solve, a fresh-encode simulation, ResidentSolve, another session) has been loaded onto it since
+  uint64_t resident_session = 0;
+};
+
 namespace {
 
 thread_local std::string g_err;
-ksched_handle* g_handle = nullptr;
-int g_device = 0;
-// g_handle holds one cluster snapshot at a time: the id of the ClusterSession whose snapshot it holds, 0 when anything else
-// (a Solve, a fresh-encode simulation, ResidentSolve, another session) has been loaded onto it since
-uint64_t g_resident_session = 0;
-uint64_t g_last_session = 0;
+kh_context g_default;
+ksched_handle*& g_handle = g_default.h;
+int& g_device = g_default.device;
+uint64_t& g_resident_session = g_default.resident_session;
+std::atomic<uint64_t> g_last_session{0};
+// Serializes the kh_* functions that use the process-wide context, so that threads calling them do not race on g_handle.
+// Contexts of their own take no lock: each is used by one thread at a time.
+std::recursive_mutex g_default_mu;
+#define KH_DEFAULT_LOCK std::lock_guard<std::recursive_mutex> default_lock(g_default_mu)
+// the same lock for work on ctx, taken only when ctx is the process-wide context
+std::unique_lock<std::recursive_mutex> lock_if_default(const kh_context* ctx) {
+  return ctx == &g_default ? std::unique_lock<std::recursive_mutex>(g_default_mu) : std::unique_lock<std::recursive_mutex>();
+}
 // The same for ResidentSolve (kh_gpu_*): the encoding kh_gpu_load / kh_gpu_solve_e2e last put on g_handle, and whether
 // g_handle still holds it. kh_gpu_run loads it again when something else took the handle since.
 const Encoded* g_gpu_encoded = nullptr;
@@ -45,12 +64,20 @@ void handle_taken() {
   g_resident_session = 0;
   g_gpu_current = false;
 }
+// the same for any context
+void context_taken(kh_context* ctx) {
+  if (ctx == &g_default) handle_taken();
+  else ctx->resident_session = 0;
+}
 }  // namespace
 
 int ksched_k1_plan(const ksched_handle* h, int out[5]);  // csrc/ksched.cu, outside the C-ABI
+extern "C" int kh_context_solve(kh_context* ctx, const Problem* P, const int* candidates, int ncand, Result* out);
 
 namespace {
-int g_count_visited = 0;  // exact nodes_visited statistic (opt-in: tests); switches the pack kernel's steady-state paths off
+// exact nodes_visited statistic (opt-in: tests); switches the pack kernel's steady-state paths off. Per calling thread, so that
+// one controller's setting never reaches another context's Solves and simulations.
+thread_local int g_count_visited = 0;
 
 int fail(int code, const std::string& msg) {
   g_err = msg;
@@ -61,6 +88,12 @@ int ensure_handle() {
   int rc = ksched_create(g_device, &g_handle);
   if (rc != KSCHED_OK) return fail(rc, "ksched_create failed: no usable CUDA device (the product has no CPU path)");
   return KSCHED_OK;
+}
+// ctx's handle, created on first use for the process-wide context
+ksched_handle* context_handle(kh_context* ctx) {
+  if (ctx != &g_default) return ctx->h;
+  if (ensure_handle() != KSCHED_OK) throw std::runtime_error(g_err);
+  return g_handle;
 }
 
 struct ResultBuffers {
@@ -231,14 +264,16 @@ int error_code(const std::exception& e) {
   return m.rfind("unsupported:", 0) == 0 ? KSCHED_ERR_UNSUPPORTED : KSCHED_ERR_INVALID;
 }
 
-// One ksched_solve of E on h (default: the scheduler handle, whose cluster snapshot this displaces).
-int solve_encoded(Encoded& E, ResultBuffers& B, bool want_feasibility, ksched_handle* h = nullptr) {
+// One ksched_solve of E on h, or without h on ctx's handle, whose cluster snapshot this displaces.
+int solve_encoded(Encoded& E, ResultBuffers& B, bool want_feasibility, ksched_handle* h = nullptr, kh_context* ctx = &g_default) {
   if (!h) {
-    int rc = ensure_handle();
-    if (rc != KSCHED_OK) return rc;
-    h = g_handle;
+    if (ctx == &g_default) {
+      int rc = ensure_handle();
+      if (rc != KSCHED_OK) return rc;
+    }
+    h = ctx->h;
   }
-  if (h == g_handle) handle_taken();
+  if (h == ctx->h) context_taken(ctx);
   int rc = ksched_load_catalog(h, &E.catalog);
   if (rc != KSCHED_OK) return fail(rc, ksched_last_error(h));
   B.prepare(E, want_feasibility);
@@ -288,6 +323,7 @@ extern "C" {
 
 const char* kh_scheduler_error() { return g_err.c_str(); }
 int kh_set_device(int ordinal) {
+  KH_DEFAULT_LOCK;
   if (g_handle) { ksched_destroy(g_handle); g_handle = nullptr; }
   handle_taken();
   g_gpu_encoded = nullptr;
@@ -295,25 +331,14 @@ int kh_set_device(int ordinal) {
   return KSCHED_OK;
 }
 void kh_set_count_visited(int on) { g_count_visited = on; }
-ksched_handle* kh_handle() { return ensure_handle() == KSCHED_OK ? g_handle : nullptr; }
+ksched_handle* kh_handle() {
+  KH_DEFAULT_LOCK;
+  return ensure_handle() == KSCHED_OK ? g_handle : nullptr;
+}
 
 // Scheduler.Solve through the C-ABI with host buffers (upload + kernels + download inside the call).
 int kh_scheduler_solve(const Problem* P, const int* candidates, int ncand, Result* out) {
-  *out = Result();
-  try {
-    std::vector<int> c(candidates, candidates + ncand);
-    auto E = khost::encode(*P, c);
-    E->problem.count_nodes_visited = g_count_visited;
-    static thread_local ResultBuffers B;
-    int rc = solve_encoded(*E, B, false);
-    if (rc != KSCHED_OK) { out->error = g_err; return rc; }
-    decode(*E, B, *out);
-    set_verdicts(*E, B, *out);
-    return KSCHED_OK;
-  } catch (const std::exception& e) {
-    out->error = e.what();
-    return fail(error_code(e), e.what());
-  }
+  return kh_context_solve(&g_default, P, candidates, ncand, out);
 }
 
 // The same call with its host phases timed (bench.py's end-to-end leg): phases_us = [encode, catalog, solve, decode, total].
@@ -321,6 +346,7 @@ int kh_scheduler_solve(const Problem* P, const int* candidates, int ncand, Resul
 // byte-identical catalog is already resident); solve = ksched_solve (upload + kernels + download); decode = the
 // ([]*Node, []*ExistingNode) shape.
 int kh_scheduler_solve_timed(const Problem* P, const int* candidates, int ncand, Result* out, double* phases_us) {
+  KH_DEFAULT_LOCK;
   *out = Result();
   try {
     using clk = std::chrono::steady_clock;
@@ -372,6 +398,7 @@ Encoded* kh_encode_cluster(const Problem* P, const int* candidates, int ncand) {
   }
 }
 void kh_encoded_free(Encoded* E) {
+  KH_DEFAULT_LOCK;
   if (E == g_gpu_encoded) { g_gpu_encoded = nullptr; g_gpu_current = false; }
   delete E;
 }
@@ -473,6 +500,7 @@ void kh_encoded_set_count_visited(Encoded* E, int on) { E->problem.count_nodes_v
 const ksched_catalog* kh_encoded_catalog(const Encoded* E) { return &E->catalog; }
 const ksched_problem* kh_encoded_problem(const Encoded* E) { return &E->problem; }
 int kh_gpu_load(Encoded* E) {
+  KH_DEFAULT_LOCK;
   int rc = ensure_handle();
   if (rc != KSCHED_OK) return rc;
   handle_taken();
@@ -491,6 +519,7 @@ int gpu_make_current() {
   return kh_gpu_load(const_cast<Encoded*>(g_gpu_encoded));
 }
 int kh_gpu_run(int flush_l2) {
+  KH_DEFAULT_LOCK;
   if (!g_handle) return fail(KSCHED_ERR_INVALID, "no handle");
   int rc = gpu_make_current();
   if (rc != KSCHED_OK) return rc;
@@ -500,6 +529,7 @@ int kh_gpu_run(int flush_l2) {
   return rc;
 }
 int kh_gpu_run_feasibility(int flush_l2, float* us) {
+  KH_DEFAULT_LOCK;
   if (!g_handle) return fail(KSCHED_ERR_INVALID, "no handle");
   int rc = gpu_make_current();
   if (rc != KSCHED_OK) return rc;
@@ -511,6 +541,7 @@ int kh_gpu_run_feasibility(int flush_l2, float* us) {
 // download + decode; feasibility_out (optional) receives [pods][templates][type_words] uint64 in caller pod order,
 // columns in the caller's instance-type order (bit i of template v = instance_types[i])
 int kh_gpu_download(Encoded* E, Result* out, unsigned long long* feasibility_out, unsigned long long* best_out) {
+  KH_DEFAULT_LOCK;
   if (!g_handle) return fail(KSCHED_ERR_INVALID, "no handle");
   *out = Result();
   if (g_gpu_encoded && !g_gpu_current) return fail(KSCHED_ERR_INVALID, "the handle was used for other work since this problem's run: run it again");
@@ -536,6 +567,7 @@ int kh_gpu_download(Encoded* E, Result* out, unsigned long long* feasibility_out
 // One Scheduler.Solve through the C-ABI with HOST buffers: pod/node/topology upload, kernels and result download are
 // all inside the call (the catalog stays resident, as it would across reconciles). Returns wall-clock microseconds.
 int kh_gpu_solve_e2e(Encoded* E, Result* out, double* wall_us) {
+  KH_DEFAULT_LOCK;
   if (!g_handle) return fail(KSCHED_ERR_INVALID, "no handle");
   handle_taken();
   g_gpu_encoded = nullptr;
@@ -552,6 +584,7 @@ int kh_gpu_solve_e2e(Encoded* E, Result* out, double* wall_us) {
   return KSCHED_OK;
 }
 int kh_gpu_load_catalog(Encoded* E) {
+  KH_DEFAULT_LOCK;
   int rc = ensure_handle();
   if (rc != KSCHED_OK) return rc;
   g_resident_session = 0;
@@ -559,9 +592,16 @@ int kh_gpu_load_catalog(Encoded* E) {
   if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
   return KSCHED_OK;
 }
-int kh_gpu_timings(ksched_timings* t) { return g_handle ? ksched_get_timings(g_handle, t) : KSCHED_ERR_INVALID; }
-int kh_gpu_k1_plan(int* out) { return g_handle ? ksched_k1_plan(g_handle, out) : fail(KSCHED_ERR_INVALID, "no handle"); }
+int kh_gpu_timings(ksched_timings* t) {
+  KH_DEFAULT_LOCK;
+  return g_handle ? ksched_get_timings(g_handle, t) : KSCHED_ERR_INVALID;
+}
+int kh_gpu_k1_plan(int* out) {
+  KH_DEFAULT_LOCK;
+  return g_handle ? ksched_k1_plan(g_handle, out) : fail(KSCHED_ERR_INVALID, "no handle");
+}
 int kh_gpu_set_shard(int rank, int world) {
+  KH_DEFAULT_LOCK;
   int rc = ensure_handle();
   if (rc != KSCHED_OK) return rc;
   rc = ksched_set_shard(g_handle, rank, world);
@@ -601,12 +641,12 @@ bool candidate_node(const Problem* P, const StateNode& n, const Provisioner** pr
 // candidateNodes + sortAndFilterCandidates (deprovisioning/helpers.go:171-249,339-366, consolidation.go:85-118). The string /
 // API-object side (labels, annotations, PDB selectors) is decided here; the disruption costs, their lifetime scaling and the
 // order come from the device (ksched_rank_candidates) - there is no host-side sort to fall back to.
-void rank_on_device(const Problem* P, std::vector<int>* order, std::vector<double>* cost) {
+void rank_on_device(const Problem* P, std::vector<int>* order, std::vector<double>* cost, kh_context* ctx = &g_default) {
   const size_t N = P->nodes.size();
   order->clear();
   cost->clear();
   if (N == 0) return;
-  if (ensure_handle() != KSCHED_OK) throw std::runtime_error(g_err);
+  ksched_handle* h = context_handle(ctx);
   std::vector<uint8_t> eligible(N, 0), flags;
   std::vector<int32_t> off(N + 1, 0), prio;
   std::vector<double> dc, age(N, 0.0), ttl(N, -1.0), given(N, 0.0);
@@ -647,16 +687,16 @@ void rank_on_device(const Problem* P, std::vector<int>* order, std::vector<doubl
   std::vector<int32_t> ord(N);
   std::vector<double> cst(N);
   int32_t n = 0;
-  int rc = ksched_rank_candidates(g_handle, &in, ord.data(), cst.data(), &n);
-  if (rc != KSCHED_OK) throw std::runtime_error(ksched_last_error(g_handle));
+  int rc = ksched_rank_candidates(h, &in, ord.data(), cst.data(), &n);
+  if (rc != KSCHED_OK) throw std::runtime_error(ksched_last_error(h));
   order->assign(ord.begin(), ord.begin() + n);
   cost->assign(cst.begin(), cst.begin() + n);
 }
 
-std::vector<Cand> sorted_candidates(const Problem* P) {
+std::vector<Cand> sorted_candidates(const Problem* P, kh_context* ctx = &g_default) {
   std::vector<int> order;
   std::vector<double> cost;
-  rank_on_device(P, &order, &cost);
+  rank_on_device(P, &order, &cost, ctx);
   std::vector<Cand> cands;
   for (size_t q = 0; q < order.size(); ++q) {
     const StateNode& n = P->nodes[(size_t)order[q]];
@@ -747,13 +787,13 @@ Cmd finish_command(const Problem* P, const Encoded& E, const std::vector<Cand>& 
 }
 
 // One simulateScheduling = one ksched_solve of a freshly encoded problem (the path for clusters the snapshot cannot hold).
-Cmd compute_consolidation_encoded(const Problem* P, const std::vector<Cand>& sel, bool multi) {
+Cmd compute_consolidation_encoded(const Problem* P, const std::vector<Cand>& sel, bool multi, kh_context* ctx) {
   std::vector<int> nodes;
   for (auto& c : sel) nodes.push_back(c.node);
   auto E = khost::encode(*P, nodes);
   E->problem.count_nodes_visited = g_count_visited;
   ResultBuffers B;
-  int rc = solve_encoded(*E, B, false);
+  int rc = solve_encoded(*E, B, false, nullptr, ctx);
   if (rc != KSCHED_OK) throw std::runtime_error(g_err);
   size_t scheduled = 0;
   for (auto a : B.assign) if (a >= 0) ++scheduled;
@@ -875,7 +915,7 @@ struct ValidationSnapshot {
   std::vector<int> slot_of_node;
   bool resident = false;
 
-  explicit ValidationSnapshot(const Problem* a) : A(a), problem_id(a->id) {
+  ValidationSnapshot(const Problem* a, int device) : A(a), problem_id(a->id) {
     for (size_t i = 0; i < A->nodes.size(); ++i) {
       const StateNode& n = A->nodes[i];
       if (n.nominated) nominated.insert(n.name);
@@ -884,7 +924,7 @@ struct ValidationSnapshot {
       if (A->derive_candidates ? candidate_node(A, n, &prov) : n.candidate && !n.marked_for_deletion) cands.push_back((int)i);
     }
     ksched_handle* raw = nullptr;
-    if (ksched_create(g_device, &raw) != KSCHED_OK) throw std::runtime_error("ksched_create failed: no usable CUDA device (the product has no CPU path)");
+    if (ksched_create(device, &raw) != KSCHED_OK) throw std::runtime_error("ksched_create failed: no usable CUDA device (the product has no CPU path)");
     h.reset(raw);
     auto sup = khost::encode(*A, cands, true);
     sup->problem.count_nodes_visited = 0;
@@ -941,9 +981,10 @@ struct ValidationSnapshot {
 // The consolidation pass over one cluster: candidates ranked once, the cluster resident on the device once
 // (ksched_load_cluster), every computeConsolidation a ksched_simulate_batch entry. Clusters the snapshot cannot hold
 // (topology groups) are simulated one freshly encoded ksched_solve at a time - still on the GPU, never on the CPU.
-// Sessions share the scheduler handle: a session whose snapshot something else displaced loads it again before its next
-// batch (g_resident_session).
+// Sessions share their context's handle: a session whose snapshot something else displaced loads it again before its next
+// batch (kh_context::resident_session).
 struct ClusterSession {
+  kh_context* ctx = &g_default;
   const Problem* P = nullptr;
   std::vector<Cand> cands;            // disruption order
   std::unique_ptr<Encoded> E;         // superset encoding (resident == true)
@@ -953,22 +994,22 @@ struct ClusterSession {
   int simulations = 0;
   std::unique_ptr<ValidationSnapshot> validation_snapshot;  // opened at the first command that needs validation
 
-  explicit ClusterSession(const Problem* p) : P(p), cands(sorted_candidates(p)) {
-    if (ensure_handle() != KSCHED_OK) throw std::runtime_error(g_err);
+  explicit ClusterSession(const Problem* p, kh_context* c = &g_default) : ctx(c), P(p), cands(sorted_candidates(p, c)) {
+    ksched_handle* h = context_handle(ctx);
     std::vector<int> nodes;
     for (auto& c : cands) nodes.push_back(c.node);
     auto sup = khost::encode(*P, nodes, true);
     sup->problem.count_nodes_visited = 0;
-    handle_taken();
-    int rc = load_snapshot(g_handle, *sup, nodes);
+    context_taken(ctx);
+    int rc = load_snapshot(h, *sup, nodes);
     if (rc == KSCHED_ERR_UNSUPPORTED) return;  // resident stays false
-    if (rc != KSCHED_OK) throw std::runtime_error(ksched_last_error(g_handle));
+    if (rc != KSCHED_OK) throw std::runtime_error(ksched_last_error(h));
     E = std::move(sup);
     slot_of_node.assign(P->nodes.size(), -1);
     for (size_t e = 0; e < E->existing_state_index.size(); ++e) slot_of_node[(size_t)E->existing_state_index[e]] = (int)e;
     resident = true;
     id = ++g_last_session;
-    g_resident_session = id;
+    ctx->resident_session = id;
   }
 
   // computeConsolidation for every set (positions in the disruption order), one ksched_simulate_batch call
@@ -979,7 +1020,7 @@ struct ClusterSession {
       for (size_t q = 0; q < sets.size(); ++q) {
         std::vector<Cand> sel;
         for (int i : sets[q]) sel.push_back(cands.at((size_t)i));
-        out[q] = compute_consolidation_encoded(P, sel, multi);
+        out[q] = compute_consolidation_encoded(P, sel, multi, ctx);
       }
       return out;
     }
@@ -991,7 +1032,7 @@ struct ClusterSession {
         slots[q].push_back(e);
       }
     make_current();
-    SimBatch sb = simulate_on(g_handle, *E, slots);
+    SimBatch sb = simulate_on(ctx->h, *E, slots);
     for (size_t q = 0; q < sets.size(); ++q) {
       if (sb.skip[q]) continue;
       std::vector<Cand> sel;
@@ -1000,15 +1041,16 @@ struct ClusterSession {
     }
     return out;
   }
-  // the session's snapshot on g_handle again when something else displaced it: the time of one reload, the same answers
+  // the session's snapshot on its context's handle again when something else displaced it: the time of one reload, the same
+  // answers
   void make_current() {
-    if (g_resident_session == id) return;
-    if (ensure_handle() != KSCHED_OK) throw std::runtime_error(g_err);
-    handle_taken();
+    if (ctx->resident_session == id) return;
+    ksched_handle* h = context_handle(ctx);
+    context_taken(ctx);
     std::vector<int> nodes;
     for (auto& c : cands) nodes.push_back(c.node);
-    if (load_snapshot(g_handle, *E, nodes) != KSCHED_OK) throw std::runtime_error(ksched_last_error(g_handle));
-    g_resident_session = id;
+    if (load_snapshot(h, *E, nodes) != KSCHED_OK) throw std::runtime_error(ksched_last_error(h));
+    ctx->resident_session = id;
   }
 
   // simulateScheduling's whole result for every set (Problem.nodes indices, candidates of the session, in the caller's
@@ -1030,7 +1072,7 @@ struct ClusterSession {
         auto F = khost::encode(*P, sets[q]);
         F->problem.count_nodes_visited = g_count_visited;
         ResultBuffers B;
-        if (solve_encoded(*F, B, false) != KSCHED_OK) throw std::runtime_error(g_err);
+        if (solve_encoded(*F, B, false, nullptr, ctx) != KSCHED_OK) throw std::runtime_error(g_err);
         decode(*F, B, out[q]);
         set_verdicts(*F, B, out[q]);
       }
@@ -1058,7 +1100,7 @@ struct ClusterSession {
     make_current();
     std::vector<ksched_result> res(n);
     for (size_t q = 0; q < n; ++q) res[q] = B[q].r;
-    if (ksched_simulate_full(g_handle, cs.data(), (int)n, res.data()) != KSCHED_OK) throw std::runtime_error(ksched_last_error(g_handle));
+    if (ksched_simulate_full(ctx->h, cs.data(), (int)n, res.data()) != KSCHED_OK) throw std::runtime_error(ksched_last_error(ctx->h));
     std::vector<char> removed(P->nodes.size(), 0);
     for (size_t q = 0; q < n; ++q) {
       B[q].r = res[q];
@@ -1090,7 +1132,7 @@ struct ClusterSession {
   std::vector<char> validate(const Problem* after, const std::vector<VCmd>& cmds) {
     if (!validation_snapshot || validation_snapshot->problem_id != after->id) {
       validation_snapshot.reset();  // one extra device handle at a time
-      validation_snapshot = std::make_unique<ValidationSnapshot>(after);
+      validation_snapshot = std::make_unique<ValidationSnapshot>(after, ctx->device);
     }
     return validation_snapshot->validate(cmds);
   }
@@ -1162,10 +1204,12 @@ Sweep single_sweep(ClusterSession& cs, const Problem* after, int first, int last
 extern "C" {
 // number of consolidation candidates
 int kh_consolidate_candidates(const Problem* P) {
+  KH_DEFAULT_LOCK;
   try { return (int)sorted_candidates(P).size(); } catch (const std::exception& e) { return fail(error_code(e), e.what()); }
 }
 // candidate ranking on the device: order = Problem.nodes indices by disruption cost, cost parallel; returns their number
 int kh_rank_candidates(const Problem* P, int* order, double* cost, int cap) {
+  KH_DEFAULT_LOCK;
   try {
     std::vector<int> o;
     std::vector<double> c;
@@ -1177,11 +1221,54 @@ int kh_rank_candidates(const Problem* P, int* order, double* cost, int cap) {
   }
 }
 
-// A consolidation pass over one cluster (ClusterSession): open once, probe many times, close. The session keeps the
-// cluster resident on the device (ksched_load_cluster); `resident` tells whether the snapshot path took it.
-ClusterSession* kh_cluster_open(const Problem* P, int* resident, int* n_candidates) {
+// ---- scheduler contexts: a handle of their own on `device`, with the session bookkeeping g_default keeps for the others
+kh_context* kh_context_create(int device) {
+  auto* ctx = new kh_context();
+  ctx->device = device;
+  int rc = ksched_create(device, &ctx->h);
+  if (rc != KSCHED_OK) {
+    delete ctx;
+    fail(rc, "ksched_create failed: no usable CUDA device (the product has no CPU path)");
+    return nullptr;
+  }
+  return ctx;
+}
+void kh_context_destroy(kh_context* ctx) {
+  if (!ctx || ctx == &g_default) return;
+  ksched_destroy(ctx->h);
+  delete ctx;
+}
+// Scheduler.Solve on ctx's handle (kh_scheduler_solve on the process-wide one)
+int kh_context_solve(kh_context* ctx, const Problem* P, const int* candidates, int ncand, Result* out) {
+  if (!ctx || !P || !out || ncand < 0 || (ncand > 0 && !candidates)) return fail(KSCHED_ERR_INVALID, "null context, problem or result");
+  auto lock = lock_if_default(ctx);
+  *out = Result();
   try {
-    auto* cs = new ClusterSession(P);
+    std::vector<int> c(candidates, candidates + ncand);
+    auto E = khost::encode(*P, c);
+    E->problem.count_nodes_visited = g_count_visited;
+    static thread_local ResultBuffers B;
+    int rc = solve_encoded(*E, B, false, nullptr, ctx);
+    if (rc != KSCHED_OK) { out->error = g_err; return rc; }
+    decode(*E, B, *out);
+    set_verdicts(*E, B, *out);
+    return KSCHED_OK;
+  } catch (const std::exception& e) {
+    out->error = e.what();
+    return fail(error_code(e), e.what());
+  }
+}
+// ksched_get_timings of ctx's handle
+int kh_context_timings(kh_context* ctx, ksched_timings* t) {
+  if (!ctx || !t) return fail(KSCHED_ERR_INVALID, "null context or timings");
+  auto lock = lock_if_default(ctx);
+  return ctx->h ? ksched_get_timings(ctx->h, t) : fail(KSCHED_ERR_INVALID, "no handle");
+}
+ClusterSession* kh_context_cluster_open(kh_context* ctx, const Problem* P, int* resident, int* n_candidates) {
+  if (!ctx || !P) { fail(KSCHED_ERR_INVALID, "null context or problem"); return nullptr; }
+  auto lock = lock_if_default(ctx);
+  try {
+    auto* cs = new ClusterSession(P, ctx);
     if (resident) *resident = cs->resident ? 1 : 0;
     if (n_candidates) *n_candidates = (int)cs->cands.size();
     return cs;
@@ -1190,12 +1277,22 @@ ClusterSession* kh_cluster_open(const Problem* P, int* resident, int* n_candidat
     return nullptr;
   }
 }
-void kh_cluster_close(ClusterSession* cs) { delete cs; }
+
+// A consolidation pass over one cluster (ClusterSession): open once, probe many times, close. The session keeps the
+// cluster resident on the device (ksched_load_cluster); `resident` tells whether the snapshot path took it.
+ClusterSession* kh_cluster_open(const Problem* P, int* resident, int* n_candidates) { return kh_context_cluster_open(&g_default, P, resident, n_candidates); }
+void kh_cluster_close(ClusterSession* cs) {
+  if (!cs) return;
+  auto lock = lock_if_default(cs->ctx);
+  delete cs;
+}
 // computeConsolidation for n_sets candidate sets in ONE ksched_simulate_batch call. sets = positions in the disruption order,
 // set q = sets[set_off[q] .. set_off[q+1]); multi = apply the multi-node caller's filterOutSameType.
 // actions[q] = 0 / 1 / 2; options of set q are written to options[q * options_stride ...], n_options[q] of them.
 int kh_cluster_probe_sets(ClusterSession* cs, const int* sets, const int* set_off, int n_sets, int multi, int* actions, int* options, int options_stride,
                           int* n_options) {
+  if (!cs) return fail(KSCHED_ERR_INVALID, "no session");
+  auto lock = lock_if_default(cs->ctx);
   try {
     std::vector<std::vector<int>> v((size_t)n_sets);
     for (int q = 0; q < n_sets; ++q) v[(size_t)q].assign(sets + set_off[q], sets + set_off[q + 1]);
@@ -1213,6 +1310,8 @@ int kh_cluster_probe_sets(ClusterSession* cs, const int* sets, const int* set_of
 // simulateScheduling's whole result for n_sets candidate sets in ONE ksched_simulate_full call (ClusterSession::simulate).
 // set q = sets[set_off[q] .. set_off[q+1]) as Problem.nodes indices; out[q] = what kh_scheduler_solve returns for that set.
 int kh_cluster_simulate(ClusterSession* cs, const int* sets, const int* set_off, int n_sets, Result** out) {
+  if (!cs) return fail(KSCHED_ERR_INVALID, "no session");
+  auto lock = lock_if_default(cs->ctx);
   try {
     if (!cs || n_sets < 0 || (n_sets > 0 && (!set_off || !out || set_off[0] < 0))) return fail(KSCHED_ERR_INVALID, "n_sets / set_off out of range");
     std::vector<std::vector<int>> v((size_t)n_sets);
@@ -1230,6 +1329,7 @@ int kh_cluster_simulate(ClusterSession* cs, const int* sets, const int* set_off,
 }
 // disruption order of the session's candidates (Problem.nodes indices)
 int kh_cluster_candidates(const ClusterSession* cs, int* nodes, int cap) {
+  auto lock = lock_if_default(cs->ctx);
   for (size_t i = 0; i < cs->cands.size() && (int)i < cap; ++i) nodes[i] = cs->cands[i].node;
   return (int)cs->cands.size();
 }
@@ -1237,6 +1337,7 @@ int kh_cluster_candidates(const ClusterSession* cs, int* nodes, int cap) {
 // One probe of the multi-node search: computeConsolidation over the `count` cheapest-to-disrupt candidates.
 // Returns the action (0 nothing, 1 delete, 2 replace) or a negative error; options = surviving replacement types.
 int kh_consolidate_probe(const Problem* P, int count, int* options, int options_cap, int* n_options) {
+  KH_DEFAULT_LOCK;
   try {
     ClusterSession cs(P);
     if (count < 1 || count > (int)cs.cands.size()) return fail(KSCHED_ERR_INVALID, "probe size out of range");
@@ -1252,6 +1353,7 @@ int kh_consolidate_probe(const Problem* P, int count, int* options, int options_
 // MultiNodeConsolidation.firstNNodeConsolidationOption (multinodeconsolidation.go:74-114): binary search, one probe per step.
 // out ints: [action, nodes_removed, simulations, n_options]; options = instance type indices.
 int kh_consolidate(const Problem* P, int* out4, int* options, int options_cap, int* probes, int* probe_actions, int probes_cap, int* n_probes) {
+  KH_DEFAULT_LOCK;
   try {
     ClusterSession cs(P);
     const Search s = first_n_search(cs);
@@ -1273,6 +1375,7 @@ int kh_consolidate(const Problem* P, int* out4, int* options, int options_cap, i
 // validation becomes retry (out4 = [3, 0, simulations, 0]). *verdict = 1 valid, 0 invalid, -1 nothing to validate.
 int kh_consolidate_validated(const Problem* before, const Problem* after, int* out4, int* options, int options_cap, int* probes, int* probe_actions,
                              int probes_cap, int* n_probes, int* verdict) {
+  KH_DEFAULT_LOCK;
   try {
     ClusterSession cs(before);
     const Search s = first_n_search(cs);
@@ -1305,6 +1408,8 @@ int kh_consolidate_validated(const Problem* before, const Problem* after, int* o
 // different problem (Problem::id): every validation of one ComputeCommand passes the same one (DESIGN.md §6 R7).
 int kh_cluster_validate(ClusterSession* cs, const Problem* after, const int* sets, const int* set_off, int n_sets, const int* actions, const int* options,
                         int options_stride, const int* n_options, int* valid) {
+  if (!cs) return fail(KSCHED_ERR_INVALID, "no session");
+  auto lock = lock_if_default(cs->ctx);
   try {
     std::vector<VCmd> cmds;
     if (n_sets < 0 || (n_sets > 0 && set_off[0] < 0)) return fail(KSCHED_ERR_INVALID, "n_sets / set_off out of range");
@@ -1328,6 +1433,7 @@ int kh_cluster_validate(ClusterSession* cs, const Problem* after, const int* set
 
 // ncclAllGather of n ints per rank on the scheduler handle's communicator (kh_nccl_init first)
 int kh_allgather_i32(const int* send, int n, int* recv) {
+  KH_DEFAULT_LOCK;
   int rc = ensure_handle();
   if (rc != KSCHED_OK) return rc;
   rc = ksched_allgather(g_handle, send, (size_t)n * sizeof(int), recv);
@@ -1336,6 +1442,7 @@ int kh_allgather_i32(const int* send, int n, int* recv) {
 }
 // communicator for the scheduler handle without column sharding (replicas / sharded consolidation)
 int kh_nccl_init(const void* id128, int rank, int world) {
+  KH_DEFAULT_LOCK;
   int rc = ensure_handle();
   if (rc != KSCHED_OK) return rc;
   rc = ksched_nccl_init(g_handle, id128, rank, world);
@@ -1350,6 +1457,7 @@ int kh_nccl_init(const void* id128, int rank, int world) {
 // simulations, n_options]; *node = its Problem.nodes index. first / last bound the positions tried (a rank's share of the
 // sweep); last < 0 = all.
 int kh_consolidate_single(const Problem* P, int first, int last, int batch, int* out4, int* node, int* options, int options_cap) {
+  KH_DEFAULT_LOCK;
   try {
     ClusterSession cs(P);
     const Sweep s = single_sweep(cs, nullptr, first, last, batch);
@@ -1372,6 +1480,7 @@ int kh_consolidate_single(const Problem* P, int first, int last, int batch, int*
 // merge as: the first share with a winner gives the command; with none, retry when any share failed a validation.
 int kh_consolidate_single_validated(const Problem* before, const Problem* after, int first, int last, int batch, int* out4, int* node, int* options,
                                     int options_cap, int* trace, int* trace_valid, int trace_cap, int* n_trace, int* failed_validation) {
+  KH_DEFAULT_LOCK;
   try {
     ClusterSession cs(before);
     const Sweep s = single_sweep(cs, after, first, last, batch);
@@ -1395,6 +1504,7 @@ int kh_consolidate_single_validated(const Problem* before, const Problem* after,
 // ordering in run_pack(); this entry point lets the GPU tests prove it. Returns 0 when every repetition of each problem
 // reproduced that problem's first result bit for bit, a negative ksched error otherwise, or 1 on a mismatch.
 extern "C" int kh_selftest_two_handles(const Problem* A, const Problem* B, int iters) {
+  KH_DEFAULT_LOCK;
   int rc = ensure_handle();
   if (rc != KSCHED_OK) return rc;
   const Problem* probs[2] = {A, B};
@@ -1438,6 +1548,7 @@ extern "C" int kh_selftest_two_handles(const Problem* A, const Problem* B, int i
 // the same problem, e.g. the oracle's) recompute the launch choice from the ENCODED offering table exactly as the device
 // kernel does, and compare with the fields `ref` carries. Returns the number of nodes that differ, or a negative error.
 extern "C" int kh_launch_table_selfcheck(const Problem* P, const Result* ref) {
+  KH_DEFAULT_LOCK;
   try {
     auto E = khost::encode(*P, {});
     int zone_key = -1, ct_key = -1;

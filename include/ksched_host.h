@@ -67,13 +67,14 @@ int kh_result_uninitialized_existing(const kh_result* r);
 
 /* ---- the device */
 int kh_set_device(int ordinal);   /* CUDA device of this process's scheduler handle (default 0) */
-/* ---- scheduler contexts. Every kh_* function without a context argument uses one process-wide context (one device
- * handle) and takes a process-wide lock, so concurrent callers are serialized. A context made here owns a handle of its
- * own: two contexts may be used from two threads at once, without a lock between them, and their kernels run
- * concurrently on one device when their handles hold different parameter slots (ksched_create). One context is used by
- * one thread at a time. A session opened on a context lives on the context's handle (its validation snapshot on a
- * handle of its own, as always), and displaces only that context's snapshot. NULL from kh_context_create without a
- * CUDA device (KSCHED_ERR_NO_DEVICE, kh_scheduler_error()): there is no CPU path. Destroy a context after its sessions. */
+/* ---- scheduler contexts. A context owns one device handle and one lock, which every kh_* call on the context takes: one
+ * context used from two threads is serialized. Every kh_* function without a context argument runs on one process-wide
+ * context, whose handle is created at its first use. A context made here owns a handle of its own: two contexts may be
+ * used from two threads at once, without a lock between them, and their kernels run concurrently on one device when
+ * their handles hold different parameter slots (ksched_create). One context per controller thread is the recommended
+ * use. A session opened on a context lives on the context's handle (its validation snapshot on a handle of its own, as
+ * always), and displaces only that context's snapshot. NULL from kh_context_create without a CUDA device
+ * (KSCHED_ERR_NO_DEVICE, kh_scheduler_error()): there is no CPU path. Destroy a context after its sessions. */
 typedef struct kh_context kh_context;
 kh_context* kh_context_create(int device);
 void kh_context_destroy(kh_context* ctx);

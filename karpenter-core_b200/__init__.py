@@ -118,7 +118,6 @@ def lib():
     L.kh_encoded_digest.restype = C.c_ulonglong
     L.kh_encoded_digest.argtypes = [C.c_void_p]
     L.kh_launch_table_selfcheck.argtypes = [C.c_void_p, C.c_void_p]
-    L.kh_selftest_two_handles.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
     L.kh_set_device.argtypes = [C.c_int]
     L.kh_set_count_visited.argtypes = [C.c_int]
     L.kh_handle.restype = C.c_void_p

@@ -15,7 +15,6 @@
 #include <mutex>
 #include <set>
 #include <string>
-#include <thread>
 #include <unordered_map>
 #include <vector>
 
@@ -28,53 +27,31 @@
 using namespace kmodel;
 using khost::Encoded;
 
-// A scheduler context: one device handle and the session-displacement bookkeeping of the snapshot it holds. The kh_*
-// functions without a context argument share one process-wide context (g_default); kh_context_create makes others.
+// A scheduler context: one device handle, the lock every kh_* call on it takes, and the record of what the handle holds.
+// The kh_* functions without a context argument share one process-wide context (g_default); kh_context_create makes others.
 struct kh_context {
   ksched_handle* h = nullptr;
   int device = 0;
-  // h holds one cluster snapshot at a time: the id of the ClusterSession whose snapshot it holds, 0 when anything else
-  // (a Solve, a fresh-encode simulation, ResidentSolve, another session) has been loaded onto it since
-  uint64_t resident_session = 0;
+  // recursive: kh_gpu_run reloads the ResidentSolve encoding through kh_gpu_load
+  std::recursive_mutex mu;
+  // h holds one problem at a time: the id of the ClusterSession whose snapshot it holds or of the ResidentSolve encoding
+  // (process-wide context only), 0 when anything else (a Solve, a fresh-encode simulation) has been loaded onto it since
+  uint64_t resident = 0;
 };
 
+int ksched_k1_plan(const ksched_handle* h, int out[5]);  // csrc/ksched.cu, outside the C-ABI
+
 namespace {
 
+using Lock = std::lock_guard<std::recursive_mutex>;
 thread_local std::string g_err;
 kh_context g_default;
-ksched_handle*& g_handle = g_default.h;
-int& g_device = g_default.device;
-uint64_t& g_resident_session = g_default.resident_session;
-std::atomic<uint64_t> g_last_session{0};
-// Serializes the kh_* functions that use the process-wide context, so that threads calling them do not race on g_handle.
-// Contexts of their own take no lock: each is used by one thread at a time.
-std::recursive_mutex g_default_mu;
-#define KH_DEFAULT_LOCK std::lock_guard<std::recursive_mutex> default_lock(g_default_mu)
-// the same lock for work on ctx, taken only when ctx is the process-wide context
-std::unique_lock<std::recursive_mutex> lock_if_default(const kh_context* ctx) {
-  return ctx == &g_default ? std::unique_lock<std::recursive_mutex>(g_default_mu) : std::unique_lock<std::recursive_mutex>();
-}
-// The same for ResidentSolve (kh_gpu_*): the encoding kh_gpu_load / kh_gpu_solve_e2e last put on g_handle, and whether
-// g_handle still holds it. kh_gpu_run loads it again when something else took the handle since.
+std::atomic<uint64_t> g_last_session{0};  // ids of ClusterSessions and ResidentSolve loads, never 0
+// ResidentSolve (kh_gpu_*): the encoding kh_gpu_load / kh_gpu_solve_e2e last put on the process-wide handle, and its id
+// there. kh_gpu_run loads it again when something else took the handle since.
 const Encoded* g_gpu_encoded = nullptr;
-bool g_gpu_current = false;
-
-// something other than the recorded session / ResidentSolve encoding is about to be loaded onto g_handle
-void handle_taken() {
-  g_resident_session = 0;
-  g_gpu_current = false;
-}
-// the same for any context
-void context_taken(kh_context* ctx) {
-  if (ctx == &g_default) handle_taken();
-  else ctx->resident_session = 0;
-}
-}  // namespace
-
-int ksched_k1_plan(const ksched_handle* h, int out[5]);  // csrc/ksched.cu, outside the C-ABI
-extern "C" int kh_context_solve(kh_context* ctx, const Problem* P, const int* candidates, int ncand, Result* out);
-
-namespace {
+uint64_t g_gpu_id = 0;
+bool gpu_current() { return g_gpu_encoded && g_default.resident == g_gpu_id; }
 // exact nodes_visited statistic (opt-in: tests); switches the pack kernel's steady-state paths off. Per calling thread, so that
 // one controller's setting never reaches another context's Solves and simulations.
 thread_local int g_count_visited = 0;
@@ -83,17 +60,12 @@ int fail(int code, const std::string& msg) {
   g_err = msg;
   return code;
 }
-int ensure_handle() {
-  if (g_handle) return KSCHED_OK;
-  int rc = ksched_create(g_device, &g_handle);
-  if (rc != KSCHED_OK) return fail(rc, "ksched_create failed: no usable CUDA device (the product has no CPU path)");
-  return KSCHED_OK;
-}
-// ctx's handle, created on first use for the process-wide context
-ksched_handle* context_handle(kh_context* ctx) {
-  if (ctx != &g_default) return ctx->h;
-  if (ensure_handle() != KSCHED_OK) throw std::runtime_error(g_err);
-  return g_handle;
+// ctx->h, created on first use: kh_context_create creates its contexts' handles at once, the process-wide one is created by
+// the first call that needs it
+int open_handle(kh_context* ctx) {
+  if (ctx->h) return KSCHED_OK;
+  int rc = ksched_create(ctx->device, &ctx->h);
+  return rc == KSCHED_OK ? rc : fail(rc, "ksched_create failed: no usable CUDA device (the product has no CPU path)");
 }
 
 struct ResultBuffers {
@@ -264,22 +236,54 @@ int error_code(const std::exception& e) {
   return m.rfind("unsupported:", 0) == 0 ? KSCHED_ERR_UNSUPPORTED : KSCHED_ERR_INVALID;
 }
 
-// One ksched_solve of E on h, or without h on ctx's handle, whose cluster snapshot this displaces.
-int solve_encoded(Encoded& E, ResultBuffers& B, bool want_feasibility, ksched_handle* h = nullptr, kh_context* ctx = &g_default) {
-  if (!h) {
-    if (ctx == &g_default) {
-      int rc = ensure_handle();
-      if (rc != KSCHED_OK) return rc;
-    }
-    h = ctx->h;
-  }
-  if (h == ctx->h) context_taken(ctx);
+using clk = std::chrono::steady_clock;
+
+// One ksched_solve of E on h: its catalog (*catalog_loaded = when that is done), then the Solve into B
+int solve_on(ksched_handle* h, Encoded& E, ResultBuffers& B, clk::time_point* catalog_loaded = nullptr) {
   int rc = ksched_load_catalog(h, &E.catalog);
   if (rc != KSCHED_OK) return fail(rc, ksched_last_error(h));
-  B.prepare(E, want_feasibility);
+  if (catalog_loaded) *catalog_loaded = clk::now();
+  B.prepare(E, false);
   rc = ksched_solve(h, &E.problem, &B.r);
-  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(h));
-  return KSCHED_OK;
+  return rc == KSCHED_OK ? rc : fail(rc, ksched_last_error(h));
+}
+// the same on ctx's handle, displacing whatever it holds
+int solve_on(kh_context* ctx, Encoded& E, ResultBuffers& B, clk::time_point* catalog_loaded = nullptr) {
+  int rc = open_handle(ctx);
+  if (rc != KSCHED_OK) return rc;
+  ctx->resident = 0;
+  return solve_on(ctx->h, E, B, catalog_loaded);
+}
+
+// Scheduler.Solve through the C-ABI with host buffers (upload + kernels + download inside the call) on ctx. phases_us
+// (optional) = [encode, catalog, solve, decode, total]: encode = NewScheduler's marshalling (string-level model -> flat
+// structs); catalog = ksched_load_catalog (a no-op when the byte-identical catalog is already resident); solve = ksched_solve
+// (upload + kernels + download); decode = the ([]*Node, []*ExistingNode) shape and simulateScheduling's verdicts.
+int context_solve(kh_context* ctx, const Problem* P, const int* candidates, int ncand, Result* out, double* phases_us) {
+  if (!ctx || !P || !out || ncand < 0 || (ncand > 0 && !candidates)) return fail(KSCHED_ERR_INVALID, "null context, problem or result");
+  Lock lock(ctx->mu);
+  *out = Result();
+  try {
+    auto us = [](clk::time_point a, clk::time_point b) { return std::chrono::duration<double, std::micro>(b - a).count(); };
+    const auto t0 = clk::now();
+    std::vector<int> c(candidates, candidates + ncand);
+    auto E = khost::encode(*P, c);
+    E->problem.count_nodes_visited = g_count_visited;
+    const auto t1 = clk::now();
+    clk::time_point t2;
+    static thread_local ResultBuffers B;
+    int rc = solve_on(ctx, *E, B, &t2);
+    if (rc != KSCHED_OK) { out->error = g_err; return rc; }
+    const auto t3 = clk::now();
+    decode(*E, B, *out);
+    set_verdicts(*E, B, *out);
+    const auto t4 = clk::now();
+    if (phases_us) { phases_us[0] = us(t0, t1); phases_us[1] = us(t1, t2); phases_us[2] = us(t2, t3); phases_us[3] = us(t3, t4); phases_us[4] = us(t0, t4); }
+    return KSCHED_OK;
+  } catch (const std::exception& e) {
+    out->error = e.what();
+    return fail(error_code(e), e.what());
+  }
 }
 
 // ---- consolidation price helpers (deprovisioning/helpers.go:148-157,292-315) on the decoded new node
@@ -323,58 +327,25 @@ extern "C" {
 
 const char* kh_scheduler_error() { return g_err.c_str(); }
 int kh_set_device(int ordinal) {
-  KH_DEFAULT_LOCK;
-  if (g_handle) { ksched_destroy(g_handle); g_handle = nullptr; }
-  handle_taken();
+  Lock lock(g_default.mu);
+  if (g_default.h) { ksched_destroy(g_default.h); g_default.h = nullptr; }
+  g_default.resident = 0;
   g_gpu_encoded = nullptr;
-  g_device = ordinal;
+  g_default.device = ordinal;
   return KSCHED_OK;
 }
 void kh_set_count_visited(int on) { g_count_visited = on; }
 ksched_handle* kh_handle() {
-  KH_DEFAULT_LOCK;
-  return ensure_handle() == KSCHED_OK ? g_handle : nullptr;
+  Lock lock(g_default.mu);
+  return open_handle(&g_default) == KSCHED_OK ? g_default.h : nullptr;
 }
 
-// Scheduler.Solve through the C-ABI with host buffers (upload + kernels + download inside the call).
 int kh_scheduler_solve(const Problem* P, const int* candidates, int ncand, Result* out) {
-  return kh_context_solve(&g_default, P, candidates, ncand, out);
+  return context_solve(&g_default, P, candidates, ncand, out, nullptr);
 }
-
-// The same call with its host phases timed (bench.py's end-to-end leg): phases_us = [encode, catalog, solve, decode, total].
-// encode = NewScheduler's marshalling (string-level model -> flat structs); catalog = ksched_load_catalog (a no-op when the
-// byte-identical catalog is already resident); solve = ksched_solve (upload + kernels + download); decode = the
-// ([]*Node, []*ExistingNode) shape.
+// the same call with its host phases timed (bench.py's end-to-end leg)
 int kh_scheduler_solve_timed(const Problem* P, const int* candidates, int ncand, Result* out, double* phases_us) {
-  KH_DEFAULT_LOCK;
-  *out = Result();
-  try {
-    using clk = std::chrono::steady_clock;
-    auto us = [](clk::time_point a, clk::time_point b) { return std::chrono::duration<double, std::micro>(b - a).count(); };
-    const auto t0 = clk::now();
-    std::vector<int> c(candidates, candidates + ncand);
-    auto E = khost::encode(*P, c);
-    E->problem.count_nodes_visited = g_count_visited;
-    const auto t1 = clk::now();
-    int rc = ensure_handle();
-    if (rc != KSCHED_OK) return rc;
-    handle_taken();
-    rc = ksched_load_catalog(g_handle, &E->catalog);
-    if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
-    const auto t2 = clk::now();
-    static thread_local ResultBuffers B;
-    B.prepare(*E, false);
-    rc = ksched_solve(g_handle, &E->problem, &B.r);
-    if (rc != KSCHED_OK) { out->error = ksched_last_error(g_handle); return fail(rc, out->error); }
-    const auto t3 = clk::now();
-    decode(*E, B, *out);
-    const auto t4 = clk::now();
-    if (phases_us) { phases_us[0] = us(t0, t1); phases_us[1] = us(t1, t2); phases_us[2] = us(t2, t3); phases_us[3] = us(t3, t4); phases_us[4] = us(t0, t4); }
-    return KSCHED_OK;
-  } catch (const std::exception& e) {
-    out->error = e.what();
-    return fail(error_code(e), e.what());
-  }
+  return context_solve(&g_default, P, candidates, ncand, out, phases_us);
 }
 
 // ---- split API for benchmarking / kernel tests: encode once, keep the problem resident, time kernels only
@@ -398,8 +369,8 @@ Encoded* kh_encode_cluster(const Problem* P, const int* candidates, int ncand) {
   }
 }
 void kh_encoded_free(Encoded* E) {
-  KH_DEFAULT_LOCK;
-  if (E == g_gpu_encoded) { g_gpu_encoded = nullptr; g_gpu_current = false; }
+  Lock lock(g_default.mu);
+  if (E == g_gpu_encoded) g_gpu_encoded = nullptr;
   delete E;
 }
 // dims: [pods, classes, existing, groups, types, templates, keys, resources, type_words, class_topo, taintsets, resources_ext,
@@ -500,55 +471,56 @@ void kh_encoded_set_count_visited(Encoded* E, int on) { E->problem.count_nodes_v
 const ksched_catalog* kh_encoded_catalog(const Encoded* E) { return &E->catalog; }
 const ksched_problem* kh_encoded_problem(const Encoded* E) { return &E->problem; }
 int kh_gpu_load(Encoded* E) {
-  KH_DEFAULT_LOCK;
-  int rc = ensure_handle();
+  Lock lock(g_default.mu);
+  int rc = open_handle(&g_default);
   if (rc != KSCHED_OK) return rc;
-  handle_taken();
+  g_default.resident = 0;
   g_gpu_encoded = nullptr;
-  rc = ksched_load_catalog(g_handle, &E->catalog);
-  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
-  rc = ksched_upload(g_handle, &E->problem);
-  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
+  rc = ksched_load_catalog(g_default.h, &E->catalog);
+  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_default.h));
+  rc = ksched_upload(g_default.h, &E->problem);
+  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_default.h));
   g_gpu_encoded = E;
-  g_gpu_current = true;
+  g_default.resident = g_gpu_id = ++g_last_session;
   return KSCHED_OK;
 }
-// the ResidentSolve encoding back on g_handle when a session, a Solve or a fresh-encode simulation took it since its load
+// the ResidentSolve encoding back on the process-wide handle when a session, a Solve or a fresh-encode simulation took it
+// since its load. Without one, a run works on whatever the handle holds and displaces a session's snapshot.
 int gpu_make_current() {
-  if (!g_gpu_encoded || g_gpu_current) return KSCHED_OK;
-  return kh_gpu_load(const_cast<Encoded*>(g_gpu_encoded));
+  if (gpu_current()) return KSCHED_OK;
+  if (g_gpu_encoded) return kh_gpu_load(const_cast<Encoded*>(g_gpu_encoded));
+  g_default.resident = 0;
+  return KSCHED_OK;
 }
 int kh_gpu_run(int flush_l2) {
-  KH_DEFAULT_LOCK;
-  if (!g_handle) return fail(KSCHED_ERR_INVALID, "no handle");
+  Lock lock(g_default.mu);
+  if (!g_default.h) return fail(KSCHED_ERR_INVALID, "no handle");
   int rc = gpu_make_current();
   if (rc != KSCHED_OK) return rc;
-  g_resident_session = 0;
-  rc = ksched_run_resident(g_handle, flush_l2);
-  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
+  rc = ksched_run_resident(g_default.h, flush_l2);
+  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_default.h));
   return rc;
 }
 int kh_gpu_run_feasibility(int flush_l2, float* us) {
-  KH_DEFAULT_LOCK;
-  if (!g_handle) return fail(KSCHED_ERR_INVALID, "no handle");
+  Lock lock(g_default.mu);
+  if (!g_default.h) return fail(KSCHED_ERR_INVALID, "no handle");
   int rc = gpu_make_current();
   if (rc != KSCHED_OK) return rc;
-  g_resident_session = 0;
-  rc = ksched_run_feasibility_only(g_handle, flush_l2, us);
-  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
+  rc = ksched_run_feasibility_only(g_default.h, flush_l2, us);
+  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_default.h));
   return rc;
 }
 // download + decode; feasibility_out (optional) receives [pods][templates][type_words] uint64 in caller pod order,
 // columns in the caller's instance-type order (bit i of template v = instance_types[i])
 int kh_gpu_download(Encoded* E, Result* out, unsigned long long* feasibility_out, unsigned long long* best_out) {
-  KH_DEFAULT_LOCK;
-  if (!g_handle) return fail(KSCHED_ERR_INVALID, "no handle");
+  Lock lock(g_default.mu);
+  if (!g_default.h) return fail(KSCHED_ERR_INVALID, "no handle");
   *out = Result();
-  if (g_gpu_encoded && !g_gpu_current) return fail(KSCHED_ERR_INVALID, "the handle was used for other work since this problem's run: run it again");
+  if (g_gpu_encoded && !gpu_current()) return fail(KSCHED_ERR_INVALID, "the handle was used for other work since this problem's run: run it again");
   ResultBuffers B;
   B.prepare(*E, feasibility_out != nullptr || best_out != nullptr);
-  int rc = ksched_download(g_handle, &E->problem, &B.r);
-  if (rc != KSCHED_OK) { out->error = ksched_last_error(g_handle); return fail(rc, out->error); }
+  int rc = ksched_download(g_default.h, &E->problem, &B.r);
+  if (rc != KSCHED_OK) { out->error = ksched_last_error(g_default.h); return fail(rc, out->error); }
   decode(*E, B, *out);
   if (feasibility_out) {
     const size_t P = E->pods.size(), V = E->templates.size(), W = (size_t)E->type_words, T = E->types.size();
@@ -567,44 +539,44 @@ int kh_gpu_download(Encoded* E, Result* out, unsigned long long* feasibility_out
 // One Scheduler.Solve through the C-ABI with HOST buffers: pod/node/topology upload, kernels and result download are
 // all inside the call (the catalog stays resident, as it would across reconciles). Returns wall-clock microseconds.
 int kh_gpu_solve_e2e(Encoded* E, Result* out, double* wall_us) {
-  KH_DEFAULT_LOCK;
-  if (!g_handle) return fail(KSCHED_ERR_INVALID, "no handle");
-  handle_taken();
+  Lock lock(g_default.mu);
+  if (!g_default.h) return fail(KSCHED_ERR_INVALID, "no handle");
+  g_default.resident = 0;
   g_gpu_encoded = nullptr;
   ResultBuffers B;
   B.prepare(*E, false);
   auto t0 = std::chrono::steady_clock::now();
-  int rc = ksched_solve(g_handle, &E->problem, &B.r);
+  int rc = ksched_solve(g_default.h, &E->problem, &B.r);
   auto t1 = std::chrono::steady_clock::now();
   if (wall_us) *wall_us = std::chrono::duration<double, std::micro>(t1 - t0).count();
-  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
+  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_default.h));
   g_gpu_encoded = E;
-  g_gpu_current = true;
+  g_default.resident = g_gpu_id = ++g_last_session;
   if (out) { *out = Result(); decode(*E, B, *out); }
   return KSCHED_OK;
 }
 int kh_gpu_load_catalog(Encoded* E) {
-  KH_DEFAULT_LOCK;
-  int rc = ensure_handle();
+  Lock lock(g_default.mu);
+  int rc = open_handle(&g_default);
   if (rc != KSCHED_OK) return rc;
-  g_resident_session = 0;
-  rc = ksched_load_catalog(g_handle, &E->catalog);
-  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
+  if (!gpu_current()) g_default.resident = 0;  // a session loads its snapshot again after this; a current ResidentSolve stays current
+  rc = ksched_load_catalog(g_default.h, &E->catalog);
+  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_default.h));
   return KSCHED_OK;
 }
 int kh_gpu_timings(ksched_timings* t) {
-  KH_DEFAULT_LOCK;
-  return g_handle ? ksched_get_timings(g_handle, t) : KSCHED_ERR_INVALID;
+  Lock lock(g_default.mu);
+  return g_default.h ? ksched_get_timings(g_default.h, t) : KSCHED_ERR_INVALID;
 }
 int kh_gpu_k1_plan(int* out) {
-  KH_DEFAULT_LOCK;
-  return g_handle ? ksched_k1_plan(g_handle, out) : fail(KSCHED_ERR_INVALID, "no handle");
+  Lock lock(g_default.mu);
+  return g_default.h ? ksched_k1_plan(g_default.h, out) : fail(KSCHED_ERR_INVALID, "no handle");
 }
 int kh_gpu_set_shard(int rank, int world) {
-  KH_DEFAULT_LOCK;
-  int rc = ensure_handle();
+  Lock lock(g_default.mu);
+  int rc = open_handle(&g_default);
   if (rc != KSCHED_OK) return rc;
-  rc = ksched_set_shard(g_handle, rank, world);
+  rc = ksched_set_shard(g_default.h, rank, world);
   return rc == KSCHED_OK ? rc : fail(rc, "ksched_set_shard: invalid rank / world");
 }
 
@@ -646,7 +618,8 @@ void rank_on_device(const Problem* P, std::vector<int>* order, std::vector<doubl
   order->clear();
   cost->clear();
   if (N == 0) return;
-  ksched_handle* h = context_handle(ctx);
+  if (open_handle(ctx) != KSCHED_OK) throw std::runtime_error(g_err);
+  ksched_handle* h = ctx->h;
   std::vector<uint8_t> eligible(N, 0), flags;
   std::vector<int32_t> off(N + 1, 0), prio;
   std::vector<double> dc, age(N, 0.0), ttl(N, -1.0), given(N, 0.0);
@@ -793,8 +766,7 @@ Cmd compute_consolidation_encoded(const Problem* P, const std::vector<Cand>& sel
   auto E = khost::encode(*P, nodes);
   E->problem.count_nodes_visited = g_count_visited;
   ResultBuffers B;
-  int rc = solve_encoded(*E, B, false, nullptr, ctx);
-  if (rc != KSCHED_OK) throw std::runtime_error(g_err);
+  if (solve_on(ctx, *E, B) != KSCHED_OK) throw std::runtime_error(g_err);
   size_t scheduled = 0;
   for (auto a : B.assign) if (a >= 0) ++scheduled;
   // helpers.go:109-113 walks EVERY ExistingNode Solve returns (all owned nodes that are neither candidates nor marked for
@@ -967,7 +939,7 @@ struct ValidationSnapshot {
       auto F = khost::encode(*A, mapped[j]);
       F->problem.count_nodes_visited = 0;
       ResultBuffers B;
-      if (solve_encoded(*F, B, false, h.get()) != KSCHED_OK) throw std::runtime_error(g_err);
+      if (solve_on(h.get(), *F, B) != KSCHED_OK) throw std::runtime_error(g_err);
       bool init = true;
       for (size_t e = 0; e < F->existing.size(); ++e) init = init && F->existing_initialized[e];
       size_t scheduled = 0;
@@ -982,7 +954,7 @@ struct ValidationSnapshot {
 // (ksched_load_cluster), every computeConsolidation a ksched_simulate_batch entry. Clusters the snapshot cannot hold
 // (topology groups) are simulated one freshly encoded ksched_solve at a time - still on the GPU, never on the CPU.
 // Sessions share their context's handle: a session whose snapshot something else displaced loads it again before its next
-// batch (kh_context::resident_session).
+// batch (kh_context::resident).
 struct ClusterSession {
   kh_context* ctx = &g_default;
   const Problem* P = nullptr;
@@ -995,12 +967,13 @@ struct ClusterSession {
   std::unique_ptr<ValidationSnapshot> validation_snapshot;  // opened at the first command that needs validation
 
   explicit ClusterSession(const Problem* p, kh_context* c = &g_default) : ctx(c), P(p), cands(sorted_candidates(p, c)) {
-    ksched_handle* h = context_handle(ctx);
+    if (open_handle(ctx) != KSCHED_OK) throw std::runtime_error(g_err);
+    ksched_handle* h = ctx->h;
     std::vector<int> nodes;
     for (auto& c : cands) nodes.push_back(c.node);
     auto sup = khost::encode(*P, nodes, true);
     sup->problem.count_nodes_visited = 0;
-    context_taken(ctx);
+    ctx->resident = 0;
     int rc = load_snapshot(h, *sup, nodes);
     if (rc == KSCHED_ERR_UNSUPPORTED) return;  // resident stays false
     if (rc != KSCHED_OK) throw std::runtime_error(ksched_last_error(h));
@@ -1008,8 +981,7 @@ struct ClusterSession {
     slot_of_node.assign(P->nodes.size(), -1);
     for (size_t e = 0; e < E->existing_state_index.size(); ++e) slot_of_node[(size_t)E->existing_state_index[e]] = (int)e;
     resident = true;
-    id = ++g_last_session;
-    ctx->resident_session = id;
+    ctx->resident = id = ++g_last_session;
   }
 
   // computeConsolidation for every set (positions in the disruption order), one ksched_simulate_batch call
@@ -1044,13 +1016,13 @@ struct ClusterSession {
   // the session's snapshot on its context's handle again when something else displaced it: the time of one reload, the same
   // answers
   void make_current() {
-    if (ctx->resident_session == id) return;
-    ksched_handle* h = context_handle(ctx);
-    context_taken(ctx);
+    if (ctx->resident == id) return;
+    if (open_handle(ctx) != KSCHED_OK) throw std::runtime_error(g_err);
+    ctx->resident = 0;
     std::vector<int> nodes;
     for (auto& c : cands) nodes.push_back(c.node);
-    if (load_snapshot(h, *E, nodes) != KSCHED_OK) throw std::runtime_error(ksched_last_error(h));
-    ctx->resident_session = id;
+    if (load_snapshot(ctx->h, *E, nodes) != KSCHED_OK) throw std::runtime_error(ksched_last_error(ctx->h));
+    ctx->resident = id;
   }
 
   // simulateScheduling's whole result for every set (Problem.nodes indices, candidates of the session, in the caller's
@@ -1072,7 +1044,7 @@ struct ClusterSession {
         auto F = khost::encode(*P, sets[q]);
         F->problem.count_nodes_visited = g_count_visited;
         ResultBuffers B;
-        if (solve_encoded(*F, B, false, nullptr, ctx) != KSCHED_OK) throw std::runtime_error(g_err);
+        if (solve_on(ctx, *F, B) != KSCHED_OK) throw std::runtime_error(g_err);
         decode(*F, B, out[q]);
         set_verdicts(*F, B, out[q]);
       }
@@ -1204,12 +1176,12 @@ Sweep single_sweep(ClusterSession& cs, const Problem* after, int first, int last
 extern "C" {
 // number of consolidation candidates
 int kh_consolidate_candidates(const Problem* P) {
-  KH_DEFAULT_LOCK;
+  Lock lock(g_default.mu);
   try { return (int)sorted_candidates(P).size(); } catch (const std::exception& e) { return fail(error_code(e), e.what()); }
 }
 // candidate ranking on the device: order = Problem.nodes indices by disruption cost, cost parallel; returns their number
 int kh_rank_candidates(const Problem* P, int* order, double* cost, int cap) {
-  KH_DEFAULT_LOCK;
+  Lock lock(g_default.mu);
   try {
     std::vector<int> o;
     std::vector<double> c;
@@ -1221,14 +1193,12 @@ int kh_rank_candidates(const Problem* P, int* order, double* cost, int cap) {
   }
 }
 
-// ---- scheduler contexts: a handle of their own on `device`, with the session bookkeeping g_default keeps for the others
+// ---- scheduler contexts: a handle of their own on `device`, created at once, and a lock and residency record like g_default's
 kh_context* kh_context_create(int device) {
   auto* ctx = new kh_context();
   ctx->device = device;
-  int rc = ksched_create(device, &ctx->h);
-  if (rc != KSCHED_OK) {
+  if (open_handle(ctx) != KSCHED_OK) {
     delete ctx;
-    fail(rc, "ksched_create failed: no usable CUDA device (the product has no CPU path)");
     return nullptr;
   }
   return ctx;
@@ -1240,33 +1210,17 @@ void kh_context_destroy(kh_context* ctx) {
 }
 // Scheduler.Solve on ctx's handle (kh_scheduler_solve on the process-wide one)
 int kh_context_solve(kh_context* ctx, const Problem* P, const int* candidates, int ncand, Result* out) {
-  if (!ctx || !P || !out || ncand < 0 || (ncand > 0 && !candidates)) return fail(KSCHED_ERR_INVALID, "null context, problem or result");
-  auto lock = lock_if_default(ctx);
-  *out = Result();
-  try {
-    std::vector<int> c(candidates, candidates + ncand);
-    auto E = khost::encode(*P, c);
-    E->problem.count_nodes_visited = g_count_visited;
-    static thread_local ResultBuffers B;
-    int rc = solve_encoded(*E, B, false, nullptr, ctx);
-    if (rc != KSCHED_OK) { out->error = g_err; return rc; }
-    decode(*E, B, *out);
-    set_verdicts(*E, B, *out);
-    return KSCHED_OK;
-  } catch (const std::exception& e) {
-    out->error = e.what();
-    return fail(error_code(e), e.what());
-  }
+  return context_solve(ctx, P, candidates, ncand, out, nullptr);
 }
 // ksched_get_timings of ctx's handle
 int kh_context_timings(kh_context* ctx, ksched_timings* t) {
   if (!ctx || !t) return fail(KSCHED_ERR_INVALID, "null context or timings");
-  auto lock = lock_if_default(ctx);
+  Lock lock(ctx->mu);
   return ctx->h ? ksched_get_timings(ctx->h, t) : fail(KSCHED_ERR_INVALID, "no handle");
 }
 ClusterSession* kh_context_cluster_open(kh_context* ctx, const Problem* P, int* resident, int* n_candidates) {
   if (!ctx || !P) { fail(KSCHED_ERR_INVALID, "null context or problem"); return nullptr; }
-  auto lock = lock_if_default(ctx);
+  Lock lock(ctx->mu);
   try {
     auto* cs = new ClusterSession(P, ctx);
     if (resident) *resident = cs->resident ? 1 : 0;
@@ -1283,7 +1237,7 @@ ClusterSession* kh_context_cluster_open(kh_context* ctx, const Problem* P, int* 
 ClusterSession* kh_cluster_open(const Problem* P, int* resident, int* n_candidates) { return kh_context_cluster_open(&g_default, P, resident, n_candidates); }
 void kh_cluster_close(ClusterSession* cs) {
   if (!cs) return;
-  auto lock = lock_if_default(cs->ctx);
+  Lock lock(cs->ctx->mu);
   delete cs;
 }
 // computeConsolidation for n_sets candidate sets in ONE ksched_simulate_batch call. sets = positions in the disruption order,
@@ -1292,7 +1246,7 @@ void kh_cluster_close(ClusterSession* cs) {
 int kh_cluster_probe_sets(ClusterSession* cs, const int* sets, const int* set_off, int n_sets, int multi, int* actions, int* options, int options_stride,
                           int* n_options) {
   if (!cs) return fail(KSCHED_ERR_INVALID, "no session");
-  auto lock = lock_if_default(cs->ctx);
+  Lock lock(cs->ctx->mu);
   try {
     std::vector<std::vector<int>> v((size_t)n_sets);
     for (int q = 0; q < n_sets; ++q) v[(size_t)q].assign(sets + set_off[q], sets + set_off[q + 1]);
@@ -1311,9 +1265,9 @@ int kh_cluster_probe_sets(ClusterSession* cs, const int* sets, const int* set_of
 // set q = sets[set_off[q] .. set_off[q+1]) as Problem.nodes indices; out[q] = what kh_scheduler_solve returns for that set.
 int kh_cluster_simulate(ClusterSession* cs, const int* sets, const int* set_off, int n_sets, Result** out) {
   if (!cs) return fail(KSCHED_ERR_INVALID, "no session");
-  auto lock = lock_if_default(cs->ctx);
+  Lock lock(cs->ctx->mu);
   try {
-    if (!cs || n_sets < 0 || (n_sets > 0 && (!set_off || !out || set_off[0] < 0))) return fail(KSCHED_ERR_INVALID, "n_sets / set_off out of range");
+    if (n_sets < 0 || (n_sets > 0 && (!set_off || !out || set_off[0] < 0))) return fail(KSCHED_ERR_INVALID, "n_sets / set_off out of range");
     std::vector<std::vector<int>> v((size_t)n_sets);
     for (int q = 0; q < n_sets; ++q) {
       if (set_off[q + 1] < set_off[q]) return fail(KSCHED_ERR_INVALID, "set_off must be non-decreasing");
@@ -1329,7 +1283,8 @@ int kh_cluster_simulate(ClusterSession* cs, const int* sets, const int* set_off,
 }
 // disruption order of the session's candidates (Problem.nodes indices)
 int kh_cluster_candidates(const ClusterSession* cs, int* nodes, int cap) {
-  auto lock = lock_if_default(cs->ctx);
+  if (!cs) return fail(KSCHED_ERR_INVALID, "no session");
+  Lock lock(cs->ctx->mu);
   for (size_t i = 0; i < cs->cands.size() && (int)i < cap; ++i) nodes[i] = cs->cands[i].node;
   return (int)cs->cands.size();
 }
@@ -1337,7 +1292,7 @@ int kh_cluster_candidates(const ClusterSession* cs, int* nodes, int cap) {
 // One probe of the multi-node search: computeConsolidation over the `count` cheapest-to-disrupt candidates.
 // Returns the action (0 nothing, 1 delete, 2 replace) or a negative error; options = surviving replacement types.
 int kh_consolidate_probe(const Problem* P, int count, int* options, int options_cap, int* n_options) {
-  KH_DEFAULT_LOCK;
+  Lock lock(g_default.mu);
   try {
     ClusterSession cs(P);
     if (count < 1 || count > (int)cs.cands.size()) return fail(KSCHED_ERR_INVALID, "probe size out of range");
@@ -1350,32 +1305,13 @@ int kh_consolidate_probe(const Problem* P, int count, int* options, int options_
   }
 }
 
-// MultiNodeConsolidation.firstNNodeConsolidationOption (multinodeconsolidation.go:74-114): binary search, one probe per step.
-// out ints: [action, nodes_removed, simulations, n_options]; options = instance type indices.
-int kh_consolidate(const Problem* P, int* out4, int* options, int options_cap, int* probes, int* probe_actions, int probes_cap, int* n_probes) {
-  KH_DEFAULT_LOCK;
-  try {
-    ClusterSession cs(P);
-    const Search s = first_n_search(cs);
-    *n_probes = (int)s.probes.size();
-    for (int i = 0; i < *n_probes && i < probes_cap; ++i) { probes[i] = s.probes[(size_t)i]; probe_actions[i] = s.actions[(size_t)i]; }
-    out4[0] = s.cmd.action;
-    out4[1] = s.count;
-    out4[2] = s.sims;
-    out4[3] = (int)s.cmd.options.size();
-    for (size_t i = 0; i < s.cmd.options.size() && (int)i < options_cap; ++i) options[i] = s.cmd.options[i];
-    return KSCHED_OK;
-  } catch (const std::exception& e) {
-    return fail(error_code(e), e.what());
-  }
-}
-
 // MultiNodeConsolidation.ComputeCommand (multinodeconsolidation.go:41-70): the search on `before`, then Validation.IsValid of
 // its command against `after`, the cluster when the TTL ends. out4 and the probes as kh_consolidate; a command that fails
-// validation becomes retry (out4 = [3, 0, simulations, 0]). *verdict = 1 valid, 0 invalid, -1 nothing to validate.
+// validation becomes retry (out4 = [3, 0, simulations, 0]). *verdict = 1 valid, 0 invalid, -1 nothing to validate (also
+// without `after`, which is kh_consolidate).
 int kh_consolidate_validated(const Problem* before, const Problem* after, int* out4, int* options, int options_cap, int* probes, int* probe_actions,
                              int probes_cap, int* n_probes, int* verdict) {
-  KH_DEFAULT_LOCK;
+  Lock lock(g_default.mu);
   try {
     ClusterSession cs(before);
     const Search s = first_n_search(cs);
@@ -1384,7 +1320,7 @@ int kh_consolidate_validated(const Problem* before, const Problem* after, int* o
     Cmd cmd = s.cmd;
     int removed = s.count;
     *verdict = -1;
-    if (cmd.action == 1 || cmd.action == 2) {
+    if (after && (cmd.action == 1 || cmd.action == 2)) {
       std::vector<int> positions;
       for (int i = 0; i < s.count; ++i) positions.push_back(i);
       *verdict = cs.validate(after, {cs.command(positions, cmd.action, cmd.options)})[0] ? 1 : 0;
@@ -1401,6 +1337,13 @@ int kh_consolidate_validated(const Problem* before, const Problem* after, int* o
   }
 }
 
+// MultiNodeConsolidation.firstNNodeConsolidationOption (multinodeconsolidation.go:74-114): binary search, one probe per step.
+// out ints: [action, nodes_removed, simulations, n_options]; options = instance type indices.
+int kh_consolidate(const Problem* P, int* out4, int* options, int options_cap, int* probes, int* probe_actions, int probes_cap, int* n_probes) {
+  int verdict;
+  return kh_consolidate_validated(P, nullptr, out4, options, options_cap, probes, probe_actions, probes_cap, n_probes, &verdict);
+}
+
 // Validation.IsValid (validation.go:63-172) of n_sets commands of an open session against `after`, the cluster when the TTL
 // ends: command q removes the candidates at positions sets[set_off[q] .. set_off[q+1]) of the session's disruption order,
 // actions[q] is 1 (delete) or 2 (replace) and its options are options[q * options_stride ...], n_options[q] of them - what
@@ -1409,7 +1352,7 @@ int kh_consolidate_validated(const Problem* before, const Problem* after, int* o
 int kh_cluster_validate(ClusterSession* cs, const Problem* after, const int* sets, const int* set_off, int n_sets, const int* actions, const int* options,
                         int options_stride, const int* n_options, int* valid) {
   if (!cs) return fail(KSCHED_ERR_INVALID, "no session");
-  auto lock = lock_if_default(cs->ctx);
+  Lock lock(cs->ctx->mu);
   try {
     std::vector<VCmd> cmds;
     if (n_sets < 0 || (n_sets > 0 && set_off[0] < 0)) return fail(KSCHED_ERR_INVALID, "n_sets / set_off out of range");
@@ -1433,44 +1376,22 @@ int kh_cluster_validate(ClusterSession* cs, const Problem* after, const int* set
 
 // ncclAllGather of n ints per rank on the scheduler handle's communicator (kh_nccl_init first)
 int kh_allgather_i32(const int* send, int n, int* recv) {
-  KH_DEFAULT_LOCK;
-  int rc = ensure_handle();
+  Lock lock(g_default.mu);
+  int rc = open_handle(&g_default);
   if (rc != KSCHED_OK) return rc;
-  rc = ksched_allgather(g_handle, send, (size_t)n * sizeof(int), recv);
-  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
+  rc = ksched_allgather(g_default.h, send, (size_t)n * sizeof(int), recv);
+  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_default.h));
   return KSCHED_OK;
 }
 // communicator for the scheduler handle without column sharding (replicas / sharded consolidation)
 int kh_nccl_init(const void* id128, int rank, int world) {
-  KH_DEFAULT_LOCK;
-  int rc = ensure_handle();
+  Lock lock(g_default.mu);
+  int rc = open_handle(&g_default);
   if (rc != KSCHED_OK) return rc;
-  rc = ksched_nccl_init(g_handle, id128, rank, world);
-  if (rc == KSCHED_OK) rc = ksched_set_shard(g_handle, 0, 1);
-  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_handle));
+  rc = ksched_nccl_init(g_default.h, id128, rank, world);
+  if (rc == KSCHED_OK) rc = ksched_set_shard(g_default.h, 0, 1);
+  if (rc != KSCHED_OK) return fail(rc, ksched_last_error(g_default.h));
   return KSCHED_OK;
-}
-
-// SingleNodeConsolidation.ComputeCommand (singlenodeconsolidation.go:43-84) without validation: the candidates in disruption
-// order, the first whose computeConsolidation yields delete / replace wins. The independent simulations go to the device
-// `batch` at a time (ksched_simulate_batch). out4: [action, position of the winning candidate in the disruption order or -1,
-// simulations, n_options]; *node = its Problem.nodes index. first / last bound the positions tried (a rank's share of the
-// sweep); last < 0 = all.
-int kh_consolidate_single(const Problem* P, int first, int last, int batch, int* out4, int* node, int* options, int options_cap) {
-  KH_DEFAULT_LOCK;
-  try {
-    ClusterSession cs(P);
-    const Sweep s = single_sweep(cs, nullptr, first, last, batch);
-    out4[0] = s.cmd.action;
-    out4[1] = s.position;
-    out4[2] = s.sims;
-    out4[3] = (int)s.cmd.options.size();
-    *node = s.position >= 0 ? cs.cands[(size_t)s.position].node : -1;
-    for (size_t i = 0; i < s.cmd.options.size() && (int)i < options_cap; ++i) options[i] = s.cmd.options[i];
-    return KSCHED_OK;
-  } catch (const std::exception& e) {
-    return fail(error_code(e), e.what());
-  }
 }
 
 // SingleNodeConsolidation.ComputeCommand with Validation against `after` (singlenodeconsolidation.go:52-84): the first
@@ -1480,7 +1401,7 @@ int kh_consolidate_single(const Problem* P, int first, int last, int batch, int*
 // merge as: the first share with a winner gives the command; with none, retry when any share failed a validation.
 int kh_consolidate_single_validated(const Problem* before, const Problem* after, int first, int last, int batch, int* out4, int* node, int* options,
                                     int options_cap, int* trace, int* trace_valid, int trace_cap, int* n_trace, int* failed_validation) {
-  KH_DEFAULT_LOCK;
+  Lock lock(g_default.mu);
   try {
     ClusterSession cs(before);
     const Sweep s = single_sweep(cs, after, first, last, batch);
@@ -1499,56 +1420,21 @@ int kh_consolidate_single_validated(const Problem* before, const Problem* after,
   }
 }
 
-// Two handles on one device, one host thread each, solving different problems at the same time. The pack kernel's
-// parameter block is one __constant__ object per device, so concurrent handles only stay correct through the device-side
-// ordering in run_pack(); this entry point lets the GPU tests prove it. Returns 0 when every repetition of each problem
-// reproduced that problem's first result bit for bit, a negative ksched error otherwise, or 1 on a mismatch.
-extern "C" int kh_selftest_two_handles(const Problem* A, const Problem* B, int iters) {
-  KH_DEFAULT_LOCK;
-  int rc = ensure_handle();
-  if (rc != KSCHED_OK) return rc;
-  const Problem* probs[2] = {A, B};
-  int status[2] = {0, 0};
-  std::thread workers[2];
-  for (int w = 0; w < 2; ++w) {
-    workers[w] = std::thread([&, w]() {
-      try {
-        ksched_handle* h = nullptr;
-        if (ksched_create(g_device, &h) != KSCHED_OK) { status[w] = KSCHED_ERR_CUDA; return; }
-        auto E = khost::encode(*probs[w], {});
-        E->problem.count_nodes_visited = 0;
-        std::vector<int32_t> first;
-        for (int it = 0; it < iters && status[w] == 0; ++it) {
-          ResultBuffers R;
-          int r2 = ksched_load_catalog(h, &E->catalog);
-          if (r2 == KSCHED_OK) { R.prepare(*E, false); r2 = ksched_solve(h, &E->problem, &R.r); }
-          if (r2 != KSCHED_OK) { status[w] = r2; break; }
-          std::vector<int32_t> sig(R.assign.begin(), R.assign.end());
-          sig.push_back(R.r.n_new_nodes);
-          for (int n = 0; n < R.r.n_new_nodes; ++n)
-            for (int k = 0; k < E->type_words; ++k) {
-              const uint64_t b = R.types[(size_t)n * E->type_words + k];
-              sig.push_back((int32_t)b);
-              sig.push_back((int32_t)(b >> 32));
-            }
-          if (it == 0) first = sig;
-          else if (sig != first) status[w] = 1;
-        }
-        ksched_destroy(h);
-      } catch (const std::exception& e) {
-        status[w] = error_code(e);
-      }
-    });
-  }
-  for (auto& t : workers) t.join();
-  return status[0] ? status[0] : status[1];
+// SingleNodeConsolidation.ComputeCommand (singlenodeconsolidation.go:43-84) without validation: the candidates in disruption
+// order, the first whose computeConsolidation yields delete / replace wins. The independent simulations go to the device
+// `batch` at a time (ksched_simulate_batch). out4: [action, position of the winning candidate in the disruption order or -1,
+// simulations, n_options]; *node = its Problem.nodes index. first / last bound the positions tried (a rank's share of the
+// sweep); last < 0 = all.
+int kh_consolidate_single(const Problem* P, int first, int last, int batch, int* out4, int* node, int* options, int options_cap) {
+  int n_trace, failed_validation;
+  return kh_consolidate_single_validated(P, nullptr, first, last, batch, out4, node, options, options_cap, nullptr, nullptr, 0, &n_trace,
+                                         &failed_validation);
 }
 
 // ---- launch-choice table + shared core (csrc/launch.cuh) checked on the CPU: for every new node of `ref` (a Result of
 // the same problem, e.g. the oracle's) recompute the launch choice from the ENCODED offering table exactly as the device
 // kernel does, and compare with the fields `ref` carries. Returns the number of nodes that differ, or a negative error.
 extern "C" int kh_launch_table_selfcheck(const Problem* P, const Result* ref) {
-  KH_DEFAULT_LOCK;
   try {
     auto E = khost::encode(*P, {});
     int zone_key = -1, ct_key = -1;

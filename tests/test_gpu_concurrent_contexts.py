@@ -11,6 +11,7 @@ import consolidation_answers as ca
 import fixtures as fx
 import validation_oracle as vo
 from known_answers import CASES
+from oracle_compare import compare
 
 pytestmark = pytest.mark.gpu
 
@@ -184,6 +185,23 @@ def test_contexts_sharing_a_slot_keep_their_answers(pkg, prov):
     alone = [provisioning(pkg, c, j) for c, j in zip(ctxs, jobs)]
     got = _run_together(*[(lambda c=c, j=j: provisioning(pkg, c, j)) for c, j in zip(ctxs, jobs)])
     assert got == alone
+    for c in ctxs:
+        c.destroy()
+
+
+def test_two_contexts_repeat_their_own_solves(pkg, oracle):
+    """Two contexts driven by two host threads, each solving its own problem six times: every repetition equals that
+    context's first result bit for bit (assignment, new nodes and their options), and the process-wide handle still agrees
+    with the oracle afterwards."""
+    problems = [pkg.Problem.synth(4, 1500, 1000, 5, 0), pkg.Problem.synth(3, 2000, 1000, 6, 0)]
+    ctxs = [pkg.Context(0), pkg.Context(0)]
+
+    def repeat(ctx, problem):
+        return [_solve_key(pkg.Scheduler(problem, context=ctx).solve(count_visited=False)) for _ in range(6)]
+    got = _run_together(*[(lambda c=c, p=p: repeat(c, p)) for c, p in zip(ctxs, problems)])
+    for runs in got:
+        assert all(r == runs[0] for r in runs[1:])
+    compare(pkg, oracle, problems[0])
     for c in ctxs:
         c.destroy()
 

@@ -107,16 +107,6 @@ def test_feasibility_matrix_matches_fresh_node_options(pkg, oracle):
     assert checked > 1500
 
 
-def test_two_handles_on_one_device_solve_concurrently(pkg, oracle):
-    """The pack kernel's parameters live in one __constant__ block per device: two handles driven by two host threads must
-    still each reproduce their own result (device-side ordering in run_pack)."""
-    a = pkg.Problem.synth(4, 1500, 1000, 5, 0)
-    b = pkg.Problem.synth(3, 2000, 1000, 6, 0)
-    assert pkg.lib().kh_selftest_two_handles(a.ptr, b.ptr, 6) == 0
-    # and the singleton handle still agrees with the oracle afterwards
-    compare(pkg, oracle, a, [])
-
-
 from consolidation_answers import CASES as _CONS, CPU_ONLY_CASES as _CONS_LATE
 
 CONSOLIDATION_CASES = _CONS + _CONS_LATE

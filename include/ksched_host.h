@@ -159,6 +159,10 @@ int kh_encoded_volume_claim(const void* enc, int id, char* out, int cap);
 int kh_encoded_class_row(const void* enc, int c, uint64_t* out);
 int kh_gpu_k1_plan(int* out);
 int kh_gpu_set_shard(int rank, int world);
+/* ---- the pack kernel's class-run records (tests): the first n records of the process handle's last resident Solve, 128
+ * bytes per class (csrc/pack_state.cuh: RunRec), into out. Returns the number of classes the Solve built records for (0
+ * when class runs could not run), or a negative error. */
+int kh_gpu_run_records(void* out, int n);
 
 /* ---- self-test of the encoder's value classes (CPU, no device): random wide keys and requirement pairs, the exact string
  * algebra against the collapsed masks (host form and region form). Returns the number of mismatches. */

@@ -154,6 +154,7 @@ def lib():
     L.kh_gpu_load_catalog.argtypes = [C.c_void_p]
     L.kh_encoded_class_row.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     L.kh_gpu_k1_plan.argtypes = [C.POINTER(C.c_int)]
+    L.kh_gpu_run_records.argtypes = [C.c_void_p, C.c_int]
     L.kh_gpu_set_shard.argtypes = [C.c_int, C.c_int]
     L.kh_consolidate.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int,
                                  C.POINTER(C.c_int)]
@@ -762,6 +763,19 @@ class ResidentSolve:
         out = (C.c_int * 5)()
         _check(lib().kh_gpu_k1_plan(out))
         return dict(zip(["blocks", "chunk", "cacheable", "alloc_in_smem", "tables_in_smem"], list(out)))
+
+    RUN_REC_DTYPE = np.dtype([("ok", "<i4"), ("n_host", "<i4"), ("n_mask", "<i4"), ("h_row", "<i4", 4), ("h_group", "<i4", 4),
+                              ("h_lim", "<i4", 4), ("m_group", "<i4", 2), ("m_skew", "<i4", 2), ("m_neutral", "<u4", 2),
+                              ("m_tallow", "<u4", 2), ("m_dict", "<u4", 2), ("h_times", "u1", 4), ("m_key", "u1", 2),
+                              ("m_self", "u1", 2), ("m_rec", "u1", 2), ("m_wk", "u1", 2), ("pad", "<u4", 4)])
+
+    def run_records(self):
+        """the class runs' relation tables of this problem's last run(): one record per class (csrc/pack_state.cuh: RunRec)
+        as a structured array, or None when that Solve built none (class runs could not run)"""
+        out = np.zeros(max(self.dims["classes"], 1), dtype=self.RUN_REC_DTYPE)
+        n = lib().kh_gpu_run_records(out.ctypes.data, self.dims["classes"])
+        _check(min(n, 0))
+        return out[:self.dims["classes"]] if n > 0 else None
 
     def resource_id(self, name):
         """id of a resource in this encoding: a row slot below 8, an ext resource from 8 on; -1 when it is not carried"""

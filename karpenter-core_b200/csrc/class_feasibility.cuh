@@ -3,16 +3,16 @@
 // Part of the single translation unit ksched.cu, which includes it once per parameter slot (namespaces slot0, slot1, each
 // followed by topology.cuh and pack_kernel.cuh); not a standalone header.
 
-__device__ void vt_build_block(int b);  // pack_kernel.cuh
+__device__ void k0_extra_block(int b);  // pack_kernel.cuh
 // FFD-ordered dense pod-row matrix: row j = class row of the j-th pod of the queue. One warp per row,
-// 256-byte coalesced loads and stores. kTable: the blocks from `blocks` on build the pack kernel's variant table
-// (vt_build_block), which depends on nothing this launch writes; the launches without a table keep the gather's small
+// 256-byte coalesced loads and stores. kTable: the blocks from `blocks` on build the pack kernel's variant table and run
+// records (k0_extra_block), which depend on nothing this launch writes; the launches without them keep the gather's small
 // register and shared-memory footprint.
 template <bool kTable>
 __global__ void gather_rows_kernel(int n, const ksched_pod_row* __restrict__ classes, const uint32_t* __restrict__ pod_class,
                                    const uint32_t* __restrict__ order, uint64_t* __restrict__ rows, int blocks) {
   if (kTable && (int)blockIdx.x >= blocks) {
-    vt_build_block((int)blockIdx.x - blocks);
+    k0_extra_block((int)blockIdx.x - blocks);
     return;
   }
   int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;

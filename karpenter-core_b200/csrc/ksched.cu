@@ -328,6 +328,7 @@ struct ksched_handle {
   DevBuf<long long> d_ov_q, d_ov_bound, d_ov_bound2, d_fc_bound, d_fc_bound2, d_fc_q, d_fd_bound, d_fd_bound2;
   DevBuf<RunVariant> d_vtable;
   DevBuf<uint32_t> d_vt_ok;
+  DevBuf<RunRec> d_run_rec;
   // ---- device-resident cluster snapshot (ksched_load_cluster)
   bool have_cluster = false;
   int sup_pods = 0, sup_pending = 0;
@@ -1275,6 +1276,7 @@ static int bind_problem(ksched_handle* h, const ksched_problem* pb) {
     CUDA_TRY(h, bind(h, h->d_vtable, s.vtable, n));
     CUDA_TRY(h, bind_zeroed(h, h->d_vt_ok, s.vt_ok, n));
   }
+  CUDA_TRY(h, bind(h, h->d_run_rec, s.run_rec, (size_t)std::max(1, s.n_classes)));
   {
     size_t need = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, need, (uint64_t*)nullptr, (uint64_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)p1, 0, 64, h->stream);
@@ -1308,8 +1310,8 @@ int ksched_upload(ksched_handle* h, const ksched_problem* pb) {
 static std::mutex g_k2_mu[64][KSCHED_PARAM_SLOTS];
 static cudaEvent_t g_k2_done[64][KSCHED_PARAM_SLOTS] = {};
 static int set_k2(ksched_handle* h, int n_pods, int stop_new_nodes, bool with_table);
-// with_table: the row gather's launch also builds the pack kernel's variant table (vt_build_block), for the pack launch
-// that follows with the same flag
+// with_table: the row gather's launch also builds the pack kernel's variant table and run records (k0_extra_block), for the
+// pack launch that follows with the same flag
 static int run_sort(ksched_handle* h, int P, bool with_table = false) {
   if (P == 0) return KSCHED_OK;
   const int threads = 256, blocks = (P + threads - 1) / threads;
@@ -1325,8 +1327,8 @@ static int run_sort(ksched_handle* h, int P, bool with_table = false) {
     std::lock_guard<std::mutex> lock(g_k2_mu[h->device][h->slot]);
     int rc = set_k2(h, P, 0, true);
     if (rc != KSCHED_OK) return rc;
-    const int vt_blocks = h->k2_host.st.vt_classes * h->vt_ndom;
-    g_slot_kernels[h->slot].gather_table<<<gblocks + vt_blocks, 256, 0, h->stream>>>(P, h->d_classes.ptr, h->d_pod_class.ptr, h->d_order.ptr,
+    const int vt_blocks = h->k2_host.st.vt_classes * h->vt_ndom, rec_blocks = (h->k2_host.st.rec_classes + 255) / 256;
+    g_slot_kernels[h->slot].gather_table<<<gblocks + vt_blocks + rec_blocks, 256, 0, h->stream>>>(P, h->d_classes.ptr, h->d_pod_class.ptr, h->d_order.ptr,
                                                                                      h->d_rows.ptr, gblocks);
     CUDA_TRY(h, cudaGetLastError());
     CUDA_TRY(h, cudaEventRecord(g_k2_done[h->device][h->slot], h->stream));
@@ -1490,6 +1492,9 @@ static int set_k2(ksched_handle* h, int n_pods, int stop_new_nodes, bool with_ta
   s.any_limits = 0;
   for (const ksched_template& tm : h->h_templates) if (tm.has_limits && tm.limit_present) s.any_limits = 1;
   s.use_class_run = getenv("KSCHED_NO_CLASSRUN") ? 0 : 1;
+  // the run records are built by a launch with the table (the resident Solve) when a class run can start: no existing node
+  // and no nodes_visited statistic (the pack kernel's fast_allowed); the pack kernel starts none without them
+  s.rec_classes = with_table && s.use_class_run && s.n_existing == 0 && !s.count_visited ? s.n_classes : 0;
   s.use_level_run = std::getenv("KSCHED_NO_LEVELRUN") ? 0 : 1;
   s.use_mask_run = std::getenv("KSCHED_NO_MASKRUN") ? 0 : 1;
   s.use_level_warp = std::getenv("KSCHED_NO_LEVELWARP") ? 0 : 1;
@@ -2112,6 +2117,21 @@ int ksched_get_timings(const ksched_handle* h, ksched_timings* out) {
 }
 
 }  // extern "C"
+
+// The class runs' relation tables the handle's last resident Solve built (host layer: kh_gpu_run_records): the first n
+// classes' 128-byte records (pack_state.cuh: RunRec) into out. Returns the number of records built (0: none, class runs
+// could not run), or a negative error. Not part of the C-ABI.
+int ksched_run_records(ksched_handle* h, void* out, int n) {
+  if (!h || !h->uploaded || (n > 0 && !out)) return KSCHED_ERR_INVALID;
+  const int built = h->k2_host.st.rec_classes;
+  const int m = std::min(n, built);
+  if (m > 0) {
+    CUDA_TRY(h, cudaSetDevice(h->device));
+    CUDA_TRY(h, cudaMemcpyAsync(out, h->st.run_rec, (size_t)m * sizeof(RunRec), cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  }
+  return built;
+}
 
 // The launch plan of the handle's last K1 class pass (host layer: kh_gpu_k1_plan). Not part of the C-ABI.
 int ksched_k1_plan(const ksched_handle* h, int out[5]) {

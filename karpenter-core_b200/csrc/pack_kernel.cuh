@@ -1303,17 +1303,16 @@ constexpr size_t kRunArrayBytes = (size_t)kTopoCap * (kRunMask * 4 + kRunHost * 
 // RunVariant lives in pack_state.cuh (PackState points at the variant table) with the same three sizes
 static_assert(sizeof(RunVariant::b1) == kHotRes * sizeof(long long) && sizeof(RunVariant::dom) == kRunMask && sizeof(RunVariant::opts) == kRunW32 * 4,
               "RunVariant is sized by kHotRes, kRunMask and kRunW32");
+static_assert(sizeof(RunRec::h_row) == kRunHost * 4 && sizeof(RunRec::m_group) == kRunMask * 4, "RunRec is sized by kRunHost and kRunMask");
 struct RunCtx {
-  uint32_t cls;           // class the relation tables and variants belong to (KSCHED_NONE: none)
+  uint32_t cls;           // class the variants belong to (KSCHED_NONE: none)
   int eligible;
-  int n_host, n_mask, n_var, var_next;
+  int n_var, var_next;
   int tomb;               // nodes tombstoned by the current run
-  int h_row[kRunHost], h_group[kRunHost], h_lim[kRunHost];  // h_lim: largest count of the group on a node that still admits the pod
+  RunRec rec;             // the class's relation tables (PackState::run_rec)
   int h_inc[kRunHost];    // hostnames that got their first matching pod in this run (grp_host_total)
-  uint8_t h_times[kRunHost];
-  int m_group[kRunMask], m_skew[kRunMask];
-  uint8_t m_key[kRunMask], m_self[kRunMask], m_rec[kRunMask], m_wk[kRunMask];
-  uint32_t m_registered[kRunMask], m_neutral[kRunMask], m_tallow[kRunMask];
+  int h_zero;             // bit j: hostname relation j's group counted no slot at entry (grp_host_total 0: every count is 0)
+  uint32_t m_registered[kRunMask];
   int32_t cnt[kRunWarps][kRunMask][kRunDom];  // one copy of the spread counters per warp (updated by its lane 0)
   unsigned long long red_key[2][32];
   unsigned red_pay[2][32];
@@ -1467,11 +1466,11 @@ __device__ __forceinline__ uint32_t run_record_host(const RunCtx& rc, uint16_t* 
 #pragma unroll
   for (int j = 0; j < kRunHost; ++j) {
     if (j >= n_host) break;
-    const int times = rc.h_times[j];
+    const int times = rc.rec.h_times[j];
     const int old = hc[j * kTopoCap + a];
     const int now = old + t * times > 0xFFFF ? 0xFFFF : old + t * times;
     if (times) hc[j * kTopoCap + a] = (uint16_t)now;
-    if (now > rc.h_lim[j]) rp2 |= kRpDead;
+    if (now > rc.rec.h_lim[j]) rp2 |= kRpDead;
   }
   return rp2;
 }
@@ -1528,9 +1527,9 @@ __device__ __forceinline__ void run_fresh(const RunEnv& e, const RunVariant& v, 
   const RunCtx& rc = g_rc;
   HotSmem* hs = e.hs;
   for (int j = 0; j < e.n_host; ++j) {
-    const int times = rc.h_times[j];
+    const int times = rc.rec.h_times[j];
     e.hc[j * kTopoCap + a] = (uint16_t)times;
-    if (times) s.grp_host[(size_t)rc.h_row[j] * e.hstride + e.NE + n] = (uint16_t)times;
+    if (times) s.grp_host[(size_t)rc.rec.h_row[j] * e.hstride + e.NE + n] = (uint16_t)times;
   }
   hs->key[a] = order_key(1, tb);
 #pragma unroll
@@ -1545,7 +1544,7 @@ __device__ __forceinline__ void run_fresh(const RunEnv& e, const RunVariant& v, 
 // nn_meta: the load would stall the commit for an L2 round trip (a node has one writer, and nothing in the run reads it).
 __device__ __forceinline__ void run_pin(const RunEnv& e, int j, int a, int d) {
   KS_K2
-  const int n = e.hs->node[a], k = g_rc.m_key[j];
+  const int n = e.hs->node[a], k = g_rc.rec.m_key[j];
   e.zv[j * kTopoCap + a] = (1u << d) | (3u << 16);
   s.nn_vals[(size_t)k * e.MAXN + n] = 1ull << d;
   atomicOr(reinterpret_cast<unsigned long long*>(&s.nn_meta[n]), 1ull << (KSCHED_META_PRESENT_SHIFT + k));
@@ -1562,7 +1561,7 @@ __device__ __forceinline__ int run_ring_find(const RunCtx& rc, int n_mask, int d
 __device__ __forceinline__ int run_fill_cap(const RunEnv& e, int a, int cap) {
   const RunCtx& rc = g_rc;
   for (int j = 0; j < e.n_host; ++j) {
-    const int times = rc.h_times[j], lim = rc.h_lim[j];
+    const int times = rc.rec.h_times[j], lim = rc.rec.h_lim[j];
     if (!times || lim >= 0x10000) continue;
     if (lim >= 0xFFF0) { cap = 1; continue; }  // saturating counters nearby: one pod at a time
     const int td = (lim - (int)e.hc[j * kTopoCap + a]) / times + 1;
@@ -1894,11 +1893,11 @@ __device__ __forceinline__ int m1_round(const RunEnv& e, int buf, M1Lane& l, M1W
       if (R < 2 && s.use_fill_stretch)
 #endif
         Rf = __reduce_min_sync(kFull, m1_fill_len(e, l, act, okm, na, cap, ukey, w.ltick, fp));
-    } else if (hv == 0 && ukey == ~0ull && (okm & ~rc.m_tallow[0]) == 0) {  // fresh nodes that never re-enter a list
+    } else if (hv == 0 && ukey == ~0ull && (okm & ~rc.rec.m_tallow[0]) == 0) {  // fresh nodes that never re-enter a list
       if (act) vi_s = run_ring_find(rc, 1, L, 0);
       const bool shut = vi_s >= 0 && ((rc.var[vi_s].rp & 0xFFFF) == 0 || (rc.var[vi_s].rp & kRpDead));
       bool ok = !__any_sync(kFull, act && !shut);
-      for (int j = 0; j < e.n_host; ++j) ok = ok && rc.h_lim[j] >= 0;
+      for (int j = 0; j < e.n_host; ++j) ok = ok && rc.rec.h_lim[j] >= 0;
       int room = e.MAXN - w.lnew;
       if (kActCap - w.lact < room) room = kActCap - w.lact;
       if (kTopoCap - w.lact < room) room = kTopoCap - w.lact;
@@ -1962,7 +1961,7 @@ __device__ __forceinline__ int m1_round(const RunEnv& e, int buf, M1Lane& l, M1W
       const int d = __ffs(m) - 1;
       const int vi = __shfl_sync(kFull, vi_s, d);
       if (L < np) m1_fresh(e, buf, vi, w.lact + L, w.lnew + L, w.ltick + L + 1, w.li + L, d, w.nfr + L);
-      if (L < e.n_host && rc.h_times[L]) rc.h_inc[L] = rc.h_inc[L] + np;
+      if (L < e.n_host && rc.rec.h_times[L]) rc.h_inc[L] = rc.h_inc[L] + np;
       if (act) w.cnt_d += R;
       w.lnew += np;
       w.lact += np;
@@ -1982,9 +1981,9 @@ __device__ __forceinline__ int m1_round(const RunEnv& e, int buf, M1Lane& l, M1W
   if (fv) {
     const bool fl = act && l.h < 0;
     if (fl) vi_l = run_ring_find(rc, 1, L, 0);
-    fresh_ok = ukey == ~0ull && (fv & ~rc.m_tallow[0]) == 0 && !__any_sync(kFull, fl && vi_l < 0) && w.lnew + nf <= e.MAXN &&
+    fresh_ok = ukey == ~0ull && (fv & ~rc.rec.m_tallow[0]) == 0 && !__any_sync(kFull, fl && vi_l < 0) && w.lnew + nf <= e.MAXN &&
                w.lact + nf <= kActCap && w.lact + nf <= kTopoCap;
-    for (int j = 0; j < e.n_host; ++j) fresh_ok = fresh_ok && rc.h_lim[j] >= 0;
+    for (int j = 0; j < e.n_host; ++j) fresh_ok = fresh_ok && rc.rec.h_lim[j] >= 0;
   }
   if (!fresh_ok || __any_sync(kFull, bad_l) || (hv != 0 && ukey <= mx)) return 0;
   w.fr_used |= __reduce_or_sync(kFull, (act && !hd) ? 1u << vi_l : 0u);
@@ -2011,7 +2010,7 @@ __device__ __forceinline__ int m1_round(const RunEnv& e, int buf, M1Lane& l, M1W
     if ((v.rp & 0xFFFF) != 0 && !(v.rp & kRpDead)) l.insert_back1(e, w.lact + idx, order_key(1, mytick + 1), v.rp);
     ++w.cnt_d;
   }
-  if (nf && L < e.n_host && rc.h_times[L]) rc.h_inc[L] = rc.h_inc[L] + nf;
+  if (nf && L < e.n_host && rc.rec.h_times[L]) rc.h_inc[L] = rc.h_inc[L] + nf;
   const unsigned tb = __ballot_sync(kFull, closed_l);
   if (L == 0 && tb) rc.tomb = rc.tomb + __popc(tb);
 #ifdef KSCHED_PROFILE_PACK
@@ -2067,7 +2066,7 @@ __device__ __forceinline__ int m1_pin_step(const RunEnv& e, int buf, M1Lane& l, 
   }
   const bool same_c = (int)(k_t >> 32) == c, below = k_t < pmin;
   const bool ok_t = in && same_c && below && (rp_t & 0xFFFF) != kRoomSlow && c + 1 < kM1Lv &&
-                    ((rc.m_neutral[0] >> d_t) & 1) && ((z_t & (1u << 17)) || rc.m_wk[0]);
+                    ((rc.rec.m_neutral[0] >> d_t) & 1) && ((z_t & (1u << 17)) || rc.rec.m_wk[0]);
   const unsigned okb = __ballot_sync(kFull, ok_t);
   const int J = okb == kFull ? 32 : __ffs(~okb) - 1;
 #ifdef KSCHED_PROFILE_PACK
@@ -2123,7 +2122,7 @@ __device__ __forceinline__ int m1_single(const RunEnv& e, int buf, M1Lane& l, M1
   const bool pin = wl == kM1Dom;
   if (pin) {  // the placement pins the node's domain: fewest pods, lowest id among the admissible ones (run_pick)
     d = warp_pick(allowed, w.cnt_d);
-    if (!((rc.m_neutral[0] >> d) & 1) || !((e.zv[a] & (1u << 17)) || rc.m_wk[0])) { why = kStopOther; return 1; }
+    if (!((rc.rec.m_neutral[0] >> d) & 1) || !((e.zv[a] & (1u << 17)) || rc.rec.m_wk[0])) { why = kStopOther; return 1; }
 #ifdef KSCHED_PROFILE_PACK
     if (L == 0) s.counters[kCtrMaskUnpinnedSingle] += 1;
 #endif
@@ -2134,11 +2133,11 @@ __device__ __forceinline__ int m1_single(const RunEnv& e, int buf, M1Lane& l, M1
   uint32_t rp2 = rp - 1 + (1u << 16);
   bool dead_l = false;
   if (L < e.n_host) {  // Topology.Record, hostname groups
-    const int times = rc.h_times[L];
+    const int times = rc.rec.h_times[L];
     const int old = e.hc[L * kTopoCap + a];
     const int now = old + times > 0xFFFF ? 0xFFFF : old + times;
     if (times) e.hc[L * kTopoCap + a] = (uint16_t)now;
-    dead_l = now > rc.h_lim[L];
+    dead_l = now > rc.rec.h_lim[L];
   }
   if (e.n_host > 0 && __any_sync(kFull, dead_l)) rp2 |= kRpDead;
   if (L == 0) {
@@ -2165,8 +2164,8 @@ __device__ __forceinline__ int m1_single_fresh(const RunEnv& e, int buf, M1Lane&
   const int L = l.L;
   if (w.lnew >= e.MAXN || w.lact >= kActCap || w.lact >= kTopoCap) { why = kStopCapacity; return 1; }
   bool ok = true;
-  for (int j = 0; j < e.n_host; ++j) ok = ok && rc.h_lim[j] >= 0;
-  const unsigned cand = rc.m_tallow[0] & okm;
+  for (int j = 0; j < e.n_host; ++j) ok = ok && rc.rec.h_lim[j] >= 0;
+  const unsigned cand = rc.rec.m_tallow[0] & okm;
   if (!ok || !cand) { why = kStopOther; return 1; }
   const int fd = warp_pick((cand >> L) & 1, w.cnt_d);  // (cand is a subset of okm: lanes below kM1Dom)
   int vi = run_ring_find(rc, 1, fd, 0);
@@ -2174,7 +2173,7 @@ __device__ __forceinline__ int m1_single_fresh(const RunEnv& e, int buf, M1Lane&
   if (vi < 0) { why = kStopNoVariant; return 1; }
   const RunVariant& v = rc.var[vi];
   w.fr_used |= 1u << vi;
-  if (L < e.n_host && rc.h_times[L]) rc.h_inc[L] = rc.h_inc[L] + 1;
+  if (L < e.n_host && rc.rec.h_times[L]) rc.h_inc[L] = rc.h_inc[L] + 1;
   if (L == 0) m1_fresh(e, buf, vi, w.lact, w.lnew, w.ltick + 1, w.li, fd, w.nfr);  // nothing in this loop reads the node's global state
   ++w.nfr;
   if (L == fd) {
@@ -2476,7 +2475,7 @@ __device__ __forceinline__ int run_argmin_step(const RunEnv& e, int buf, int i, 
       else {  // the placement pins the node's domain
         d = run_pick(cand, rc.cnt[warp][j]);
         pay |= 1u << (13 + j);
-        if (!((rc.m_neutral[j] >> d) & 1) || !((z & (1u << 17)) || rc.m_wk[j])) pay |= 1u << 11;
+        if (!((rc.rec.m_neutral[j] >> d) & 1) || !((z & (1u << 17)) || rc.rec.m_wk[j])) pay |= 1u << 11;
       }
       pay |= (unsigned)d << (15 + 4 * j);
     }
@@ -2528,14 +2527,14 @@ __device__ __forceinline__ bool run_fresh_step(const RunEnv& e, int buf, int i, 
   if (n_new >= MAXN || n_active >= kActCap || (e.topo && n_active >= kTopoCap)) { why = kStopCapacity; return false; }
   bool ok = true;
 #pragma unroll
-  for (int j = 0; j < kRunHost; ++j) ok = ok && (j >= e.n_host || rc.h_lim[j] >= 0);  // a fresh hostname has count 0
+  for (int j = 0; j < kRunHost; ++j) ok = ok && (j >= e.n_host || rc.rec.h_lim[j] >= 0);  // a fresh hostname has count 0
   int fd0 = 0, fd1 = 0;
   if (n_mask > 0 && ok) {
-    const uint32_t cand = rc.m_tallow[0] & okm0;
+    const uint32_t cand = rc.rec.m_tallow[0] & okm0;
     if (!cand) ok = false; else fd0 = run_pick(cand, rc.cnt[warp][0]);
   }
   if (n_mask > 1 && ok) {
-    const uint32_t cand = rc.m_tallow[1] & okm1;
+    const uint32_t cand = rc.rec.m_tallow[1] & okm1;
     if (!cand) ok = false; else fd1 = run_pick(cand, rc.cnt[warp][1]);
   }
   int vi = ok ? run_ring_find(rc, n_mask, fd0, fd1) : -1;
@@ -2557,7 +2556,7 @@ __device__ __forceinline__ bool run_fresh_step(const RunEnv& e, int buf, int i, 
     if (!(v.rp & kRpDead)) {
       cap = (int)(v.rp & 0xFFFF);
       for (int j = 0; j < e.n_host; ++j) {
-        const int times = rc.h_times[j], lim = rc.h_lim[j];
+        const int times = rc.rec.h_times[j], lim = rc.rec.h_lim[j];
         if (!times || lim >= 0x10000) continue;
         if (lim >= 0xFFF0) { cap = 0; cap_exact = false; continue; }  // saturating counters nearby: one pod at a time
         const int td = (lim - times) / times + 1;  // the count is `times` after the first pod
@@ -2577,7 +2576,7 @@ __device__ __forceinline__ bool run_fresh_step(const RunEnv& e, int buf, int i, 
   for (int idx = tid; idx < c.n_keys * F; idx += T) { const int k = idx / F, j = idx - k * F; s.nn_vals[(size_t)k * MAXN + n_new + j] = v.vals[k]; }
   for (int idx = tid; idx < KSCHED_MAX_RES * F; idx += T) { const int r = idx / F, j = idx - r * F; s.nn_req[(size_t)r * MAXN + n_new + j] = v.q[r]; }
   for (int x = tid; x < K; x += T) rc.q_node[buf][i + x] = e.NE + n_new + x / m;
-  if (tid == 0) for (int j = 0; j < e.n_host; ++j) if (rc.h_times[j]) rc.h_inc[j] = rc.h_inc[j] + F;
+  if (tid == 0) for (int j = 0; j < e.n_host; ++j) if (rc.rec.h_times[j]) rc.h_inc[j] = rc.h_inc[j] + F;
   for (int j = (tid + T - n_active % T) % T; j < F; j += T) {  // the new slots this thread owns
     const int a = n_active + j, n = n_new + j;
     const int t = (K - j * m < m ? K - j * m : m) - 1;  // further pods on this node (the last one may get fewer)
@@ -2661,9 +2660,9 @@ __device__ __noinline__ int run_derive(const PodRegs& first_in, int fpos, int n_
   uint32_t* zv = reinterpret_cast<uint32_t*>(dyn_smem + sizeof(HotSmem) + s.run_off);
   uint32_t* rpv = zv + (size_t)kRunMask * kTopoCap;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int n_mask = rc.n_mask, n_host = rc.n_host, MAXN = s.max_new;
+  const int n_mask = rc.rec.n_mask, n_host = rc.rec.n_host, MAXN = s.max_new;
   for (int j = 0; j < n_mask; ++j)
-    if (rc.m_rec[j] && warp == 0 && lane < kRunDom && ((rc.m_registered[j] >> lane) & 1)) s.grp_cnt[(size_t)rc.m_group[j] * 64 + lane] = rc.cnt[0][j][lane];
+    if (rc.rec.m_rec[j] && warp == 0 && lane < kRunDom && ((rc.m_registered[j] >> lane) & 1)) s.grp_cnt[(size_t)rc.rec.m_group[j] * 64 + lane] = rc.cnt[0][j][lane];
   if (tid == 0) g_rio.staged = 1;
   int fatal = 0;
   uint32_t epoch = 0;
@@ -2676,10 +2675,10 @@ __device__ __noinline__ int run_derive(const PodRegs& first_in, int fpos, int n_
   if (tid == 0) {  // the slot's per-run inputs as class_run's entry computes them (its hostname counts: the relations' times)
     long long p_req[kHotRes];
     for (int r = 0; r < kHotRes; ++r) p_req[r] = first_in.req[r];
-    rpv[a] = fresh_room_word(run_room(hs, a, p_req, first_in.res, c.n_res < kHotRes ? c.n_res : kHotRes), n_host, rc.h_times, rc.h_lim);
+    rpv[a] = fresh_room_word(run_room(hs, a, p_req, first_in.res, c.n_res < kHotRes ? c.n_res : kHotRes), n_host, rc.rec.h_times, rc.rec.h_lim);
     const uint64_t meta = s.nn_meta[n];
     for (int j = 0; j < n_mask; ++j) {
-      const int k = rc.m_key[j];
+      const int k = rc.rec.m_key[j];
       const Req r = load_soa(s.nn_vals, meta, MAXN, n, k);
       const uint32_t allowed = (uint32_t)(r.present ? ksched::req_allowed(r, c.keys[k].dict_mask, key_meta(c, k)) : c.keys[k].dict_mask);
       zv[j * kTopoCap + a] = allowed | ((r.present && !r.complement) ? 1u << 16 : 0) | (r.present ? 1u << 17 : 0);
@@ -2842,6 +2841,64 @@ __device__ void vt_build_block(int b) {
   }
 }
 
+// ---- run records: class cls's relation tables for class_run, from the class's topology relations and the catalog alone.
+// A class is eligible (ok) when every relation constrains, none records through a TopologyNodeFilter, a topology class has
+// one template, and the relations fit the tables: at most kRunHost hostname relations (spread or anti-affinity), at most
+// kRunMask spread relations over distinct mask keys with fewer than kRunDom domains and no inverse record. Whether each
+// relation's group exists and counts every slot (relaxation) changes during a Solve: class_run checks it at entry.
+// One thread per class; an ineligible class's record is all 0 but ok.
+__device__ __noinline__ void run_rec_build(unsigned cls) {
+  KS_K2
+  const ksched_pod_row& row = s.classes[cls];
+  RunRec r = {};
+  int ok = row.topo_begin == row.topo_end || c.n_templates == 1;
+  for (uint32_t e = row.topo_begin; e < row.topo_end && ok; ++e) {
+    const RelX x = s.relx[e];
+    if (!(x.flags & KSCHED_TOPO_CONSTRAINS)) { ok = 0; break; }            // record-only relations: generic step
+    if ((x.flags & KSCHED_TOPO_RECORDS) && x.has_filter) { ok = 0; break; }  // TopologyNodeFilter: generic step
+    const int times = ((x.flags & KSCHED_TOPO_RECORDS) ? 1 : 0) + ((x.flags & KSCHED_TOPO_RECORDS_INVERSE) ? 1 : 0);
+    const int self = (x.flags & KSCHED_TOPO_SELECTS) ? 1 : 0;
+    if (x.key == KSCHED_KEY_HOSTNAME) {
+      if (x.type == 1 || r.n_host == kRunHost) { ok = 0; break; }
+      const int j = r.n_host++;
+      r.h_row[j] = x.host_row; r.h_group[j] = (int)x.group; r.h_times[j] = (uint8_t)times;
+      // spread: count + self <= maxSkew (min is 0 for hostnames, topologygroup.go:186-188); anti-affinity: count == 0
+      const long long lim = x.type == 0 ? (long long)x.max_skew - self : 0;
+      r.h_lim[j] = lim > 0x10000 ? 0x10000 : (lim < -1 ? -1 : (int)lim);
+    } else {
+      const int k = x.key;
+      const uint64_t dict = c.keys[k].dict_mask;
+      if (x.type != 0 || r.n_mask == kRunMask || (x.flags & KSCHED_TOPO_RECORDS_INVERSE) || (dict >> kRunDom)) { ok = 0; break; }
+      static_assert(kRunMask == 2, "one earlier mask key to compare");
+      if (r.n_mask == 1 && r.m_key[0] == k) { ok = 0; break; }
+      const int j = r.n_mask++;
+      r.m_group[j] = (int)x.group; r.m_skew[j] = x.max_skew; r.m_key[j] = (uint8_t)k;
+      r.m_self[j] = (uint8_t)self; r.m_rec[j] = (x.flags & KSCHED_TOPO_RECORDS) ? 1 : 0;
+      r.m_wk[j] = c.keys[k].well_known != 0; r.m_neutral[j] = (uint32_t)c.pin_neutral[k]; r.m_dict[j] = (uint32_t)dict;
+      const Req tr = ksched::req_load(c.templates[0].reqs, nullptr, k);
+      r.m_tallow[j] = (uint32_t)(tr.present ? ksched::req_allowed(tr, dict, key_meta(c, k)) : dict);
+    }
+  }
+  if (!ok) r = RunRec{};
+  r.ok = ok;
+  uint4* dst = reinterpret_cast<uint4*>(&s.run_rec[cls]);
+  const uint4* src = reinterpret_cast<const uint4*>(&r);
+#pragma unroll
+  for (int w = 0; w < (int)(sizeof(RunRec) / 16); ++w) dst[w] = src[w];
+}
+
+// block b of the row gather's launch past the gather itself: the variant table's entries first, then the run records
+__device__ void k0_extra_block(int b) {
+  KS_K2
+  const int vt_blocks = s.vt_classes * s.vt_ndom;
+  if (b < vt_blocks) {
+    vt_build_block(b);
+    return;
+  }
+  const int cls = (b - vt_blocks) * blockDim.x + threadIdx.x;
+  if (cls < s.rec_classes) run_rec_build((unsigned)cls);
+}
+
 __device__ __noinline__ void class_run(const PodRegs& first_in) {
   KS_K2
   RunCtx& rc = g_rc;
@@ -2869,7 +2926,6 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
   const bool topo = first_in.topo_begin != first_in.topo_end;
   const bool plain = plain_pod_regs(first_in);
   const bool simple = !topo;
-  const uint32_t topo_begin = first_in.topo_begin, topo_end = first_in.topo_end;
   const bool resume = io.resume;
   const int qi0 = resume ? io.r_qi0 : io.qi, seq0 = resume ? io.r_seq0 : io.seq;
   int qi = io.qi, qlen = io.qlen, tick = io.tick, n_active = io.n_active, n_new = io.n_new, parity = io.parity;
@@ -2879,58 +2935,8 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
   const bool new_cls = rc.cls != cls;  // read BEFORE the barrier: thread 0 rewrites rc.cls right after it (racecheck, round 2)
   __syncthreads();  // everybody has read g_rio; earlier readers of g_rc are done
 
-  // ---- relation tables (once per class)
-  if (new_cls) {
-    if (tid == 0) {
-      rc.cls = cls;
-      rc.n_var = 0; rc.var_next = 0; rc.n_host = 0; rc.n_mask = 0;
-      int ok = 1;
-      if (topo) {
-        if (c.n_templates != 1) ok = 0;
-        for (uint32_t e = topo_begin; e < topo_end && ok; ++e) {
-          const RelX x = s.relx[e];
-          const int g = (int)x.group;
-          if (!(x.flags & KSCHED_TOPO_CONSTRAINS)) { ok = 0; break; }            // record-only relations: generic step
-          if (!s.grp_active[g] || s.grp_min_slot[g] != 0) { ok = 0; break; }      // relaxation-created groups: generic step
-          if ((x.flags & KSCHED_TOPO_RECORDS) && x.has_filter) { ok = 0; break; }  // TopologyNodeFilter: generic step
-          const int times = ((x.flags & KSCHED_TOPO_RECORDS) ? 1 : 0) + ((x.flags & KSCHED_TOPO_RECORDS_INVERSE) ? 1 : 0);
-          const int self = (x.flags & KSCHED_TOPO_SELECTS) ? 1 : 0;
-          if (x.key == KSCHED_KEY_HOSTNAME) {
-            if (x.type == 1 || rc.n_host == kRunHost) { ok = 0; break; }
-            const int j = rc.n_host++;
-            rc.h_row[j] = x.host_row; rc.h_group[j] = g; rc.h_times[j] = (uint8_t)times;
-            // spread: count + self <= maxSkew (min is 0 for hostnames, topologygroup.go:186-188); anti-affinity: count == 0
-            long long lim = x.type == 0 ? (long long)x.max_skew - self : 0;
-            rc.h_lim[j] = lim > 0x10000 ? 0x10000 : (lim < -1 ? -1 : (int)lim);
-          } else {
-            const int k = x.key;
-            if (x.type != 0 || rc.n_mask == kRunMask || (x.flags & KSCHED_TOPO_RECORDS_INVERSE) || (c.keys[k].dict_mask >> kRunDom)) { ok = 0; break; }
-            for (int i = 0; i < rc.n_mask; ++i) if (rc.m_key[i] == k) ok = 0;
-            if (!ok) break;
-            const int j = rc.n_mask++;
-            rc.m_group[j] = g; rc.m_skew[j] = x.max_skew; rc.m_key[j] = (uint8_t)k;
-            rc.m_self[j] = (uint8_t)self; rc.m_rec[j] = (x.flags & KSCHED_TOPO_RECORDS) ? 1 : 0;
-            rc.m_wk[j] = c.keys[k].well_known != 0; rc.m_neutral[j] = (uint32_t)c.pin_neutral[k];
-            const Req tr = ksched::req_load(c.templates[0].reqs, nullptr, k);
-            rc.m_tallow[j] = (uint32_t)(tr.present ? ksched::req_allowed(tr, c.keys[k].dict_mask, key_meta(c, k)) : c.keys[k].dict_mask);
-          }
-        }
-      }
-      rc.eligible = ok;
-    }
-    __syncthreads();
-  }
-  if (!rc.eligible || (topo && n_active > kTopoCap)) {
-    if (tid == 0) { io.status = rc.eligible ? 1 : 2; io.placed = 0; io.parity = parity; }
-#ifdef KSCHED_PROFILE_PACK
-    if (tid == 0 && rc.eligible) s.counters[kCtrStopCapacity] += 1;
-#endif
-    __syncthreads();
-    return;
-  }
-  const int n_host = rc.n_host, n_mask = rc.n_mask;
-
-  // ---- queue staging: the next CH (pod, class) entries; the chunk after them is fetched into registers meanwhile
+  // ---- queue staging: the next CH (pod, class) entries; the chunk after them is fetched into registers meanwhile. Issued
+  // first: its loads do not depend on the class's record.
   const ksched_pod_row* ffd_rows = reinterpret_cast<const ksched_pod_row*>(s.rows);
   int cb = resume ? io.r_cb : qi, buf = resume ? io.r_buf : 0;
   uint32_t nx_pod = 0, nx_cls = KSCHED_NONE;
@@ -2950,19 +2956,63 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
     const bool in = idx < s.n_pods;
     stage(0, in ? s.order[idx] : 0, in ? (uint32_t)ffd_rows[idx].reserved : KSCHED_NONE);
   }
-  // ---- per-run state: spread counters (one copy per warp), per-node inputs (each thread fills the slots it owns). A run
-  // that resumes has them in shared memory as it left them.
-  if (tid == 0 && !resume) rc.tomb = 0;
-  if (tid < kRunHost && !resume) rc.h_inc[tid] = 0;
-  if (topo && !resume) {
-    for (int j = 0; j < n_mask; ++j) {
-      if (lane < kRunDom) rc.cnt[warp][j][lane] = s.grp_cnt[(size_t)rc.m_group[j] * 64 + lane];
-      if (tid == 0) rc.m_registered[j] = (uint32_t)s.grp_registered[rc.m_group[j]];
+  // ---- relation tables: the class's record (run_rec_build) and the group state it is checked against. Every warp loads the
+  // record, one word per lane, so that its copy of the spread counters needs no barrier; warp 0 keeps it in rc.rec and
+  // decides eligibility from its lanes' loads of the groups: a relaxation-created group that does not exist yet, or that
+  // never registered some slots, sends the class to the generic step. A run that resumes has all of it as it left it.
+  constexpr int kWHGroup = offsetof(RunRec, h_group) / 4, kWMGroup = offsetof(RunRec, m_group) / 4;
+  static_assert(offsetof(RunRec, ok) == 0 && offsetof(RunRec, n_host) == 4 && offsetof(RunRec, n_mask) == 8, "RunRec's first words");
+  if (!resume) {
+    const uint32_t rw = reinterpret_cast<const uint32_t*>(s.run_rec + cls)[lane];
+    const int r_ok = __shfl_sync(0xffffffffu, rw, 0), r_nh = __shfl_sync(0xffffffffu, rw, 1), r_nm = __shfl_sync(0xffffffffu, rw, 2);
+    const int hg = (int)__shfl_sync(0xffffffffu, rw, kWHGroup + (lane & 3)), mg = (int)__shfl_sync(0xffffffffu, rw, kWMGroup + (lane & 1));
+    for (int j = 0; j < r_nm; ++j) {
+      const int g = __shfl_sync(0xffffffffu, mg, j);
+      if (lane < kRunDom) rc.cnt[warp][j][lane] = s.grp_cnt[(size_t)g * 64 + lane];
+    }
+    if (warp == 0) {
+      reinterpret_cast<uint32_t*>(&rc.rec)[lane] = rw;
+      const bool host = lane < kRunHost && lane < r_nh, mask = lane >= kRunHost && lane - kRunHost < r_nm;  // lane 4 + j: mask relation j
+      const int g = host ? hg : mg;
+      bool bad = false, zero = false;
+      if (host || mask) {
+        const uint8_t act = s.grp_active[g];
+        const int32_t ms = s.grp_min_slot[g];
+        const int32_t tot = host ? s.grp_host_total[g] : 1;
+        const uint64_t reg = mask ? s.grp_registered[g] : 0;
+        bad = !act || ms != 0;
+        zero = host && tot == 0;
+        if (mask) rc.m_registered[lane - kRunHost] = (uint32_t)reg;
+      }
+      const unsigned nbad = __ballot_sync(0xffffffffu, bad), nzero = __ballot_sync(0xffffffffu, zero);
+      if (lane == 0) {
+        rc.eligible = r_ok && !nbad;
+        rc.h_zero = (int)nzero;
+        if (new_cls) { rc.cls = cls; rc.n_var = 0; rc.var_next = 0; }
+      }
     }
   }
+
+  if (tid == 0 && !resume) rc.tomb = 0;
+  if (tid < kRunHost && !resume) rc.h_inc[tid] = 0;
+  __syncthreads();  // rc.rec, rc.eligible, rc.h_zero, rc.m_registered and the spread counters are in place
+  if (!rc.eligible || (topo && n_active > kTopoCap)) {
+    if (tid == 0) { io.status = rc.eligible ? 1 : 2; io.placed = 0; io.parity = parity; }
+#ifdef KSCHED_PROFILE_PACK
+    if (tid == 0 && rc.eligible) s.counters[kCtrStopCapacity] += 1;
+#endif
+    __syncthreads();
+    return;
+  }
+  const int n_host = rc.rec.n_host, n_mask = rc.rec.n_mask;
+
+  // ---- per-node inputs (each thread fills the slots it owns), every global load of a slot issued at once: the mask keys'
+  // values are loaded whatever nn_meta says and masked afterwards, a hostname relation whose group counted no slot at entry
+  // (grp_host_total 0) has the count 0 on every slot. A run that resumes has them in shared memory as it left them.
 #ifdef KSCHED_PROFILE_PACK
   const long long cr_in0 = clock64();
 #endif
+  const int h_zero = rc.h_zero;
   for (int a = tid; a < (resume ? 0 : n_active); a += T) {
     const unsigned short fl = hs->flags[a];
     unsigned rm;
@@ -2972,16 +3022,21 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
     else rm = run_room(hs, a, p_req, p_res, RH);
     if (topo) {
       const int n = hs->node[a];
-      for (int j = 0; j < n_host; ++j) {
-        const uint16_t v = s.grp_host[(size_t)rc.h_row[j] * hstride + NE + n];
-        hc[j * kTopoCap + a] = v;
-        if ((int)v > rc.h_lim[j]) rm |= kRpDead;
-      }
       const uint64_t meta = s.nn_meta[n];
-      for (int j = 0; j < n_mask; ++j) {
-        const int k = rc.m_key[j];
-        const Req r = load_soa(s.nn_vals, meta, MAXN, n, k);
-        const uint32_t allowed = (uint32_t)(r.present ? ksched::req_allowed(r, c.keys[k].dict_mask, key_meta(c, k)) : c.keys[k].dict_mask);
+      uint64_t mval[kRunMask];
+#pragma unroll
+      for (int j = 0; j < kRunMask; ++j) mval[j] = j < n_mask ? s.nn_vals[(size_t)rc.rec.m_key[j] * MAXN + n] : 0;
+      for (int j = 0; j < n_host; ++j) {
+        const uint16_t v = ((h_zero >> j) & 1) ? 0 : s.grp_host[(size_t)rc.rec.h_row[j] * hstride + NE + n];
+        hc[j * kTopoCap + a] = v;
+        if ((int)v > rc.rec.h_lim[j]) rm |= kRpDead;
+      }
+#pragma unroll
+      for (int j = 0; j < kRunMask; ++j) {
+        if (j >= n_mask) break;
+        const int k = rc.rec.m_key[j];
+        const Req r = soa_req(mval[j], meta, k);
+        const uint32_t allowed = r.present ? (uint32_t)ksched::req_allowed(r, rc.rec.m_dict[j], key_meta(c, k)) : rc.rec.m_dict[j];
         zv[j * kTopoCap + a] = allowed | ((r.present && !r.complement) ? 1u << 16 : 0) | (r.present ? 1u << 17 : 0);
       }
     }
@@ -3004,8 +3059,8 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
 #pragma unroll
   for (int r = 0; r < kHotRes; ++r) { e.p_req[r] = p_req[r]; e.min_req[r] = r < RH ? s.min_req[r] : 0; }
   e.m_reg0 = n_mask > 0 ? rc.m_registered[0] : 0; e.m_reg1 = n_mask > 1 ? rc.m_registered[1] : 0;
-  e.m_bias0 = n_mask > 0 ? (int)rc.m_self[0] - rc.m_skew[0] : 0; e.m_bias1 = n_mask > 1 ? (int)rc.m_self[1] - rc.m_skew[1] : 0;
-  e.m_rec0 = n_mask > 0 && rc.m_rec[0]; e.m_rec1 = n_mask > 1 && rc.m_rec[1];
+  e.m_bias0 = n_mask > 0 ? (int)rc.rec.m_self[0] - rc.rec.m_skew[0] : 0; e.m_bias1 = n_mask > 1 ? (int)rc.rec.m_self[1] - rc.rec.m_skew[1] : 0;
+  e.m_rec0 = n_mask > 0 && rc.rec.m_rec[0]; e.m_rec1 = n_mask > 1 && rc.rec.m_rec[1];
   int status = 0;
   int why = kStopNone;  // StopCause of a status-1 stop
   // a stop for want of a variant ends the call with status 3 (the variant is derived and the run resumes, see RunIO::resume),
@@ -3149,17 +3204,17 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
     s.nn_count[n] = (int)(key >> 32);
     s.nn_tb[n] = (int)((unsigned)key ^ 0x80000000u);
     for (int j = 0; j < n_host; ++j) {
-      const int times = rc.h_times[j];
+      const int times = rc.rec.h_times[j];
       if (!times) continue;
       const int now = hc[j * kTopoCap + a];
-      s.grp_host[(size_t)rc.h_row[j] * hstride + NE + n] = (uint16_t)now;
+      s.grp_host[(size_t)rc.rec.h_row[j] * hstride + NE + n] = (uint16_t)now;
       if (now - placed * times == 0) atomicAdd(&rc.h_inc[j], 1);  // the hostname's first matching pod (not saturated: counts <= pods per node)
     }
   }
   for (int j = 0; j < n_mask; ++j)
-    if (rc.m_rec[j] && warp == 0 && lane < kRunDom && ((rc.m_registered[j] >> lane) & 1)) s.grp_cnt[(size_t)rc.m_group[j] * 64 + lane] = rc.cnt[0][j][lane];
+    if (rc.rec.m_rec[j] && warp == 0 && lane < kRunDom && ((rc.m_registered[j] >> lane) & 1)) s.grp_cnt[(size_t)rc.rec.m_group[j] * 64 + lane] = rc.cnt[0][j][lane];
   __syncthreads();
-  if (tid < n_host && rc.h_inc[tid]) s.grp_host_total[rc.h_group[tid]] += rc.h_inc[tid];
+  if (tid < n_host && rc.h_inc[tid]) s.grp_host_total[rc.rec.h_group[tid]] += rc.h_inc[tid];
 #ifdef KSCHED_PROFILE_PACK
   const long long cr_t2 = clock64();
   const int cr_slots = rc.tomb > 0 ? n_active : 0;  // slots the compaction scans
@@ -3208,6 +3263,17 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
     if (status == 1 && why != kStopNone) s.counters[kCtrNoVariantStops + why - 1] += 1;
   }
 #endif
+  // the pack loop's next steps load the next entry's pod row and, for the next class run, its record: into L2 now (the
+  // entry's class is staged, or thread 0 holds it when the staged chunk is consumed)
+  if (qlen > 0 && qi < s.n_pods && tid < 3) {
+    if (tid == 0) {
+      const int i = qi - cb;
+      const uint32_t nc = i < CH ? rc.q_cls[buf][i] : (i == CH ? nx_cls : KSCHED_NONE);
+      if (nc < (uint32_t)s.rec_classes) prefetch_l2(s.run_rec + nc);
+    } else {
+      prefetch_l2(reinterpret_cast<const char*>(ffd_rows + qi) + (tid - 1) * 128);
+    }
+  }
   if (tid == 0) {
     const int qcap = s.n_pods + 1;
     io.qi = qi; io.head = (io.head + placed_total) % qcap; io.qlen = qlen; io.tick = tick; io.seq = seq0 + placed_total; io.n_active = n_active; io.n_new = n_new; io.parity = parity;
@@ -3319,7 +3385,7 @@ __global__ void __launch_bounds__(kMaxThreads, 1) pack_kernel() {
     PK_T(0)
     // ---- class-run mode (see class_run): first-pass pods of a class whose accept test is exact from shared memory
     bool skip_run = true;
-    if (fast_allowed && s.use_class_run && qi < s.n_pods && n_active <= kActCap) {
+    if (fast_allowed && s.use_class_run && s.rec_classes > 0 && qi < s.n_pods && n_active <= kActCap) {  // (a run reads the class's record)
       const bool topo_cls = nxt.topo_begin != nxt.topo_end;
       // (host-port classes never get here)
       // (with the instance-type slot state, PackState::nn_it, only the generic step writes it: instance-type classes stay there)

@@ -33,6 +33,23 @@ struct RunVariant {
   uint8_t dom[kRunMask];  // domain each spread relation pinned
 };
 
+// a class run's relation tables for one class (pack_kernel.cuh: run_rec_build): what class_run's entry needs of the class's
+// topology relations that depends on the class and the catalog alone, built before the pack kernel. 128 bytes, one word
+// per lane: a warp copies it with one coalesced load.
+constexpr int kRunHost = 4;
+struct alignas(16) RunRec {
+  int32_t ok;                 // the class's relations pass the run's static checks (the group state is checked at entry)
+  int32_t n_host, n_mask;
+  int32_t h_row[kRunHost], h_group[kRunHost], h_lim[kRunHost];  // h_lim: largest count of the group on a node that still admits the pod
+  int32_t m_group[kRunMask], m_skew[kRunMask];
+  uint32_t m_neutral[kRunMask], m_tallow[kRunMask], m_dict[kRunMask];  // m_dict: the key's dictionary mask
+  uint8_t h_times[kRunHost];
+  uint8_t m_key[kRunMask], m_self[kRunMask], m_rec[kRunMask], m_wk[kRunMask];
+  uint32_t pad[4];
+};
+static_assert(sizeof(RunRec) == 128 && offsetof(RunRec, h_times) == 100 && offsetof(RunRec, pad) == 112,
+              "RunRec is one word per lane (and karpenter-core_b200/__init__.py: ResidentSolve.RUN_REC_DTYPE)");
+
 struct PackState {
   const RelX* relx;                  // [n_class_topo], parallel to class_topo
   // problem (read-only)
@@ -138,6 +155,8 @@ struct PackState {
   uint32_t* vt_ok;                   // [vt_classes][kM1Dom] 1: the entry holds a variant
   int vt_classes;                    // classes the table covers in this launch (0: no table; KSCHED_NO_VARSTORE=1 turns it off)
   int vt_ndom;                       // domain ids the table covers (below kM1Dom; the build has vt_classes * vt_ndom blocks)
+  RunRec* run_rec;                   // [n_classes] class runs' relation tables (pack_kernel.cuh: run_rec_build)
+  int rec_classes;                   // classes the row gather's launch builds records for: n_classes when class runs can run, else 0
   // topology counters
   int32_t* grp_cnt;                  // [n_groups][64]
   uint64_t* grp_registered;          // [n_groups]
@@ -194,6 +213,17 @@ __device__ __forceinline__ Req load_soa(const uint64_t* vals, uint64_t meta, int
   r.has_gt = r.has_lt = false;
   r.gt = r.lt = 0;
   r.values = r.present ? vals[(size_t)k * stride + idx] : 0;
+  return r;
+}
+// load_soa from a value loaded without waiting for meta (vals[k * stride + idx] whatever meta says): the value load need
+// not follow the meta load
+__device__ __forceinline__ Req soa_req(uint64_t value, uint64_t meta, int k) {
+  Req r;
+  r.present = (meta >> (KSCHED_META_PRESENT_SHIFT + k)) & 1;
+  r.complement = (meta >> (KSCHED_META_COMPLEMENT_SHIFT + k)) & 1;
+  r.has_gt = r.has_lt = false;
+  r.gt = r.lt = 0;
+  r.values = r.present ? value : 0;
   return r;
 }
 

@@ -40,6 +40,7 @@ struct kh_context {
 };
 
 int ksched_k1_plan(const ksched_handle* h, int out[5]);  // csrc/ksched.cu, outside the C-ABI
+int ksched_run_records(ksched_handle* h, void* out, int n);  // csrc/ksched.cu, outside the C-ABI
 
 namespace {
 
@@ -571,6 +572,12 @@ int kh_gpu_timings(ksched_timings* t) {
 int kh_gpu_k1_plan(int* out) {
   Lock lock(g_default.mu);
   return g_default.h ? ksched_k1_plan(g_default.h, out) : fail(KSCHED_ERR_INVALID, "no handle");
+}
+int kh_gpu_run_records(void* out, int n) {
+  Lock lock(g_default.mu);
+  if (!g_default.h) return fail(KSCHED_ERR_INVALID, "no handle");
+  if (g_gpu_encoded && !gpu_current()) return fail(KSCHED_ERR_INVALID, "the handle was used for other work since this problem's run: run it again");
+  return ksched_run_records(g_default.h, out, n);
 }
 int kh_gpu_set_shard(int rank, int world) {
   Lock lock(g_default.mu);

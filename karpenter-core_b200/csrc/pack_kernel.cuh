@@ -1486,10 +1486,22 @@ __device__ __forceinline__ bool run_closes(const HotSmem* hs, int a, uint32_t rp
   return node_closed(nq, min_req, RH, b1, b2, hs->flags[a]);
 }
 
+// A slot's domain word for one mask relation, from the node's requirement r on key k (dictionary mask dict): bits 0..15
+// the domains r admits, kZvExact when r is an In, kZvPresent when the node has a requirement on the key
+constexpr uint32_t kZvExact = 1u << 16, kZvPresent = 1u << 17;
+__device__ __forceinline__ uint32_t zv_word(const Req& r, uint32_t dict, int k) {
+  KS_K2
+  const uint32_t allowed = r.present ? (uint32_t)ksched::req_allowed(r, dict, key_meta(c, k)) : dict;
+  return allowed | ((r.present && !r.complement) ? kZvExact : 0) | (r.present ? kZvPresent : 0);
+}
+// the word of a node pinned to domain d (requirements.Add(In{d})): a node is pinned to one domain exactly when its word
+// has this form
+__device__ __forceinline__ uint32_t zv_pinned(int d) { return (1u << d) | kZvExact | kZvPresent; }
+
 // The class run's constants for one call, shared by its steps (all inlined into class_run)
 struct RunEnv {
   HotSmem* hs;
-  uint32_t* zv;   // [kRunMask][kTopoCap] bits 0..15 admitted domains, 16 exact (In), 17 present
+  uint32_t* zv;   // [kRunMask][kTopoCap] domain words (zv_word)
   uint32_t* rpv;  // [kActCap] room | placed << 16 | dead
   uint16_t* hc;   // [kRunHost][kTopoCap] the hostname groups' counts
   int NE, MAXN, W32, RH, hstride, n_host, n_mask;
@@ -1545,7 +1557,7 @@ __device__ __forceinline__ void run_fresh(const RunEnv& e, const RunVariant& v, 
 __device__ __forceinline__ void run_pin(const RunEnv& e, int j, int a, int d) {
   KS_K2
   const int n = e.hs->node[a], k = g_rc.rec.m_key[j];
-  e.zv[j * kTopoCap + a] = (1u << d) | (3u << 16);
+  e.zv[j * kTopoCap + a] = zv_pinned(d);
   s.nn_vals[(size_t)k * e.MAXN + n] = 1ull << d;
   atomicOr(reinterpret_cast<unsigned long long*>(&s.nn_meta[n]), 1ull << (KSCHED_META_PRESENT_SHIFT + k));
   atomicAnd(reinterpret_cast<unsigned long long*>(&s.nn_meta[n]), ~(1ull << (KSCHED_META_COMPLEMENT_SHIFT + k)));
@@ -1604,7 +1616,7 @@ __device__ __forceinline__ bool m1_build(const RunEnv& e, int n_active) {
       const uint32_t z = e.zv[a], adm = z & 0xFFFF;
       const unsigned cn = (unsigned)(hs->key[a] >> 32);
       int list = -1;
-      if (adm && !(adm & (adm - 1)) && (z & (1u << 16))) {  // pinned to one domain
+      if (adm && !(adm & (adm - 1)) && (z & kZvExact)) {  // pinned to one domain
         if (adm & e.m_reg0) list = __ffs(adm) - 1;           // (a domain that is not registered never admits a pod)
       } else if ((adm & e.m_reg0) == e.m_reg0) list = kM1Dom;  // admits every registered domain
       else if (adm & e.m_reg0) m1.bad = 1;                    // some of them: per-pod loop
@@ -1789,7 +1801,7 @@ __device__ __forceinline__ uint32_t m1_commit(const RunEnv& e, int buf, int a, u
 __device__ __forceinline__ void m1_fresh(const RunEnv& e, int buf, int vi, int a, int n, int tb, int q, int d, int f) {
   run_fresh(e, g_rc.var[vi], a, n, tb);
   g_rc.q_node[buf][q] = e.NE + n;
-  e.zv[a] = (1u << d) | (3u << 16);
+  e.zv[a] = zv_pinned(d);
   g_m1.fr[f] = (uint32_t)a | ((uint32_t)vi << 16);
 }
 
@@ -2066,7 +2078,7 @@ __device__ __forceinline__ int m1_pin_step(const RunEnv& e, int buf, M1Lane& l, 
   }
   const bool same_c = (int)(k_t >> 32) == c, below = k_t < pmin;
   const bool ok_t = in && same_c && below && (rp_t & 0xFFFF) != kRoomSlow && c + 1 < kM1Lv &&
-                    ((rc.rec.m_neutral[0] >> d_t) & 1) && ((z_t & (1u << 17)) || rc.rec.m_wk[0]);
+                    ((rc.rec.m_neutral[0] >> d_t) & 1) && ((z_t & kZvPresent) || rc.rec.m_wk[0]);
   const unsigned okb = __ballot_sync(kFull, ok_t);
   const int J = okb == kFull ? 32 : __ffs(~okb) - 1;
 #ifdef KSCHED_PROFILE_PACK
@@ -2122,7 +2134,7 @@ __device__ __forceinline__ int m1_single(const RunEnv& e, int buf, M1Lane& l, M1
   const bool pin = wl == kM1Dom;
   if (pin) {  // the placement pins the node's domain: fewest pods, lowest id among the admissible ones (run_pick)
     d = warp_pick(allowed, w.cnt_d);
-    if (!((rc.rec.m_neutral[0] >> d) & 1) || !((e.zv[a] & (1u << 17)) || rc.rec.m_wk[0])) { why = kStopOther; return 1; }
+    if (!((rc.rec.m_neutral[0] >> d) & 1) || !((e.zv[a] & kZvPresent) || rc.rec.m_wk[0])) { why = kStopOther; return 1; }
 #ifdef KSCHED_PROFILE_PACK
     if (L == 0) s.counters[kCtrMaskUnpinnedSingle] += 1;
 #endif
@@ -2471,11 +2483,11 @@ __device__ __forceinline__ int run_argmin_step(const RunEnv& e, int buf, int i, 
       if (j >= n_mask) break;
       const uint32_t z = j ? best_z1 : best_z0, cand = z & (j ? okm1 : okm0);
       int d;
-      if (!(z & 0xFFFF & ((z & 0xFFFF) - 1)) && (z & (1u << 16))) d = __ffs(cand) - 1;  // pinned already
+      if (!(z & 0xFFFF & ((z & 0xFFFF) - 1)) && (z & kZvExact)) d = __ffs(cand) - 1;  // pinned already
       else {  // the placement pins the node's domain
         d = run_pick(cand, rc.cnt[warp][j]);
         pay |= 1u << (13 + j);
-        if (!((rc.rec.m_neutral[j] >> d) & 1) || !((z & (1u << 17)) || rc.rec.m_wk[j])) pay |= 1u << 11;
+        if (!((rc.rec.m_neutral[j] >> d) & 1) || !((z & kZvPresent) || rc.rec.m_wk[j])) pay |= 1u << 11;
       }
       pay |= (unsigned)d << (15 + 4 * j);
     }
@@ -2583,8 +2595,8 @@ __device__ __forceinline__ bool run_fresh_step(const RunEnv& e, int buf, int i, 
     const int tk = tick + j * m;                          // tick of its first pod
     run_fresh(e, v, a, n, tk + 1);
     open_node(s, n, v.fl >> 8, v.meta, v.qp, 0, false, 0, KSCHED_NONE, true, tk + 1);
-    if (n_mask > 0) e.zv[a] = (1u << fd0) | (3u << 16);
-    if (n_mask > 1) e.zv[kTopoCap + a] = (1u << fd1) | (3u << 16);
+    if (n_mask > 0) e.zv[a] = zv_pinned(fd0);
+    if (n_mask > 1) e.zv[kTopoCap + a] = zv_pinned(fd1);
     // the fill's t further pods (the slot holds the variant's requests and front, and v.rp carries no placed pod)
     if (t > 0 && run_settle(e, a, run_record_host(rc, e.hc, e.n_host, a, v.rp, t), 1 + t, -(tk + 1 + t))) atomicAdd(&rc.tomb, 1);
   }
@@ -2617,7 +2629,7 @@ __device__ __forceinline__ int run_capture(const HotSmem* hs, const uint32_t* zv
   for (int j = 0; j < kRunMask; ++j) {
     if (j >= n_mask) continue;
     const uint32_t z = zv[j * kTopoCap + a], v = z & 0xFFFF;
-    if (!v || (v & (v - 1)) || !(z & (1u << 16))) ok = false;
+    if (!v || (v & (v - 1)) || !(z & kZvExact)) ok = false;
     else dom[j] = __ffs(v) - 1;
   }
   for (int i = 0; i < rc.n_var && ok; ++i) {
@@ -2679,9 +2691,7 @@ __device__ __noinline__ int run_derive(const PodRegs& first_in, int fpos, int n_
     const uint64_t meta = s.nn_meta[n];
     for (int j = 0; j < n_mask; ++j) {
       const int k = rc.rec.m_key[j];
-      const Req r = load_soa(s.nn_vals, meta, MAXN, n, k);
-      const uint32_t allowed = (uint32_t)(r.present ? ksched::req_allowed(r, c.keys[k].dict_mask, key_meta(c, k)) : c.keys[k].dict_mask);
-      zv[j * kTopoCap + a] = allowed | ((r.present && !r.complement) ? 1u << 16 : 0) | (r.present ? 1u << 17 : 0);
+      zv[j * kTopoCap + a] = zv_word(load_soa(s.nn_vals, meta, MAXN, n, k), (uint32_t)c.keys[k].dict_mask, k);
     }
   }
   __syncthreads();
@@ -2702,13 +2712,58 @@ __device__ __forceinline__ bool run_derive_at(const PodRegs& first_in, int fpos,
   return vi >= 0;
 }
 
+// ---- run records: class cls's relation tables for class_run, from the class's topology relations and the catalog alone.
+// A class is eligible (ok) when every relation constrains, none records through a TopologyNodeFilter, a topology class has
+// one template, and the relations fit the tables: at most kRunHost hostname relations (spread or anti-affinity), at most
+// kRunMask spread relations over distinct mask keys with fewer than kRunDom domains and no inverse record. Whether each
+// relation's group exists and counts every slot (relaxation) changes during a Solve: class_run checks it at entry.
+// An ineligible class's record is all 0. first_mask: the class_topo entry of its first mask relation (when n_mask > 0).
+__device__ __forceinline__ RunRec run_rec_of(unsigned cls, int& first_mask) {
+  KS_K2
+  const ksched_pod_row& row = s.classes[cls];
+  RunRec r = {};
+  first_mask = -1;
+  int ok = row.topo_begin == row.topo_end || c.n_templates == 1;
+  for (uint32_t e = row.topo_begin; e < row.topo_end && ok; ++e) {
+    const RelX x = s.relx[e];
+    if (!(x.flags & KSCHED_TOPO_CONSTRAINS)) { ok = 0; break; }            // record-only relations: generic step
+    if ((x.flags & KSCHED_TOPO_RECORDS) && x.has_filter) { ok = 0; break; }  // TopologyNodeFilter: generic step
+    const int times = ((x.flags & KSCHED_TOPO_RECORDS) ? 1 : 0) + ((x.flags & KSCHED_TOPO_RECORDS_INVERSE) ? 1 : 0);
+    const int self = (x.flags & KSCHED_TOPO_SELECTS) ? 1 : 0;
+    if (x.key == KSCHED_KEY_HOSTNAME) {
+      if (x.type == 1 || r.n_host == kRunHost) { ok = 0; break; }
+      const int j = r.n_host++;
+      r.h_row[j] = x.host_row; r.h_group[j] = (int)x.group; r.h_times[j] = (uint8_t)times;
+      // spread: count + self <= maxSkew (min is 0 for hostnames, topologygroup.go:186-188); anti-affinity: count == 0
+      const long long lim = x.type == 0 ? (long long)x.max_skew - self : 0;
+      r.h_lim[j] = lim > 0x10000 ? 0x10000 : (lim < -1 ? -1 : (int)lim);
+    } else {
+      const int k = x.key;
+      const uint64_t dict = c.keys[k].dict_mask;
+      if (x.type != 0 || r.n_mask == kRunMask || (x.flags & KSCHED_TOPO_RECORDS_INVERSE) || (dict >> kRunDom)) { ok = 0; break; }
+      static_assert(kRunMask == 2, "one earlier mask key to compare");
+      if (r.n_mask == 1 && r.m_key[0] == k) { ok = 0; break; }
+      if (r.n_mask == 0) first_mask = (int)e;
+      const int j = r.n_mask++;
+      r.m_group[j] = (int)x.group; r.m_skew[j] = x.max_skew; r.m_key[j] = (uint8_t)k;
+      r.m_self[j] = (uint8_t)self; r.m_rec[j] = (x.flags & KSCHED_TOPO_RECORDS) ? 1 : 0;
+      r.m_wk[j] = c.keys[k].well_known != 0; r.m_neutral[j] = (uint32_t)c.pin_neutral[k]; r.m_dict[j] = (uint32_t)dict;
+      const Req tr = ksched::req_load(c.templates[0].reqs, nullptr, k);
+      r.m_tallow[j] = (uint32_t)(tr.present ? ksched::req_allowed(tr, dict, key_meta(c, k)) : dict);
+    }
+  }
+  if (!ok) r = RunRec{};
+  r.ok = ok;
+  return r;
+}
+
 // ---- variant table, entry (cls, d): the generic step's NewNode + Add for the class's fresh node with its mask relation
 // pinned to domain d (templates in weight order, the first that opens a node), captured as run_capture captures it.
-// Block-wide, in a launch before the pack kernel; reads only what is fixed for the Solve. The guards are the derivation's
-// (no provisioner limit, W32 <= kRunW32) and the classes a shared variant used to need (no instance-type or hostname
-// requirement, no volumes, no ext resource), with at most one mask relation and the relation checks of class_run's table
-// that depend on the class alone. The entry is none when no template opens a node, the node closes at once or it is not
-// pinned to exactly d (the pod's own requirement excludes d).
+// Block-wide, in a launch before the pack kernel; reads only what is fixed for the Solve. Covered: an eligible run record
+// (run_rec_of) with at most one mask relation, whose group registers d (d == 0 without one), and no hostname limit below 0
+// (no pod goes on a fresh node then), plus the table's guards: no provisioner limit, W32 <= kRunW32, no instance-type or
+// hostname requirement, no volumes, no ext resource. The entry is none when no template opens a node, the node closes at
+// once or it is not pinned to exactly d (the pod's own requirement excludes d).
 __device__ void vt_build_entry(unsigned cls, int d) {
   KS_K2
   KS_PT
@@ -2718,46 +2773,28 @@ __device__ void vt_build_entry(unsigned cls, int d) {
   const int tid = threadIdx.x, W32 = c.W32, V = c.n_templates, NE = s.n_existing;
   const int RH = c.n_res < kHotRes ? c.n_res : kHotRes;
   const ksched_pod_row* src = s.classes + cls;
-  __shared__ int vt_go, vt_key, vt_nhost;
-  __shared__ uint8_t vt_times[kRunHost];
-  __shared__ int vt_lim[kRunHost];
+  __shared__ int vt_go;
+  __shared__ RunRec vt_rec;
   if (tid < 32) reinterpret_cast<uint64_t*>(&g_row)[tid] = reinterpret_cast<const uint64_t*>(src)[tid];
   if (tid == 0) {
-    const ksched_pod_row& r = *src;
-    bool ok = !s.any_limits && W32 <= kRunW32 && r.itype_req == KSCHED_NONE && r.hostname_req == KSCHED_NONE &&
-              !class_has_volumes(s, cls) && !class_ext(s, cls) && !(r.topo_begin != r.topo_end && V != 1);
-    int n_mask = 0, n_host = 0, key = -1;
-    for (uint32_t e = r.topo_begin; e < r.topo_end && ok; ++e) {
-      const RelX x = s.relx[e];
-      if (!(x.flags & KSCHED_TOPO_CONSTRAINS) || ((x.flags & KSCHED_TOPO_RECORDS) && x.has_filter)) { ok = false; break; }
-      const int times = ((x.flags & KSCHED_TOPO_RECORDS) ? 1 : 0) + ((x.flags & KSCHED_TOPO_RECORDS_INVERSE) ? 1 : 0);
-      const int self = (x.flags & KSCHED_TOPO_SELECTS) ? 1 : 0;
-      if (x.key == KSCHED_KEY_HOSTNAME) {
-        if (x.type == 1 || n_host == kRunHost) { ok = false; break; }
-        const long long lim = x.type == 0 ? (long long)x.max_skew - self : 0;
-        if (lim < 0) { ok = false; break; }  // the run places no pod on a fresh node then
-        vt_times[n_host] = (uint8_t)times;
-        vt_lim[n_host++] = lim > 0x10000 ? 0x10000 : (int)lim;
-      } else {
-        const int k = x.key;
-        if (x.type != 0 || n_mask == 1 || (x.flags & KSCHED_TOPO_RECORDS_INVERSE) || (c.keys[k].dict_mask >> kRunDom) ||
-            !((s.grp_registered[x.group] >> d) & 1)) { ok = false; break; }
-        // the pin: d is the one admissible domain in (count, id) order, so the node gets d exactly when it admits d
-        fill_pod_topo_static(x, pt, 0);
-        pt.registered[0] = s.grp_registered[x.group];
-        pt.n_sorted[0] = 1;
-        pt.sorted[0][0] = (uint8_t)d;
-        pt.min_slot[0] = 0;
-        n_mask = 1;
-        key = k;
-      }
-    }
-    // (a fresh node's hostname count is 0 on every hostname relation, which admits it by lim >= 0: only the mask relation pins)
-    pt.n = n_mask;
+    int e_mask;
+    vt_rec = run_rec_of(cls, e_mask);
+    bool ok = vt_rec.ok && vt_rec.n_mask <= 1 && !s.any_limits && W32 <= kRunW32 && src->itype_req == KSCHED_NONE &&
+              src->hostname_req == KSCHED_NONE && !class_has_volumes(s, cls) && !class_ext(s, cls);
+    for (int j = 0; j < vt_rec.n_host; ++j) ok = ok && vt_rec.h_lim[j] >= 0;
+    if (vt_rec.n_mask) {
+      const uint64_t reg = s.grp_registered[vt_rec.m_group[0]];
+      ok = ok && ((reg >> d) & 1);
+      // the pin: d is the one admissible domain in (count, id) order, so the node gets d exactly when it admits d
+      fill_pod_topo_static(s.relx[e_mask], pt, 0);
+      pt.registered[0] = reg;
+      pt.n_sorted[0] = 1;
+      pt.sorted[0][0] = (uint8_t)d;
+      pt.min_slot[0] = 0;
+    } else ok = ok && d == 0;
+    pt.n = vt_rec.n_mask;
     pt.overflow = 0;
-    vt_go = ok && (n_mask == 1 || d == 0);
-    vt_key = key;
-    vt_nhost = n_host;
+    vt_go = ok;
   }
   __syncthreads();
   const size_t idx = vt_index(cls, d);
@@ -2797,11 +2834,9 @@ __device__ void vt_build_entry(unsigned cls, int d) {
     if (tid == 0) {
       bool ok = !node_closed(sh.q, s.min_req, RH, sh.bound, sh.bound2, sh.front_bits);
       const uint64_t meta = sh.meta;
-      if (ok && vt_key >= 0) {  // pinned to exactly d (an In requirement of the one value)
-        const int k = vt_key;
-        const Req r = load_soa(out.vals, meta, 1, 0, k);
-        const uint64_t allowed = r.present ? ksched::req_allowed(r, c.keys[k].dict_mask, key_meta(c, k)) : c.keys[k].dict_mask;
-        ok = r.present && !r.complement && allowed == (1ull << d);
+      if (ok && vt_rec.n_mask) {
+        const int k = vt_rec.m_key[0];
+        ok = zv_word(load_soa(out.vals, meta, 1, 0, k), vt_rec.m_dict[0], k) == zv_pinned(d);
       }
       if (ok) {
         const unsigned short fl = (unsigned short)(sh.front_bits | ((sh.qp & 0xF) << 1) | (v << 8));
@@ -2812,8 +2847,8 @@ __device__ void vt_build_entry(unsigned cls, int d) {
         for (int r = 0; r < kHotRes; ++r) { out.b1[r] = sh.bound[r]; out.b2[r] = sh.bound2[r]; }
         out.qp = sh.qp;
         out.fl = fl;
-        out.rp = fresh_room_word(room_of(fl, sh.q, sh.bound, sh.bound2, p_req, p_res, RH), vt_nhost, vt_times, vt_lim);
-        out.dom[0] = (uint8_t)(vt_key >= 0 ? d : 0);
+        out.rp = fresh_room_word(room_of(fl, sh.q, sh.bound, sh.bound2, p_req, p_res, RH), vt_rec.n_host, vt_rec.h_times, vt_rec.h_lim);
+        out.dom[0] = (uint8_t)d;
         out.dom[1] = 0;
       }
       s.vt_ok[idx] = ok ? 1 : 0;
@@ -2841,50 +2876,11 @@ __device__ void vt_build_block(int b) {
   }
 }
 
-// ---- run records: class cls's relation tables for class_run, from the class's topology relations and the catalog alone.
-// A class is eligible (ok) when every relation constrains, none records through a TopologyNodeFilter, a topology class has
-// one template, and the relations fit the tables: at most kRunHost hostname relations (spread or anti-affinity), at most
-// kRunMask spread relations over distinct mask keys with fewer than kRunDom domains and no inverse record. Whether each
-// relation's group exists and counts every slot (relaxation) changes during a Solve: class_run checks it at entry.
-// One thread per class; an ineligible class's record is all 0 but ok.
+// the run records' build in the row gather's launch: one thread per class
 __device__ __noinline__ void run_rec_build(unsigned cls) {
   KS_K2
-  const ksched_pod_row& row = s.classes[cls];
-  RunRec r = {};
-  int ok = row.topo_begin == row.topo_end || c.n_templates == 1;
-  for (uint32_t e = row.topo_begin; e < row.topo_end && ok; ++e) {
-    const RelX x = s.relx[e];
-    if (!(x.flags & KSCHED_TOPO_CONSTRAINS)) { ok = 0; break; }            // record-only relations: generic step
-    if ((x.flags & KSCHED_TOPO_RECORDS) && x.has_filter) { ok = 0; break; }  // TopologyNodeFilter: generic step
-    const int times = ((x.flags & KSCHED_TOPO_RECORDS) ? 1 : 0) + ((x.flags & KSCHED_TOPO_RECORDS_INVERSE) ? 1 : 0);
-    const int self = (x.flags & KSCHED_TOPO_SELECTS) ? 1 : 0;
-    if (x.key == KSCHED_KEY_HOSTNAME) {
-      if (x.type == 1 || r.n_host == kRunHost) { ok = 0; break; }
-      const int j = r.n_host++;
-      r.h_row[j] = x.host_row; r.h_group[j] = (int)x.group; r.h_times[j] = (uint8_t)times;
-      // spread: count + self <= maxSkew (min is 0 for hostnames, topologygroup.go:186-188); anti-affinity: count == 0
-      const long long lim = x.type == 0 ? (long long)x.max_skew - self : 0;
-      r.h_lim[j] = lim > 0x10000 ? 0x10000 : (lim < -1 ? -1 : (int)lim);
-    } else {
-      const int k = x.key;
-      const uint64_t dict = c.keys[k].dict_mask;
-      if (x.type != 0 || r.n_mask == kRunMask || (x.flags & KSCHED_TOPO_RECORDS_INVERSE) || (dict >> kRunDom)) { ok = 0; break; }
-      static_assert(kRunMask == 2, "one earlier mask key to compare");
-      if (r.n_mask == 1 && r.m_key[0] == k) { ok = 0; break; }
-      const int j = r.n_mask++;
-      r.m_group[j] = (int)x.group; r.m_skew[j] = x.max_skew; r.m_key[j] = (uint8_t)k;
-      r.m_self[j] = (uint8_t)self; r.m_rec[j] = (x.flags & KSCHED_TOPO_RECORDS) ? 1 : 0;
-      r.m_wk[j] = c.keys[k].well_known != 0; r.m_neutral[j] = (uint32_t)c.pin_neutral[k]; r.m_dict[j] = (uint32_t)dict;
-      const Req tr = ksched::req_load(c.templates[0].reqs, nullptr, k);
-      r.m_tallow[j] = (uint32_t)(tr.present ? ksched::req_allowed(tr, dict, key_meta(c, k)) : dict);
-    }
-  }
-  if (!ok) r = RunRec{};
-  r.ok = ok;
-  uint4* dst = reinterpret_cast<uint4*>(&s.run_rec[cls]);
-  const uint4* src = reinterpret_cast<const uint4*>(&r);
-#pragma unroll
-  for (int w = 0; w < (int)(sizeof(RunRec) / 16); ++w) dst[w] = src[w];
+  int first_mask;
+  s.run_rec[cls] = run_rec_of(cls, first_mask);
 }
 
 // block b of the row gather's launch past the gather itself: the variant table's entries first, then the run records
@@ -2908,7 +2904,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
   if (threadIdx.x == 0) s.counters[kCtrRunActiveSum] += io.n_active;
 #endif
   HotSmem* hs = reinterpret_cast<HotSmem*>(dyn_smem);
-  uint32_t* zv = reinterpret_cast<uint32_t*>(dyn_smem + sizeof(HotSmem) + s.run_off);  // [kRunMask][kTopoCap] bits 0..15 admitted domains, 16 exact (In), 17 present
+  uint32_t* zv = reinterpret_cast<uint32_t*>(dyn_smem + sizeof(HotSmem) + s.run_off);  // [kRunMask][kTopoCap] domain words (zv_word)
   uint32_t* rpv = zv + (size_t)kRunMask * kTopoCap;                                      // [kActCap] room | placed << 16 | dead
   uint16_t* hc = reinterpret_cast<uint16_t*>(rpv + kActCap);                             // [kRunHost][kTopoCap]
   const uint32_t* tmpl_taintset = g_tmpl_taintset;
@@ -3035,9 +3031,7 @@ __device__ __noinline__ void class_run(const PodRegs& first_in) {
       for (int j = 0; j < kRunMask; ++j) {
         if (j >= n_mask) break;
         const int k = rc.rec.m_key[j];
-        const Req r = soa_req(mval[j], meta, k);
-        const uint32_t allowed = r.present ? (uint32_t)ksched::req_allowed(r, rc.rec.m_dict[j], key_meta(c, k)) : rc.rec.m_dict[j];
-        zv[j * kTopoCap + a] = allowed | ((r.present && !r.complement) ? 1u << 16 : 0) | (r.present ? 1u << 17 : 0);
+        zv[j * kTopoCap + a] = zv_word(soa_req(mval[j], meta, k), rc.rec.m_dict[j], k);
       }
     }
     rpv[a] = rm;

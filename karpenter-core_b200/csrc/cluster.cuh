@@ -73,33 +73,44 @@ __global__ void cluster_topology_kernel(int n_sup, const int32_t* __restrict__ p
   }
 }
 
-// What computeConsolidation reads of a simulation (consolidation.go:190-274): how many pods landed, how many nodes were
-// opened and, for the price guards, the first new node in full.
-struct SimResultDev {
-  int32_t n_pods, n_unscheduled, n_new_nodes, error;
-  int32_t template_index, pod_count;
-  uint32_t requests_present, pad;
-  int64_t requests[KSCHED_MAX_RES];
-  uint64_t values[KSCHED_MAX_KEYS];
-  uint64_t meta;
-};
-__global__ void cluster_collect_kernel(const long long* __restrict__ counters, int n_pods, const uint8_t* nn_tmpl, const int32_t* nn_count,
-                                       const int64_t* nn_req, const uint32_t* nn_req_present, const uint64_t* nn_vals, const uint64_t* nn_meta,
-                                       const uint32_t* nn_opts, int max_new, int W32, SimResultDev* out, uint32_t* out_types) {
-  const int tid = threadIdx.x;
-  if (tid == 0) {
-    out->n_pods = n_pods;
-    out->n_new_nodes = (int32_t)counters[kCtrNewNodes];
-    out->n_unscheduled = (int32_t)counters[kCtrUnscheduled];
-    out->error = (int32_t)counters[kCtrError];
-    out->template_index = nn_tmpl[0];
-    out->pod_count = nn_count[0];
-    out->requests_present = nn_req_present[0];
-    out->meta = nn_meta[0];
+// New node n's row and its W32 option words, gathered from the pack kernel's columns (PackState nn_*) by the threads
+// t = 0 .. nt-1 of a group together
+__device__ __forceinline__ void gather_new_node(const PackState& s, int W32, int n, int t, int nt, ksched_new_node* row, uint32_t* opts) {
+  const size_t mn = (size_t)s.max_new;
+  if (t == 0) {
+    const int32_t tmpl = s.nn_tmpl[n], count = s.nn_count[n];
+    const uint32_t present = s.nn_req_present[n];
+    const uint64_t meta = s.nn_meta[n];
+    row->template_index = tmpl;
+    row->pod_count = count;
+    row->requests_present = present;
+    row->pad = 0;
+    row->reqs.meta = meta;
   }
-  if (tid < KSCHED_MAX_RES) out->requests[tid] = nn_req[(size_t)tid * max_new];
-  if (tid < KSCHED_MAX_KEYS) out->values[tid] = nn_vals[(size_t)tid * max_new];
-  for (int w = tid; w < W32; w += blockDim.x) out_types[w] = nn_opts[(size_t)w * max_new];
+  for (int r = t; r < KSCHED_MAX_RES; r += nt) row->requests[r] = s.nn_req[r * mn + n];
+  for (int k = t; k < KSCHED_MAX_KEYS; k += nt) row->reqs.values[k] = s.nn_vals[k * mn + n];
+  for (int w = t; w < W32; w += nt) opts[w] = s.nn_opts[w * mn + n];
+}
+
+// What computeConsolidation reads of a simulation (consolidation.go:190-274): how many pods landed, how many nodes were
+// opened and, for the price guards, the first new node in full with its option words (W32 / 2 64-bit words), zeros when
+// no node was opened. One warp.
+__global__ void cluster_collect_kernel(PackState s, int W32, int n_pods, ksched_sim_result* out, uint64_t* node0_types) {
+  const int t = threadIdx.x;
+  const int n_new = (int)s.counters[kCtrNewNodes];
+  uint32_t* opts = reinterpret_cast<uint32_t*>(node0_types);
+  if (t == 0) {
+    out->n_pods = n_pods;
+    out->n_unscheduled = (int32_t)s.counters[kCtrUnscheduled];
+    out->n_new_nodes = n_new;
+    out->error = (int32_t)s.counters[kCtrError];
+  }
+  if (n_new >= 1) {
+    gather_new_node(s, W32, 0, t, blockDim.x, &out->node0, opts);
+    return;
+  }
+  if (t == 0) out->node0 = ksched_new_node{};
+  for (int w = t; w < W32; w += blockDim.x) opts[w] = 0;
 }
 
 // The scalars of one full simulation (ksched_simulate_full), copied out with its arrays.
@@ -122,54 +133,40 @@ struct SimFullOut {
 // the set's offsets): batch position b goes to pod b, b + n_removed_pods or b - n_pending + n_lead. slot_map[e] = the slot's
 // index among the slots that stay, -1 for a removed one. The new nodes are gathered from the pack kernel's columns
 // (PackState nn_*) into rows. One block per simulation, a few thousand pods and nodes: microseconds.
-__global__ void cluster_full_collect_kernel(const long long* __restrict__ counters, int n_pods, int n_pending, int n_lead, int n_removed_pods,
-                                            const int32_t* __restrict__ assign, const int32_t* __restrict__ relax, const int32_t* __restrict__ seq,
-                                            const int32_t* __restrict__ slot_map, const uint8_t* __restrict__ initialized, int n_existing,
-                                            int n_stay, const uint8_t* __restrict__ nn_tmpl, const int32_t* __restrict__ nn_count,
-                                            const int64_t* __restrict__ nn_req, const uint32_t* __restrict__ nn_req_present,
-                                            const uint64_t* __restrict__ nn_vals, const uint64_t* __restrict__ nn_meta,
-                                            const uint32_t* __restrict__ nn_opts, const int64_t* __restrict__ nn_req_ext,
-                                            const uint32_t* __restrict__ nn_ext_present, int max_new, int W32, int X, SimFullOut out) {
+__global__ void cluster_full_collect_kernel(PackState s, int W32, int X, int n_pods, int n_pending, int n_lead, int n_removed_pods,
+                                            const int32_t* __restrict__ slot_map, const uint8_t* __restrict__ initialized, int n_stay,
+                                            SimFullOut out) {
   __shared__ int uninit;
-  const int tid = threadIdx.x;
-  const int n_new = (int)counters[kCtrNewNodes];
+  const int tid = threadIdx.x, n_existing = s.n_existing;
+  const int n_new = (int)s.counters[kCtrNewNodes];
   if (tid == 0) uninit = 0;
   __syncthreads();
   for (int b = tid; b < n_pods; b += blockDim.x) {
     const int p = b < n_lead ? b : (b < n_pending ? b + n_removed_pods : b - n_pending + n_lead);
-    const int a = assign[b];
+    const int a = s.assign[b], relax = s.relax_level[b], seq = s.place_seq[b];
     out.assign[p] = a < 0 ? -1 : (a < n_existing ? slot_map[a] : n_stay + (a - n_existing));
-    out.relax[p] = relax[b];
-    out.seq[p] = seq[b];
+    out.relax[p] = relax;
+    out.seq[p] = seq;
   }
   for (int e = tid; e < n_existing; e += blockDim.x)
     if (slot_map[e] >= 0 && initialized && !initialized[e]) uninit = 1;  // helpers.go:104-110 walks every node that stays
   const int W64 = W32 / 2;  // DevCatalog::W32 is even
-  for (int n = tid; n < n_new; n += blockDim.x) {
-    ksched_new_node o;
-    o.template_index = nn_tmpl[n];
-    o.pod_count = nn_count[n];
-    o.requests_present = nn_req_present[n];
-    o.pad = 0;
-    for (int r = 0; r < KSCHED_MAX_RES; ++r) o.requests[r] = nn_req[(size_t)r * max_new + n];
-    for (int k = 0; k < KSCHED_MAX_KEYS; ++k) o.reqs.values[k] = nn_vals[(size_t)k * max_new + n];
-    o.reqs.meta = nn_meta[n];
-    out.nodes[n] = o;
-    uint32_t* row = reinterpret_cast<uint32_t*>(out.types + (size_t)n * W64);
-    for (int w = 0; w < W32; ++w) row[w] = nn_opts[(size_t)w * max_new + n];
+  const int lane = tid & 31, warps = blockDim.x >> 5;
+  for (int n = tid >> 5; n < n_new; n += warps) {  // one warp per node
+    gather_new_node(s, W32, n, lane, 32, out.nodes + n, reinterpret_cast<uint32_t*>(out.types + (size_t)n * W64));
     if (out.ext) {
-      for (int x = 0; x < X; ++x) out.ext[(size_t)n * X + x] = nn_req_ext[(size_t)n * X + x];
-      out.ext_present[n] = nn_ext_present[n];
+      for (int x = lane; x < X; x += 32) out.ext[(size_t)n * X + x] = s.nn_req_ext[(size_t)n * X + x];
+      if (lane == 0) out.ext_present[n] = s.nn_ext_present[n];
     }
   }
   __syncthreads();
   if (tid == 0) {
     SimFullDev d;
-    d.nodes_visited = counters[kCtrNodesVisited];
-    d.add_calls = counters[kCtrAddCalls];
+    d.nodes_visited = s.counters[kCtrNodesVisited];
+    d.add_calls = s.counters[kCtrAddCalls];
     d.n_new_nodes = n_new;
-    d.n_unscheduled = (int32_t)counters[kCtrUnscheduled];
-    d.error = (int32_t)counters[kCtrError];
+    d.n_unscheduled = (int32_t)s.counters[kCtrUnscheduled];
+    d.error = (int32_t)s.counters[kCtrError];
     d.all_pods_scheduled = d.n_unscheduled == 0 ? 1 : 0;
     d.uninitialized_existing = uninit;
     d.pad = 0;

@@ -334,10 +334,11 @@ struct ksched_handle {
   int sup_pods = 0, sup_pending = 0;
   std::vector<int32_t> h_node_first, h_node_count;   // per existing slot: first superset pod bound to it, how many
   DevBuf<int32_t> d_sup_pod_node, d_node_first, d_node_dst, d_set_nodes, d_pod_src;
-  DevBuf<uint32_t> d_sup_class, d_sup_uid, d_sim_types;
+  DevBuf<uint32_t> d_sup_class, d_sup_uid;
   DevBuf<int64_t> d_sup_ts, d_sim_remaining;
   DevBuf<uint8_t> d_in_set;
-  DevBuf<SimResultDev> d_sim_results;
+  DevBuf<ksched_sim_result> d_sim_results;
+  DevBuf<uint64_t> d_sim_types;
   // full simulations (ksched_simulate_full): which slots a set may remove, the initialised flags, the leading pending pods,
   // and the staging arrays every set's results are gathered into before they are copied out
   std::vector<uint8_t> h_node_removable;
@@ -1665,6 +1666,11 @@ static void print_pack_profile(const long long* counters) {
 }
 #endif
 
+// What the pack kernel's error counter (kCtrError) reports
+static const char* pack_error_text(long long code) {
+  return code == KSCHED_ERR_OVERFLOW ? "new-node capacity exceeded" : "a pod is constrained by more topology groups than the kernel supports";
+}
+
 int ksched_download(ksched_handle* h, const ksched_problem* pb, ksched_result* res) {
   if (!h || !pb || !res || !h->uploaded) return KSCHED_ERR_INVALID;
   CUDA_TRY(h, cudaSetDevice(h->device));
@@ -1678,7 +1684,7 @@ int ksched_download(ksched_handle* h, const ksched_problem* pb, ksched_result* r
   print_pack_profile(counters);
 #endif
   if (counters[kCtrError] != 0) {
-    h->err = counters[kCtrError] == KSCHED_ERR_OVERFLOW ? "new-node capacity exceeded" : "a pod is constrained by more topology groups than the kernel supports";
+    h->err = pack_error_text(counters[kCtrError]);
     return (int)counters[kCtrError];
   }
   const int n_new = (int)counters[kCtrNewNodes];
@@ -1920,7 +1926,7 @@ int ksched_simulate_batch(ksched_handle* h, const ksched_candidate_set* sets, in
   int rc = stage_sets(h, sets, n_sets, false, node_off, batch);
   if (rc != KSCHED_OK) return rc;
   CUDA_TRY(h, h->d_sim_results.ensure((size_t)n_sets));
-  CUDA_TRY(h, h->d_sim_types.ensure((size_t)n_sets * W32));
+  CUDA_TRY(h, h->d_sim_types.ensure((size_t)n_sets * W64));
   CUDA_TRY(h, cudaEventRecord(h->ev[0], h->stream));
   // nothing computeConsolidation can return depends on what happens after a second new node is opened
   // (consolidation.go:214-224: len(newNodes) != 1 -> do nothing): the simulation stops there
@@ -1928,9 +1934,7 @@ int ksched_simulate_batch(ksched_handle* h, const ksched_candidate_set* sets, in
   for (int q = 0; q < n_sets && rc == KSCHED_OK; ++q) {
     const int P = batch[(size_t)q];
     if ((rc = run_simulation(h, q, node_off, P, q == 0, stop_new_nodes)) != KSCHED_OK) break;
-    cluster_collect_kernel<<<1, 64, 0, h->stream>>>(h->d_counters.ptr, P, h->d_nn_tmpl.ptr, h->d_nn_count.ptr, h->d_nn_req.ptr, h->d_nn_req_present.ptr,
-                                                    h->d_nn_vals.ptr, h->d_nn_meta.ptr, h->d_nn_opts.ptr, h->st.max_new, W32, h->d_sim_results.ptr + q,
-                                                    h->d_sim_types.ptr + (size_t)q * W32);
+    cluster_collect_kernel<<<1, 32, 0, h->stream>>>(h->st, W32, P, h->d_sim_results.ptr + q, h->d_sim_types.ptr + (size_t)q * W64);
   }
   if (rc != KSCHED_OK) return rc;
   CUDA_TRY(h, cudaEventRecord(h->ev[4], h->stream));
@@ -1942,31 +1946,14 @@ int ksched_simulate_batch(ksched_handle* h, const ksched_candidate_set* sets, in
     print_pack_profile(counters);  // the last simulation of the batch
   }
 #endif
-  std::vector<SimResultDev> dev((size_t)n_sets);
-  std::vector<uint32_t> types((size_t)n_sets * W32);
-  CUDA_TRY(h, cudaMemcpyAsync(dev.data(), h->d_sim_results.ptr, dev.size() * sizeof(SimResultDev), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaMemcpyAsync(types.data(), h->d_sim_types.ptr, types.size() * 4, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(results, h->d_sim_results.ptr, (size_t)n_sets * sizeof(ksched_sim_result), cudaMemcpyDeviceToHost, h->stream));
+  if (node0_types)
+    CUDA_TRY(h, cudaMemcpyAsync(node0_types, h->d_sim_types.ptr, (size_t)n_sets * W64 * 8, cudaMemcpyDeviceToHost, h->stream));
   // the last simulation's pack launch (its counters stay until the next reset)
   CUDA_TRY(h, cudaMemcpyAsync(h->tm.pack_interval_ns, h->d_counters.ptr + kCtrPackStart, 2 * sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   CUDA_TRY(h, cudaGetLastError());
   h->tm.total_us = ev_us(h->ev[0], h->ev[4]);
-  for (int q = 0; q < n_sets; ++q) {
-    const SimResultDev& d = dev[(size_t)q];
-    ksched_sim_result& o = results[q];
-    std::memset(&o, 0, sizeof o);
-    o.n_pods = d.n_pods; o.n_unscheduled = d.n_unscheduled; o.n_new_nodes = d.n_new_nodes; o.error = d.error;
-    if (d.n_new_nodes >= 1) {
-      o.node0.template_index = d.template_index; o.node0.pod_count = d.pod_count; o.node0.requests_present = d.requests_present;
-      std::memcpy(o.node0.requests, d.requests, sizeof d.requests);
-      std::memcpy(o.node0.reqs.values, d.values, sizeof d.values);
-      o.node0.reqs.meta = d.meta;
-    }
-    if (node0_types) {
-      std::memset(node0_types + (size_t)q * W64, 0, (size_t)W64 * 8);
-      if (d.n_new_nodes >= 1) std::memcpy(node0_types + (size_t)q * W64, &types[(size_t)q * W32], (size_t)W32 * 4);
-    }
-  }
   return KSCHED_OK;
 }
 
@@ -2019,11 +2006,8 @@ int ksched_simulate_full(ksched_handle* h, const ksched_candidate_set* sets, int
                    h->d_full_types.ptr + o * W64, X ? h->d_full_ext.ptr + o * X : nullptr, h->d_full_ext_present.ptr + o, h->d_full_scalars.ptr + q};
     int removed_pods = 0;
     for (int i = 0; i < n_nodes; ++i) removed_pods += h->h_node_count[(size_t)sets[q].nodes[i]];
-    cluster_full_collect_kernel<<<1, 256, 0, h->stream>>>(h->d_counters.ptr, P, h->sup_pending, h->sup_lead, removed_pods, h->d_assign.ptr, h->d_relax.ptr,
-                                                          h->d_place_seq.ptr, h->d_slot_map.ptr + (size_t)q * NE, h->d_node_init.ptr, NE, NE - n_nodes,
-                                                          h->d_nn_tmpl.ptr, h->d_nn_count.ptr, h->d_nn_req.ptr, h->d_nn_req_present.ptr, h->d_nn_vals.ptr,
-                                                          h->d_nn_meta.ptr, h->d_nn_opts.ptr, h->d_nn_req_ext.ptr, h->d_nn_ext_present.ptr, h->st.max_new, W32,
-                                                          X, out);
+    cluster_full_collect_kernel<<<1, 256, 0, h->stream>>>(h->st, W32, X, P, h->sup_pending, h->sup_lead, removed_pods, h->d_slot_map.ptr + (size_t)q * NE,
+                                                          h->d_node_init.ptr, NE - n_nodes, out);
     CUDA_TRY(h, cudaGetLastError());
   }
   if (rc != KSCHED_OK) return rc;
@@ -2053,7 +2037,7 @@ int ksched_simulate_full(ksched_handle* h, const ksched_candidate_set* sets, int
   for (int q = 0; q < n_sets; ++q) {
     const SimFullDev& d = sc[(size_t)q];
     if (d.error != 0) {
-      h->err = "set " + std::to_string(q) + ": " + (d.error == KSCHED_ERR_OVERFLOW ? "new-node capacity exceeded" : "a pod is constrained by more topology groups than the kernel supports");
+      h->err = "set " + std::to_string(q) + ": " + pack_error_text(d.error);
       return d.error;
     }
     ksched_result& r = results[q];

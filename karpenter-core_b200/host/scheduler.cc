@@ -693,15 +693,25 @@ std::vector<Cand> sorted_candidates(const Problem* P, kh_context* ctx = &g_defau
   return cands;
 }
 
+// What computeConsolidation and ValidateCommand read of one simulateScheduling (helpers.go:96-114)
+struct Outcome {
+  bool gave_up = false;  // an existing node that stays is not initialised: the reference returns nil, false (helpers.go:109-113)
+  bool all_scheduled = false;
+  int n_new = 0;
+  std::shared_ptr<const Encoded> E;   // the encoding node 0 refers to: the snapshot's superset or the set's own fresh one
+  ksched_reqset node0{};              // the first new node's requirements
+  std::vector<uint64_t> node0_types;  // [E->type_words] its InstanceTypeOptions, unfiltered
+};
+
 // computeConsolidation after the simulation (consolidation.go:206-274) + the multi-node caller's filterOutSameType
-// (multinodeconsolidation.go:132-165, `multi`): sel = the candidates being removed, node0 / bits = the single new node.
-Cmd finish_command(const Problem* P, const Encoded& E, const std::vector<Cand>& sel, bool all_scheduled, int n_new, const ksched_reqset& node0_reqs,
-                   const uint64_t* bits, bool multi) {
+// (multinodeconsolidation.go:132-165, `multi`): sel = the candidates being removed, o = what the simulation returned.
+Cmd finish_command(const Problem* P, const std::vector<Cand>& sel, const Outcome& o, bool multi) {
   Cmd cmd;
   const int count = (int)sel.size();
-  if (!all_scheduled) return cmd;
-  if (n_new == 0) { cmd.action = 1; return cmd; }
-  if (n_new != 1) return cmd;
+  if (o.gave_up || !o.all_scheduled) return cmd;
+  if (o.n_new == 0) { cmd.action = 1; return cmd; }
+  if (o.n_new != 1) return cmd;
+  const Encoded& E = *o.E;
   double price = 0;  // getNodePrices consolidation.go:277-287
   for (int i = 0; i < count; ++i) {
     const Cand& c = sel[i];
@@ -710,10 +720,10 @@ Cmd finish_command(const Problem* P, const Encoded& E, const std::vector<Cand>& 
     for (auto& o : c.it->offerings) if (o.capacity_type == c.ct && o.zone == c.zone) { price += o.price; ok = true; break; }
     if (!ok) throw std::runtime_error("unable to determine offering");
   }
-  ksched_reqset reqs = node0_reqs;
+  ksched_reqset reqs = o.node0;
   std::vector<int> opts;
   for (size_t c = 0; c < E.type_input_index.size(); ++c)
-    if ((bits[c / 64] >> (c % 64)) & 1) opts.push_back(E.type_input_index[c]);
+    if ((o.node0_types[c / 64] >> (c % 64)) & 1) opts.push_back(E.type_input_index[c]);
   std::sort(opts.begin(), opts.end());
   std::vector<int> kept;
   for (int t : opts) if (worst_launch_price(E, P->instance_types[t], reqs) < price) kept.push_back(t);  // filterByPrice
@@ -766,59 +776,56 @@ Cmd finish_command(const Problem* P, const Encoded& E, const std::vector<Cand>& 
   return cmd;
 }
 
-// One simulateScheduling = one ksched_solve of a freshly encoded problem (the path for clusters the snapshot cannot hold).
-Cmd compute_consolidation_encoded(const Problem* P, const std::vector<Cand>& sel, bool multi, kh_context* ctx) {
-  std::vector<int> nodes;
-  for (auto& c : sel) nodes.push_back(c.node);
-  auto E = khost::encode(*P, nodes);
-  E->problem.count_nodes_visited = g_count_visited;
-  ResultBuffers B;
-  if (solve_on(ctx, *E, B) != KSCHED_OK) throw std::runtime_error(g_err);
-  size_t scheduled = 0;
-  for (auto a : B.assign) if (a >= 0) ++scheduled;
-  // helpers.go:109-113 walks EVERY ExistingNode Solve returns (all owned nodes that are neither candidates nor marked for
-  // deletion) and gives up when one of them is not initialised - whether or not a pod landed on it
-  for (size_t e = 0; e < E->existing.size(); ++e)
-    if (!E->existing_initialized[e]) return Cmd();
-  return finish_command(P, *E, sel, scheduled == E->pods.size(), B.r.n_new_nodes, B.nodes[0].reqs, &B.types[0], multi);
-}
-
-// ksched_load_catalog + ksched_load_cluster of a superset encoding (khost::encode(..., true)) of the candidates `cands`
-// (Problem.nodes indices) on h
-int load_snapshot(ksched_handle* h, Encoded& E, const std::vector<int>& cands) {
-  int rc = ksched_load_catalog(h, &E.catalog);
-  if (rc != KSCHED_OK) return rc;
-  ksched_cluster cl{};
-  cl.problem = &E.problem;
-  cl.pod_node = E.pod_node.data();
-  // what a full simulation needs: the candidates' slots, the initialised nodes, and Solve's pod order (helpers.go:74-88:
-  // the pending pods, the candidates' pods, the pods of nodes marked for deletion)
-  const std::set<int> cand(cands.begin(), cands.end());
-  std::vector<uint8_t> removable, initialized;
-  for (size_t e = 0; e < E.existing.size(); ++e) {
-    removable.push_back(cand.count(E.existing_state_index[e]) ? 1 : 0);
-    initialized.push_back(E.existing_initialized[e] ? 1 : 0);
-  }
-  cl.node_removable = removable.data();
-  cl.node_initialized = initialized.data();
-  cl.n_pending_lead = (int32_t)E.problem_ref->pods.size();
-  if (E.problem.n_groups > 0) {
-    cl.class_count_begin = E.class_count_begin.data();
-    cl.class_count = E.class_count.data();
-    cl.node_domain = E.node_domain.data();
-    cl.node_has_hostname_label = E.node_has_hostname_label.data();
-    cl.group_filter_match = E.group_filter_match.data();
-  }
-  return ksched_load_cluster(h, &cl);
-}
-
-// One ksched_simulate_batch on the snapshot of E that h holds: simulation q removes the existing slots slot_sets[q].
-// skip[q]: an uninitialised node stays, and simulateScheduling gives up on it (helpers.go:109-113).
-struct SimBatch {
-  std::vector<ksched_sim_result> res;
-  std::vector<uint64_t> types;  // [simulation][type_words]: the first new node's InstanceTypeOptions
-  std::vector<char> skip;
+// A cluster on the device: the superset encoding (khost::encode(..., true)) of P whose candidates are `cands` (Problem.nodes
+// indices, in the caller's order), loaded on a handle with ksched_load_cluster. A cluster the snapshot refuses
+// (KSCHED_ERR_UNSUPPORTED) is not resident, and each of its simulations is a freshly encoded ksched_solve.
+struct ClusterSnapshot {
+  const Problem* P = nullptr;
+  std::vector<int> cands;
+  std::shared_ptr<const Encoded> E;
+  std::vector<int> slot_of_node;  // Problem.nodes index -> existing slot of E, -1 for none
+  bool resident = false;
 };
+
+// ksched_load_catalog + ksched_load_cluster of S on h, encoding the superset first when S has none yet (a reload keeps it)
+void load_snapshot(ksched_handle* h, ClusterSnapshot& S) {
+  if (!S.E) {
+    auto sup = khost::encode(*S.P, S.cands, true);
+    sup->problem.count_nodes_visited = 0;
+    S.slot_of_node.assign(S.P->nodes.size(), -1);
+    for (size_t e = 0; e < sup->existing_state_index.size(); ++e) S.slot_of_node[(size_t)sup->existing_state_index[e]] = (int)e;
+    S.E = std::move(sup);
+  }
+  const Encoded& E = *S.E;
+  int rc = ksched_load_catalog(h, &E.catalog);
+  if (rc == KSCHED_OK) {
+    ksched_cluster cl{};
+    cl.problem = &E.problem;
+    cl.pod_node = E.pod_node.data();
+    // what a full simulation needs: the candidates' slots, the initialised nodes, and Solve's pod order (helpers.go:74-88:
+    // the pending pods, the candidates' pods, the pods of nodes marked for deletion)
+    const std::set<int> cand(S.cands.begin(), S.cands.end());
+    std::vector<uint8_t> removable, initialized;
+    for (size_t e = 0; e < E.existing.size(); ++e) {
+      removable.push_back(cand.count(E.existing_state_index[e]) ? 1 : 0);
+      initialized.push_back(E.existing_initialized[e] ? 1 : 0);
+    }
+    cl.node_removable = removable.data();
+    cl.node_initialized = initialized.data();
+    cl.n_pending_lead = (int32_t)E.problem_ref->pods.size();
+    if (E.problem.n_groups > 0) {
+      cl.class_count_begin = E.class_count_begin.data();
+      cl.class_count = E.class_count.data();
+      cl.node_domain = E.node_domain.data();
+      cl.node_has_hostname_label = E.node_has_hostname_label.data();
+      cl.group_filter_match = E.group_filter_match.data();
+    }
+    rc = ksched_load_cluster(h, &cl);
+  }
+  S.resident = rc == KSCHED_OK;
+  if (rc != KSCHED_OK && rc != KSCHED_ERR_UNSUPPORTED) throw std::runtime_error(ksched_last_error(h));
+}
+
 // scheduler.go:221-248 only charges the nodes that stay: the provisioner limits left when the existing slots `slots` of E's
 // snapshot are removed - the exact remaining with their capacity given back, then held at remaining_minus's floor like a
 // Solve's
@@ -833,26 +840,61 @@ std::vector<int64_t> remaining_without(const Encoded& E, const std::vector<int32
   return rem;
 }
 
-SimBatch simulate_on(ksched_handle* h, const Encoded& E, const std::vector<std::vector<int32_t>>& slot_sets) {
-  const size_t n = slot_sets.size(), NE = E.existing.size();
-  SimBatch out;
-  out.skip.assign(n, 0);
+// simulateScheduling of every set (Problem.nodes indices, existing nodes of S) as computeConsolidation and ValidateCommand read
+// it. A resident S (h holds it) simulates them all in one ksched_simulate_batch; a refused one solves each set freshly encoded
+// on h, through ctx when h is that context's handle (a fresh solve displaces what the context holds), nullptr for a handle of
+// its own. The fresh solves never keep the nodes_visited statistic: no verdict reads it.
+std::vector<Outcome> simulate_sets(const ClusterSnapshot& S, ksched_handle* h, kh_context* ctx, const std::vector<std::vector<int>>& sets) {
+  const size_t n = sets.size();
+  std::vector<Outcome> out(n);
+  if (!S.resident) {
+    for (size_t q = 0; q < n; ++q) {
+      auto F = khost::encode(*S.P, sets[q]);
+      F->problem.count_nodes_visited = 0;
+      ResultBuffers B;
+      if ((ctx ? solve_on(ctx, *F, B) : solve_on(h, *F, B)) != KSCHED_OK) throw std::runtime_error(g_err);
+      Outcome& o = out[q];
+      // helpers.go:109-113 walks EVERY ExistingNode Solve returns (all owned nodes that are neither candidates nor marked for
+      // deletion) and gives up when one of them is not initialised - whether or not a pod landed on it
+      o.gave_up = std::find(F->existing_initialized.begin(), F->existing_initialized.end(), false) != F->existing_initialized.end();
+      o.all_scheduled = (size_t)std::count_if(B.assign.begin(), B.assign.end(), [](int32_t a) { return a >= 0; }) == F->pods.size();
+      o.n_new = B.r.n_new_nodes;
+      o.node0 = B.nodes[0].reqs;
+      o.node0_types.assign(B.types.begin(), B.types.begin() + F->type_words);
+      o.E = std::move(F);
+    }
+    return out;
+  }
+  const Encoded& E = *S.E;
+  const size_t NE = E.existing.size(), TW = (size_t)E.type_words;
+  std::vector<std::vector<int32_t>> slots(n);
   std::vector<std::vector<int64_t>> rem(n);
   std::vector<ksched_candidate_set> cs(n);
   std::vector<char> removed(NE);
   for (size_t q = 0; q < n; ++q) {
     std::fill(removed.begin(), removed.end(), 0);
-    for (int32_t e : slot_sets[q]) removed[(size_t)e] = 1;
-    rem[q] = remaining_without(E, slot_sets[q]);
-    for (size_t e = 0; e < NE; ++e) if (!removed[e] && !E.existing_initialized[e]) out.skip[q] = 1;
-    cs[q] = ksched_candidate_set{slot_sets[q].data(), (int32_t)slot_sets[q].size(), 0, rem[q].data()};
+    for (int i : sets[q]) {
+      const int e = S.slot_of_node.at((size_t)i);
+      if (e < 0) throw std::runtime_error("candidate is not an existing node of the snapshot");
+      slots[q].push_back(e);
+      removed[(size_t)e] = 1;
+    }
+    rem[q] = remaining_without(E, slots[q]);
+    for (size_t e = 0; e < NE; ++e) if (!removed[e] && !E.existing_initialized[e]) out[q].gave_up = true;
+    cs[q] = ksched_candidate_set{slots[q].data(), (int32_t)slots[q].size(), 0, rem[q].data()};
   }
-  out.res.resize(n);
-  out.types.resize(n * (size_t)E.type_words);
-  int rc = ksched_simulate_batch(h, cs.data(), (int)cs.size(), out.res.data(), out.types.data());
-  if (rc != KSCHED_OK) throw std::runtime_error(ksched_last_error(h));
-  for (size_t q = 0; q < n; ++q)
-    if (!out.skip[q] && out.res[q].error) throw std::runtime_error("simulation failed on the device");
+  std::vector<ksched_sim_result> res(n);
+  std::vector<uint64_t> types(n * TW);
+  if (ksched_simulate_batch(h, cs.data(), (int)n, res.data(), types.data()) != KSCHED_OK) throw std::runtime_error(ksched_last_error(h));
+  for (size_t q = 0; q < n; ++q) {
+    Outcome& o = out[q];
+    if (!o.gave_up && res[q].error) throw std::runtime_error("simulation failed on the device");
+    o.all_scheduled = res[q].n_unscheduled == 0;
+    o.n_new = res[q].n_new_nodes;
+    o.E = S.E;
+    o.node0 = res[q].node0.reqs;
+    o.node0_types.assign(types.begin() + (ptrdiff_t)(q * TW), types.begin() + (ptrdiff_t)((q + 1) * TW));
+  }
   return out;
 }
 
@@ -864,15 +906,15 @@ struct VCmd {
   std::vector<std::string> options;
 };
 
-// ValidateCommand after its simulateScheduling (validation.go:122-171); bits = the first new node's options (unfiltered)
-bool command_valid(const Problem* A, const Encoded& E, const VCmd& c, bool all_scheduled, int n_new, const uint64_t* bits) {
-  if (!all_scheduled) return false;
-  if (n_new == 0) return c.action == 1;          // :132-140 valid only when no replacement was expected
-  if (n_new > 1 || c.action != 2) return false;  // :142-151
-  std::set<std::string> rhs;                     // instanceTypesAreSubset (helpers.go:118-122), by name
-  for (size_t col = 0; col < E.type_input_index.size(); ++col)
-    if ((bits[col / 64] >> (col % 64)) & 1) rhs.insert(A->instance_types[(size_t)E.type_input_index[col]].name);
-  for (auto& o : c.options) if (!rhs.count(o)) return false;
+// ValidateCommand after its simulateScheduling (validation.go:122-171)
+bool command_valid(const Problem* A, const VCmd& c, const Outcome& o) {
+  if (o.gave_up || !o.all_scheduled) return false;
+  if (o.n_new == 0) return c.action == 1;          // :132-140 valid only when no replacement was expected
+  if (o.n_new > 1 || c.action != 2) return false;  // :142-151
+  std::set<std::string> rhs;                       // instanceTypesAreSubset (helpers.go:118-122), by name
+  for (size_t col = 0; col < o.E->type_input_index.size(); ++col)
+    if ((o.node0_types[col / 64] >> (col % 64)) & 1) rhs.insert(A->instance_types[(size_t)o.E->type_input_index[col]].name);
+  for (auto& name : c.options) if (!rhs.count(name)) return false;
   return true;
 }
 
@@ -882,41 +924,29 @@ struct HandleDeleter { void operator()(ksched_handle* h) const { ksched_destroy(
 // validation of one ComputeCommand reads this one snapshot (DESIGN.md §6 R7). The validation candidates are
 // candidateNodes(after, Validation.ShouldDeprovision) in node-list order (validation.go:78-83): they do not go through
 // sortAndFilterCandidates, so a node that a PDB or a DeletionTimestamp keeps out of the pass is still validated. With
-// "deriveCandidates": false they are the nodes marked "candidate" that are not marked for deletion. Clusters the snapshot refuses are validated one freshly
-// encoded ksched_solve at a time on the same handle.
-struct ValidationSnapshot {
-  const Problem* A = nullptr;
-  uint64_t problem_id = 0;          // Problem::id of A: never shared with a problem allocated later at the same address
-  std::vector<int> cands;           // Problem.nodes indices
+// "deriveCandidates": false they are the nodes marked "candidate" that are not marked for deletion.
+struct Validation {
+  uint64_t problem_id = 0;          // Problem::id of the cluster: never shared with a problem allocated later at the same address
   std::set<std::string> nominated;  // Cluster.IsNodeNominated
   std::unique_ptr<ksched_handle, HandleDeleter> h;
-  std::unique_ptr<Encoded> E;       // superset encoding (resident == true)
-  std::vector<int> slot_of_node;
-  bool resident = false;
+  ClusterSnapshot snap;
 
-  ValidationSnapshot(const Problem* a, int device) : A(a), problem_id(a->id) {
+  Validation(const Problem* A, int device) : problem_id(A->id) {
+    snap.P = A;
     for (size_t i = 0; i < A->nodes.size(); ++i) {
       const StateNode& n = A->nodes[i];
       if (n.nominated) nominated.insert(n.name);
       const Provisioner* prov = nullptr;
       // candidateNodes skips nodes marked for deletion in either mode (helpers.go:185-188)
-      if (A->derive_candidates ? candidate_node(A, n, &prov) : n.candidate && !n.marked_for_deletion) cands.push_back((int)i);
+      if (A->derive_candidates ? candidate_node(A, n, &prov) : n.candidate && !n.marked_for_deletion) snap.cands.push_back((int)i);
     }
     ksched_handle* raw = nullptr;
     if (ksched_create(device, &raw) != KSCHED_OK) throw std::runtime_error("ksched_create failed: no usable CUDA device (the product has no CPU path)");
     h.reset(raw);
-    auto sup = khost::encode(*A, cands, true);
-    sup->problem.count_nodes_visited = 0;
-    int rc = load_snapshot(h.get(), *sup, cands);
-    if (rc == KSCHED_ERR_UNSUPPORTED) return;  // resident stays false
-    if (rc != KSCHED_OK) throw std::runtime_error(ksched_last_error(h.get()));
-    E = std::move(sup);
-    slot_of_node.assign(A->nodes.size(), -1);
-    for (size_t e = 0; e < E->existing_state_index.size(); ++e) slot_of_node[(size_t)E->existing_state_index[e]] = (int)e;
-    resident = true;
+    load_snapshot(h.get(), snap);
   }
 
-  // Validation.IsValid for every command: the simulations of all of them in one ksched_simulate_batch call
+  // Validation.IsValid for every command: the simulations of all of them in one simulate_sets call
   std::vector<char> validate(const std::vector<VCmd>& cmds) {
     std::vector<char> ok(cmds.size(), 0);
     std::vector<size_t> run;               // commands that reach simulateScheduling
@@ -927,32 +957,14 @@ struct ValidationSnapshot {
       if (nom) continue;
       std::set<std::string> names(cmds[q].nodes.begin(), cmds[q].nodes.end());
       std::vector<int> m;
-      for (int i : cands) if (names.count(A->nodes[(size_t)i].name)) m.push_back(i);  // mapNodes helpers.go:328-337
-      if (m.empty()) continue;                                                         // validation.go:113-116
+      for (int i : snap.cands) if (names.count(snap.P->nodes[(size_t)i].name)) m.push_back(i);  // mapNodes helpers.go:328-337
+      if (m.empty()) continue;                                                                   // validation.go:113-116
       run.push_back(q);
       mapped.push_back(std::move(m));
     }
     if (run.empty()) return ok;
-    if (resident) {
-      std::vector<std::vector<int32_t>> slots(run.size());
-      for (size_t j = 0; j < run.size(); ++j) for (int i : mapped[j]) slots[j].push_back(slot_of_node[(size_t)i]);
-      SimBatch sb = simulate_on(h.get(), *E, slots);
-      for (size_t j = 0; j < run.size(); ++j)
-        if (!sb.skip[j])
-          ok[run[j]] = command_valid(A, *E, cmds[run[j]], sb.res[j].n_unscheduled == 0, sb.res[j].n_new_nodes, &sb.types[j * (size_t)E->type_words]);
-      return ok;
-    }
-    for (size_t j = 0; j < run.size(); ++j) {
-      auto F = khost::encode(*A, mapped[j]);
-      F->problem.count_nodes_visited = 0;
-      ResultBuffers B;
-      if (solve_on(h.get(), *F, B) != KSCHED_OK) throw std::runtime_error(g_err);
-      bool init = true;
-      for (size_t e = 0; e < F->existing.size(); ++e) init = init && F->existing_initialized[e];
-      size_t scheduled = 0;
-      for (auto a : B.assign) if (a >= 0) ++scheduled;
-      ok[run[j]] = init && command_valid(A, *F, cmds[run[j]], scheduled == F->pods.size(), B.r.n_new_nodes, &B.types[0]);
-    }
+    const std::vector<Outcome> o = simulate_sets(snap, h.get(), nullptr, mapped);
+    for (size_t j = 0; j < run.size(); ++j) ok[run[j]] = command_valid(snap.P, cmds[run[j]], o[j]);
     return ok;
   }
 };
@@ -965,71 +977,46 @@ struct ValidationSnapshot {
 struct ClusterSession {
   kh_context* ctx = &g_default;
   const Problem* P = nullptr;
-  std::vector<Cand> cands;            // disruption order
-  std::unique_ptr<Encoded> E;         // superset encoding (resident == true)
-  std::vector<int> slot_of_node;      // Problem.nodes index -> existing slot
-  bool resident = false;
-  uint64_t id = 0;
+  std::vector<Cand> cands;  // disruption order
+  ClusterSnapshot snap;     // whose candidates are cands' nodes
+  uint64_t id = 0;          // what ctx->resident holds while the context's handle holds snap
   int simulations = 0;
-  std::unique_ptr<ValidationSnapshot> validation_snapshot;  // opened at the first command that needs validation
+  std::unique_ptr<Validation> validation;  // opened at the first command that needs validation
 
-  explicit ClusterSession(const Problem* p, kh_context* c = &g_default) : ctx(c), P(p), cands(sorted_candidates(p, c)) {
+  explicit ClusterSession(const Problem* p, kh_context* c = &g_default)
+      : ctx(c), P(p), cands(sorted_candidates(p, c)), id(++g_last_session) {
     if (open_handle(ctx) != KSCHED_OK) throw std::runtime_error(g_err);
-    ksched_handle* h = ctx->h;
-    std::vector<int> nodes;
-    for (auto& c : cands) nodes.push_back(c.node);
-    auto sup = khost::encode(*P, nodes, true);
-    sup->problem.count_nodes_visited = 0;
-    ctx->resident = 0;
-    int rc = load_snapshot(h, *sup, nodes);
-    if (rc == KSCHED_ERR_UNSUPPORTED) return;  // resident stays false
-    if (rc != KSCHED_OK) throw std::runtime_error(ksched_last_error(h));
-    E = std::move(sup);
-    slot_of_node.assign(P->nodes.size(), -1);
-    for (size_t e = 0; e < E->existing_state_index.size(); ++e) slot_of_node[(size_t)E->existing_state_index[e]] = (int)e;
-    resident = true;
-    ctx->resident = id = ++g_last_session;
+    snap.P = p;
+    for (auto& c : cands) snap.cands.push_back(c.node);
+    load();
   }
-
-  // computeConsolidation for every set (positions in the disruption order), one ksched_simulate_batch call
-  std::vector<Cmd> compute_many(const std::vector<std::vector<int>>& sets, bool multi) {
-    std::vector<Cmd> out(sets.size());
-    simulations += (int)sets.size();
-    if (!resident) {
-      for (size_t q = 0; q < sets.size(); ++q) {
-        std::vector<Cand> sel;
-        for (int i : sets[q]) sel.push_back(cands.at((size_t)i));
-        out[q] = compute_consolidation_encoded(P, sel, multi, ctx);
-      }
-      return out;
-    }
-    std::vector<std::vector<int32_t>> slots(sets.size());
-    for (size_t q = 0; q < sets.size(); ++q)
-      for (int i : sets[q]) {
-        const int e = slot_of_node.at((size_t)cands.at((size_t)i).node);
-        if (e < 0) throw std::runtime_error("candidate is not an existing node of the snapshot");
-        slots[q].push_back(e);
-      }
-    make_current();
-    SimBatch sb = simulate_on(ctx->h, *E, slots);
-    for (size_t q = 0; q < sets.size(); ++q) {
-      if (sb.skip[q]) continue;
-      std::vector<Cand> sel;
-      for (int i : sets[q]) sel.push_back(cands[(size_t)i]);
-      out[q] = finish_command(P, *E, sel, sb.res[q].n_unscheduled == 0, sb.res[q].n_new_nodes, sb.res[q].node0.reqs, &sb.types[q * (size_t)E->type_words], multi);
-    }
-    return out;
+  // snap onto the context's handle, displacing what it held
+  void load() {
+    ctx->resident = 0;
+    load_snapshot(ctx->h, snap);
+    if (snap.resident) ctx->resident = id;
   }
   // the session's snapshot on its context's handle again when something else displaced it: the time of one reload, the same
   // answers
   void make_current() {
-    if (ctx->resident == id) return;
-    if (open_handle(ctx) != KSCHED_OK) throw std::runtime_error(g_err);
-    ctx->resident = 0;
-    std::vector<int> nodes;
-    for (auto& c : cands) nodes.push_back(c.node);
-    if (load_snapshot(ctx->h, *E, nodes) != KSCHED_OK) throw std::runtime_error(ksched_last_error(ctx->h));
-    ctx->resident = id;
+    if (snap.resident && ctx->resident != id) load();
+  }
+
+  // computeConsolidation for every set (positions in the disruption order), one simulate_sets call
+  std::vector<Cmd> compute_many(const std::vector<std::vector<int>>& sets, bool multi) {
+    simulations += (int)sets.size();
+    std::vector<std::vector<int>> nodes(sets.size());
+    for (size_t q = 0; q < sets.size(); ++q)
+      for (int i : sets[q]) nodes[q].push_back(cands.at((size_t)i).node);
+    make_current();
+    const std::vector<Outcome> o = simulate_sets(snap, ctx->h, ctx, nodes);
+    std::vector<Cmd> out(sets.size());
+    for (size_t q = 0; q < sets.size(); ++q) {
+      std::vector<Cand> sel;
+      for (int i : sets[q]) sel.push_back(cands[(size_t)i]);
+      out[q] = finish_command(P, sel, o[q], multi);
+    }
+    return out;
   }
 
   // simulateScheduling's whole result for every set (Problem.nodes indices, candidates of the session, in the caller's
@@ -1046,7 +1033,7 @@ struct ClusterSession {
       }
     simulations += (int)sets.size();
     std::vector<Result> out(sets.size());
-    if (!resident) {
+    if (!snap.resident) {
       for (size_t q = 0; q < sets.size(); ++q) {
         auto F = khost::encode(*P, sets[q]);
         F->problem.count_nodes_visited = g_count_visited;
@@ -1057,7 +1044,7 @@ struct ClusterSession {
       }
       return out;
     }
-    const size_t n = sets.size(), NE = E->existing.size();
+    const size_t n = sets.size(), NE = snap.E->existing.size();
     std::vector<std::vector<int32_t>> slots(n);
     std::vector<std::vector<int64_t>> rem(n);
     std::vector<ksched_candidate_set> cs(n);
@@ -1065,15 +1052,15 @@ struct ClusterSession {
     std::vector<size_t> pods_in_batch(n);
     size_t pending = 0;
     std::vector<size_t> node_pods(NE, 0);  // the snapshot's pods per slot
-    for (int32_t e : E->pod_node) if (e >= 0) ++node_pods[(size_t)e]; else ++pending;
+    for (int32_t e : snap.E->pod_node) if (e >= 0) ++node_pods[(size_t)e]; else ++pending;
     for (size_t q = 0; q < n; ++q) {
       pods_in_batch[q] = pending;
       for (int i : sets[q]) {
-        slots[q].push_back(slot_of_node[(size_t)i]);
+        slots[q].push_back(snap.slot_of_node[(size_t)i]);
         pods_in_batch[q] += node_pods[(size_t)slots[q].back()];
       }
-      rem[q] = remaining_without(*E, slots[q]);
-      B[q].prepare(*E, false, pods_in_batch[q]);
+      rem[q] = remaining_without(*snap.E, slots[q]);
+      B[q].prepare(*snap.E, false, pods_in_batch[q]);
       cs[q] = ksched_candidate_set{slots[q].data(), (int32_t)slots[q].size(), (int32_t)pods_in_batch[q], rem[q].data()};
     }
     make_current();
@@ -1085,9 +1072,9 @@ struct ClusterSession {
       B[q].r = res[q];
       for (int i : sets[q]) removed[(size_t)i] = 1;
       std::vector<int> existing_index;
-      for (int si : E->existing_state_index) if (!removed[(size_t)si]) existing_index.push_back(si);
+      for (int si : snap.E->existing_state_index) if (!removed[(size_t)si]) existing_index.push_back(si);
       for (int i : sets[q]) removed[(size_t)i] = 0;
-      decode(*E, B[q], pods_in_batch[q], existing_index, out[q]);
+      decode(*snap.E, B[q], pods_in_batch[q], existing_index, out[q]);
       out[q].all_pods_scheduled = res[q].all_pods_scheduled != 0;
       out[q].uninitialized_existing = res[q].uninitialized_existing != 0;
     }
@@ -1109,11 +1096,11 @@ struct ClusterSession {
     return c;
   }
   std::vector<char> validate(const Problem* after, const std::vector<VCmd>& cmds) {
-    if (!validation_snapshot || validation_snapshot->problem_id != after->id) {
-      validation_snapshot.reset();  // one extra device handle at a time
-      validation_snapshot = std::make_unique<ValidationSnapshot>(after, ctx->device);
+    if (!validation || validation->problem_id != after->id) {
+      validation.reset();  // one extra device handle at a time
+      validation = std::make_unique<Validation>(after, ctx->device);
     }
-    return validation_snapshot->validate(cmds);
+    return validation->validate(cmds);
   }
 };
 
@@ -1230,7 +1217,7 @@ ClusterSession* kh_context_cluster_open(kh_context* ctx, const Problem* P, int* 
   Lock lock(ctx->mu);
   try {
     auto* cs = new ClusterSession(P, ctx);
-    if (resident) *resident = cs->resident ? 1 : 0;
+    if (resident) *resident = cs->snap.resident ? 1 : 0;
     if (n_candidates) *n_candidates = (int)cs->cands.size();
     return cs;
   } catch (const std::exception& e) {

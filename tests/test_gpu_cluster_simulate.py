@@ -3,7 +3,8 @@ is, set for set, what a freshly encoded Solve with that set as the candidates re
 what the oracle returns: the whole result in the fresh problem's numbering and both verdicts. nodes_visited is the one
 field left out: a simulation also counts the removed nodes the pack kernel skips. Checked at three pack-kernel block
 sizes, under every mode switch, with one and with 64 sets per call, on a refused snapshot, at C5's full size, and for the
-snapshot's state: probes and validations before and after a simulation agree."""
+snapshot's state: probes and validations before and after a simulation agree. A refused snapshot's probes and single-node
+search equal the oracle too."""
 import copy
 import ctypes as C
 
@@ -13,7 +14,7 @@ import consolidation_answers as ca
 import fixtures as fx
 import full_simulation_problems as fp
 import validation_answers as va
-from oracle_compare import INSTANCE_TYPE, MODE_SWITCHES, set_modes
+from oracle_compare import INSTANCE_TYPE, MODE_SWITCHES, compare_probes, set_modes
 
 pytestmark = pytest.mark.gpu
 
@@ -94,12 +95,19 @@ def test_simulation_leaves_the_snapshot_as_it_found_it(pkg, oracle):
     assert cs.validate(problem, commands) == valid
 
 
-def test_refused_snapshot_simulates_through_fresh_solves(pkg, oracle):
-    a = va._cluster()
+def _crowded_cluster(pod_cpu="1"):
+    """a cluster the snapshot refuses: node "crowd" (the last in the node list) hosts a pod with more topology groups than
+    the pack kernel carries"""
+    a = va._cluster(pod_cpu=pod_cpu)
     big = ca.on_demand_by_price(a["instanceTypes"])[-1]
     crowd = fx.pod({"cpu": "100m"}, nodeName="crowd", labels={f"k{j}": "v" for j in range(10)},
                    topologySpreadConstraints=[fx.spread(fx.HOSTNAME, {f"k{j}": "v"}) for j in range(10)])
     a["nodes"].append(ca.node_of_type("crowd", big, [crowd], 1.0))
+    return a
+
+
+def test_refused_snapshot_simulates_through_fresh_solves(pkg, oracle):
+    a = _crowded_cluster()
     problem = pkg.Problem.from_dict(a)
     cs = pkg.ClusterSession(problem)
     assert not cs.resident
@@ -109,6 +117,25 @@ def test_refused_snapshot_simulates_through_fresh_solves(pkg, oracle):
     for s, got in zip(sets, cs.simulate(sets)):
         want = pkg.Scheduler(problem).solve(candidates=s)
         assert _whole(got) == _whole(want), s
+
+
+@pytest.mark.parametrize("pod_cpu", ["1", "24"])
+def test_refused_snapshot_consolidates_through_fresh_solves(pkg, oracle, pod_cpu):
+    """computeConsolidation on a session whose snapshot is refused, each set a freshly encoded solve: every probe that
+    leaves the crowd node's pod bound, and the single-node search, equal the oracle. With 1-CPU pods every probe deletes;
+    with 24-CPU pods the two cheapest nodes are replaced by one and removing three does nothing."""
+    a = _crowded_cluster(pod_cpu)
+    problem = pkg.Problem.from_dict(a)
+    cs = pkg.ClusterSession(problem)
+    assert not cs.resident
+    order = cs.candidate_nodes()
+    assert order[-1] == len(a["nodes"]) - 1
+    n = len(order) - 1
+    compare_probes(pkg, oracle, problem, cs, [list(range(c)) for c in range(1, n + 1)], [[i] for i in range(n)])
+    got = pkg.SingleNodeConsolidation(problem).compute_command(batch=1)
+    want = oracle.consolidate_single(problem)
+    keys = ("action", "node", "options")
+    assert {k: got[k] for k in keys} == {k: want[k] for k in keys}
 
 
 def test_refusals(pkg, oracle):

@@ -539,8 +539,9 @@ int ksched_simulate_batch(ksched_handle* h, const ksched_candidate_set* sets, in
    index among the slots that stay; new node i is n_existing - n_nodes + i. Filled: assign, relax_level, place_seq,
    new_nodes, new_node_types, launch (when not NULL; needs ksched_catalog.offering_keys), the ext arrays (when not NULL),
    the counts and the two flags; existing_reqs, feasibility and best_column are not written. nodes_visited counts the
-   removed slots the pack kernel skips as well. A slot out of range, repeated or not removable, or a capacity below the
-   set's batch, is KSCHED_ERR_INVALID. The snapshot is left as it was; one stream synchronisation per call. */
+   removed slots the pack kernel skips as well. A slot out of range, repeated or not removable, a capacity below the
+   set's batch, or a batch with pods and one of the five arrays NULL, is KSCHED_ERR_INVALID. The snapshot is left as it
+   was; one stream synchronisation per call. */
 int ksched_simulate_full(ksched_handle* h, const ksched_candidate_set* sets, int n_sets, ksched_result* results);
 
 /* order[0..*n_candidates) = node indices by ascending disruption cost (ties: input order), cost[i] = cost of order[i]. */

@@ -118,16 +118,44 @@ struct SimFullDev {
   long long nodes_visited, add_calls;
   int32_t n_new_nodes, n_unscheduled, error, all_pods_scheduled, uninitialized_existing, pad;
 };
-// Where cluster_full_collect_kernel writes one simulation: arrays laid out as the caller's ksched_result, so that each copies
-// out in one piece.
-struct SimFullOut {
+// The arrays of one result on the device, laid out as the caller's ksched_result so that each copies out in one piece
+// (copy_out): where the collect kernels write, or the pack kernel's own per-pod arrays.
+struct ResultArrays {
   int32_t *assign, *relax, *seq;
   ksched_new_node* nodes;
-  uint64_t* types;                 // [capacity][W64]
-  int64_t* ext;                    // [capacity][X]
-  uint32_t* ext_present;           // [capacity]
-  SimFullDev* scalars;
+  uint64_t* types;                 // [nodes][W64]
+  int64_t* ext;                    // [nodes][X]
+  uint32_t* ext_present;           // [nodes]
+  ksched_launch_choice* launch;    // [nodes]
+  // the same arrays from pod o and new node o on
+  ResultArrays at(size_t o, int W64, int X) const {
+    return {assign + o, relax + o, seq + o, nodes + o, types + o * W64, ext + o * X, ext_present + o, launch + o};
+  }
 };
+
+// New node n's row, option words and, with ext resources (X > 0), its ext requests and ext-present word, into row n of
+// `out`: the 32 lanes of one warp.
+__device__ __forceinline__ void collect_new_node(const PackState& s, int W32, int X, int n, int lane, const ResultArrays& out) {
+  gather_new_node(s, W32, n, lane, 32, out.nodes + n, reinterpret_cast<uint32_t*>(out.types + (size_t)n * (W32 / 2)));  // W32 is even
+  for (int x = lane; x < X; x += 32) out.ext[(size_t)n * X + x] = s.nn_req_ext[(size_t)n * X + x];
+  if (X && lane == 0) out.ext_present[n] = s.nn_ext_present[n];
+}
+
+// A Solve's new nodes 0 .. n_new-1 (one warp per node) and, when `ex_rows` is given, the existing nodes' final
+// requirements as rows (one thread per node).
+__global__ void solve_collect_kernel(PackState s, int W32, int X, int n_new, ResultArrays out, ksched_reqset* ex_rows) {
+  const int tid = blockIdx.x * blockDim.x + threadIdx.x, nth = gridDim.x * blockDim.x;
+  for (int n = tid >> 5; n < n_new; n += nth >> 5) collect_new_node(s, W32, X, n, threadIdx.x & 31, out);
+  if (!ex_rows) return;
+  const int NE = s.n_existing;
+  for (int e = tid; e < NE; e += nth) {
+    ksched_reqset r;
+    for (int k = 0; k < KSCHED_MAX_KEYS; ++k) r.values[k] = s.ex_vals[(size_t)k * NE + e];
+    r.meta = s.ex_meta[e];
+    ex_rows[e] = r;
+  }
+}
+
 // simulateScheduling's whole answer in the numbering of the problem encoded fresh for this set. The batch holds the
 // pending pods (the first n_lead of them lead), then the removed nodes' pods in the set's order (cluster_select_kernel with
 // the set's offsets): batch position b goes to pod b, b + n_removed_pods or b - n_pending + n_lead. slot_map[e] = the slot's
@@ -135,7 +163,7 @@ struct SimFullOut {
 // (PackState nn_*) into rows. One block per simulation, a few thousand pods and nodes: microseconds.
 __global__ void cluster_full_collect_kernel(PackState s, int W32, int X, int n_pods, int n_pending, int n_lead, int n_removed_pods,
                                             const int32_t* __restrict__ slot_map, const uint8_t* __restrict__ initialized, int n_stay,
-                                            SimFullOut out) {
+                                            ResultArrays out, SimFullDev* scalars) {
   __shared__ int uninit;
   const int tid = threadIdx.x, n_existing = s.n_existing;
   const int n_new = (int)s.counters[kCtrNewNodes];
@@ -150,15 +178,7 @@ __global__ void cluster_full_collect_kernel(PackState s, int W32, int X, int n_p
   }
   for (int e = tid; e < n_existing; e += blockDim.x)
     if (slot_map[e] >= 0 && initialized && !initialized[e]) uninit = 1;  // helpers.go:104-110 walks every node that stays
-  const int W64 = W32 / 2;  // DevCatalog::W32 is even
-  const int lane = tid & 31, warps = blockDim.x >> 5;
-  for (int n = tid >> 5; n < n_new; n += warps) {  // one warp per node
-    gather_new_node(s, W32, n, lane, 32, out.nodes + n, reinterpret_cast<uint32_t*>(out.types + (size_t)n * W64));
-    if (out.ext) {
-      for (int x = lane; x < X; x += 32) out.ext[(size_t)n * X + x] = s.nn_req_ext[(size_t)n * X + x];
-      if (lane == 0) out.ext_present[n] = s.nn_ext_present[n];
-    }
-  }
+  for (int n = tid >> 5; n < n_new; n += blockDim.x >> 5) collect_new_node(s, W32, X, n, tid & 31, out);
   __syncthreads();
   if (tid == 0) {
     SimFullDev d;
@@ -170,7 +190,7 @@ __global__ void cluster_full_collect_kernel(PackState s, int W32, int X, int n_p
     d.all_pods_scheduled = d.n_unscheduled == 0 ? 1 : 0;
     d.uninitialized_existing = uninit;
     d.pad = 0;
-    *out.scalars = d;
+    *scalars = d;
   }
 }
 

@@ -22,6 +22,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <cub/cub.cuh>
 #include <string>
 #include <mutex>
@@ -339,17 +340,18 @@ struct ksched_handle {
   DevBuf<uint8_t> d_in_set;
   DevBuf<ksched_sim_result> d_sim_results;
   DevBuf<uint64_t> d_sim_types;
-  // full simulations (ksched_simulate_full): which slots a set may remove, the initialised flags, the leading pending pods,
-  // and the staging arrays every set's results are gathered into before they are copied out
+  // full simulations (ksched_simulate_full): which slots a set may remove, the initialised flags, the leading pending pods;
+  // and the staging arrays a result is gathered into before it is copied out (stage_result: full simulations, Solves)
   std::vector<uint8_t> h_node_removable;
   int sup_lead = 0;
   DevBuf<uint8_t> d_node_init;
-  DevBuf<int32_t> d_slot_map, d_full_i32;
-  DevBuf<ksched_new_node> d_full_nodes;
-  DevBuf<uint64_t> d_full_types;
-  DevBuf<int64_t> d_full_ext;
-  DevBuf<uint32_t> d_full_ext_present;
-  DevBuf<ksched_launch_choice> d_full_launch;
+  DevBuf<int32_t> d_slot_map, d_res_i32;
+  DevBuf<ksched_new_node> d_res_nodes;
+  DevBuf<uint64_t> d_res_types;
+  DevBuf<int64_t> d_res_ext;
+  DevBuf<uint32_t> d_res_ext_present;
+  DevBuf<ksched_launch_choice> d_res_launch;
+  DevBuf<ksched_reqset> d_res_ex_reqs;
   DevBuf<SimFullDev> d_full_scalars;
   bool cluster_topology = false;
   int filt_words = 0;
@@ -361,8 +363,7 @@ struct ksched_handle {
   DevBuf<int32_t> d_rk_off, d_rk_prio, d_rk_order, d_rk_n;
   DevBuf<double> d_rk_dc, d_rk_age, d_rk_ttl, d_rk_cost_in, d_rk_cost, d_rk_cost_out;
   DevBuf<uint8_t> d_rk_flags, d_rk_elig_in, d_rk_elig;
-  // ---- launch choices, all-gather, L2 flush, K1 profile
-  DevBuf<ksched_launch_choice> d_launch;
+  // ---- all-gather, L2 flush, K1 profile
   DevBuf<uint8_t> d_gather_send, d_gather_recv;
   DevBuf<uint32_t> d_flush;
   DevBuf<long long> d_k1dbg;
@@ -389,21 +390,6 @@ template <class T>
 static cudaError_t download(ksched_handle* h, T* dst, const T* src, size_t n) {
   h->tm.d2h_bytes += (int64_t)(n * sizeof(T));
   return cudaMemcpyAsync(dst, src, n * sizeof(T), cudaMemcpyDeviceToHost, h->stream);
-}
-// The first n columns of a device SoA array [rows][pitch] (new nodes), packed to [rows][n] on the host.
-template <class T>
-static cudaError_t download_soa(ksched_handle* h, std::vector<T>& dst, const T* src, int rows, size_t pitch, int n) {
-  dst.resize((size_t)rows * n);
-  h->tm.d2h_bytes += (int64_t)(dst.size() * sizeof(T));
-  return cudaMemcpy2DAsync(dst.data(), (size_t)n * sizeof(T), src, pitch * sizeof(T), (size_t)n * sizeof(T), rows, cudaMemcpyDeviceToHost, h->stream);
-}
-// Node i's entries of a host copy [rows][n] of a SoA array, to row_of(i)[0 .. rows).
-template <class T, class RowOf>
-static void soa_to_rows(const std::vector<T>& soa, int rows, int n, RowOf row_of) {
-  for (int i = 0; i < n; ++i) {
-    T* row = row_of(i);
-    for (int r = 0; r < rows; ++r) row[r] = soa[(size_t)r * n + i];
-  }
 }
 
 static cudaError_t record_reset(ResetTable& t, void* dst, const void* src, size_t bytes) {
@@ -1671,11 +1657,44 @@ static const char* pack_error_text(long long code) {
   return code == KSCHED_ERR_OVERFLOW ? "new-node capacity exceeded" : "a pod is constrained by more topology groups than the kernel supports";
 }
 
+// The handle's staging arrays (ResultArrays) sized for n_pods pods and n_nodes new nodes.
+static int stage_result(ksched_handle* h, size_t n_pods, size_t n_nodes, ResultArrays& out) {
+  const size_t W64 = h->cat.W32 / 2, X = h->cat.n_res_ext;
+  CUDA_TRY(h, h->d_res_i32.ensure(3 * n_pods));
+  CUDA_TRY(h, h->d_res_nodes.ensure(n_nodes));
+  CUDA_TRY(h, h->d_res_types.ensure(n_nodes * W64));
+  CUDA_TRY(h, h->d_res_ext.ensure(n_nodes * X));
+  CUDA_TRY(h, h->d_res_ext_present.ensure(n_nodes));
+  CUDA_TRY(h, h->d_res_launch.ensure(n_nodes));
+  int32_t* i32 = h->d_res_i32.ptr;
+  out = ResultArrays{i32, i32 + n_pods, i32 + 2 * n_pods, h->d_res_nodes.ptr, h->d_res_types.ptr, h->d_res_ext.ptr, h->d_res_ext_present.ptr,
+                     h->d_res_launch.ptr};
+  return KSCHED_OK;
+}
+
+// The device-to-host copies of one result from `src` into the arrays the caller gave in `r`: n_pods entries of each per-pod
+// array, and n_nodes new nodes' launch choices and, when both new_nodes and new_node_types are given, their rows, option
+// words and ext arrays.
+static int copy_out(ksched_handle* h, const ResultArrays& src, size_t n_pods, size_t n_nodes, const ksched_result& r) {
+  const size_t W64 = h->cat.W32 / 2, X = h->cat.n_res_ext;
+  if (r.assign) CUDA_TRY(h, download(h, r.assign, src.assign, n_pods));
+  if (r.relax_level) CUDA_TRY(h, download(h, r.relax_level, src.relax, n_pods));
+  if (r.place_seq) CUDA_TRY(h, download(h, r.place_seq, src.seq, n_pods));
+  if (r.new_nodes && r.new_node_types) {
+    CUDA_TRY(h, download(h, r.new_nodes, src.nodes, n_nodes));
+    CUDA_TRY(h, download(h, r.new_node_types, src.types, n_nodes * W64));
+    if (X && r.new_node_requests_ext) CUDA_TRY(h, download(h, r.new_node_requests_ext, src.ext, n_nodes * X));
+    if (X && r.new_node_requests_ext_present) CUDA_TRY(h, download(h, r.new_node_requests_ext_present, src.ext_present, n_nodes));
+  }
+  if (r.launch) CUDA_TRY(h, download(h, r.launch, src.launch, n_nodes));
+  return KSCHED_OK;
+}
+
 int ksched_download(ksched_handle* h, const ksched_problem* pb, ksched_result* res) {
   if (!h || !pb || !res || !h->uploaded) return KSCHED_ERR_INVALID;
   CUDA_TRY(h, cudaSetDevice(h->device));
   const PackState& s = h->st;
-  const int P = s.n_pods, NE = s.n_existing, W32 = h->cat.W32, W64 = W32 / 2, V = h->cat.n_templates;
+  const int P = s.n_pods, NE = s.n_existing, W32 = h->cat.W32, V = h->cat.n_templates;
   long long counters[kNumCounters];
   h->tm.d2h_bytes = 0;
   CUDA_TRY(h, download(h, counters, s.counters, kNumCounters));
@@ -1698,75 +1717,33 @@ int ksched_download(ksched_handle* h, const ksched_problem* pb, ksched_result* r
   h->tm.vt_build_us = counters[kCtrVtEnd] ? (double)(counters[kCtrVtEnd] - (long long)~(unsigned long long)counters[kCtrVtStart]) / 1000.0 : 0.0;
   h->tm.pack_interval_ns[0] = counters[kCtrPackStart];
   h->tm.pack_interval_ns[1] = counters[kCtrPackEnd];
-  if (res->assign) CUDA_TRY(h, download(h, res->assign, s.assign, (size_t)P));
-  if (res->relax_level) CUDA_TRY(h, download(h, res->relax_level, s.relax_level, (size_t)P));
-  if (res->place_seq) CUDA_TRY(h, download(h, res->place_seq, s.place_seq, (size_t)P));
-  if (n_new > 0 && res->new_nodes && res->new_node_types) {
-    std::vector<uint8_t> tmpl(n_new);
-    std::vector<int32_t> count(n_new);
-    std::vector<uint32_t> reqp(n_new), opts;
-    std::vector<uint64_t> meta(n_new), vals;
-    std::vector<int64_t> req;
-    CUDA_TRY(h, download(h, tmpl.data(), s.nn_tmpl, (size_t)n_new));
-    CUDA_TRY(h, download(h, count.data(), s.nn_count, (size_t)n_new));
-    CUDA_TRY(h, download(h, reqp.data(), s.nn_req_present, (size_t)n_new));
-    CUDA_TRY(h, download(h, meta.data(), s.nn_meta, (size_t)n_new));
-    CUDA_TRY(h, download_soa(h, req, s.nn_req, 8, (size_t)s.max_new, n_new));
-    CUDA_TRY(h, download_soa(h, vals, s.nn_vals, 16, (size_t)s.max_new, n_new));
-    CUDA_TRY(h, download_soa(h, opts, s.nn_opts, W32, (size_t)s.max_new, n_new));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    auto types_of = [&](int n) { return reinterpret_cast<uint32_t*>(res->new_node_types + (size_t)n * W64); };
-    for (int n = 0; n < n_new; ++n) {
-      ksched_new_node& o = res->new_nodes[n];
-      std::memset(&o, 0, sizeof o);
-      o.template_index = tmpl[n];
-      o.pod_count = count[n];
-      o.requests_present = reqp[n];
-      o.reqs.meta = meta[n];
-      if (W32 & 1) types_of(n)[W32] = 0;  // the row is W64 64-bit words: the caller's buffer need not be cleared
-    }
-    soa_to_rows(req, 8, n_new, [&](int n) { return res->new_nodes[n].requests; });
-    soa_to_rows(vals, 16, n_new, [&](int n) { return res->new_nodes[n].reqs.values; });
-    soa_to_rows(opts, W32, n_new, types_of);
-    if (const int X = h->cat.n_res_ext) {
-      if (res->new_node_requests_ext) CUDA_TRY(h, download(h, res->new_node_requests_ext, s.nn_req_ext, (size_t)n_new * X));
-      if (res->new_node_requests_ext_present) CUDA_TRY(h, download(h, res->new_node_requests_ext_present, s.nn_ext_present, (size_t)n_new));
-      CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    }
-  }
-  if (res->launch && n_new > 0) {
-    if (!h->cat.offer_keys) { h->err = "ksched_result.launch needs ksched_catalog.offering_keys"; return KSCHED_ERR_INVALID; }
-    CUDA_TRY(h, h->d_launch.ensure((size_t)n_new));
-    launch_choice_kernel<<<h->n_sm, 256, 0, h->stream>>>(h->cat, s.counters, s.nn_vals, s.nn_meta, s.nn_opts, s.max_new, h->d_launch.ptr);
-    CUDA_TRY(h, download(h, res->launch, h->d_launch.ptr, (size_t)n_new));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  }
-  if (res->existing_reqs && NE > 0) {
-    std::vector<uint64_t> vals((size_t)16 * NE), meta(NE);
-    CUDA_TRY(h, download(h, vals.data(), s.ex_vals, vals.size()));
-    CUDA_TRY(h, download(h, meta.data(), s.ex_meta, meta.size()));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    soa_to_rows(vals, 16, NE, [&](int e) { return res->existing_reqs[e].values; });
-    for (int e = 0; e < NE; ++e) res->existing_reqs[e].meta = meta[e];
-  }
-  if (res->feasibility) {
-    // device rows are in FFD (queue) order; the caller gets them in its own pod order
-    std::vector<uint32_t> order(P), F((size_t)P * V * W32);
-    CUDA_TRY(h, download(h, order.data(), s.order, order.size()));
-    CUDA_TRY(h, download(h, F.data(), s.F, F.size()));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    const size_t rowb = (size_t)V * W32;
-    for (int j = 0; j < P; ++j) std::memcpy(reinterpret_cast<uint32_t*>(res->feasibility) + (size_t)order[j] * rowb, &F[(size_t)j * rowb], rowb * 4);
-  }
-  if (res->best_column) {
-    std::vector<uint32_t> order(P);
-    std::vector<unsigned long long> best(P);
-    CUDA_TRY(h, download(h, order.data(), s.order, order.size()));
-    CUDA_TRY(h, download(h, best.data(), s.best, best.size()));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    for (int j = 0; j < P; ++j) res->best_column[order[j]] = best[j];
-  }
+  if (res->launch && n_new > 0 && !h->cat.offer_keys) { h->err = "ksched_result.launch needs ksched_catalog.offering_keys"; return KSCHED_ERR_INVALID; }
+  // the new nodes (and the existing nodes' requirements) gathered into rows on the device
+  const bool nodes = n_new > 0 && res->new_nodes && res->new_node_types, ex_rows = res->existing_reqs && NE > 0;
+  ResultArrays src;
+  int rc = stage_result(h, 0, (size_t)n_new, src);
+  if (rc != KSCHED_OK) return rc;
+  src.assign = s.assign, src.relax = s.relax_level, src.seq = s.place_seq;  // the pack kernel's own per-pod arrays
+  if (ex_rows) CUDA_TRY(h, h->d_res_ex_reqs.ensure((size_t)NE));
+  if (nodes || ex_rows)
+    solve_collect_kernel<<<h->n_sm, 256, 0, h->stream>>>(s, W32, h->cat.n_res_ext, nodes ? n_new : 0, src, ex_rows ? h->d_res_ex_reqs.ptr : nullptr);
+  if (res->launch && n_new > 0)
+    launch_choice_kernel<<<h->n_sm, 256, 0, h->stream>>>(h->cat, s.counters, s.nn_vals, s.nn_meta, s.nn_opts, s.max_new, src.launch);
+  if ((rc = copy_out(h, src, (size_t)P, (size_t)n_new, *res)) != KSCHED_OK) return rc;
+  if (ex_rows) CUDA_TRY(h, download(h, res->existing_reqs, h->d_res_ex_reqs.ptr, (size_t)NE));
+  // feasibility rows and best columns are in FFD (queue) order on the device; the caller gets them in its own pod order
+  const size_t rowb = (size_t)V * W32;
+  std::vector<uint32_t> order(res->feasibility || res->best_column ? P : 0), F(res->feasibility ? P * rowb : 0);
+  std::vector<unsigned long long> best(res->best_column ? P : 0);
+  if (!order.empty()) CUDA_TRY(h, download(h, order.data(), s.order, order.size()));
+  if (!F.empty()) CUDA_TRY(h, download(h, F.data(), s.F, F.size()));
+  if (!best.empty()) CUDA_TRY(h, download(h, best.data(), s.best, best.size()));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaGetLastError());
+  for (int j = 0; j < P; ++j) {
+    if (res->feasibility) std::memcpy(reinterpret_cast<uint32_t*>(res->feasibility) + (size_t)order[j] * rowb, &F[(size_t)j * rowb], rowb * 4);
+    if (res->best_column) res->best_column[order[j]] = best[j];
+  }
   return KSCHED_OK;
 }
 
@@ -1916,39 +1893,34 @@ static int run_simulation(ksched_handle* h, int q, const std::vector<int32_t>& n
   return run_pack(h, P, stop_new_nodes);
 }
 
-int ksched_simulate_batch(ksched_handle* h, const ksched_candidate_set* sets, int n_sets, ksched_sim_result* results, uint64_t* node0_types) {
+// The set loop of both simulation calls: the checks, the sets staged (stage_sets), `prepare(batch)`, and per set one
+// simulation (run_simulation) followed by `collect(q, P)`; after the last set `finish(batch)` issues the copies out, then
+// the last pack launch's interval, one synchronisation and the call's time. batch[q] = set q's pod count.
+using SetsStep = std::function<int(const std::vector<int32_t>& batch)>;
+static int run_sets(ksched_handle* h, const ksched_candidate_set* sets, int n_sets, const void* results, bool full, const SetsStep& prepare,
+                    const std::function<int(int q, int P)>& collect, const SetsStep& finish) {
   if (!h || !sets || n_sets < 0 || (n_sets > 0 && !results)) return KSCHED_ERR_INVALID;
   if (!h->have_cluster) { h->err = "ksched_load_cluster must be called first"; return KSCHED_ERR_INVALID; }
   if (n_sets == 0) return KSCHED_OK;
   CUDA_TRY(h, cudaSetDevice(h->device));
-  const int W32 = h->cat.W32, W64 = W32 / 2;
   std::vector<int32_t> node_off, batch;
-  int rc = stage_sets(h, sets, n_sets, false, node_off, batch);
-  if (rc != KSCHED_OK) return rc;
-  CUDA_TRY(h, h->d_sim_results.ensure((size_t)n_sets));
-  CUDA_TRY(h, h->d_sim_types.ensure((size_t)n_sets * W64));
+  int rc = stage_sets(h, sets, n_sets, full, node_off, batch);
+  if (rc != KSCHED_OK || (rc = prepare(batch)) != KSCHED_OK) return rc;
   CUDA_TRY(h, cudaEventRecord(h->ev[0], h->stream));
-  // nothing computeConsolidation can return depends on what happens after a second new node is opened
-  // (consolidation.go:214-224: len(newNodes) != 1 -> do nothing): the simulation stops there
-  const int stop_new_nodes = 2;
-  for (int q = 0; q < n_sets && rc == KSCHED_OK; ++q) {
+  // K1's class pass depends on the classes and the catalog alone, but does nothing on an empty batch: it runs at each set
+  // until a set with pods has had it
+  bool class_pass = true;
+  for (int q = 0; q < n_sets; ++q) {
     const int P = batch[(size_t)q];
-    if ((rc = run_simulation(h, q, node_off, P, q == 0, stop_new_nodes)) != KSCHED_OK) break;
-    cluster_collect_kernel<<<1, 32, 0, h->stream>>>(h->st, W32, P, h->d_sim_results.ptr + q, h->d_sim_types.ptr + (size_t)q * W64);
+    // nothing computeConsolidation can return depends on what happens after a second new node is opened
+    // (consolidation.go:214-224: len(newNodes) != 1 -> do nothing): its simulation stops there; simulateScheduling places
+    // every pod
+    if ((rc = run_simulation(h, q, node_off, P, class_pass, full ? 0 : 2)) != KSCHED_OK) return rc;
+    class_pass = class_pass && P == 0;
+    if ((rc = collect(q, P)) != KSCHED_OK) return rc;
   }
-  if (rc != KSCHED_OK) return rc;
   CUDA_TRY(h, cudaEventRecord(h->ev[4], h->stream));
-#ifdef KSCHED_PROFILE_PACK
-  {
-    long long counters[kNumCounters];
-    CUDA_TRY(h, cudaMemcpyAsync(counters, h->d_counters.ptr, sizeof counters, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    print_pack_profile(counters);  // the last simulation of the batch
-  }
-#endif
-  CUDA_TRY(h, cudaMemcpyAsync(results, h->d_sim_results.ptr, (size_t)n_sets * sizeof(ksched_sim_result), cudaMemcpyDeviceToHost, h->stream));
-  if (node0_types)
-    CUDA_TRY(h, cudaMemcpyAsync(node0_types, h->d_sim_types.ptr, (size_t)n_sets * W64 * 8, cudaMemcpyDeviceToHost, h->stream));
+  if ((rc = finish(batch)) != KSCHED_OK) return rc;
   // the last simulation's pack launch (its counters stay until the next reset)
   CUDA_TRY(h, cudaMemcpyAsync(h->tm.pack_interval_ns, h->d_counters.ptr + kCtrPackStart, 2 * sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
@@ -1957,85 +1929,91 @@ int ksched_simulate_batch(ksched_handle* h, const ksched_candidate_set* sets, in
   return KSCHED_OK;
 }
 
+int ksched_simulate_batch(ksched_handle* h, const ksched_candidate_set* sets, int n_sets, ksched_sim_result* results, uint64_t* node0_types) {
+  auto prepare = [&](const std::vector<int32_t>&) -> int {
+    CUDA_TRY(h, h->d_sim_results.ensure((size_t)n_sets));
+    CUDA_TRY(h, h->d_sim_types.ensure((size_t)n_sets * (h->cat.W32 / 2)));
+    return KSCHED_OK;
+  };
+  auto collect = [&](int q, int P) -> int {
+    const int W32 = h->cat.W32;
+    cluster_collect_kernel<<<1, 32, 0, h->stream>>>(h->st, W32, P, h->d_sim_results.ptr + q, h->d_sim_types.ptr + (size_t)q * (W32 / 2));
+    return KSCHED_OK;
+  };
+  auto finish = [&](const std::vector<int32_t>&) -> int {
+#ifdef KSCHED_PROFILE_PACK
+    long long counters[kNumCounters];
+    CUDA_TRY(h, cudaMemcpyAsync(counters, h->d_counters.ptr, sizeof counters, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    print_pack_profile(counters);  // the last simulation of the batch
+#endif
+    CUDA_TRY(h, cudaMemcpyAsync(results, h->d_sim_results.ptr, (size_t)n_sets * sizeof(ksched_sim_result), cudaMemcpyDeviceToHost, h->stream));
+    if (node0_types)
+      CUDA_TRY(h, cudaMemcpyAsync(node0_types, h->d_sim_types.ptr, (size_t)n_sets * (h->cat.W32 / 2) * 8, cudaMemcpyDeviceToHost, h->stream));
+    return KSCHED_OK;
+  };
+  return run_sets(h, sets, n_sets, results, false, prepare, collect, finish);
+}
+
 int ksched_simulate_full(ksched_handle* h, const ksched_candidate_set* sets, int n_sets, ksched_result* results) {
-  if (!h || !sets || n_sets < 0 || (n_sets > 0 && !results)) return KSCHED_ERR_INVALID;
-  if (!h->have_cluster) { h->err = "ksched_load_cluster must be called first"; return KSCHED_ERR_INVALID; }
-  if (n_sets == 0) return KSCHED_OK;
-  CUDA_TRY(h, cudaSetDevice(h->device));
-  const int NE = h->st.n_existing, W32 = h->cat.W32, W64 = W32 / 2, X = h->cat.n_res_ext;
-  std::vector<int32_t> node_off, batch;
-  int rc = stage_sets(h, sets, n_sets, true, node_off, batch);
-  if (rc != KSCHED_OK) return rc;
-  // the sets' staging regions (one per set, `batch` pods and as many new nodes) and their slot maps
-  std::vector<size_t> off((size_t)n_sets + 1, 0);
-  std::vector<int32_t> slot_map((size_t)n_sets * std::max(NE, 1), 0);
-  for (int q = 0; q < n_sets; ++q) {
-    const ksched_result& r = results[q];
-    if (sets[q].capacity < batch[(size_t)q]) {
-      h->err = "result of set " + std::to_string(q) + " holds " + std::to_string(sets[q].capacity) + " pods, its batch has " + std::to_string(batch[(size_t)q]);
-      return KSCHED_ERR_INVALID;
+  std::vector<size_t> off;  // the sets' staging regions: one per set, `batch` pods and as many new nodes
+  ResultArrays stage{};
+  std::vector<SimFullDev> sc;
+  auto region = [&](int q) { return stage.at(off[(size_t)q], h->cat.W32 / 2, h->cat.n_res_ext); };
+  auto prepare = [&](const std::vector<int32_t>& batch) -> int {
+    const int NE = h->st.n_existing;
+    off.assign((size_t)n_sets + 1, 0);
+    std::vector<int32_t> slot_map((size_t)n_sets * std::max(NE, 1), 0);  // per set: a slot's index among the slots that stay
+    for (int q = 0; q < n_sets; ++q) {
+      const ksched_result& r = results[q];
+      if (sets[q].capacity < batch[(size_t)q]) {
+        h->err = "result of set " + std::to_string(q) + " holds " + std::to_string(sets[q].capacity) + " pods, its batch has " + std::to_string(batch[(size_t)q]);
+        return KSCHED_ERR_INVALID;
+      }
+      if (batch[(size_t)q] > 0 && (!r.assign || !r.relax_level || !r.place_seq || !r.new_nodes || !r.new_node_types)) {
+        h->err = "a result array is missing";  // an empty batch writes none of them
+        return KSCHED_ERR_INVALID;
+      }
+      if (r.launch && !h->cat.offer_keys) { h->err = "ksched_result.launch needs ksched_catalog.offering_keys"; return KSCHED_ERR_INVALID; }
+      off[(size_t)q + 1] = off[(size_t)q] + (size_t)std::max(batch[(size_t)q], 1);
+      int32_t* map = &slot_map[(size_t)q * NE];
+      for (int i = 0; i < sets[q].n_nodes; ++i) map[sets[q].nodes[i]] = -1;
+      for (int e = 0, stay = 0; e < NE; ++e) if (map[e] == 0) map[e] = stay++; else map[e] = -1;
     }
-    if (!r.assign || !r.relax_level || !r.place_seq || !r.new_nodes || !r.new_node_types) { h->err = "a result array is missing"; return KSCHED_ERR_INVALID; }
-    if (r.launch && !h->cat.offer_keys) { h->err = "ksched_result.launch needs ksched_catalog.offering_keys"; return KSCHED_ERR_INVALID; }
-    off[(size_t)q + 1] = off[(size_t)q] + (size_t)std::max(batch[(size_t)q], 1);
-    int32_t* map = &slot_map[(size_t)q * NE];
-    for (int i = node_off[(size_t)q]; i < node_off[(size_t)q + 1]; ++i) map[sets[q].nodes[i - node_off[(size_t)q]]] = -1;
-    for (int e = 0, stay = 0; e < NE; ++e) if (map[e] == 0) map[e] = stay++; else map[e] = -1;
-  }
-  const size_t total = off[(size_t)n_sets];
-  if (!slot_map.empty()) CUDA_TRY(h, upload_vec(h, h->d_slot_map, slot_map));
-  CUDA_TRY(h, h->d_full_i32.ensure(3 * total));
-  CUDA_TRY(h, h->d_full_nodes.ensure(total));
-  CUDA_TRY(h, h->d_full_types.ensure(total * W64));
-  CUDA_TRY(h, h->d_full_ext.ensure(total * std::max(X, 1)));
-  CUDA_TRY(h, h->d_full_ext_present.ensure(total));
-  CUDA_TRY(h, h->d_full_launch.ensure(total));
-  CUDA_TRY(h, h->d_full_scalars.ensure((size_t)n_sets));
-  CUDA_TRY(h, cudaEventRecord(h->ev[0], h->stream));
-  bool class_pass = true;
-  for (int q = 0; q < n_sets && rc == KSCHED_OK; ++q) {
-    const int P = batch[(size_t)q], n_nodes = node_off[(size_t)q + 1] - node_off[(size_t)q];
-    // simulateScheduling places every pod: no stop after a second new node
-    if ((rc = run_simulation(h, q, node_off, P, class_pass, 0)) != KSCHED_OK) break;
-    class_pass = class_pass && P == 0;  // K1's class pass returns early on an empty batch
-    const size_t o = off[(size_t)q];
+    if (!slot_map.empty()) CUDA_TRY(h, upload_vec(h, h->d_slot_map, slot_map));
+    CUDA_TRY(h, h->d_full_scalars.ensure((size_t)n_sets));
+    return stage_result(h, off[(size_t)n_sets], off[(size_t)n_sets], stage);
+  };
+  auto collect = [&](int q, int P) -> int {
+    const int NE = h->st.n_existing, n_nodes = sets[q].n_nodes;
+    const ResultArrays out = region(q);
     if (results[q].launch)
       launch_choice_kernel<<<h->n_sm, 256, 0, h->stream>>>(h->cat, h->d_counters.ptr, h->d_nn_vals.ptr, h->d_nn_meta.ptr, h->d_nn_opts.ptr, h->st.max_new,
-                                                           h->d_full_launch.ptr + o);
-    SimFullOut out{h->d_full_i32.ptr + o, h->d_full_i32.ptr + total + o, h->d_full_i32.ptr + 2 * total + o, h->d_full_nodes.ptr + o,
-                   h->d_full_types.ptr + o * W64, X ? h->d_full_ext.ptr + o * X : nullptr, h->d_full_ext_present.ptr + o, h->d_full_scalars.ptr + q};
+                                                           out.launch);
     int removed_pods = 0;
     for (int i = 0; i < n_nodes; ++i) removed_pods += h->h_node_count[(size_t)sets[q].nodes[i]];
-    cluster_full_collect_kernel<<<1, 256, 0, h->stream>>>(h->st, W32, X, P, h->sup_pending, h->sup_lead, removed_pods, h->d_slot_map.ptr + (size_t)q * NE,
-                                                          h->d_node_init.ptr, NE - n_nodes, out);
+    cluster_full_collect_kernel<<<1, 256, 0, h->stream>>>(h->st, h->cat.W32, h->cat.n_res_ext, P, h->sup_pending, h->sup_lead, removed_pods,
+                                                          h->d_slot_map.ptr + (size_t)q * NE, h->d_node_init.ptr, NE - n_nodes, out,
+                                                          h->d_full_scalars.ptr + q);
     CUDA_TRY(h, cudaGetLastError());
-  }
-  if (rc != KSCHED_OK) return rc;
-  CUDA_TRY(h, cudaEventRecord(h->ev[4], h->stream));
+    return KSCHED_OK;
+  };
   // every set's arrays straight into the caller's buffers (capacity-sized: the counts are not known before the one
   // synchronisation), then the scalars
-  std::vector<SimFullDev> sc((size_t)n_sets);
-  for (int q = 0; q < n_sets; ++q) {
-    ksched_result& r = results[q];
-    const size_t o = off[(size_t)q], P = (size_t)batch[(size_t)q];
-    if (P == 0) continue;
-    CUDA_TRY(h, download(h, r.assign, h->d_full_i32.ptr + o, P));
-    CUDA_TRY(h, download(h, r.relax_level, h->d_full_i32.ptr + total + o, P));
-    CUDA_TRY(h, download(h, r.place_seq, h->d_full_i32.ptr + 2 * total + o, P));
-    CUDA_TRY(h, download(h, r.new_nodes, h->d_full_nodes.ptr + o, P));
-    CUDA_TRY(h, download(h, r.new_node_types, h->d_full_types.ptr + o * W64, P * W64));
-    if (r.launch) CUDA_TRY(h, download(h, r.launch, h->d_full_launch.ptr + o, P));
-    if (X && r.new_node_requests_ext) CUDA_TRY(h, download(h, r.new_node_requests_ext, h->d_full_ext.ptr + o * X, P * X));
-    if (X && r.new_node_requests_ext_present) CUDA_TRY(h, download(h, r.new_node_requests_ext_present, h->d_full_ext_present.ptr + o, P));
-  }
-  CUDA_TRY(h, download(h, sc.data(), h->d_full_scalars.ptr, sc.size()));
-  // the last simulation's pack launch (its counters stay until the next reset)
-  CUDA_TRY(h, cudaMemcpyAsync(h->tm.pack_interval_ns, h->d_counters.ptr + kCtrPackStart, 2 * sizeof(long long), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  CUDA_TRY(h, cudaGetLastError());
-  h->tm.total_us = ev_us(h->ev[0], h->ev[4]);
-  for (int q = 0; q < n_sets; ++q) {
-    const SimFullDev& d = sc[(size_t)q];
+  auto finish = [&](const std::vector<int32_t>& batch) -> int {
+    for (int q = 0; q < n_sets; ++q) {
+      const size_t P = (size_t)batch[(size_t)q];
+      const int rc = copy_out(h, region(q), P, P, results[q]);
+      if (rc != KSCHED_OK) return rc;
+    }
+    sc.resize((size_t)n_sets);
+    CUDA_TRY(h, download(h, sc.data(), h->d_full_scalars.ptr, sc.size()));
+    return KSCHED_OK;
+  };
+  const int rc = run_sets(h, sets, n_sets, results, true, prepare, collect, finish);
+  if (rc != KSCHED_OK) return rc;
+  for (size_t q = 0; q < sc.size(); ++q) {
+    const SimFullDev& d = sc[q];
     if (d.error != 0) {
       h->err = "set " + std::to_string(q) + ": " + pack_error_text(d.error);
       return d.error;
